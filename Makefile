@@ -1,6 +1,6 @@
-# Build the sm_100a shared library (C ABI in include/loftr_b200.h) and the test helpers.
+# Build the sm_90a shared library (C ABI in include/loftr_b200.h) and the test helpers.
 NVCC      ?= nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC
 LIB       := loftr_b200/lib/libloftr_b200.so
 CSRC      := loftr_b200/csrc

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the matching hot path: image-pairs/sec @640x480, indoor_ds dual-softmax (BASELINE.json).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--no-extra]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--no-extra] [--dump-outputs DIR]
 
 One "step" = one `matcher(batch)` call on a batch of 8 synthetic 640x480 grayscale pairs per GPU
 (BASELINE.json configs[1]; weak scaling: every rank processes its own 8 pairs, then ONE NCCL all-gather of the
@@ -20,6 +20,9 @@ Prints ONE JSON line (rank 0).  Keys follow the driver's contract:
   extra_workloads  the other BASELINE.json configs, same timing rules (N = 1: configs[2] shard, configs[3] sweep,
              configs[4] Sinkhorn, thr 0.2; N > 1: configs[2] = 4 pairs 832x832 per GPU + the all-gather)
 `--impl reference` times that CPU port as the whole arm (rank 0 only).
+`--dump-outputs DIR` (rank 0) writes the match lists of the last timed step as DIR/<key>.npy (float32 coordinates and
+confidences, float64 indices) so that two builds can be compared output for output on identical seeded inputs: the
+local lists of DUMP_KEYS with one GPU, the all-gathered lists of GATHER_KEYS (what every rank receives) with several.
 """
 from __future__ import annotations
 
@@ -38,8 +41,11 @@ sys.path.insert(0, ROOT)
 H, W_IMG = 480, 640
 BATCH_PER_GPU = 8
 METRIC = "image-pairs/sec @640x480 indoor_ds dual-softmax"
-DTYPE = ("f32-equivalent: every product (backbone convolutions, transformer, score matrix) = 3x fp16 tcgen05 MMA "
+DTYPE = ("f32-equivalent: every product (backbone convolutions, transformer, score matrix) = 3x fp16 wgmma "
          "(hi*hi + hi*lo + lo*hi) with fp32 accumulate; CUDA-core kernels fp32")
+# keys of the matcher's output written by --dump-outputs: one row per match
+DUMP_KEYS = ("b_ids", "i_ids", "j_ids", "mconf", "mkpts0_c", "mkpts1_c", "mkpts0_f", "mkpts1_f")
+GATHER_KEYS = ("m_bids", "mconf", "mkpts0_f", "mkpts1_f")
 
 
 def parse():
@@ -53,7 +59,9 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra_workloads block")
     ap.add_argument("--backbone", default="b200", choices=["b200", "torch"],
-                    help="b200: implicit-GEMM convolutions on tcgen05 (default); torch: PyTorch/cuDNN fp32 backbone")
+                    help="b200: implicit-GEMM convolutions on the tensor cores (default); torch: PyTorch/cuDNN fp32 backbone")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the match lists of the last timed step as DIR/<key>.npy")
     return ap.parse_args()
 
 
@@ -63,7 +71,8 @@ def peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- not reached, an upper bound
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 # ------------------------------------------------------------------------------------------------ CPU arm
@@ -73,8 +82,7 @@ def cpu_pairs_per_sec(thr, steps, warmup, pairs_per_step=1):
     import torch
     import loftr_b200
     from oracle import loftr_oracle as O
-    # all host cores up to 32 threads: beyond that the ~1-10 ms numpy / BLAS calls of this workload only
-    # oversubscribe (measured on the 128-core GPU host: 12.1 s/pair with 128 threads)
+    # all host cores up to 32 threads: beyond that the ~1-10 ms numpy / BLAS calls of this workload only oversubscribe
     cores = min(os.cpu_count() or 1, 32)
     torch.set_num_threads(cores)
     try:
@@ -198,7 +206,7 @@ class ClockSampler:
                 "sampled": where, "reasons": sorted(reasons)}
 
 
-# ------------------------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------------------------ GPU arm
 def run_b200(args):
     import torch
     import torch.distributed as dist
@@ -209,7 +217,7 @@ def run_b200(args):
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 arm has no CPU fallback (use --impl reference for the CPU port)")
+        raise SystemExit("bench.py: no CUDA device; the GPU arm has no CPU fallback (use --impl reference for the CPU port)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     clk = ClockSampler(local)                        # sampling from now on; the timed region is marked with `with clk:`
@@ -218,7 +226,7 @@ def run_b200(args):
     torch.backends.cudnn.benchmark = True
 
     B = args.batch
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 50 MB L2
     lib = _lib.load()
     stream = torch.cuda.current_stream()
     pk = peaks()
@@ -331,9 +339,8 @@ def run_b200(args):
         copy.deepcopy(main.model.backbone).to("meta")(torch.empty(2 * B, 1, H, W_IMG, device="meta"))
     backbone_flops = float(fcm.get_total_flops())
 
-    # Phase A -- everything that loads CUDA kernels runs BEFORE the NCCL communicator exists.  With the
-    # communicator created first, the first launch of every not-yet-loaded kernel module stalls for tens of
-    # seconds on this image (measured with tools/mgpu_diag.py) -- slow module loading, not a deadlock.
+    # Phase A -- everything that loads CUDA kernels runs BEFORE the NCCL communicator exists: with the communicator
+    # created first, the first launch of every not-yet-loaded kernel module can stall for seconds (slow module loading).
     extra_defs = []
     if not args.no_extra:
         if world == 1:
@@ -374,11 +381,9 @@ def run_b200(args):
         for wl in [w for _, w in extras] + [main]:   # collective warm-up (NCCL channels, all-gather kernel)
             for _ in range(2):
                 wl.step()
-        # the GPUs idled (and dropped their clocks) while the communicators were being created: repeat the W warm-up
-        # steps of the headline workload right before the timed region (measured at N = 2: 28.4 ms/step for the first
-        # ten steps after the idle gap vs 24.8 ms afterwards, 1665 MHz vs 1965 MHz)
-        # (r2w: eight steps were not always enough -- 28.05 ms/step timed right after them vs 22.5 ms a second later;
-        # the count is fixed, not time-based, so that every rank issues the same number of collectives)
+        # the GPUs idled (and dropped their clocks) while the communicators were being created: repeat the warm-up steps
+        # of the headline workload right before the timed region (the count is fixed, not time-based, so that every
+        # rank issues the same number of collectives)
         for _ in range(max(Wm, 60)):
             main.step()
         torch.cuda.synchronize()
@@ -411,9 +416,22 @@ def run_b200(args):
     # ---- device-resident throughput
     barrier()
     launches0 = lib.lb_launch_count()
+    last_out = {}
+
+    def timed_step():
+        data, gathered = main.step()
+        last_out["data"], last_out["keys"] = (data, DUMP_KEYS) if gathered is None else (gathered, GATHER_KEYS)
+
     with clk:
-        ms_steps = timed(lambda: main.step(), K)
+        ms_steps = timed(timed_step, K)
         barrier()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for k in last_out["keys"]:
+            v = last_out["data"][k].detach().cpu()
+            v = v.double() if not v.is_floating_point() else v.float()
+            np.save(os.path.join(args.dump_outputs, f"{k}.npy"), v.numpy())
     launches = lib.lb_launch_count() - launches0
     my_ms = sum(ms_steps) / K
     rank_ms_list = all_ranks(my_ms)
@@ -475,11 +493,7 @@ def run_b200(args):
             if cnt:
                 kernels[tag] = {"launches_per_step": cnt / nprof, "avg_ms": ms / cnt, "total_ms_per_step": ms / nprof}
         if sf:
-            traffic, traffic_src = None, None
-            tp = os.path.join(ROOT, "profiles", "r2_score_lse_traffic.json")
-            if os.path.exists(tp):
-                tj = json.load(open(tp))
-                traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("source")
+            traffic, traffic_src = None, "not measured"
             roof = {"kernel": "gemm_split_kernel<256, EpiScoreLse<rows,cols>> (score matrix + dual-softmax statistics)",
                     "bound": "tensor", "achieved": sf["achieved_tflops"], "peak": pk["bf16_tflops_sustained"],
                     "unit": "TFLOP/s", "frac": sf["frac"], "traffic": traffic, "traffic_source": traffic_src,
@@ -515,7 +529,7 @@ def run_b200(args):
             "config": {"workload": f"batch={B} 640x480 pairs per GPU, indoor_ds dual-softmax, thr={args.thr}",
                        "global_batch": B * world, "thr": args.thr, "weights": "random-init seed 0",
                        "matches_per_step_rank0": m_per_step, "l2": "256 MiB flush buffer written before every timed step",
-                       "backbone": ("ResNetFPN_8_2 as implicit-GEMM convolutions on tcgen05 (3x fp16 split, fp32 accumulate)"
+                       "backbone": ("ResNetFPN_8_2 as implicit-GEMM convolutions on wgmma (3x fp16 split, fp32 accumulate)"
                                     if args.backbone == "b200" else "PyTorch/cuDNN fp32 (TF32 off)"),
                        "parallelism": f"pairs sharded over {world} GPU(s), one NCCL all-gather of match lists"},
             "clocks": clk.summary(),

@@ -1,5 +1,5 @@
 /*
- * loftr_b200 -- C ABI of the B200-native LoFTR matching hot path.
+ * loftr_b200 -- C ABI of the H100-native LoFTR matching hot path.
  *
  * Every entry point replaces one `forward` of the reference (zju3dv/LoFTR, paths relative to the
  * reference root) and is what a binding from the reference side would call:
@@ -22,7 +22,7 @@
  *   - Workspaces are caller-provided; query the size with the matching *_workspace_bytes function.
  *   - "planes": an fp32 matrix x kept as two fp16 matrices hi, lo with x ~= hi + lo (see DESIGN.md).
  *     A "cat buffer" is a [rows, 2C] pair of planes; columns [0, C) hold the token features.
- *   - There is no CPU fallback: on a machine without an sm_100 device every compute entry point fails.
+ *   - There is no CPU fallback: on a machine without an sm_90 (H100) device every compute entry point fails.
  */
 #ifndef LOFTR_B200_H_
 #define LOFTR_B200_H_

@@ -1,4 +1,4 @@
-"""loftr_b200 -- B200-native LoFTR matching engine; drop-in for `from src.loftr import LoFTR, default_cfg`."""
+"""loftr_b200 -- H100-native LoFTR matching engine; drop-in for `from src.loftr import LoFTR, default_cfg`."""
 from .config import default_cfg, get_cfg
 from .loftr import LoFTR
 

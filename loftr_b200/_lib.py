@@ -2,7 +2,7 @@
 
 The CUDA library is mandatory: there is no PyTorch / CPU fallback for the hot path.  Importing this
 module on a machine where the library has not been built raises immediately; calling a compute entry
-point without an sm_100 device fails inside the library with a clear message.
+point without an sm_90 (H100) device fails inside the library with a clear message.
 """
 from __future__ import annotations
 

@@ -18,8 +18,8 @@
 #include "gemm_split.cuh"
 #include "simt_kernels.cuh"
 #include "kv_gemm.cuh"
-#include "comm.cuh"
 #include "stem_tc.cuh"
+#include "comm.cuh"
 
 namespace lb {
 
@@ -113,8 +113,8 @@ static int device_check(int* sm_count) {
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, dev);
     if (e != cudaSuccess) return fail("cudaGetDeviceProperties: %s", cudaGetErrorString(e));
-    if (prop.major != 10)
-      return fail("loftr_b200 requires an sm_100 (B200) device, found sm_%d%d; there is no fallback", prop.major,
+    if (prop.major != 9 || prop.minor != 0)
+      return fail("loftr_b200 requires an sm_90 (H100) device, found sm_%d%d; there is no fallback", prop.major,
                   prop.minor);
     sms[dev] = prop.multiProcessorCount;
   }
@@ -228,23 +228,6 @@ static int make_out_map_nhwc(CUtensorMap* m, const void* base, bool f32, int C, 
   if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (NHWC output) failed with CUresult %d", static_cast<int>(r));
   return 0;
 }
-// FPN upsample source planes [N, H, W, ld] (C valid channels) as unswizzled (box_c, kUpW, kUpH, 1) load boxes: the
-// window EpiConv<., true> stages per output tile; channels / pixels outside the tensor arrive as zeros.
-static int make_up_map(CUtensorMap* m, const void* base, int C, int W, int H, int N, long ld, int box_c) {
-  auto enc = get_encode();
-  if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld * 2) % 16 != 0) return fail("upsample source planes not 16-byte aligned");
-  cuuint64_t dims[4] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H), static_cast<cuuint64_t>(N)};
-  cuuint64_t strides[3] = {static_cast<cuuint64_t>(ld * 2), static_cast<cuuint64_t>(ld * 2) * W,
-                           static_cast<cuuint64_t>(ld * 2) * W * H};
-  cuuint32_t box[4] = {static_cast<cuuint32_t>(box_c), static_cast<cuuint32_t>(kUpW), static_cast<cuuint32_t>(kUpH), 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (upsample source) failed with CUresult %d", static_cast<int>(r));
-  return 0;
-}
 // planes (+ optional fp32) of a [batches][rows][cols] output
 static int fill_out_maps(OutMaps* om, const void* hi, const void* lo, long ld_pl, const float* f32, long ld_f32, long cols,
                          long rows, long batches) {
@@ -271,52 +254,9 @@ struct Planes {
 };
 
 // ------------------------------------------------------------------------------------------------ GEMM launch
-// Execution mode of the tensor-core kernels (gemm_split.cuh kMode): 0 = single CTA, 1 = cluster of two with TMA
-// multicast of the B tile, 2 = CTA pairs with tcgen05.mma.cta_group::2.  Default policy from the A/B measurement
-// in profiles/r1_kernel_variants_ab.md: the pair kernels win where the MMA phase dominates (convolutions -7 %,
-// mlp[0] -9 %, fine merge -8 %) and lose a little where the epilogue dominates (projections, score passes), so
-// they are used for exactly those launches.  LOFTR_B200_MODE=0|1|2 forces one mode for every launch.
-static int kernel_mode(int tag, int block_n = 0) {
-  static int forced = -2;
-  if (forced == -2) {
-    const char* e = getenv("LOFTR_B200_MODE");
-    forced = e ? atoi(e) : -1;
-    if (forced < -1 || forced > 2) forced = -1;
-  }
-  if (forced >= 0) return forced;
-  // per-kernel-kind override for A/B runs: LOFTR_B200_MODE_TAGS="merge_ln=2,mlp2_ln_res=2" (names of kTagNames)
-  static int per_tag[TAG_COUNT];
-  static bool parsed = false;
-  if (!parsed) {
-    for (int t = 0; t < TAG_COUNT; ++t) per_tag[t] = -1;
-    if (const char* e = getenv("LOFTR_B200_MODE_TAGS")) {
-      std::string spec(e);
-      size_t pos = 0;
-      while (pos < spec.size()) {
-        const size_t end = spec.find(',', pos);
-        const std::string item = spec.substr(pos, end == std::string::npos ? std::string::npos : end - pos);
-        const size_t eq = item.find('=');
-        if (eq != std::string::npos) {
-          for (int t = 0; t < TAG_COUNT; ++t)
-            if (item.substr(0, eq) == kTagNames[t]) per_tag[t] = atoi(item.c_str() + eq + 1);
-        }
-        if (end == std::string::npos) break;
-        pos = end + 1;
-      }
-    }
-    parsed = true;
-  }
-  if (tag >= 0 && tag < TAG_COUNT && per_tag[tag] >= 0 && per_tag[tag] <= 2) return per_tag[tag];
-  // the two LayerNorm GEMMs of the coarse transformer (N = 256, K = 256 / 512): with the pair's half-B stages the ring is
-  // three deep instead of two, 1172 -> 1105 us per step (profiles/r2u_*); the fine ones (N = 128) do not gain
-  if ((tag == TAG_MERGE_LN || tag == TAG_MLP2_LN) && block_n == 256) return 2;
-  return (tag == TAG_CONV || tag == TAG_MLP1 || tag == TAG_FINE_MERGE) ? 2 : 0;
-}
-
 // Second-generation CUDA-core kernels (kv_partial_v2, conv_stem7x7_v2).  They produce bit-identical results to the
 // first versions (checked on the device by lb_selftest, which also times both); LOFTR_B200_V2=0|1 overrides.
-// Measured (profiles/r1_selftest_v2_kernels.log): the stem v2 is 29 % faster (582 vs 816 us at batch 8) -> default;
-// kv_partial v2 is slower (129 vs 110 us: its 32-accumulator inner loop is shared-memory-read bound) -> v1 stays.
+// Defaults: the stem v2, kv_partial v1 (the v2's 32-accumulator inner loop is shared-memory-read bound).
 #ifndef LB_KV_V2_DEFAULT
 #define LB_KV_V2_DEFAULT 0
 #endif
@@ -348,14 +288,13 @@ struct GemmMaps {
   CUtensorMap ar_hi, ar_lo, br_hi, br_lo;  // convolution channel remainder (16-element boxes); copies of the above if unused
 };
 
-template <int BN, class Epi, bool kDual, int kMode>
+template <int BN, class Epi>
 static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const typename Epi::Params& ep, int sms,
                       cudaStream_t st) {
-  constexpr int kCluster = kMode == 0 ? 1 : 2;
-  using S = GemmSmem<BN, kMode == 2, Epi::kSmemBytes>;
+  using S = GemmSmem<BN, Epi::kSmemBytes>;
   constexpr int smem_bytes = S::kRingBytes + S::kBarBytes + Epi::kSmemBytes;
   static_assert(smem_bytes <= 232448, "shared memory budget exceeded");
-  auto kern = gemm_split_kernel<BN, Epi, kDual, kMode>;
+  auto kern = gemm_split_kernel<BN, Epi>;
   static bool configured[kMaxDevices] = {false};  // per instantiation and device
   int dev = 0;
   LB_CUDA(cudaGetDevice(&dev));
@@ -363,10 +302,8 @@ static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const t
     LB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     configured[dev] = true;
   }
-  const long m_groups = (s.m_tiles + kCluster - 1) / kCluster;
-  const long items = static_cast<long>(s.batches) * m_groups * s.n_chunks;
-  const long max_groups = sms / kCluster;
-  const int grid = static_cast<int>((items < max_groups ? items : max_groups) * kCluster);
+  const long items = static_cast<long>(s.batches) * s.m_tiles * s.n_chunks;
+  const int grid = static_cast<int>(items < sms ? items : sms);
   TimingRec rec{nullptr, nullptr, tag};
   if (g_timing) {
     LB_CUDA(cudaEventCreate(&rec.e0));
@@ -379,25 +316,20 @@ static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const t
   cfg.blockDim = dim3(kGemmThreads);
   cfg.dynamicSmemBytes = smem_bytes;
   cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = kCluster;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
+  cudaLaunchAttribute attr[1];
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  cfg.numAttrs = 0;
   // programmatic dependent launch of the tensor-core kernels (gemm_split.cuh): the next kernel's set-up overlaps this
-  // one's tail.  LOFTR_B200_PDL=0 disables it (4 alternating A/B pairs: median 21.08 vs 21.25 ms/step,
-  // profiles/r2y_ab_pdl_alternating.txt)
+  // one's tail.  LOFTR_B200_PDL=0 disables it.
   static int pdl = -1;
   if (pdl < 0) {
     const char* e = getenv("LOFTR_B200_PDL");
     pdl = e ? (atoi(e) != 0 ? 1 : 0) : 1;
   }
   if (pdl) {
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.numAttrs = 2;
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.numAttrs = 1;
   }
   LB_CUDA(cudaLaunchKernelEx(&cfg, kern, maps.a_hi, maps.a_lo, maps.b_hi, maps.b_lo, maps.ar_hi, maps.ar_lo, maps.br_hi,
                              maps.br_lo, s, ep));
@@ -430,18 +362,14 @@ static int launch_gemm(int tag, const Planes& A, const Planes& B, int batches, i
   s.n_chunks = (s.n_tiles + s.tiles_per_chunk - 1) / s.tiles_per_chunk;
   s.conv = ConvGeom{0, 0, 0, 0, 0, 0, 0, 0, 0};
 
-  const int mode = s.m_tiles >= 2 ? kernel_mode(tag, BN) : 0;
-  const int cl = mode == 0 ? 1 : 2;
   GemmMaps mp;
   LB_TRY(make_map(&mp.a_hi, A.hi, K, M, batches, A.ld, A.batch_stride, kBlockM));
   LB_TRY(make_map(&mp.a_lo, A.lo, K, M, batches, A.ld, A.batch_stride, kBlockM));
   const int bb = s.b_batched ? batches : 1;
-  LB_TRY(make_map(&mp.b_hi, B.hi, K, N, bb, B.ld, B.batch_stride, BN / cl));
-  LB_TRY(make_map(&mp.b_lo, B.lo, K, N, bb, B.ld, B.batch_stride, BN / cl));
+  LB_TRY(make_map(&mp.b_hi, B.hi, K, N, bb, B.ld, B.batch_stride, BN));
+  LB_TRY(make_map(&mp.b_lo, B.lo, K, N, bb, B.ld, B.batch_stride, BN));
   mp.ar_hi = mp.a_hi; mp.ar_lo = mp.a_lo; mp.br_hi = mp.b_hi; mp.br_lo = mp.b_lo;
-  if (mode == 2) return launch_raw<BN, Epi, false, 2>(tag, mp, s, ep, sms, st);
-  if (mode == 1) return launch_raw<BN, Epi, false, 1>(tag, mp, s, ep, sms, st);
-  return launch_raw<BN, Epi, false, 0>(tag, mp, s, ep, sms, st);
+  return launch_raw<BN, Epi>(tag, mp, s, ep, sms, st);
 }
 
 // Implicit-GEMM convolution launch: in = NHWC planes [N, H_in, W_in, ld_in] with Cin valid channels; weights =
@@ -467,10 +395,10 @@ static void conv_layout(int cin, int* cin_blocks, int* rem) {
     *rem = 0;
   }
 }
-template <int BN, int kUpMode = 0, bool kDualAcc = true>
+template <int BN, int kUpMode = 0>
 static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_rem, const ConvDesc& d,
-                       const typename EpiConv<BN, kUpMode, kDualAcc>::Params& ep_in, cudaStream_t st) {
-  using Epi = EpiConv<BN, kUpMode, kDualAcc>;
+                       const typename EpiConv<BN, kUpMode>::Params& ep_in, cudaStream_t st) {
+  using Epi = EpiConv<BN, kUpMode>;
   int sms = 0;
   LB_TRY(device_check(&sms));
   GemmShape s;
@@ -491,18 +419,16 @@ static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_re
   const int rem_groups = rem ? (taps + kRemTapsPerStage - 1) / kRemTapsPerStage : 0;
   s.conv = ConvGeom{1, tiles_w, d.stride, d.pad, d.ksize, cin_blocks, taps, taps * cin_blocks, rem_groups};
   if (rem && (!wgt_rem.hi || !wgt_rem.lo)) return fail("convolution with Cin=%d needs remainder weight planes", d.Cin);
-  const int mode = s.m_tiles >= 2 ? kernel_mode(TAG_CONV) : 0;
-  const int cl = mode == 0 ? 1 : 2;
   GemmMaps mp;
   LB_TRY(make_map_nhwc(&mp.a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride));
   LB_TRY(make_map_nhwc(&mp.a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride));
-  LB_TRY(make_map(&mp.b_hi, wgt.hi, s.K, d.Cout, 1, wgt.ld, 0, BN / cl));
-  LB_TRY(make_map(&mp.b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN / cl));
+  LB_TRY(make_map(&mp.b_hi, wgt.hi, s.K, d.Cout, 1, wgt.ld, 0, BN));
+  LB_TRY(make_map(&mp.b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN));
   if (rem) {
     LB_TRY(make_map_nhwc(&mp.ar_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, kRemChannels));
     LB_TRY(make_map_nhwc(&mp.ar_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, kRemChannels));
-    LB_TRY(make_map(&mp.br_hi, wgt_rem.hi, taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN / cl, kRemChannels));
-    LB_TRY(make_map(&mp.br_lo, wgt_rem.lo, taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN / cl, kRemChannels));
+    LB_TRY(make_map(&mp.br_hi, wgt_rem.hi, taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
+    LB_TRY(make_map(&mp.br_lo, wgt_rem.lo, taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
   } else {
     mp.ar_hi = mp.a_hi; mp.ar_lo = mp.a_lo; mp.br_hi = mp.b_hi; mp.br_lo = mp.b_lo;
   }
@@ -510,16 +436,7 @@ static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_re
   ep.H_out = d.H_out;
   ep.W_out = d.W_out;
   ep.tiles_w = tiles_w;
-  // dual accumulator (3x3 layers): EpiConv adds the correction accumulator; single accumulator for the short-K 1x1 layers
-  if (mode == 2) return launch_raw<BN, Epi, kDualAcc, 2>(TAG_CONV, mp, s, ep, sms, st);
-  if constexpr (kUpMode == 1) {   // the staged window only fits beside the pair mode's (half-B) ring
-    return fail("staged-upsample convolution needs the CTA-pair mode");
-  } else {
-    if constexpr (kUpMode == 0 && kDualAcc) {   // the multicast experiment is only built for the plain epilogue
-      if (mode == 1) return launch_raw<BN, Epi, true, 1>(TAG_CONV, mp, s, ep, sms, st);
-    }
-    return launch_raw<BN, Epi, kDualAcc, 0>(TAG_CONV, mp, s, ep, sms, st);
-  }
+  return launch_raw<BN, Epi>(TAG_CONV, mp, s, ep, sms, st);
 }
 
 // number of n-chunks that gives every SM a few work items when a CTA must sweep many n tiles
@@ -662,19 +579,14 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
       om.use |= 2;
     }
   }
-#define LB_CONV_CASE_UP(BN, UP) LB_CONV_CASE_ACC(BN, UP, true)
-#define LB_CONV_CASE_ACC(BN, UP, DUAL)                                                                                \
+#define LB_CONV_CASE_UP(BN, UP)                                                                                       \
   {                                                                                                                   \
-    EpiConv<BN, UP, DUAL>::Params ep{w.scale, w.shift, r.act, r.res ? r.res->hi : nullptr, r.res ? r.res->lo : nullptr,   \
+    EpiConv<BN, UP>::Params ep{w.scale, w.shift, r.act, r.res ? r.res->hi : nullptr, r.res ? r.res->lo : nullptr,     \
                                r.res ? r.res->ld : 0, r.up ? r.up->hi : nullptr, r.up ? r.up->lo : nullptr,          \
                                r.up ? r.up->ld : 0, r.up_h, r.up_w, r.out ? r.out->hi : nullptr,                      \
                                r.out ? r.out->lo : nullptr, r.out ? r.out->ld : 0, r.out_f32, r.f32_ld, 0, 0, 0, om, \
                                um};                                                                                   \
-    if (UP == 1) {                                                                                                    \
-      LB_TRY(make_up_map(&ep.um.hi, r.up->hi, d.Cout, r.up_w, r.up_h, N, r.up->ld, EpiConv<BN, UP, DUAL>::kUpBoxC));  \
-      LB_TRY(make_up_map(&ep.um.lo, r.up->lo, d.Cout, r.up_w, r.up_h, N, r.up->ld, EpiConv<BN, UP, DUAL>::kUpBoxC));  \
-    }                                                                                                                 \
-    return launch_conv<BN, UP, DUAL>(in, wg, wr, d, ep, st);                                                          \
+    return launch_conv<BN, UP>(in, wg, wr, d, ep, st);                                                                \
   }
 #define LB_CONV_CASE(BN)                                                                                              \
   {                                                                                                                   \
@@ -683,45 +595,17 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
   }
   UpMaps um;
   memset(&um, 0, sizeof(um));
-  // FPN laterals: stage the upsample source window in shared memory (exact x2 grids; LOFTR_B200_UP_STAGE=0: the
-  // per-thread global loads of the first generation)
-  static int up_stage = -1;
-  if (up_stage < 0) {
-    const char* e = getenv("LOFTR_B200_UP_STAGE");
-    up_stage = e ? (atoi(e) != 0 ? 1 : 0) : 1;
-  }
-  const bool staged_up = up_stage && r.up && d.H_out == 2 * r.up_h && d.W_out == 2 * r.up_w && w.cout > 128 &&
-                         kernel_mode(TAG_CONV) == 2 &&
-                         ((d.H_out + kConvTileH - 1) / kConvTileH) * ((d.W_out + kConvTileW - 1) / kConvTileW) >= 2;
   // output-channel tile: the smallest built N that covers Cout (196 -> 208: 13 x 16, no MMAs on 60 padding columns)
   static int n208 = -1;   // LOFTR_B200_CONV_N208=0: 256-column tiles for Cout = 196 (first-generation tiling)
   if (n208 < 0) {
     const char* e = getenv("LOFTR_B200_CONV_N208");
     n208 = e ? (atoi(e) != 0 ? 1 : 0) : 1;
   }
-  // 1x1 layers (K = Cin <= 256): single accumulator, two TMEM stages (LOFTR_B200_CONV1X1_DUAL=1: the dual layout)
-  static int dual1x1 = -1;
-  if (dual1x1 < 0) {
-    const char* e = getenv("LOFTR_B200_CONV1X1_DUAL");
-    dual1x1 = e ? (atoi(e) != 0 ? 1 : 0) : 0;
-  }
-  const bool single_acc = w.ksize == 1 && !dual1x1 && w.cout > 128 && (staged_up || !r.up);
   if (w.cout <= 128) LB_CONV_CASE(128)
-  if (w.cout <= 208 && n208) {
-    if (staged_up && single_acc) LB_CONV_CASE_ACC(208, 1, false)
-    if (staged_up) LB_CONV_CASE_UP(208, 1)
-    if (single_acc) LB_CONV_CASE_ACC(208, 0, false)
-    LB_CONV_CASE(208)
-  }
-  if (w.cout <= 256) {
-    if (staged_up && w.cout > 208 && single_acc) LB_CONV_CASE_ACC(256, 1, false)
-    if (staged_up && w.cout > 208) LB_CONV_CASE_UP(256, 1)
-    if (single_acc) LB_CONV_CASE_ACC(256, 0, false)
-    LB_CONV_CASE(256)
-  }
+  if (w.cout <= 208 && n208) LB_CONV_CASE(208)
+  if (w.cout <= 256) LB_CONV_CASE(256)
 #undef LB_CONV_CASE
 #undef LB_CONV_CASE_UP
-#undef LB_CONV_CASE_ACC
   return fail("convolutions with more than 256 output channels are not built");
 }
 
@@ -1309,8 +1193,7 @@ int lb_backbone_forward(const LbBackboneWeights* w, const float* images, int N, 
   // FPN                                                                             [resnet_fpn.py:107-116]
   // The x2 bilinear upsampling of the coarser level is gathered inside the lateral 1x1 convolution's epilogue (default).
   // LOFTR_B200_FUSED_UPSAMPLE=0 runs it as a separate bandwidth kernel into a buffer that is dead at that point
-  // (m2 / m1 are only written two launches later) and adds it through the residual path -- measured slower
-  // (l1_outconv: 487 + 1079 us vs 1244 us fused; profiles/r2f_launches_step_separate_upsample.csv).
+  // (m2 / m1 are only written two launches later) and adds it through the residual path.
   static int fused_up = -1;
   if (fused_up < 0) {
     const char* e = getenv("LOFTR_B200_FUSED_UPSAMPLE");

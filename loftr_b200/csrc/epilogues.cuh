@@ -1,5 +1,5 @@
 // Epilogue functors for gemm_split_kernel.  Each one is the fused tail of a reference op group
-// (SURVEY.md §2a G1-G7): the thread that owns accumulator row r (TMEM lane r) applies the
+// (SURVEY.md §2a G1-G7): the thread that owns accumulator row r applies the
 // elementwise / row-wise work that the reference runs as separate eager kernels.
 #pragma once
 #include <cuda_fp16.h>
@@ -19,15 +19,14 @@ __device__ __forceinline__ float ex2_approx(float x) {
 __device__ __forceinline__ float exp_fast(float x) { return ex2_approx(x * kLog2e); }
 // elu(x) + 1 = x + 1 (x > 0) | exp(x) (x <= 0): the feature map of the linear attention (linear_attention.py:7-8).
 // Branch-free: the exponential is always evaluated (ex2.approx of min(x, 0) * log2 e, relative error ~1e-6, the level
-// of the split-precision GEMMs around it) and selected.  expf() compiled to a guarded slow path per element and was
-// 25 % of the k|v projection kernel's samples (profiles/r3a_*).
+// of the split-precision GEMMs around it) and selected.  expf() compiles to a guarded slow path per element.
 __device__ __forceinline__ float elu_plus1(float x) {
   const float e = exp_fast(fminf(x, 0.f));
   return x > 0.f ? x + 1.f : e;
 }
 
 __device__ __forceinline__ int epi_tid() { return threadIdx.x - kEpiWarp0 * 32; }   // 0..255
-__device__ __forceinline__ int epi_row() { return epi_tid() & 127; }                  // accumulator row (TMEM lane)
+__device__ __forceinline__ int epi_row() { return epi_tid() & 127; }                  // accumulator row
 __device__ __forceinline__ int epi_half() { return epi_tid() >> 7; }                  // column half of the tile
 __device__ __forceinline__ void epi_bar_sync() { epi_group_sync(); }
 
@@ -70,13 +69,15 @@ __device__ __forceinline__ void store_f32x32(float* p, const float (&x)[32]) {
   for (int j = 0; j < 8; ++j) q[j] = make_float4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
 }
 
-__device__ __forceinline__ void load_acc32(uint32_t tmem_acc, int col, float (&x)[32]) {
-  uint32_t v[32];
-  const uint32_t lane_base = static_cast<uint32_t>(((epi_tid() >> 5) & 3) * 32) << 16;  // warp%4 owns 32 lanes
-  tmem_ld32(tmem_acc + col + lane_base, v);
-  tmem_ld_wait();
+// 32 consecutive fp32 accumulator columns of this thread's row (acc_row: shared-memory address of the staged row)
+__device__ __forceinline__ void load_acc32(uint32_t acc_row, int col, float (&x)[32]) {
+  const uint32_t a = acc_row + static_cast<uint32_t>(col) * 4u;
 #pragma unroll
-  for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(v[j]);
+  for (int j = 0; j < 8; ++j)
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                 : "=f"(x[4 * j]), "=f"(x[4 * j + 1]), "=f"(x[4 * j + 2]), "=f"(x[4 * j + 3])
+                 : "r"(a + 16u * j)
+                 : "memory");
 }
 
 __device__ __forceinline__ void load_planes32(const __half* hp, const __half* lp, float (&x)[32]) {
@@ -96,20 +97,6 @@ __device__ __forceinline__ void load_planes32(const __half* hp, const __half* lp
   }
 }
 
-
-// two 32-column groups (e.g. main and correction accumulator) with ONE wait: one exposed TMEM latency instead of two
-__device__ __forceinline__ void load_acc32_pair(uint32_t tmem_acc, int col_a, int col_b, float (&x)[32], float (&y)[32]) {
-  uint32_t v[32], w[32];
-  const uint32_t lane_base = static_cast<uint32_t>(((epi_tid() >> 5) & 3) * 32) << 16;
-  tmem_ld32(tmem_acc + col_a + lane_base, v);
-  tmem_ld32(tmem_acc + col_b + lane_base, w);
-  tmem_ld_wait();
-#pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    x[j] = __uint_as_float(v[j]);
-    y[j] = __uint_as_float(w[j]);
-  }
-}
 
 // ------------------------------------------------------------------------------------------------
 // Coalesced epilogue I/O.  An epilogue thread owns one accumulator ROW, so a warp-wide 16-byte store of "my row's
@@ -392,7 +379,7 @@ struct EpiActStore {
     int elu_cols;            // columns [0, elu_cols) get elu+1
     const uint8_t* rowmask;  // optional [batches*M] (1 = valid)
     float acc_scale;         // 2^-e: undoes the power-of-two pre-scaling of the weight planes (exact)
-    int skip;                // probe mode (LOFTR_B200_PROBE_NULL_EPI, lb_gemm_split only): 1 = drain nothing, 2 = TMEM loads only
+    int skip;                // probe mode (LOFTR_B200_PROBE_NULL_EPI, lb_gemm_split only): 1 = drain nothing, 2 = accumulator loads only
     OutMaps om;              // om.use & 2: fp32 output through TMA stores
   };
   static constexpr int kSmemBytes = kEpiScratchBytes;
@@ -403,7 +390,7 @@ struct EpiActStore {
   __device__ void item_begin(int, int, int) {}
   __device__ void item_end(int, int, int) {}
   __device__ void prefetch(int, int, int) {}
-  __device__ void tile(uint32_t tmem_acc, int batch, int m0, int n0) {
+  __device__ void tile(uint32_t acc_row, int batch, int m0, int n0) {
     if (p.skip == 1) return;
     const int r = m0 + epi_row();
     const bool row_ok = r < s.M;
@@ -416,7 +403,7 @@ struct EpiActStore {
       const int col = n0 + c * 32;
       if (col >= s.N) break;  // warp-uniform
       float x[32];
-      load_acc32(tmem_acc, c * 32, x);
+      load_acc32(acc_row, c * 32, x);
       if (p.skip == 2) {   // keep the loads alive without storing
         float acc = 0.f;
 #pragma unroll
@@ -480,7 +467,7 @@ struct EpiKv {
   __device__ void item_begin(int, int, int) {}
   __device__ void item_end(int, int, int) {}
   __device__ void prefetch(int, int, int) {}
-  __device__ void tile(uint32_t tmem_acc, int batch, int m0, int n0) {
+  __device__ void tile(uint32_t acc_row, int batch, int m0, int n0) {
     const int t = epi_tid();
     const int row = epi_row();
     const int half = epi_half();
@@ -495,7 +482,7 @@ struct EpiKv {
     for (int j = 0; j < kHeads; ++j) {
       {  // stage this head's K (column half 0) / V (column half 1) columns of my row
         float x[32];
-        load_acc32(tmem_acc, (half * kHeads + j) * 32, x);
+        load_acc32(acc_row, (half * kHeads + j) * 32, x);
 #pragma unroll
         for (int i = 0; i < 32; ++i) x[i] *= p.acc_scale;
         if (half == 0) {
@@ -600,7 +587,7 @@ struct EpiAttn {
   }
   __device__ void item_end(int, int, int) {}
   __device__ void prefetch(int, int, int) {}
-  __device__ void tile(uint32_t tmem_acc, int batch, int m0, int) {
+  __device__ void tile(uint32_t acc_row, int batch, int m0, int) {
     const int r = m0 + epi_row();
     const bool row_ok = r < s.M;
     const long grow = static_cast<long>(batch) * s.M + r;
@@ -610,7 +597,7 @@ struct EpiAttn {
 #pragma unroll 1
     for (int c = c_begin; c < c_begin + BLOCK_N / 64; ++c) {
       float q[32];
-      load_acc32(tmem_acc, c * 32, q);
+      load_acc32(acc_row, c * 32, q);
       const float* kvh = sKV + c * kPer;   // head = column group
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
@@ -711,7 +698,7 @@ struct EpiLayerNorm {
     epi_bar_sync();
     return make_float2(u.x + v.x, u.y + v.y);
   }
-  __device__ void tile(uint32_t tmem_acc, int batch, int m0, int) {
+  __device__ void tile(uint32_t acc_row, int batch, int m0, int) {
     const int r = m0 + epi_row();
     const bool row_ok = r < s.M;
     const long grow = static_cast<long>(batch) * s.M + r;
@@ -723,7 +710,7 @@ struct EpiLayerNorm {
 #pragma unroll 1
     for (int c = c_begin; c < c_end; ++c) {
       float x[32];
-      load_acc32(tmem_acc, c * 32, x);
+      load_acc32(acc_row, c * 32, x);
       if (c == c_begin) shift = x[0] * p.acc_scale;
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
@@ -759,7 +746,7 @@ struct EpiLayerNorm {
                             row_ok ? p.res_lo + grow * p.ld_res_pl + c * 32 : nullptr, rh, rl);
 #endif
       float x[32];
-      load_acc32(tmem_acc, c * 32, x);
+      load_acc32(acc_row, c * 32, x);
 #pragma unroll
       for (int j4 = 0; j4 < 8; ++j4) {
         const float4 g4 = __ldg(reinterpret_cast<const float4*>(p.gamma + c * 32) + j4);
@@ -833,7 +820,7 @@ struct EpiPlanes {
   __device__ void item_begin(int, int, int) {}
   __device__ void item_end(int, int, int) {}
   __device__ void prefetch(int, int, int) {}
-  __device__ void tile(uint32_t tmem_acc, int batch, int m0, int n0) {
+  __device__ void tile(uint32_t acc_row, int batch, int m0, int n0) {
     const int r = m0 + epi_row();
     const bool row_ok = r < s.M;
     const long grow = static_cast<long>(batch) * s.M + r;
@@ -845,7 +832,7 @@ struct EpiPlanes {
       const int col = n0 + c * 32;
       if (col >= s.N) break;
       float x[32];
-      load_acc32(tmem_acc, c * 32, x);
+      load_acc32(acc_row, c * 32, x);
 #pragma unroll
       for (int j = 0; j < 32; ++j) x[j] *= p.acc_scale;
       if (p.relu) {
@@ -891,7 +878,8 @@ struct EpiPlanes {
 // written as NHWC fp16 planes (the next convolution's A operand) and / or NHWC fp32.
 //
 // kUpMode selects the FPN merge: 0 = none (every other layer: no upsample code, leanest registers), 1 = staged window,
-// 2 = per-thread global gathers (any shape).
+// 2 = per-thread global gathers (any shape).  The engine dispatches 0 and 2: the staged window's shared memory does
+// not fit beside the TMA ring and the accumulator staging of gemm_split_kernel.
 // kUpMode = 1 (the two FPN lateral 1x1 convolutions): the 6 x 10 source pixels whose bilinear footprints cover the
 // 8 x 16 output tile are fetched ONCE per tile by TMA into shared memory (boxes of 200 / 2 x 136 channels: the pixel
 // stride of 100 / 68 words keeps the quarter-warp LDS.128 conflict-free) while the tile's MMAs run; the four
@@ -901,10 +889,7 @@ struct UpMaps {
   CUtensorMap hi, lo;   // upsample source planes [batches, up_h, up_w, C], unswizzled boxes (kUpBoxC, 10, 6, 1)
 };
 constexpr int kUpW = 10, kUpH = 6;
-// kDualAcc mirrors the kernel's kDual: the 3x3 layers (K up to 2304) keep the correction products in a second
-// accumulator; the 1x1 layers (K <= 256: at most 48 MMAs per output) use one accumulator, which halves their TMEM
-// reads and leaves room for two TMEM stages at N = 208 / 256 (their epilogue then overlaps the next tile's MMAs).
-template <int BLOCK_N, int kUpMode = 0, bool kDualAcc = true>
+template <int BLOCK_N, int kUpMode = 0>
 struct EpiConv {
   static constexpr bool kUp = kUpMode == 1;      // staged window
   static constexpr bool kUpAny = kUpMode != 0;
@@ -1041,7 +1026,7 @@ struct EpiConv {
         }
     }
   }
-  __device__ void tile(uint32_t tmem_acc, int batch, int m0, int n0) {
+  __device__ void tile(uint32_t acc_row, int batch, int m0, int n0) {
     if (s.n_tiles > 1) {
       stage_affine(n0);
       epi_bar_sync();
@@ -1102,14 +1087,7 @@ struct EpiConv {
         warp_issue_planes32(ok ? p.res_hi + pix * p.res_ld + col : nullptr, ok ? p.res_lo + pix * p.res_ld + col : nullptr, rh, rl);
 #endif
       float v[32];
-      if constexpr (kDualAcc) {  // dual accumulator: add the correction products (hi*lo + lo*hi), see gemm_split.cuh
-        float corr[32];
-        load_acc32_pair(tmem_acc, c * 32, BLOCK_N + c * 32, v, corr);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] += corr[j];
-      } else {
-        load_acc32(tmem_acc, c * 32, v);
-      }
+      load_acc32(acc_row, c * 32, v);
 #pragma unroll
       for (int j = 0; j < 32; ++j) v[j] = fmaf(v[j], s_scale[c * 32 + j], s_shift[c * 32 + j]);
       if (nvalid == 32) {
@@ -1126,8 +1104,7 @@ struct EpiConv {
           for (int j = 0; j < 32; ++j) v[j] += r[j];
         }
         if (kUpAny && p.up_hi) {
-          // the four bilinear neighbours: plain per-thread loads (two rounds of two neighbours); routing these gathers
-          // through the transposer cost more than it saved (l1_out: 1.82 ms vs 1.31 ms, profiles/r2_*)
+          // the four bilinear neighbours: plain per-thread loads (two rounds of two neighbours)
           if (ok) {
             // kUp: the staged window (box = column / 128 when the tile spans two boxes), else the global planes
             const __half* uh = p.up_hi + col;
@@ -1254,7 +1231,7 @@ struct EpiKvProj {
   __device__ void item_begin(int, int, int) {}
   __device__ void item_end(int, int, int) {}
   __device__ void prefetch(int, int, int) {}
-  __device__ void tile(uint32_t tmem_acc, int batch, int m0, int n0) {
+  __device__ void tile(uint32_t acc_row, int batch, int m0, int n0) {
     const int r = m0 + epi_row();
     const bool row_ok = r < s.M;
     float mk = row_ok ? 1.f : 0.f;
@@ -1265,7 +1242,7 @@ struct EpiKvProj {
 #pragma unroll 1
     for (int c = c_begin; c < c_begin + 4; ++c) {
       float x[32];
-      load_acc32(tmem_acc, c * 32, x);
+      load_acc32(acc_row, c * 32, x);
 #pragma unroll
       for (int j = 0; j < 32; ++j) x[j] *= p.acc_scale;
       if (is_k) {
@@ -1346,7 +1323,7 @@ struct EpiScoreLse {
       epi_bar_sync();
     }
   }
-  __device__ void tile(uint32_t tmem_acc, int batch, int m0, int n0) {
+  __device__ void tile(uint32_t acc_row, int batch, int m0, int n0) {
     const int t = epi_tid();
     const int w = t >> 5;        // 0..7
     const int q = w & 3;         // row quarter
@@ -1373,7 +1350,7 @@ struct EpiScoreLse {
     for (int c = c_begin; c < c_begin + BLOCK_N / 64; ++c) {
       if (n0 + c * 32 >= s.N) break;
       float z[32];
-      load_acc32(tmem_acc, c * 32, z);
+      load_acc32(acc_row, c * 32, z);
 #pragma unroll
       for (int j = 0; j < 32; ++j) z[j] *= p.scale;
 
@@ -1480,7 +1457,7 @@ struct EpiConfStore {
   __device__ void item_begin(int, int, int) {}
   __device__ void item_end(int, int, int) {}
   __device__ void prefetch(int, int, int) {}
-  __device__ void tile(uint32_t tmem_acc, int batch, int m0, int n0) {
+  __device__ void tile(uint32_t acc_row, int batch, int m0, int n0) {
     const int t = epi_tid();
     for (int j = t; j < BLOCK_N; j += kEpiThreads) {
       const int col = n0 + j;
@@ -1498,7 +1475,7 @@ struct EpiConfStore {
       const int col = n0 + c * 32;
       if (col >= s.N) break;
       float z[32];
-      load_acc32(tmem_acc, c * 32, z);
+      load_acc32(acc_row, c * 32, z);
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const float ct = s_ct[c * 32 + j];
@@ -1578,7 +1555,7 @@ struct EpiScoreArgmax {
     }
     epi_bar_sync();
   }
-  __device__ void tile(uint32_t tmem_acc, int batch, int m0, int n0) {
+  __device__ void tile(uint32_t acc_row, int batch, int m0, int n0) {
     const int t = epi_tid();
     const int q = (t >> 5) & 3;
     const int lane = t & 31;
@@ -1596,7 +1573,7 @@ struct EpiScoreArgmax {
     for (int c = c_begin; c < c_begin + BLOCK_N / 64; ++c) {
       if (n0 + c * 32 >= s.N) break;
       float z[32];
-      load_acc32(tmem_acc, c * 32, z);
+      load_acc32(acc_row, c * 32, z);
 #pragma unroll
       for (int j = 0; j < 32; ++j) z[j] *= sa;
       // row direction: thread-local, strict '>' keeps the first (smallest j) maximum

@@ -8,16 +8,19 @@
 // Precision: the reference computes these products in fp32.  The mconf tolerance (rtol 1e-3 on logits
 // of magnitude ~100) rules out single-pass fp16/bf16/tf32 operands (SURVEY.md §7 hard part 1), so each
 // operand lives in HBM as two fp16 planes, x = hi + lo (|lo| <= ulp(hi)/2), and every k-step issues
-// three tcgen05.mma (hi*hi + hi*lo + lo*hi) into one fp32 TMEM accumulator.  The dropped lo*lo term is
+// three wgmma (hi*hi + hi*lo + lo*hi) into one fp32 register accumulator.  The dropped lo*lo term is
 // <= 2^-22 relative.
 //
-// Structure (one persistent CTA per SM, 384 threads):
-//   warp 0    : TMA producer    (global -> 128B-swizzled smem ring, 4 tiles per stage)
-//   warp 1    : MMA issuer      (one elected lane, tcgen05.mma cta_group::1, M=128, N=BLOCK_N, K=16)
-//   warp 2    : TMEM allocator
-//   warps 4-11: epilogue        (tcgen05.ld: thread t owns accumulator row t%128 and the column half t/128;
-//                                two warps per SM sub-partition hide the TMEM / MUFU / shuffle latencies)
-// The fp32 accumulator is double buffered in TMEM so the epilogue of tile i overlaps the MMAs of tile i+1.
+// Structure (one persistent CTA per SM, 288 threads: with one CTA per SM every thread may hold up to 224 registers,
+// room for the 128-register accumulator next to the epilogue's working set):
+//   warps 0-7  : two consumer warpgroups.  Warpgroup h issues the wgmma of the tile's column half h (M = 128 as two
+//                m64 instructions, N = BLOCK_N / 2, K = 16), stages its fp32 accumulator in shared memory (row-major,
+//                padded rows) and then runs the epilogue on it: thread t owns accumulator row t%128 and column half
+//                t/128.  The staging area aliases the TMA ring, so the producer starts the next tile's loads only
+//                once the epilogue has released it.
+//   warp 8     : TMA producer    (global -> 128B-swizzled smem ring, 4 tiles per stage)
+// Everything between the first wgmma of a tile and its last wait_group is warpgroup-uniform (no per-lane branches,
+// every consumer thread arrives on the ring's empty barriers): otherwise ptxas serialises the asynchronous MMAs.
 #pragma once
 #include "ptx.cuh"
 
@@ -31,10 +34,11 @@ constexpr int kBlockM = 128;
 // as many, half as large stages in the same shared memory -> deeper TMA pipeline)
 constexpr int kBlockK = LB_BLOCK_K;
 static_assert(kBlockK == 64 || kBlockK == 32, "supported k-block sizes");
-constexpr int kUmmaK = 16;
-constexpr int kGemmThreads = 384;
+constexpr int kMmaK = 16;
+constexpr int kGemmThreads = 288;
 constexpr int kEpiThreads = 256;  // two epilogue warpgroups: rows x {left, right} half of the tile's columns
-constexpr int kEpiWarp0 = 4;
+constexpr int kEpiWarp0 = 0;
+constexpr int kProducerWarp = 8;
 // named barrier 1 over the 256 epilogue threads (also used by the epilogues themselves)
 __device__ __forceinline__ void epi_group_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
@@ -75,130 +79,84 @@ struct GemmShape {
 };
 
 // K-major operand tile descriptor for the configured k-block (128-byte or 64-byte swizzle rows).
-__device__ __forceinline__ uint64_t umma_desc_k(uint32_t smem_addr) {
-  return kBlockK == 64 ? umma_desc_k_sw128(smem_addr) : umma_desc_k_sw64(smem_addr);
+__device__ __forceinline__ uint64_t desc_k(uint32_t smem_addr) {
+  return kBlockK == 64 ? wgmma_desc_k_sw128(smem_addr) : wgmma_desc_k_sw64(smem_addr);
 }
-// power of two >= x (TMEM allocations)
-constexpr uint32_t pow2_at_least(uint32_t x) { return x <= 32 ? 32 : x <= 64 ? 64 : x <= 128 ? 128 : x <= 256 ? 256 : 512; }
 
-// Shared-memory ring.  kPair (cta_group::2): a CTA stages its own 128 rows of A and only its HALF of the B tile.
-// kEpiBytes = the epilogue's own area: an epilogue that stages a lot (EpiConv<., true>) gets a shallower ring.
-template <int BLOCK_N, bool kPair = false, int kEpiBytes = 0>
+// Shared memory: [TMA ring | accumulator staging (aliased)][epilogue area][mbarriers].
+// The staging tile is 128 rows of BLOCK_N + 4 fp32: a row stride of an odd multiple of 16 bytes keeps the epilogue's
+// row-per-lane 16-byte reads free of bank conflicts.  +32 floats: an epilogue's last 32-column group may run past N.
+template <int BLOCK_N, int kEpiBytes = 0>
 struct GemmSmem {
-  static constexpr int kATile = kBlockM * kBlockK * 2;                       // 16 KB per plane
-  static constexpr int kBTile = (kPair ? BLOCK_N / 2 : BLOCK_N) * kBlockK * 2;  // per plane
-  static constexpr int kStageBytes = 2 * kATile + 2 * kBTile;                // hi + lo of A and B
-  static constexpr int kBarBytes = 256;    // barriers + TMEM slot, placed behind the epilogue area
+  static constexpr int kATile = kBlockM * kBlockK * 2;          // 16 KB per plane
+  static constexpr int kBTile = BLOCK_N * kBlockK * 2;          // per plane
+  static constexpr int kStageBytes = 2 * kATile + 2 * kBTile;   // hi + lo of A and B
+  static constexpr int kBarBytes = 256;
+  static constexpr int kAccStride = BLOCK_N + 4;                // floats
+  static constexpr int kAccBytes = (kBlockM * kAccStride + 32) * 4;
   static constexpr int kFit = (232448 - kBarBytes - kEpiBytes) / kStageBytes;
-  static constexpr int kWant = (192 * 1024) / kStageBytes;                   // 2 (96 KB) / 3 (64 KB) / 4 (48 KB)
+  static constexpr int kWant = (192 * 1024) / kStageBytes;      // 2 (96 KB) / 3 (64 KB) / 4 (48 KB)
   static constexpr int kStages = kFit < kWant ? kFit : kWant;
   static_assert(kStages >= 2, "the TMA ring needs two stages");
-  static constexpr int kRingBytes = kStages * kStageBytes;
+  static constexpr int kRingBytes = kStages * kStageBytes > kAccBytes ? kStages * kStageBytes : kAccBytes;
 };
 
-// TMEM layout.  kDual: the two correction products (hi*lo, lo*hi) accumulate into a SECOND accumulator that the
-// epilogue adds once.  tcgen05 rounds the fp32 accumulator by truncation at every MMA, so with a single accumulator
-// a K-long contraction suffers 3K/16 biased roundings at full magnitude; with the split only the K/16 hi*hi adds do
-// (the corrections are ~2^-11 of the result, their rounding is negligible).  Used for the long-K convolutions.
-// Columns per stage = BLOCK_N (single) or 2*BLOCK_N (dual); two stages whenever they fit in 512 columns.
-template <int BLOCK_N, bool kDual>
-struct AccLayout {
-  static constexpr int kColsPerStage = kDual ? 2 * BLOCK_N : BLOCK_N;
-  static constexpr int kStages = (2 * kColsPerStage <= 512) ? 2 : 1;
-  // the epilogues read whole 32-column groups: the last group of a stage may run up to 31 columns past it
-  static_assert(kStages * kColsPerStage + 31 <= 512 || BLOCK_N % 32 == 0, "accumulator layout exceeds TMEM");
-  static constexpr uint32_t kTmemCols = pow2_at_least(kStages * kColsPerStage);
-};
-
-// Execution modes (kMode):
-//   0  single CTA per tile (cta_group::1).
-//   1  cluster of two CTAs on adjacent row tiles; each fetches half of the B tile and TMA-multicasts it to both
-//      (cta_group::1 MMAs).  Bit-identical, measured NOT faster: the kernels are bound by bytes delivered per SM.
-//   2  CTA pair with tcgen05.mma.cta_group::2: the leader (even CTA) issues M = 256 MMAs over both CTAs' TMEM; each
-//      CTA stages its own A rows and only HALF of B, so the L2 -> SM bytes per MMA drop from A + B to A + B/2.
-//      Barrier protocol (CUTLASS/DeepGEMM 2-SM scheme): both producers' TMA bytes are credited to the LEADER's full
-//      barrier (count 2: the leader arms expect_tx for both CTAs, the peer arrives remotely); the leader's
-//      tcgen05.commit multicasts to both CTAs' empty / tmem_full barriers; one thread per CTA arrives (remotely for
-//      the peer) on the leader's tmem_empty barrier once its epilogue has drained the accumulator.
-//
-// Epilogue contract (all methods are called by the 256 epilogue threads only):
+// Epilogue contract (all methods are called by the 256 consumer threads only):
 //   struct Params;                               // trivially copyable, passed by value to the kernel
 //   static constexpr int kSmemBytes;             // extra dynamic smem the epilogue wants
 //   __device__ Epi(const Params&, uint8_t* smem, const GemmShape&);
 //   __device__ void item_begin(int batch, int m0, int chunk);
-//   __device__ void prefetch(int batch, int m0, int n0);   // called BEFORE the wait for the tile's accumulator: the
-//                                                          // place to pull residual / bias data towards L2
-//   __device__ void tile(uint32_t tmem_acc, int batch, int m0, int n0);   // tmem_acc: column base of this
-//                                                                         // tile's accumulator (lane field 0)
+//   __device__ void prefetch(int batch, int m0, int n0);   // called before the tile's main loop: the place to pull
+//                                                          // residual / bias data towards L2
+//   __device__ void tile(uint32_t acc_row, int batch, int m0, int n0);   // acc_row: shared-memory address of this
+//                                                                        // thread's staged accumulator row
 //   __device__ void item_end(int batch, int m0, int chunk);
-template <int BLOCK_N, class Epi, bool kDual = false, int kMode = 0>
+template <int BLOCK_N, class Epi>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                   const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
                   const __grid_constant__ CUtensorMap tm_ar_hi, const __grid_constant__ CUtensorMap tm_ar_lo,
                   const __grid_constant__ CUtensorMap tm_br_hi, const __grid_constant__ CUtensorMap tm_br_lo,
                   const GemmShape shape, const __grid_constant__ typename Epi::Params epi_params) {
-  constexpr bool kPair = kMode == 2;
-  constexpr bool kMcast = kMode == 1;
-  constexpr int kCluster = kMode == 0 ? 1 : 2;
-  using S = GemmSmem<BLOCK_N, kPair, Epi::kSmemBytes>;
+  using S = GemmSmem<BLOCK_N, Epi::kSmemBytes>;
+  constexpr int kN = BLOCK_N / 2;   // columns per consumer warpgroup
+  static_assert(kN % 8 == 0, "wgmma N must be a multiple of 8");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // Layout: [TMA ring][epilogue area][mbarriers + TMEM slot].  The swizzled tiles (ring, TMA-store staging) need a
-  // 1024-byte aligned base.  With no static shared memory the dynamic window starts 1024-aligned (checked below: a
-  // misaligned base traps instead of corrupting tiles), so nothing is spent on padding; and the pointers stay plain
-  // offsets of the __shared__ array -- through an integer round trip the compiler loses the address space and every
-  // epilogue smem access becomes a generic LD/ST (measured: stall_lg, 3x slower).
-  uint8_t* smem = smem_raw;
-  uint8_t* ring = smem;
-  uint8_t* epi_smem = smem + S::kRingBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kRingBytes + Epi::kSmemBytes);
+  // The swizzled tiles (ring, TMA-store staging) need a 1024-byte aligned base.  With no static shared memory the
+  // dynamic window starts 1024-aligned (checked below: a misaligned base traps instead of corrupting tiles); the
+  // pointers stay plain offsets of the __shared__ array -- through an integer round trip the compiler loses the
+  // address space and every epilogue smem access becomes a generic LD/ST.
+  uint8_t* ring = smem_raw;
+  uint8_t* epi_smem = smem_raw + S::kRingBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_raw + S::kRingBytes + Epi::kSmemBytes);
   uint64_t* empty_bar = full_bar + S::kStages;
-  uint64_t* tmem_full = empty_bar + S::kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint64_t* acc_free = empty_bar + S::kStages;
   static_assert(Epi::kSmemBytes % 16 == 0, "epilogue area must keep the barriers aligned");
   if ((smem_u32(smem_raw) & 1023u) != 0) asm volatile("trap;");
 
-  const int warp = threadIdx.x >> 5;
+  // warp index broadcast from lane 0: provably warp-uniform, so the role branches below are not divergent paths
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
-  using AL = AccLayout<BLOCK_N, kDual>;
-  constexpr uint32_t kTmemCols = AL::kTmemCols;
-  const int crank = kCluster > 1 ? static_cast<int>(cluster_ctarank()) : 0;
-  const bool leader = crank == 0;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&tm_a_hi);
     tma_prefetch_desc(&tm_a_lo);
     tma_prefetch_desc(&tm_b_hi);
     tma_prefetch_desc(&tm_b_lo);
   }
-  if (warp == 1 && lane == 0) {
+  if (warp == 0 && lane == 0) {
     for (int s = 0; s < S::kStages; ++s) {
-      mbar_init(&full_bar[s], kPair ? 2 : 1);          // pair: one arrival per CTA's producer (on the leader's copy)
-      mbar_init(&empty_bar[s], kMcast ? 2 : 1);        // multicast mode: both CTAs' MMAs must have read the slot
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], kEpiThreads);   // every consumer thread arrives (keeps the MMA window uniform)
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], kPair ? 2 : kEpiThreads);  // pair: one elected thread per CTA
-    }
+    mbar_init(acc_free, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if (kPair) {
-      tmem_alloc_2sm(tmem_slot, kTmemCols);
-    } else {
-      tmem_alloc(tmem_slot, kTmemCols);
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if (kCluster > 1) cluster_sync_all();   // peer barriers are initialised before anyone signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // Programmatic dependent launch (engine.cu sets the launch attribute unless LOFTR_B200_PDL=0; without it both
   // instructions are no-ops): the NEXT kernel of the stream may be scheduled as soon as every CTA of this grid got
-  // here -- its CTAs take over SMs as ours exit and run their own set-up (barriers, TMEM allocation, descriptor
-  // prefetch) -- while everything below this line first waits until the PREVIOUS grid has completed and flushed.
+  // here -- its CTAs take over SMs as ours exit and run their own set-up (barriers, descriptor prefetch) -- while
+  // everything below this line first waits until the PREVIOUS grid has completed and flushed.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
 
@@ -209,51 +167,35 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   constexpr int kRemBTile = S::kBTile / (kBlockK / kRemChannels);
   static_assert(kBlockK != 64 || (kTapBytes == 2 * kRemATile + 2 * kRemBTile && kTapBytes % 256 == 0 &&
                                   kRemBTile % 256 == 0), "remainder group layout");
-  // Work items.  Single CTA: (batch, m_tile, chunk).  Cluster: (batch, m_tile group, chunk); CTA rank r of the
-  // cluster takes m_tile = group * kCluster + r (a phantom tile past the end is loaded/multiplied but not emitted).
-  const int m_groups = (shape.m_tiles + kCluster - 1) / kCluster;
-  const int total_items = shape.batches * m_groups * shape.n_chunks;
-  const int first_item = blockIdx.x / kCluster;
-  const int item_step = gridDim.x / kCluster;
-  constexpr uint16_t kMcMask = static_cast<uint16_t>((1u << kCluster) - 1);
+  // work items (batch, m_tile, chunk), strided over the persistent CTAs
+  const int total_items = shape.batches * shape.m_tiles * shape.n_chunks;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ------------------------------------------------------------ TMA producer
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int item = first_item; item < total_items; item += item_step) {
+      uint32_t tiles = 0;
+      for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
         const int chunk = item % shape.n_chunks;
-        const int mt = ((item / shape.n_chunks) % m_groups) * kCluster + crank;
-        const int batch = item / (shape.n_chunks * m_groups);
+        const int mt = (item / shape.n_chunks) % shape.m_tiles;
+        const int batch = item / (shape.n_chunks * shape.m_tiles);
         const int nt_begin = chunk * shape.tiles_per_chunk;
         const int nt_end = min(nt_begin + shape.tiles_per_chunk, shape.n_tiles);
         for (int nt = nt_begin; nt < nt_end; ++nt) {
+          if (tiles > 0) mbar_wait(acc_free, (tiles - 1) & 1);   // the previous tile's staged accumulator is consumed
+          ++tiles;
           for (int kb = 0; kb < num_kb; ++kb) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
             uint8_t* st = ring + stage * S::kStageBytes;
             uint64_t* fb = &full_bar[stage];
             const bool rem_group = shape.conv.enabled && kb >= shape.conv.n_main;
-            int rem_t0 = 0, rem_nt = 0;
-            uint32_t stage_tx = S::kStageBytes;
-            if (rem_group) {
-              rem_t0 = (kb - shape.conv.n_main) * kRemTapsPerStage;
-              rem_nt = min(kRemTapsPerStage, shape.conv.taps - rem_t0);
-              stage_tx = static_cast<uint32_t>(rem_nt) * kTapBytes;
-            }
-            if (kPair) {
-              // both CTAs' bytes are credited to the leader's barrier
-              if (leader) {
-                mbar_arrive_expect_tx(fb, 2 * stage_tx);
-              } else {
-                mbar_arrive_remote(fb, 0);
-              }
-            } else {
-              mbar_arrive_expect_tx(fb, stage_tx);
-            }
             if (rem_group) {
               // ---- channel remainder: up to four taps, each a 16-channel box of A (hi, lo) and of the weights
               const ConvGeom& g = shape.conv;
+              const int rem_t0 = (kb - g.n_main) * kRemTapsPerStage;
+              const int rem_nt = min(kRemTapsPerStage, g.taps - rem_t0);
+              mbar_arrive_expect_tx(fb, static_cast<uint32_t>(rem_nt) * kTapBytes);
               const int ty = mt / g.tiles_w, tx = mt - ty * g.tiles_w;
               for (int t = 0; t < rem_nt; ++t) {
                 const int tap = rem_t0 + t;
@@ -262,65 +204,31 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                 const int y = ty * kConvTileH * g.stride + ky - g.pad;
                 uint8_t* base = st + t * kTapBytes;
                 const int c0 = g.cin_blocks * kBlockK;
-                if (kPair) {
-                  const int row0 = nt * BLOCK_N + crank * (BLOCK_N / 2);
-                  tma_load_4d_2sm(base, &tm_ar_hi, fb, c0, x, y, batch);
-                  tma_load_4d_2sm(base + kRemATile, &tm_ar_lo, fb, c0, x, y, batch);
-                  tma_load_3d_2sm(base + 2 * kRemATile, &tm_br_hi, fb, tap * kRemChannels, row0, 0);
-                  tma_load_3d_2sm(base + 2 * kRemATile + kRemBTile, &tm_br_lo, fb, tap * kRemChannels, row0, 0);
-                } else {
-                  tma_load_4d(base, &tm_ar_hi, fb, c0, x, y, batch);
-                  tma_load_4d(base + kRemATile, &tm_ar_lo, fb, c0, x, y, batch);
-                  tma_load_3d(base + 2 * kRemATile, &tm_br_hi, fb, tap * kRemChannels, nt * BLOCK_N, 0);
-                  tma_load_3d(base + 2 * kRemATile + kRemBTile, &tm_br_lo, fb, tap * kRemChannels, nt * BLOCK_N, 0);
-                }
+                tma_load_4d(base, &tm_ar_hi, fb, c0, x, y, batch);
+                tma_load_4d(base + kRemATile, &tm_ar_lo, fb, c0, x, y, batch);
+                tma_load_3d(base + 2 * kRemATile, &tm_br_hi, fb, tap * kRemChannels, nt * BLOCK_N, 0);
+                tma_load_3d(base + 2 * kRemATile + kRemBTile, &tm_br_lo, fb, tap * kRemChannels, nt * BLOCK_N, 0);
               }
-              if (++stage == S::kStages) {
-                stage = 0;
-                phase ^= 1;
-              }
-              continue;
-            }
-            // ---- A: this CTA's 128 rows (or 8 x 16 pixel patch shifted by the tap)
-            if (shape.conv.enabled) {
-              const ConvGeom& g = shape.conv;
-              const int tap = kb / g.cin_blocks, cb = kb - tap * g.cin_blocks;
-              const int ky = tap / g.taps_w, kx = tap - ky * g.taps_w;
-              const int ty = mt / g.tiles_w, tx = mt - ty * g.tiles_w;
-              const int x = tx * kConvTileW * g.stride + kx - g.pad;
-              const int y = ty * kConvTileH * g.stride + ky - g.pad;
-              if (kPair) {
-                tma_load_4d_2sm(st, &tm_a_hi, fb, cb * kBlockK, x, y, batch);
-                tma_load_4d_2sm(st + S::kATile, &tm_a_lo, fb, cb * kBlockK, x, y, batch);
-              } else {
+            } else {
+              mbar_arrive_expect_tx(fb, S::kStageBytes);
+              // ---- A: 128 rows (or an 8 x 16 pixel patch shifted by the tap)
+              if (shape.conv.enabled) {
+                const ConvGeom& g = shape.conv;
+                const int tap = kb / g.cin_blocks, cb = kb - tap * g.cin_blocks;
+                const int ky = tap / g.taps_w, kx = tap - ky * g.taps_w;
+                const int ty = mt / g.tiles_w, tx = mt - ty * g.tiles_w;
+                const int x = tx * kConvTileW * g.stride + kx - g.pad;
+                const int y = ty * kConvTileH * g.stride + ky - g.pad;
                 tma_load_4d(st, &tm_a_hi, fb, cb * kBlockK, x, y, batch);
                 tma_load_4d(st + S::kATile, &tm_a_lo, fb, cb * kBlockK, x, y, batch);
+              } else {
+                tma_load_3d(st, &tm_a_hi, fb, kb * kBlockK, mt * kBlockM, batch);
+                tma_load_3d(st + S::kATile, &tm_a_lo, fb, kb * kBlockK, mt * kBlockM, batch);
               }
-            } else if (kPair) {
-              tma_load_3d_2sm(st, &tm_a_hi, fb, kb * kBlockK, mt * kBlockM, batch);
-              tma_load_3d_2sm(st + S::kATile, &tm_a_lo, fb, kb * kBlockK, mt * kBlockM, batch);
-            } else {
-              tma_load_3d(st, &tm_a_hi, fb, kb * kBlockK, mt * kBlockM, batch);
-              tma_load_3d(st + S::kATile, &tm_a_lo, fb, kb * kBlockK, mt * kBlockM, batch);
-            }
-            // ---- B
-            const int bb = shape.b_batched ? batch : 0;
-            uint8_t* sb_hi = st + 2 * S::kATile;
-            uint8_t* sb_lo = sb_hi + S::kBTile;
-            if (kPair) {            // this CTA's half of the tile's rows, into its own shared memory
-              const int row0 = nt * BLOCK_N + crank * (BLOCK_N / 2);
-              tma_load_3d_2sm(sb_hi, &tm_b_hi, fb, kb * kBlockK, row0, bb);
-              tma_load_3d_2sm(sb_lo, &tm_b_lo, fb, kb * kBlockK, row0, bb);
-            } else if (kMcast) {    // this CTA's slice, delivered to every CTA of the cluster
-              constexpr int kSliceRows = BLOCK_N / kCluster;
-              constexpr int kSliceBytes = S::kBTile / kCluster;
-              tma_load_3d_mc(sb_hi + crank * kSliceBytes, &tm_b_hi, fb, kb * kBlockK, nt * BLOCK_N + crank * kSliceRows,
-                             bb, kMcMask);
-              tma_load_3d_mc(sb_lo + crank * kSliceBytes, &tm_b_lo, fb, kb * kBlockK, nt * BLOCK_N + crank * kSliceRows,
-                             bb, kMcMask);
-            } else {
-              tma_load_3d(sb_hi, &tm_b_hi, fb, kb * kBlockK, nt * BLOCK_N, bb);
-              tma_load_3d(sb_lo, &tm_b_lo, fb, kb * kBlockK, nt * BLOCK_N, bb);
+              // ---- B
+              const int bb = shape.b_batched ? batch : 0;
+              tma_load_3d(st + 2 * S::kATile, &tm_b_hi, fb, kb * kBlockK, nt * BLOCK_N, bb);
+              tma_load_3d(st + 2 * S::kATile + S::kBTile, &tm_b_lo, fb, kb * kBlockK, nt * BLOCK_N, bb);
             }
             if (++stage == S::kStages) {
               stage = 0;
@@ -330,148 +238,109 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer (pair mode: the leader CTA only)
-    if (lane == 0 && (!kPair || leader)) {
-      constexpr uint32_t idesc = umma_idesc_f16_f32(kPair ? 2 * kBlockM : kBlockM, BLOCK_N);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int item = first_item; item < total_items; item += item_step) {
-        const int chunk = item % shape.n_chunks;
-        const int nt_begin = chunk * shape.tiles_per_chunk;
-        const int nt_end = min(nt_begin + shape.tiles_per_chunk, shape.n_tiles);
-        for (int nt = nt_begin; nt < nt_end; ++nt) {
-          mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + acc * AL::kColsPerStage;
-          const uint32_t d_corr = kDual ? d_tmem + BLOCK_N : d_tmem;
-          for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            const uint32_t st = smem_u32(ring + stage * S::kStageBytes);
-            if (shape.conv.enabled && kb >= shape.conv.n_main) {
-              // remainder group: one K = 16 step per tap, 32-byte swizzle rows (kb > 0 here: always accumulate)
-              const int rem_t0 = (kb - shape.conv.n_main) * kRemTapsPerStage;
-              const int rem_nt = min(kRemTapsPerStage, shape.conv.taps - rem_t0);
-              for (int t = 0; t < rem_nt; ++t) {
-                const uint32_t base = st + t * kTapBytes;
-                const uint64_t ra_hi = umma_desc_k_sw32(base);
-                const uint64_t ra_lo = umma_desc_k_sw32(base + kRemATile);
-                const uint64_t rb_hi = umma_desc_k_sw32(base + 2 * kRemATile);
-                const uint64_t rb_lo = umma_desc_k_sw32(base + 2 * kRemATile + kRemBTile);
-                if (kPair) {
-                  umma_f16_2sm(d_tmem, ra_hi, rb_hi, idesc, 1u);
-                  umma_f16_2sm(d_corr, ra_hi, rb_lo, idesc, 1u);
-                  umma_f16_2sm(d_corr, ra_lo, rb_hi, idesc, 1u);
-                } else {
-                  umma_f16(d_tmem, ra_hi, rb_hi, idesc, 1u);
-                  umma_f16(d_corr, ra_hi, rb_lo, idesc, 1u);
-                  umma_f16(d_corr, ra_lo, rb_hi, idesc, 1u);
-                }
-              }
-              if (kPair) {
-                umma_commit_2sm_mc(&empty_bar[stage], kMcMask);
-              } else if (kMcast) {
-                umma_commit_mc(&empty_bar[stage], kMcMask);
-              } else {
-                umma_commit(&empty_bar[stage]);
-              }
-              if (++stage == S::kStages) {
-                stage = 0;
-                phase ^= 1;
-              }
-              continue;
-            }
-            const uint64_t da_hi = umma_desc_k(st);
-            const uint64_t da_lo = umma_desc_k(st + S::kATile);
-            const uint64_t db_hi = umma_desc_k(st + 2 * S::kATile);
-            const uint64_t db_lo = umma_desc_k(st + 2 * S::kATile + S::kBTile);
-#pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-              // advance 16 fp16 = 32 bytes along K inside the 128B swizzle row: +2 in 16-byte units
-              const uint64_t adv = static_cast<uint64_t>(k * 2);
-              const uint32_t not_first = (kb | k) != 0 ? 1u : 0u;
-              if (kPair) {
-                umma_f16_2sm(d_tmem, da_hi + adv, db_hi + adv, idesc, not_first);
-                umma_f16_2sm(d_corr, da_hi + adv, db_lo + adv, idesc, kDual ? not_first : 1u);
-                umma_f16_2sm(d_corr, da_lo + adv, db_hi + adv, idesc, 1u);
-              } else {
-                umma_f16(d_tmem, da_hi + adv, db_hi + adv, idesc, not_first);
-                umma_f16(d_corr, da_hi + adv, db_lo + adv, idesc, kDual ? not_first : 1u);
-                umma_f16(d_corr, da_lo + adv, db_hi + adv, idesc, 1u);
-              }
-            }
-            if (kPair) {
-              umma_commit_2sm_mc(&empty_bar[stage], kMcMask);   // frees the slot in both CTAs
-            } else if (kMcast) {
-              umma_commit_mc(&empty_bar[stage], kMcMask);
-            } else {
-              umma_commit(&empty_bar[stage]);
-            }
-            if (++stage == S::kStages) {
-              stage = 0;
-              phase ^= 1;
-            }
-          }
-          if (kPair) {
-            umma_commit_2sm_mc(&tmem_full[acc], kMcMask);       // both CTAs' epilogues own half of the rows
-          } else {
-            umma_commit(&tmem_full[acc]);
-          }
-          if (++acc == AL::kStages) {
-            acc = 0;
-            acc_phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp >= kEpiWarp0) {
-    // ------------------------------------------------------------ epilogue
+  } else {
+    // ------------------------------------------------------------ consumer warpgroups: wgmma + epilogue
+    const int ct = threadIdx.x - kEpiWarp0 * 32;   // 0..255
+    const int h = ct >> 7;                          // column half of the tile
+    const int wt = ct & 127;                        // thread within the warpgroup
     Epi epi(epi_params, epi_smem, shape);
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int item = first_item; item < total_items; item += item_step) {
+    float acc[2][kN / 2];                           // rows [0, 64) and [64, 128) of this warpgroup's column half
+    float* stg = reinterpret_cast<float*>(ring);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
       const int chunk = item % shape.n_chunks;
-      const int mt = ((item / shape.n_chunks) % m_groups) * kCluster + crank;
-      const int batch = item / (shape.n_chunks * m_groups);
+      const int mt = (item / shape.n_chunks) % shape.m_tiles;
+      const int batch = item / (shape.n_chunks * shape.m_tiles);
       const int nt_begin = chunk * shape.tiles_per_chunk;
       const int nt_end = min(nt_begin + shape.tiles_per_chunk, shape.n_tiles);
-      const bool real = mt < shape.m_tiles;   // phantom row tile of an odd tail: consume, emit nothing
-      if (real) epi.item_begin(batch, mt * kBlockM, chunk);
+      epi.item_begin(batch, mt * kBlockM, chunk);
       for (int nt = nt_begin; nt < nt_end; ++nt) {
-        if (real) epi.prefetch(batch, mt * kBlockM, nt * BLOCK_N);
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-        if (real) epi.tile(tmem_base + acc * AL::kColsPerStage, batch, mt * kBlockM, nt * BLOCK_N);
-        tc_fence_before();
-        if (kPair) {
-          epi_group_sync();                                          // every thread of this CTA has drained TMEM
-          if (threadIdx.x == kEpiWarp0 * 32) mbar_arrive_remote(&tmem_empty[acc], 0);
-        } else {
-          mbar_arrive(&tmem_empty[acc]);
+        epi.prefetch(batch, mt * kBlockM, nt * BLOCK_N);
+        // a zeroed accumulator instead of a first MMA with scale-d = 0: the previous tile's values are dead after
+        // staging, so the epilogue does not have to keep them in registers
+#pragma unroll
+        for (int i = 0; i < kN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
+        int prev = -1;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t st = smem_u32(ring + stage * S::kStageBytes);
+          wgmma_fence();
+          if (shape.conv.enabled && kb >= shape.conv.n_main) {
+            // remainder group: one K = 16 step per tap, 32-byte swizzle rows (kb > 0 here: always accumulate)
+            const int rem_t0 = (kb - shape.conv.n_main) * kRemTapsPerStage;
+            const int rem_nt = min(kRemTapsPerStage, shape.conv.taps - rem_t0);
+            for (int t = 0; t < rem_nt; ++t) {
+              const uint32_t base = st + t * kTapBytes;
+              const uint32_t b_off = static_cast<uint32_t>(h * kN * kRemChannels * 2);
+#pragma unroll
+              for (int mh = 0; mh < 2; ++mh) {
+                const uint32_t a_off = static_cast<uint32_t>(mh * 64 * kRemChannels * 2);
+                const uint64_t ra_hi = wgmma_desc_k_sw32(base + a_off);
+                const uint64_t ra_lo = wgmma_desc_k_sw32(base + kRemATile + a_off);
+                const uint64_t rb_hi = wgmma_desc_k_sw32(base + 2 * kRemATile + b_off);
+                const uint64_t rb_lo = wgmma_desc_k_sw32(base + 2 * kRemATile + kRemBTile + b_off);
+                wgmma_f16<kN>(acc[mh], ra_hi, rb_hi, 1u);
+                wgmma_f16<kN>(acc[mh], ra_hi, rb_lo, 1u);
+                wgmma_f16<kN>(acc[mh], ra_lo, rb_hi, 1u);
+              }
+            }
+          } else {
+            const uint32_t b_off = static_cast<uint32_t>(h * kN * kBlockK * 2);
+#pragma unroll
+            for (int mh = 0; mh < 2; ++mh) {
+              const uint32_t a_off = static_cast<uint32_t>(mh * 64 * kBlockK * 2);
+              const uint64_t da_hi = desc_k(st + a_off);
+              const uint64_t da_lo = desc_k(st + S::kATile + a_off);
+              const uint64_t db_hi = desc_k(st + 2 * S::kATile + b_off);
+              const uint64_t db_lo = desc_k(st + 2 * S::kATile + S::kBTile + b_off);
+#pragma unroll
+              for (int k = 0; k < kBlockK / kMmaK; ++k) {
+                // advance 16 fp16 = 32 bytes along K inside the swizzle row: +2 in 16-byte units
+                const uint64_t adv = static_cast<uint64_t>(k * 2);
+                wgmma_f16<kN>(acc[mh], da_hi + adv, db_hi + adv, 1u);
+                wgmma_f16<kN>(acc[mh], da_hi + adv, db_lo + adv, 1u);
+                wgmma_f16<kN>(acc[mh], da_lo + adv, db_hi + adv, 1u);
+              }
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<1>();   // the previous k-block's MMAs are done: its slot may be refilled
+          if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+          prev = stage;
+          if (++stage == S::kStages) {
+            stage = 0;
+            phase ^= 1;
+          }
         }
-        if (++acc == AL::kStages) {
-          acc = 0;
-          acc_phase ^= 1;
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc[0]);
+        wgmma_fence_regs(acc[1]);
+        mbar_arrive(&empty_bar[prev]);
+        // ---- stage the accumulator (row-major) over the ring, once both warpgroups' MMAs have read it
+        epi_group_sync();
+        {
+          const int r0 = 16 * (wt >> 5) + ((wt & 31) >> 2);
+          const int c0 = h * kN + 2 * (wt & 3);
+#pragma unroll
+          for (int mh = 0; mh < 2; ++mh) {
+#pragma unroll
+            for (int j = 0; j < kN / 8; ++j) {
+              float* p = stg + (mh * 64 + r0) * S::kAccStride + c0 + 8 * j;
+              *reinterpret_cast<float2*>(p) = make_float2(acc[mh][4 * j], acc[mh][4 * j + 1]);
+              *reinterpret_cast<float2*>(p + 8 * S::kAccStride) = make_float2(acc[mh][4 * j + 2], acc[mh][4 * j + 3]);
+            }
+          }
         }
+        epi_group_sync();
+        epi.tile(smem_u32(stg + (ct & 127) * S::kAccStride), batch, mt * kBlockM, nt * BLOCK_N);
+        fence_proxy_async();   // staging reads / writes (generic proxy) before the next TMA writes into the ring
+        epi_group_sync();
+        if (ct == 0) mbar_arrive(acc_free);
       }
-      if (real) epi.item_end(batch, mt * kBlockM, chunk);
+      epi.item_end(batch, mt * kBlockM, chunk);
     }
     tma_store_wait_all();   // bulk stores issued by this thread (if any) have landed before the CTA may exit
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (kCluster > 1) cluster_sync_all();   // no CTA may exit (or free TMEM) while its peer can still touch it
-  if (warp == 2) {
-    tc_fence_after();
-    if (kPair) {
-      tmem_dealloc_2sm(tmem_base, kTmemCols);
-    } else {
-      tmem_dealloc(tmem_base, kTmemCols);
-    }
   }
 }
 

@@ -5,10 +5,11 @@
 // gemm_split_kernel, and a single-channel image cannot be im2col'ed by a tensor map (the tap stride would be 2 or 4
 // bytes).  So this kernel builds the A tile in software: per 8 x 16 output-pixel tile the 21 x 37 input patch is
 // staged in shared memory, every warp writes its rows of the [128 x 64] fp16 hi/lo operand tiles straight into the
-// 128-byte-swizzled K-major layout tcgen05.mma expects, and one thread issues the 12 MMAs (4 k-steps x (hi*hi + hi*lo +
-// lo*hi)) into one of two TMEM stages while all 8 warps run the epilogue of the previous tile (BN + ReLU + split,
-// TMA store of 2 x 16 pixel x 32 channel boxes).  The weights (128 x 49 fp32) are scaled by a power of two, split and
-// swizzled into shared memory once per CTA.  One persistent CTA per SM, 256 threads.
+// 128-byte-swizzled K-major layout wgmma expects, and each of the two warpgroups issues the wgmma of one 64-channel
+// half (rows 0-63 and 64-127 x 4 k-steps x (hi*hi + hi*lo + lo*hi)).  The accumulator is staged row-major in shared
+// memory and all 8 warps run the epilogue (BN + ReLU + split, TMA store of 2 x 16 pixel x 32 channel boxes).  The
+// weights (128 x 49 fp32) are scaled by a power of two, split and swizzled into shared memory once per CTA.  One
+// persistent CTA per SM, 256 threads.
 #pragma once
 #include "epilogues.cuh"
 
@@ -29,10 +30,12 @@ constexpr int kStemPatchH = 2 * kConvTileH + 5;    // 21 input rows feed 8 outpu
 constexpr int kStemPatchW = 2 * kConvTileW + 5;    // 37
 constexpr int kStemPatchPitch = 40;
 constexpr int kStemATile = 128 * 128;              // [128 rows][64 fp16] = 16 KB per plane
-constexpr int kStemSmemBytes = 4 * kStemATile      // A hi/lo x 2 buffers
+constexpr int kStemAccStride = 132;                // floats per staged accumulator row (conflict-free row reads)
+constexpr int kStemSmemBytes = 2 * kStemATile      // A hi/lo
                                + 2 * kStemATile    // W hi/lo
+                               + 128 * kStemAccStride * 4   // staged accumulator
                                + 8 * 4096          // per-warp TMA-store staging
-                               + 2 * kStemPatchH * kStemPatchPitch * 4 + 2 * 128 * 4 + 64 * 4 + 64;
+                               + kStemPatchH * kStemPatchPitch * 4 + 2 * 128 * 4 + 64 * 4;
 
 __device__ __forceinline__ uint32_t stem_sw128(int row, int k) {   // byte offset of fp16 element (row, k) in a SW128 K-major tile
   return static_cast<uint32_t>(row * 128 + ((((k >> 3) ^ (row & 7)) << 4) | ((k & 7) << 1)));
@@ -42,23 +45,17 @@ __global__ void __launch_bounds__(kStemThreads, 1) conv_stem7x7_tc_kernel(const 
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // the first convolution may set up meanwhile
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) asm volatile("trap;");
-  uint8_t* sA = smem;                                   // [buf][hi|lo][16 KB]
-  uint8_t* sW = smem + 4 * kStemATile;                  // [hi|lo][16 KB]
-  uint32_t* sStage = reinterpret_cast<uint32_t*>(smem + 6 * kStemATile);
-  float* sPatch = reinterpret_cast<float*>(smem + 6 * kStemATile + 8 * 4096);   // [2][21][40]
-  float* sScale = sPatch + 2 * kStemPatchH * kStemPatchPitch;
+  uint8_t* sA = smem;                                   // [hi|lo][16 KB]
+  uint8_t* sW = smem + 2 * kStemATile;                  // [hi|lo][16 KB]
+  float* sAcc = reinterpret_cast<float*>(smem + 4 * kStemATile);                 // [128][kStemAccStride]
+  uint32_t* sStage = reinterpret_cast<uint32_t*>(sAcc + 128 * kStemAccStride);
+  float* sPatch = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(sStage) + 8 * 4096);   // [21][40]
+  float* sScale = sPatch + kStemPatchH * kStemPatchPitch;
   float* sShift = sScale + 128;
   float* sRed = sShift + 128;                           // [64]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sRed + 64);                      // [2] accumulator-ready barriers
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_slot, 256);
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // warp-uniform: keeps the wgmma window convergent
 
   // ---- weights: power-of-two scale (keeps the fp16 `lo` residuals out of the subnormal range), split, swizzle
   float amax = 0.f;
@@ -80,114 +77,108 @@ __global__ void __launch_bounds__(kStemThreads, 1) conv_stem7x7_tc_kernel(const 
     *reinterpret_cast<uint32_t*>(sW + stem_sw128(n, k)) = h;
     *reinterpret_cast<uint32_t*>(sW + kStemATile + stem_sw128(n, k)) = l;
   }
-  for (int i = tid; i < 4 * kStemATile / 16; i += kStemThreads) reinterpret_cast<uint4*>(sA)[i] = make_uint4(0u, 0u, 0u, 0u);
+  for (int i = tid; i < 2 * kStemATile / 16; i += kStemThreads) reinterpret_cast<uint4*>(sA)[i] = make_uint4(0u, 0u, 0u, 0u);
   if (tid < 128) {
     sScale[tid] = p.scale[tid] * inv;
     sShift[tid] = p.shift[tid];
   }
-  fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  const int Ho = p.H / 2, Wo = p.W / 2;
   const long tiles_per_img = static_cast<long>(p.tiles_w) * p.tiles_h;
   const long total = tiles_per_img * p.N;
-  constexpr uint32_t idesc = umma_idesc_f16_f32(128, 128);
-  const uint32_t lane_base = static_cast<uint32_t>((warp & 3) * 32) << 16;
-  const int half = warp >> 2;                     // column half of the accumulator this warp drains
+  const int half = warp >> 2;                     // warpgroup = 64-channel half of the accumulator
+  const int wt = tid & 127;                       // thread within the warpgroup
   uint32_t* stage = sStage + warp * 1024;
 
-  uint32_t phase[2] = {0u, 0u};
-  long prev = -1;
-  int it = 0;
-  for (long t = blockIdx.x;; t += gridDim.x, ++it) {
-    const bool have = t < total;
-    const int b = it & 1;
-    if (have) {
-      const int n = static_cast<int>(t / tiles_per_img);
-      const int rem = static_cast<int>(t - n * tiles_per_img);
-      const int ty = rem / p.tiles_w, tx = rem - ty * p.tiles_w;
-      // (a) input patch -> shared memory (zero outside the image = the convolution's padding)
-      float* patch = sPatch + b * kStemPatchH * kStemPatchPitch;
-      const int iy0 = 2 * ty * kConvTileH - 3, ix0 = 2 * tx * kConvTileW - 3;
-      for (int i = tid; i < kStemPatchH * kStemPatchW; i += kStemThreads) {
-        const int py = i / kStemPatchW, px = i - py * kStemPatchW;
-        const int iy = iy0 + py, ix = ix0 + px;
-        float v = 0.f;
-        if (iy >= 0 && iy < p.H && ix >= 0 && ix < p.W) v = p.img[(static_cast<long>(n) * p.H + iy) * p.W + ix];
-        patch[py * kStemPatchPitch + px] = v;
+  for (long t = blockIdx.x; t < total; t += gridDim.x) {
+    const int n = static_cast<int>(t / tiles_per_img);
+    const int rem = static_cast<int>(t - n * tiles_per_img);
+    const int ty = rem / p.tiles_w, tx = rem - ty * p.tiles_w;
+    // (a) input patch -> shared memory (zero outside the image = the convolution's padding)
+    const int iy0 = 2 * ty * kConvTileH - 3, ix0 = 2 * tx * kConvTileW - 3;
+    for (int i = tid; i < kStemPatchH * kStemPatchW; i += kStemThreads) {
+      const int py = i / kStemPatchW, px = i - py * kStemPatchW;
+      const int iy = iy0 + py, ix = ix0 + px;
+      float v = 0.f;
+      if (iy >= 0 && iy < p.H && ix >= 0 && ix < p.W) v = p.img[(static_cast<long>(n) * p.H + iy) * p.W + ix];
+      sPatch[py * kStemPatchPitch + px] = v;
+    }
+    __syncthreads();
+    // (b) software im2col: warp w writes rows w, w+8, ...; lane = pair of taps (k, k+1)
+    if (lane < 25) {
+      const int k0 = 2 * lane, k1 = k0 + 1;
+      const int ky0 = k0 / 7, kx0 = k0 - ky0 * 7;
+      const int ky1 = k1 / 7, kx1 = k1 - ky1 * 7;
+      for (int r = warp; r < 128; r += kStemThreads / 32) {
+        const int py = r >> 4, px = r & 15;
+        const float v0 = sPatch[(2 * py + ky0) * kStemPatchPitch + 2 * px + kx0];
+        const float v1 = k1 < 49 ? sPatch[(2 * py + ky1) * kStemPatchPitch + 2 * px + kx1] : 0.f;
+        uint32_t h, l;
+        split_f16x2(v0, v1, h, l);
+        *reinterpret_cast<uint32_t*>(sA + stem_sw128(r, k0)) = h;
+        *reinterpret_cast<uint32_t*>(sA + kStemATile + stem_sw128(r, k0)) = l;
       }
-      __syncthreads();
-      // (b) software im2col: warp w writes rows w, w+8, ...; lane = pair of taps (k, k+1)
-      uint8_t* a_hi = sA + b * 2 * kStemATile;
-      uint8_t* a_lo = a_hi + kStemATile;
-      if (lane < 25) {
-        const int k0 = 2 * lane, k1 = k0 + 1;
-        const int ky0 = k0 / 7, kx0 = k0 - ky0 * 7;
-        const int ky1 = k1 / 7, kx1 = k1 - ky1 * 7;
-        for (int r = warp; r < 128; r += kStemThreads / 32) {
-          const int py = r >> 4, px = r & 15;
-          const float v0 = patch[(2 * py + ky0) * kStemPatchPitch + 2 * px + kx0];
-          const float v1 = k1 < 49 ? patch[(2 * py + ky1) * kStemPatchPitch + 2 * px + kx1] : 0.f;
-          uint32_t h, l;
-          split_f16x2(v0, v1, h, l);
-          *reinterpret_cast<uint32_t*>(a_hi + stem_sw128(r, k0)) = h;
-          *reinterpret_cast<uint32_t*>(a_lo + stem_sw128(r, k0)) = l;
+    }
+    fence_proxy_async();   // generic-proxy operand writes before the wgmma (async proxy) reads them
+    __syncthreads();
+    // (c) wgmma: warpgroup `half` computes output channels [64 half, 64 half + 64) for all 128 pixels
+    float acc[2][32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[0][i] = acc[1][i] = 0.f;
+    {
+      const uint32_t a0 = smem_u32(sA), w0 = smem_u32(sW) + static_cast<uint32_t>(half * 64 * 128);
+      wgmma_fence();
+#pragma unroll
+      for (int mh = 0; mh < 2; ++mh) {
+        const uint32_t a_off = static_cast<uint32_t>(mh * 64 * 128);
+        const uint64_t da_hi = wgmma_desc_k_sw128(a0 + a_off), da_lo = wgmma_desc_k_sw128(a0 + kStemATile + a_off);
+        const uint64_t db_hi = wgmma_desc_k_sw128(w0), db_lo = wgmma_desc_k_sw128(w0 + kStemATile);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t adv = static_cast<uint64_t>(k * 2);
+          wgmma_f16<64>(acc[mh], da_hi + adv, db_hi + adv, 1u);
+          wgmma_f16<64>(acc[mh], da_hi + adv, db_lo + adv, 1u);
+          wgmma_f16<64>(acc[mh], da_lo + adv, db_hi + adv, 1u);
         }
       }
-      fence_proxy_async();
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc[0]);
+      wgmma_fence_regs(acc[1]);
     }
-    tc_fence_before();
-    __syncthreads();          // A(b) complete; every warp has finished draining the TMEM stage that MMA(b) overwrites
-    if (have && tid == 0) {
-      tc_fence_after();
-      const uint32_t a0 = smem_u32(sA + b * 2 * kStemATile), w0 = smem_u32(sW);
-      const uint64_t da_hi = umma_desc_k_sw128(a0), da_lo = umma_desc_k_sw128(a0 + kStemATile);
-      const uint64_t db_hi = umma_desc_k_sw128(w0), db_lo = umma_desc_k_sw128(w0 + kStemATile);
-      const uint32_t d = tmem_base + b * 128;
+    // (d) stage the accumulator row-major: thread holds rows 16 (wt/32) + (wt%32)/4 (+8, +64), columns 8 j + 2 (wt%4)
+    {
+      const int r0 = 16 * (wt >> 5) + ((wt & 31) >> 2);
+      const int c0 = half * 64 + 2 * (wt & 3);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const uint64_t adv = static_cast<uint64_t>(k * 2);
-        umma_f16(d, da_hi + adv, db_hi + adv, idesc, k != 0 ? 1u : 0u);
-        umma_f16(d, da_hi + adv, db_lo + adv, idesc, 1u);
-        umma_f16(d, da_lo + adv, db_hi + adv, idesc, 1u);
+      for (int mh = 0; mh < 2; ++mh) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          float* q = sAcc + (mh * 64 + r0) * kStemAccStride + c0 + 8 * j;
+          *reinterpret_cast<float2*>(q) = make_float2(acc[mh][4 * j], acc[mh][4 * j + 1]);
+          *reinterpret_cast<float2*>(q + 8 * kStemAccStride) = make_float2(acc[mh][4 * j + 2], acc[mh][4 * j + 3]);
+        }
       }
-      umma_commit(&bars[b]);
     }
-    // (c) epilogue of the previous tile while the tensor core works on this one
-    if (prev >= 0) {
-      const int pb = b ^ 1;
-      mbar_wait(&bars[pb], phase[pb]);
-      phase[pb] ^= 1u;
-      tc_fence_after();
-      const int n = static_cast<int>(prev / tiles_per_img);
-      const int rem = static_cast<int>(prev - n * tiles_per_img);
-      const int ty = rem / p.tiles_w, tx = rem - ty * p.tiles_w;
+    __syncthreads();
+    // (e) epilogue: warp w drains pixel rows 32 (w%4) + lane, channel groups of its half
+    const float* row = sAcc + ((warp & 3) * 32 + lane) * kStemAccStride;
 #pragma unroll 1
-      for (int c = half * 2; c < half * 2 + 2; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + pb * 128 + c * 32 + lane_base, v);
-        tmem_ld_wait();
-        float x[32];
+    for (int c = half * 2; c < half * 2 + 2; ++c) {
+      float x[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] = fmaxf(fmaf(__uint_as_float(v[j]), sScale[c * 32 + j], sShift[c * 32 + j]), 0.f);
-        warp_tma_store_planes32(stage, p.om, OutCoord{c * 32, tx * kConvTileW, ty * kConvTileH + (warp & 3) * 2, n}, x);
+      for (int j = 0; j < 32; j += 4) {
+        const float4 v = *reinterpret_cast<const float4*>(row + c * 32 + j);
+        x[j] = fmaxf(fmaf(v.x, sScale[c * 32 + j], sShift[c * 32 + j]), 0.f);
+        x[j + 1] = fmaxf(fmaf(v.y, sScale[c * 32 + j + 1], sShift[c * 32 + j + 1]), 0.f);
+        x[j + 2] = fmaxf(fmaf(v.z, sScale[c * 32 + j + 2], sShift[c * 32 + j + 2]), 0.f);
+        x[j + 3] = fmaxf(fmaf(v.w, sScale[c * 32 + j + 3], sShift[c * 32 + j + 3]), 0.f);
       }
+      warp_tma_store_planes32(stage, p.om, OutCoord{c * 32, tx * kConvTileW, ty * kConvTileH + (warp & 3) * 2, n}, x);
     }
-    prev = have ? t : -1;
-    if (!have) break;
+    __syncthreads();   // the staged accumulator and the operand tile are rewritten by the next tile
   }
-  (void)Ho;
-  (void)Wo;
   tma_store_wait_all();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
-  }
 }
 
 }  // namespace lb

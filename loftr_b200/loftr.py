@@ -2,12 +2,12 @@
 
 Same constructor argument (the lower-case config dict), same sub-module and parameter names (so
 `state_dict`s and released checkpoints round-trip), same `forward(data) -> None` contract that
-mutates `data` with the reference's output keys.  Everything runs in the hand-written sm_100a kernels behind the
+mutates `data` with the reference's output keys.  Everything runs in the hand-written sm_90a kernels behind the
 C ABI of include/loftr_b200.h: the ResNet-FPN backbone as implicit-GEMM convolutions on the tensor cores
 (`backbone_impl="b200"`, the default for the shipped ResNetFPN_8_2 shape; `"torch"` keeps the PyTorch/cuDNN fp32
-forward, which is ~9x closer to fp64 -- DESIGN.md §9), then position encoding, coarse transformer, coarse
+forward, which is closer to fp64 -- DESIGN.md §10), then position encoding, coarse transformer, coarse
 matching, fine windows, fine transformer and fine matching.
-There is no fallback path: without the built library / a B200 the forward raises.
+There is no fallback path: without the built library / an H100 the forward raises.
 
 Packed-weight caches.  The kernels read fp16 hi/lo planes packed lazily from the parameters.  The caches are
 rebuilt when a parameter is replaced or modified through autograd-visible in-place ops (`_version` / `data_ptr`
@@ -65,7 +65,7 @@ class _PackedCacheMixin:
 
 def _require_cuda(t: torch.Tensor, name: str):
     if not t.is_cuda:
-        raise RuntimeError(f"loftr_b200: `{name}` must live on a CUDA (B200) device; the matching hot path has "
+        raise RuntimeError(f"loftr_b200: `{name}` must live on a CUDA (H100) device; the matching hot path has "
                            "no CPU implementation")
 
 
@@ -97,7 +97,7 @@ def split_planes(x: torch.Tensor, hi: torch.Tensor | None = None, lo: torch.Tens
 
 
 class TensorCoreBackbone:
-    """ResNetFPN_8_2 forward through `lb_backbone_forward` (implicit-GEMM convolutions on tcgen05).  Holds no
+    """ResNetFPN_8_2 forward through `lb_backbone_forward` (implicit-GEMM convolutions on wgmma).  Holds no
     parameters of its own: it packs the weights of the PyTorch `ResNetFPN` module it wraps (BatchNorm folded
     with its running statistics = eval mode), lazily and again whenever a parameter or buffer changes."""
 

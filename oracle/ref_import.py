@@ -1,5 +1,6 @@
-"""Import the UNMODIFIED reference (zju3dv/LoFTR at /root/reference) for oracle validation and golden-vector
-generation -- TEST INFRASTRUCTURE, only usable in the authoring container (the GPU box has no /root/reference).
+"""Import the UNMODIFIED reference (a zju3dv/LoFTR checkout named by $LOFTR_REFERENCE) for oracle validation and
+golden-vector generation -- TEST INFRASTRUCTURE, only usable where such a checkout exists; the tests themselves read
+the stored golden vectors and never need it.
 
 The reference needs three modules that are not installed / not shipped:
   * kornia (pinned 0.4.1): only `dsnt.spatial_expectation2d` and `create_meshgrid` are on the hot path
@@ -19,7 +20,7 @@ import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("LOFTR_REFERENCE", "/root/reference")
+REF_ROOT = os.environ.get("LOFTR_REFERENCE", "")
 
 
 def available() -> bool:

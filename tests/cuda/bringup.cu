@@ -1,4 +1,4 @@
-// Stand-alone bring-up check of the split-precision tcgen05 contraction core through the C ABI
+// Stand-alone bring-up check of the split-precision wgmma contraction core through the C ABI
 // (no Python, no torch): random fp32 operands -> lb_split_planes -> lb_gemm_split, compared against a
 // double-precision host product of the same fp32 operands.  Also prints a throughput figure.
 // Build: see Makefile target `bringup`.  Run on the GPU box: build/bringup

@@ -1,9 +1,9 @@
 """Generate the golden vectors that pin `oracle/loftr_oracle.py` (and, through it, the CUDA engine) to the
-reference.  Runs ONLY in the authoring container: it imports the unmodified reference from /root/reference
+reference.  Needs a reference checkout: it imports the unmodified reference from $LOFTR_REFERENCE
 (oracle/ref_import.py) and executes its forward on CPU in fp32.  Only OUTPUTS are stored; weights and
 inputs are regenerated at test time from tests/golden/weights.py (frozen numpy RandomState streams).
 
-    python tests/golden/make_golden.py            # rewrites tests/golden/*.npz
+    LOFTR_REFERENCE=<checkout> python tests/golden/make_golden.py   # rewrites tests/golden/*.npz
 """
 from __future__ import annotations
 

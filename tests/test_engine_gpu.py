@@ -343,10 +343,9 @@ def test_tensor_core_backbone_matches_torch(shape):
         err_torch = (ref.double() - ex).abs().max().item()
         util.record(f"backbone_{name}_{n}x{h}x{w}", {"err_ours_vs_fp64": err_ours, "err_torch_fp32_vs_fp64": err_torch,
                                                       "scale": scale})
-        # The tensor-core path is less accurate than cuDNN's fp32 FMA chain (measured ~4e-5 vs ~1.5e-6 of the
-        # feature scale): tcgen05 accumulates in fp32 with truncation, once per MMA (K/16*3 adds per output), and
-        # the bias compounds over the ~20 convolutions.  It stays well inside what the matcher tolerances need
-        # (end-to-end mconf rel err 5e-4 < 1e-3, see parity_stats); bound it so regressions are caught.
+        # The tensor-core path (fp16 hi/lo operand planes, three MMAs per product) is less accurate than cuDNN's
+        # fp32 FMA chain, and the error compounds over the ~20 convolutions.  It stays well inside what the matcher
+        # tolerances need (end-to-end mconf rel err < 1e-3, see parity_stats); bound it so regressions are caught.
         assert err_ours <= 1e-4 * scale, f"{name}: {err_ours:.3e} (torch fp32: {err_torch:.3e}, scale {scale:.3e})"
 
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Per-layer backbone table from an ncu launch list of one step (tools/profile_step.py, batch 8 x 640x480):
-    python tools/conv_layer_table.py profiles/<launches>.csv [more.csv ...]
+    python tools/conv_layer_table.py <launches>.csv [more.csv ...]
 Launch ids 1..22 of a step are the stem and the 21 convolutions in execution order."""
 import csv
 import sys
@@ -13,7 +13,7 @@ LAYERS = [  # (name, issued GFLOP at batch 8: 3 products x k-steps x N tile, Non
     ("layer3.1.conv2 +skip", 272), ("layer3_outconv 1x1", 30), ("layer2_outconv 1x1 + upsample", 98),
     ("layer2_outconv2.0", 1087), ("layer2_outconv2.3", 883), ("layer1_outconv 1x1 + upsample", 196),
     ("layer1_outconv2.0", 2871), ("layer1_outconv2.3", 1767)]
-PEAK = 1436.0  # measured sustained bf16 TFLOP/s
+PEAK = 989.0  # H100 SXM data sheet, dense bf16 TFLOP/s (an upper bound, not reached)
 
 
 def load(path):
