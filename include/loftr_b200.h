@@ -58,7 +58,8 @@ int lb_selftest(char* report /*host*/, int report_len);
 /* Optional per-launch CUDA-event timing of the tensor-core kernels (events recorded on the launching
  * stream around each kernel while enabled).  lb_timing_enable(1) clears old records and starts recording,
  * lb_timing_collect synchronises the recorded events and returns per-tag total milliseconds and launch counts
- * (arrays of lb_timing_num_tags() entries; names via lb_timing_tag_name). */
+ * (arrays of lb_timing_num_tags() entries; names via lb_timing_tag_name).  Timed launches cannot be recorded into a
+ * CUDA graph: while timing is enabled, a launch on a capturing stream fails. */
 int lb_timing_enable(int on);
 int lb_timing_num_tags(void);
 const char* lb_timing_tag_name(int tag);
@@ -147,6 +148,10 @@ typedef struct LbTransformerState {
   int n_groups;         /* images (coarse) or windows (fine) per set */
   int group_rows0;      /* L  (or 25) */
   int group_rows1;      /* S  (or 25) */
+  /* optional device int (fine / window transformer only): live windows per set.  NULL = all n_groups.  When set,
+   * n_groups is the capacity that fixes the buffer layout and the grids; only windows [0, min(*n_groups_live,
+   * n_groups)) of each set are computed, read on the device (no host synchronisation). */
+  const int* n_groups_live;
 } LbTransformerState;
 
 size_t lb_transformer_workspace_bytes(int d_model, int nhead, int n_groups, int group_rows0, int group_rows1);
@@ -215,6 +220,9 @@ typedef struct LbFinePreprocessArgs {
   float* x_f32;           /* [2*M*W*W, Cf] */
   void* cat_hi;           /* [2*M*W*W, 2Cf] */
   void* cat_lo;
+  /* optional device int: live match count.  NULL = M.  When set, M is the capacity (layout and grids as above) and
+   * only windows m < min(*M_live, M) of each side are gathered and merged. */
+  const int* M_live;
 } LbFinePreprocessArgs;
 
 size_t lb_fine_preprocess_workspace_bytes(long M, int W, int Cf);
@@ -231,6 +239,7 @@ typedef struct LbFineMatchArgs {
   const float* mkpts1_c;  /* [M, 2] */
   float* expec_f;         /* [M, 3] */
   float* mkpts1_f;        /* [M, 2] */
+  const int* M_live;      /* optional device int: live match count (NULL = M; when set, M is the capacity) */
 } LbFineMatchArgs;
 
 int lb_fine_match(const LbFineMatchArgs* args /*host*/, void* stream);

@@ -49,7 +49,7 @@ class LbBackboneWeights(C.Structure):
 
 class LbTransformerState(C.Structure):
     _fields_ = [("x_f32", c_void_p), ("cat_hi", c_void_p), ("cat_lo", c_void_p), ("mask", c_void_p),
-                ("n_groups", c_int), ("group_rows0", c_int), ("group_rows1", c_int)]
+                ("n_groups", c_int), ("group_rows0", c_int), ("group_rows1", c_int), ("n_groups_live", c_void_p)]
 
 
 class LbCoarseMatchArgs(C.Structure):
@@ -80,6 +80,7 @@ class LbFinePreprocessArgs(C.Structure):
         ("down_wt", c_void_p), ("down_b", c_void_p), ("merge_w2t", c_void_p), ("merge_b", c_void_p),
         ("merge_w_hi", c_void_p), ("merge_w_lo", c_void_p), ("merge_acc_scale", c_float),
         ("x_f32", c_void_p), ("cat_hi", c_void_p), ("cat_lo", c_void_p),
+        ("M_live", c_void_p),
     ]
 
 
@@ -88,6 +89,7 @@ class LbFineMatchArgs(C.Structure):
         ("f0", c_void_p), ("f1", c_void_p), ("W", c_int), ("C", c_int), ("M", c_long),
         ("img_scale", c_float), ("scale1", c_void_p), ("b_ids", c_void_p), ("mkpts1_c", c_void_p),
         ("expec_f", c_void_p), ("mkpts1_f", c_void_p),
+        ("M_live", c_void_p),
     ]
 
 
@@ -131,6 +133,9 @@ SIGNATURES = {
 }
 
 NCCL_UNIQUE_ID_BYTES = 128
+# oldest library whose ABI matches the structures above (101: the device-count fields at the end of
+# LbTransformerState / LbFinePreprocessArgs / LbFineMatchArgs)
+MIN_VERSION = 101
 
 
 class LibraryMissing(RuntimeError):
@@ -150,6 +155,10 @@ def load():
             f"{LIB_PATH} not found: build it with `make` (or `python -c 'import __graft_entry__ as g; g.build()'`). "
             "loftr_b200 has no CPU or PyTorch fallback for the matching hot path.")
     lib = C.CDLL(LIB_PATH)
+    lib.lb_version.restype = c_int
+    if lib.lb_version() < MIN_VERSION:
+        raise LibraryMissing(f"{LIB_PATH} is version {lib.lb_version()}, older than the binding ({MIN_VERSION}): "
+                             "rebuild it with `make`")
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the library does not export a declared symbol
         fn.restype = res

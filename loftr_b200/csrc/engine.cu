@@ -306,6 +306,11 @@ static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const t
   const int grid = static_cast<int>(items < sms ? items : sms);
   TimingRec rec{nullptr, nullptr, tag};
   if (g_timing) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    LB_CUDA(cudaStreamIsCapturing(st, &cs));
+    if (cs != cudaStreamCaptureStatusNone)
+      return fail("kernel timing is enabled (lb_timing_enable) but the stream is being captured into a CUDA graph: "
+                  "timing events cannot be recorded into a graph; disable timing before capture");
     LB_CUDA(cudaEventCreate(&rec.e0));
     LB_CUDA(cudaEventCreate(&rec.e1));
     LB_CUDA(cudaEventRecord(rec.e0, st));
@@ -342,13 +347,16 @@ static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const t
   return 0;
 }
 
+// live / live_unit_rows: optional device bound on the rows of every batch (GemmShape::live_count)
 template <int BN, class Epi>
 static int launch_gemm(int tag, const Planes& A, const Planes& B, int batches, int M, int N, int K, int n_chunks,
-                       const typename Epi::Params& ep, cudaStream_t st) {
+                       const typename Epi::Params& ep, cudaStream_t st, const int* live = nullptr,
+                       int live_unit_rows = 0) {
   int sms = 0;
   LB_TRY(device_check(&sms));
   if (K % kBlockK != 0 || K <= 0) return fail("K=%d must be a positive multiple of %d", K, kBlockK);
   if (M <= 0 || N <= 0 || batches <= 0) return 0;  // nothing to do
+  if (live && !EpiRowBound<Epi>::value) return fail("this GEMM epilogue is built without a device row bound");
   GemmShape s;
   s.batches = batches;
   s.M = M;
@@ -361,6 +369,8 @@ static int launch_gemm(int tag, const Planes& A, const Planes& B, int batches, i
   s.tiles_per_chunk = (s.n_tiles + n_chunks - 1) / n_chunks;
   s.n_chunks = (s.n_tiles + s.tiles_per_chunk - 1) / s.tiles_per_chunk;
   s.conv = ConvGeom{0, 0, 0, 0, 0, 0, 0, 0, 0};
+  s.live_count = live;
+  s.live_unit_rows = live_unit_rows;
 
   GemmMaps mp;
   LB_TRY(make_map(&mp.a_hi, A.hi, K, M, batches, A.ld, A.batch_stride, kBlockM));
@@ -418,6 +428,8 @@ static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_re
   s.tiles_per_chunk = 1;
   const int rem_groups = rem ? (taps + kRemTapsPerStage - 1) / kRemTapsPerStage : 0;
   s.conv = ConvGeom{1, tiles_w, d.stride, d.pad, d.ksize, cin_blocks, taps, taps * cin_blocks, rem_groups};
+  s.live_count = nullptr;
+  s.live_unit_rows = 0;
   if (rem && (!wgt_rem.hi || !wgt_rem.lo)) return fail("convolution with Cin=%d needs remainder weight planes", d.Cin);
   GemmMaps mp;
   LB_TRY(make_map_nhwc(&mp.a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride));
@@ -500,7 +512,8 @@ static void carve_tf(Bump& b, TfWs& w, int C, int H, long R, int n_groups, bool 
 template <int BN>
 static int tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st, const TfWs& w,
                          long x_base, long x_rows, int x_group_rows, long s_base, long s_rows, int s_group_rows,
-                         int n_groups_x, bool self_pass, bool write_f32, cudaStream_t stream);
+                         int n_groups_x, bool self_pass, bool write_f32, cudaStream_t stream, const int* live,
+                         int live_cap);
 
 
 // ------------------------------------------------------------------------------------------------ backbone
@@ -618,7 +631,8 @@ using namespace lb;
 template <int BN>
 static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st,
                              const TfWs& w, long x_base, long x_rows, int x_group_rows, long s_base, long s_rows,
-                             int s_group_rows, int n_groups_x, bool self_pass, bool write_f32, cudaStream_t stream) {
+                             int s_group_rows, int n_groups_x, bool self_pass, bool write_f32, cudaStream_t stream,
+                             const int* live, int live_cap) {
   const int D = C / H;
   const long ldc = 2L * C;
   const __half* cat_hi = static_cast<const __half*>(st.cat_hi);
@@ -628,6 +642,16 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   const int per = D * D + D;
   if (n_groups_x != n_groups_s && !self_pass) return fail("query / source group counts differ");
   const bool fused = (D == 32) && use_fused_attn() && lw.wkv_hi != nullptr;
+  // Device-bounded window transformer (`live` != nullptr): every set of live_cap windows is one GEMM batch of
+  // live_cap * group_rows rows whose live prefix is read on the device, so a self pass over both sets is a two-batch
+  // GEMM.  Without a bound every row range is one batch (xb = sb = 1), as it always was.
+  const int xb = live ? static_cast<int>(x_rows / (static_cast<long>(live_cap) * x_group_rows)) : 1;
+  const int sb = live ? static_cast<int>(s_rows / (static_cast<long>(live_cap) * s_group_rows)) : 1;
+  const int xM = static_cast<int>(x_rows / xb), sM = static_cast<int>(s_rows / sb);
+  const long xbs = xb > 1 ? static_cast<long>(xM) * ldc : 0, sbs = sb > 1 ? static_cast<long>(sM) * ldc : 0;
+  const long xbs_a = xb > 1 ? static_cast<long>(xM) * C : 0;       // attention planes [R, C]
+  if (live && (fused || D != 16 || x_group_rows != s_group_rows))
+    return fail("device-bounded group counts are built for the fine (window) transformer only");
 
   if constexpr (BN == 256) {
     if (fused) {
@@ -707,25 +731,25 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   {
     using Epi = EpiActStore<BN>;
     if (self_pass) {
-      Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, 0};
+      Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, xbs};
       Planes B{lw.wqkv_hi, lw.wqkv_lo, C, 0};
       OutMaps om;
-      LB_TRY(fill_out_maps(&om, nullptr, nullptr, 0, w.qkv + x_base * 3 * C, 3 * C, 3 * C, x_rows, 1));
+      LB_TRY(fill_out_maps(&om, nullptr, nullptr, 0, w.qkv + x_base * 3 * C, 3 * C, 3 * C, xM, xb));
       typename Epi::Params ep{w.qkv + x_base * 3 * C, 3 * C, 2 * C, mask ? mask + x_base : nullptr, lw.s_qkv, 0, om};
-      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, 1, static_cast<int>(x_rows), 3 * C, C, 0, ep, stream)));
+      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, xb, xM, 3 * C, C, 0, ep, stream, live, x_group_rows)));
     } else {
-      Planes Aq{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, 0};
+      Planes Aq{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, xbs};
       Planes Bq{lw.wqkv_hi, lw.wqkv_lo, C, 0};
       OutMaps omq, omk;
-      LB_TRY(fill_out_maps(&omq, nullptr, nullptr, 0, w.qkv + x_base * 3 * C, 3 * C, C, x_rows, 1));
-      LB_TRY(fill_out_maps(&omk, nullptr, nullptr, 0, w.qkv + s_base * 3 * C + C, 3 * C, 2 * C, s_rows, 1));
+      LB_TRY(fill_out_maps(&omq, nullptr, nullptr, 0, w.qkv + x_base * 3 * C, 3 * C, C, xM, xb));
+      LB_TRY(fill_out_maps(&omk, nullptr, nullptr, 0, w.qkv + s_base * 3 * C + C, 3 * C, 2 * C, sM, sb));
       typename Epi::Params eq{w.qkv + x_base * 3 * C, 3 * C, C, mask ? mask + x_base : nullptr, lw.s_qkv, 0, omq};
-      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Aq, Bq, 1, static_cast<int>(x_rows), C, C, 0, eq, stream)));
-      Planes Ak{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, 0};
+      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Aq, Bq, xb, xM, C, C, 0, eq, stream, live, x_group_rows)));
+      Planes Ak{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, sbs};
       Planes Bk{static_cast<const __half*>(lw.wqkv_hi) + static_cast<long>(C) * C,
                 static_cast<const __half*>(lw.wqkv_lo) + static_cast<long>(C) * C, C, 0};
       typename Epi::Params ek{w.qkv + s_base * 3 * C + C, 3 * C, C, mask ? mask + s_base : nullptr, lw.s_qkv, 0, omk};
-      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Ak, Bk, 1, static_cast<int>(s_rows), 2 * C, C, 0, ek, stream)));
+      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Ak, Bk, sb, sM, 2 * C, C, 0, ek, stream, live, s_group_rows)));
     }
   }
   // 2+3 for the fine windows: one kernel per pass, KV stays in shared memory (LOFTR_B200_WINDOW_ATTN=0: two kernels)
@@ -750,9 +774,11 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
       wa_configured[dev] = true;
     }
     window_attn_kernel<16, 8><<<grid, 256, wa_smem, stream>>>(w.qkv, 3 * C, 0, C, 2 * C, x_base, s_base, x_group_rows,
-                                                              n_groups_x, 1e-6f, w.att_hi, w.att_lo, C);
+                                                              n_groups_x, 1e-6f, w.att_hi, w.att_lo, C, live, live_cap);
     LB_LAUNCHED();
   } else {
+  if (live) return fail("the device-bounded window transformer needs the one-kernel window attention "
+                        "(LOFTR_B200_WINDOW_ATTN=0 selects a path without a device bound)");
   // 2. KV = K^T V and Ksum per (source group, head)            [linear_attention.py:43-44]
   if (D == 32) {
     const int rps = cdiv(cdiv(s_group_rows, kKvSplits), 32) * 32;
@@ -788,50 +814,50 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   // 4. merge + norm1 -> cat[:, C:2C]                            [transformer.py:51-52]
   {
     using Epi = EpiLayerNorm<BN>;
-    Planes A{w.att_hi + x_base * C, w.att_lo + x_base * C, C, 0};
+    Planes A{w.att_hi + x_base * C, w.att_lo + x_base * C, C, xbs_a};
     Planes B{lw.wm_hi, lw.wm_lo, C, 0};
     OutMaps om;
     LB_TRY(fill_out_maps(&om, static_cast<__half*>(st.cat_hi) + x_base * ldc + C, static_cast<__half*>(st.cat_lo) + x_base * ldc + C,
-                         ldc, nullptr, 0, C, x_rows, 1));
+                         ldc, nullptr, 0, C, xM, xb));
     typename Epi::Params ep{lw.ln1_g, lw.ln1_b, 1e-5f, nullptr, 0, nullptr, nullptr, 0, nullptr, 0,
                             static_cast<__half*>(st.cat_hi) + x_base * ldc,
                             static_cast<__half*>(st.cat_lo) + x_base * ldc, static_cast<int>(ldc), C, lw.s_m, om};
-    LB_TRY((launch_gemm<BN, Epi>(TAG_MERGE_LN, A, B, 1, static_cast<int>(x_rows), C, C, 0, ep, stream)));
+    LB_TRY((launch_gemm<BN, Epi>(TAG_MERGE_LN, A, B, xb, xM, C, C, 0, ep, stream, live, x_group_rows)));
   }
   // 5. mlp[0] + ReLU on cat([x, message]) -> h planes           [transformer.py:55, mlp 22-26]
   {
     using Epi = EpiPlanes<BN>;
-    Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, 0};
+    Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, xbs};
     Planes B{lw.w1_hi, lw.w1_lo, 2 * C, 0};
     OutMaps om;
-    LB_TRY(fill_out_maps(&om, w.h_hi + x_base * ldc, w.h_lo + x_base * ldc, ldc, nullptr, 0, 2 * C, x_rows, 1));
+    LB_TRY(fill_out_maps(&om, w.h_hi + x_base * ldc, w.h_lo + x_base * ldc, ldc, nullptr, 0, 2 * C, xM, xb));
     typename Epi::Params ep{1, nullptr, 1, nullptr, 0, w.h_hi + x_base * ldc, w.h_lo + x_base * ldc,
                             static_cast<int>(ldc), 0, lw.s_1, om};
-    LB_TRY((launch_gemm<BN, Epi>(TAG_MLP1, A, B, 1, static_cast<int>(x_rows), 2 * C, 2 * C, 0, ep, stream)));
+    LB_TRY((launch_gemm<BN, Epi>(TAG_MLP1, A, B, xb, xM, 2 * C, 2 * C, 0, ep, stream, live, x_group_rows)));
   }
   // 6. mlp[2] + norm2 + residual -> cat[:, 0:C] (and x_f32 after the last layer)   [transformer.py:55-58]
   // The residual stream lives in the fp16 planes (x = hi + lo, exact to 2^-22 relative): no fp32 master copy is read
   // or written between layers.
   {
     using Epi = EpiLayerNorm<BN>;
-    Planes A{w.h_hi + x_base * ldc, w.h_lo + x_base * ldc, ldc, 0};
+    Planes A{w.h_hi + x_base * ldc, w.h_lo + x_base * ldc, ldc, xbs};
     Planes B{lw.w2_hi, lw.w2_lo, 2 * C, 0};
     float* xf = write_f32 ? st.x_f32 + x_base * C : nullptr;
     OutMaps om;
     LB_TRY(fill_out_maps(&om, static_cast<__half*>(st.cat_hi) + x_base * ldc, static_cast<__half*>(st.cat_lo) + x_base * ldc, ldc, xf,
-                         C, C, x_rows, 1));
+                         C, C, xM, xb));
     typename Epi::Params ep{lw.ln2_g, lw.ln2_b, 1e-5f, nullptr, 0, cat_hi + x_base * ldc, cat_lo + x_base * ldc,
                             static_cast<int>(ldc), xf, C,
                             static_cast<__half*>(st.cat_hi) + x_base * ldc,
                             static_cast<__half*>(st.cat_lo) + x_base * ldc, static_cast<int>(ldc), 0, lw.s_2, om};
-    LB_TRY((launch_gemm<BN, Epi>(TAG_MLP2_LN, A, B, 1, static_cast<int>(x_rows), C, 2 * C, 0, ep, stream)));
+    LB_TRY((launch_gemm<BN, Epi>(TAG_MLP2_LN, A, B, xb, xM, C, 2 * C, 0, ep, stream, live, x_group_rows)));
   }
   return 0;
 }
 
 extern "C" {
 
-int lb_version(void) { return 100; }
+int lb_version(void) { return 101; }
 int lb_block_k(void) { return kBlockK; }
 int lb_conv_layout(int cin, int* cin_blocks, int* rem_channels) {
   if (!cin_blocks || !rem_channels || cin <= 0) return fail("lb_conv_layout: bad arguments");
@@ -1070,6 +1096,8 @@ int lb_transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds
   const bool fine = (C == 128 && H == 8);
   if (!coarse && !fine) return fail("unsupported transformer shape d_model=%d nhead=%d (built: 256/8 and 128/8)", C, H);
   if (st->n_groups <= 0) return 0;
+  const int* live = st->n_groups_live;
+  if (live && !fine) return fail("n_groups_live is built for the fine (window) transformer only");
   const long rows0 = static_cast<long>(st->n_groups) * st->group_rows0;
   const long rows1 = static_cast<long>(st->n_groups) * st->group_rows1;
   if (!ws) return fail("workspace pointer is null");
@@ -1084,8 +1112,9 @@ int lb_transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds
     const LbEncoderLayerWeights& lw = layers[l];
     const bool last = l == n_layers - 1;   // the fp32 copy of the features is only written after the last layer
     auto pass = [&](long xb, long xr, int xg, long sb, long sr, int sg, int ng, bool self_pass) -> int {
-      return coarse ? tf_layer_pass<256>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s)
-                    : tf_layer_pass<128>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s);
+      return coarse ? tf_layer_pass<256>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s, nullptr, 0)
+                    : tf_layer_pass<128>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s, live,
+                                         st->n_groups);
     };
     if (kinds[l] == LB_LAYER_SELF) {
       // feat0 = layer(feat0, feat0); feat1 = layer(feat1, feat1)  [transformer.py:93-94]; same weights,
@@ -1505,6 +1534,7 @@ int lb_fine_preprocess(const LbFinePreprocessArgs* a, void* ws, size_t ws_bytes,
   g.w0c = a->w0c; g.w1c = a->w1c; g.stride = a->stride; g.W = a->W; g.Cf = a->Cf; g.M = a->M;
   g.b_ids = a->b_ids; g.i_ids = a->i_ids; g.j_ids = a->j_ids;
   g.out_hi = win_hi; g.out_lo = win_lo; g.ld = a->Cf;
+  g.live = a->M_live;
   const bool vec8 = a->sc0 == 1 && a->sc1 == 1 && a->Cf % 8 == 0 && g.ld % 8 == 0 && a->sw0 % 4 == 0 && a->sw1 % 4 == 0 &&
                     a->sh0 % 4 == 0 && a->sh1 % 4 == 0 && a->sn0 % 4 == 0 && a->sn1 % 4 == 0 &&
                     (reinterpret_cast<uintptr_t>(a->feat_f0) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->feat_f1) & 15) == 0;
@@ -1519,18 +1549,22 @@ int lb_fine_preprocess(const LbFinePreprocessArgs* a, void* ws, size_t ws_bytes,
   fb.b_ids = a->b_ids; fb.i_ids = a->i_ids; fb.j_ids = a->j_ids;
   fb.WdT = a->down_wt; fb.bd = a->down_b; fb.Wm2T = a->merge_w2t; fb.bm = a->merge_b;
   fb.gbias = gbias;
+  fb.live = a->M_live;
   fine_bias_kernel<<<static_cast<unsigned>(cdiv(2 * a->M, kFineBiasWin)), 128, 0, st>>>(fb);
   LB_LAUNCHED();
 
   // merge_feat over [window | coarse] = window @ Wm[:, :Cf]^T + per-window bias     [fine_preprocess.py:52-56]
+  // With a device bound each side is one GEMM batch of M*WW rows (M = capacity) with its own live prefix.
   using Epi = EpiPlanes<128>;
-  Planes A{win_hi, win_lo, a->Cf, 0};
+  const int nb = a->M_live ? 2 : 1;
+  const long rows_b = rows / nb;
+  Planes A{win_hi, win_lo, a->Cf, nb > 1 ? rows_b * a->Cf : 0};
   Planes B{a->merge_w_hi, a->merge_w_lo, a->Cf, 0};
   OutMaps om;
-  LB_TRY(fill_out_maps(&om, a->cat_hi, a->cat_lo, 2 * a->Cf, a->x_f32, a->Cf, a->Cf, rows, 1));
+  LB_TRY(fill_out_maps(&om, a->cat_hi, a->cat_lo, 2 * a->Cf, a->x_f32, a->Cf, a->Cf, rows_b, nb));
   Epi::Params ep{0, gbias, WW, a->x_f32, a->Cf, static_cast<__half*>(a->cat_hi), static_cast<__half*>(a->cat_lo),
                  2 * a->Cf, 0, a->merge_acc_scale, om};
-  return launch_gemm<128, Epi>(TAG_FINE_MERGE, A, B, 1, static_cast<int>(rows), a->Cf, a->Cf, 0, ep, st);
+  return launch_gemm<128, Epi>(TAG_FINE_MERGE, A, B, nb, static_cast<int>(rows_b), a->Cf, a->Cf, 0, ep, st, a->M_live, WW);
 }
 
 int lb_fine_match(const LbFineMatchArgs* a, void* stream) {
@@ -1544,6 +1578,7 @@ int lb_fine_match(const LbFineMatchArgs* a, void* stream) {
   p.f0 = a->f0; p.f1 = a->f1; p.W = a->W; p.C = a->C; p.M = a->M;
   p.scale = a->img_scale; p.scale1 = a->scale1; p.b_ids = a->b_ids;
   p.mkpts1_c = a->mkpts1_c; p.expec_f = a->expec_f; p.mkpts1_f = a->mkpts1_f;
+  p.live = a->M_live;
   const int warps_per_block = 8;
   fine_match_kernel<<<cdiv(a->M, warps_per_block), warps_per_block * 32, 0, static_cast<cudaStream_t>(stream)>>>(p);
   LB_LAUNCHED();

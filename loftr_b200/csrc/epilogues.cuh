@@ -891,6 +891,7 @@ struct UpMaps {
 constexpr int kUpW = 10, kUpH = 6;
 template <int BLOCK_N, int kUpMode = 0>
 struct EpiConv {
+  static constexpr bool kNoRowBound = true;      // backbone shapes are static: no device row bound (gemm_split.cuh)
   static constexpr bool kUp = kUpMode == 1;      // staged window
   static constexpr bool kUpAny = kUpMode != 0;
   struct Params {

@@ -76,6 +76,23 @@ struct GemmShape {
   int n_chunks;     // a work item = (batch, m_tile, chunk); chunk = tiles_per_chunk consecutive n tiles
   int tiles_per_chunk;
   ConvGeom conv;
+  // optional device bound on the rows of every batch (capacity-sized buffers whose filled prefix is only known on the
+  // device): rows [0, min(*live_count * live_unit_rows, M)) are computed, the m tiles past them are skipped.  nullptr:
+  // all M rows.
+  const int* live_count;
+  int live_unit_rows;
+};
+
+// Epilogues that can never run under a device row bound (GemmShape::live_count) declare
+// `static constexpr bool kNoRowBound = true;`: the kernel then compiles without the bound's code, so their register
+// allocation is exactly that of an unbounded kernel.
+template <class Epi, class = void>
+struct EpiRowBound {
+  static constexpr bool value = true;
+};
+template <class Epi>
+struct EpiRowBound<Epi, decltype(void(Epi::kNoRowBound))> {
+  static constexpr bool value = !Epi::kNoRowBound;
 };
 
 // K-major operand tile descriptor for the configured k-block (128-byte or 64-byte swizzle rows).
@@ -167,8 +184,15 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   constexpr int kRemBTile = S::kBTile / (kBlockK / kRemChannels);
   static_assert(kBlockK != 64 || (kTapBytes == 2 * kRemATile + 2 * kRemBTile && kTapBytes % 256 == 0 &&
                                   kRemBTile % 256 == 0), "remainder group layout");
+  // m tiles per batch: all of them, or those that hold live rows.  The count is written by an earlier kernel of the
+  // stream, so it is read only here, after griddepcontrol.wait; producer and consumers read the same value.
+  int m_tiles = shape.m_tiles;
+  if (EpiRowBound<Epi>::value && shape.live_count != nullptr) {
+    const long live = min(static_cast<long>(max(*shape.live_count, 0)) * shape.live_unit_rows, static_cast<long>(shape.M));
+    m_tiles = min(m_tiles, static_cast<int>((live + kBlockM - 1) / kBlockM));
+  }
   // work items (batch, m_tile, chunk), strided over the persistent CTAs
-  const int total_items = shape.batches * shape.m_tiles * shape.n_chunks;
+  const int total_items = shape.batches * m_tiles * shape.n_chunks;
 
   if (warp == kProducerWarp) {
     // ------------------------------------------------------------ TMA producer
@@ -178,8 +202,8 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       uint32_t tiles = 0;
       for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
         const int chunk = item % shape.n_chunks;
-        const int mt = (item / shape.n_chunks) % shape.m_tiles;
-        const int batch = item / (shape.n_chunks * shape.m_tiles);
+        const int mt = (item / shape.n_chunks) % m_tiles;
+        const int batch = item / (shape.n_chunks * m_tiles);
         const int nt_begin = chunk * shape.tiles_per_chunk;
         const int nt_end = min(nt_begin + shape.tiles_per_chunk, shape.n_tiles);
         for (int nt = nt_begin; nt < nt_end; ++nt) {
@@ -250,8 +274,8 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     uint32_t phase = 0;
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
       const int chunk = item % shape.n_chunks;
-      const int mt = (item / shape.n_chunks) % shape.m_tiles;
-      const int batch = item / (shape.n_chunks * shape.m_tiles);
+      const int mt = (item / shape.n_chunks) % m_tiles;
+      const int batch = item / (shape.n_chunks * m_tiles);
       const int nt_begin = chunk * shape.tiles_per_chunk;
       const int nt_end = min(nt_begin + shape.tiles_per_chunk, shape.n_tiles);
       epi.item_begin(batch, mt * kBlockM, chunk);

@@ -395,7 +395,7 @@ __global__ void __launch_bounds__(32 * H, 3) window_attn_kernel(const float* __r
                                                                 int v_col0, long x_row_base, long s_row_base,
                                                                 int rows_per_group, int n_groups, float eps,
                                                                 __half* __restrict__ att_hi, __half* __restrict__ att_lo,
-                                                                int ld_att) {
+                                                                int ld_att, const int* __restrict__ live, int live_cap) {
   pdl_trigger();
   static_assert(D == 16 && H == 8, "fine head layout");
   constexpr int C = D * H;  // 128
@@ -428,19 +428,32 @@ __global__ void __launch_bounds__(32 * H, 3) window_attn_kernel(const float* __r
     }
   };
 
+  // Optional device bound (`live` != nullptr): the groups are sets of live_cap windows of which only the first
+  // min(*live, live_cap) are filled, i.e. groups [0, n) U [cap, cap + n) U ...  Work item v maps to group
+  // (v / n_live) * cap + v % n_live (the identity without a bound).
+  int n_items = n_groups, n_live = n_groups, cap = n_groups;
+  if (live != nullptr) {
+    cap = live_cap;
+    n_live = min(max(*live, 0), live_cap);
+    n_items = n_live * (n_groups / live_cap);
+  }
+  auto group_of = [&](int v) { return v / n_live * cap + v % n_live; };
+
   float q[D], qn[D];
 #pragma unroll
   for (int j = 0; j < D; ++j) q[j] = qn[j] = 0.f;
-  int g = blockIdx.x;
-  if (g < n_groups) {
-    issue(g, 0);
-    if (has_row) load_q(g, q);
+  int v = blockIdx.x;
+  if (v < n_items) {
+    issue(group_of(v), 0);
+    if (has_row) load_q(group_of(v), q);
   }
   cp_async_commit();
   int b = 0;
-  for (; g < n_groups; g += gridDim.x, b ^= 1) {
-    const int gn = g + gridDim.x;
-    if (gn < n_groups) {
+  for (; v < n_items; v += gridDim.x, b ^= 1) {
+    const int g = group_of(v);
+    const int vn = v + gridDim.x;
+    if (vn < n_items) {
+      const int gn = group_of(vn);
       issue(gn, b ^ 1);
       if (has_row) load_q(gn, qn);
     }
@@ -801,12 +814,14 @@ struct FineGatherParams {
   __half* out_hi;   // [2*M*WW, ld]
   __half* out_lo;
   int ld;
+  const int* live;  // optional device count: windows m >= min(*live, M) of each side are skipped (M = capacity)
 };
 __global__ void fine_gather_kernel(const FineGatherParams p) {
   const int WW = p.W * p.W;
   const long win = blockIdx.x;             // 0 .. 2M-1
   const int side = win >= p.M ? 1 : 0;
   const long m = side ? win - p.M : win;
+  if (p.live != nullptr && m >= *p.live) return;
   const int b = static_cast<int>(p.b_ids[m]);
   const int idx = static_cast<int>(side ? p.j_ids[m] : p.i_ids[m]);
   const int wc = side ? p.w1c : p.w0c;
@@ -838,6 +853,7 @@ __global__ void __launch_bounds__(256) fine_gather_vec8_kernel(const FineGatherP
   const long win = blockIdx.x;             // 0 .. 2M-1
   const int side = win >= p.M ? 1 : 0;
   const long m = side ? win - p.M : win;
+  if (p.live != nullptr && m >= *p.live) return;
   const int b = static_cast<int>(p.b_ids[m]);
   const int idx = static_cast<int>(side ? p.j_ids[m] : p.i_ids[m]);
   const int wc = side ? p.w1c : p.w0c;
@@ -886,6 +902,7 @@ struct FineBiasParams {
   const float* Wm2T;       // [Cf, Cf]  merge_feat.weight[:, Cf:2Cf]^T
   const float* bm;         // [Cf]
   float* gbias;            // [2M, Cf]
+  const int* live;         // optional device count: windows m >= min(*live, M) of each side are skipped
 };
 __global__ void __launch_bounds__(128) fine_bias_kernel(const FineBiasParams p) {
   pdl_trigger();
@@ -893,9 +910,16 @@ __global__ void __launch_bounds__(128) fine_bias_kernel(const FineBiasParams p) 
   __shared__ float s_c[kFineBiasWin][128];
   const long win0 = static_cast<long>(blockIdx.x) * kFineBiasWin;
   const long nwin = 2 * p.M;
+  const long n_live = p.live != nullptr ? min(static_cast<long>(*p.live), p.M) : p.M;
+  auto is_live = [&](long win) { return win < nwin && (win >= p.M ? win - p.M : win) < n_live; };
+  {
+    bool any = false;
+    for (int wv = 0; wv < kFineBiasWin; ++wv) any |= is_live(win0 + wv);
+    if (!any) return;   // block-uniform
+  }
   for (int wv = 0; wv < kFineBiasWin; ++wv) {
     const long win = win0 + wv;
-    if (win < nwin) {
+    if (is_live(win)) {
       const int side = win >= p.M ? 1 : 0;
       const long m = side ? win - p.M : win;
       const long b = p.b_ids[m];
@@ -931,7 +955,7 @@ __global__ void __launch_bounds__(128) fine_bias_kernel(const FineBiasParams p) 
     }
 #pragma unroll
     for (int wv = 0; wv < kFineBiasWin; ++wv)
-      if (win0 + wv < nwin) p.gbias[(win0 + wv) * p.Cf + o] = a[wv];
+      if (is_live(win0 + wv)) p.gbias[(win0 + wv) * p.Cf + o] = a[wv];
   }
 }
 
@@ -950,11 +974,12 @@ struct FineMatchParams {
   const float* mkpts1_c; // [M,2]
   float* expec_f;        // [M,3]
   float* mkpts1_f;       // [M,2]
+  const int* live;       // optional device count: matches m >= min(*live, M) are skipped (M = capacity)
 };
 __global__ void fine_match_kernel(const FineMatchParams p) {
   const long m = (blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
-  if (m >= p.M) return;
+  if (m >= p.M || (p.live != nullptr && m >= *p.live)) return;
   const int WW = p.W * p.W;
   const float* c0 = p.f0 + (m * WW + WW / 2) * p.C;
   const float* w1 = p.f1 + m * WW * p.C;

@@ -311,12 +311,14 @@ class LocalFeatureTransformer(_PackedCacheMixin, nn.Module):
         self._packed_key = key
         return self._packed
 
-    def run(self, state: _TokenState, n_groups, group_rows0, group_rows1, mask_u8=None):
-        """In-place transformer over a prepared token state (used by LoFTR.forward)."""
+    def run(self, state: _TokenState, n_groups, group_rows0, group_rows1, mask_u8=None, live=None):
+        """In-place transformer over a prepared token state (used by LoFTR.forward).  `live` (fine windows only): an
+        int32 device count; `n_groups` is then the capacity and only the first min(live, n_groups) windows of each set
+        are computed."""
         lib = _lib.load()
         arr, kinds, _ = self._pack(state.x.device)
         st = _lib.LbTransformerState(state.x.data_ptr(), state.cat_hi.data_ptr(), state.cat_lo.data_ptr(),
-                                     _lib.ptr(mask_u8), n_groups, group_rows0, group_rows1)
+                                     _lib.ptr(mask_u8), n_groups, group_rows0, group_rows1, _lib.ptr(live))
         nbytes = lib.lb_transformer_workspace_bytes(self.d_model, self.nhead, n_groups, group_rows0, group_rows1)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=state.x.device)
         _lib.check(lib.lb_transformer_forward(arr, kinds, len(self.layers), self.d_model, self.nhead, C.byref(st),
@@ -361,14 +363,56 @@ class CoarseMatching(nn.Module):
         else:
             raise NotImplementedError()
 
+    @staticmethod
+    def default_capacity(n, L, S, masked):
+        """Exact bound on the number of coarse matches: mutual nearest neighbours pair each row with at most one
+        column, so n*min(L, S) without masks (n*L with masks, as padding may leave columns unmatched)."""
+        return max(n * min(L, S) if not masked else n * L, 1)
+
     def run(self, hi, lo, ld, n, L, S, c, data, mask_u8_0=None, mask_u8_1=None):
         """Planes of feat_c0 (rows [0, n*L)) / feat_c1 (rows [n*L, ...)) -> coarse match keys in `data`."""
+        cap = self.default_capacity(n, L, S, mask_u8_0 is not None)
+        b_ids, i_ids, j_ids, mconf, mk0, mk1, count, conf = self._launch(hi, lo, ld, n, L, S, c, data, mask_u8_0,
+                                                                         mask_u8_1, cap)
+        dev = hi.device
+        m = int(count.item())  # the one host sync of the coarse stage (sizes the match list)
+        if m > cap:
+            raise RuntimeError(f"loftr_b200: {m} coarse matches exceed the buffer capacity {cap}")
+        b_ids, i_ids, j_ids, mconf, mk0, mk1 = b_ids[:m], i_ids[:m], j_ids[:m], mconf[:m], mk0[:m], mk1[:m]
+        data.update({"b_ids": b_ids, "i_ids": i_ids, "j_ids": j_ids})
+        if conf is not None:
+            data["conf_matrix"] = conf
+        if self.thr >= 0:  # conf > thr >= 0  =>  the reference's `mconf != 0` filter keeps everything
+            data.update({"gt_mask": torch.zeros(m, dtype=torch.bool, device=dev), "m_bids": b_ids,
+                         "mkpts0_c": mk0, "mkpts1_c": mk1, "mconf": mconf})
+        else:
+            nz = mconf != 0
+            data.update({"gt_mask": ~nz, "m_bids": b_ids[nz], "mkpts0_c": mk0[nz], "mkpts1_c": mk1[nz],
+                         "mconf": mconf[nz]})
+
+    def run_static(self, hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1, cap):
+        """`run` without the host sync: the match keys of `data` are the fixed-capacity buffers ([cap] first
+        dimension; entries at or past min(count, cap) unspecified) and the returned int32 device tensor [1] holds the
+        true count.  Requires thr >= 0 (the `mconf != 0` filter of thr < 0 would be a second, data-dependent list)."""
+        if self.thr < 0:
+            raise ValueError("forward_static needs match_coarse.thr >= 0: with thr < 0 the mconf != 0 filter makes the "
+                             "output list depend on the data")
+        b_ids, i_ids, j_ids, mconf, mk0, mk1, count, conf = self._launch(hi, lo, ld, n, L, S, c, data, mask_u8_0,
+                                                                         mask_u8_1, cap)
+        data.update({"b_ids": b_ids, "i_ids": i_ids, "j_ids": j_ids,
+                     "gt_mask": torch.zeros(cap, dtype=torch.bool, device=hi.device), "m_bids": b_ids,
+                     "mkpts0_c": mk0, "mkpts1_c": mk1, "mconf": mconf, "num_matches": count})
+        if conf is not None:
+            data["conf_matrix"] = conf
+        return count
+
+    def _launch(self, hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1, cap):
+        """Enqueues lb_coarse_match into buffers of `cap` entries -> (b_ids, i_ids, j_ids, mconf, mkpts0_c, mkpts1_c,
+        count, conf_matrix or None); no host sync."""
         if self.training:
             raise NotImplementedError("loftr_b200 builds the inference path only (no training-time sampling)")
         lib = _lib.load()
         dev = hi.device
-        cap = n * min(L, S) if mask_u8_0 is None else n * L
-        cap = max(cap, 1)
         b_ids = torch.empty(cap, dtype=torch.int64, device=dev)
         i_ids = torch.empty(cap, dtype=torch.int64, device=dev)
         j_ids = torch.empty(cap, dtype=torch.int64, device=dev)
@@ -407,20 +451,7 @@ class CoarseMatching(nn.Module):
         nbytes = lib.lb_coarse_match_workspace_bytes(n, L, S)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         _lib.check(lib.lb_coarse_match(C.byref(a), ws.data_ptr(), nbytes, _stream(hi)))
-        m = int(count.item())  # the one host sync of the coarse stage (sizes the match list)
-        if m > cap:
-            raise RuntimeError(f"loftr_b200: {m} coarse matches exceed the buffer capacity {cap}")
-        b_ids, i_ids, j_ids, mconf, mk0, mk1 = b_ids[:m], i_ids[:m], j_ids[:m], mconf[:m], mk0[:m], mk1[:m]
-        data.update({"b_ids": b_ids, "i_ids": i_ids, "j_ids": j_ids})
-        if conf is not None:
-            data["conf_matrix"] = conf
-        if self.thr >= 0:  # conf > thr >= 0  =>  the reference's `mconf != 0` filter keeps everything
-            data.update({"gt_mask": torch.zeros(m, dtype=torch.bool, device=dev), "m_bids": b_ids,
-                         "mkpts0_c": mk0, "mkpts1_c": mk1, "mconf": mconf})
-        else:
-            nz = mconf != 0
-            data.update({"gt_mask": ~nz, "m_bids": b_ids[nz], "mkpts0_c": mk0[nz], "mkpts1_c": mk1[nz],
-                         "mconf": mconf[nz]})
+        return b_ids, i_ids, j_ids, mconf, mk0, mk1, count, conf
 
     @torch.no_grad()
     def forward(self, feat_c0, feat_c1, data, mask_c0=None, mask_c1=None):
@@ -471,8 +502,10 @@ class FinePreprocess(_PackedCacheMixin, nn.Module):
             self._packed_key = key
         return self._packed
 
-    def run(self, feat_f0, feat_f1, feat_c_all, n, L, S, data):
-        """-> _TokenState of the fine transformer (rows: side, match, window position), or None if M == 0."""
+    def run(self, feat_f0, feat_f1, feat_c_all, n, L, S, data, live=None):
+        """-> _TokenState of the fine transformer (rows: side, match, window position), or None if M == 0.
+        `live`: int32 device count; the match keys of `data` are then capacity buffers and only windows below the
+        count are gathered (rows keep the capacity layout side*cap*WW + m*WW + k)."""
         lib = _lib.load()
         W = self.W
         stride = data["hw0_f"][0] // data["hw0_c"][0]
@@ -498,6 +531,7 @@ class FinePreprocess(_PackedCacheMixin, nn.Module):
                                                        p["bm"].data_ptr())
         a.merge_w_hi, a.merge_w_lo, a.merge_acc_scale = p["wm_hi"].data_ptr(), p["wm_lo"].data_ptr(), p["wm_scale"]
         a.x_f32, a.cat_hi, a.cat_lo = state.x.data_ptr(), state.cat_hi.data_ptr(), state.cat_lo.data_ptr()
+        a.M_live = _lib.ptr(live)
         nbytes = lib.lb_fine_preprocess_workspace_bytes(m, W, cf)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         _lib.check(lib.lb_fine_preprocess(C.byref(a), ws.data_ptr(), nbytes, _stream(feat_f0)))
@@ -523,7 +557,8 @@ class FineMatching(nn.Module):
     """Correlation + soft-argmax refinement (reference fine_matching.py:9-74)."""
 
     @torch.no_grad()
-    def forward(self, feat_f0, feat_f1, data):
+    def forward(self, feat_f0, feat_f1, data, live=None):
+        """`live`: int32 device count; M is then the capacity and only matches below the count are refined."""
         M, WW, Cf = feat_f0.shape
         W = int(math.sqrt(WW))
         scale = data["hw0_i"][0] / data["hw0_f"][0]
@@ -551,6 +586,7 @@ class FineMatching(nn.Module):
             a.scale1 = keep.data_ptr()
         a.b_ids, a.mkpts1_c = data["b_ids"].data_ptr(), mk1c.data_ptr()
         a.expec_f, a.mkpts1_f = expec.data_ptr(), mk1f.data_ptr()
+        a.M_live = _lib.ptr(live)
         _lib.check(lib.lb_fine_match(C.byref(a), _stream(f0)))
         data.update({"expec_f": expec, "mkpts0_f": data["mkpts0_c"], "mkpts1_f": mk1f})
 
@@ -599,8 +635,85 @@ class LoFTR(nn.Module):
         optional scale0/scale1 [N, 2]."""
         if self.training:
             raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
+        _require_cuda(data["image0"], "image0")
+        state, feat_f0, feat_f1, bs, L, S, c, m0, m1 = self._coarse_features(data)
+        img0 = data["image0"]
+
+        # 3. coarse matching                                                           [loftr.py:67]
+        self.coarse_matching.run(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1)
+
+        # 4. fine-level refinement                                                     [loftr.py:70-72]
+        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, bs, L, S, data)
+        ww = self.fine_preprocess.W ** 2
+        if fstate is not None:
+            m = fstate.rows0 // ww
+            self.loftr_fine.run(fstate, m, ww, ww)
+            f0u, f1u = fstate.x[: m * ww].view(m, ww, -1), fstate.x[m * ww:].view(m, ww, -1)
+        else:
+            f0u = torch.empty(0, ww, self.fine_preprocess.d_model_f, device=img0.device)
+            f1u = f0u.clone()
+
+        # 5. fine matching                                                             [loftr.py:75]
+        self.fine_matching(f0u, f1u, data)
+        if self.expose_coarse_features:   # test / debugging tap, off by default: not a reference key
+            data["_feat_c0"], data["_feat_c1"] = state.x[: bs * L].view(bs, L, c), state.x[bs * L:].view(bs, S, c)
+
+    @torch.no_grad()
+    def forward_static(self, data, capacity=None):
+        """Sync-free, static-shape forward: the same inputs and keys as `forward`, without any host synchronisation,
+        so that it can be captured by `torch.cuda.graph` (after one eager call, which packs the weights).
+
+        Every input, masks and scales included, must already be on the device.  The match keys (b_ids, i_ids, j_ids,
+        m_bids, gt_mask, mconf, mkpts0_c/1_c, mkpts0_f/1_f, expec_f) are fixed-capacity tensors with first dimension
+        `capacity`, and data["num_matches"] is an int32 device tensor [1] with the true match count.  The count may
+        exceed `capacity`; entries at or past min(count, capacity) are unspecified.  Only windows below the count are
+        refined: the fine stage reads the count on the device.
+
+        capacity: defaults to the exact bound of the coarse stage, n*min(L, S) (n*L with masks).  The fine stage keeps
+        about 5 KB of state per window row, i.e. about 256 KB per match of capacity (about 10 GB at batch 8 640x480):
+        a smaller capacity trades that memory for the risk of overflow, which stays visible in num_matches.
+
+        Configurations whose output list depends on the data (match_coarse.thr < 0) raise ValueError."""
+        if self.training:
+            raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
+        if self.coarse_matching.thr < 0:
+            raise ValueError("forward_static needs match_coarse.thr >= 0: with thr < 0 the reference's mconf != 0 "
+                             "filter makes the output list depend on the data")
+        if capacity is not None and int(capacity) < 1:
+            raise ValueError(f"capacity must be a positive number of matches (got {capacity})")
+        dev = None
+        for k in ("image0", "image1", "mask0", "mask1", "scale0", "scale1"):
+            if k not in data:
+                continue
+            t = data[k]
+            if not torch.is_tensor(t) or not t.is_cuda:
+                raise ValueError(f"forward_static: `{k}` must already be a CUDA tensor (copying a host tensor to the "
+                                 "device would synchronise)")
+            if dev is None:
+                dev = t.device
+            elif t.device != dev:
+                raise ValueError(f"forward_static: `{k}` is on {t.device}, image0 on {dev}")
+        state, feat_f0, feat_f1, bs, L, S, c, m0, m1 = self._coarse_features(data)
+        cap = self.coarse_matching.default_capacity(bs, L, S, m0 is not None) if capacity is None else int(capacity)
+
+        # 3. coarse matching into capacity buffers; `count` stays on the device
+        count = self.coarse_matching.run_static(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1, cap)
+
+        # 4. fine-level refinement over the capacity layout, bounded on the device by `count`
+        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, bs, L, S, data, live=count)
+        ww = self.fine_preprocess.W ** 2
+        self.loftr_fine.run(fstate, cap, ww, ww, live=count)
+        f0u, f1u = fstate.x[: cap * ww].view(cap, ww, -1), fstate.x[cap * ww:].view(cap, ww, -1)
+
+        # 5. fine matching
+        self.fine_matching(f0u, f1u, data, live=count)
+        if self.expose_coarse_features:
+            data["_feat_c0"], data["_feat_c1"] = state.x[: bs * L].view(bs, L, c), state.x[bs * L:].view(bs, S, c)
+
+    def _coarse_features(self, data):
+        """Steps 1-2 of the forward (no host sync): backbone, position encoding and coarse transformer.
+        -> (coarse token state, feat_f0, feat_f1, n, L, S, C, mask0 u8, mask1 u8)."""
         img0, img1 = data["image0"], data["image1"]
-        _require_cuda(img0, "image0")
         lib = _lib.load()
         bs = img0.size(0)
         data.update({"bs": bs, "hw0_i": img0.shape[2:], "hw1_i": img1.shape[2:]})
@@ -643,25 +756,7 @@ class LoFTR(nn.Module):
             mask_all = torch.cat([m0, m1]).contiguous()
             m0, m1 = mask_all[: bs * L], mask_all[bs * L:]
         self.loftr_coarse.run(state, bs, L, S, mask_all)
-
-        # 3. coarse matching                                                           [loftr.py:67]
-        self.coarse_matching.run(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1)
-
-        # 4. fine-level refinement                                                     [loftr.py:70-72]
-        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, bs, L, S, data)
-        ww = self.fine_preprocess.W ** 2
-        if fstate is not None:
-            m = fstate.rows0 // ww
-            self.loftr_fine.run(fstate, m, ww, ww)
-            f0u, f1u = fstate.x[: m * ww].view(m, ww, -1), fstate.x[m * ww:].view(m, ww, -1)
-        else:
-            f0u = torch.empty(0, ww, self.fine_preprocess.d_model_f, device=img0.device)
-            f1u = f0u.clone()
-
-        # 5. fine matching                                                             [loftr.py:75]
-        self.fine_matching(f0u, f1u, data)
-        if self.expose_coarse_features:   # test / debugging tap, off by default: not a reference key
-            data["_feat_c0"], data["_feat_c1"] = state.x[: bs * L].view(bs, L, c), state.x[bs * L:].view(bs, S, c)
+        return state, feat_f0, feat_f1, bs, L, S, c, m0, m1
 
     def invalidate_packed(self):
         """Drop every packed-weight cache (fp16 hi/lo planes, folded BatchNorm): required after parameter writes
@@ -683,3 +778,117 @@ class LoFTR(nn.Module):
                 state_dict[k.replace("matcher.", "", 1)] = state_dict.pop(k)
         self.invalidate_packed()
         return super().load_state_dict(state_dict, *args, **kwargs)
+
+
+def _weight_refs(model):
+    """(packed-weight cache objects, parameters + buffers, their (data_ptr, _version) key) of `model`: everything a
+    captured graph holds raw device pointers into."""
+    caches = [model.loftr_coarse._packed, model.loftr_fine._packed, model.fine_preprocess._packed]
+    if model._tc_backbone is not None:
+        caches.append(model._tc_backbone._packed)
+    tensors = list(model.parameters()) + list(model.buffers())
+    return caches, tensors, tuple((t.data_ptr(), t._version) for t in tensors)
+
+
+class CapturedMatcher:
+    """`model(data)` replayed from one CUDA graph: a drop-in for the matcher call in a loop over fixed-size batches
+    (video, SLAM front ends, webcam demos), where the host cost of enqueueing every launch would otherwise be paid per
+    frame.
+
+    The constructor allocates static input buffers for `batch` pairs of `hw0` / `hw1` images (plus masks and scales
+    when asked for), runs one eager `model.forward_static` to warm up (weight packing, kernel attributes, cuDNN
+    algorithm selection) and captures the next one.  `__call__(data)` copies the inputs into the static buffers,
+    replays the graph and reads the match count once (the only host sync); it fills `data` with the same keys, shapes
+    and values as `model(data)`.  The trimmed outputs are copies, valid after later replays.
+
+    The graph holds raw pointers into the model's packed-weight caches, parameters and buffers.  The captured matcher
+    keeps those objects alive and, on every call, checks on the host that the model still uses them: after
+    `load_state_dict`, `.to()`, `invalidate_packed()` or a parameter change a call raises instead of replaying against
+    stale weights; `recapture()` rebuilds the graph.  See `LoFTR.forward_static` for `capacity` and its memory cost."""
+
+    _TRIMMED = ("b_ids", "i_ids", "j_ids", "gt_mask", "mconf", "mkpts0_c", "mkpts1_c", "mkpts1_f", "expec_f")
+
+    def __init__(self, model, batch, hw0, hw1=None, masks=False, scales=False, capacity=None):
+        if model.training:
+            raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
+        if model.coarse_matching.thr < 0:
+            raise ValueError("CapturedMatcher needs match_coarse.thr >= 0: with thr < 0 the reference's mconf != 0 "
+                             "filter makes the output list depend on the data")
+        if capacity is not None and int(capacity) < 1:
+            raise ValueError(f"capacity must be a positive number of matches (got {capacity})")
+        dev = next(model.parameters()).device
+        if dev.type != "cuda":
+            raise ValueError("CapturedMatcher: the model must live on a CUDA (H100) device; call .cuda() first")
+        hw1 = hw0 if hw1 is None else hw1
+        (h0, w0), (h1, w1) = hw0, hw1
+        res = model.config["resolution"][0]
+        self.model, self.device, self.capacity_arg = model, dev, capacity
+        self.static = {"image0": torch.zeros(batch, 1, h0, w0, device=dev),
+                       "image1": torch.zeros(batch, 1, h1, w1, device=dev)}
+        if masks:
+            self.static["mask0"] = torch.ones(batch, h0 // res, w0 // res, dtype=torch.bool, device=dev)
+            self.static["mask1"] = torch.ones(batch, h1 // res, w1 // res, dtype=torch.bool, device=dev)
+        if scales:
+            self.static["scale0"] = torch.ones(batch, 2, device=dev)
+            self.static["scale1"] = torch.ones(batch, 2, device=dev)
+        self.graph = None
+        self.recapture()
+
+    @property
+    def capacity(self):
+        return int(self.out["b_ids"].shape[0])
+
+    def recapture(self):
+        """(Re)runs the eager warm-up and captures a new graph against the model's current weights."""
+        self.graph = self.out = self._refs = None
+        with torch.cuda.device(self.device):
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                self.model.forward_static(dict(self.static), self.capacity_arg)
+            torch.cuda.current_stream().wait_stream(side)
+            graph, out = torch.cuda.CUDAGraph(), dict(self.static)
+            with torch.cuda.graph(graph):
+                self.model.forward_static(out, self.capacity_arg)
+        self.graph, self.out, self._refs = graph, out, _weight_refs(self.model)
+
+    def _check_weights(self):
+        caches, tensors, key = _weight_refs(self.model)
+        c0, t0, k0 = self._refs
+        if len(caches) != len(c0) or any(a is not b for a, b in zip(caches, c0)) or len(tensors) != len(t0) or \
+                any(a is not b for a, b in zip(tensors, t0)) or key != k0:
+            raise RuntimeError("loftr_b200.CapturedMatcher: weights changed since capture (load_state_dict, .to(), "
+                               "invalidate_packed() or a parameter update); call recapture()")
+
+    def __call__(self, data):
+        if self.graph is None:
+            raise RuntimeError("loftr_b200.CapturedMatcher: no captured graph; call recapture()")
+        self._check_weights()
+        for k, buf in self.static.items():
+            if k not in data:
+                raise ValueError(f"CapturedMatcher was built with `{k}` but the call does not provide it")
+            if tuple(data[k].shape) != tuple(buf.shape):
+                raise ValueError(f"CapturedMatcher: `{k}` has shape {tuple(data[k].shape)}, captured {tuple(buf.shape)}")
+        for k in ("mask0", "mask1", "scale0", "scale1"):
+            if k in data and k not in self.static:
+                raise ValueError(f"CapturedMatcher was built without `{k}`; construct it with masks=/scales=True")
+        with torch.cuda.device(self.device):
+            for k, buf in self.static.items():
+                buf.copy_(data[k])
+            self.graph.replay()
+            m = int(self.out["num_matches"].item())   # the one host sync
+        if m > self.capacity:
+            raise RuntimeError(f"loftr_b200.CapturedMatcher: {m} coarse matches exceed the capacity {self.capacity}; "
+                               "construct it with a larger capacity")
+        res = {}
+        for k, v in self.out.items():
+            if k in self.static or k in ("num_matches", "m_bids", "mkpts0_f"):
+                continue
+            if k in self._TRIMMED:
+                res[k] = v[:m].clone()
+            elif torch.is_tensor(v):
+                res[k] = v.clone()
+            else:
+                res[k] = v
+        res["m_bids"], res["mkpts0_f"] = res["b_ids"], res["mkpts0_c"]   # aliased as in `forward`
+        data.update(res)
