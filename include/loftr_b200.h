@@ -7,7 +7,8 @@
  *   lb_coarse_prep            <- PositionEncodingSine.forward + rearrange   src/loftr/utils/position_encoding.py:37-42,
  *                                                                           src/loftr/loftr.py:58-59
  *   lb_transformer_forward    <- LocalFeatureTransformer.forward            src/loftr/loftr_module/transformer.py:80-101
- *                                (LoFTREncoderLayer.forward :35-58, LinearAttention.forward linear_attention.py:20-47)
+ *                                (LoFTREncoderLayer.forward :35-58, LinearAttention.forward linear_attention.py:20-47,
+ *                                 FullAttention.forward :56-81 for the *_FULL layer kinds)
  *   lb_coarse_match           <- CoarseMatching.forward + get_coarse_match  src/loftr/utils/coarse_matching.py:87-148,150-261
  *                                (Sinkhorn branch: log_optimal_transport, third_party/SuperGluePretrainedNetwork/
  *                                 models/superglue.py:141-170)
@@ -38,6 +39,10 @@ extern "C" {
 #define LB_MATCH_SINKHORN 1
 #define LB_LAYER_SELF 0
 #define LB_LAYER_CROSS 1
+/* full (softmax) attention layers (reference FullAttention, linear_attention.py:50-81): the same weights and token
+ * state as the linear kinds.  Libraries before version 102 reject these kinds ("unknown layer kind"). */
+#define LB_LAYER_SELF_FULL 2
+#define LB_LAYER_CROSS_FULL 3
 
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */

@@ -19,6 +19,8 @@ MATCH_DUAL_SOFTMAX = 0
 MATCH_SINKHORN = 1
 LAYER_SELF = 0
 LAYER_CROSS = 1
+LAYER_SELF_FULL = 2
+LAYER_CROSS_FULL = 3
 
 c_void_p = C.c_void_p
 c_int = C.c_int
@@ -136,6 +138,8 @@ NCCL_UNIQUE_ID_BYTES = 128
 # oldest library whose ABI matches the structures above (101: the device-count fields at the end of
 # LbTransformerState / LbFinePreprocessArgs / LbFineMatchArgs)
 MIN_VERSION = 101
+# oldest library that runs full (softmax) attention layers (LAYER_SELF_FULL / LAYER_CROSS_FULL); older ones reject them
+FULL_ATTENTION_VERSION = 102
 
 
 class LibraryMissing(RuntimeError):
@@ -165,6 +169,14 @@ def load():
         fn.argtypes = args
     _lib = lib
     return lib
+
+
+def require_full_attention(lib):
+    """Raise unless `lib` runs full-attention layers (library version >= FULL_ATTENTION_VERSION)."""
+    v = lib.lb_version()
+    if v < FULL_ATTENTION_VERSION:
+        raise RuntimeError(f"loftr_b200: full attention needs library version {FULL_ATTENTION_VERSION} or newer, but "
+                           f"{LIB_PATH} is version {v}: rebuild it with `make`")
 
 
 def check(rc: int):

@@ -18,6 +18,7 @@
 #include "gemm_split.cuh"
 #include "simt_kernels.cuh"
 #include "kv_gemm.cuh"
+#include "full_attn.cuh"
 #include "stem_tc.cuh"
 #include "comm.cuh"
 
@@ -57,10 +58,10 @@ static int fail(const char* fmt, ...) {
 // Optional per-launch CUDA-event timing of the tensor-core kernels (bench.py's roofline leg): events are
 // recorded on the launching stream right around the kernel, and only while timing is enabled.
 enum Tag { TAG_GEMM_TEST = 0, TAG_PROJ, TAG_MERGE_LN, TAG_MLP1, TAG_MLP2_LN, TAG_SCORE_LSE, TAG_SCORE_ARGMAX,
-           TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_COUNT };
+           TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_FULL_ATTN, TAG_COUNT };
 static const char* kTagNames[TAG_COUNT] = {"gemm_test", "proj_act", "merge_ln", "mlp1_relu", "mlp2_ln_res",
                                            "score_lse", "score_argmax", "fine_merge", "backbone_conv",
-                                           "tf_kv_proj_fused", "tf_q_attn_fused"};
+                                           "tf_kv_proj_fused", "tf_q_attn_fused", "tf_full_attn"};
 struct TimingRec {
   cudaEvent_t e0, e1;
   int tag;
@@ -68,6 +69,27 @@ struct TimingRec {
 static bool g_timing = false;
 static std::vector<TimingRec> g_recs;
 static std::mutex g_timing_mu;
+// Around a launch on `st`: events are only created and recorded while timing is enabled.
+static int timing_begin(TimingRec& rec, cudaStream_t st) {
+  if (!g_timing) return 0;
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  cudaError_t e = cudaStreamIsCapturing(st, &cs);
+  if (e != cudaSuccess) return fail("cudaStreamIsCapturing failed: %s", cudaGetErrorString(e));
+  if (cs != cudaStreamCaptureStatusNone)
+    return fail("kernel timing is enabled (lb_timing_enable) but the stream is being captured into a CUDA graph: "
+                "timing events cannot be recorded into a graph; disable timing before capture");
+  if (cudaEventCreate(&rec.e0) != cudaSuccess || cudaEventCreate(&rec.e1) != cudaSuccess ||
+      cudaEventRecord(rec.e0, st) != cudaSuccess)
+    return fail("timing event set-up failed");
+  return 0;
+}
+static int timing_end(const TimingRec& rec, cudaStream_t st) {
+  if (!g_timing) return 0;
+  if (cudaEventRecord(rec.e1, st) != cudaSuccess) return fail("timing event record failed");
+  std::lock_guard<std::mutex> lk(g_timing_mu);
+  g_recs.push_back(rec);
+  return 0;
+}
 
 // The library carries its own (static) CUDA runtime, whose notion of "current device" is independent of the
 // caller's (e.g. torch's).  Every entry point therefore binds the calling thread to the device that owns the
@@ -305,16 +327,7 @@ static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const t
   const long items = static_cast<long>(s.batches) * s.m_tiles * s.n_chunks;
   const int grid = static_cast<int>(items < sms ? items : sms);
   TimingRec rec{nullptr, nullptr, tag};
-  if (g_timing) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    LB_CUDA(cudaStreamIsCapturing(st, &cs));
-    if (cs != cudaStreamCaptureStatusNone)
-      return fail("kernel timing is enabled (lb_timing_enable) but the stream is being captured into a CUDA graph: "
-                  "timing events cannot be recorded into a graph; disable timing before capture");
-    LB_CUDA(cudaEventCreate(&rec.e0));
-    LB_CUDA(cudaEventCreate(&rec.e1));
-    LB_CUDA(cudaEventRecord(rec.e0, st));
-  }
+  LB_TRY(timing_begin(rec, st));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(grid);
@@ -339,12 +352,7 @@ static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const t
   LB_CUDA(cudaLaunchKernelEx(&cfg, kern, maps.a_hi, maps.a_lo, maps.b_hi, maps.b_lo, maps.ar_hi, maps.ar_lo, maps.br_hi,
                              maps.br_lo, s, ep));
   LB_LAUNCHED();
-  if (g_timing) {
-    LB_CUDA(cudaEventRecord(rec.e1, st));
-    std::lock_guard<std::mutex> lk(g_timing_mu);
-    g_recs.push_back(rec);
-  }
-  return 0;
+  return timing_end(rec, st);
 }
 
 // live / live_unit_rows: optional device bound on the rows of every batch (GemmShape::live_count)
@@ -513,7 +521,7 @@ template <int BN>
 static int tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st, const TfWs& w,
                          long x_base, long x_rows, int x_group_rows, long s_base, long s_rows, int s_group_rows,
                          int n_groups_x, bool self_pass, bool write_f32, cudaStream_t stream, const int* live,
-                         int live_cap);
+                         int live_cap, bool full);
 
 
 // ------------------------------------------------------------------------------------------------ backbone
@@ -626,13 +634,83 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
 
 using namespace lb;
 
+// Steps 1-3 of a coarse (D = 32) encoder-layer call with full (softmax) attention: the message planes att[x rows] =
+// softmax(Q K^T / sqrt(D)) V per group and head            [transformer.py:47-50, linear_attention.py:56-81]
+// Projections carry no feature map and no row zeroing: masks act inside the attention (key weight 0, padded query 0).
+// Q goes to the att planes [R, C] (overwritten in place by the message), K|V to the MLP hidden planes [R, 2C], which
+// are dead at this point of the layer; full_attn_wgmma_kernel (full_attn.cuh) reads both through tensor maps.
+template <int BN>
+static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st,
+                                    const TfWs& w, long x_base, long x_rows, int x_group_rows, long s_base,
+                                    long s_rows, int s_group_rows, int n_groups_x, bool self_pass, cudaStream_t stream) {
+  const long ldc = 2L * C;
+  const __half* cat_hi = static_cast<const __half*>(st.cat_hi);
+  const __half* cat_lo = static_cast<const __half*>(st.cat_lo);
+  const int n_groups_s = static_cast<int>(s_rows / s_group_rows);
+  if (C != 256 || H != 8) return fail("full attention of the coarse transformer is built for d_model 256, 8 heads");
+  if (n_groups_x != n_groups_s && !self_pass) return fail("query / source group counts differ");
+  const __half* wq_hi = static_cast<const __half*>(lw.wqkv_hi);
+  const __half* wq_lo = static_cast<const __half*>(lw.wqkv_lo);
+  const long wkv_off = static_cast<long>(C) * C;   // k_proj, v_proj rows of wqkv
+  {
+    using Epi = EpiPlanes<BN>;
+    Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, 0};
+    Planes B{wq_hi, wq_lo, C, 0};
+    OutMaps om;
+    LB_TRY(fill_out_maps(&om, w.att_hi + x_base * C, w.att_lo + x_base * C, C, nullptr, 0, C, x_rows, 1));
+    typename Epi::Params ep{0, nullptr, 1, nullptr, 0, w.att_hi + x_base * C, w.att_lo + x_base * C, C, 0, lw.s_qkv, om};
+    LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, 1, static_cast<int>(x_rows), C, C, 0, ep, stream)));
+  }
+  {
+    using Epi = EpiPlanes<BN>;
+    Planes A{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, 0};
+    Planes B{wq_hi + wkv_off, wq_lo + wkv_off, C, 0};
+    OutMaps om;
+    LB_TRY(fill_out_maps(&om, w.h_hi + s_base * ldc, w.h_lo + s_base * ldc, ldc, nullptr, 0, 2 * C, s_rows, 1));
+    typename Epi::Params ep{0, nullptr, 1, nullptr, 0, w.h_hi + s_base * ldc, w.h_lo + s_base * ldc,
+                            static_cast<int>(ldc), 0, lw.s_qkv, om};
+    LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, 1, static_cast<int>(s_rows), 2 * C, C, 0, ep, stream)));
+  }
+  const long qbs = static_cast<long>(x_group_rows) * C, kvbs = static_cast<long>(s_group_rows) * ldc;
+  CUtensorMap tq_hi, tq_lo, tkv_hi, tkv_lo;
+  LB_TRY(make_map(&tq_hi, w.att_hi + x_base * C, C, x_group_rows, n_groups_x, C, qbs, kFaRows, kFaD));
+  LB_TRY(make_map(&tq_lo, w.att_lo + x_base * C, C, x_group_rows, n_groups_x, C, qbs, kFaRows, kFaD));
+  LB_TRY(make_map(&tkv_hi, w.h_hi + s_base * ldc, 2 * C, s_group_rows, n_groups_s, ldc, kvbs, kFaKeys, kFaD));
+  LB_TRY(make_map(&tkv_lo, w.h_lo + s_base * ldc, 2 * C, s_group_rows, n_groups_s, ldc, kvbs, kFaKeys, kFaD));
+  static bool configured[kMaxDevices] = {false};
+  int dev = 0;
+  LB_CUDA(cudaGetDevice(&dev));
+  if (!configured[dev]) {
+    LB_CUDA(cudaFuncSetAttribute(full_attn_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwSmem));
+    configured[dev] = true;
+  }
+  FullAttnWgParams wp;
+  wp.Lx = x_group_rows;
+  wp.Ls = s_group_rows;
+  wp.v_col0 = C;
+  wp.x_base = x_base;
+  wp.s_base = s_base;
+  wp.mask = st.mask;
+  wp.o_hi = w.att_hi;
+  wp.o_lo = w.att_lo;
+  wp.ld_o = C;
+  wp.scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(kFaD));
+  const dim3 grid(cdiv(x_group_rows, kFaRows), H, n_groups_x);
+  TimingRec rec{nullptr, nullptr, TAG_FULL_ATTN};
+  LB_TRY(timing_begin(rec, stream));
+  full_attn_wgmma_kernel<<<grid, kFwThreads, kFwSmem, stream>>>(tq_hi, tq_lo, tkv_hi, tkv_lo, wp);
+  LB_LAUNCHED();
+  LB_TRY(timing_end(rec, stream));
+  return 0;
+}
+
 // Runs one encoder-layer call `x <- layer(x, source)` for the row range x (queries) / s (source).
 // self_pass: x range == source range (q, k, v in one projection launch).
 template <int BN>
 static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st,
                              const TfWs& w, long x_base, long x_rows, int x_group_rows, long s_base, long s_rows,
                              int s_group_rows, int n_groups_x, bool self_pass, bool write_f32, cudaStream_t stream,
-                             const int* live, int live_cap) {
+                             const int* live, int live_cap, bool full) {
   const int D = C / H;
   const long ldc = 2L * C;
   const __half* cat_hi = static_cast<const __half*>(st.cat_hi);
@@ -641,7 +719,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   const int n_groups_s = static_cast<int>(s_rows / s_group_rows);
   const int per = D * D + D;
   if (n_groups_x != n_groups_s && !self_pass) return fail("query / source group counts differ");
-  const bool fused = (D == 32) && use_fused_attn() && lw.wkv_hi != nullptr;
+  const bool fused = !full && (D == 32) && use_fused_attn() && lw.wkv_hi != nullptr;
   // Device-bounded window transformer (`live` != nullptr): every set of live_cap windows is one GEMM batch of
   // live_cap * group_rows rows whose live prefix is read on the device, so a self pass over both sets is a two-batch
   // GEMM.  Without a bound every row range is one batch (xb = sb = 1), as it always was.
@@ -652,6 +730,14 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   const long xbs_a = xb > 1 ? static_cast<long>(xM) * C : 0;       // attention planes [R, C]
   if (live && (fused || D != 16 || x_group_rows != s_group_rows))
     return fail("device-bounded group counts are built for the fine (window) transformer only");
+  // full attention: the coarse layers run tf_full_attention_coarse; the fine (window) layers share the projections of
+  // the window path below (no elu+1 feature map, no row zeroing) and run window_full_attn_kernel
+  const bool full_coarse = full && D == 32;
+  if (full_coarse) {
+    if (live) return fail("device-bounded group counts are built for the fine (window) transformer only");
+    LB_TRY(tf_full_attention_coarse<BN>(lw, C, H, st, w, x_base, x_rows, x_group_rows, s_base, s_rows, s_group_rows,
+                                        n_groups_x, self_pass, stream));
+  }
 
   if constexpr (BN == 256) {
     if (fused) {
@@ -725,9 +811,12 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
       }
     }
   }
-  if (!fused) {
+  if (!fused && !full_coarse) {
   if (!w.qkv) return fail("first-generation attention path needs LOFTR_B200_FUSED_ATTN=0 (no q/k/v workspace was carved)");
   // 1. projections (+ elu+1 feature map + padding mask)      [transformer.py:47-49, linear_attention.py:31-39]
+  //    full attention: plain projections; the window kernel applies the mask
+  const int elu_self = full ? 0 : 2 * C, elu_q = full ? 0 : C, elu_kv = full ? 0 : C;
+  const uint8_t* pmask = full ? nullptr : mask;
   {
     using Epi = EpiActStore<BN>;
     if (self_pass) {
@@ -735,7 +824,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
       Planes B{lw.wqkv_hi, lw.wqkv_lo, C, 0};
       OutMaps om;
       LB_TRY(fill_out_maps(&om, nullptr, nullptr, 0, w.qkv + x_base * 3 * C, 3 * C, 3 * C, xM, xb));
-      typename Epi::Params ep{w.qkv + x_base * 3 * C, 3 * C, 2 * C, mask ? mask + x_base : nullptr, lw.s_qkv, 0, om};
+      typename Epi::Params ep{w.qkv + x_base * 3 * C, 3 * C, elu_self, pmask ? pmask + x_base : nullptr, lw.s_qkv, 0, om};
       LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, xb, xM, 3 * C, C, 0, ep, stream, live, x_group_rows)));
     } else {
       Planes Aq{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, xbs};
@@ -743,12 +832,12 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
       OutMaps omq, omk;
       LB_TRY(fill_out_maps(&omq, nullptr, nullptr, 0, w.qkv + x_base * 3 * C, 3 * C, C, xM, xb));
       LB_TRY(fill_out_maps(&omk, nullptr, nullptr, 0, w.qkv + s_base * 3 * C + C, 3 * C, 2 * C, sM, sb));
-      typename Epi::Params eq{w.qkv + x_base * 3 * C, 3 * C, C, mask ? mask + x_base : nullptr, lw.s_qkv, 0, omq};
+      typename Epi::Params eq{w.qkv + x_base * 3 * C, 3 * C, elu_q, pmask ? pmask + x_base : nullptr, lw.s_qkv, 0, omq};
       LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Aq, Bq, xb, xM, C, C, 0, eq, stream, live, x_group_rows)));
       Planes Ak{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, sbs};
       Planes Bk{static_cast<const __half*>(lw.wqkv_hi) + static_cast<long>(C) * C,
                 static_cast<const __half*>(lw.wqkv_lo) + static_cast<long>(C) * C, C, 0};
-      typename Epi::Params ek{w.qkv + s_base * 3 * C + C, 3 * C, C, mask ? mask + s_base : nullptr, lw.s_qkv, 0, omk};
+      typename Epi::Params ek{w.qkv + s_base * 3 * C + C, 3 * C, elu_kv, pmask ? pmask + s_base : nullptr, lw.s_qkv, 0, omk};
       LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Ak, Bk, sb, sM, 2 * C, C, 0, ek, stream, live, s_group_rows)));
     }
   }
@@ -760,7 +849,18 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   }
   const bool one_kernel = D == 16 && H == 8 && window_fused && s_group_rows <= 32 && x_group_rows == s_group_rows &&
                           n_groups_x == n_groups_s;
-  if (one_kernel) {
+  if (full) {
+    // 2+3 full (softmax) attention of the windows, exact fp32                [linear_attention.py:56-81]
+    if (!(D == 16 && H == 8 && s_group_rows <= 32 && x_group_rows == s_group_rows && n_groups_x == n_groups_s))
+      return fail("full window attention is built for 128/8 with equal groups of at most 32 rows");
+    int sms = 0;
+    LB_TRY(device_check(&sms));
+    const int grid = n_groups_x < 4 * sms ? n_groups_x : 4 * sms;
+    window_full_attn_kernel<16, 8, 32><<<grid, 256, 0, stream>>>(w.qkv, 3 * C, 0, C, 2 * C, x_base, s_base,
+                                                                 x_group_rows, n_groups_x, mask, w.att_hi, w.att_lo,
+                                                                 C, live, live_cap);
+    LB_LAUNCHED();
+  } else if (one_kernel) {
     int sms = 0;
     LB_TRY(device_check(&sms));
     const int grid = n_groups_x < 3 * sms ? n_groups_x : 3 * sms;   // 3 resident blocks per SM (60 KB, <= 85 registers)
@@ -810,7 +910,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   }
   LB_LAUNCHED();
   }  // !one_kernel
-  }  // !fused
+  }  // !fused && !full_coarse
   // 4. merge + norm1 -> cat[:, C:2C]                            [transformer.py:51-52]
   {
     using Epi = EpiLayerNorm<BN>;
@@ -857,7 +957,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
 
 extern "C" {
 
-int lb_version(void) { return 101; }
+int lb_version(void) { return 102; }
 int lb_block_k(void) { return kBlockK; }
 int lb_conv_layout(int cin, int* cin_blocks, int* rem_channels) {
   if (!cin_blocks || !rem_channels || cin <= 0) return fail("lb_conv_layout: bad arguments");
@@ -1111,12 +1211,15 @@ int lb_transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds
   for (int l = 0; l < n_layers; ++l) {
     const LbEncoderLayerWeights& lw = layers[l];
     const bool last = l == n_layers - 1;   // the fp32 copy of the features is only written after the last layer
+    const int kind = kinds[l];
+    const bool full = kind == LB_LAYER_SELF_FULL || kind == LB_LAYER_CROSS_FULL;
     auto pass = [&](long xb, long xr, int xg, long sb, long sr, int sg, int ng, bool self_pass) -> int {
-      return coarse ? tf_layer_pass<256>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s, nullptr, 0)
+      return coarse ? tf_layer_pass<256>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s, nullptr, 0,
+                                         full)
                     : tf_layer_pass<128>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s, live,
-                                         st->n_groups);
+                                         st->n_groups, full);
     };
-    if (kinds[l] == LB_LAYER_SELF) {
+    if (kind == LB_LAYER_SELF || kind == LB_LAYER_SELF_FULL) {
       // feat0 = layer(feat0, feat0); feat1 = layer(feat1, feat1)  [transformer.py:93-94]; same weights,
       // independent -> one pass over both sets when the group sizes agree.
       if (same_groups) {
@@ -1125,12 +1228,12 @@ int lb_transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds
         LB_TRY(pass(0, rows0, st->group_rows0, 0, rows0, st->group_rows0, st->n_groups, true));
         LB_TRY(pass(rows0, rows1, st->group_rows1, rows0, rows1, st->group_rows1, st->n_groups, true));
       }
-    } else if (kinds[l] == LB_LAYER_CROSS) {
+    } else if (kind == LB_LAYER_CROSS || kind == LB_LAYER_CROSS_FULL) {
       // feat0 = layer(feat0, feat1); feat1 = layer(feat1, feat0_new)  [transformer.py:96-97]
       LB_TRY(pass(0, rows0, st->group_rows0, rows0, rows1, st->group_rows1, st->n_groups, false));
       LB_TRY(pass(rows0, rows1, st->group_rows1, 0, rows0, st->group_rows0, st->n_groups, false));
     } else {
-      return fail("unknown layer kind %d", kinds[l]);
+      return fail("unknown layer kind %d", kind);
     }
   }
   return 0;

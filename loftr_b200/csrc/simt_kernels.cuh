@@ -522,6 +522,107 @@ __global__ void __launch_bounds__(32 * H, 3) window_attn_kernel(const float* __r
 }
 
 // ------------------------------------------------------------------------------------------------
+// Fine (window) full attention: message = softmax(q k^T / sqrt(D)) v over the rows of one window per head (reference
+// linear_attention.py:56-81 on the [M, 25, 128] window sequences), exact fp32 on the CUDA cores.  One block takes
+// windows g, g + gridDim.x, ...; the window's K / V rows are staged in shared memory and warp h / lane r computes
+// query row r of head h: scores, max, exponentials, sum and the weighted V rows in a fixed order (deterministic).
+// Keys with mask 0 get weight 0; padded query rows and rows without a valid key write 0.  Same device bound as
+// window_attn_kernel: with `live`, only windows [0, min(*live, live_cap)) of every set of live_cap are visited.
+template <int D, int H, int MAXR>
+__global__ void __launch_bounds__(32 * H) window_full_attn_kernel(const float* __restrict__ qkv, int ld, int q_col0,
+                                                                  int k_col0, int v_col0, long x_row_base,
+                                                                  long s_row_base, int rows_per_group, int n_groups,
+                                                                  const uint8_t* __restrict__ mask,
+                                                                  __half* __restrict__ att_hi,
+                                                                  __half* __restrict__ att_lo, int ld_att,
+                                                                  const int* __restrict__ live, int live_cap) {
+  pdl_trigger();
+  static_assert(D % 8 == 0 && MAXR <= 32, "window head layout");
+  constexpr int C = D * H;
+  __shared__ __align__(16) float sK[MAXR * C];
+  __shared__ __align__(16) float sV[MAXR * C];
+  __shared__ float sBias[MAXR];
+  const int tid = threadIdx.x;
+  const int hd = tid >> 5, lane = tid & 31;
+  const bool has_row = lane < rows_per_group;
+  const float scale = rsqrtf(static_cast<float>(D));
+
+  int n_items = n_groups, n_live = n_groups, cap = n_groups;
+  if (live != nullptr) {
+    cap = live_cap;
+    n_live = min(max(*live, 0), live_cap);
+    n_items = n_live * (n_groups / live_cap);
+  }
+  for (int v = blockIdx.x; v < n_items; v += gridDim.x) {
+    const int g = v / n_live * cap + v % n_live;
+    const long srow = s_row_base + static_cast<long>(g) * rows_per_group;
+    const long xrow = x_row_base + static_cast<long>(g) * rows_per_group + lane;
+    for (int i = tid; i < rows_per_group * (C / 4); i += 32 * H) {
+      const int r = i / (C / 4), c4 = (i % (C / 4)) * 4;
+      const float* rowp = qkv + (srow + r) * ld;
+      *reinterpret_cast<float4*>(sK + r * C + c4) = *reinterpret_cast<const float4*>(rowp + k_col0 + c4);
+      *reinterpret_cast<float4*>(sV + r * C + c4) = *reinterpret_cast<const float4*>(rowp + v_col0 + c4);
+    }
+    if (tid < rows_per_group) sBias[tid] = (mask == nullptr || mask[srow + tid] != 0) ? 0.f : -INFINITY;
+    float q[D];
+    if (has_row) {
+      const float4* qp = reinterpret_cast<const float4*>(qkv + xrow * ld + q_col0 + hd * D);
+#pragma unroll
+      for (int j = 0; j < D / 4; ++j) {
+        const float4 t = qp[j];
+        q[4 * j] = t.x; q[4 * j + 1] = t.y; q[4 * j + 2] = t.z; q[4 * j + 3] = t.w;
+      }
+    }
+    __syncthreads();
+    if (has_row) {
+      float s[MAXR];
+      float m = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < MAXR; ++j) {
+        s[j] = -INFINITY;
+        if (j < rows_per_group) {
+          const float* kr = sK + j * C + hd * D;
+          float a = 0.f;
+#pragma unroll
+          for (int d = 0; d < D; ++d) a = fmaf(q[d], kr[d], a);
+          s[j] = a * scale + sBias[j];
+          m = fmaxf(m, s[j]);
+        }
+      }
+      float o[D];
+#pragma unroll
+      for (int d = 0; d < D; ++d) o[d] = 0.f;
+      float sum = 0.f;
+      if (m != -INFINITY) {
+#pragma unroll
+        for (int j = 0; j < MAXR; ++j) {
+          if (j < rows_per_group) {
+            const float pj = expf(s[j] - m);
+            sum += pj;
+            const float* vr = sV + j * C + hd * D;
+#pragma unroll
+            for (int d = 0; d < D; ++d) o[d] = fmaf(pj, vr[d], o[d]);
+          }
+        }
+      }
+      const bool q_ok = mask == nullptr || mask[xrow] != 0;
+      const float inv = (q_ok && sum > 0.f) ? 1.f / sum : 0.f;
+      __half* hp = att_hi + xrow * ld_att + hd * D;
+      __half* lp = att_lo + xrow * ld_att + hd * D;
+#pragma unroll
+      for (int v8 = 0; v8 < D; v8 += 8) {
+        uint32_t hw[4], lw[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) split_f16x2(o[v8 + 2 * j] * inv, o[v8 + 2 * j + 1] * inv, hw[j], lw[j]);
+        *reinterpret_cast<uint4*>(hp + v8) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+        *reinterpret_cast<uint4*>(lp + v8) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+      }
+    }
+    __syncthreads();   // the K / V rows are overwritten by the next window
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Merge log-sum-exp partials: out[i] = base - LSE(parts[:, i] U {dustbin term}).
 //   dual-softmax:  base = 0, no dustbin   -> out = -LSE (the additive log-normaliser)
 //   Sinkhorn:      base = log_mu / log_nu, dustbin term = bin + bin_pot[pair]   (superglue.py:146-147)

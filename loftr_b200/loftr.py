@@ -27,7 +27,9 @@ import torch.nn as nn
 from . import _lib
 from .backbone import build_backbone
 
-_KIND = {"self": _lib.LAYER_SELF, "cross": _lib.LAYER_CROSS}
+_KIND = {("self", "linear"): _lib.LAYER_SELF, ("cross", "linear"): _lib.LAYER_CROSS,
+         ("self", "full"): _lib.LAYER_SELF_FULL, ("cross", "full"): _lib.LAYER_CROSS_FULL}
+ATTENTIONS = ("linear", "full")   # reference config: coarse.attention / fine.attention, options ['linear', 'full']
 
 
 def _stream(ref=None):
@@ -230,12 +232,14 @@ class PositionEncodingSine(nn.Module):
 
 
 class LoFTREncoderLayer(nn.Module):
-    """Parameter holder with the reference's names/shapes (transformer.py:8-33)."""
+    """Parameter holder with the reference's names/shapes (transformer.py:8-33).  `attention` ('linear' | 'full')
+    selects the attention kernels; both kinds have the same parameters."""
 
     def __init__(self, d_model, nhead, attention="linear"):
         super().__init__()
-        if attention != "linear":
-            raise NotImplementedError("only the linear-attention encoder is built (no shipped config uses 'full')")
+        if attention not in ATTENTIONS:
+            raise ValueError(f"attention must be one of {ATTENTIONS} (got {attention!r})")
+        self.attention = attention
         self.dim = d_model // nhead
         self.nhead = nhead
         self.q_proj = nn.Linear(d_model, d_model, bias=False)
@@ -260,7 +264,7 @@ class _TokenState:
 
 
 class LocalFeatureTransformer(_PackedCacheMixin, nn.Module):
-    """Interleaved self/cross linear-attention encoder (reference transformer.py:61-101)."""
+    """Interleaved self/cross encoder with linear or full (softmax) attention (reference transformer.py:61-101)."""
 
     def __init__(self, config):
         super().__init__()
@@ -293,7 +297,7 @@ class LocalFeatureTransformer(_PackedCacheMixin, nn.Module):
                 lns = [t.detach().float().contiguous() for t in lns]
                 w = arr[i]
                 c, d = self.d_model, self.d_model // self.nhead
-                if d == 32 and c == 256:
+                if d == 32 and c == 256 and layer.attention == "linear":
                     # fused k|v projection: k and v rows regrouped in blocks of 4 heads (128 rows)
                     idx = torch.cat([torch.arange(c + blk * 128, c + blk * 128 + 128).repeat(1) if part == 0 else
                                      torch.arange(2 * c + blk * 128, 2 * c + blk * 128 + 128)
@@ -306,7 +310,8 @@ class LocalFeatureTransformer(_PackedCacheMixin, nn.Module):
                     (h.data_ptr(), l.data_ptr()) for h, l in planes[:4]]
                 w.ln1_g, w.ln1_b, w.ln2_g, w.ln2_b = [t.data_ptr() for t in lns]
                 w.s_qkv, w.s_m, w.s_1, w.s_2 = [sc for _, _, sc in scaled]
-        kinds = (C.c_int * len(self.layers))(*[_KIND[n] for n in self.layer_names])
+        kinds = (C.c_int * len(self.layers))(*[_KIND[n, layer.attention] for n, layer in zip(self.layer_names,
+                                                                                              self.layers)])
         self._packed = (arr, kinds, keep)
         self._packed_key = key
         return self._packed
@@ -316,6 +321,8 @@ class LocalFeatureTransformer(_PackedCacheMixin, nn.Module):
         int32 device count; `n_groups` is then the capacity and only the first min(live, n_groups) windows of each set
         are computed."""
         lib = _lib.load()
+        if any(layer.attention == "full" for layer in self.layers):
+            _lib.require_full_attention(lib)   # an older library would reject the layer kinds at the first launch
         arr, kinds, _ = self._pack(state.x.device)
         st = _lib.LbTransformerState(state.x.data_ptr(), state.cat_hi.data_ptr(), state.cat_lo.data_ptr(),
                                      _lib.ptr(mask_u8), n_groups, group_rows0, group_rows1, _lib.ptr(live))
