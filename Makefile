@@ -16,11 +16,6 @@ build/bringup: tests/cuda/bringup.cu $(LIB)
 	@mkdir -p build
 	$(NVCC) $(ARCH) -O2 -std=c++17 tests/cuda/bringup.cu -o $@ -Lloftr_b200/lib -lloftr_b200 -Xlinker -rpath -Xlinker '$$ORIGIN/../loftr_b200/lib'
 
-# A/B build variants of the same sources (selected at run time with LOFTR_B200_LIB=<variant>)
-variants: loftr_b200/lib/libloftr_b200_nocoal.so
-loftr_b200/lib/libloftr_b200_nocoal.so: $(CSRC)/engine.cu $(HDRS)
-	$(NVCC) $(NVFLAGS) -DLB_COALESCE=0 -shared $(CSRC)/engine.cu -o $@ -ldl
-
 clean:
 	rm -rf build loftr_b200/lib
 

@@ -44,6 +44,8 @@ extern "C" {
 #define LB_LAYER_SELF_FULL 2
 #define LB_LAYER_CROSS_FULL 3
 
+/* 101: device-count fields appended to LbTransformerState / LbFinePreprocessArgs / LbFineMatchArgs;
+ * 102: full-attention layer kinds; 103: lb_selftest removed (no structure changes). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -54,11 +56,6 @@ int lb_conv_layout(int cin, int* cin_blocks /*host*/, int* rem_channels /*host*/
 const char* lb_last_error(void);
 /* number of kernels this library has launched in this process (for bench.py's gpu_launches) */
 long long lb_launch_count(void);
-
-/* Device self-test: runs both generations of the CUDA-core kernels that have two (kv_partial, stem convolution) on
- * identical inputs at production shapes, compares the outputs bit for bit and times them; writes a text report.
- * Returns non-zero if any pair differs.  Allocates and frees its own device buffers; synchronises. */
-int lb_selftest(char* report /*host*/, int report_len);
 
 /* Optional per-launch CUDA-event timing of the tensor-core kernels (events recorded on the launching
  * stream around each kernel while enabled).  lb_timing_enable(1) clears old records and starts recording,

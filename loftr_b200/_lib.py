@@ -10,8 +10,8 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# LOFTR_B200_LIB selects an alternative build of the same sources (e.g. "k32" -> libloftr_b200_k32.so, the
-# 32-element k-block variant used for A/B measurements)
+# LOFTR_B200_LIB selects another build of the library under lib/ (e.g. "base" -> libloftr_b200_base.so), so that two
+# builds can be compared in the same tree
 _VARIANT = os.environ.get("LOFTR_B200_LIB", "")
 LIB_PATH = os.path.join(_HERE, "lib", f"libloftr_b200{'_' + _VARIANT if _VARIANT else ''}.so")
 
@@ -102,7 +102,6 @@ SIGNATURES = {
     "lb_conv_layout": (c_int, [c_int, C.POINTER(c_int), C.POINTER(c_int)]),
     "lb_last_error": (C.c_char_p, []),
     "lb_launch_count": (C.c_longlong, []),
-    "lb_selftest": (c_int, [C.c_char_p, c_int]),
     "lb_timing_enable": (c_int, [c_int]),
     "lb_timing_num_tags": (c_int, []),
     "lb_timing_tag_name": (C.c_char_p, [c_int]),

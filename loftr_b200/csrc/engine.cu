@@ -205,16 +205,7 @@ static int make_map_nhwc(CUtensorMap* m, const void* base, int C, int W, int H, 
   return 0;
 }
 
-// ---- output tensor maps for the TMA-store epilogues (epilogues.cuh OutMaps).  LOFTR_B200_TMA_STORE=0 disables them
-// (the epilogues then use their pointer-based store paths) for A/B measurements.
-static bool use_tma_store() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("LOFTR_B200_TMA_STORE");
-    v = e ? (atoi(e) != 0 ? 1 : 0) : 1;
-  }
-  return v == 1;
-}
+// ---- output tensor maps for the TMA-store epilogues (epilogues.cuh OutMaps)
 // [batches][rows][cols] matrix (row stride ld, batch stride bs elements; bs = 0 -> rows * ld): box 32 x 32 x 1,
 // 64-byte swizzle for fp16 planes, 128-byte swizzle for fp32
 static int make_out_map(CUtensorMap* m, const void* base, bool f32, long cols, long rows, long batches, long ld, long bs) {
@@ -255,7 +246,6 @@ static int fill_out_maps(OutMaps* om, const void* hi, const void* lo, long ld_pl
                          long rows, long batches) {
   memset(om, 0, sizeof(*om));
   om->dims = 3;
-  if (!use_tma_store()) return 0;
   if (hi) {
     LB_TRY(make_out_map(&om->hi, hi, false, cols, rows, batches, ld_pl, 0));
     LB_TRY(make_out_map(&om->lo, lo, false, cols, rows, batches, ld_pl, 0));
@@ -276,35 +266,6 @@ struct Planes {
 };
 
 // ------------------------------------------------------------------------------------------------ GEMM launch
-// Second-generation CUDA-core kernels (kv_partial_v2, conv_stem7x7_v2).  They produce bit-identical results to the
-// first versions (checked on the device by lb_selftest, which also times both); LOFTR_B200_V2=0|1 overrides.
-// Defaults: the stem v2, kv_partial v1 (the v2's 32-accumulator inner loop is shared-memory-read bound).
-#ifndef LB_KV_V2_DEFAULT
-#define LB_KV_V2_DEFAULT 0
-#endif
-#ifndef LB_STEM_V2_DEFAULT
-#define LB_STEM_V2_DEFAULT 1
-#endif
-// Fused linear attention (EpiKv / EpiAttn epilogues, coarse transformer): LOFTR_B200_FUSED_ATTN=0 restores the
-// first-generation path (fp32 q/k/v in HBM + kv_partial / attn_apply kernels) for A/B measurements.
-static bool use_fused_attn() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("LOFTR_B200_FUSED_ATTN");
-    v = e ? (atoi(e) != 0 ? 1 : 0) : 1;
-  }
-  return v == 1;
-}
-static bool use_v2(int which /*0 = kv_partial, 1 = stem*/) {
-  static int forced = -2;
-  if (forced == -2) {
-    const char* e = getenv("LOFTR_B200_V2");
-    forced = e ? (atoi(e) != 0 ? 1 : 0) : -1;
-  }
-  if (forced >= 0) return forced == 1;
-  return which == 0 ? (LB_KV_V2_DEFAULT != 0) : (LB_STEM_V2_DEFAULT != 0);
-}
-
 struct GemmMaps {
   CUtensorMap a_hi, a_lo, b_hi, b_lo;      // 64-element k-blocks
   CUtensorMap ar_hi, ar_lo, br_hi, br_lo;  // convolution channel remainder (16-element boxes); copies of the above if unused
@@ -399,13 +360,8 @@ struct ConvDesc {
 // K layout of a convolution's implicit GEMM: `cin_blocks` 64-channel blocks per tap, plus `rem` (<= 16) remainder
 // channels per tap that travel as 16-channel boxes (gemm_split.cuh ConvGeom).
 static void conv_layout(int cin, int* cin_blocks, int* rem) {
-  static int enabled = -1;   // LOFTR_B200_CONV_REM=0: pad every tap to whole 64-channel blocks (first-generation layout)
-  if (enabled < 0) {
-    const char* e = getenv("LOFTR_B200_CONV_REM");
-    enabled = e ? (atoi(e) != 0 ? 1 : 0) : 1;
-  }
   const int r = cin % kBlockK;
-  if (enabled && kBlockK == 64 && cin > kBlockK && r > 0 && r <= kRemChannels) {
+  if (kBlockK == 64 && cin > kBlockK && r > 0 && r <= kRemChannels) {
     *cin_blocks = cin / kBlockK;
     *rem = r;
   } else {
@@ -493,20 +449,23 @@ static inline int cdiv(long a, long b) { return static_cast<int>((a + b - 1) / b
 
 // ------------------------------------------------------------------------------------------------ transformer
 struct TfWs {
-  float* qkv;       // [R, 3C]
+  float* qkv;       // fine only: [R, 3C]
   __half* att_hi;   // [R, C]
   __half* att_lo;
   __half* h_hi;     // [R, 2C]
   __half* h_lo;
   float* kv;        // [2*n_groups, H, D*D + D]
-  float* kv_part;   // coarse only: max([2*n_groups, H, splits, per], [2*n_groups, m_tiles, H, per]) (split / tile partials)
+  float* kv_part;   // coarse only: [2*n_groups, max(m_tiles, kKvSplits), H, per] (K^T V split partials)
 };
+// kv_gemm_kernel sums K^T V over at most max(m_tiles, kKvSplits) row splits per group.  That bound sizes kv_part here
+// and caps `splits` in tf_linear_attention_coarse; `splits` fixes the summation order of K^T V, so changing either
+// formula changes the output bits.
 constexpr int kKvSplits = 8;
 
 static void carve_tf(Bump& b, TfWs& w, int C, int H, long R, int n_groups, bool coarse, int max_group_rows) {
   const int D = C / H;
-  // fp32 q|k|v: the fine (window) transformer and the first-generation coarse path
-  w.qkv = (coarse && use_fused_attn()) ? nullptr : b.take<float>(static_cast<size_t>(R) * 3 * C);
+  // fp32 q|k|v of the fine (window) transformer; the coarse projections write planes
+  w.qkv = coarse ? nullptr : b.take<float>(static_cast<size_t>(R) * 3 * C);
   w.att_hi = b.take<__half>(static_cast<size_t>(R) * C);
   w.att_lo = b.take<__half>(static_cast<size_t>(R) * C);
   w.h_hi = b.take<__half>(static_cast<size_t>(R) * 2 * C);
@@ -589,16 +548,14 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
   OutMaps om;
   memset(&om, 0, sizeof(om));
   om.dims = 4;
-  if (use_tma_store()) {
-    if (r.out) {
-      LB_TRY(make_out_map_nhwc(&om.hi, r.out->hi, false, d.Cout, d.W_out, d.H_out, N, r.out->ld));
-      LB_TRY(make_out_map_nhwc(&om.lo, r.out->lo, false, d.Cout, d.W_out, d.H_out, N, r.out->ld));
-      om.use |= 1;
-    }
-    if (r.out_f32) {
-      LB_TRY(make_out_map_nhwc(&om.f32, r.out_f32, true, d.Cout, d.W_out, d.H_out, N, r.f32_ld));
-      om.use |= 2;
-    }
+  if (r.out) {
+    LB_TRY(make_out_map_nhwc(&om.hi, r.out->hi, false, d.Cout, d.W_out, d.H_out, N, r.out->ld));
+    LB_TRY(make_out_map_nhwc(&om.lo, r.out->lo, false, d.Cout, d.W_out, d.H_out, N, r.out->ld));
+    om.use |= 1;
+  }
+  if (r.out_f32) {
+    LB_TRY(make_out_map_nhwc(&om.f32, r.out_f32, true, d.Cout, d.W_out, d.H_out, N, r.f32_ld));
+    om.use |= 2;
   }
 #define LB_CONV_CASE_UP(BN, UP)                                                                                       \
   {                                                                                                                   \
@@ -617,13 +574,8 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
   UpMaps um;
   memset(&um, 0, sizeof(um));
   // output-channel tile: the smallest built N that covers Cout (196 -> 208: 13 x 16, no MMAs on 60 padding columns)
-  static int n208 = -1;   // LOFTR_B200_CONV_N208=0: 256-column tiles for Cout = 196 (first-generation tiling)
-  if (n208 < 0) {
-    const char* e = getenv("LOFTR_B200_CONV_N208");
-    n208 = e ? (atoi(e) != 0 ? 1 : 0) : 1;
-  }
   if (w.cout <= 128) LB_CONV_CASE(128)
-  if (w.cout <= 208 && n208) LB_CONV_CASE(208)
+  if (w.cout <= 208) LB_CONV_CASE(208)
   if (w.cout <= 256) LB_CONV_CASE(256)
 #undef LB_CONV_CASE
 #undef LB_CONV_CASE_UP
@@ -704,6 +656,73 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
   return 0;
 }
 
+// Steps 1-3 of a coarse (D = 32) encoder-layer call with linear attention (SURVEY.md §2a G1/G2): the k|v projection
+// writes K = elu(k)+1 and V as planes, kv_gemm_kernel reduces them to K^T V and Ksum on the tensor cores, and the q
+// projection applies the attention in its epilogue; q, k, v never reach HBM.
+//                                                   [transformer.py:47-50, linear_attention.py:31-46]
+static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st,
+                                      const TfWs& w, long x_base, int x_group_rows, long s_base, int s_group_rows,
+                                      int n_groups_x, int n_groups_s, cudaStream_t stream) {
+  if (!lw.wkv_hi || !lw.wkv_lo)
+    return fail("linear attention of the coarse transformer needs the fused k|v weight planes (wkv_hi / wkv_lo)");
+  const int D = C / H;
+  const int per = D * D + D;
+  const long ldc = 2L * C;
+  const __half* cat_hi = static_cast<const __half*>(st.cat_hi);
+  const __half* cat_lo = static_cast<const __half*>(st.cat_lo);
+  const uint8_t* mask = st.mask;
+  int sms = 0;
+  LB_TRY(device_check(&sms));
+  __half* kvp_hi = w.h_hi + s_base * ldc;   // the MLP hidden planes [R, 2C] are free at this point of the layer
+  __half* kvp_lo = w.h_lo + s_base * ldc;
+  {
+    using Epi = EpiKvProj<256>;
+    Planes A{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, static_cast<long>(s_group_rows) * ldc};
+    Planes B{lw.wkv_hi, lw.wkv_lo, C, 0};
+    typename Epi::Params ep;
+    ep.rowmask = mask ? mask + s_base : nullptr;
+    ep.acc_scale = lw.s_qkv;
+    LB_TRY(fill_out_maps(&ep.om, kvp_hi, kvp_lo, ldc, nullptr, 0, 2 * C, s_group_rows, n_groups_s));
+    LB_TRY((launch_gemm<256, Epi>(TAG_KV, A, B, n_groups_s, s_group_rows, 2 * C, C, 0, ep, stream)));
+  }
+  {
+    CUtensorMap tm_hi, tm_lo;
+    LB_TRY(make_map(&tm_hi, kvp_hi, 2 * C, s_group_rows, n_groups_s, ldc, static_cast<long>(s_group_rows) * ldc, 64, 64));
+    LB_TRY(make_map(&tm_lo, kvp_lo, 2 * C, s_group_rows, n_groups_s, ldc, static_cast<long>(s_group_rows) * ldc, 64, 64));
+    const int kb_total = cdiv(s_group_rows, 64);
+    const int m_tiles_s = cdiv(s_group_rows, kBlockM);
+    const int parts_cap = m_tiles_s > kKvSplits ? m_tiles_s : kKvSplits;   // capacity of kv_part (see kKvSplits)
+    int splits = sms / (2 * n_groups_s);
+    if (splits < 1) splits = 1;
+    if (splits > kb_total) splits = kb_total;
+    if (splits > parts_cap) splits = parts_cap;
+    const int kb_per = cdiv(kb_total, splits);
+    splits = cdiv(kb_total, kb_per);
+    static bool configured[kMaxDevices] = {false};
+    int dev = 0;
+    LB_CUDA(cudaGetDevice(&dev));
+    if (!configured[dev]) {
+      LB_CUDA(cudaFuncSetAttribute(kv_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kKvGemmSmem));
+      configured[dev] = true;
+    }
+    KvGemmParams kp{w.kv_part, kb_total, kb_per, splits};
+    kv_gemm_kernel<<<dim3(splits, 2, n_groups_s), kKvGemmThreads, kKvGemmSmem, stream>>>(tm_hi, tm_lo, kp);
+    LB_LAUNCHED();
+    const long total = static_cast<long>(n_groups_s) * H * per;
+    kv_tile_merge_kernel<<<cdiv(total, 256), 256, 0, stream>>>(w.kv_part, splits, H * per, w.kv, total);
+    LB_LAUNCHED();
+  }
+  {
+    using Epi = EpiAttn<256, 32>;
+    Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, static_cast<long>(x_group_rows) * ldc};
+    Planes B{lw.wqkv_hi, lw.wqkv_lo, C, 0};
+    typename Epi::Params ep{mask ? mask + x_base : nullptr, lw.s_qkv, w.kv, 1e-6f, w.att_hi + x_base * C,
+                            w.att_lo + x_base * C, C};
+    LB_TRY((launch_gemm<256, Epi>(TAG_QATTN, A, B, n_groups_x, x_group_rows, C, C, 0, ep, stream)));
+  }
+  return 0;
+}
+
 // Runs one encoder-layer call `x <- layer(x, source)` for the row range x (queries) / s (source).
 // self_pass: x range == source range (q, k, v in one projection launch).
 template <int BN>
@@ -717,107 +736,35 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   const __half* cat_lo = static_cast<const __half*>(st.cat_lo);
   const uint8_t* mask = st.mask;
   const int n_groups_s = static_cast<int>(s_rows / s_group_rows);
-  const int per = D * D + D;
   if (n_groups_x != n_groups_s && !self_pass) return fail("query / source group counts differ");
-  const bool fused = !full && (D == 32) && use_fused_attn() && lw.wkv_hi != nullptr;
   // Device-bounded window transformer (`live` != nullptr): every set of live_cap windows is one GEMM batch of
   // live_cap * group_rows rows whose live prefix is read on the device, so a self pass over both sets is a two-batch
-  // GEMM.  Without a bound every row range is one batch (xb = sb = 1), as it always was.
+  // GEMM.  Without a bound every row range is one batch (xb = sb = 1).
   const int xb = live ? static_cast<int>(x_rows / (static_cast<long>(live_cap) * x_group_rows)) : 1;
   const int sb = live ? static_cast<int>(s_rows / (static_cast<long>(live_cap) * s_group_rows)) : 1;
   const int xM = static_cast<int>(x_rows / xb), sM = static_cast<int>(s_rows / sb);
   const long xbs = xb > 1 ? static_cast<long>(xM) * ldc : 0, sbs = sb > 1 ? static_cast<long>(sM) * ldc : 0;
   const long xbs_a = xb > 1 ? static_cast<long>(xM) * C : 0;       // attention planes [R, C]
-  if (live && (fused || D != 16 || x_group_rows != s_group_rows))
+  if (live && (D != 16 || x_group_rows != s_group_rows))
     return fail("device-bounded group counts are built for the fine (window) transformer only");
-  // full attention: the coarse layers run tf_full_attention_coarse; the fine (window) layers share the projections of
-  // the window path below (no elu+1 feature map, no row zeroing) and run window_full_attn_kernel
-  const bool full_coarse = full && D == 32;
-  if (full_coarse) {
-    if (live) return fail("device-bounded group counts are built for the fine (window) transformer only");
+
+  // 1-3. attention message -> att planes [x rows, C]
+  if (D == 32 && !full) {
+    LB_TRY(tf_linear_attention_coarse(lw, C, H, st, w, x_base, x_group_rows, s_base, s_group_rows, n_groups_x,
+                                      n_groups_s, stream));
+  } else if (D == 32) {
     LB_TRY(tf_full_attention_coarse<BN>(lw, C, H, st, w, x_base, x_rows, x_group_rows, s_base, s_rows, s_group_rows,
                                         n_groups_x, self_pass, stream));
-  }
-
-  if constexpr (BN == 256) {
-    if (fused) {
-      // 1-3 fused (SURVEY.md §2a G1/G2): k|v projection with the K^T V reduction in its epilogue, then the q projection
-      // with the attention product in its epilogue; q, k, v never reach HBM.   [transformer.py:47-50, linear_attention.py:31-46]
-      const int m_tiles_s = cdiv(s_group_rows, kBlockM);
-      // K^T V on the tensor cores (kv_gemm.cuh; LOFTR_B200_KV_GEMM=0: the CUDA-core reduction inside EpiKv)
-      static int kv_gemm = -1;
-      if (kv_gemm < 0) {
-        const char* e = getenv("LOFTR_B200_KV_GEMM");
-        kv_gemm = e ? (atoi(e) != 0 ? 1 : 0) : 1;
-      }
-      if (kv_gemm && use_tma_store() && C == 256 && H == 8) {
-        int sms = 0;
-        LB_TRY(device_check(&sms));
-        __half* kvp_hi = w.h_hi + s_base * ldc;   // the MLP hidden planes [R, 2C] are free at this point of the layer
-        __half* kvp_lo = w.h_lo + s_base * ldc;
-        {
-          using Epi = EpiKvProj<256>;
-          Planes A{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, static_cast<long>(s_group_rows) * ldc};
-          Planes B{lw.wkv_hi, lw.wkv_lo, C, 0};
-          typename Epi::Params ep;
-          ep.rowmask = mask ? mask + s_base : nullptr;
-          ep.acc_scale = lw.s_qkv;
-          LB_TRY(fill_out_maps(&ep.om, kvp_hi, kvp_lo, ldc, nullptr, 0, 2 * C, s_group_rows, n_groups_s));
-          LB_TRY((launch_gemm<256, Epi>(TAG_KV, A, B, n_groups_s, s_group_rows, 2 * C, C, 0, ep, stream)));
-        }
-        {
-          CUtensorMap tm_hi, tm_lo;
-          LB_TRY(make_map(&tm_hi, kvp_hi, 2 * C, s_group_rows, n_groups_s, ldc, static_cast<long>(s_group_rows) * ldc, 64, 64));
-          LB_TRY(make_map(&tm_lo, kvp_lo, 2 * C, s_group_rows, n_groups_s, ldc, static_cast<long>(s_group_rows) * ldc, 64, 64));
-          const int kb_total = cdiv(s_group_rows, 64);
-          const int parts_cap = m_tiles_s > kKvSplits ? m_tiles_s : kKvSplits;   // capacity of kv_part in 1056-float partials per (group, head)
-          int splits = sms / (2 * n_groups_s);
-          if (splits < 1) splits = 1;
-          if (splits > kb_total) splits = kb_total;
-          if (splits > parts_cap) splits = parts_cap;
-          const int kb_per = cdiv(kb_total, splits);
-          splits = cdiv(kb_total, kb_per);
-          static bool configured[kMaxDevices] = {false};
-          int dev = 0;
-          LB_CUDA(cudaGetDevice(&dev));
-          if (!configured[dev]) {
-            LB_CUDA(cudaFuncSetAttribute(kv_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kKvGemmSmem));
-            configured[dev] = true;
-          }
-          KvGemmParams kp{w.kv_part, kb_total, kb_per, splits};
-          kv_gemm_kernel<<<dim3(splits, 2, n_groups_s), kKvGemmThreads, kKvGemmSmem, stream>>>(tm_hi, tm_lo, kp);
-          LB_LAUNCHED();
-          const long total = static_cast<long>(n_groups_s) * H * per;
-          kv_tile_merge_kernel<<<cdiv(total, 256), 256, 0, stream>>>(w.kv_part, splits, H * per, w.kv, total);
-          LB_LAUNCHED();
-        }
-      } else {
-        using Epi = EpiKv<256, 32>;
-        Planes A{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, static_cast<long>(s_group_rows) * ldc};
-        Planes B{lw.wkv_hi, lw.wkv_lo, C, 0};
-        typename Epi::Params ep{mask ? mask + s_base : nullptr, lw.s_qkv, w.kv_part, H};
-        LB_TRY((launch_gemm<256, Epi>(TAG_KV, A, B, n_groups_s, s_group_rows, 2 * C, C, 0, ep, stream)));
-        const long total = static_cast<long>(n_groups_s) * H * per;
-        kv_tile_merge_kernel<<<cdiv(total, 256), 256, 0, stream>>>(w.kv_part, m_tiles_s, H * per, w.kv, total);
-        LB_LAUNCHED();
-      }
-      {
-        using Epi = EpiAttn<256, 32>;
-        Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, static_cast<long>(x_group_rows) * ldc};
-        Planes B{lw.wqkv_hi, lw.wqkv_lo, C, 0};
-        typename Epi::Params ep{mask ? mask + x_base : nullptr, lw.s_qkv, w.kv, 1e-6f, w.att_hi + x_base * C,
-                                w.att_lo + x_base * C, C};
-        LB_TRY((launch_gemm<256, Epi>(TAG_QATTN, A, B, n_groups_x, x_group_rows, C, C, 0, ep, stream)));
-      }
-    }
-  }
-  if (!fused && !full_coarse) {
-  if (!w.qkv) return fail("first-generation attention path needs LOFTR_B200_FUSED_ATTN=0 (no q/k/v workspace was carved)");
-  // 1. projections (+ elu+1 feature map + padding mask)      [transformer.py:47-49, linear_attention.py:31-39]
-  //    full attention: plain projections; the window kernel applies the mask
-  const int elu_self = full ? 0 : 2 * C, elu_q = full ? 0 : C, elu_kv = full ? 0 : C;
-  const uint8_t* pmask = full ? nullptr : mask;
-  {
+  } else {
+    // windows of the fine transformer (D = 16, H = 8): the window kernels give every query / source row one lane
+    if (x_group_rows > 32 || s_group_rows > 32)
+      return fail("window transformer supports at most 32 rows per window (got %d query and %d source rows)",
+                  x_group_rows, s_group_rows);
+    if (full && x_group_rows != s_group_rows) return fail("full window attention is built for equal window sizes");
+    // q|k|v projection (linear: + elu+1 feature map + padding mask; full: plain, the window kernel applies the mask)
+    //                                                                 [transformer.py:47-49, linear_attention.py:31-39]
+    const int elu_self = full ? 0 : 2 * C, elu_q = full ? 0 : C, elu_kv = full ? 0 : C;
+    const uint8_t* pmask = full ? nullptr : mask;
     using Epi = EpiActStore<BN>;
     if (self_pass) {
       Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, xbs};
@@ -840,77 +787,38 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
       typename Epi::Params ek{w.qkv + s_base * 3 * C + C, 3 * C, elu_kv, pmask ? pmask + s_base : nullptr, lw.s_qkv, 0, omk};
       LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Ak, Bk, sb, sM, 2 * C, C, 0, ek, stream, live, s_group_rows)));
     }
-  }
-  // 2+3 for the fine windows: one kernel per pass, KV stays in shared memory (LOFTR_B200_WINDOW_ATTN=0: two kernels)
-  static int window_fused = -1;
-  if (window_fused < 0) {
-    const char* e = getenv("LOFTR_B200_WINDOW_ATTN");
-    window_fused = e ? (atoi(e) != 0 ? 1 : 0) : 1;
-  }
-  const bool one_kernel = D == 16 && H == 8 && window_fused && s_group_rows <= 32 && x_group_rows == s_group_rows &&
-                          n_groups_x == n_groups_s;
-  if (full) {
-    // 2+3 full (softmax) attention of the windows, exact fp32                [linear_attention.py:56-81]
-    if (!(D == 16 && H == 8 && s_group_rows <= 32 && x_group_rows == s_group_rows && n_groups_x == n_groups_s))
-      return fail("full window attention is built for 128/8 with equal groups of at most 32 rows");
     int sms = 0;
     LB_TRY(device_check(&sms));
-    const int grid = n_groups_x < 4 * sms ? n_groups_x : 4 * sms;
-    window_full_attn_kernel<16, 8, 32><<<grid, 256, 0, stream>>>(w.qkv, 3 * C, 0, C, 2 * C, x_base, s_base,
-                                                                 x_group_rows, n_groups_x, mask, w.att_hi, w.att_lo,
-                                                                 C, live, live_cap);
-    LB_LAUNCHED();
-  } else if (one_kernel) {
-    int sms = 0;
-    LB_TRY(device_check(&sms));
-    const int grid = n_groups_x < 3 * sms ? n_groups_x : 3 * sms;   // 3 resident blocks per SM (60 KB, <= 85 registers)
-    const int wa_smem = (H * (D * D + D) + 4 * x_group_rows * C) * static_cast<int>(sizeof(float));
-    static bool wa_configured[kMaxDevices] = {false};
-    int dev = 0;
-    LB_CUDA(cudaGetDevice(&dev));
-    if (!wa_configured[dev]) {
-      LB_CUDA(cudaFuncSetAttribute(window_attn_kernel<16, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (8 * (16 * 16 + 16) + 4 * 32 * 128) * static_cast<int>(sizeof(float))));
-      wa_configured[dev] = true;
-    }
-    window_attn_kernel<16, 8><<<grid, 256, wa_smem, stream>>>(w.qkv, 3 * C, 0, C, 2 * C, x_base, s_base, x_group_rows,
-                                                              n_groups_x, 1e-6f, w.att_hi, w.att_lo, C, live, live_cap);
-    LB_LAUNCHED();
-  } else {
-  if (live) return fail("the device-bounded window transformer needs the one-kernel window attention "
-                        "(LOFTR_B200_WINDOW_ATTN=0 selects a path without a device bound)");
-  // 2. KV = K^T V and Ksum per (source group, head)            [linear_attention.py:43-44]
-  if (D == 32) {
-    const int rps = cdiv(cdiv(s_group_rows, kKvSplits), 32) * 32;
-    const int splits = cdiv(s_group_rows, rps);
-    if (use_v2(0)) {
-      kv_partial_v2_kernel<32, 8><<<dim3(n_groups_s, splits), 256, 0, stream>>>(w.qkv, 3 * C, C, s_base, s_group_rows,
-                                                                                 rps, w.kv_part);
+    if (full) {
+      // full (softmax) attention of the windows, exact fp32                      [linear_attention.py:56-81]
+      const int grid = n_groups_x < 4 * sms ? n_groups_x : 4 * sms;
+      window_full_attn_kernel<16, 8, 32><<<grid, 256, 0, stream>>>(w.qkv, 3 * C, 0, C, 2 * C, x_base, s_base,
+                                                                   x_group_rows, n_groups_x, mask, w.att_hi, w.att_lo,
+                                                                   C, live, live_cap);
+    } else if (x_group_rows == s_group_rows) {
+      // linear attention, one kernel per pass: KV stays in shared memory      [linear_attention.py:43-46]
+      const int grid = n_groups_x < 3 * sms ? n_groups_x : 3 * sms;   // 3 resident blocks per SM (60 KB, <= 85 registers)
+      const int wa_smem = (H * (D * D + D) + 4 * x_group_rows * C) * static_cast<int>(sizeof(float));
+      static bool wa_configured[kMaxDevices] = {false};
+      int dev = 0;
+      LB_CUDA(cudaGetDevice(&dev));
+      if (!wa_configured[dev]) {
+        LB_CUDA(cudaFuncSetAttribute(window_attn_kernel<16, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (8 * (16 * 16 + 16) + 4 * 32 * 128) * static_cast<int>(sizeof(float))));
+        wa_configured[dev] = true;
+      }
+      window_attn_kernel<16, 8><<<grid, 256, wa_smem, stream>>>(w.qkv, 3 * C, 0, C, 2 * C, x_base, s_base, x_group_rows,
+                                                                n_groups_x, 1e-6f, w.att_hi, w.att_lo, C, live, live_cap);
     } else {
-      kv_partial_kernel<32><<<dim3(n_groups_s, H, splits), 256, 0, stream>>>(w.qkv, 3 * C, C, 2 * C, s_base,
-                                                                               s_group_rows, rps, w.kv_part);
+      // linear attention between windows of different sizes (a cross pass of the standalone fine transformer): KV and
+      // Ksum per source window through HBM, then one 32-row block per query window   [linear_attention.py:43-46]
+      kv_window_kernel<16, 8><<<n_groups_s, 256, 0, stream>>>(w.qkv, 3 * C, C, 2 * C, s_base, s_group_rows, w.kv);
+      LB_LAUNCHED();
+      attn_apply_kernel<16, 8><<<dim3(n_groups_x, 1), 256, 0, stream>>>(w.qkv, 3 * C, 0, x_base, x_group_rows, 32,
+                                                                        w.kv, 1e-6f, w.att_hi, w.att_lo, C);
     }
     LB_LAUNCHED();
-    const long total = static_cast<long>(n_groups_s) * H * per;
-    kv_merge_kernel<<<cdiv(total, 256), 256, 0, stream>>>(w.kv_part, splits, per, w.kv, total);
-    LB_LAUNCHED();
-  } else {
-    if (s_group_rows > 32) return fail("window transformer supports at most 32 rows per window");
-    kv_window_kernel<16, 8><<<n_groups_s, 256, 0, stream>>>(w.qkv, 3 * C, C, 2 * C, s_base, s_group_rows, w.kv);
-    LB_LAUNCHED();
   }
-  // 3. message = (Q KV) / (Q Ksum + eps) -> planes             [linear_attention.py:45-46]
-  if (D == 32) {
-    const int rpb = 128;
-    attn_apply_kernel<32, 8><<<dim3(n_groups_x, cdiv(x_group_rows, rpb)), 256, 0, stream>>>(
-        w.qkv, 3 * C, 0, x_base, x_group_rows, rpb, w.kv, 1e-6f, w.att_hi, w.att_lo, C);
-  } else {
-    attn_apply_kernel<16, 8><<<dim3(n_groups_x, 1), 256, 0, stream>>>(w.qkv, 3 * C, 0, x_base, x_group_rows, 32,
-                                                                      w.kv, 1e-6f, w.att_hi, w.att_lo, C);
-  }
-  LB_LAUNCHED();
-  }  // !one_kernel
-  }  // !fused && !full_coarse
   // 4. merge + norm1 -> cat[:, C:2C]                            [transformer.py:51-52]
   {
     using Epi = EpiLayerNorm<BN>;
@@ -957,7 +865,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
 
 extern "C" {
 
-int lb_version(void) { return 102; }
+int lb_version(void) { return 103; }
 int lb_block_k(void) { return kBlockK; }
 int lb_conv_layout(int cin, int* cin_blocks, int* rem_channels) {
   if (!cin_blocks || !rem_channels || cin <= 0) return fail("lb_conv_layout: bad arguments");
@@ -995,129 +903,6 @@ int lb_timing_collect(double* total_ms, long long* counts, int n) {
     }
   }
   return 0;
-}
-
-// Device self-test of the second-generation CUDA-core kernels: runs both versions on identical pseudo-random
-// inputs at production shapes, compares the outputs bit for bit and times them.  Allocates its own buffers.
-static __global__ void selftest_fill_kernel(float* p, long n, unsigned seed, float lo, float hi) {
-  for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<long>(gridDim.x) * blockDim.x) {
-    unsigned x = static_cast<unsigned>(i) * 747796405u + seed * 2891336453u + 1u;
-    x = ((x >> ((x >> 28) + 4u)) ^ x) * 277803737u;
-    x = (x >> 22) ^ x;
-    p[i] = lo + (hi - lo) * (static_cast<float>(x >> 8) * (1.0f / 16777216.0f));
-  }
-}
-static __global__ void selftest_diff_kernel(const unsigned* a, const unsigned* b, long n, unsigned long long* ndiff) {
-  unsigned long long c = 0;
-  for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<long>(gridDim.x) * blockDim.x)
-    c += a[i] != b[i];
-  if (c) atomicAdd(ndiff, c);
-}
-
-int lb_selftest(char* report, int report_len) {
-  int sms;
-  LB_TRY(device_check(&sms));
-  auto say = [&](const char* fmt, ...) {
-    const int used = static_cast<int>(strlen(report));
-    if (used >= report_len - 1) return;
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(report + used, report_len - used, fmt, ap);
-    va_end(ap);
-  };
-  if (report_len > 0) report[0] = 0;
-  cudaEvent_t e0, e1;
-  LB_CUDA(cudaEventCreate(&e0));
-  LB_CUDA(cudaEventCreate(&e1));
-  unsigned long long* d_ndiff;
-  LB_CUDA(cudaMalloc(&d_ndiff, 8));
-  auto diff = [&](const void* a, const void* b, long words, unsigned long long* out) -> int {
-    LB_CUDA(cudaMemset(d_ndiff, 0, 8));
-    selftest_diff_kernel<<<1024, 256>>>(static_cast<const unsigned*>(a), static_cast<const unsigned*>(b), words, d_ndiff);
-    LB_CUDA(cudaMemcpy(out, d_ndiff, 8, cudaMemcpyDeviceToHost));
-    return 0;
-  };
-  int failures = 0;
-  {  // ---- kv_partial: 16 images x 4800 tokens, C = 256 (batch 8 at 640x480)
-    const int C = 256, H = 8, D = 32, groups = 16, rows_per_group = 4800;
-    const long R = static_cast<long>(groups) * rows_per_group;
-    const int rps = cdiv(cdiv(rows_per_group, kKvSplits), 32) * 32;
-    const int splits = cdiv(rows_per_group, rps);
-    const long part_elems = static_cast<long>(groups) * H * splits * (D * D + D);
-    float *qkv, *p1, *p2;
-    LB_CUDA(cudaMalloc(&qkv, R * 3 * C * 4));
-    LB_CUDA(cudaMalloc(&p1, part_elems * 4));
-    LB_CUDA(cudaMalloc(&p2, part_elems * 4));
-    selftest_fill_kernel<<<2048, 256>>>(qkv, R * 3 * C, 1u, -1.f, 2.f);
-    LB_CUDA(cudaMemset(p1, 0xFF, part_elems * 4));
-    LB_CUDA(cudaMemset(p2, 0x7F, part_elems * 4));
-    float ms1 = 0, ms2 = 0;
-    for (int v = 0; v < 2; ++v) {
-      for (int it = 0; it < 12; ++it) {
-        if (it == 2) LB_CUDA(cudaEventRecord(e0));
-        if (v == 0)
-          kv_partial_kernel<32><<<dim3(groups, H, splits), 256>>>(qkv, 3 * C, C, 2 * C, 0, rows_per_group, rps, p1);
-        else
-          kv_partial_v2_kernel<32, 8><<<dim3(groups, splits), 256>>>(qkv, 3 * C, C, 0, rows_per_group, rps, p2);
-      }
-      LB_CUDA(cudaEventRecord(e1));
-      LB_CUDA(cudaEventSynchronize(e1));
-      LB_CUDA(cudaEventElapsedTime(v == 0 ? &ms1 : &ms2, e0, e1));
-    }
-    LB_CUDA(cudaGetLastError());
-    unsigned long long nd = 0;
-    LB_TRY(diff(p1, p2, part_elems, &nd));
-    say("kv_partial: v1 %.1f us, v2 %.1f us, differing words %llu of %ld -> %s\n", ms1 * 100.f, ms2 * 100.f, nd,
-        part_elems, nd == 0 ? "IDENTICAL" : "DIFFERENT");
-    failures += nd != 0;
-    cudaFree(qkv); cudaFree(p1); cudaFree(p2);
-  }
-  {  // ---- stem: 16 images 480 x 640
-    const int N = 16, Hh = 480, Ww = 640, CO = 128;
-    const long pix = static_cast<long>(N) * (Hh / 2) * (Ww / 2);
-    float *img, *wt, *sc, *sh;
-    __half *h1, *l1, *h2, *l2;
-    LB_CUDA(cudaMalloc(&img, static_cast<long>(N) * Hh * Ww * 4));
-    LB_CUDA(cudaMalloc(&wt, 49 * CO * 4));
-    LB_CUDA(cudaMalloc(&sc, CO * 4));
-    LB_CUDA(cudaMalloc(&sh, CO * 4));
-    LB_CUDA(cudaMalloc(&h1, pix * CO * 2)); LB_CUDA(cudaMalloc(&l1, pix * CO * 2));
-    LB_CUDA(cudaMalloc(&h2, pix * CO * 2)); LB_CUDA(cudaMalloc(&l2, pix * CO * 2));
-    selftest_fill_kernel<<<2048, 256>>>(img, static_cast<long>(N) * Hh * Ww, 2u, 0.f, 1.f);
-    selftest_fill_kernel<<<32, 256>>>(wt, 49 * CO, 3u, -0.3f, 0.3f);
-    selftest_fill_kernel<<<1, 128>>>(sc, CO, 4u, 0.5f, 1.5f);
-    selftest_fill_kernel<<<1, 128>>>(sh, CO, 5u, -0.2f, 0.2f);
-    LB_CUDA(cudaMemset(h1, 0xFF, pix * CO * 2)); LB_CUDA(cudaMemset(h2, 0x7F, pix * CO * 2));
-    LB_CUDA(cudaMemset(l1, 0xFF, pix * CO * 2)); LB_CUDA(cudaMemset(l2, 0x7F, pix * CO * 2));
-    float ms1 = 0, ms2 = 0;
-    for (int v = 0; v < 2; ++v) {
-      for (int it = 0; it < 7; ++it) {
-        if (it == 2) LB_CUDA(cudaEventRecord(e0));
-        if (v == 0)
-          conv_stem7x7_kernel<128><<<dim3(cdiv(Ww / 2, 128), Hh / 2, N), 128>>>(img, Hh, Ww, wt, sc, sh, h1, l1, CO);
-        else
-          conv_stem7x7_v2_kernel<128><<<dim3(cdiv(Ww / 2, 256), Hh / 2, N), 128>>>(img, Hh, Ww, wt, sc, sh, h2, l2, CO);
-      }
-      LB_CUDA(cudaEventRecord(e1));
-      LB_CUDA(cudaEventSynchronize(e1));
-      LB_CUDA(cudaEventElapsedTime(v == 0 ? &ms1 : &ms2, e0, e1));
-    }
-    LB_CUDA(cudaGetLastError());
-    unsigned long long nd_h = 0, nd_l = 0;
-    LB_TRY(diff(h1, h2, pix * CO / 2, &nd_h));
-    LB_TRY(diff(l1, l2, pix * CO / 2, &nd_l));
-    say("stem7x7: v1 %.1f us, v2 %.1f us, differing words hi %llu lo %llu of %ld -> %s\n", ms1 * 200.f, ms2 * 200.f,
-        nd_h, nd_l, pix * CO / 2, (nd_h | nd_l) == 0 ? "IDENTICAL" : "DIFFERENT");
-    failures += (nd_h | nd_l) != 0;
-    cudaFree(img); cudaFree(wt); cudaFree(sc); cudaFree(sh);
-    cudaFree(h1); cudaFree(l1); cudaFree(h2); cudaFree(l2);
-  }
-  cudaFree(d_ndiff);
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  return failures ? fail("lb_selftest: %d kernel pair(s) differ", failures) : 0;
 }
 
 int lb_split_planes(const float* x, long rows, int cols, int ld_x, void* hi, void* lo, int ld_pl, int col0,
@@ -1265,14 +1050,8 @@ int lb_backbone_forward(const LbBackboneWeights* w, const float* images, int N, 
   if (!b.ok) return fail("backbone workspace too small: need %zu bytes", lb_backbone_workspace_bytes(w, N, H, W));
   const int H2 = H / 2, W2 = W / 2, H4 = H / 4, W4 = W / 4, H8 = H / 8, W8 = W / 8;
 
-  // stem: conv 7x7 s2 + BN + ReLU                                                  [resnet_fpn.py:101]
-  // default: tensor-core kernel with software im2col (stem_tc.cuh); LOFTR_B200_STEM_TC=0 keeps the CUDA-core kernels
-  static int stem_tc = -1;
-  if (stem_tc < 0) {
-    const char* e = getenv("LOFTR_B200_STEM_TC");
-    stem_tc = e ? (atoi(e) != 0 ? 1 : 0) : 1;
-  }
-  if (stem_tc) {
+  // stem: conv 7x7 s2 + BN + ReLU on the tensor cores, software im2col (stem_tc.cuh)  [resnet_fpn.py:101]
+  {
     StemTcParams sp;
     memset(&sp, 0, sizeof(sp));
     sp.img = images; sp.N = N; sp.H = H; sp.W = W;
@@ -1292,14 +1071,8 @@ int lb_backbone_forward(const LbBackboneWeights* w, const float* images, int N, 
     const long tiles = static_cast<long>(sp.tiles_w) * sp.tiles_h * N;
     const int grid = static_cast<int>(tiles < sms ? tiles : sms);
     conv_stem7x7_tc_kernel<<<grid, kStemThreads, kStemSmemBytes, st>>>(sp);
-  } else if (use_v2(1)) {
-    conv_stem7x7_v2_kernel<128><<<dim3(cdiv(W2, 256), H2, N), 128, 0, st>>>(images, H, W, w->stem_wt, w->stem_scale,
-                                                                            w->stem_shift, B.s0.hi, B.s0.lo, B.s0.ld);
-  } else {
-    conv_stem7x7_kernel<128><<<dim3(cdiv(W2, 128), H2, N), 128, 0, st>>>(images, H, W, w->stem_wt, w->stem_scale,
-                                                                          w->stem_shift, B.s0.hi, B.s0.lo, B.s0.ld);
+    LB_LAUNCHED();
   }
-  LB_LAUNCHED();
   auto conv = [&](const LbConvWeights& cw, const BbBuf& in, int hin, int win, int act, const BbBuf* res,
                   const BbBuf* up, int uph, int upw, const BbBuf* out, float* of32, int f32ld) -> int {
     ConvRun r{&cw, in, hin, win, act, res, up, uph, upw, out, of32, f32ld};
@@ -1323,39 +1096,12 @@ int lb_backbone_forward(const LbBackboneWeights* w, const float* images, int N, 
   LB_TRY(conv(w->l3[2], B.a3, H8, W8, 1, nullptr, nullptr, 0, 0, &B.t3, nullptr, 0));
   LB_TRY(conv(w->l3[3], B.t3, H8, W8, 1, &B.a3, nullptr, 0, 0, &B.x3, nullptr, 0));
   // FPN                                                                             [resnet_fpn.py:107-116]
-  // The x2 bilinear upsampling of the coarser level is gathered inside the lateral 1x1 convolution's epilogue (default).
-  // LOFTR_B200_FUSED_UPSAMPLE=0 runs it as a separate bandwidth kernel into a buffer that is dead at that point
-  // (m2 / m1 are only written two launches later) and adds it through the residual path.
-  static int fused_up = -1;
-  if (fused_up < 0) {
-    const char* e = getenv("LOFTR_B200_FUSED_UPSAMPLE");
-    fused_up = e ? (atoi(e) != 0 ? 1 : 0) : 1;
-  }
-  auto upsample = [&](const BbBuf& src, int sh, int sw, int C, const BbBuf& dst, int dh, int dw) -> int {
-    if (src.ld != dst.ld) return fail("upsample buffers must share the channel stride");
-    const int groups = src.ld / 8;
-    const long total = static_cast<long>(N) * dh * dw * groups;
-    (void)C;
-    upsample2x_planes_kernel<<<cdiv(total, 256), 256, 0, st>>>(src.hi, src.lo, src.ld, sh, sw, dst.hi, dst.lo, dst.ld, dh, dw,
-                                                              groups, total);
-    LB_LAUNCHED();
-    return 0;
-  };
+  // The x2 bilinear upsampling of the coarser level is gathered inside the lateral 1x1 convolution's epilogue.
   LB_TRY(conv(w->l3_out, B.x3, H8, W8, 0, nullptr, nullptr, 0, 0, &B.x3o, feat_c_nhwc, d3));
-  if (fused_up) {
-    LB_TRY(conv(w->l2_out, B.x2, H4, W4, 0, nullptr, &B.x3o, H8, W8, &B.x2l, nullptr, 0));
-  } else {
-    LB_TRY(upsample(B.x3o, H8, W8, d3, B.m2, H4, W4));
-    LB_TRY(conv(w->l2_out, B.x2, H4, W4, 0, &B.m2, nullptr, 0, 0, &B.x2l, nullptr, 0));
-  }
+  LB_TRY(conv(w->l2_out, B.x2, H4, W4, 0, nullptr, &B.x3o, H8, W8, &B.x2l, nullptr, 0));
   LB_TRY(conv(w->l2_out2[0], B.x2l, H4, W4, 2, nullptr, nullptr, 0, 0, &B.m2, nullptr, 0));
   LB_TRY(conv(w->l2_out2[1], B.m2, H4, W4, 0, nullptr, nullptr, 0, 0, &B.x2o, nullptr, 0));
-  if (fused_up) {
-    LB_TRY(conv(w->l1_out, B.x1, H2, W2, 0, nullptr, &B.x2o, H4, W4, &B.x1l, nullptr, 0));
-  } else {
-    LB_TRY(upsample(B.x2o, H4, W4, d2, B.m1, H2, W2));
-    LB_TRY(conv(w->l1_out, B.x1, H2, W2, 0, &B.m1, nullptr, 0, 0, &B.x1l, nullptr, 0));
-  }
+  LB_TRY(conv(w->l1_out, B.x1, H2, W2, 0, nullptr, &B.x2o, H4, W4, &B.x1l, nullptr, 0));
   LB_TRY(conv(w->l1_out2[0], B.x1l, H2, W2, 2, nullptr, nullptr, 0, 0, &B.m1, nullptr, 0));
   LB_TRY(conv(w->l1_out2[1], B.m1, H2, W2, 0, nullptr, nullptr, 0, 0, nullptr, feat_f_nhwc, w->l1_out2[1].cout));
   return 0;

@@ -47,22 +47,6 @@ __device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi, uint
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
-// Write 32 consecutive values of one row as fp16 hi/lo planes (64 bytes each, 16B-aligned).
-__device__ __forceinline__ void store_planes32(__half* hi_ptr, __half* lo_ptr, const float (&x)[32]) {
-  uint32_t h[16], l[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    split_f16x2(x[2 * j], x[2 * j + 1], h[j], l[j]);
-  }
-  uint4* hp = reinterpret_cast<uint4*>(hi_ptr);
-  uint4* lp = reinterpret_cast<uint4*>(lo_ptr);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    hp[j] = make_uint4(h[4 * j], h[4 * j + 1], h[4 * j + 2], h[4 * j + 3]);
-    lp[j] = make_uint4(l[4 * j], l[4 * j + 1], l[4 * j + 2], l[4 * j + 3]);
-  }
-}
-
 __device__ __forceinline__ void store_f32x32(float* p, const float (&x)[32]) {
   float4* q = reinterpret_cast<float4*>(p);
 #pragma unroll
@@ -105,9 +89,6 @@ __device__ __forceinline__ void load_planes32(const __half* hp, const __half* lp
 // a 2 KB per-warp shared-memory scratch (XOR-swizzled, bank-conflict free both ways) so that every global access
 // instruction covers 8 rows x 64 contiguous bytes.  Rows are addressed by a per-lane pointer (lane = row; nullptr =
 // row not stored / read as zero), so the same code serves row-major matrices and NHWC pixel rows.
-#ifndef LB_COALESCE
-#define LB_COALESCE 1
-#endif
 // Per-warp 4 KB staging tile at the START of the epilogue area (1024-byte aligned): a [32 rows x 128 B] fp32 block or
 // two [32 rows x 64 B] plane blocks (hi at +0, lo at +2048) for TMA stores; its first 2 KB double as the transposer
 // scratch of the coalesced load / store helpers below.
@@ -122,7 +103,6 @@ __device__ __forceinline__ T* shfl_ptr(T* p, int src_lane) {
 }
 // w[16]: 64 bytes of this lane's row -> *(row_ptr + 0..63) for every lane with row_ptr != nullptr
 __device__ __forceinline__ void warp_store_rows64(uint32_t* scr, uint8_t* row_ptr, const uint32_t (&w)[16]) {
-#if LB_COALESCE
   const int lane = threadIdx.x & 31;
   __syncwarp();
 #pragma unroll
@@ -138,18 +118,9 @@ __device__ __forceinline__ void warp_store_rows64(uint32_t* scr, uint8_t* row_pt
     const uint4 v = *reinterpret_cast<const uint4*>(scr + r * 16 + ((g ^ ((r >> 1) & 3)) << 2));
     if (dst) *reinterpret_cast<uint4*>(dst + g * 16) = v;
   }
-#else
-  (void)scr;
-  if (row_ptr) {
-    uint4* d = reinterpret_cast<uint4*>(row_ptr);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) d[q] = make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
-  }
-#endif
 }
 // inverse: 64 bytes at row_ptr (zeros for nullptr) -> w[16] of the owning lane
 __device__ __forceinline__ void warp_load_rows64(uint32_t* scr, const uint8_t* row_ptr, uint32_t (&w)[16]) {
-#if LB_COALESCE
   const int lane = threadIdx.x & 31;
   const int g = lane & 3;
   __syncwarp();
@@ -167,15 +138,6 @@ __device__ __forceinline__ void warp_load_rows64(uint32_t* scr, const uint8_t* r
     const uint4 v = *reinterpret_cast<const uint4*>(scr + lane * 16 + ((q ^ ((lane >> 1) & 3)) << 2));
     w[4 * q] = v.x; w[4 * q + 1] = v.y; w[4 * q + 2] = v.z; w[4 * q + 3] = v.w;
   }
-#else
-  (void)scr;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (row_ptr) v = reinterpret_cast<const uint4*>(row_ptr)[q];
-    w[4 * q] = v.x; w[4 * q + 1] = v.y; w[4 * q + 2] = v.z; w[4 * q + 3] = v.w;
-  }
-#endif
 }
 // 32 values of my row as fp16 hi/lo planes: hi_ptr / lo_ptr address (row, first column) or nullptr
 __device__ __forceinline__ void warp_store_planes32(uint32_t* scr, __half* hi_ptr, __half* lo_ptr, const float (&x)[32]) {
@@ -197,7 +159,7 @@ __device__ __forceinline__ void warp_store_f32x32(uint32_t* scr, float* ptr, con
   warp_store_rows64(scr, reinterpret_cast<uint8_t*>(ptr), a);
   warp_store_rows64(scr, ptr ? reinterpret_cast<uint8_t*>(ptr) + 64 : nullptr, b);
 }
-// Split form of warp_load_planes32 (coalesced build only): `issue` puts the lane's eight 16-byte global loads in flight
+// 32 values of my row from fp16 hi/lo planes, in two steps: `issue` puts the lane's eight 16-byte global loads in flight
 // (rows lane/4 + 8i, 16-byte group lane%4), `finish` transposes them through the scratch into this lane's row.  An
 // epilogue can issue before it waits for / converts its accumulator group and finish afterwards.
 __device__ __forceinline__ void warp_issue_planes32(const __half* hi_ptr, const __half* lo_ptr, uint4 (&vh)[4], uint4 (&vl)[4]) {
@@ -245,54 +207,6 @@ __device__ __forceinline__ void warp_finish_planes32(uint32_t* scr, const uint4 
     x[2 * j + 1] = fh.y + fl.y;
   }
 }
-__device__ __forceinline__ void warp_load_planes32(uint32_t* scr, const __half* hi_ptr, const __half* lo_ptr, float (&x)[32]) {
-  uint32_t h[16], l[16];
-#if LB_COALESCE
-  // all eight 16-byte global loads of the lane are issued before the first one is consumed (one exposed latency)
-  const int lane = threadIdx.x & 31;
-  const int g = lane & 3;
-  uint4 vh[4], vl[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = (lane >> 2) + 8 * i;
-    const uint8_t* sh = shfl_ptr(reinterpret_cast<const uint8_t*>(hi_ptr), r);
-    const uint8_t* sl = shfl_ptr(reinterpret_cast<const uint8_t*>(lo_ptr), r);
-    vh[i] = make_uint4(0u, 0u, 0u, 0u);
-    vl[i] = make_uint4(0u, 0u, 0u, 0u);
-    if (sh) vh[i] = *reinterpret_cast<const uint4*>(sh + g * 16);
-    if (sl) vl[i] = *reinterpret_cast<const uint4*>(sl + g * 16);
-  }
-#pragma unroll
-  for (int pass = 0; pass < 2; ++pass) {
-    __syncwarp();
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int r = (lane >> 2) + 8 * i;
-      *reinterpret_cast<uint4*>(scr + r * 16 + ((g ^ ((r >> 1) & 3)) << 2)) = pass == 0 ? vh[i] : vl[i];
-    }
-    __syncwarp();
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const uint4 v = *reinterpret_cast<const uint4*>(scr + lane * 16 + ((q ^ ((lane >> 1) & 3)) << 2));
-      if (pass == 0) {
-        h[4 * q] = v.x; h[4 * q + 1] = v.y; h[4 * q + 2] = v.z; h[4 * q + 3] = v.w;
-      } else {
-        l[4 * q] = v.x; l[4 * q + 1] = v.y; l[4 * q + 2] = v.z; l[4 * q + 3] = v.w;
-      }
-    }
-  }
-#else
-  warp_load_rows64(scr, reinterpret_cast<const uint8_t*>(hi_ptr), h);
-  warp_load_rows64(scr, reinterpret_cast<const uint8_t*>(lo_ptr), l);
-#endif
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&h[j]));
-    const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&l[j]));
-    x[2 * j] = fh.x + fl.x;
-    x[2 * j + 1] = fh.y + fl.y;
-  }
-}
 __device__ __forceinline__ void warp_load_f32x32(uint32_t* scr, const float* ptr, float (&x)[32]) {
   uint32_t a[16], b[16];
   warp_load_rows64(scr, reinterpret_cast<const uint8_t*>(ptr), a);
@@ -310,9 +224,11 @@ __device__ __forceinline__ void warp_load_f32x32(uint32_t* scr, const float* ptr
 // and ONE lane hands it to the copy engine (cp.async.bulk.tensor ... bulk_group): full-line writes, no per-lane
 // address generation, rows / channels beyond the tensor's extent are clipped by the map (no predicates).  The staging
 // tile is reused only after the engine has read the previous block (wait_group.read).
-struct OutMaps {            // filled on the host (engine.cu make_out_map_*); use == 0 -> the pointer paths are taken
+struct OutMaps {            // filled on the host (engine.cu make_out_map_*) for the outputs an epilogue writes
   CUtensorMap hi, lo, f32;
-  int use;                  // bit 0: planes through TMA, bit 1: fp32 output through TMA
+  int use;                  // bit 0: planes map set, bit 1: fp32 map set.  The host always sets the bits of the outputs
+                            // it passes; EpiLayerNorm and EpiConv keep pointer stores for a clear bit because without
+                            // that code ptxas allocates their registers worse (more spills in EpiConv<256, 0>)
   int dims;                 // 3: (col, row, batch) coordinates;  4: NHWC (channel, x, y, image) coordinates
 };
 struct OutCoord {           // where this warp's 32-row block goes
@@ -374,13 +290,13 @@ __device__ __forceinline__ void stage_quiesce() {
 template <int BLOCK_N>
 struct EpiActStore {
   struct Params {
-    float* out;              // [batches*M, ld]
+    float* out;              // [batches*M, ld] (written through om.f32)
     int ld;
     int elu_cols;            // columns [0, elu_cols) get elu+1
     const uint8_t* rowmask;  // optional [batches*M] (1 = valid)
     float acc_scale;         // 2^-e: undoes the power-of-two pre-scaling of the weight planes (exact)
     int skip;                // probe mode (LOFTR_B200_PROBE_NULL_EPI, lb_gemm_split only): 1 = drain nothing, 2 = accumulator loads only
-    OutMaps om;              // om.use & 2: fp32 output through TMA stores
+    OutMaps om;              // om.f32: the fp32 output
   };
   static constexpr int kSmemBytes = kEpiScratchBytes;
   const Params& p;
@@ -419,11 +335,7 @@ struct EpiActStore {
       }
 #pragma unroll
       for (int j = 0; j < 32; ++j) x[j] *= mk;
-      if (p.om.use & 2) {
-        warp_tma_store_f32x32(scr, p.om, OutCoord{col, m0 + ((epi_tid() >> 5) & 3) * 32, batch, 0}, x);
-        continue;
-      }
-      warp_store_f32x32(scr, row_ok ? p.out + grow * p.ld + col : nullptr, x);
+      warp_tma_store_f32x32(scr, p.om, OutCoord{col, m0 + ((epi_tid() >> 5) & 3) * 32, batch, 0}, x);
     }
   }
 };
@@ -431,124 +343,9 @@ struct EpiActStore {
 
 // ------------------------------------------------------------------------------------------------
 // Linear attention fused into the projections (SURVEY.md §2a G1/G2; reference linear_attention.py:31-46).
-// The fp32 q / k / v tensors of the reference never reach HBM.
+// The fp32 q / k / v tensors of the reference never reach HBM: the k|v projection writes K and V as planes (EpiKvProj,
+// below), kv_gemm_kernel reduces them to KV / Ksum, and the q projection applies them (EpiAttn).
 //
-// EpiKv: epilogue of the k|v projection.  The B operand is the row-permuted weight [Wk(heads 4t..4t+3) ; Wv(same
-// heads)] so that n-tile t holds, for kHeads = BLOCK_N / (2 D) heads, K in columns [0, BLOCK_N/2) and V in columns
-// [BLOCK_N/2, BLOCK_N).  K = elu(k)+1 and the padding mask are applied (linear_attention.py:32-39); per head the
-// 128-row tile contributes
-//     KV[d][v] += sum_r K[r][d] V[r][v],   Ksum[d] += sum_r K[r][d]                          (:43-44)
-// which is evaluated on the CUDA cores from a shared-memory staging of the head's K and V columns (thread = 2 d x 8 v
-// outputs over a quarter of the rows, then a 4-way merge) and written as ONE partial per (group, row tile, head):
-// part[batch][m_tile][head][D*D + D]; kv_tile_merge_kernel sums the row tiles in fixed order (bit-reproducible).
-template <int BLOCK_N, int D>
-struct EpiKv {
-  static_assert(D == 32 && BLOCK_N == 256, "built for the coarse transformer (d_model 256, 8 heads)");
-  struct Params {
-    const uint8_t* rowmask;  // optional [batches*M] (1 = valid)
-    float acc_scale;
-    float* part;             // [batches][m_tiles][H][D*D + D]
-    int H;
-  };
-  static constexpr int kHeads = BLOCK_N / (2 * D);      // heads per n-tile (4)
-  static constexpr int kPer = D * D + D;
-  static constexpr int kSmemBytes = 2 * 128 * D * 4;    // K and V staging (aliased by the 4-way merge buffer)
-  static_assert(4 * kPer * 4 <= kSmemBytes, "merge buffer must fit in the staging area");
-  const Params& p;
-  const GemmShape& s;
-  float* sK;   // [128][D], float4 index q of row r stored at q ^ (r & 7)
-  float* sV;
-  float* red;  // [4][kPer] aliasing sK/sV
-  __device__ EpiKv(const Params& p_, uint8_t* smem, const GemmShape& s_) : p(p_), s(s_) {
-    sK = reinterpret_cast<float*>(smem);
-    sV = sK + 128 * D;
-    red = sK;
-  }
-  __device__ void item_begin(int, int, int) {}
-  __device__ void item_end(int, int, int) {}
-  __device__ void prefetch(int, int, int) {}
-  __device__ void tile(uint32_t acc_row, int batch, int m0, int n0) {
-    const int t = epi_tid();
-    const int row = epi_row();
-    const int half = epi_half();
-    const int r = m0 + row;
-    const bool row_ok = r < s.M;
-    float mk = row_ok ? 1.f : 0.f;
-    if (row_ok && p.rowmask) mk = p.rowmask[static_cast<long>(batch) * s.M + r] ? 1.f : 0.f;
-    // compute-phase mapping: row quarter g, d pair, v octet
-    const int g = t >> 6, lt = t & 63, d2 = lt >> 2, v8 = lt & 3;
-    const int head0 = (n0 / BLOCK_N) * kHeads;
-#pragma unroll 1
-    for (int j = 0; j < kHeads; ++j) {
-      {  // stage this head's K (column half 0) / V (column half 1) columns of my row
-        float x[32];
-        load_acc32(acc_row, (half * kHeads + j) * 32, x);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) x[i] *= p.acc_scale;
-        if (half == 0) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) x[i] = elu_plus1(x[i]);
-        }
-        float* dst = (half == 0 ? sK : sV) + row * D;
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          *reinterpret_cast<float4*>(dst + ((q ^ (row & 7)) << 2)) =
-              make_float4(x[4 * q] * mk, x[4 * q + 1] * mk, x[4 * q + 2] * mk, x[4 * q + 3] * mk);
-      }
-      epi_bar_sync();
-      float acc0[8], acc1[8], ks0 = 0.f, ks1 = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        acc0[i] = 0.f;
-        acc1[i] = 0.f;
-      }
-#pragma unroll 4
-      for (int rr = g * 32; rr < g * 32 + 32; ++rr) {
-        const int sw = rr & 7;
-        const float2 k2 = *reinterpret_cast<const float2*>(sK + rr * D + (((d2 >> 1) ^ sw) << 2) + ((d2 & 1) << 1));
-        const float4 va = *reinterpret_cast<const float4*>(sV + rr * D + (((2 * v8) ^ sw) << 2));
-        const float4 vb = *reinterpret_cast<const float4*>(sV + rr * D + (((2 * v8 + 1) ^ sw) << 2));
-        acc0[0] = fmaf(k2.x, va.x, acc0[0]); acc0[1] = fmaf(k2.x, va.y, acc0[1]);
-        acc0[2] = fmaf(k2.x, va.z, acc0[2]); acc0[3] = fmaf(k2.x, va.w, acc0[3]);
-        acc0[4] = fmaf(k2.x, vb.x, acc0[4]); acc0[5] = fmaf(k2.x, vb.y, acc0[5]);
-        acc0[6] = fmaf(k2.x, vb.z, acc0[6]); acc0[7] = fmaf(k2.x, vb.w, acc0[7]);
-        acc1[0] = fmaf(k2.y, va.x, acc1[0]); acc1[1] = fmaf(k2.y, va.y, acc1[1]);
-        acc1[2] = fmaf(k2.y, va.z, acc1[2]); acc1[3] = fmaf(k2.y, va.w, acc1[3]);
-        acc1[4] = fmaf(k2.y, vb.x, acc1[4]); acc1[5] = fmaf(k2.y, vb.y, acc1[5]);
-        acc1[6] = fmaf(k2.y, vb.z, acc1[6]); acc1[7] = fmaf(k2.y, vb.w, acc1[7]);
-        ks0 += k2.x;
-        ks1 += k2.y;
-      }
-      epi_bar_sync();   // everyone is done reading the staging area: it becomes the merge buffer
-      {
-        float* rg = red + g * kPer;
-        const int da = 2 * d2, db = 2 * d2 + 1;
-        *reinterpret_cast<float4*>(rg + da * D + (((2 * v8) ^ (da & 7)) << 2)) = make_float4(acc0[0], acc0[1], acc0[2], acc0[3]);
-        *reinterpret_cast<float4*>(rg + da * D + (((2 * v8 + 1) ^ (da & 7)) << 2)) = make_float4(acc0[4], acc0[5], acc0[6], acc0[7]);
-        *reinterpret_cast<float4*>(rg + db * D + (((2 * v8) ^ (db & 7)) << 2)) = make_float4(acc1[0], acc1[1], acc1[2], acc1[3]);
-        *reinterpret_cast<float4*>(rg + db * D + (((2 * v8 + 1) ^ (db & 7)) << 2)) = make_float4(acc1[4], acc1[5], acc1[6], acc1[7]);
-        if (v8 == 0) {
-          rg[D * D + da] = ks0;
-          rg[D * D + db] = ks1;
-        }
-      }
-      epi_bar_sync();
-      {
-        float* out = p.part + ((static_cast<long>(batch) * s.m_tiles + m0 / kBlockM) * p.H + head0 + j) * kPer;
-        for (int e = t; e < kPer; e += kEpiThreads) {
-          int src = e;
-          if (e < D * D) {
-            const int d = e / D, v = e - d * D;
-            src = d * D + ((((v >> 2) ^ (d & 7)) << 2) | (v & 3));
-          }
-          out[e] = (red[src] + red[kPer + src]) + (red[2 * kPer + src] + red[3 * kPer + src]);
-        }
-      }
-      epi_bar_sync();   // the merge buffer is the next head's staging area
-    }
-  }
-};
-
 // EpiAttn: epilogue of the q projection.  Q = elu(q)+1 (masked), then for the head that owns each 32-column group
 //     out[r, h, :] = (Q[r,h,:] . KV[g,h]) / (Q[r,h,:] . Ksum[g,h] + eps)                    (linear_attention.py:44-46)
 // with KV / Ksum of the row's group (batch) staged in shared memory, written as fp16 planes = the A operand of the
@@ -737,14 +534,12 @@ struct EpiLayerNorm {
     const float rstd = rsqrtf(var + p.eps);
 #pragma unroll 1
     for (int c = c_begin; c < c_end; ++c) {
-#if LB_COALESCE
       // residual rows of this 32-column group: requested before the accumulator group is fetched and normalised
       // (18 % of the mlp[2]+norm2 kernel's samples waited on them when they were loaded after the arithmetic)
       uint4 rh[4], rl[4];
       if (p.res_hi)
         warp_issue_planes32(row_ok ? p.res_hi + grow * p.ld_res_pl + c * 32 : nullptr,
                             row_ok ? p.res_lo + grow * p.ld_res_pl + c * 32 : nullptr, rh, rl);
-#endif
       float x[32];
       load_acc32(acc_row, c * 32, x);
 #pragma unroll
@@ -766,12 +561,7 @@ struct EpiLayerNorm {
       }
       if (p.res_hi) {
         float r[32];
-#if LB_COALESCE
         warp_finish_planes32(scr, rh, rl, r);
-#else
-        warp_load_planes32(scr, row_ok ? p.res_hi + grow * p.ld_res_pl + c * 32 : nullptr,
-                           row_ok ? p.res_lo + grow * p.ld_res_pl + c * 32 : nullptr, r);
-#endif
 #pragma unroll
         for (int j = 0; j < 32; ++j) x[j] += r[j];
       }
@@ -851,18 +641,8 @@ struct EpiPlanes {
         }
       }
       const OutCoord oc{col, m0 + ((epi_tid() >> 5) & 3) * 32, batch, 0};
-      if (p.out_f32) {
-        if (p.om.use & 2) warp_tma_store_f32x32(scr, p.om, oc, x);
-        else warp_store_f32x32(scr, row_ok ? p.out_f32 + grow * p.ld_f32 + col : nullptr, x);
-      }
-      if (p.out_hi) {
-        if (p.om.use & 1) {
-          warp_tma_store_planes32(scr, p.om, oc, x);
-        } else {
-          const long off = grow * p.ld_pl + p.pl_col0 + col;
-          warp_store_planes32(scr, row_ok ? p.out_hi + off : nullptr, row_ok ? p.out_lo + off : nullptr, x);
-        }
-      }
+      if (p.out_f32) warp_tma_store_f32x32(scr, p.om, oc, x);
+      if (p.out_hi) warp_tma_store_planes32(scr, p.om, oc, x);
     }
   }
 };
@@ -1080,13 +860,11 @@ struct EpiConv {
       const int col = n0 + c * 32;
       if (col >= s.N) break;
       const int nvalid = min(32, s.N - col);   // warp-uniform
-#if LB_COALESCE
       // residual rows of this 32-channel group: requested before the accumulator is fetched and converted
       const bool res_early = p.res_hi != nullptr && nvalid == 32;
       uint4 rh[4], rl[4];
       if (res_early)
         warp_issue_planes32(ok ? p.res_hi + pix * p.res_ld + col : nullptr, ok ? p.res_lo + pix * p.res_ld + col : nullptr, rh, rl);
-#endif
       float v[32];
       load_acc32(acc_row, c * 32, v);
 #pragma unroll
@@ -1096,11 +874,7 @@ struct EpiConv {
         if (p.res_hi) {
           if (p.om.use && !kOwnXpose) stage_quiesce();
           float r[32];
-#if LB_COALESCE
           warp_finish_planes32(xscr, rh, rl, r);
-#else
-          warp_load_planes32(xscr, ok ? p.res_hi + pix * p.res_ld + col : nullptr, ok ? p.res_lo + pix * p.res_ld + col : nullptr, r);
-#endif
 #pragma unroll
           for (int j = 0; j < 32; ++j) v[j] += r[j];
         }

@@ -74,203 +74,30 @@ __global__ void coarse_prep_kernel(const float* __restrict__ feat, int nhwc, con
 }
 
 // ------------------------------------------------------------------------------------------------
-// Backbone stem: conv 7x7 stride 2, 1 -> Cout channels, + folded BatchNorm + ReLU
-// (reference resnet_fpn.py:58-60,101), written as NHWC fp16 planes.  One thread per output pixel keeps all
-// 128 output channels in registers; the 49 x Cout weights sit in shared memory (broadcast reads).
-template <int COUT>
-__global__ void __launch_bounds__(128) conv_stem7x7_kernel(const float* __restrict__ img, int H, int W,
-                                                           const float* __restrict__ wt /*[49][COUT]*/,
-                                                           const float* __restrict__ scale,
-                                                           const float* __restrict__ shift,
-                                                           __half* __restrict__ out_hi, __half* __restrict__ out_lo,
-                                                           int out_ld) {
-  __shared__ __align__(16) float s_w[49 * COUT];
-  __shared__ float s_sc[COUT], s_sh[COUT];
-  for (int i = threadIdx.x; i < 49 * COUT; i += blockDim.x) s_w[i] = wt[i];
-  for (int i = threadIdx.x; i < COUT; i += blockDim.x) {
-    s_sc[i] = scale[i];
-    s_sh[i] = shift[i];
-  }
-  __syncthreads();
-  const int Ho = H / 2, Wo = W / 2;
-  const int n = blockIdx.z;
-  const int oy = blockIdx.y;
-  const int ox = blockIdx.x * blockDim.x + threadIdx.x;
-  if (ox >= Wo) return;
-  float in[49];
-#pragma unroll
-  for (int ky = 0; ky < 7; ++ky) {
-    const int iy = oy * 2 + ky - 3;
-#pragma unroll
-    for (int kx = 0; kx < 7; ++kx) {
-      const int ix = ox * 2 + kx - 3;
-      in[ky * 7 + kx] = (iy >= 0 && iy < H && ix >= 0 && ix < W) ? img[(static_cast<long>(n) * H + iy) * W + ix] : 0.f;
-    }
-  }
-  const long pix = (static_cast<long>(n) * Ho + oy) * Wo + ox;
-#pragma unroll 1
-  for (int c0 = 0; c0 < COUT; c0 += 32) {
-    float acc[32];
-#pragma unroll
-    for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-#pragma unroll
-    for (int t = 0; t < 49; ++t) {
-      const float v = in[t];
-      const float4* wp = reinterpret_cast<const float4*>(&s_w[t * COUT + c0]);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 w4 = wp[j];
-        acc[4 * j] = fmaf(v, w4.x, acc[4 * j]);
-        acc[4 * j + 1] = fmaf(v, w4.y, acc[4 * j + 1]);
-        acc[4 * j + 2] = fmaf(v, w4.z, acc[4 * j + 2]);
-        acc[4 * j + 3] = fmaf(v, w4.w, acc[4 * j + 3]);
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < 32; ++j) acc[j] = fmaxf(fmaf(acc[j], s_sc[c0 + j], s_sh[c0 + j]), 0.f);
-    store_planes32(out_hi + pix * out_ld + c0, out_lo + pix * out_ld + c0, acc);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
 // Linear attention, source side (reference linear_attention.py:43-44):
 //   KV[g,h,d,v] = sum_s K[s,h,d] * V[s,h,v],   Ksum[g,h,d] = sum_s K[s,h,d]
-// over the rows s of group g (an image at coarse level).  K = elu+1 and the padding mask were already
-// applied by the projection epilogue.  The reference's V/S ... *S rescale is an fp16-overflow guard
-// and a mathematical no-op in fp32 (SURVEY.md §9 V3), so it is not reproduced.
-// Two-stage and atomics-free so the result is bit-reproducible: (g, h, split) partials, then a merge.
-template <int D>
-__global__ void __launch_bounds__(256) kv_partial_kernel(const float* __restrict__ qkv, int ld, int k_col0,
-                                                         int v_col0, long row_base, int rows_per_group,
-                                                         int rows_per_split, float* __restrict__ part) {
-  static_assert(D == 32, "coarse head dim");
-  constexpr int TOK = 32;
-  __shared__ float sK[TOK][D];
-  __shared__ __align__(16) float sV[TOK][D];
-  const int g = blockIdx.x, hd = blockIdx.y, split = blockIdx.z, nsplit = gridDim.z;
-  const int tid = threadIdx.x;
-  const int d = tid >> 3;           // 0..31
-  const int v0 = (tid & 7) * 4;     // 0,4,..,28
-  float acc[4] = {0.f, 0.f, 0.f, 0.f};
-  float ks = 0.f;
-  const int s_begin = split * rows_per_split;
-  const int s_end = min(s_begin + rows_per_split, rows_per_group);
-  for (int s0 = s_begin; s0 < s_end; s0 += TOK) {
-    // 256 threads load 32 tokens x (32 K + 32 V) floats: thread -> (token = tid/8, 4 floats at (tid%8)*4)
-    {
-      const int tok = tid >> 3;
-      const int s = s0 + tok;
-      float4 kk = make_float4(0.f, 0.f, 0.f, 0.f), vv = kk;
-      if (s < s_end) {
-        const float* rowp = qkv + (row_base + static_cast<long>(g) * rows_per_group + s) * ld;
-        kk = *reinterpret_cast<const float4*>(rowp + k_col0 + hd * D + v0);
-        vv = *reinterpret_cast<const float4*>(rowp + v_col0 + hd * D + v0);
-      }
-      sK[tok][v0] = kk.x; sK[tok][v0 + 1] = kk.y; sK[tok][v0 + 2] = kk.z; sK[tok][v0 + 3] = kk.w;
-      *reinterpret_cast<float4*>(&sV[tok][v0]) = vv;
-    }
-    __syncthreads();
-#pragma unroll 8
-    for (int tok = 0; tok < TOK; ++tok) {
-      const float k = sK[tok][d];
-      const float4 vv = *reinterpret_cast<const float4*>(&sV[tok][v0]);
-      acc[0] = fmaf(k, vv.x, acc[0]);
-      acc[1] = fmaf(k, vv.y, acc[1]);
-      acc[2] = fmaf(k, vv.z, acc[2]);
-      acc[3] = fmaf(k, vv.w, acc[3]);
-      ks += k;
-    }
-    __syncthreads();
-  }
-  float* out = part + ((static_cast<long>(g) * gridDim.y + hd) * nsplit + split) * (D * D + D);
-  *reinterpret_cast<float4*>(out + d * D + v0) = make_float4(acc[0], acc[1], acc[2], acc[3]);
-  if ((tid & 7) == 0) out[D * D + d] = ks;
-}
+// over the rows s of group g.  K = elu+1 and the padding mask were already applied by the projection epilogue.  The
+// reference's V/S ... *S rescale is an fp16-overflow guard and a mathematical no-op in fp32 (SURVEY.md §9 V3), so it is
+// not reproduced.  Atomics-free so the result is bit-reproducible.
 
-// Second version of the (group, split) partial: one block covers ALL heads of a token range, so every token's
-// K|V segment (2*H*D contiguous floats) is fetched as one coalesced 2 KB read instead of 2*H separate 128-byte
-// pieces; warp = head, lane = v column, 32 accumulators (one per d) per lane.  Same summation order per output
-// element as kv_partial_kernel (sequential over tokens) -> bit-identical partials.
-template <int D, int H>
-__global__ void __launch_bounds__(32 * H) kv_partial_v2_kernel(const float* __restrict__ qkv, int ld, int k_col0,
-                                                               long row_base, int rows_per_group, int rows_per_split,
-                                                               float* __restrict__ part) {
-  static_assert(D == 32 && H == 8, "coarse head layout");
-  constexpr int C = D * H;      // 256
-  constexpr int TOK = 16;
-  __shared__ __align__(16) float sKV[TOK][2 * C];   // K | V of 16 tokens: 32 KB
-  const int g = blockIdx.x, split = blockIdx.y, nsplit = gridDim.y;
-  const int tid = threadIdx.x, hd = tid >> 5, lane = tid & 31;
-  float acc[D];
-#pragma unroll
-  for (int d = 0; d < D; ++d) acc[d] = 0.f;
-  float ks = 0.f;
-  const int s_begin = split * rows_per_split;
-  const int s_end = min(s_begin + rows_per_split, rows_per_group);
-  for (int s0 = s_begin; s0 < s_end; s0 += TOK) {
-#pragma unroll
-    for (int i = 0; i < (TOK * 2 * C / 4) / (32 * H); ++i) {   // 8 float4 per thread
-      const int idx = tid + i * 32 * H;
-      const int tok = idx / (2 * C / 4), c4 = idx % (2 * C / 4);
-      const int srow = s0 + tok;
-      float4 v4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (srow < s_end) {
-        const float* rowp = qkv + (row_base + static_cast<long>(g) * rows_per_group + srow) * ld + k_col0;
-        v4 = *reinterpret_cast<const float4*>(rowp + c4 * 4);
-      }
-      *reinterpret_cast<float4*>(&sKV[tok][c4 * 4]) = v4;
-    }
-    __syncthreads();
-#pragma unroll 4
-    for (int tok = 0; tok < TOK; ++tok) {
-      const float v = sKV[tok][C + hd * D + lane];
-      ks += sKV[tok][hd * D + lane];
-#pragma unroll
-      for (int d4 = 0; d4 < D / 4; ++d4) {
-        const float4 k4 = *reinterpret_cast<const float4*>(&sKV[tok][hd * D + d4 * 4]);
-        acc[4 * d4] = fmaf(k4.x, v, acc[4 * d4]);
-        acc[4 * d4 + 1] = fmaf(k4.y, v, acc[4 * d4 + 1]);
-        acc[4 * d4 + 2] = fmaf(k4.z, v, acc[4 * d4 + 2]);
-        acc[4 * d4 + 3] = fmaf(k4.w, v, acc[4 * d4 + 3]);
-      }
-    }
-    __syncthreads();
-  }
-  float* out = part + ((static_cast<long>(g) * H + hd) * nsplit + split) * (D * D + D);
-#pragma unroll
-  for (int d = 0; d < D; ++d) out[d * D + lane] = acc[d];
-  out[D * D + lane] = ks;
-}
-
-// kv[g,h,:] = sum over splits (fixed order).  Layout of kv: [g][h][D*D + D] (KV then Ksum).
-__global__ void kv_merge_kernel(const float* __restrict__ part, int nsplit, int per, float* __restrict__ kv,
-                                long total) {
-  const long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x;
-  if (i >= total) return;
-  const long gh = i / per;
-  const int e = static_cast<int>(i - gh * per);
-  float s = 0.f;
-  for (int k = 0; k < nsplit; ++k) s += part[(gh * nsplit + k) * per + e];
-  kv[i] = s;
-}
-
-// Sum of the per-row-tile partials written by the EpiKv epilogue: part [groups][m_tiles][H*per] -> kv [groups][H*per]
-// (fixed order over the row tiles: bit-reproducible).
-__global__ void kv_tile_merge_kernel(const float* __restrict__ part, int m_tiles, int hper, float* __restrict__ kv,
+// Sum of the per-split partials written by kv_gemm_kernel (coarse level): part [groups][nparts][H*per] ->
+// kv [groups][H*per] (fixed order over the splits: bit-reproducible).
+__global__ void kv_tile_merge_kernel(const float* __restrict__ part, int nparts, int hper, float* __restrict__ kv,
                                      long total) {
   pdl_trigger();
   const long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x;
   if (i >= total) return;
   const long g = i / hper;
   const int e = static_cast<int>(i - g * hper);
-  const float* src = part + g * m_tiles * hper + e;
+  const float* src = part + g * nparts * hper + e;
   float acc = 0.f;
-  for (int k = 0; k < m_tiles; ++k) acc += src[static_cast<long>(k) * hper];
+  for (int k = 0; k < nparts; ++k) acc += src[static_cast<long>(k) * hper];
   kv[i] = acc;
 }
 
-// Window variant for the fine transformer (group = one 5x5 window = 25 rows, D = 16, H = 8):
-// one block per window, all heads; writes kv directly.
+// Window variant for the fine transformer (group = one window of at most 32 rows, D = 16, H = 8): one block per
+// window, all heads; writes kv directly.  Only the cross pass between windows of different sizes uses it (with
+// attn_apply_kernel<16, 8>); equal windows run window_attn_kernel.
 template <int D, int H>
 __global__ void __launch_bounds__(256) kv_window_kernel(const float* __restrict__ qkv, int ld, int k_col0,
                                                         int v_col0, long row_base, int rows_per_group,
@@ -1130,57 +957,6 @@ __global__ void fine_match_kernel(const FineMatchParams p) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// FPN top-down path: F.interpolate(x, scale_factor=2, mode='bilinear', align_corners=True) of an NHWC plane pair
-// (reference resnet_fpn.py:107-113), written as planes so that the lateral 1x1 convolution adds it through its
-// coalesced, L2-prefetched residual path (the four-neighbour gather inside that convolution's epilogue was latency
-// bound: 1.24 ms for 0.14 ms of MMA work).  One thread per (pixel, 8 channels); the small source stays L2-resident.
-__global__ void upsample2x_planes_kernel(const __half* __restrict__ src_hi, const __half* __restrict__ src_lo, int src_ld,
-                                         int sh, int sw, __half* __restrict__ dst_hi, __half* __restrict__ dst_lo,
-                                         int dst_ld, int dh, int dw, int groups, long total) {
-  const long idx = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x;
-  if (idx >= total) return;
-  const int g = static_cast<int>(idx % groups);
-  const long pix = idx / groups;
-  const int x = static_cast<int>(pix % dw);
-  const int y = static_cast<int>((pix / dw) % dh);
-  const long n = pix / (static_cast<long>(dw) * dh);
-  // PyTorch upsample_bilinear2d, align_corners=True: src = dst * (in - 1) / (out - 1)
-  const float sy = dh > 1 ? static_cast<float>(sh - 1) / static_cast<float>(dh - 1) : 0.f;
-  const float sx = dw > 1 ? static_cast<float>(sw - 1) / static_cast<float>(dw - 1) : 0.f;
-  const float fy = sy * y, fx = sx * x;
-  const int y0 = static_cast<int>(fy), x0 = static_cast<int>(fx);
-  const int y1 = y0 + (y0 < sh - 1 ? 1 : 0), x1 = x0 + (x0 < sw - 1 ? 1 : 0);
-  const float wy1 = fy - y0, wx1 = fx - x0, wy0 = 1.f - wy1, wx0 = 1.f - wx1;
-  const long base = n * sh * sw;
-  const long o[4] = {(base + static_cast<long>(y0) * sw + x0) * src_ld + g * 8, (base + static_cast<long>(y0) * sw + x1) * src_ld + g * 8,
-                     (base + static_cast<long>(y1) * sw + x0) * src_ld + g * 8, (base + static_cast<long>(y1) * sw + x1) * src_ld + g * 8};
-  float v[4][8];
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const uint4 h4 = *reinterpret_cast<const uint4*>(src_hi + o[q]);
-    const uint4 l4 = *reinterpret_cast<const uint4*>(src_lo + o[q]);
-    const uint32_t hw[4] = {h4.x, h4.y, h4.z, h4.w}, lw[4] = {l4.x, l4.y, l4.z, l4.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&hw[k]));
-      const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&lw[k]));
-      v[q][2 * k] = fh.x + fl.x;
-      v[q][2 * k + 1] = fh.y + fl.y;
-    }
-  }
-  uint32_t oh[4], ol[4];
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const float u0 = wy0 * (wx0 * v[0][2 * k] + wx1 * v[1][2 * k]) + wy1 * (wx0 * v[2][2 * k] + wx1 * v[3][2 * k]);
-    const float u1 = wy0 * (wx0 * v[0][2 * k + 1] + wx1 * v[1][2 * k + 1]) + wy1 * (wx0 * v[2][2 * k + 1] + wx1 * v[3][2 * k + 1]);
-    split_f16x2(u0, u1, oh[k], ol[k]);
-  }
-  const long d = pix * dst_ld + g * 8;
-  *reinterpret_cast<uint4*>(dst_hi + d) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-  *reinterpret_cast<uint4*>(dst_lo + d) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
-}
-
-// ------------------------------------------------------------------------------------------------
 // Evaluation harness (SURVEY.md §8(f) rank 3): squared symmetric epipolar distance of every match against the
 // ground-truth relative pose of its pair (reference src/utils/metrics.py:30-72): E = [t]_x R from T_0to1, points
 // normalised by the intrinsics, d = (p1^T E p0)^2 (1 / |(E p0)_xy|^2 + 1 / |(E^T p1)_xy|^2).  One thread per match.
@@ -1216,96 +992,6 @@ __global__ void epipolar_error_kernel(const float* __restrict__ mk0, const float
   const float c1 = E[1] * x1 + E[4] * y1 + E[7];
   const float pep = x1 * a0 + y1 * a1 + a2;
   err[m] = pep * pep * (1.0f / (a0 * a0 + a1 * a1) + 1.0f / (c0 * c0 + c1 * c1));
-}
-
-// Second version of the stem: two horizontally adjacent output pixels per thread share every weight fetch
-// (7 x 9 input patch in registers), halving the shared-memory reads per FMA.
-template <int COUT>
-__global__ void __launch_bounds__(128) conv_stem7x7_v2_kernel(const float* __restrict__ img, int H, int W,
-                                                              const float* __restrict__ wt /*[49][COUT]*/,
-                                                              const float* __restrict__ scale,
-                                                              const float* __restrict__ shift,
-                                                              __half* __restrict__ out_hi, __half* __restrict__ out_lo,
-                                                              int out_ld) {
-  __shared__ __align__(16) float s_w[49 * COUT];
-  __shared__ float s_sc[COUT], s_sh[COUT];
-  for (int i = threadIdx.x; i < 49 * COUT; i += blockDim.x) s_w[i] = wt[i];
-  for (int i = threadIdx.x; i < COUT; i += blockDim.x) {
-    s_sc[i] = scale[i];
-    s_sh[i] = shift[i];
-  }
-  __syncthreads();
-  const int Ho = H / 2, Wo = W / 2;
-  const int n = blockIdx.z;
-  const int oy = blockIdx.y;
-  const int ox = (blockIdx.x * blockDim.x + threadIdx.x) * 2;
-  if (ox >= Wo) return;
-  const bool two = ox + 1 < Wo;
-  float in[7][9];
-#pragma unroll
-  for (int ky = 0; ky < 7; ++ky) {
-    const int iy = oy * 2 + ky - 3;
-#pragma unroll
-    for (int kx = 0; kx < 9; ++kx) {
-      const int ix = ox * 2 + kx - 3;
-      in[ky][kx] = (iy >= 0 && iy < H && ix >= 0 && ix < W) ? img[(static_cast<long>(n) * H + iy) * W + ix] : 0.f;
-    }
-  }
-  const long pix = (static_cast<long>(n) * Ho + oy) * Wo + ox;
-#pragma unroll 1
-  for (int c0 = 0; c0 < COUT; c0 += 16) {
-    float a0[16], a1[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      a0[j] = 0.f;
-      a1[j] = 0.f;
-    }
-#pragma unroll
-    for (int ky = 0; ky < 7; ++ky) {
-#pragma unroll
-      for (int kx = 0; kx < 7; ++kx) {
-        const float v0 = in[ky][kx], v1 = in[ky][kx + 2];
-        const float4* wp = reinterpret_cast<const float4*>(&s_w[(ky * 7 + kx) * COUT + c0]);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float4 w4 = wp[j];
-          a0[4 * j] = fmaf(v0, w4.x, a0[4 * j]);
-          a0[4 * j + 1] = fmaf(v0, w4.y, a0[4 * j + 1]);
-          a0[4 * j + 2] = fmaf(v0, w4.z, a0[4 * j + 2]);
-          a0[4 * j + 3] = fmaf(v0, w4.w, a0[4 * j + 3]);
-          a1[4 * j] = fmaf(v1, w4.x, a1[4 * j]);
-          a1[4 * j + 1] = fmaf(v1, w4.y, a1[4 * j + 1]);
-          a1[4 * j + 2] = fmaf(v1, w4.z, a1[4 * j + 2]);
-          a1[4 * j + 3] = fmaf(v1, w4.w, a1[4 * j + 3]);
-        }
-      }
-    }
-    // 16 channels = 32 bytes per plane per pixel
-    uint32_t h0[8], l0[8], h1[8], l1[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float x = fmaxf(fmaf(a0[2 * j], s_sc[c0 + 2 * j], s_sh[c0 + 2 * j]), 0.f);
-      float y = fmaxf(fmaf(a0[2 * j + 1], s_sc[c0 + 2 * j + 1], s_sh[c0 + 2 * j + 1]), 0.f);
-      split_f16x2(x, y, h0[j], l0[j]);
-      x = fmaxf(fmaf(a1[2 * j], s_sc[c0 + 2 * j], s_sh[c0 + 2 * j]), 0.f);
-      y = fmaxf(fmaf(a1[2 * j + 1], s_sc[c0 + 2 * j + 1], s_sh[c0 + 2 * j + 1]), 0.f);
-      split_f16x2(x, y, h1[j], l1[j]);
-    }
-    uint4* ph = reinterpret_cast<uint4*>(out_hi + pix * out_ld + c0);
-    uint4* pl = reinterpret_cast<uint4*>(out_lo + pix * out_ld + c0);
-    ph[0] = make_uint4(h0[0], h0[1], h0[2], h0[3]);
-    ph[1] = make_uint4(h0[4], h0[5], h0[6], h0[7]);
-    pl[0] = make_uint4(l0[0], l0[1], l0[2], l0[3]);
-    pl[1] = make_uint4(l0[4], l0[5], l0[6], l0[7]);
-    if (two) {
-      uint4* qh = reinterpret_cast<uint4*>(out_hi + (pix + 1) * out_ld + c0);
-      uint4* ql = reinterpret_cast<uint4*>(out_lo + (pix + 1) * out_ld + c0);
-      qh[0] = make_uint4(h1[0], h1[1], h1[2], h1[3]);
-      qh[1] = make_uint4(h1[4], h1[5], h1[6], h1[7]);
-      ql[0] = make_uint4(l1[0], l1[1], l1[2], l1[3]);
-      ql[1] = make_uint4(l1[4], l1[5], l1[6], l1[7]);
-    }
-  }
 }
 
 }  // namespace lb

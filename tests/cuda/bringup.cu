@@ -7,7 +7,6 @@
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
-#include <string>
 #include <vector>
 
 #include "../../include/loftr_b200.h"
@@ -110,15 +109,8 @@ static int run_case(int batches, int M, int N, int K, bool b_batched, float amp,
   return rc;
 }
 
-int main(int argc, char** argv) {
+int main() {
   int rc = 0;
-  if (argc > 1 && std::string(argv[1]) == "selftest") {   // second-generation CUDA-core kernels vs the first
-    static char report[4096];
-    const int r = lb_selftest(report, sizeof(report));
-    printf("%s", report);
-    printf(r == 0 ? "SELFTEST PASS\n" : "SELFTEST FAIL: %s\n", lb_last_error());
-    return r;
-  }
   printf("lb_version=%d\n", lb_version());
   rc |= run_case(1, 128, 256, 64, false, 1.f, true);     // one tile, one k-block
   rc |= run_case(1, 128, 256, 256, false, 1.f, true);    // k loop, ring wrap

@@ -50,14 +50,15 @@ def _layer_weights(model_tf):
     return [{k: sd[f"layers.{i}.{k}"] for k in names} for i in range(len(model_tf.layers))]
 
 
-@pytest.mark.parametrize("cfgname", ["coarse_equal", "coarse_masked_unequal", "fine_windows"])
+@pytest.mark.parametrize("cfgname", ["coarse_equal", "coarse_masked_unequal", "fine_windows", "fine_windows_unequal"])
 def test_transformer_matches_oracle(cfgname):
     case = CASES[0]
     model, cfg, _ = util.build_model(case, DEV)
     rs = np.random.RandomState(3)
-    if cfgname == "fine_windows":
+    if cfgname.startswith("fine_windows"):
+        # unequal: the cross layer pairs 25-row with 16-row windows (kv_window_kernel + attn_apply_kernel<16, 8>)
         tf, tcfg = model.loftr_fine, cfg["fine"]
-        n, l, s, c = 37, 25, 25, 128
+        n, l, s, c = (37, 25, 16, 128) if cfgname == "fine_windows_unequal" else (37, 25, 25, 128)
         m0 = m1 = None
     else:
         tf, tcfg = model.loftr_coarse, cfg["coarse"]
@@ -76,6 +77,18 @@ def test_transformer_matches_oracle(cfgname):
     for g, o in ((g0, o0), (g1, o1)):
         err = np.abs(g.cpu().numpy() - o).max()
         assert err < 2e-4, f"{cfgname}: transformer output differs by {err:.3e}"
+
+
+def test_fine_transformer_rejects_windows_over_32_rows():
+    """A cross layer between windows of different sizes serves at most 32 query rows per window."""
+    import loftr_b200
+    cfg = build_cfg(CASES[0])
+    cfg["fine"]["layer_names"] = ["cross", "self"]
+    model = loftr_b200.LoFTR(cfg).eval().to(DEV)
+    f0 = torch.randn(3, 36, 128, device=DEV)
+    f1 = torch.randn(3, 16, 128, device=DEV)
+    with pytest.raises(RuntimeError, match="at most 32 rows"):
+        model.loftr_fine(f0, f1)
 
 
 # ------------------------------------------------------------------------------------------------ coarse matching

@@ -42,5 +42,5 @@ for (m, n, k) in [(76800, 256, 256), (76800, 768, 256), (76800, 512, 512), (7680
     ref = (a.double() @ w.double().T)
     same = f"{float((outs[0].double() - ref).abs().max() / ref.abs().max()):.2e}"
     fl = 2.0 * m * n * k * 3
-    print(f"M={m} N={n} K={k}: " + "  ".join(f"{kk} {v * 1e3:7.1f} us ({fl / v / 1e9:6.0f} TF/s issued)" for kk, v in res.items()) + f"  rel err vs fp64: {same}  (TMA_STORE={os.environ.get('LOFTR_B200_TMA_STORE', '1')})", flush=True)
+    print(f"M={m} N={n} K={k}: " + "  ".join(f"{kk} {v * 1e3:7.1f} us ({fl / v / 1e9:6.0f} TF/s issued)" for kk, v in res.items()) + f"  rel err vs fp64: {same}", flush=True)
 os.environ["LOFTR_B200_PROBE_NULL_EPI"] = "0"
