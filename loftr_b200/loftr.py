@@ -617,6 +617,9 @@ class LoFTR(nn.Module):
                              f"{fc['nhead']})")
         if config["fine_window_size"] ** 2 > 32 or config["fine_window_size"] % 2 == 0:
             raise ValueError("loftr_b200 builds fine windows of odd size with at most 32 cells (fine_window_size <= 5)")
+        if config["fine_window_size"] < 3:   # the refinement grid steps by 2 / (W - 1)  [fine_matching.py:50]
+            raise ValueError(f"fine_window_size must be 3 or 5 (got {config['fine_window_size']}): a 1-cell window has no "
+                             "sub-pixel grid to refine on")
         self.expose_coarse_features = False   # True: forward also writes data['_feat_c0'/'_feat_c1'] (not reference keys)
         self.backbone = build_backbone(config)
         if backbone_impl == "auto":

@@ -135,6 +135,17 @@ def test_unsupported_shapes_fail_at_construction():
         loftr_b200.LoFTR(cfg)
 
 
+@pytest.mark.parametrize("w", [1, -1])
+def test_window_below_3_is_rejected(w):
+    """W = 1 would divide the refinement grid by W - 1 = 0 (NaN coordinates in the reference)."""
+    cfg = loftr_b200.get_cfg("indoor_ds")
+    cfg["fine_window_size"] = w
+    with pytest.raises(ValueError, match="must be 3 or 5"):
+        loftr_b200.LoFTR(cfg)
+    cfg["fine_window_size"] = 3
+    assert loftr_b200.LoFTR(cfg).fine_preprocess.W == 3
+
+
 def test_bench_clock_sampler_filters_by_timestamp():
     """bench.py's nvidia-smi sampler runs for the whole process; only rows stamped inside the timed region count
     (rows within 0.25 s of its end are the fallback when the region was shorter than one sampling period)."""
