@@ -144,6 +144,20 @@ static int device_check(int* sm_count) {
   return 0;
 }
 
+// Allows `Kernel` up to `bytes` of dynamic shared memory on the current device (needed above 48 KB); the attribute is
+// set on the first launch per device.
+template <auto Kernel>
+static int set_max_dynamic_smem(int bytes) {
+  static bool configured[kMaxDevices] = {false};
+  int dev = 0;
+  LB_CUDA(cudaGetDevice(&dev));
+  if (!configured[dev]) {
+    LB_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    configured[dev] = true;
+  }
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------------ TMA maps
 static PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
   static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
@@ -277,14 +291,8 @@ static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const t
   using S = GemmSmem<BN, Epi::kSmemBytes>;
   constexpr int smem_bytes = S::kRingBytes + S::kBarBytes + Epi::kSmemBytes;
   static_assert(smem_bytes <= 232448, "shared memory budget exceeded");
-  auto kern = gemm_split_kernel<BN, Epi>;
-  static bool configured[kMaxDevices] = {false};  // per instantiation and device
-  int dev = 0;
-  LB_CUDA(cudaGetDevice(&dev));
-  if (!configured[dev]) {
-    LB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    configured[dev] = true;
-  }
+  constexpr auto kern = &gemm_split_kernel<BN, Epi>;
+  LB_TRY(set_max_dynamic_smem<kern>(smem_bytes));
   const long items = static_cast<long>(s.batches) * s.m_tiles * s.n_chunks;
   const int grid = static_cast<int>(items < sms ? items : sms);
   TimingRec rec{nullptr, nullptr, tag};
@@ -361,7 +369,7 @@ struct ConvDesc {
 // channels per tap that travel as 16-channel boxes (gemm_split.cuh ConvGeom).
 static void conv_layout(int cin, int* cin_blocks, int* rem) {
   const int r = cin % kBlockK;
-  if (kBlockK == 64 && cin > kBlockK && r > 0 && r <= kRemChannels) {
+  if (cin > kBlockK && r > 0 && r <= kRemChannels) {
     *cin_blocks = cin / kBlockK;
     *rem = r;
   } else {
@@ -369,10 +377,10 @@ static void conv_layout(int cin, int* cin_blocks, int* rem) {
     *rem = 0;
   }
 }
-template <int BN, int kUpMode = 0>
+template <int BN, bool kUpsample>
 static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_rem, const ConvDesc& d,
-                       const typename EpiConv<BN, kUpMode>::Params& ep_in, cudaStream_t st) {
-  using Epi = EpiConv<BN, kUpMode>;
+                       const typename EpiConv<BN, kUpsample>::Params& ep_in, cudaStream_t st) {
+  using Epi = EpiConv<BN, kUpsample>;
   int sms = 0;
   LB_TRY(device_check(&sms));
   GemmShape s;
@@ -562,17 +570,14 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
     EpiConv<BN, UP>::Params ep{w.scale, w.shift, r.act, r.res ? r.res->hi : nullptr, r.res ? r.res->lo : nullptr,     \
                                r.res ? r.res->ld : 0, r.up ? r.up->hi : nullptr, r.up ? r.up->lo : nullptr,          \
                                r.up ? r.up->ld : 0, r.up_h, r.up_w, r.out ? r.out->hi : nullptr,                      \
-                               r.out ? r.out->lo : nullptr, r.out ? r.out->ld : 0, r.out_f32, r.f32_ld, 0, 0, 0, om, \
-                               um};                                                                                   \
+                               r.out ? r.out->lo : nullptr, r.out ? r.out->ld : 0, r.out_f32, r.f32_ld, 0, 0, 0, om}; \
     return launch_conv<BN, UP>(in, wg, wr, d, ep, st);                                                                \
   }
 #define LB_CONV_CASE(BN)                                                                                              \
   {                                                                                                                   \
-    if (r.up) LB_CONV_CASE_UP(BN, 2)                                                                                  \
-    LB_CONV_CASE_UP(BN, 0)                                                                                            \
+    if (r.up) LB_CONV_CASE_UP(BN, true)                                                                               \
+    LB_CONV_CASE_UP(BN, false)                                                                                        \
   }
-  UpMaps um;
-  memset(&um, 0, sizeof(um));
   // output-channel tile: the smallest built N that covers Cout (196 -> 208: 13 x 16, no MMAs on 60 padding columns)
   if (w.cout <= 128) LB_CONV_CASE(128)
   if (w.cout <= 208) LB_CONV_CASE(208)
@@ -608,19 +613,16 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
     using Epi = EpiPlanes<BN>;
     Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, 0};
     Planes B{wq_hi, wq_lo, C, 0};
-    OutMaps om;
-    LB_TRY(fill_out_maps(&om, w.att_hi + x_base * C, w.att_lo + x_base * C, C, nullptr, 0, C, x_rows, 1));
-    typename Epi::Params ep{0, nullptr, 1, nullptr, 0, w.att_hi + x_base * C, w.att_lo + x_base * C, C, 0, lw.s_qkv, om};
+    typename Epi::Params ep{0, nullptr, 1, lw.s_qkv, {}};
+    LB_TRY(fill_out_maps(&ep.om, w.att_hi + x_base * C, w.att_lo + x_base * C, C, nullptr, 0, C, x_rows, 1));
     LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, 1, static_cast<int>(x_rows), C, C, 0, ep, stream)));
   }
   {
     using Epi = EpiPlanes<BN>;
     Planes A{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, 0};
     Planes B{wq_hi + wkv_off, wq_lo + wkv_off, C, 0};
-    OutMaps om;
-    LB_TRY(fill_out_maps(&om, w.h_hi + s_base * ldc, w.h_lo + s_base * ldc, ldc, nullptr, 0, 2 * C, s_rows, 1));
-    typename Epi::Params ep{0, nullptr, 1, nullptr, 0, w.h_hi + s_base * ldc, w.h_lo + s_base * ldc,
-                            static_cast<int>(ldc), 0, lw.s_qkv, om};
+    typename Epi::Params ep{0, nullptr, 1, lw.s_qkv, {}};
+    LB_TRY(fill_out_maps(&ep.om, w.h_hi + s_base * ldc, w.h_lo + s_base * ldc, ldc, nullptr, 0, 2 * C, s_rows, 1));
     LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, 1, static_cast<int>(s_rows), 2 * C, C, 0, ep, stream)));
   }
   const long qbs = static_cast<long>(x_group_rows) * C, kvbs = static_cast<long>(s_group_rows) * ldc;
@@ -629,13 +631,7 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
   LB_TRY(make_map(&tq_lo, w.att_lo + x_base * C, C, x_group_rows, n_groups_x, C, qbs, kFaRows, kFaD));
   LB_TRY(make_map(&tkv_hi, w.h_hi + s_base * ldc, 2 * C, s_group_rows, n_groups_s, ldc, kvbs, kFaKeys, kFaD));
   LB_TRY(make_map(&tkv_lo, w.h_lo + s_base * ldc, 2 * C, s_group_rows, n_groups_s, ldc, kvbs, kFaKeys, kFaD));
-  static bool configured[kMaxDevices] = {false};
-  int dev = 0;
-  LB_CUDA(cudaGetDevice(&dev));
-  if (!configured[dev]) {
-    LB_CUDA(cudaFuncSetAttribute(full_attn_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwSmem));
-    configured[dev] = true;
-  }
+  LB_TRY(set_max_dynamic_smem<&full_attn_wgmma_kernel>(kFwSmem));
   FullAttnWgParams wp;
   wp.Lx = x_group_rows;
   wp.Ls = s_group_rows;
@@ -698,13 +694,7 @@ static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, in
     if (splits > parts_cap) splits = parts_cap;
     const int kb_per = cdiv(kb_total, splits);
     splits = cdiv(kb_total, kb_per);
-    static bool configured[kMaxDevices] = {false};
-    int dev = 0;
-    LB_CUDA(cudaGetDevice(&dev));
-    if (!configured[dev]) {
-      LB_CUDA(cudaFuncSetAttribute(kv_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kKvGemmSmem));
-      configured[dev] = true;
-    }
+    LB_TRY(set_max_dynamic_smem<&kv_gemm_kernel>(kKvGemmSmem));
     KvGemmParams kp{w.kv_part, kb_total, kb_per, splits};
     kv_gemm_kernel<<<dim3(splits, 2, n_groups_s), kKvGemmThreads, kKvGemmSmem, stream>>>(tm_hi, tm_lo, kp);
     LB_LAUNCHED();
@@ -771,7 +761,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
       Planes B{lw.wqkv_hi, lw.wqkv_lo, C, 0};
       OutMaps om;
       LB_TRY(fill_out_maps(&om, nullptr, nullptr, 0, w.qkv + x_base * 3 * C, 3 * C, 3 * C, xM, xb));
-      typename Epi::Params ep{w.qkv + x_base * 3 * C, 3 * C, elu_self, pmask ? pmask + x_base : nullptr, lw.s_qkv, 0, om};
+      typename Epi::Params ep{elu_self, pmask ? pmask + x_base : nullptr, lw.s_qkv, om};
       LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, xb, xM, 3 * C, C, 0, ep, stream, live, x_group_rows)));
     } else {
       Planes Aq{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, xbs};
@@ -779,12 +769,12 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
       OutMaps omq, omk;
       LB_TRY(fill_out_maps(&omq, nullptr, nullptr, 0, w.qkv + x_base * 3 * C, 3 * C, C, xM, xb));
       LB_TRY(fill_out_maps(&omk, nullptr, nullptr, 0, w.qkv + s_base * 3 * C + C, 3 * C, 2 * C, sM, sb));
-      typename Epi::Params eq{w.qkv + x_base * 3 * C, 3 * C, elu_q, pmask ? pmask + x_base : nullptr, lw.s_qkv, 0, omq};
+      typename Epi::Params eq{elu_q, pmask ? pmask + x_base : nullptr, lw.s_qkv, omq};
       LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Aq, Bq, xb, xM, C, C, 0, eq, stream, live, x_group_rows)));
       Planes Ak{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, sbs};
       Planes Bk{static_cast<const __half*>(lw.wqkv_hi) + static_cast<long>(C) * C,
                 static_cast<const __half*>(lw.wqkv_lo) + static_cast<long>(C) * C, C, 0};
-      typename Epi::Params ek{w.qkv + s_base * 3 * C + C, 3 * C, elu_kv, pmask ? pmask + s_base : nullptr, lw.s_qkv, 0, omk};
+      typename Epi::Params ek{elu_kv, pmask ? pmask + s_base : nullptr, lw.s_qkv, omk};
       LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Ak, Bk, sb, sM, 2 * C, C, 0, ek, stream, live, s_group_rows)));
     }
     int sms = 0;
@@ -799,14 +789,8 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
       // linear attention, one kernel per pass: KV stays in shared memory      [linear_attention.py:43-46]
       const int grid = n_groups_x < 3 * sms ? n_groups_x : 3 * sms;   // 3 resident blocks per SM (60 KB, <= 85 registers)
       const int wa_smem = (H * (D * D + D) + 4 * x_group_rows * C) * static_cast<int>(sizeof(float));
-      static bool wa_configured[kMaxDevices] = {false};
-      int dev = 0;
-      LB_CUDA(cudaGetDevice(&dev));
-      if (!wa_configured[dev]) {
-        LB_CUDA(cudaFuncSetAttribute(window_attn_kernel<16, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (8 * (16 * 16 + 16) + 4 * 32 * 128) * static_cast<int>(sizeof(float))));
-        wa_configured[dev] = true;
-      }
+      LB_TRY((set_max_dynamic_smem<&window_attn_kernel<16, 8>>(
+          (8 * (16 * 16 + 16) + 4 * 32 * 128) * static_cast<int>(sizeof(float)))));   // largest (32-row) window
       window_attn_kernel<16, 8><<<grid, 256, wa_smem, stream>>>(w.qkv, 3 * C, 0, C, 2 * C, x_base, s_base, x_group_rows,
                                                                 n_groups_x, 1e-6f, w.att_hi, w.att_lo, C, live, live_cap);
     } else {
@@ -837,10 +821,8 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
     using Epi = EpiPlanes<BN>;
     Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, xbs};
     Planes B{lw.w1_hi, lw.w1_lo, 2 * C, 0};
-    OutMaps om;
-    LB_TRY(fill_out_maps(&om, w.h_hi + x_base * ldc, w.h_lo + x_base * ldc, ldc, nullptr, 0, 2 * C, xM, xb));
-    typename Epi::Params ep{1, nullptr, 1, nullptr, 0, w.h_hi + x_base * ldc, w.h_lo + x_base * ldc,
-                            static_cast<int>(ldc), 0, lw.s_1, om};
+    typename Epi::Params ep{1, nullptr, 1, lw.s_1, {}};
+    LB_TRY(fill_out_maps(&ep.om, w.h_hi + x_base * ldc, w.h_lo + x_base * ldc, ldc, nullptr, 0, 2 * C, xM, xb));
     LB_TRY((launch_gemm<BN, Epi>(TAG_MLP1, A, B, xb, xM, 2 * C, 2 * C, 0, ep, stream, live, x_group_rows)));
   }
   // 6. mlp[2] + norm2 + residual -> cat[:, 0:C] (and x_f32 after the last layer)   [transformer.py:55-58]
@@ -931,17 +913,15 @@ int lb_gemm_split(const void* a_hi, const void* a_lo, long lda, long a_batch_str
   Planes A{a_hi, a_lo, lda, batches > 1 ? a_batch_stride : 0};
   Planes B{b_hi, b_lo, ldb, b_batch_stride};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const char* pe = getenv("LOFTR_B200_PROBE_NULL_EPI");   // measurement probe of the main loop (tools/gemm_probe.py)
-  const int skip = pe ? atoi(pe) : 0;
   OutMaps om;
   LB_TRY(fill_out_maps(&om, nullptr, nullptr, 0, out, ldo, N, M, batches));
   if (N % 256 == 0 || N > 128) {
     using Epi = EpiActStore<256>;
-    Epi::Params ep{out, static_cast<int>(ldo), 0, nullptr, 1.f, skip, om};
+    Epi::Params ep{0, nullptr, 1.f, om};
     return launch_gemm<256, Epi>(TAG_GEMM_TEST, A, B, batches, M, N, K, 0, ep, st);
   }
   using Epi = EpiActStore<128>;
-  Epi::Params ep{out, static_cast<int>(ldo), 0, nullptr, 1.f, skip, om};
+  Epi::Params ep{0, nullptr, 1.f, om};
   return launch_gemm<128, Epi>(TAG_GEMM_TEST, A, B, batches, M, N, K, 0, ep, st);
 }
 
@@ -953,7 +933,6 @@ int lb_coarse_prep(const float* feat, int nhwc, const float* pe, int n_img, int 
   LB_TRY(dev_guard.bind(x_f32));
   LB_TRY(device_check(&sms));
   if (h > pe_h || w > pe_w) return fail("feature map %dx%d exceeds the position-encoding table %dx%d", h, w, pe_h, pe_w);
-  if (n_img <= 0) return 0;
   dim3 grid(cdiv(static_cast<long>(h) * w, 32), cdiv(C, 32), n_img);
   coarse_prep_kernel<<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
       feat, nhwc, pe, C, h, w, pe_h, pe_w, x_f32, static_cast<__half*>(cat_hi), static_cast<__half*>(cat_lo));
@@ -980,7 +959,6 @@ int lb_transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds
   const bool coarse = (C == 256 && H == 8);
   const bool fine = (C == 128 && H == 8);
   if (!coarse && !fine) return fail("unsupported transformer shape d_model=%d nhead=%d (built: 256/8 and 128/8)", C, H);
-  if (st->n_groups <= 0) return 0;
   const int* live = st->n_groups_live;
   if (live && !fine) return fail("n_groups_live is built for the fine (window) transformer only");
   const long rows0 = static_cast<long>(st->n_groups) * st->group_rows0;
@@ -1061,13 +1039,7 @@ int lb_backbone_forward(const LbBackboneWeights* w, const float* images, int N, 
     LB_TRY(make_out_map_nhwc(&sp.om.hi, B.s0.hi, false, 128, W2, H2, N, B.s0.ld));
     LB_TRY(make_out_map_nhwc(&sp.om.lo, B.s0.lo, false, 128, W2, H2, N, B.s0.ld));
     sp.om.use = 1;
-    static bool configured[kMaxDevices] = {false};
-    int dev = 0;
-    LB_CUDA(cudaGetDevice(&dev));
-    if (!configured[dev]) {
-      LB_CUDA(cudaFuncSetAttribute(conv_stem7x7_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kStemSmemBytes));
-      configured[dev] = true;
-    }
+    LB_TRY(set_max_dynamic_smem<&conv_stem7x7_tc_kernel>(kStemSmemBytes));
     const long tiles = static_cast<long>(sp.tiles_w) * sp.tiles_h * N;
     const int grid = static_cast<int>(tiles < sms ? tiles : sms);
     conv_stem7x7_tc_kernel<<<grid, kStemThreads, kStemSmemBytes, st>>>(sp);
@@ -1409,10 +1381,8 @@ int lb_fine_preprocess(const LbFinePreprocessArgs* a, void* ws, size_t ws_bytes,
   const long rows_b = rows / nb;
   Planes A{win_hi, win_lo, a->Cf, nb > 1 ? rows_b * a->Cf : 0};
   Planes B{a->merge_w_hi, a->merge_w_lo, a->Cf, 0};
-  OutMaps om;
-  LB_TRY(fill_out_maps(&om, a->cat_hi, a->cat_lo, 2 * a->Cf, a->x_f32, a->Cf, a->Cf, rows_b, nb));
-  Epi::Params ep{0, gbias, WW, a->x_f32, a->Cf, static_cast<__half*>(a->cat_hi), static_cast<__half*>(a->cat_lo),
-                 2 * a->Cf, 0, a->merge_acc_scale, om};
+  Epi::Params ep{0, gbias, WW, a->merge_acc_scale, {}};
+  LB_TRY(fill_out_maps(&ep.om, a->cat_hi, a->cat_lo, 2 * a->Cf, a->x_f32, a->Cf, a->Cf, rows_b, nb));
   return launch_gemm<128, Epi>(TAG_FINE_MERGE, A, B, nb, static_cast<int>(rows_b), a->Cf, a->Cf, 0, ep, st, a->M_live, WW);
 }
 

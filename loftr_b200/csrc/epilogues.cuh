@@ -290,12 +290,9 @@ __device__ __forceinline__ void stage_quiesce() {
 template <int BLOCK_N>
 struct EpiActStore {
   struct Params {
-    float* out;              // [batches*M, ld] (written through om.f32)
-    int ld;
     int elu_cols;            // columns [0, elu_cols) get elu+1
     const uint8_t* rowmask;  // optional [batches*M] (1 = valid)
     float acc_scale;         // 2^-e: undoes the power-of-two pre-scaling of the weight planes (exact)
-    int skip;                // probe mode (LOFTR_B200_PROBE_NULL_EPI, lb_gemm_split only): 1 = drain nothing, 2 = accumulator loads only
     OutMaps om;              // om.f32: the fp32 output
   };
   static constexpr int kSmemBytes = kEpiScratchBytes;
@@ -307,7 +304,6 @@ struct EpiActStore {
   __device__ void item_end(int, int, int) {}
   __device__ void prefetch(int, int, int) {}
   __device__ void tile(uint32_t acc_row, int batch, int m0, int n0) {
-    if (p.skip == 1) return;
     const int r = m0 + epi_row();
     const bool row_ok = r < s.M;
     const long grow = static_cast<long>(batch) * s.M + r;
@@ -320,13 +316,6 @@ struct EpiActStore {
       if (col >= s.N) break;  // warp-uniform
       float x[32];
       load_acc32(acc_row, c * 32, x);
-      if (p.skip == 2) {   // keep the loads alive without storing
-        float acc = 0.f;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc += x[j];
-        if (acc == 1.2345e-30f) p.out[0] = acc;
-        continue;
-      }
 #pragma unroll
       for (int j = 0; j < 32; ++j) x[j] *= p.acc_scale;
       if (col < p.elu_cols) {
@@ -593,14 +582,8 @@ struct EpiPlanes {
     int relu;
     const float* gbias;   // optional [groups, N]
     int group_rows;
-    float* out_f32;       // optional
-    int ld_f32;
-    __half* out_hi;
-    __half* out_lo;
-    int ld_pl;
-    int pl_col0;
     float acc_scale;      // 2^-e of the weight planes
-    OutMaps om;           // TMA-store maps of (out_hi, out_lo) [based at column pl_col0] and out_f32
+    OutMaps om;           // TMA-store maps of the outputs: om.use bit 0 = fp16 planes, bit 1 = fp32 (either or both)
   };
   static constexpr int kSmemBytes = kEpiScratchBytes;
   const Params& p;
@@ -641,8 +624,8 @@ struct EpiPlanes {
         }
       }
       const OutCoord oc{col, m0 + ((epi_tid() >> 5) & 3) * 32, batch, 0};
-      if (p.out_f32) warp_tma_store_f32x32(scr, p.om, oc, x);
-      if (p.out_hi) warp_tma_store_planes32(scr, p.om, oc, x);
+      if (p.om.use & 2) warp_tma_store_f32x32(scr, p.om, oc, x);
+      if (p.om.use & 1) warp_tma_store_planes32(scr, p.om, oc, x);
     }
   }
 };
@@ -657,23 +640,12 @@ struct EpiPlanes {
 //   y = relu / leaky_relu(0.01) / identity
 // written as NHWC fp16 planes (the next convolution's A operand) and / or NHWC fp32.
 //
-// kUpMode selects the FPN merge: 0 = none (every other layer: no upsample code, leanest registers), 1 = staged window,
-// 2 = per-thread global gathers (any shape).  The engine dispatches 0 and 2: the staged window's shared memory does
-// not fit beside the TMA ring and the accumulator staging of gemm_split_kernel.
-// kUpMode = 1 (the two FPN lateral 1x1 convolutions): the 6 x 10 source pixels whose bilinear footprints cover the
-// 8 x 16 output tile are fetched ONCE per tile by TMA into shared memory (boxes of 200 / 2 x 136 channels: the pixel
-// stride of 100 / 68 words keeps the quarter-warp LDS.128 conflict-free) while the tile's MMAs run; the four
-// neighbours of a pixel are then shared-memory reads.  With per-thread global loads (kUpMode = 2) the
-// kernel is bound by L1 tag lookups: 32 LDG.128 per thread and 32-channel group, each touching ~16 lines.
-struct UpMaps {
-  CUtensorMap hi, lo;   // upsample source planes [batches, up_h, up_w, C], unswizzled boxes (kUpBoxC, 10, 6, 1)
-};
-constexpr int kUpW = 10, kUpH = 6;
-template <int BLOCK_N, int kUpMode = 0>
+// kUpsample selects the FPN merge at compile time.  false: every layer but the two FPN laterals, built without any
+// upsample code (leanest registers).  true: the two FPN lateral 1x1 convolutions; each thread gathers the four
+// bilinear neighbours of its pixel from the source planes in global memory (any shape).
+template <int BLOCK_N, bool kUpsample>
 struct EpiConv {
   static constexpr bool kNoRowBound = true;      // backbone shapes are static: no device row bound (gemm_split.cuh)
-  static constexpr bool kUp = kUpMode == 1;      // staged window
-  static constexpr bool kUpAny = kUpMode != 0;
   struct Params {
     const float* scale;   // [N]
     const float* shift;   // [N]
@@ -691,61 +663,30 @@ struct EpiConv {
     int f32_ld;
     int H_out, W_out, tiles_w;
     OutMaps om;           // NHWC TMA-store maps (channel, x, y, image): box 32 channels x 16 x 2 pixels
-    UpMaps um;            // kUp only
   };
   static constexpr int kChunks = (BLOCK_N + 31) / 32;        // 32-column groups of the tile (the last may be partial)
   static constexpr int kChunksHalf0 = (kChunks + 1) / 2;     // column half 0 takes the first ones
   static constexpr int kCols = kChunks * 32;
-  static constexpr int kUpBoxC = BLOCK_N <= 208 ? 200 : 136; // channels per staged pixel (one box / two boxes at 0, 128)
-  static constexpr int kUpBoxes = BLOCK_N <= 208 ? 1 : 2;
-  static constexpr int kUpBoxData = kUpH * kUpW * kUpBoxC * 2;          // bytes one TMA box delivers
-  static constexpr int kUpBoxBytes = (kUpBoxData + 127) & ~127;         // its (128-byte aligned) slot
-  static constexpr int kUpPlaneBytes = kUpBoxes * kUpBoxBytes;
-  static constexpr int kUpOffset = kEpiScratchBytes + 2 * kCols * 4;
+  static constexpr int kXposeOffset = kEpiScratchBytes + 2 * kCols * 4;   // behind the staging tiles and scale / shift
   // N = 208 has 17.9 KB of shared memory to spare beside its three-stage ring: the residual transposer gets its own
   // 2 KB per warp there instead of aliasing the TMA-store staging tile, so a chunk's residual read no longer waits for
   // the copy engine to finish reading the previous chunk's store (11 us per tile in the layer2 conv2 kernels)
-  static constexpr bool kOwnXpose = BLOCK_N == 208 && kUpMode == 0;
-  static constexpr int kSmemBytes = kUpOffset + (kUp ? 2 * kUpPlaneBytes + 16 : 0) + (kOwnXpose ? 8 * 2048 : 0);
-  static_assert(kUpOffset % 128 == 0 && kUpBoxBytes % 128 == 0, "TMA destinations are 128-byte aligned");
-  static_assert(!kUp || BLOCK_N > 128, "the staged upsample is built for the 196- and 256-channel laterals");
+  static constexpr bool kOwnXpose = BLOCK_N == 208 && !kUpsample;
+  static constexpr int kSmemBytes = kXposeOffset + (kOwnXpose ? 8 * 2048 : 0);
   const Params& p;
   const GemmShape& s;
   float* s_scale;
   float* s_shift;
   uint32_t* scr;
   uint32_t* xscr;       // transposer scratch of the residual loads (== scr unless kOwnXpose)
-  uint8_t* s_up;        // [hi | lo][box][6][10][kUpBoxC] fp16
-  uint64_t* up_bar;
-  uint32_t up_phase = 0;
   __device__ EpiConv(const Params& p_, uint8_t* smem, const GemmShape& s_) : p(p_), s(s_), scr(epi_scratch(smem)) {
     s_scale = reinterpret_cast<float*>(smem + kEpiScratchBytes);
     s_shift = s_scale + kCols;
-    s_up = smem + kUpOffset;
-    xscr = kOwnXpose ? reinterpret_cast<uint32_t*>(smem + kUpOffset + ((epi_tid() >> 5) << 11)) : scr;
-    up_bar = reinterpret_cast<uint64_t*>(smem + kUpOffset + 2 * kUpPlaneBytes);
-    if (kUp) {
-      if ((smem_u32(s_up) & 127u) != 0) asm volatile("trap;");
-      if (epi_tid() == 0) {
-        mbar_init(up_bar, 1);
-        fence_barrier_init();
-        tma_prefetch_desc(&p.um.hi);
-        tma_prefetch_desc(&p.um.lo);
-      }
-    }
+    xscr = kOwnXpose ? reinterpret_cast<uint32_t*>(smem + kXposeOffset + ((epi_tid() >> 5) << 11)) : scr;
     if (s.n_tiles == 1) {   // every layer of the backbone: one n-tile -> the folded BatchNorm is staged once per CTA
       stage_affine(0);
       epi_bar_sync();
-    } else if (kUp) {
-      epi_bar_sync();
     }
-  }
-  // first source row / column of the staged window of tile (ty, tx): the footprint of its first pixel
-  __device__ void up_window(int ty, int tx, int& ybase, int& xbase) const {
-    const float sh = p.H_out > 1 ? static_cast<float>(p.up_h - 1) / static_cast<float>(p.H_out - 1) : 0.f;
-    const float sw = p.W_out > 1 ? static_cast<float>(p.up_w - 1) / static_cast<float>(p.W_out - 1) : 0.f;
-    ybase = static_cast<int>(sh * (ty * kConvTileH));
-    xbase = static_cast<int>(sw * (tx * kConvTileW));
   }
   __device__ void stage_affine(int n0) {
     for (int j = epi_tid(); j < kCols; j += kEpiThreads) {
@@ -758,23 +699,7 @@ struct EpiConv {
   __device__ void item_end(int, int, int) {}
   // residual / FPN-upsample source rows of this thread's pixel -> L2, issued while the tile's MMAs still run
   __device__ void prefetch(int batch, int m0, int n0) {
-    if (kUp) {
-      // every epilogue thread has finished reading the previous tile's window (it got here); then one thread refills it
-      epi_bar_sync();
-      if (epi_tid() == 0) {
-        const int mt = m0 / kBlockM;
-        const int ty = mt / p.tiles_w, tx = mt - ty * p.tiles_w;
-        int ybase, xbase;
-        up_window(ty, tx, ybase, xbase);
-        mbar_arrive_expect_tx(up_bar, 2 * kUpBoxes * kUpBoxData);
-#pragma unroll
-        for (int b = 0; b < kUpBoxes; ++b) {
-          tma_load_4d(s_up + b * kUpBoxBytes, &p.um.hi, up_bar, b * 128, xbase, ybase, batch);
-          tma_load_4d(s_up + kUpPlaneBytes + b * kUpBoxBytes, &p.um.lo, up_bar, b * 128, xbase, ybase, batch);
-        }
-      }
-    }
-    if (!p.res_hi && (kUp || !p.up_hi)) return;
+    if (!p.res_hi && !p.up_hi) return;
     const int row = epi_row();
     const int mt = m0 / kBlockM;
     const int ty = mt / p.tiles_w, tx = mt - ty * p.tiles_w;
@@ -792,7 +717,7 @@ struct EpiConv {
         prefetch_l2(p.res_lo + pix * p.res_ld + c);
       }
     }
-    if (kUpMode == 2 && p.up_hi) {
+    if (kUpsample && p.up_hi) {
       const float sh = p.H_out > 1 ? static_cast<float>(p.up_h - 1) / static_cast<float>(p.H_out - 1) : 0.f;
       const float sw = p.W_out > 1 ? static_cast<float>(p.up_w - 1) / static_cast<float>(p.W_out - 1) : 0.f;
       const int y0 = static_cast<int>(sh * y), x0 = static_cast<int>(sw * x);
@@ -819,11 +744,11 @@ struct EpiConv {
     const int x = tx * kConvTileW + row % kConvTileW;
     const bool ok = y < p.H_out && x < p.W_out;
     const long pix = (static_cast<long>(batch) * p.H_out + y) * p.W_out + x;
-    // bilinear source coordinates (PyTorch upsample_bilinear2d, align_corners=True)
-    // kUp: u.. are fp16-element offsets of the neighbour pixels inside one staged box, else into the global planes
+    // bilinear source coordinates (PyTorch upsample_bilinear2d, align_corners=True); u.. are the fp16-element offsets
+    // of the four neighbour pixels in the source planes
     long u00 = 0, u01 = 0, u10 = 0, u11 = 0;
     float wy1 = 0.f, wx1 = 0.f;
-    if (kUpAny && p.up_hi && ok) {
+    if (kUpsample && p.up_hi && ok) {
       const float sh = p.H_out > 1 ? static_cast<float>(p.up_h - 1) / static_cast<float>(p.H_out - 1) : 0.f;
       const float sw = p.W_out > 1 ? static_cast<float>(p.up_w - 1) / static_cast<float>(p.W_out - 1) : 0.f;
       const float fy = sh * y, fx = sw * x;
@@ -831,24 +756,11 @@ struct EpiConv {
       const int y1 = y0 + (y0 < p.up_h - 1 ? 1 : 0), x1 = x0 + (x0 < p.up_w - 1 ? 1 : 0);
       wy1 = fy - y0;
       wx1 = fx - x0;
-      if (kUp) {
-        int ybase, xbase;
-        up_window(ty, tx, ybase, xbase);
-        u00 = ((y0 - ybase) * kUpW + (x0 - xbase)) * kUpBoxC;
-        u01 = ((y0 - ybase) * kUpW + (x1 - xbase)) * kUpBoxC;
-        u10 = ((y1 - ybase) * kUpW + (x0 - xbase)) * kUpBoxC;
-        u11 = ((y1 - ybase) * kUpW + (x1 - xbase)) * kUpBoxC;
-      } else {
-        const long base = static_cast<long>(batch) * p.up_h * p.up_w;
-        u00 = (base + static_cast<long>(y0) * p.up_w + x0) * p.up_ld;
-        u01 = (base + static_cast<long>(y0) * p.up_w + x1) * p.up_ld;
-        u10 = (base + static_cast<long>(y1) * p.up_w + x0) * p.up_ld;
-        u11 = (base + static_cast<long>(y1) * p.up_w + x1) * p.up_ld;
-      }
-    }
-    if (kUp) {   // this tile's window has landed
-      mbar_wait(up_bar, up_phase);
-      up_phase ^= 1u;
+      const long base = static_cast<long>(batch) * p.up_h * p.up_w;
+      u00 = (base + static_cast<long>(y0) * p.up_w + x0) * p.up_ld;
+      u01 = (base + static_cast<long>(y0) * p.up_w + x1) * p.up_ld;
+      u10 = (base + static_cast<long>(y1) * p.up_w + x0) * p.up_ld;
+      u11 = (base + static_cast<long>(y1) * p.up_w + x1) * p.up_ld;
     }
     const int c_begin = epi_half() == 0 ? 0 : kChunksHalf0;
     const int c_end = epi_half() == 0 ? kChunksHalf0 : kChunks;
@@ -878,17 +790,11 @@ struct EpiConv {
 #pragma unroll
           for (int j = 0; j < 32; ++j) v[j] += r[j];
         }
-        if (kUpAny && p.up_hi) {
+        if (kUpsample && p.up_hi) {
           // the four bilinear neighbours: plain per-thread loads (two rounds of two neighbours)
           if (ok) {
-            // kUp: the staged window (box = column / 128 when the tile spans two boxes), else the global planes
             const __half* uh = p.up_hi + col;
             const __half* ul = p.up_lo + col;
-            if (kUp) {
-              const int box = kUpBoxes > 1 ? (c * 32) / 128 : 0;
-              uh = reinterpret_cast<const __half*>(s_up + box * kUpBoxBytes) + (c * 32 - box * 128);
-              ul = reinterpret_cast<const __half*>(s_up + kUpPlaneBytes + box * kUpBoxBytes) + (c * 32 - box * 128);
-            }
             float a[32], b[32];
             load_planes32(uh + u00, ul + u00, a);
             load_planes32(uh + u01, ul + u01, b);
@@ -913,11 +819,9 @@ struct EpiConv {
             const long o = pix * p.res_ld + col + j;
             v[j] += __half2float(p.res_hi[o]) + __half2float(p.res_lo[o]);
           }
-          if (kUpAny && p.up_hi) {
-            const int box = kUpBoxes > 1 ? (c * 32) / 128 : 0;
-            const __half* uh = kUp ? reinterpret_cast<const __half*>(s_up + box * kUpBoxBytes) + (c * 32 - box * 128) : p.up_hi + col;
-            const __half* ul = kUp ? reinterpret_cast<const __half*>(s_up + kUpPlaneBytes + box * kUpBoxBytes) + (c * 32 - box * 128)
-                                   : p.up_lo + col;
+          if (kUpsample && p.up_hi) {
+            const __half* uh = p.up_hi + col;
+            const __half* ul = p.up_lo + col;
             auto at = [&](long o) { return __half2float(uh[o + j]) + __half2float(ul[o + j]); };
             v[j] += wy0 * (wx0 * at(u00) + wx1 * at(u01)) + wy1 * (wx0 * at(u10) + wx1 * at(u11));
           }

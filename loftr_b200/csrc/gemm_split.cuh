@@ -27,13 +27,7 @@
 namespace lb {
 
 constexpr int kBlockM = 128;
-#ifndef LB_BLOCK_K
-#define LB_BLOCK_K 64
-#endif
-// k-block of one pipeline stage: 64 fp16 = one 128-byte swizzle row, or 32 fp16 = one 64-byte swizzle row (twice
-// as many, half as large stages in the same shared memory -> deeper TMA pipeline)
-constexpr int kBlockK = LB_BLOCK_K;
-static_assert(kBlockK == 64 || kBlockK == 32, "supported k-block sizes");
+constexpr int kBlockK = 64;   // k-block of one pipeline stage: 64 fp16 = one 128-byte swizzle row
 constexpr int kMmaK = 16;
 constexpr int kGemmThreads = 288;
 constexpr int kEpiThreads = 256;  // two epilogue warpgroups: rows x {left, right} half of the tile's columns
@@ -95,10 +89,8 @@ struct EpiRowBound<Epi, decltype(void(Epi::kNoRowBound))> {
   static constexpr bool value = !Epi::kNoRowBound;
 };
 
-// K-major operand tile descriptor for the configured k-block (128-byte or 64-byte swizzle rows).
-__device__ __forceinline__ uint64_t desc_k(uint32_t smem_addr) {
-  return kBlockK == 64 ? wgmma_desc_k_sw128(smem_addr) : wgmma_desc_k_sw64(smem_addr);
-}
+// K-major operand tile descriptor of a k-block (128-byte swizzle rows).
+__device__ __forceinline__ uint64_t desc_k(uint32_t smem_addr) { return wgmma_desc_k_sw128(smem_addr); }
 
 // Shared memory: [TMA ring | accumulator staging (aliased)][epilogue area][mbarriers].
 // The staging tile is 128 rows of BLOCK_N + 4 fp32: a row stride of an odd multiple of 16 bytes keeps the epilogue's
@@ -182,8 +174,8 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   constexpr int kTapBytes = S::kStageBytes / kRemTapsPerStage;   // one tap of a remainder group: A_hi A_lo B_hi B_lo
   constexpr int kRemATile = kBlockM * kRemChannels * 2;           // 4 KB
   constexpr int kRemBTile = S::kBTile / (kBlockK / kRemChannels);
-  static_assert(kBlockK != 64 || (kTapBytes == 2 * kRemATile + 2 * kRemBTile && kTapBytes % 256 == 0 &&
-                                  kRemBTile % 256 == 0), "remainder group layout");
+  static_assert(kTapBytes == 2 * kRemATile + 2 * kRemBTile && kTapBytes % 256 == 0 && kRemBTile % 256 == 0,
+                "remainder group layout");
   // m tiles per batch: all of them, or those that hold live rows.  The count is written by an earlier kernel of the
   // stream, so it is read only here, after griddepcontrol.wait; producer and consumers read the same value.
   int m_tiles = shape.m_tiles;
