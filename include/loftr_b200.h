@@ -6,6 +6,8 @@
  *
  *   lb_coarse_prep            <- PositionEncodingSine.forward + rearrange   src/loftr/utils/position_encoding.py:37-42,
  *                                                                           src/loftr/loftr.py:58-59
+ *                                (lb_coarse_prep_indexed / lb_fine_preprocess_indexed: the same stages reading the
+ *                                 backbone output of a per-image feature bank through a pair -> image index)
  *   lb_transformer_forward    <- LocalFeatureTransformer.forward            src/loftr/loftr_module/transformer.py:80-101
  *                                (LoFTREncoderLayer.forward :35-58, LinearAttention.forward linear_attention.py:20-47,
  *                                 FullAttention.forward :56-81 for the *_FULL layer kinds)
@@ -45,7 +47,8 @@ extern "C" {
 #define LB_LAYER_CROSS_FULL 3
 
 /* 101: device-count fields appended to LbTransformerState / LbFinePreprocessArgs / LbFineMatchArgs;
- * 102: full-attention layer kinds; 103: lb_selftest removed (no structure changes). */
+ * 102: full-attention layer kinds; 103: lb_selftest removed (no structure changes);
+ * 104: lb_coarse_prep_indexed / lb_fine_preprocess_indexed (pairs read from a per-image feature bank). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -81,6 +84,11 @@ int lb_gemm_split(const void* a_hi, const void* a_lo, long lda, long a_batch_str
  * -> x_f32 [n_img*h*w, C], cat planes [rows, 2C] cols [0,C). */
 int lb_coarse_prep(const float* feat, int nhwc, const float* pe, int n_img, int C, int h, int w, int pe_h, int pe_w,
                    float* x_f32, void* cat_hi, void* cat_lo, void* stream);
+/* lb_coarse_prep over a feature bank: `feat` holds the bank's images, output image b (of n_out) is bank image
+ * img_idx[b] (device int [n_out], every entry in [0, images in the bank); not checked on the device).  The same image
+ * may appear at several b. */
+int lb_coarse_prep_indexed(const float* feat, int nhwc, const float* pe, const int* img_idx, int n_out, int C, int h,
+                           int w, int pe_h, int pe_w, float* x_f32, void* cat_hi, void* cat_lo, void* stream);
 
 /* ResNetFPN_8_2 local-feature CNN on tensor cores (reference src/loftr/backbone/resnet_fpn.py:43-118; SURVEY.md
  * §8(f) rank 1).  One LbConvWeights per Conv2d(+BatchNorm2d in eval mode, folded to scale/shift; scale = 1,
@@ -229,6 +237,11 @@ typedef struct LbFinePreprocessArgs {
 
 size_t lb_fine_preprocess_workspace_bytes(long M, int W, int Cf);
 int lb_fine_preprocess(const LbFinePreprocessArgs* args /*host*/, void* ws, size_t ws_bytes, void* stream);
+/* lb_fine_preprocess with feat_f0 / feat_f1 holding feature banks: the windows of pair b (b_ids) are read from image
+ * img_idx0[b] of feat_f0 and image img_idx1[b] of feat_f1 (device ints [n_pairs], each in range of its bank; sn0 / sn1
+ * step from one bank image to the next).  feat_c stays pair-major.  Same workspace as lb_fine_preprocess. */
+int lb_fine_preprocess_indexed(const LbFinePreprocessArgs* args /*host*/, const int* img_idx0, const int* img_idx1,
+                               void* ws, size_t ws_bytes, void* stream);
 
 typedef struct LbFineMatchArgs {
   const float* f0;        /* [M*W*W, C] fine transformer output, window side 0 */

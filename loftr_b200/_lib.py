@@ -111,6 +111,8 @@ SIGNATURES = {
                               c_long, c_long, c_int, c_int, c_int, c_int, c_void_p]),
     "lb_coarse_prep": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                c_void_p, c_void_p, c_void_p]),
+    "lb_coarse_prep_indexed": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
+                                       c_void_p, c_void_p, c_void_p, c_void_p]),
     "lb_backbone_workspace_bytes": (c_size_t, [C.POINTER(LbBackboneWeights), c_int, c_int, c_int]),
     "lb_backbone_forward": (c_int, [C.POINTER(LbBackboneWeights), c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                                     c_void_p, c_size_t, c_void_p]),
@@ -121,6 +123,8 @@ SIGNATURES = {
     "lb_coarse_match": (c_int, [C.POINTER(LbCoarseMatchArgs), c_void_p, c_size_t, c_void_p]),
     "lb_fine_preprocess_workspace_bytes": (c_size_t, [c_long, c_int, c_int]),
     "lb_fine_preprocess": (c_int, [C.POINTER(LbFinePreprocessArgs), c_void_p, c_size_t, c_void_p]),
+    "lb_fine_preprocess_indexed": (c_int, [C.POINTER(LbFinePreprocessArgs), c_void_p, c_void_p, c_void_p, c_size_t,
+                                           c_void_p]),
     "lb_fine_match": (c_int, [C.POINTER(LbFineMatchArgs), c_void_p]),
     "lb_epipolar_errors": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_void_p]),
@@ -139,6 +143,9 @@ NCCL_UNIQUE_ID_BYTES = 128
 MIN_VERSION = 101
 # oldest library that runs full (softmax) attention layers (LAYER_SELF_FULL / LAYER_CROSS_FULL); older ones reject them
 FULL_ATTENTION_VERSION = 102
+# oldest library with the feature-bank entry points (lb_*_indexed); `load()` leaves them unbound on an older one
+FEATURE_BANK_VERSION = 104
+_SINCE = {"lb_coarse_prep_indexed": FEATURE_BANK_VERSION, "lb_fine_preprocess_indexed": FEATURE_BANK_VERSION}
 
 
 class LibraryMissing(RuntimeError):
@@ -163,6 +170,8 @@ def load():
         raise LibraryMissing(f"{LIB_PATH} is version {lib.lb_version()}, older than the binding ({MIN_VERSION}): "
                              "rebuild it with `make`")
     for name, (res, args) in SIGNATURES.items():
+        if lib.lb_version() < _SINCE.get(name, 0):
+            continue             # not in this older build; the require_* checks stop its callers
         fn = getattr(lib, name)  # AttributeError if the library does not export a declared symbol
         fn.restype = res
         fn.argtypes = args
@@ -175,6 +184,14 @@ def require_full_attention(lib):
     v = lib.lb_version()
     if v < FULL_ATTENTION_VERSION:
         raise RuntimeError(f"loftr_b200: full attention needs library version {FULL_ATTENTION_VERSION} or newer, but "
+                           f"{LIB_PATH} is version {v}: rebuild it with `make`")
+
+
+def require_feature_bank(lib):
+    """Raise unless `lib` has the indexed entry points of LoFTR.match_features (version >= FEATURE_BANK_VERSION)."""
+    v = lib.lb_version()
+    if v < FEATURE_BANK_VERSION:
+        raise RuntimeError(f"loftr_b200: match_features needs library version {FEATURE_BANK_VERSION} or newer, but "
                            f"{LIB_PATH} is version {v}: rebuild it with `make`")
 
 

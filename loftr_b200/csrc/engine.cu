@@ -847,7 +847,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
 
 extern "C" {
 
-int lb_version(void) { return 103; }
+int lb_version(void) { return 104; }
 int lb_block_k(void) { return kBlockK; }
 int lb_conv_layout(int cin, int* cin_blocks, int* rem_channels) {
   if (!cin_blocks || !rem_channels || cin <= 0) return fail("lb_conv_layout: bad arguments");
@@ -925,19 +925,34 @@ int lb_gemm_split(const void* a_hi, const void* a_lo, long lda, long a_batch_str
   return launch_gemm<128, Epi>(TAG_GEMM_TEST, A, B, batches, M, N, K, 0, ep, st);
 }
 
-int lb_coarse_prep(const float* feat, int nhwc, const float* pe, int n_img, int C, int h, int w, int pe_h, int pe_w,
-                   float* x_f32, void* cat_hi, void* cat_lo, void* stream) {
+// n_out output images; with img_idx, output image b reads image img_idx[b] of feat
+static int coarse_prep(const float* feat, int nhwc, const float* pe, const int* img_idx, int n_out, int C, int h,
+                       int w, int pe_h, int pe_w, float* x_f32, void* cat_hi, void* cat_lo, void* stream) {
   int sms;
-  if (n_img <= 0) return 0;
+  if (n_out <= 0) return 0;
   DeviceGuard dev_guard;
   LB_TRY(dev_guard.bind(x_f32));
   LB_TRY(device_check(&sms));
   if (h > pe_h || w > pe_w) return fail("feature map %dx%d exceeds the position-encoding table %dx%d", h, w, pe_h, pe_w);
-  dim3 grid(cdiv(static_cast<long>(h) * w, 32), cdiv(C, 32), n_img);
-  coarse_prep_kernel<<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
-      feat, nhwc, pe, C, h, w, pe_h, pe_w, x_f32, static_cast<__half*>(cat_hi), static_cast<__half*>(cat_lo));
+  dim3 grid(cdiv(static_cast<long>(h) * w, 32), cdiv(C, 32), n_out);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  __half* hi = static_cast<__half*>(cat_hi);
+  __half* lo = static_cast<__half*>(cat_lo);
+  if (img_idx) coarse_prep_kernel<true><<<grid, dim3(32, 8), 0, st>>>(feat, nhwc, pe, C, h, w, pe_h, pe_w, x_f32, hi, lo, img_idx);
+  else coarse_prep_kernel<false><<<grid, dim3(32, 8), 0, st>>>(feat, nhwc, pe, C, h, w, pe_h, pe_w, x_f32, hi, lo, nullptr);
   LB_LAUNCHED();
   return 0;
+}
+
+int lb_coarse_prep(const float* feat, int nhwc, const float* pe, int n_img, int C, int h, int w, int pe_h, int pe_w,
+                   float* x_f32, void* cat_hi, void* cat_lo, void* stream) {
+  return coarse_prep(feat, nhwc, pe, nullptr, n_img, C, h, w, pe_h, pe_w, x_f32, cat_hi, cat_lo, stream);
+}
+
+int lb_coarse_prep_indexed(const float* feat, int nhwc, const float* pe, const int* img_idx, int n_out, int C, int h,
+                           int w, int pe_h, int pe_w, float* x_f32, void* cat_hi, void* cat_lo, void* stream) {
+  if (n_out > 0 && !img_idx) return fail("lb_coarse_prep_indexed: img_idx is null");
+  return coarse_prep(feat, nhwc, pe, img_idx, n_out, C, h, w, pe_h, pe_w, x_f32, cat_hi, cat_lo, stream);
 }
 
 size_t lb_transformer_workspace_bytes(int d_model, int nhead, int n_groups, int group_rows0, int group_rows1) {
@@ -1330,7 +1345,9 @@ size_t lb_fine_preprocess_workspace_bytes(long M, int W, int Cf) {
   return b.off + 256;
 }
 
-int lb_fine_preprocess(const LbFinePreprocessArgs* a, void* ws, size_t ws_bytes, void* stream) {
+// img_idx0 / img_idx1: NULL, or pair b's windows are read from image img_idx0[b] of feat_f0 / img_idx1[b] of feat_f1
+static int fine_preprocess(const LbFinePreprocessArgs* a, const int* img_idx0, const int* img_idx1, void* ws,
+                           size_t ws_bytes, void* stream) {
   int sms;
   if (a->M <= 0) return 0;
   DeviceGuard dev_guard;
@@ -1356,11 +1373,18 @@ int lb_fine_preprocess(const LbFinePreprocessArgs* a, void* ws, size_t ws_bytes,
   g.b_ids = a->b_ids; g.i_ids = a->i_ids; g.j_ids = a->j_ids;
   g.out_hi = win_hi; g.out_lo = win_lo; g.ld = a->Cf;
   g.live = a->M_live;
+  g.img_idx0 = img_idx0; g.img_idx1 = img_idx1;
   const bool vec8 = a->sc0 == 1 && a->sc1 == 1 && a->Cf % 8 == 0 && g.ld % 8 == 0 && a->sw0 % 4 == 0 && a->sw1 % 4 == 0 &&
                     a->sh0 % 4 == 0 && a->sh1 % 4 == 0 && a->sn0 % 4 == 0 && a->sn1 % 4 == 0 &&
                     (reinterpret_cast<uintptr_t>(a->feat_f0) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->feat_f1) & 15) == 0;
-  if (vec8) fine_gather_vec8_kernel<<<static_cast<unsigned>(2 * a->M), 256, 0, st>>>(g);
-  else fine_gather_kernel<<<static_cast<unsigned>(2 * a->M), 256, 0, st>>>(g);
+  const unsigned wins = static_cast<unsigned>(2 * a->M);
+  if (img_idx0) {
+    if (vec8) fine_gather_vec8_kernel<true><<<wins, 256, 0, st>>>(g);
+    else fine_gather_kernel<true><<<wins, 256, 0, st>>>(g);
+  } else {
+    if (vec8) fine_gather_vec8_kernel<false><<<wins, 256, 0, st>>>(g);
+    else fine_gather_kernel<false><<<wins, 256, 0, st>>>(g);
+  }
   LB_LAUNCHED();
 
   FineBiasParams fb;
@@ -1384,6 +1408,16 @@ int lb_fine_preprocess(const LbFinePreprocessArgs* a, void* ws, size_t ws_bytes,
   Epi::Params ep{0, gbias, WW, a->merge_acc_scale, {}};
   LB_TRY(fill_out_maps(&ep.om, a->cat_hi, a->cat_lo, 2 * a->Cf, a->x_f32, a->Cf, a->Cf, rows_b, nb));
   return launch_gemm<128, Epi>(TAG_FINE_MERGE, A, B, nb, static_cast<int>(rows_b), a->Cf, a->Cf, 0, ep, st, a->M_live, WW);
+}
+
+int lb_fine_preprocess(const LbFinePreprocessArgs* a, void* ws, size_t ws_bytes, void* stream) {
+  return fine_preprocess(a, nullptr, nullptr, ws, ws_bytes, stream);
+}
+
+int lb_fine_preprocess_indexed(const LbFinePreprocessArgs* a, const int* img_idx0, const int* img_idx1, void* ws,
+                               size_t ws_bytes, void* stream) {
+  if (a->M > 0 && (!img_idx0 || !img_idx1)) return fail("lb_fine_preprocess_indexed: img_idx0 and img_idx1 are required");
+  return fine_preprocess(a, img_idx0, img_idx1, ws, ws_bytes, stream);
 }
 
 int lb_fine_match(const LbFineMatchArgs* a, void* stream) {

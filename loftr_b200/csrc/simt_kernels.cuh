@@ -34,13 +34,18 @@ __global__ void split_planes_kernel(const float* __restrict__ x, long rows, int 
 // -> token-major x_f32 [n_img*h*w, C] and fp16 planes in columns [0, C) of the [rows, 2C] cat buffer.
 // = PositionEncodingSine.forward + rearrange 'n c h w -> n (h w) c' (reference loftr.py:58-59,
 // position_encoding.py:37-42).  32x32 smem transpose so both sides are coalesced.
+// kIndexed: output image `img` reads source image img_idx[img] of `feat` (a per-image feature bank shared by several
+// pairs); otherwise it reads image `img` and img_idx is unused.
+template <bool kIndexed>
 __global__ void coarse_prep_kernel(const float* __restrict__ feat, int nhwc, const float* __restrict__ pe, int C,
                                    int h, int w, int pe_h, int pe_w, float* __restrict__ x_f32,
-                                   __half* __restrict__ cat_hi, __half* __restrict__ cat_lo) {
+                                   __half* __restrict__ cat_hi, __half* __restrict__ cat_lo,
+                                   const int* __restrict__ img_idx) {
   pdl_trigger();
   __shared__ float tile[32][33];
   const int L = h * w;
   const int img = blockIdx.z;
+  const long src = kIndexed ? img_idx[img] : 0;   // source image (indexed variant)
   const int l0 = blockIdx.x * 32;
   const int c0 = blockIdx.y * 32;
   // read: threadIdx.x along l (contiguous in the channel-major sources), threadIdx.y along c
@@ -51,7 +56,7 @@ __global__ void coarse_prep_kernel(const float* __restrict__ feat, int nhwc, con
     if (c < C && l < L) {
       const int y = l / w, x = l - y * w;
       v = pe[(static_cast<long>(c) * pe_h + y) * pe_w + x];
-      if (!nhwc) v += feat[(static_cast<long>(img) * C + c) * L + l];
+      if (!nhwc) v += feat[((kIndexed ? src : static_cast<long>(img)) * C + c) * L + l];
     }
     tile[cy][threadIdx.x] = v;
   }
@@ -63,7 +68,7 @@ __global__ void coarse_prep_kernel(const float* __restrict__ feat, int nhwc, con
     if (c < C && l < L) {
       const long row = static_cast<long>(img) * L + l;
       float v = tile[threadIdx.x][ly];
-      if (nhwc) v = feat[row * C + c] + v;
+      if (nhwc) v = feat[(kIndexed ? src * L + l : row) * C + c] + v;
       x_f32[row * C + c] = v;
       __half hh, ll;
       split_f16(v, hh, ll);
@@ -743,14 +748,22 @@ struct FineGatherParams {
   __half* out_lo;
   int ld;
   const int* live;  // optional device count: windows m >= min(*live, M) of each side are skipped (M = capacity)
+  const int* img_idx0;  // kIndexed: pair b reads image img_idx0[b] of feat0 / img_idx1[b] of feat1
+  const int* img_idx1;
 };
+// Image of `feat0` / `feat1` that pair b's side-`side` windows are read from.
+template <bool kIndexed>
+__device__ __forceinline__ int fine_gather_image(const FineGatherParams& p, int side, int b) {
+  return kIndexed ? (side ? p.img_idx1 : p.img_idx0)[b] : b;
+}
+template <bool kIndexed>
 __global__ void fine_gather_kernel(const FineGatherParams p) {
   const int WW = p.W * p.W;
   const long win = blockIdx.x;             // 0 .. 2M-1
   const int side = win >= p.M ? 1 : 0;
   const long m = side ? win - p.M : win;
   if (p.live != nullptr && m >= *p.live) return;
-  const int b = static_cast<int>(p.b_ids[m]);
+  const int img = fine_gather_image<kIndexed>(p, side, static_cast<int>(p.b_ids[m]));
   const int idx = static_cast<int>(side ? p.j_ids[m] : p.i_ids[m]);
   const int wc = side ? p.w1c : p.w0c;
   const int cy = idx / wc, cx = idx - cy * wc;
@@ -764,7 +777,7 @@ __global__ void fine_gather_kernel(const FineGatherParams p) {
     const int y = p.stride * cy - p.W / 2 + ky;
     const int x = p.stride * cx - p.W / 2 + kx;
     float v = 0.f;
-    if (y >= 0 && y < Hf && x >= 0 && x < Wf) v = feat[b * sn + c * sc + y * sh + x * sw];
+    if (y >= 0 && y < Hf && x >= 0 && x < Wf) v = feat[img * sn + c * sc + y * sh + x * sw];
     __half hh, ll;
     split_f16(v, hh, ll);
     const long row = win * WW + k;
@@ -775,6 +788,7 @@ __global__ void fine_gather_kernel(const FineGatherParams p) {
 
 // Channel-contiguous (NHWC, sc == 1) maps with Cf % 8 == 0: one thread moves 8 channels of one window position --
 // two 16-byte loads, packed split, one 16-byte store per plane (the element-wise kernel above issues 2-byte stores).
+template <bool kIndexed>
 __global__ void __launch_bounds__(256) fine_gather_vec8_kernel(const FineGatherParams p) {
   const int WW = p.W * p.W;
   const int c8n = p.Cf >> 3;
@@ -782,7 +796,7 @@ __global__ void __launch_bounds__(256) fine_gather_vec8_kernel(const FineGatherP
   const int side = win >= p.M ? 1 : 0;
   const long m = side ? win - p.M : win;
   if (p.live != nullptr && m >= *p.live) return;
-  const int b = static_cast<int>(p.b_ids[m]);
+  const int img = fine_gather_image<kIndexed>(p, side, static_cast<int>(p.b_ids[m]));
   const int idx = static_cast<int>(side ? p.j_ids[m] : p.i_ids[m]);
   const int wc = side ? p.w1c : p.w0c;
   const int cy = idx / wc, cx = idx - cy * wc;
@@ -796,7 +810,7 @@ __global__ void __launch_bounds__(256) fine_gather_vec8_kernel(const FineGatherP
     const int x = p.stride * cx - p.W / 2 + kx;
     float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
     if (y >= 0 && y < Hf && x >= 0 && x < Wf) {
-      const float4* src = reinterpret_cast<const float4*>(feat + b * sn + y * sh + x * sw + c);
+      const float4* src = reinterpret_cast<const float4*>(feat + img * sn + y * sh + x * sw + c);
       v0 = src[0];
       v1 = src[1];
     }

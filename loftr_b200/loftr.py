@@ -509,10 +509,12 @@ class FinePreprocess(_PackedCacheMixin, nn.Module):
             self._packed_key = key
         return self._packed
 
-    def run(self, feat_f0, feat_f1, feat_c_all, n, L, S, data, live=None):
+    def run(self, feat_f0, feat_f1, feat_c_all, n, L, S, data, live=None, img_idx=None):
         """-> _TokenState of the fine transformer (rows: side, match, window position), or None if M == 0.
         `live`: int32 device count; the match keys of `data` are then capacity buffers and only windows below the
-        count are gathered (rows keep the capacity layout side*cap*WW + m*WW + k)."""
+        count are gathered (rows keep the capacity layout side*cap*WW + m*WW + k).
+        `img_idx`: (idx0, idx1) int32 device tensors [n]: feat_f0 / feat_f1 are then feature banks and pair b's
+        windows are read from their images idx0[b] / idx1[b]."""
         lib = _lib.load()
         W = self.W
         stride = data["hw0_f"][0] // data["hw0_c"][0]
@@ -541,7 +543,11 @@ class FinePreprocess(_PackedCacheMixin, nn.Module):
         a.M_live = _lib.ptr(live)
         nbytes = lib.lb_fine_preprocess_workspace_bytes(m, W, cf)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        _lib.check(lib.lb_fine_preprocess(C.byref(a), ws.data_ptr(), nbytes, _stream(feat_f0)))
+        if img_idx is None:
+            _lib.check(lib.lb_fine_preprocess(C.byref(a), ws.data_ptr(), nbytes, _stream(feat_f0)))
+        else:
+            _lib.check(lib.lb_fine_preprocess_indexed(C.byref(a), img_idx[0].data_ptr(), img_idx[1].data_ptr(),
+                                                      ws.data_ptr(), nbytes, _stream(feat_f0)))
         return state
 
     @torch.no_grad()
@@ -646,27 +652,127 @@ class LoFTR(nn.Module):
         if self.training:
             raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
         _require_cuda(data["image0"], "image0")
-        state, feat_f0, feat_f1, bs, L, S, c, m0, m1 = self._coarse_features(data)
-        img0 = data["image0"]
+        self._match_and_refine(data, *self._coarse_features(data))
 
+    def _match_and_refine(self, data, state, feat_f0, feat_f1, bs, L, S, c, m0, m1, img_idx=None):
+        """Steps 3-5 of the forward over the coarse token state.  `img_idx` (int32 idx0, idx1): feat_f0 / feat_f1 are
+        feature banks, read at image idx0[b] / idx1[b] for pair b."""
         # 3. coarse matching                                                           [loftr.py:67]
         self.coarse_matching.run(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1)
 
         # 4. fine-level refinement                                                     [loftr.py:70-72]
-        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, bs, L, S, data)
+        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, bs, L, S, data, img_idx=img_idx)
         ww = self.fine_preprocess.W ** 2
         if fstate is not None:
             m = fstate.rows0 // ww
             self.loftr_fine.run(fstate, m, ww, ww)
             f0u, f1u = fstate.x[: m * ww].view(m, ww, -1), fstate.x[m * ww:].view(m, ww, -1)
         else:
-            f0u = torch.empty(0, ww, self.fine_preprocess.d_model_f, device=img0.device)
+            f0u = torch.empty(0, ww, self.fine_preprocess.d_model_f, device=feat_f0.device)
             f1u = f0u.clone()
 
         # 5. fine matching                                                             [loftr.py:75]
         self.fine_matching(f0u, f1u, data)
         if self.expose_coarse_features:   # test / debugging tap, off by default: not a reference key
             data["_feat_c0"], data["_feat_c1"] = state.x[: bs * L].view(bs, L, c), state.x[bs * L:].view(bs, S, c)
+
+    @torch.no_grad()
+    def extract_features(self, images, masks=None) -> "ImageFeatures":
+        """Runs the configured backbone once on images [K, 1, H, W] (CUDA) -> ImageFeatures, a per-image feature bank
+        for `match_features`.  masks: optional [K, H/8, W/8] padding masks (as forward's mask0 / mask1), stored with
+        the bank.  Position encoding and the transformers are not applied: they depend on the pair."""
+        if self.training:
+            raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
+        _require_cuda(images, "images")
+        if images.dim() != 4 or images.shape[1] != 1:
+            raise ValueError(f"extract_features: images must be [K, 1, H, W] (got {tuple(images.shape)})")
+        if images.shape[0] == 0:
+            raise ValueError("extract_features: no images (a feature bank holds at least one)")
+        key = self._bank_key()
+        feat_c, feat_f = self._backbone(images)
+        if masks is not None:
+            if tuple(masks.shape) != (images.shape[0], *feat_c.shape[2:]):
+                raise ValueError(f"extract_features: masks must be [K, H/8, W/8] = {(images.shape[0], *feat_c.shape[2:])} "
+                                 f"(got {tuple(masks.shape)})")
+            masks = masks.to(images.device)
+        return ImageFeatures(feat_c, feat_f, masks, images.shape[2:], feat_c.shape[2:], feat_f.shape[2:], key)
+
+    @torch.no_grad()
+    def match_features(self, feats0, idx0, feats1, idx1, scale0=None, scale1=None, data=None):
+        """Matches pair b = (image idx0[b] of feats0, image idx1[b] of feats1) for every b of the pair list, from banks
+        made by `extract_features` (feats1 may be feats0).  Writes into `data` (a new dict when None) and returns it:
+        the keys, dtypes and values `forward` writes for the batch image0 = images idx0 of feats0, image1 = images
+        idx1 of feats1, with the banks' masks and the scales gathered the same way.  `m_bids` indexes the pair list.
+
+        idx0, idx1: int32 / int64 tensors [B] on the model's device, each index within its bank.  An empty list gives
+        the outputs of a forward with no matches.  scale0 / scale1: optional [K0, 2] / [K1, 2] per-image scales of
+        feats0 / feats1 (both or neither).  A bank is tied to the backbone weights it was extracted with: after
+        load_state_dict, .to() or a parameter update it raises; extract again."""
+        if self.training:
+            raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
+        _lib.require_feature_bank(_lib.load())
+        key = self._bank_key()
+        dev = next(self.parameters()).device
+        for name, f in (("feats0", feats0), ("feats1", feats1)):
+            if not isinstance(f, ImageFeatures):
+                raise TypeError(f"match_features: `{name}` must be the ImageFeatures of extract_features")
+            if f.weights_key != key:
+                raise RuntimeError(f"match_features: `{name}` was extracted with other backbone weights (load_state_dict, "
+                                   ".to() or a parameter update since); extract the features again")
+        idx0 = self._pair_index(idx0, "idx0", len(feats0), dev)
+        idx1 = self._pair_index(idx1, "idx1", len(feats1), dev)
+        if idx0.shape != idx1.shape:
+            raise ValueError(f"match_features: idx0 and idx1 must have the same length ({idx0.numel()} vs {idx1.numel()})")
+        if (feats0.mask is None) != (feats1.mask is None):
+            raise ValueError("match_features: either both banks carry masks or neither (as mask0 / mask1 of forward)")
+        if (scale0 is None) != (scale1 is None):
+            raise ValueError("match_features: give scale0 and scale1 together")
+        bs = idx0.numel()
+        work = {}   # forward's inputs for this pair list (masks, scales), then every key forward writes
+        if feats0.mask is not None:
+            work["mask0"], work["mask1"] = feats0.mask[idx0.long()], feats1.mask[idx1.long()]
+        if scale0 is not None:
+            for name, s, f, idx in (("scale0", scale0, feats0, idx0), ("scale1", scale1, feats1, idx1)):
+                if tuple(s.shape) != (len(f), 2):
+                    raise ValueError(f"match_features: {name} must be [{len(f)}, 2] (got {tuple(s.shape)})")
+                work[name] = s.to(dev)[idx.long()]
+        work.update({"bs": bs, "hw0_i": feats0.hw_i, "hw1_i": feats1.hw_i, "hw0_c": feats0.hw_c, "hw1_c": feats1.hw_c,
+                     "hw0_f": feats0.hw_f, "hw1_f": feats1.hw_f})
+        state, L, S, c, m0, m1 = self._coarse_transformer(work, feats0.feat_c, feats1.feat_c, bs, idx0, idx1)
+        self._match_and_refine(work, state, feats0.feat_f, feats1.feat_f, bs, L, S, c, m0, m1, img_idx=(idx0, idx1))
+        out = {} if data is None else data
+        out.update({k: v for k, v in work.items() if k not in ("mask0", "mask1", "scale0", "scale1")})
+        return out
+
+    @staticmethod
+    def _pair_index(idx, name, n_images, dev):
+        """Validated pair -> bank image index as a contiguous int32 tensor on `dev` (one host sync for the range)."""
+        if not torch.is_tensor(idx) or idx.dtype not in (torch.int32, torch.int64):
+            raise TypeError(f"match_features: `{name}` must be an int32 or int64 tensor (got "
+                            f"{idx.dtype if torch.is_tensor(idx) else type(idx).__name__})")
+        if idx.device != dev:
+            raise ValueError(f"match_features: `{name}` is on {idx.device}, the model on {dev}")
+        if idx.dim() != 1:
+            raise ValueError(f"match_features: `{name}` must be one-dimensional (got shape {tuple(idx.shape)})")
+        if idx.numel():
+            lo, hi = torch.stack([idx.min(), idx.max()]).tolist()
+            if lo < 0 or hi >= n_images:
+                raise IndexError(f"match_features: `{name}` holds indices in [{lo}, {hi}], outside the bank's "
+                                 f"[0, {n_images})")
+        return idx.to(torch.int32).contiguous()
+
+    def _bank_key(self):
+        """What a feature bank depends on: the backbone implementation and its tensors' (data_ptr, _version)."""
+        tensors = list(self.backbone.parameters()) + list(self.backbone.buffers())
+        return (self.backbone_impl,) + _tensor_key(tensors)
+
+    def _backbone(self, images):
+        """The configured backbone on [N, 1, H, W] -> (feat_c, feat_f) as [N, C, h, w]; NHWC storage (channels-last
+        strides) from the tensor-core backbone, NCHW from the PyTorch one."""
+        if self._tc_backbone is not None:
+            fc, ff = self._tc_backbone(images)
+            return fc.permute(0, 3, 1, 2), ff.permute(0, 3, 1, 2)
+        return self.backbone(images)
 
     @torch.no_grad()
     def forward_static(self, data, capacity=None):
@@ -724,41 +830,44 @@ class LoFTR(nn.Module):
         """Steps 1-2 of the forward (no host sync): backbone, position encoding and coarse transformer.
         -> (coarse token state, feat_f0, feat_f1, n, L, S, C, mask0 u8, mask1 u8)."""
         img0, img1 = data["image0"], data["image1"]
-        lib = _lib.load()
         bs = img0.size(0)
         data.update({"bs": bs, "hw0_i": img0.shape[2:], "hw1_i": img1.shape[2:]})
 
         # 1. local feature CNN                                                         [loftr.py:45-49]
-        nhwc = self._tc_backbone is not None
-        if nhwc:   # NHWC outputs; viewed as [N, C, H, W] tensors with channels-last strides
-            if data["hw0_i"] == data["hw1_i"]:
-                fc, ff = self._tc_backbone(torch.cat([img0, img1], dim=0))
-                (feat_c0, feat_c1), (feat_f0, feat_f1) = fc.split(bs), ff.split(bs)
-            else:
-                (feat_c0, feat_f0), (feat_c1, feat_f1) = self._tc_backbone(img0), self._tc_backbone(img1)
-            feat_c0, feat_c1, feat_f0, feat_f1 = (t.permute(0, 3, 1, 2) for t in (feat_c0, feat_c1, feat_f0, feat_f1))
-        elif data["hw0_i"] == data["hw1_i"]:
-            feats_c, feats_f = self.backbone(torch.cat([img0, img1], dim=0))
+        if data["hw0_i"] == data["hw1_i"]:
+            feats_c, feats_f = self._backbone(torch.cat([img0, img1], dim=0))
             (feat_c0, feat_c1), (feat_f0, feat_f1) = feats_c.split(bs), feats_f.split(bs)
         else:
-            (feat_c0, feat_f0), (feat_c1, feat_f1) = self.backbone(img0), self.backbone(img1)
+            (feat_c0, feat_f0), (feat_c1, feat_f1) = self._backbone(img0), self._backbone(img1)
         data.update({"hw0_c": feat_c0.shape[2:], "hw1_c": feat_c1.shape[2:],
                      "hw0_f": feat_f0.shape[2:], "hw1_f": feat_f1.shape[2:]})
+        state, L, S, c, m0, m1 = self._coarse_transformer(data, feat_c0, feat_c1, bs)
+        return state, feat_f0, feat_f1, bs, L, S, c, m0, m1
 
+    def _coarse_transformer(self, data, feat_c0, feat_c1, bs, idx0=None, idx1=None):
+        """Step 2 of the forward (no host sync): position encoding, token layout and coarse transformer of `bs` pairs.
+        idx0 / idx1 (int32 [bs], both or neither): feat_c0 / feat_c1 are feature banks, read at image idx0[b] /
+        idx1[b] for pair b.  -> (coarse token state, L, S, C, mask0 u8, mask1 u8)."""
         # 2. position encoding + token layout + coarse transformer                     [loftr.py:58-64]
+        lib = _lib.load()
+        nhwc = self._tc_backbone is not None
         c = feat_c0.shape[1]
         (h0, w0), (h1, w1) = data["hw0_c"], data["hw1_c"]
         L, S = h0 * w0, h1 * w1
-        state = _TokenState(bs * L, bs * S, c, img0.device)
+        state = _TokenState(bs * L, bs * S, c, feat_c0.device)
         pe = self.pos_encoding.pe[0]
-        st = _stream(img0)
-        for feat, h, w, row0 in ((feat_c0, h0, w0, 0), (feat_c1, h1, w1, bs * L)):
+        st = _stream(feat_c0)
+        for feat, idx, h, w, row0 in ((feat_c0, idx0, h0, w0, 0), (feat_c1, idx1, h1, w1, bs * L)):
             feat = feat.float()
             feat = feat.permute(0, 2, 3, 1).contiguous() if nhwc else feat.contiguous()   # no copy in either case
-            _lib.check(lib.lb_coarse_prep(feat.data_ptr(), int(nhwc), pe.data_ptr(), bs, c, h, w, pe.shape[1], pe.shape[2],
-                                          state.x.data_ptr() + row0 * c * 4,
-                                          state.cat_hi.data_ptr() + row0 * 2 * c * 2,
-                                          state.cat_lo.data_ptr() + row0 * 2 * c * 2, st))
+            out = (state.x.data_ptr() + row0 * c * 4, state.cat_hi.data_ptr() + row0 * 2 * c * 2,
+                   state.cat_lo.data_ptr() + row0 * 2 * c * 2, st)
+            if idx is None:
+                _lib.check(lib.lb_coarse_prep(feat.data_ptr(), int(nhwc), pe.data_ptr(), bs, c, h, w, pe.shape[1],
+                                              pe.shape[2], *out))
+            else:
+                _lib.check(lib.lb_coarse_prep_indexed(feat.data_ptr(), int(nhwc), pe.data_ptr(), idx.data_ptr(), bs, c,
+                                                      h, w, pe.shape[1], pe.shape[2], *out))
         mask_all = m0 = m1 = None
         if "mask0" in data:
             m0 = data["mask0"].flatten(-2).reshape(-1).to(torch.uint8)
@@ -766,7 +875,7 @@ class LoFTR(nn.Module):
             mask_all = torch.cat([m0, m1]).contiguous()
             m0, m1 = mask_all[: bs * L], mask_all[bs * L:]
         self.loftr_coarse.run(state, bs, L, S, mask_all)
-        return state, feat_f0, feat_f1, bs, L, S, c, m0, m1
+        return state, L, S, c, m0, m1
 
     def invalidate_packed(self):
         """Drop every packed-weight cache (fp16 hi/lo planes, folded BatchNorm): required after parameter writes
@@ -797,7 +906,31 @@ def _weight_refs(model):
     if model._tc_backbone is not None:
         caches.append(model._tc_backbone._packed)
     tensors = list(model.parameters()) + list(model.buffers())
-    return caches, tensors, tuple((t.data_ptr(), t._version) for t in tensors)
+    return caches, tensors, _tensor_key(tensors)
+
+
+def _tensor_key(tensors):
+    """(data_ptr, _version) of every tensor: changes when one is replaced, moved or modified in place (not through
+    `.data`)."""
+    return tuple((t.data_ptr(), t._version) for t in tensors)
+
+
+class ImageFeatures:
+    """Backbone output of K images of one size (`LoFTR.extract_features`), matched pair by pair with
+    `LoFTR.match_features` without running the backbone again.
+
+    feat_c [K, C_c, H/8, W/8] and feat_f [K, C_f, H/2, W/2] are the maps as the backbone emits them (NHWC storage,
+    i.e. channels-last strides, from the tensor-core backbone; NCHW from the PyTorch one); mask: optional padding
+    masks [K, H/8, W/8]; hw_i / hw_c / hw_f: image, coarse and fine sizes.  weights_key identifies the backbone weights the
+    bank was extracted with."""
+
+    def __init__(self, feat_c, feat_f, mask, hw_i, hw_c, hw_f, weights_key):
+        self.feat_c, self.feat_f, self.mask = feat_c, feat_f, mask
+        self.hw_i, self.hw_c, self.hw_f = hw_i, hw_c, hw_f
+        self.weights_key = weights_key
+
+    def __len__(self):
+        return self.feat_c.shape[0]
 
 
 class CapturedMatcher:
