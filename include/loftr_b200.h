@@ -48,7 +48,8 @@ extern "C" {
 
 /* 101: device-count fields appended to LbTransformerState / LbFinePreprocessArgs / LbFineMatchArgs;
  * 102: full-attention layer kinds; 103: lb_selftest removed (no structure changes);
- * 104: lb_coarse_prep_indexed / lb_fine_preprocess_indexed (pairs read from a per-image feature bank). */
+ * 104: lb_coarse_prep_indexed / lb_fine_preprocess_indexed (pairs read from a per-image feature bank);
+ * 105: lb_coarse_match_capped (at most k matches per pair, chosen by confidence). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -60,8 +61,8 @@ const char* lb_last_error(void);
 /* number of kernels this library has launched in this process (for bench.py's gpu_launches) */
 long long lb_launch_count(void);
 
-/* Optional per-launch CUDA-event timing of the tensor-core kernels (events recorded on the launching
- * stream around each kernel while enabled).  lb_timing_enable(1) clears old records and starts recording,
+/* Optional per-launch CUDA-event timing of the tensor-core kernels and of the per-pair match cap (events recorded on
+ * the launching stream around each kernel while enabled).  lb_timing_enable(1) clears old records and starts recording,
  * lb_timing_collect synchronises the recorded events and returns per-tag total milliseconds and launch counts
  * (arrays of lb_timing_num_tags() entries; names via lb_timing_tag_name).  Timed launches cannot be recorded into a
  * CUDA graph: while timing is enabled, a launch on a capturing stream fails. */
@@ -202,6 +203,12 @@ typedef struct LbCoarseMatchArgs {
 
 size_t lb_coarse_match_workspace_bytes(int n_pairs, int L, int S);
 int lb_coarse_match(const LbCoarseMatchArgs* args /*host*/, void* ws, size_t ws_bytes, void* stream);
+/* lb_coarse_match keeping at most max_per_pair (>= 1) matches per pair: the ones with the largest mconf, a tie at the
+ * max_per_pair-th value going to the smaller row index i.  Pairs with at most max_per_pair matches are unchanged; the
+ * outputs stay in ascending (b, i) order, and a capacity of n_pairs*max_per_pair always suffices.  conf_matrix is not
+ * affected.  One more launch than lb_coarse_match (timing tag "match_cap"); same workspace. */
+int lb_coarse_match_capped(const LbCoarseMatchArgs* args /*host*/, int max_per_pair, void* ws, size_t ws_bytes,
+                           void* stream);
 
 typedef struct LbFinePreprocessArgs {
   const float* feat_f0;   /* fine maps, any strides (elements): index = n*sn + c*sc + y*sh + x*sw */

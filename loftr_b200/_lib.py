@@ -121,6 +121,7 @@ SIGNATURES = {
                                        C.POINTER(LbTransformerState), c_void_p, c_size_t, c_void_p]),
     "lb_coarse_match_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "lb_coarse_match": (c_int, [C.POINTER(LbCoarseMatchArgs), c_void_p, c_size_t, c_void_p]),
+    "lb_coarse_match_capped": (c_int, [C.POINTER(LbCoarseMatchArgs), c_int, c_void_p, c_size_t, c_void_p]),
     "lb_fine_preprocess_workspace_bytes": (c_size_t, [c_long, c_int, c_int]),
     "lb_fine_preprocess": (c_int, [C.POINTER(LbFinePreprocessArgs), c_void_p, c_size_t, c_void_p]),
     "lb_fine_preprocess_indexed": (c_int, [C.POINTER(LbFinePreprocessArgs), c_void_p, c_void_p, c_void_p, c_size_t,
@@ -145,7 +146,10 @@ MIN_VERSION = 101
 FULL_ATTENTION_VERSION = 102
 # oldest library with the feature-bank entry points (lb_*_indexed); `load()` leaves them unbound on an older one
 FEATURE_BANK_VERSION = 104
-_SINCE = {"lb_coarse_prep_indexed": FEATURE_BANK_VERSION, "lb_fine_preprocess_indexed": FEATURE_BANK_VERSION}
+# oldest library with the per-pair match cap (lb_coarse_match_capped)
+MATCH_CAP_VERSION = 105
+_SINCE = {"lb_coarse_prep_indexed": FEATURE_BANK_VERSION, "lb_fine_preprocess_indexed": FEATURE_BANK_VERSION,
+          "lb_coarse_match_capped": MATCH_CAP_VERSION}
 
 
 class LibraryMissing(RuntimeError):
@@ -195,6 +199,14 @@ def require_feature_bank(lib):
                            f"{LIB_PATH} is version {v}: rebuild it with `make`")
 
 
+def require_match_cap(lib):
+    """Raise unless `lib` has lb_coarse_match_capped (match_coarse.max_matches_per_pair; version >= MATCH_CAP_VERSION)."""
+    v = lib.lb_version()
+    if v < MATCH_CAP_VERSION:
+        raise RuntimeError(f"loftr_b200: match_coarse.max_matches_per_pair needs library version {MATCH_CAP_VERSION} or "
+                           f"newer, but {LIB_PATH} is version {v}: rebuild it with `make`")
+
+
 def check(rc: int):
     if rc != 0:
         msg = load().lb_last_error()
@@ -211,7 +223,8 @@ def timing_enable(on: bool):
 
 
 def timing_collect() -> dict:
-    """-> {tag: (total_ms, launches)} for every tensor-core kernel tag recorded since timing_enable(True)."""
+    """-> {tag: (total_ms, launches)} for every kernel tag (tensor-core kernels, match cap) recorded since
+    timing_enable(True)."""
     lib = load()
     n = lib.lb_timing_num_tags()
     ms = (C.c_double * n)()

@@ -55,13 +55,13 @@ static int fail(const char* fmt, ...) {
   } while (0)
 
 // ------------------------------------------------------------------------------------------------ timing hook
-// Optional per-launch CUDA-event timing of the tensor-core kernels (bench.py's roofline leg): events are
-// recorded on the launching stream right around the kernel, and only while timing is enabled.
+// Optional per-launch CUDA-event timing of the tensor-core kernels (bench.py's roofline leg) and of the per-pair match
+// cap: events are recorded on the launching stream right around the kernel, and only while timing is enabled.
 enum Tag { TAG_GEMM_TEST = 0, TAG_PROJ, TAG_MERGE_LN, TAG_MLP1, TAG_MLP2_LN, TAG_SCORE_LSE, TAG_SCORE_ARGMAX,
-           TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_FULL_ATTN, TAG_COUNT };
+           TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_FULL_ATTN, TAG_MATCH_CAP, TAG_COUNT };
 static const char* kTagNames[TAG_COUNT] = {"gemm_test", "proj_act", "merge_ln", "mlp1_relu", "mlp2_ln_res",
                                            "score_lse", "score_argmax", "fine_merge", "backbone_conv",
-                                           "tf_kv_proj_fused", "tf_q_attn_fused", "tf_full_attn"};
+                                           "tf_kv_proj_fused", "tf_q_attn_fused", "tf_full_attn", "match_cap"};
 struct TimingRec {
   cudaEvent_t e0, e1;
   int tag;
@@ -847,7 +847,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
 
 extern "C" {
 
-int lb_version(void) { return 104; }
+int lb_version(void) { return 105; }
 int lb_block_k(void) { return kBlockK; }
 int lb_conv_layout(int cin, int* cin_blocks, int* rem_channels) {
   if (!cin_blocks || !rem_channels || cin <= 0) return fail("lb_conv_layout: bad arguments");
@@ -1146,7 +1146,8 @@ size_t lb_coarse_match_workspace_bytes(int n_pairs, int L, int S) {
   return b.off + 256;
 }
 
-int lb_coarse_match(const LbCoarseMatchArgs* a, void* ws, size_t ws_bytes, void* stream) {
+// max_per_pair: 0 = every match; otherwise each pair keeps its max_per_pair most confident matches (match_cap_kernel)
+static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, size_t ws_bytes, void* stream) {
   int sms;
   DeviceGuard dev_guard;
   LB_TRY(dev_guard.bind(a->count));
@@ -1319,6 +1320,13 @@ int lb_coarse_match(const LbCoarseMatchArgs* a, void* ws, size_t ws_bytes, void*
   sp.flag = w.flag; sp.conf = w.conf;
   match_flag_kernel<<<cdiv(nl, TB), TB, 0, st>>>(sp);
   LB_LAUNCHED();
+  if (max_per_pair > 0) {
+    TimingRec rec{nullptr, nullptr, TAG_MATCH_CAP};
+    LB_TRY(timing_begin(rec, st));
+    match_cap_kernel<<<n, kCapBlock, 0, st>>>(w.flag, w.conf, L, max_per_pair);
+    LB_LAUNCHED();
+    LB_TRY(timing_end(rec, st));
+  }
 
   CompactParams cp;
   cp.total = nl; cp.L = L; cp.S = S; cp.w0c = a->w0c; cp.w1c = a->w1c;
@@ -1333,6 +1341,15 @@ int lb_coarse_match(const LbCoarseMatchArgs* a, void* ws, size_t ws_bytes, void*
   match_scatter_kernel<<<cblocks, kCompactBlock, 0, st>>>(cp, w.blk_counts);
   LB_LAUNCHED();
   return 0;
+}
+
+int lb_coarse_match(const LbCoarseMatchArgs* a, void* ws, size_t ws_bytes, void* stream) {
+  return coarse_match(a, 0, ws, ws_bytes, stream);
+}
+
+int lb_coarse_match_capped(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, size_t ws_bytes, void* stream) {
+  if (max_per_pair < 1) return fail("lb_coarse_match_capped: max_per_pair must be at least 1 (got %d)", max_per_pair);
+  return coarse_match(a, max_per_pair, ws, ws_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ fine level

@@ -665,6 +665,94 @@ __global__ void __launch_bounds__(kCompactBlock) match_scatter_kernel(const Comp
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) *p.count = s_base + tot;
 }
 
+// Per-pair cap on the coarse matches (match_coarse.max_matches_per_pair), between the flag pass and the compaction.
+// One CTA per pair keeps the k flagged rows with the largest conf (ties at the k-th value: smaller row index first)
+// and clears the other flags in place.  conf >= 0 (an exp), so its fp32 bit pattern orders as an unsigned integer:
+// the k-th largest key is found by a radix select over 8-bit digits, most significant first, with a shared-memory
+// histogram of the flagged rows that share the digits selected so far.  Every pass re-reads flag / conf from global
+// memory (n*L*5 bytes, L2-resident), so there is no limit on L.  A pair with at most k matches exits after counting.
+constexpr int kCapBlock = 1024;
+__global__ void __launch_bounds__(kCapBlock) match_cap_kernel(uint8_t* __restrict__ flag,
+                                                              const float* __restrict__ conf, int L, int k) {
+  __shared__ int s_hist[256];
+  __shared__ int s_warp[kCapBlock / 32];
+  __shared__ unsigned s_prefix;
+  __shared__ int s_rem;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint8_t* f = flag + static_cast<long>(blockIdx.x) * L;
+  const float* c = conf + static_cast<long>(blockIdx.x) * L;
+
+  int cnt = 0;
+  for (int i = threadIdx.x; i < L; i += kCapBlock) cnt += f[i] ? 1 : 0;
+  for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if (lane == 0) s_warp[warp] = cnt;
+  __syncthreads();
+  int total = 0;
+  for (int w = 0; w < kCapBlock / 32; ++w) total += s_warp[w];
+  if (total <= k) return;
+
+  // invariant: the k-th largest key starts with the digits in `prefix` (bits above `shift + 8`), and is the rem-th
+  // largest of the flagged keys that start with them
+  unsigned prefix = 0;
+  int rem = k;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    const unsigned hi_mask = shift == 24 ? 0u : ~0u << (shift + 8);
+    if (threadIdx.x < 256) s_hist[threadIdx.x] = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < L; i += kCapBlock) {
+      if (f[i]) {
+        const unsigned key = __float_as_uint(c[i]);
+        if ((key & hi_mask) == prefix) atomicAdd(&s_hist[(key >> shift) & 0xffu], 1);
+      }
+    }
+    __syncthreads();
+    if (warp == 0) {   // lane l scans digits 255-8l down to 248-8l; `above` counts the keys of higher digits
+      const int d0 = 255 - 8 * lane;
+      int sum = 0;
+      for (int d = d0; d > d0 - 8; --d) sum += s_hist[d];
+      int above = sum;
+      for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(0xffffffffu, above, o);
+        if (lane >= o) above += v;
+      }
+      above -= sum;
+      for (int d = d0; d > d0 - 8; --d) {
+        const int h = s_hist[d];
+        if (above < rem && above + h >= rem) {   // exactly one digit of one lane satisfies this
+          s_prefix = prefix | (static_cast<unsigned>(d) << shift);
+          s_rem = rem - above;
+        }
+        above += h;
+      }
+    }
+    __syncthreads();
+    prefix = s_prefix;
+    rem = s_rem;
+  }
+
+  // prefix = the k-th largest key; rem = how many rows with exactly that key are kept, the first ones in row order
+  int ties_before = 0;
+  for (int i0 = 0; i0 < L; i0 += kCapBlock) {
+    const int i = i0 + threadIdx.x;
+    bool drop = false, tie = false;
+    if (i < L && f[i]) {
+      const unsigned key = __float_as_uint(c[i]);
+      drop = key < prefix;
+      tie = key == prefix;
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, tie);
+    if (lane == 0) s_warp[warp] = __popc(bal);
+    __syncthreads();
+    int rank = ties_before + __popc(bal & ((1u << lane) - 1));
+    for (int w = 0; w < kCapBlock / 32; ++w) {
+      if (w < warp) rank += s_warp[w];
+      ties_before += s_warp[w];
+    }
+    if (drop || (tie && rank >= rem)) f[i] = 0;
+    __syncthreads();   // s_warp is rewritten for the next chunk
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Sinkhorn helpers (log_optimal_transport, third_party/SuperGluePretrainedNetwork/models/superglue.py:
 // 141-170; called from coarse_matching.py:130-131).  The (L+1)x(S+1) couplings matrix is never

@@ -20,6 +20,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import numbers
 
 import torch
 import torch.nn as nn
@@ -351,11 +352,17 @@ class LocalFeatureTransformer(_PackedCacheMixin, nn.Module):
 
 class CoarseMatching(nn.Module):
     """Dual-softmax / Sinkhorn coarse matching with mutual-nearest selection
-    (reference coarse_matching.py:59-261, eval path)."""
+    (reference coarse_matching.py:59-261, eval path).
+
+    config["max_matches_per_pair"] (optional, not a reference key): None or absent keeps every match; an int k >= 1
+    keeps, within each pair, the k matches with the largest mconf (a tie at the k-th value goes to the smaller row
+    index i), selected on the device before the fine stage.  The list stays in ascending (b, i) order.  The attribute
+    `max_matches_per_pair` may be changed later; it is validated the same way."""
 
     def __init__(self, config):
         super().__init__()
         self.config = config
+        self.max_matches_per_pair = config.get("max_matches_per_pair")
         self.thr = config["thr"]
         self.border_rm = config["border_rm"]
         self.train_coarse_percent = config["train_coarse_percent"]
@@ -370,15 +377,29 @@ class CoarseMatching(nn.Module):
         else:
             raise NotImplementedError()
 
+    @property
+    def max_matches_per_pair(self):
+        return self._max_per_pair
+
+    @max_matches_per_pair.setter
+    def max_matches_per_pair(self, k):
+        if k is not None and (isinstance(k, bool) or not isinstance(k, numbers.Integral) or k < 1):
+            raise ValueError(f"match_coarse.max_matches_per_pair must be None or an int >= 1 (got {k!r})")
+        self._max_per_pair = None if k is None else int(k)
+
     @staticmethod
-    def default_capacity(n, L, S, masked):
+    def default_capacity(n, L, S, masked, max_per_pair=None):
         """Exact bound on the number of coarse matches: mutual nearest neighbours pair each row with at most one
-        column, so n*min(L, S) without masks (n*L with masks, as padding may leave columns unmatched)."""
-        return max(n * min(L, S) if not masked else n * L, 1)
+        column, so n*min(L, S) without masks (n*L with masks, as padding may leave columns unmatched); with a per-pair
+        cap k, n*min(k, that per-pair bound)."""
+        per_pair = min(L, S) if not masked else L
+        if max_per_pair is not None:
+            per_pair = min(per_pair, max_per_pair)
+        return max(n * per_pair, 1)
 
     def run(self, hi, lo, ld, n, L, S, c, data, mask_u8_0=None, mask_u8_1=None):
         """Planes of feat_c0 (rows [0, n*L)) / feat_c1 (rows [n*L, ...)) -> coarse match keys in `data`."""
-        cap = self.default_capacity(n, L, S, mask_u8_0 is not None)
+        cap = self.default_capacity(n, L, S, mask_u8_0 is not None, self.max_matches_per_pair)
         b_ids, i_ids, j_ids, mconf, mk0, mk1, count, conf = self._launch(hi, lo, ld, n, L, S, c, data, mask_u8_0,
                                                                          mask_u8_1, cap)
         dev = hi.device
@@ -419,6 +440,9 @@ class CoarseMatching(nn.Module):
         if self.training:
             raise NotImplementedError("loftr_b200 builds the inference path only (no training-time sampling)")
         lib = _lib.load()
+        k = self.max_matches_per_pair
+        if k is not None:
+            _lib.require_match_cap(lib)
         dev = hi.device
         b_ids = torch.empty(cap, dtype=torch.int64, device=dev)
         i_ids = torch.empty(cap, dtype=torch.int64, device=dev)
@@ -457,7 +481,10 @@ class CoarseMatching(nn.Module):
             a.conf_matrix = conf.data_ptr()
         nbytes = lib.lb_coarse_match_workspace_bytes(n, L, S)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        _lib.check(lib.lb_coarse_match(C.byref(a), ws.data_ptr(), nbytes, _stream(hi)))
+        if k is None:
+            _lib.check(lib.lb_coarse_match(C.byref(a), ws.data_ptr(), nbytes, _stream(hi)))
+        else:   # k >= L keeps every match; min() keeps the argument within a C int
+            _lib.check(lib.lb_coarse_match_capped(C.byref(a), min(k, L), ws.data_ptr(), nbytes, _stream(hi)))
         return b_ids, i_ids, j_ids, mconf, mk0, mk1, count, conf
 
     @torch.no_grad()
@@ -785,9 +812,11 @@ class LoFTR(nn.Module):
         exceed `capacity`; entries at or past min(count, capacity) are unspecified.  Only windows below the count are
         refined: the fine stage reads the count on the device.
 
-        capacity: defaults to the exact bound of the coarse stage, n*min(L, S) (n*L with masks).  The fine stage keeps
-        about 5 KB of state per window row, i.e. about 256 KB per match of capacity (about 10 GB at batch 8 640x480):
-        a smaller capacity trades that memory for the risk of overflow, which stays visible in num_matches.
+        capacity: defaults to the exact bound of the coarse stage, n*min(L, S) (n*L with masks), or n*min(k, that
+        per-pair bound) with match_coarse.max_matches_per_pair = k.  The fine stage keeps about 5 KB of state per window
+        row, i.e. about 256 KB per match of capacity (about 10 GB at batch 8 640x480 without k): a smaller capacity
+        trades that memory for the risk of overflow, which stays visible in num_matches.  A capacity of n*k never
+        overflows.
 
         Configurations whose output list depends on the data (match_coarse.thr < 0) raise ValueError."""
         if self.training:
@@ -810,7 +839,8 @@ class LoFTR(nn.Module):
             elif t.device != dev:
                 raise ValueError(f"forward_static: `{k}` is on {t.device}, image0 on {dev}")
         state, feat_f0, feat_f1, bs, L, S, c, m0, m1 = self._coarse_features(data)
-        cap = self.coarse_matching.default_capacity(bs, L, S, m0 is not None) if capacity is None else int(capacity)
+        cap = int(capacity) if capacity is not None else self.coarse_matching.default_capacity(
+            bs, L, S, m0 is not None, self.coarse_matching.max_matches_per_pair)
 
         # 3. coarse matching into capacity buffers; `count` stays on the device
         count = self.coarse_matching.run_static(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1, cap)
@@ -947,7 +977,8 @@ class CapturedMatcher:
     The graph holds raw pointers into the model's packed-weight caches, parameters and buffers.  The captured matcher
     keeps those objects alive and, on every call, checks on the host that the model still uses them: after
     `load_state_dict`, `.to()`, `invalidate_packed()` or a parameter change a call raises instead of replaying against
-    stale weights; `recapture()` rebuilds the graph.  See `LoFTR.forward_static` for `capacity` and its memory cost."""
+    stale weights; `recapture()` rebuilds the graph.  The same holds for `model.coarse_matching.max_matches_per_pair`,
+    which is captured with the graph.  See `LoFTR.forward_static` for `capacity` and its memory cost."""
 
     _TRIMMED = ("b_ids", "i_ids", "j_ids", "gt_mask", "mconf", "mkpts0_c", "mkpts1_c", "mkpts1_f", "expec_f")
 
@@ -984,6 +1015,7 @@ class CapturedMatcher:
     def recapture(self):
         """(Re)runs the eager warm-up and captures a new graph against the model's current weights."""
         self.graph = self.out = self._refs = None
+        max_per_pair = self.model.coarse_matching.max_matches_per_pair
         with torch.cuda.device(self.device):
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
@@ -994,6 +1026,7 @@ class CapturedMatcher:
             with torch.cuda.graph(graph):
                 self.model.forward_static(out, self.capacity_arg)
         self.graph, self.out, self._refs = graph, out, _weight_refs(self.model)
+        self.max_matches_per_pair = max_per_pair
 
     def _check_weights(self):
         caches, tensors, key = _weight_refs(self.model)
@@ -1007,6 +1040,10 @@ class CapturedMatcher:
         if self.graph is None:
             raise RuntimeError("loftr_b200.CapturedMatcher: no captured graph; call recapture()")
         self._check_weights()
+        now = self.model.coarse_matching.max_matches_per_pair
+        if now != self.max_matches_per_pair:
+            raise RuntimeError(f"loftr_b200.CapturedMatcher: coarse_matching.max_matches_per_pair changed since capture "
+                               f"({self.max_matches_per_pair} -> {now}); call recapture()")
         for k, buf in self.static.items():
             if k not in data:
                 raise ValueError(f"CapturedMatcher was built with `{k}` but the call does not provide it")
