@@ -1,0 +1,328 @@
+// Stride-1 3x3 convolution on the split-precision core with the input patch resident in shared memory.
+//
+// gemm_split_kernel's convolution mode loads one 8 x 16 pixel patch per (tap, 64-channel block), so the nine taps of a
+// 3x3 convolution bring every input pixel from L2 to shared memory 6.4 times (1,152 pixels for a 10 x 18 patch of 180).
+// Here the producer loads the 10 x 18 halo of an output tile once per channel block and the nine taps become nine
+// shifted shared-memory descriptors over it; only the weights stream through the per-tap pipeline ring.
+//
+// Halo layout (wgmma no-swizzle K-major core matrices): [8-channel chunk][halo pixel (row-major, 18 wide)][16 bytes].
+// An m64 instruction covers output rows y = 0..7 of the tile's x-half mh; for tap (ky, kx) its 8-row group y is the
+// 8 consecutive halo pixels from (y + ky) * 18 + 8 * mh + kx -- one 128-byte core matrix -- so
+//   start = ((ky * 18) + 8 * mh + kx) * 16,   SBO = 18 * 16 (next y),   LBO = chunk stride (next 8 channels along K),
+// and k-step k of a 64-channel block starts 2k chunks further.  Row r of instruction mh is therefore tile pixel
+// (r / 8) * 16 + 8 * mh + r % 8; the accumulator is staged row-major by pixel, exactly as gemm_split_kernel stages it,
+// so the epilogue (EpiConv) is unchanged.
+//
+// Each halo plane is loaded as eight 8-channel boxes of a 4-D NHWC map whose channel extent is Cin: TMA zero-fills
+// the image border (the padding) and every channel at or past Cin, so the row-stride padding of a Cin = 196 plane
+// (channels 196..199 are never written) cannot reach the MMAs.  Chunks sit 2,944 bytes apart (2,880 rounded up to the
+// 128-byte alignment of a TMA destination).
+//
+// K order: with at most two halos per tile (Cin <= 128) both stay resident and the taps run tap-major, the order of
+// gemm_split_kernel's convolution mode, so those layers produce the same bits.  Wider inputs run channel-block-major
+// (nine taps per halo, the next block's halo loading into the other slot meanwhile); the channel remainder
+// (Cin = 64 * cin_blocks + r, r <= 16) is a last 16-channel halo with one K = 16 step per tap.
+//
+// Warp roles, the epilogue contract, the accumulator staging over the dead ring / halo memory and the tile-end drain
+// are those of gemm_split_kernel.  Where the staging fits in the weight ring (N = 128) the next tile's first halos
+// load while the epilogue runs.
+#pragma once
+#include "gemm_split.cuh"
+
+namespace lb {
+
+constexpr int kHaloW = kConvTileW + 2;
+constexpr int kHaloH = kConvTileH + 2;
+constexpr int kHaloChunkBytes = 2944;                      // 180 pixels x 16 bytes = 2,880, 128-byte aligned
+constexpr int kHaloPlaneBytes = (kBlockK / 8) * kHaloChunkBytes;
+constexpr int kHaloSlotBytes = 2 * kHaloPlaneBytes;         // hi + lo planes of one channel block
+constexpr int kHaloTaps = 9;
+static_assert(kHaloW * kHaloH * 16 <= kHaloChunkBytes && kHaloChunkBytes % 128 == 0, "halo chunk layout");
+
+// Shared memory: [weight ring | two halo slots (accumulator staging aliases both)][epilogue area][mbarriers].
+// A weight stage is one tap of a 64-channel block (kBK = 64, 128-byte swizzle rows) when three of them fit beside the
+// halo slots, else half a tap (kBK = 32, 64-byte swizzle rows): three or more stages in flight at every N.
+template <int BLOCK_N, int kEpiBytes>
+struct HaloSmem {
+  static constexpr int kBarBytes = 256;
+  static constexpr int kFree = 232448 - kBarBytes - kEpiBytes - 2 * kHaloSlotBytes;
+  static constexpr int kBK = kFree / (2 * BLOCK_N * kBlockK * 2) >= 3 ? kBlockK : kBlockK / 2;
+  static constexpr int kBTile = BLOCK_N * kBK * 2;        // per plane
+  static constexpr int kStageBytes = 2 * kBTile;
+  static constexpr int kStages = kFree / kStageBytes < 6 ? kFree / kStageBytes : 6;
+  static_assert(kStages >= 3, "the weight ring needs three stages");
+  static constexpr int kRingBytes = kStages * kStageBytes;
+  static constexpr int kAccStride = BLOCK_N + 4;         // floats, as GemmSmem
+  static constexpr int kAccBytes = (kBlockM * kAccStride + 32) * 4;
+  static constexpr int kMainBytes = kRingBytes + 2 * kHaloSlotBytes;
+  static_assert(kMainBytes >= kAccBytes && kMainBytes % 1024 == 0 && kRingBytes % 1024 == 0, "halo smem layout");
+  static constexpr int kTotalBytes = kMainBytes + kEpiBytes + kBarBytes;
+};
+
+// No-swizzle K-major descriptor: lbo / sbo = byte distance between core matrices adjacent along K / along M or N.
+__device__ __forceinline__ uint64_t wgmma_desc_k_noswz(uint32_t a, uint32_t lbo, uint32_t sbo) {
+  uint64_t d = static_cast<uint64_t>((a >> 4) & 0x3FFF);
+  d |= static_cast<uint64_t>(lbo >> 4) << 16;
+  d |= static_cast<uint64_t>(sbo >> 4) << 32;
+  return d;
+}
+
+// tm_a_*: 4-D NHWC maps (C = Cin, W, H, N), box 8 channels x 18 x 10 x 1, no swizzle.
+// tm_b_*: main weight planes [Cout, 9 * cin_blocks * 64], box kBK x BLOCK_N.  tm_br_*: remainder weight planes
+// [Cout, 9 * 16], box 16 x BLOCK_N (copies of tm_b_* when Cin has no remainder).
+// shape.conv: tiles_w, cin_blocks and rem_groups (> 0: a channel remainder) are read; stride 1, pad 1 are implied.
+template <int BLOCK_N, class Epi>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
+                    const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
+                    const __grid_constant__ CUtensorMap tm_br_hi, const __grid_constant__ CUtensorMap tm_br_lo,
+                    const GemmShape shape, const __grid_constant__ typename Epi::Params epi_params) {
+  using S = HaloSmem<BLOCK_N, Epi::kSmemBytes>;
+  constexpr int kN = BLOCK_N / 2;
+  constexpr int kBK = S::kBK;
+  constexpr int kSubs = kBlockK / kBK;                       // weight stages per (tap, 64-channel block)
+  constexpr int kRemBTile = BLOCK_N * kRemChannels * 2;      // per plane
+  constexpr bool kStagingInRing = S::kAccBytes <= S::kRingBytes;   // N = 128: the halo slots stay free at the tile end
+  static_assert(kN % 8 == 0, "wgmma N must be a multiple of 8");
+  static_assert(2 * kRemBTile <= S::kStageBytes && kRemBTile % 256 == 0, "remainder weight stage");
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* ring = smem_raw;
+  uint8_t* halo = smem_raw + S::kRingBytes;
+  uint8_t* epi_smem = smem_raw + S::kMainBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_raw + S::kMainBytes + Epi::kSmemBytes);
+  uint64_t* empty_bar = full_bar + S::kStages;
+  uint64_t* halo_full = empty_bar + S::kStages;
+  uint64_t* halo_empty = halo_full + 2;
+  uint64_t* acc_free = halo_empty + 2;
+  static_assert(Epi::kSmemBytes % 16 == 0, "epilogue area must keep the barriers aligned");
+  static_assert((2 * S::kStages + 5) * 8 <= S::kBarBytes, "barrier area");
+  if ((smem_u32(smem_raw) & 1023u) != 0) asm volatile("trap;");
+
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+
+  if (warp == kProducerWarp && lane == 0) {
+    tma_prefetch_desc(&tm_a_hi);
+    tma_prefetch_desc(&tm_a_lo);
+    tma_prefetch_desc(&tm_b_hi);
+    tma_prefetch_desc(&tm_b_lo);
+  }
+  if (warp == 0 && lane == 0) {
+    for (int s = 0; s < S::kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], kEpiThreads);
+    }
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(&halo_full[s], 1);
+      mbar_init(&halo_empty[s], kEpiThreads);
+    }
+    mbar_init(acc_free, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  // programmatic dependent launch, as in gemm_split_kernel
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+
+  const ConvGeom& g = shape.conv;
+  const int n_halo = g.cin_blocks + (g.rem_groups > 0 ? 1 : 0);   // halos (channel blocks) per output tile
+  const bool tap_major = n_halo <= 2;                               // every halo of the tile resident at once
+  const int n_steps = kHaloTaps * n_halo;                           // (tap, halo) steps of a tile
+  const int total_items = shape.batches * shape.m_tiles * shape.n_chunks;
+
+  if (warp == kProducerWarp) {
+    // ------------------------------------------------------------ TMA producer
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      uint32_t tiles = 0;
+      int halos = 0;   // halo loads issued so far: load i goes to slot i & 1
+      for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+        const int chunk = item % shape.n_chunks;
+        const int mt = (item / shape.n_chunks) % shape.m_tiles;
+        const int batch = item / (shape.n_chunks * shape.m_tiles);
+        const int ty = mt / g.tiles_w, tx = mt - ty * g.tiles_w;
+        const int x0 = tx * kConvTileW - 1, y0 = ty * kConvTileH - 1;
+        const int nt_begin = chunk * shape.tiles_per_chunk;
+        const int nt_end = min(nt_begin + shape.tiles_per_chunk, shape.n_tiles);
+        for (int nt = nt_begin; nt < nt_end; ++nt) {
+          // the previous tile's staged accumulator must be consumed before the ring (and, when the staging reaches
+          // past the ring, the halo slots) is refilled
+          bool staged = tiles > 0;
+          const uint32_t staged_parity = (tiles - 1) & 1;
+          ++tiles;
+          auto wait_staged = [&]() {
+            if (staged) mbar_wait(acc_free, staged_parity);
+            staged = false;
+          };
+          // ---- the halo of channel block hh
+          auto load_halo = [&](int hh) {
+            if (!kStagingInRing) wait_staged();
+            const int hi = halos + hh, slot = hi & 1;
+            mbar_wait(&halo_empty[slot], ((hi >> 1) & 1) ^ 1);
+            const int chunks = (hh == g.cin_blocks ? kRemChannels : kBlockK) / 8;
+            uint64_t* fb = &halo_full[slot];
+            mbar_arrive_expect_tx(fb, static_cast<uint32_t>(chunks) * 2 * kHaloW * kHaloH * 16);
+            uint8_t* dst = halo + slot * kHaloSlotBytes;
+            for (int c = 0; c < chunks; ++c) {
+              const int ch = hh * kBlockK + 8 * c;
+              tma_load_4d(dst + c * kHaloChunkBytes, &tm_a_hi, fb, ch, x0, y0, batch);
+              tma_load_4d(dst + kHaloPlaneBytes + c * kHaloChunkBytes, &tm_a_lo, fb, ch, x0, y0, batch);
+            }
+          };
+          // the halos needed first are issued before the weights (with kStagingInRing: while the previous tile's
+          // epilogue still runs); the others at their first tap
+          const int preload = tap_major ? n_halo : 1;
+          for (int hh = 0; hh < preload; ++hh) load_halo(hh);
+          for (int s = 0; s < n_steps; ++s) {
+            const int hh = tap_major ? s % n_halo : s / kHaloTaps;
+            const int tap = tap_major ? s / n_halo : s % kHaloTaps;
+            const bool rem = hh == g.cin_blocks;
+            if (tap == 0 && hh >= preload) load_halo(hh);
+            // ---- the weights of (tap, hh): kSubs stages, or one 16-channel stage for the remainder
+            for (int j = 0; j < (rem ? 1 : kSubs); ++j) {
+              wait_staged();
+              mbar_wait(&empty_bar[stage], phase ^ 1);
+              uint8_t* st = ring + stage * S::kStageBytes;
+              uint64_t* fb = &full_bar[stage];
+              if (rem) {
+                mbar_arrive_expect_tx(fb, 2 * kRemBTile);
+                tma_load_3d(st, &tm_br_hi, fb, tap * kRemChannels, nt * BLOCK_N, 0);
+                tma_load_3d(st + kRemBTile, &tm_br_lo, fb, tap * kRemChannels, nt * BLOCK_N, 0);
+              } else {
+                // the main weight planes keep gemm_split_kernel's K layout: k-block (tap, cb) at (tap * cin_blocks + cb) * 64
+                const int k0 = (tap * g.cin_blocks + hh) * kBlockK + j * kBK;
+                mbar_arrive_expect_tx(fb, S::kStageBytes);
+                tma_load_3d(st, &tm_b_hi, fb, k0, nt * BLOCK_N, 0);
+                tma_load_3d(st + S::kBTile, &tm_b_lo, fb, k0, nt * BLOCK_N, 0);
+              }
+              if (++stage == S::kStages) {
+                stage = 0;
+                phase ^= 1;
+              }
+            }
+          }
+          halos += n_halo;
+        }
+      }
+    }
+  } else {
+    // ------------------------------------------------------------ consumer warpgroups: wgmma + epilogue
+    const int ct = threadIdx.x - kEpiWarp0 * 32;
+    const int h = ct >> 7;
+    const int wt = ct & 127;
+    Epi epi(epi_params, epi_smem, shape);
+    float acc[2][kN / 2];                           // x-half mh of the tile, this warpgroup's column half
+    float* stg = reinterpret_cast<float*>(ring);
+    const uint32_t ring_u32 = smem_u32(ring);
+    const uint32_t halo_u32 = smem_u32(halo);
+    int stage = 0;
+    uint32_t phase = 0;
+    int halos = 0;
+    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+      const int chunk = item % shape.n_chunks;
+      const int mt = (item / shape.n_chunks) % shape.m_tiles;
+      const int batch = item / (shape.n_chunks * shape.m_tiles);
+      const int nt_begin = chunk * shape.tiles_per_chunk;
+      const int nt_end = min(nt_begin + shape.tiles_per_chunk, shape.n_tiles);
+      epi.item_begin(batch, mt * kBlockM, chunk);
+      for (int nt = nt_begin; nt < nt_end; ++nt) {
+        epi.prefetch(batch, mt * kBlockM, nt * BLOCK_N);
+#pragma unroll
+        for (int i = 0; i < kN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
+        int prev = -1;        // ring stage of the previous weight stage
+        int prev_halo = -1;   // halo slot whose last tap was the previous weight stage, else -1
+        for (int s = 0; s < n_steps; ++s) {
+          const int hh = tap_major ? s % n_halo : s / kHaloTaps;
+          const int tap = tap_major ? s / n_halo : s % kHaloTaps;
+          const bool rem = hh == g.cin_blocks;
+          const int hi = halos + hh, slot = hi & 1;
+          if (tap == 0) mbar_wait(&halo_full[slot], (hi >> 1) & 1);
+          const int ky = tap / 3, kx = tap - ky * 3;
+          // halo pixel of row group y = 0 of x-half 0 for this tap
+          const uint32_t a_tap = halo_u32 + slot * kHaloSlotBytes + (ky * kHaloW + kx) * 16;
+          const int subs = rem ? 1 : kSubs;
+          for (int j = 0; j < subs; ++j) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t st = ring_u32 + stage * S::kStageBytes;
+            wgmma_fence();
+            if (rem) {
+              const uint32_t b_off = static_cast<uint32_t>(h * kN * kRemChannels * 2);
+              const uint64_t rb_hi = wgmma_desc_k_sw32(st + b_off);
+              const uint64_t rb_lo = wgmma_desc_k_sw32(st + kRemBTile + b_off);
+#pragma unroll
+              for (int mh = 0; mh < 2; ++mh) {
+                const uint32_t a = a_tap + mh * 8 * 16;
+                const uint64_t ra_hi = wgmma_desc_k_noswz(a, kHaloChunkBytes, kHaloW * 16);
+                const uint64_t ra_lo = wgmma_desc_k_noswz(a + kHaloPlaneBytes, kHaloChunkBytes, kHaloW * 16);
+                wgmma_f16<kN>(acc[mh], ra_hi, rb_hi, 1u);
+                wgmma_f16<kN>(acc[mh], ra_hi, rb_lo, 1u);
+                wgmma_f16<kN>(acc[mh], ra_lo, rb_hi, 1u);
+              }
+            } else {
+              const uint32_t b_off = static_cast<uint32_t>(h * kN * kBK * 2);
+              const uint64_t db_hi = kBK == 64 ? wgmma_desc_k_sw128(st + b_off) : wgmma_desc_k_sw64(st + b_off);
+              const uint64_t db_lo =
+                  kBK == 64 ? wgmma_desc_k_sw128(st + S::kBTile + b_off) : wgmma_desc_k_sw64(st + S::kBTile + b_off);
+#pragma unroll
+              for (int mh = 0; mh < 2; ++mh) {
+                const uint32_t a = a_tap + mh * 8 * 16 + j * (kBK / kMmaK) * 2 * kHaloChunkBytes;
+                const uint64_t da_hi = wgmma_desc_k_noswz(a, kHaloChunkBytes, kHaloW * 16);
+                const uint64_t da_lo = wgmma_desc_k_noswz(a + kHaloPlaneBytes, kHaloChunkBytes, kHaloW * 16);
+#pragma unroll
+                for (int k = 0; k < kBK / kMmaK; ++k) {
+                  // A: 16 channels = two chunks further; B: 32 bytes further inside the swizzle row (16-byte units)
+                  const uint64_t a_adv = static_cast<uint64_t>(k * 2 * kHaloChunkBytes / 16);
+                  const uint64_t b_adv = static_cast<uint64_t>(k * 2);
+                  wgmma_f16<kN>(acc[mh], da_hi + a_adv, db_hi + b_adv, 1u);
+                  wgmma_f16<kN>(acc[mh], da_hi + a_adv, db_lo + b_adv, 1u);
+                  wgmma_f16<kN>(acc[mh], da_lo + a_adv, db_hi + b_adv, 1u);
+                }
+              }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();   // the previous stage's MMAs are done: its weight slot (and halo, if last) may be refilled
+            if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+            if (prev_halo >= 0) mbar_arrive(&halo_empty[prev_halo]);
+            prev = stage;
+            prev_halo = (tap == kHaloTaps - 1 && j == subs - 1) ? slot : -1;
+            if (++stage == S::kStages) {
+              stage = 0;
+              phase ^= 1;
+            }
+          }
+        }
+        halos += n_halo;
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc[0]);
+        wgmma_fence_regs(acc[1]);
+        mbar_arrive(&empty_bar[prev]);
+        if (prev_halo >= 0) mbar_arrive(&halo_empty[prev_halo]);
+        // ---- stage the accumulator by tile pixel: row r of instruction mh is pixel (r / 8) * 16 + 8 * mh + r % 8
+        epi_group_sync();
+        {
+          const int p0 = 32 * (wt >> 5) + ((wt & 31) >> 2);
+          const int c0 = h * kN + 2 * (wt & 3);
+#pragma unroll
+          for (int mh = 0; mh < 2; ++mh) {
+#pragma unroll
+            for (int j = 0; j < kN / 8; ++j) {
+              float* p = stg + (p0 + 8 * mh) * S::kAccStride + c0 + 8 * j;
+              *reinterpret_cast<float2*>(p) = make_float2(acc[mh][4 * j], acc[mh][4 * j + 1]);
+              *reinterpret_cast<float2*>(p + 16 * S::kAccStride) = make_float2(acc[mh][4 * j + 2], acc[mh][4 * j + 3]);
+            }
+          }
+        }
+        epi_group_sync();
+        epi.tile(smem_u32(stg + (ct & 127) * S::kAccStride), batch, mt * kBlockM, nt * BLOCK_N);
+        fence_proxy_async();   // staging reads / writes (generic proxy) before the next TMA writes into ring and halos
+        epi_group_sync();
+        if (ct == 0) mbar_arrive(acc_free);
+      }
+      epi.item_end(batch, mt * kBlockM, chunk);
+    }
+    tma_store_wait_all();
+  }
+}
+
+}  // namespace lb

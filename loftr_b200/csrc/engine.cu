@@ -16,6 +16,7 @@
 #include "../../include/loftr_b200.h"
 #include "epilogues.cuh"
 #include "gemm_split.cuh"
+#include "conv_halo.cuh"
 #include "simt_kernels.cuh"
 #include "kv_gemm.cuh"
 #include "full_attn.cuh"
@@ -219,6 +220,26 @@ static int make_map_nhwc(CUtensorMap* m, const void* base, int C, int W, int H, 
   return 0;
 }
 
+// NHWC fp16 plane [N][H][W][C] for conv3x3_halo_kernel: box = 8 channels x 18 x 10 pixels x 1, no swizzle (one
+// 8-channel chunk of a 10 x 18 halo).  The channel extent is C, so channels at or past C read as zeros.
+static int make_map_halo(CUtensorMap* m, const void* base, int C, int W, int H, int N, long ld) {
+  auto enc = get_encode();
+  if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail("plane pointer not 16-byte aligned");
+  if ((ld * 2) % 16 != 0) return fail("NHWC channel stride must be a multiple of 8 elements (got %ld)", ld);
+  cuuint64_t dims[4] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H),
+                        static_cast<cuuint64_t>(N)};
+  cuuint64_t strides[3] = {static_cast<cuuint64_t>(ld * 2), static_cast<cuuint64_t>(ld * 2 * W),
+                           static_cast<cuuint64_t>(ld * 2 * W) * H};
+  cuuint32_t box[4] = {8, static_cast<cuuint32_t>(kHaloW), static_cast<cuuint32_t>(kHaloH), 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (halo) failed with CUresult %d", static_cast<int>(r));
+  return 0;
+}
+
 // ---- output tensor maps for the TMA-store epilogues (epilogues.cuh OutMaps)
 // [batches][rows][cols] matrix (row stride ld, batch stride bs elements; bs = 0 -> rows * ld): box 32 x 32 x 1,
 // 64-byte swizzle for fp16 planes, 128-byte swizzle for fp32
@@ -285,13 +306,9 @@ struct GemmMaps {
   CUtensorMap ar_hi, ar_lo, br_hi, br_lo;  // convolution channel remainder (16-element boxes); copies of the above if unused
 };
 
-template <int BN, class Epi>
-static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const typename Epi::Params& ep, int sms,
-                      cudaStream_t st) {
-  using S = GemmSmem<BN, Epi::kSmemBytes>;
-  constexpr int smem_bytes = S::kRingBytes + S::kBarBytes + Epi::kSmemBytes;
-  static_assert(smem_bytes <= 232448, "shared memory budget exceeded");
-  constexpr auto kern = &gemm_split_kernel<BN, Epi>;
+// One persistent CTA per SM (at most one per work item) of a tensor-core kernel with the GemmShape work split.
+template <auto kern, class... Args>
+static int launch_persistent(int tag, const GemmShape& s, int smem_bytes, int sms, cudaStream_t st, Args... args) {
   LB_TRY(set_max_dynamic_smem<kern>(smem_bytes));
   const long items = static_cast<long>(s.batches) * s.m_tiles * s.n_chunks;
   const int grid = static_cast<int>(items < sms ? items : sms);
@@ -318,10 +335,19 @@ static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const t
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.numAttrs = 1;
   }
-  LB_CUDA(cudaLaunchKernelEx(&cfg, kern, maps.a_hi, maps.a_lo, maps.b_hi, maps.b_lo, maps.ar_hi, maps.ar_lo, maps.br_hi,
-                             maps.br_lo, s, ep));
+  LB_CUDA(cudaLaunchKernelEx(&cfg, kern, args...));
   LB_LAUNCHED();
   return timing_end(rec, st);
+}
+
+template <int BN, class Epi>
+static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const typename Epi::Params& ep, int sms,
+                      cudaStream_t st) {
+  using S = GemmSmem<BN, Epi::kSmemBytes>;
+  constexpr int smem_bytes = S::kRingBytes + S::kBarBytes + Epi::kSmemBytes;
+  static_assert(smem_bytes <= 232448, "shared memory budget exceeded");
+  return launch_persistent<&gemm_split_kernel<BN, Epi>>(tag, s, smem_bytes, sms, st, maps.a_hi, maps.a_lo, maps.b_hi,
+                                                          maps.b_lo, maps.ar_hi, maps.ar_lo, maps.br_hi, maps.br_lo, s, ep);
 }
 
 // live / live_unit_rows: optional device bound on the rows of every batch (GemmShape::live_count)
@@ -423,6 +449,56 @@ static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_re
   return launch_raw<BN, Epi>(TAG_CONV, mp, s, ep, sms, st);
 }
 
+// Stride-1 3x3 convolution through conv3x3_halo_kernel (same operands, weights and epilogue as launch_conv).
+template <int BN>
+static int launch_conv_halo(const Planes& in, const Planes& wgt, const Planes& wgt_rem, const ConvDesc& d,
+                            const typename EpiConv<BN, false>::Params& ep_in, cudaStream_t st) {
+  using Epi = EpiConv<BN, false>;
+  using S = HaloSmem<BN, Epi::kSmemBytes>;
+  static_assert(S::kTotalBytes <= 232448, "shared memory budget exceeded");
+  int sms = 0;
+  LB_TRY(device_check(&sms));
+  if (d.ksize != 3 || d.stride != 1 || d.pad != 1) return fail("the halo convolution is built for 3x3, stride 1, pad 1");
+  int cin_blocks = 0, rem = 0;
+  conv_layout(d.Cin, &cin_blocks, &rem);
+  const int taps = kHaloTaps;
+  const int tiles_h = (d.H_out + kConvTileH - 1) / kConvTileH;
+  const int tiles_w = (d.W_out + kConvTileW - 1) / kConvTileW;
+  GemmShape s;
+  s.batches = d.N;
+  s.M = tiles_h * tiles_w * kBlockM;
+  s.N = d.Cout;
+  s.K = taps * cin_blocks * kBlockK;
+  s.b_batched = 0;
+  s.m_tiles = tiles_h * tiles_w;
+  s.n_tiles = (d.Cout + BN - 1) / BN;
+  s.n_chunks = s.n_tiles;
+  s.tiles_per_chunk = 1;
+  const int rem_groups = rem ? (taps + kRemTapsPerStage - 1) / kRemTapsPerStage : 0;
+  s.conv = ConvGeom{1, tiles_w, 1, 1, 3, cin_blocks, taps, taps * cin_blocks, rem_groups};
+  s.live_count = nullptr;
+  s.live_unit_rows = 0;
+  if (rem && (!wgt_rem.hi || !wgt_rem.lo)) return fail("convolution with Cin=%d needs remainder weight planes", d.Cin);
+  CUtensorMap a_hi, a_lo, b_hi, b_lo, br_hi, br_lo;
+  LB_TRY(make_map_halo(&a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld));
+  LB_TRY(make_map_halo(&a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld));
+  LB_TRY(make_map(&b_hi, wgt.hi, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
+  LB_TRY(make_map(&b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
+  if (rem) {
+    LB_TRY(make_map(&br_hi, wgt_rem.hi, taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
+    LB_TRY(make_map(&br_lo, wgt_rem.lo, taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
+  } else {
+    br_hi = b_hi;
+    br_lo = b_lo;
+  }
+  typename Epi::Params ep = ep_in;
+  ep.H_out = d.H_out;
+  ep.W_out = d.W_out;
+  ep.tiles_w = tiles_w;
+  return launch_persistent<&conv3x3_halo_kernel<BN, Epi>>(TAG_CONV, s, S::kTotalBytes, sms, st, a_hi, a_lo, b_hi, b_lo,
+                                                            br_hi, br_lo, s, ep);
+}
+
 // number of n-chunks that gives every SM a few work items when a CTA must sweep many n tiles
 static int pick_chunks(int row_items, int n_tiles, int sms) {
   int c = 1;
@@ -493,8 +569,9 @@ static int tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const Lb
 
 // ------------------------------------------------------------------------------------------------ backbone
 // ResNetFPN_8_2 forward (reference src/loftr/backbone/resnet_fpn.py:43-118) on tensor cores: every 3x3 / 1x1
-// convolution is an implicit GEMM through gemm_split_kernel<., EpiConv> (BatchNorm, ReLU / LeakyReLU, residual
-// add and the FPN upsample-add fused in the epilogue); activations live as NHWC fp16 hi/lo planes.
+// convolution is an implicit GEMM through gemm_split_kernel<., EpiConv>, the stride-1 3x3 ones through
+// conv3x3_halo_kernel<., EpiConv> (BatchNorm, ReLU / LeakyReLU, residual add and the FPN upsample-add fused in the
+// epilogue); activations live as NHWC fp16 hi/lo planes.
 struct BbBuf {
   __half* hi;
   __half* lo;
@@ -565,18 +642,21 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
     LB_TRY(make_out_map_nhwc(&om.f32, r.out_f32, true, d.Cout, d.W_out, d.H_out, N, r.f32_ld));
     om.use |= 2;
   }
-#define LB_CONV_CASE_UP(BN, UP)                                                                                       \
+  // stride-1 3x3 convolutions (none of them carries the FPN upsample-add) load each input patch once per channel block
+  const bool halo = w.ksize == 3 && w.stride == 1 && !r.up;
+#define LB_CONV_CASE_UP(BN, UP, ...)                                                                                  \
   {                                                                                                                   \
     EpiConv<BN, UP>::Params ep{w.scale, w.shift, r.act, r.res ? r.res->hi : nullptr, r.res ? r.res->lo : nullptr,     \
                                r.res ? r.res->ld : 0, r.up ? r.up->hi : nullptr, r.up ? r.up->lo : nullptr,          \
                                r.up ? r.up->ld : 0, r.up_h, r.up_w, r.out ? r.out->hi : nullptr,                      \
                                r.out ? r.out->lo : nullptr, r.out ? r.out->ld : 0, r.out_f32, r.f32_ld, 0, 0, 0, om}; \
-    return launch_conv<BN, UP>(in, wg, wr, d, ep, st);                                                                \
+    return __VA_ARGS__(in, wg, wr, d, ep, st);                                                                        \
   }
 #define LB_CONV_CASE(BN)                                                                                              \
   {                                                                                                                   \
-    if (r.up) LB_CONV_CASE_UP(BN, true)                                                                               \
-    LB_CONV_CASE_UP(BN, false)                                                                                        \
+    if (r.up) LB_CONV_CASE_UP(BN, true, launch_conv<BN, true>)                                                        \
+    if (halo) LB_CONV_CASE_UP(BN, false, launch_conv_halo<BN>)                                                        \
+    LB_CONV_CASE_UP(BN, false, launch_conv<BN, false>)                                                                \
   }
   // output-channel tile: the smallest built N that covers Cout (196 -> 208: 13 x 16, no MMAs on 60 padding columns)
   if (w.cout <= 128) LB_CONV_CASE(128)
