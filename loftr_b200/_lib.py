@@ -175,7 +175,7 @@ def load():
                              "rebuild it with `make`")
     for name, (res, args) in SIGNATURES.items():
         if lib.lb_version() < _SINCE.get(name, 0):
-            continue             # not in this older build; the require_* checks stop its callers
+            continue             # not in this older build; `require` stops its callers
         fn = getattr(lib, name)  # AttributeError if the library does not export a declared symbol
         fn.restype = res
         fn.argtypes = args
@@ -183,28 +183,13 @@ def load():
     return lib
 
 
-def require_full_attention(lib):
-    """Raise unless `lib` runs full-attention layers (library version >= FULL_ATTENTION_VERSION)."""
-    v = lib.lb_version()
-    if v < FULL_ATTENTION_VERSION:
-        raise RuntimeError(f"loftr_b200: full attention needs library version {FULL_ATTENTION_VERSION} or newer, but "
-                           f"{LIB_PATH} is version {v}: rebuild it with `make`")
-
-
-def require_feature_bank(lib):
-    """Raise unless `lib` has the indexed entry points of LoFTR.match_features (version >= FEATURE_BANK_VERSION)."""
-    v = lib.lb_version()
-    if v < FEATURE_BANK_VERSION:
-        raise RuntimeError(f"loftr_b200: match_features needs library version {FEATURE_BANK_VERSION} or newer, but "
-                           f"{LIB_PATH} is version {v}: rebuild it with `make`")
-
-
-def require_match_cap(lib):
-    """Raise unless `lib` has lb_coarse_match_capped (match_coarse.max_matches_per_pair; version >= MATCH_CAP_VERSION)."""
-    v = lib.lb_version()
-    if v < MATCH_CAP_VERSION:
-        raise RuntimeError(f"loftr_b200: match_coarse.max_matches_per_pair needs library version {MATCH_CAP_VERSION} or "
-                           f"newer, but {LIB_PATH} is version {v}: rebuild it with `make`")
+def require(version: int, what: str):
+    """Raise unless the library is `version` or newer, naming `what` (the path or option that needs it).  `load()`
+    accepts every build from MIN_VERSION on, so that LOFTR_B200_LIB can select an older one for the paths it runs."""
+    v = load().lb_version()
+    if v < version:
+        raise RuntimeError(f"loftr_b200: {what} needs library version {version} or newer, but {LIB_PATH} is version "
+                           f"{v}: rebuild it with `make`")
 
 
 def check(rc: int):

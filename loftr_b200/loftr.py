@@ -40,22 +40,36 @@ def _stream(ref=None):
     return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
-class _PackedCacheMixin:
-    """Keeps the ctypes / device-plane weight caches out of deepcopy / pickle state and drops them whenever the
-    parameters are re-materialised (`_apply`: .to / .cuda / .float / .half) or re-loaded."""
-    _CACHE_ATTRS = ("_packed", "_packed_key")
+def _weights_key(module):
+    """(data_ptr, _version) of every parameter and buffer of `module`: changes when one is replaced, moved or modified
+    in place (not through `.data`)."""
+    return tuple((t.data_ptr(), t._version) for t in (*module.parameters(), *module.buffers()))
+
+
+class _PackedCache:
+    """A packed copy of the weights of `_packed_source()` (by default the module itself), built by `_build()`.
+    `_pack()` rebuilds it when `_weights_key` of that module changes.  It is dropped whenever the parameters are
+    re-materialised (`_apply`: .to / .cuda / .float / .half) or re-loaded, and by `invalidate_packed()`, and it never
+    enters deepcopy / pickle state: it holds ctypes structures with raw device pointers."""
+    _packed = None
+    _packed_key = None
+
+    def _packed_source(self):
+        return self
+
+    def _pack(self):
+        key = _weights_key(self._packed_source())
+        if self._packed is None or self._packed_key != key:
+            with torch.no_grad():
+                self._packed = self._build()
+            self._packed_key = key
+        return self._packed
 
     def invalidate_packed(self):
-        for a in self._CACHE_ATTRS:
-            if a in self.__dict__:
-                self.__dict__[a] = None
+        self._packed = self._packed_key = None
 
     def __getstate__(self):
-        d = dict(self.__dict__)
-        for a in self._CACHE_ATTRS:
-            if a in d:
-                d[a] = None
-        return d
+        return {**super().__getstate__(), "_packed": None, "_packed_key": None}
 
     def _apply(self, fn, *args, **kwargs):
         self.invalidate_packed()
@@ -64,6 +78,11 @@ class _PackedCacheMixin:
     def _load_from_state_dict(self, *args, **kwargs):
         self.invalidate_packed()
         return super()._load_from_state_dict(*args, **kwargs)
+
+
+def _require_eval(module):
+    if module.training:
+        raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
 
 
 def _require_cuda(t: torch.Tensor, name: str):
@@ -99,22 +118,17 @@ def split_planes(x: torch.Tensor, hi: torch.Tensor | None = None, lo: torch.Tens
     return hi, lo
 
 
-class TensorCoreBackbone:
+class TensorCoreBackbone(_PackedCache):
     """ResNetFPN_8_2 forward through `lb_backbone_forward` (implicit-GEMM convolutions on wgmma).  Holds no
     parameters of its own: it packs the weights of the PyTorch `ResNetFPN` module it wraps (BatchNorm folded
-    with its running statistics = eval mode), lazily and again whenever a parameter or buffer changes."""
+    with its running statistics = eval mode), lazily and again whenever a parameter or buffer changes.  It is not a
+    submodule, so `LoFTR` drops its cache on `_apply` / `load_state_dict`."""
 
     def __init__(self, torch_backbone):
         self.m = torch_backbone
-        self._packed = None
-        self._key = None
 
-    def invalidate_packed(self):
-        self._packed = None
-        self._key = None
-
-    def __getstate__(self):   # the cache holds ctypes structures with device pointers: never copied / pickled
-        return {"m": self.m, "_packed": None, "_key": None}
+    def _packed_source(self):
+        return self.m
 
     @staticmethod
     def supported(torch_backbone) -> bool:
@@ -159,35 +173,29 @@ class TensorCoreBackbone:
         return _lib.LbConvWeights(hi_m.data_ptr(), lo_m.data_ptr(), _lib.ptr(hi_r), _lib.ptr(lo_r), scale.data_ptr(),
                                   shift.data_ptr(), cin, cout, k, conv.stride[0])
 
-    def _pack(self):
+    def _build(self):
         m = self.m
-        tensors = list(m.parameters()) + list(m.buffers())
-        key = tuple(t._version for t in tensors) + tuple(t.data_ptr() for t in tensors)
-        if self._packed is not None and self._key == key:
-            return self._packed
         keep = []
         w = _lib.LbBackboneWeights()
-        with torch.no_grad():
-            stem = m.conv1.weight.detach().float().reshape(m.conv1.out_channels, 49).t().contiguous()
-            sc, sh = self._fold(m.bn1, m.conv1.out_channels, stem.device)
-            keep += [stem, sc, sh]
-            w.stem_wt, w.stem_scale, w.stem_shift, w.stem_cout = stem.data_ptr(), sc.data_ptr(), sh.data_ptr(), stem.shape[1]
-            for name, layer in (("l1", m.layer1), ("l2", m.layer2), ("l3", m.layer3)):
-                arr = getattr(w, name)
-                for bi, blk in enumerate(layer):
-                    arr[2 * bi] = self._conv(blk.conv1, blk.bn1, keep)
-                    arr[2 * bi + 1] = self._conv(blk.conv2, blk.bn2, keep)
-                if layer[0].downsample is not None:
-                    setattr(w, name + "_down", self._conv(layer[0].downsample[0], layer[0].downsample[1], keep))
-            w.l3_out = self._conv(m.layer3_outconv, None, keep)
-            w.l2_out = self._conv(m.layer2_outconv, None, keep)
-            w.l2_out2[0] = self._conv(m.layer2_outconv2[0], m.layer2_outconv2[1], keep)
-            w.l2_out2[1] = self._conv(m.layer2_outconv2[3], None, keep)
-            w.l1_out = self._conv(m.layer1_outconv, None, keep)
-            w.l1_out2[0] = self._conv(m.layer1_outconv2[0], m.layer1_outconv2[1], keep)
-            w.l1_out2[1] = self._conv(m.layer1_outconv2[3], None, keep)
-        self._packed, self._key = (w, keep), key
-        return self._packed
+        stem = m.conv1.weight.detach().float().reshape(m.conv1.out_channels, 49).t().contiguous()
+        sc, sh = self._fold(m.bn1, m.conv1.out_channels, stem.device)
+        keep += [stem, sc, sh]
+        w.stem_wt, w.stem_scale, w.stem_shift, w.stem_cout = stem.data_ptr(), sc.data_ptr(), sh.data_ptr(), stem.shape[1]
+        for name, layer in (("l1", m.layer1), ("l2", m.layer2), ("l3", m.layer3)):
+            arr = getattr(w, name)
+            for bi, blk in enumerate(layer):
+                arr[2 * bi] = self._conv(blk.conv1, blk.bn1, keep)
+                arr[2 * bi + 1] = self._conv(blk.conv2, blk.bn2, keep)
+            if layer[0].downsample is not None:
+                setattr(w, name + "_down", self._conv(layer[0].downsample[0], layer[0].downsample[1], keep))
+        w.l3_out = self._conv(m.layer3_outconv, None, keep)
+        w.l2_out = self._conv(m.layer2_outconv, None, keep)
+        w.l2_out2[0] = self._conv(m.layer2_outconv2[0], m.layer2_outconv2[1], keep)
+        w.l2_out2[1] = self._conv(m.layer2_outconv2[3], None, keep)
+        w.l1_out = self._conv(m.layer1_outconv, None, keep)
+        w.l1_out2[0] = self._conv(m.layer1_outconv2[0], m.layer1_outconv2[1], keep)
+        w.l1_out2[1] = self._conv(m.layer1_outconv2[3], None, keep)
+        return w, keep
 
     @torch.no_grad()
     def __call__(self, images):
@@ -263,8 +271,12 @@ class _TokenState:
         self.cat_hi = torch.empty(rows, 2 * c, dtype=torch.float16, device=device)
         self.cat_lo = torch.empty(rows, 2 * c, dtype=torch.float16, device=device)
 
+    def sides(self, n, group_rows0, group_rows1):
+        """fp32 master as views of the two sets: [n, group_rows0, C], [n, group_rows1, C]."""
+        return self.x[: self.rows0].view(n, group_rows0, self.c), self.x[self.rows0:].view(n, group_rows1, self.c)
 
-class LocalFeatureTransformer(_PackedCacheMixin, nn.Module):
+
+class LocalFeatureTransformer(_PackedCache, nn.Module):
     """Interleaved self/cross encoder with linear or full (softmax) attention (reference transformer.py:61-101)."""
 
     def __init__(self, config):
@@ -278,55 +290,47 @@ class LocalFeatureTransformer(_PackedCacheMixin, nn.Module):
         for p in self.parameters():
             if p.dim() > 1:
                 nn.init.xavier_uniform_(p)
-        self._packed = None
-        self._packed_key = None
 
-    # -- weight packing: fp16 hi/lo planes of the [out, in] matrices, built lazily per device/version
-    def _pack(self, device):
-        key = (str(device),) + tuple(p._version for p in self.parameters()) + tuple(p.data_ptr() for p in self.parameters())
-        if self._packed is not None and self._packed_key == key:
-            return self._packed
+    # -- weight packing: fp16 hi/lo planes of the [out, in] matrices
+    def _build(self):
         keep = []
         arr = (_lib.LbEncoderLayerWeights * len(self.layers))()
-        with torch.no_grad():
-            for i, layer in enumerate(self.layers):
-                wqkv = torch.cat([layer.q_proj.weight, layer.k_proj.weight, layer.v_proj.weight], 0).float()
-                scaled = [split_weight(wqkv), split_weight(layer.merge.weight), split_weight(layer.mlp[0].weight),
-                          split_weight(layer.mlp[2].weight)]
-                planes = [(h, l) for h, l, _ in scaled]
-                lns = [layer.norm1.weight, layer.norm1.bias, layer.norm2.weight, layer.norm2.bias]
-                lns = [t.detach().float().contiguous() for t in lns]
-                w = arr[i]
-                c, d = self.d_model, self.d_model // self.nhead
-                if d == 32 and c == 256 and layer.attention == "linear":
-                    # fused k|v projection: k and v rows regrouped in blocks of 4 heads (128 rows)
-                    idx = torch.cat([torch.arange(c + blk * 128, c + blk * 128 + 128).repeat(1) if part == 0 else
-                                     torch.arange(2 * c + blk * 128, 2 * c + blk * 128 + 128)
-                                     for blk in range(c // 128) for part in (0, 1)]).to(planes[0][0].device)
-                    wkv = (planes[0][0][idx].contiguous(), planes[0][1][idx].contiguous())
-                    planes.append(wkv)
-                    w.wkv_hi, w.wkv_lo = wkv[0].data_ptr(), wkv[1].data_ptr()
-                keep.append((planes, lns))
-                (w.wqkv_hi, w.wqkv_lo), (w.wm_hi, w.wm_lo), (w.w1_hi, w.w1_lo), (w.w2_hi, w.w2_lo) = [
-                    (h.data_ptr(), l.data_ptr()) for h, l in planes[:4]]
-                w.ln1_g, w.ln1_b, w.ln2_g, w.ln2_b = [t.data_ptr() for t in lns]
-                w.s_qkv, w.s_m, w.s_1, w.s_2 = [sc for _, _, sc in scaled]
+        for i, layer in enumerate(self.layers):
+            wqkv = torch.cat([layer.q_proj.weight, layer.k_proj.weight, layer.v_proj.weight], 0).float()
+            scaled = [split_weight(wqkv), split_weight(layer.merge.weight), split_weight(layer.mlp[0].weight),
+                      split_weight(layer.mlp[2].weight)]
+            planes = [(h, l) for h, l, _ in scaled]
+            lns = [layer.norm1.weight, layer.norm1.bias, layer.norm2.weight, layer.norm2.bias]
+            lns = [t.detach().float().contiguous() for t in lns]
+            w = arr[i]
+            c, d = self.d_model, self.d_model // self.nhead
+            if d == 32 and c == 256 and layer.attention == "linear":
+                # fused k|v projection: k and v rows regrouped in blocks of 4 heads (128 rows)
+                idx = torch.cat([torch.arange(c + blk * 128, c + blk * 128 + 128).repeat(1) if part == 0 else
+                                 torch.arange(2 * c + blk * 128, 2 * c + blk * 128 + 128)
+                                 for blk in range(c // 128) for part in (0, 1)]).to(planes[0][0].device)
+                wkv = (planes[0][0][idx].contiguous(), planes[0][1][idx].contiguous())
+                planes.append(wkv)
+                w.wkv_hi, w.wkv_lo = wkv[0].data_ptr(), wkv[1].data_ptr()
+            keep.append((planes, lns))
+            (w.wqkv_hi, w.wqkv_lo), (w.wm_hi, w.wm_lo), (w.w1_hi, w.w1_lo), (w.w2_hi, w.w2_lo) = [
+                (h.data_ptr(), l.data_ptr()) for h, l in planes[:4]]
+            w.ln1_g, w.ln1_b, w.ln2_g, w.ln2_b = [t.data_ptr() for t in lns]
+            w.s_qkv, w.s_m, w.s_1, w.s_2 = [sc for _, _, sc in scaled]
         kinds = (C.c_int * len(self.layers))(*[_KIND[n, layer.attention] for n, layer in zip(self.layer_names,
                                                                                               self.layers)])
-        self._packed = (arr, kinds, keep)
-        self._packed_key = key
-        return self._packed
+        return arr, kinds, keep
 
     def run(self, state: _TokenState, n_groups, group_rows0, group_rows1, mask_u8=None, live=None):
         """In-place transformer over a prepared token state (used by LoFTR.forward).  `live` (fine windows only): an
         int32 device count; `n_groups` is then the capacity and only the first min(live, n_groups) windows of each set
         are computed."""
-        lib = _lib.load()
         if any(layer.attention == "full" for layer in self.layers):
-            _lib.require_full_attention(lib)   # an older library would reject the layer kinds at the first launch
-        arr, kinds, _ = self._pack(state.x.device)
+            _lib.require(_lib.FULL_ATTENTION_VERSION, "full attention")   # an older library rejects the layer kinds
+        lib = _lib.load()
         st = _lib.LbTransformerState(state.x.data_ptr(), state.cat_hi.data_ptr(), state.cat_lo.data_ptr(),
                                      _lib.ptr(mask_u8), n_groups, group_rows0, group_rows1, _lib.ptr(live))
+        arr, kinds, _ = self._pack()
         nbytes = lib.lb_transformer_workspace_bytes(self.d_model, self.nhead, n_groups, group_rows0, group_rows1)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=state.x.device)
         _lib.check(lib.lb_transformer_forward(arr, kinds, len(self.layers), self.d_model, self.nhead, C.byref(st),
@@ -397,52 +401,19 @@ class CoarseMatching(nn.Module):
             per_pair = min(per_pair, max_per_pair)
         return max(n * per_pair, 1)
 
-    def run(self, hi, lo, ld, n, L, S, c, data, mask_u8_0=None, mask_u8_1=None):
-        """Planes of feat_c0 (rows [0, n*L)) / feat_c1 (rows [n*L, ...)) -> coarse match keys in `data`."""
-        cap = self.default_capacity(n, L, S, mask_u8_0 is not None, self.max_matches_per_pair)
-        b_ids, i_ids, j_ids, mconf, mk0, mk1, count, conf = self._launch(hi, lo, ld, n, L, S, c, data, mask_u8_0,
-                                                                         mask_u8_1, cap)
-        dev = hi.device
-        m = int(count.item())  # the one host sync of the coarse stage (sizes the match list)
-        if m > cap:
-            raise RuntimeError(f"loftr_b200: {m} coarse matches exceed the buffer capacity {cap}")
-        b_ids, i_ids, j_ids, mconf, mk0, mk1 = b_ids[:m], i_ids[:m], j_ids[:m], mconf[:m], mk0[:m], mk1[:m]
-        data.update({"b_ids": b_ids, "i_ids": i_ids, "j_ids": j_ids})
-        if conf is not None:
-            data["conf_matrix"] = conf
-        if self.thr >= 0:  # conf > thr >= 0  =>  the reference's `mconf != 0` filter keeps everything
-            data.update({"gt_mask": torch.zeros(m, dtype=torch.bool, device=dev), "m_bids": b_ids,
-                         "mkpts0_c": mk0, "mkpts1_c": mk1, "mconf": mconf})
-        else:
-            nz = mconf != 0
-            data.update({"gt_mask": ~nz, "m_bids": b_ids[nz], "mkpts0_c": mk0[nz], "mkpts1_c": mk1[nz],
-                         "mconf": mconf[nz]})
-
-    def run_static(self, hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1, cap):
-        """`run` without the host sync: the match keys of `data` are the fixed-capacity buffers ([cap] first
-        dimension; entries at or past min(count, cap) unspecified) and the returned int32 device tensor [1] holds the
-        true count.  Requires thr >= 0 (the `mconf != 0` filter of thr < 0 would be a second, data-dependent list)."""
-        if self.thr < 0:
-            raise ValueError("forward_static needs match_coarse.thr >= 0: with thr < 0 the mconf != 0 filter makes the "
-                             "output list depend on the data")
-        b_ids, i_ids, j_ids, mconf, mk0, mk1, count, conf = self._launch(hi, lo, ld, n, L, S, c, data, mask_u8_0,
-                                                                         mask_u8_1, cap)
-        data.update({"b_ids": b_ids, "i_ids": i_ids, "j_ids": j_ids,
-                     "gt_mask": torch.zeros(cap, dtype=torch.bool, device=hi.device), "m_bids": b_ids,
-                     "mkpts0_c": mk0, "mkpts1_c": mk1, "mconf": mconf, "num_matches": count})
-        if conf is not None:
-            data["conf_matrix"] = conf
-        return count
-
-    def _launch(self, hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1, cap):
-        """Enqueues lb_coarse_match into buffers of `cap` entries -> (b_ids, i_ids, j_ids, mconf, mkpts0_c, mkpts1_c,
-        count, conf_matrix or None); no host sync."""
-        if self.training:
-            raise NotImplementedError("loftr_b200 builds the inference path only (no training-time sampling)")
-        lib = _lib.load()
+    def run(self, hi, lo, ld, n, L, S, c, data, mask_u8_0=None, mask_u8_1=None, static=False, capacity=None):
+        """Planes of feat_c0 (rows [0, n*L)) / feat_c1 (rows [n*L, ...)) -> coarse match keys in `data`.
+        Eager (static=False): the lists are trimmed to the match count, read with one host sync.
+        Static: no host sync; the match keys are buffers of `capacity` entries (default_capacity when None; entries at
+        or past min(count, capacity) unspecified) and data["num_matches"] is the int32 device count [1].  Static needs
+        thr >= 0, where the `mconf != 0` filter keeps every row.
+        -> the device count when static (the live bound of the fine stage), else None."""
+        _require_eval(self)
         k = self.max_matches_per_pair
         if k is not None:
-            _lib.require_match_cap(lib)
+            _lib.require(_lib.MATCH_CAP_VERSION, "match_coarse.max_matches_per_pair")
+        lib = _lib.load()
+        cap = int(capacity) if capacity is not None else self.default_capacity(n, L, S, mask_u8_0 is not None, k)
         dev = hi.device
         b_ids = torch.empty(cap, dtype=torch.int64, device=dev)
         i_ids = torch.empty(cap, dtype=torch.int64, device=dev)
@@ -485,7 +456,26 @@ class CoarseMatching(nn.Module):
             _lib.check(lib.lb_coarse_match(C.byref(a), ws.data_ptr(), nbytes, _stream(hi)))
         else:   # k >= L keeps every match; min() keeps the argument within a C int
             _lib.check(lib.lb_coarse_match_capped(C.byref(a), min(k, L), ws.data_ptr(), nbytes, _stream(hi)))
-        return b_ids, i_ids, j_ids, mconf, mk0, mk1, count, conf
+        m = cap
+        if not static:
+            m = int(count.item())  # the one host sync of the coarse stage (sizes the match list)
+            if m > cap:
+                raise RuntimeError(f"loftr_b200: {m} coarse matches exceed the buffer capacity {cap}")
+            b_ids, i_ids, j_ids, mconf, mk0, mk1 = b_ids[:m], i_ids[:m], j_ids[:m], mconf[:m], mk0[:m], mk1[:m]
+        data.update({"b_ids": b_ids, "i_ids": i_ids, "j_ids": j_ids})
+        if conf is not None:
+            data["conf_matrix"] = conf
+        if self.thr >= 0:  # conf > thr >= 0  =>  the reference's `mconf != 0` filter keeps everything
+            data.update({"gt_mask": torch.zeros(m, dtype=torch.bool, device=dev), "m_bids": b_ids,
+                         "mkpts0_c": mk0, "mkpts1_c": mk1, "mconf": mconf})
+        else:
+            nz = mconf != 0
+            data.update({"gt_mask": ~nz, "m_bids": b_ids[nz], "mkpts0_c": mk0[nz], "mkpts1_c": mk1[nz],
+                         "mconf": mconf[nz]})
+        if static:
+            data["num_matches"] = count
+            return count
+        return None
 
     @torch.no_grad()
     def forward(self, feat_c0, feat_c1, data, mask_c0=None, mask_c1=None):
@@ -500,7 +490,7 @@ class CoarseMatching(nn.Module):
         self.run(hi, lo, c, n, L, S, c, data, m0, m1)
 
 
-class FinePreprocess(_PackedCacheMixin, nn.Module):
+class FinePreprocess(_PackedCache, nn.Module):
     """Window gather + coarse-feature merge (reference fine_preprocess.py:7-59)."""
 
     def __init__(self, config):
@@ -518,26 +508,19 @@ class FinePreprocess(_PackedCacheMixin, nn.Module):
         for p in self.parameters():
             if p.dim() > 1:
                 nn.init.kaiming_normal_(p, mode="fan_out", nonlinearity="relu")
-        self._packed = None
-        self._packed_key = None
 
-    def _pack(self):
-        ps = list(self.parameters())
-        key = tuple(p._version for p in ps) + tuple(p.data_ptr() for p in ps)
-        if self._packed is None or self._packed_key != key:
-            with torch.no_grad():
-                wm = self.merge_feat.weight.detach().float().contiguous()
-                hi, lo, msc = split_weight(wm[:, : self.d_model_f])
-                self._packed = {"wdt": self.down_proj.weight.detach().float().t().contiguous(),
-                                "bd": self.down_proj.bias.detach().float().contiguous(),
-                                "wm2t": wm[:, self.d_model_f:].t().contiguous(),
-                                "bm": self.merge_feat.bias.detach().float().contiguous(),
-                                "wm_hi": hi, "wm_lo": lo, "wm_scale": msc}
-            self._packed_key = key
-        return self._packed
+    def _build(self):
+        wm = self.merge_feat.weight.detach().float().contiguous()
+        hi, lo, msc = split_weight(wm[:, : self.d_model_f])
+        return {"wdt": self.down_proj.weight.detach().float().t().contiguous(),
+                "bd": self.down_proj.bias.detach().float().contiguous(),
+                "wm2t": wm[:, self.d_model_f:].t().contiguous(),
+                "bm": self.merge_feat.bias.detach().float().contiguous(),
+                "wm_hi": hi, "wm_lo": lo, "wm_scale": msc}
 
     def run(self, feat_f0, feat_f1, feat_c_all, n, L, S, data, live=None, img_idx=None):
-        """-> _TokenState of the fine transformer (rows: side, match, window position), or None if M == 0.
+        """-> _TokenState of the fine transformer (rows: side, match, window position); with M == 0 it has no rows
+        and nothing is launched.  M is the length of data["b_ids"].
         `live`: int32 device count; the match keys of `data` are then capacity buffers and only windows below the
         count are gathered (rows keep the capacity layout side*cap*WW + m*WW + k).
         `img_idx`: (idx0, idx1) int32 device tensors [n]: feat_f0 / feat_f1 are then feature banks and pair b's
@@ -547,12 +530,12 @@ class FinePreprocess(_PackedCacheMixin, nn.Module):
         stride = data["hw0_f"][0] // data["hw0_c"][0]
         data.update({"W": W})
         m = int(data["b_ids"].shape[0])
-        if m == 0:
-            return None
-        p = self._pack()
         cf = self.d_model_f
         dev = feat_f0.device
         state = _TokenState(m * W * W, m * W * W, cf, dev)
+        if m == 0:
+            return state
+        p = self._pack()
         a = _lib.LbFinePreprocessArgs()
         a.feat_f0, a.feat_f1 = feat_f0.data_ptr(), feat_f1.data_ptr()
         a.sn0, a.sc0, a.sh0, a.sw0 = feat_f0.stride()
@@ -586,11 +569,7 @@ class FinePreprocess(_PackedCacheMixin, nn.Module):
         feat_c_all = torch.cat([feat_c0.reshape(n * L, cc), feat_c1.reshape(n * S, cc)], 0).float().contiguous()
         state = self.run(feat_f0.float(), feat_f1.float(), feat_c_all, n, L, S, data)
         ww = self.W ** 2
-        if state is None:
-            e = torch.empty(0, ww, self.d_model_f, device=feat_f0.device)
-            return e, e.clone()
-        m = state.rows0 // ww
-        return state.x[: m * ww].view(m, ww, -1), state.x[m * ww:].view(m, ww, -1)
+        return state.sides(state.rows0 // ww, ww, ww)
 
 
 class FineMatching(nn.Module):
@@ -676,40 +655,16 @@ class LoFTR(nn.Module):
         """Updates `data` in place with the reference's keys; returns None.
         Inputs: image0/image1 [N, 1, H, W] float32 (H, W divisible by 8), optional mask0/mask1 [N, H/8, W/8],
         optional scale0/scale1 [N, 2]."""
-        if self.training:
-            raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
+        _require_eval(self)
         _require_cuda(data["image0"], "image0")
-        self._match_and_refine(data, *self._coarse_features(data))
-
-    def _match_and_refine(self, data, state, feat_f0, feat_f1, bs, L, S, c, m0, m1, img_idx=None):
-        """Steps 3-5 of the forward over the coarse token state.  `img_idx` (int32 idx0, idx1): feat_f0 / feat_f1 are
-        feature banks, read at image idx0[b] / idx1[b] for pair b."""
-        # 3. coarse matching                                                           [loftr.py:67]
-        self.coarse_matching.run(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1)
-
-        # 4. fine-level refinement                                                     [loftr.py:70-72]
-        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, bs, L, S, data, img_idx=img_idx)
-        ww = self.fine_preprocess.W ** 2
-        if fstate is not None:
-            m = fstate.rows0 // ww
-            self.loftr_fine.run(fstate, m, ww, ww)
-            f0u, f1u = fstate.x[: m * ww].view(m, ww, -1), fstate.x[m * ww:].view(m, ww, -1)
-        else:
-            f0u = torch.empty(0, ww, self.fine_preprocess.d_model_f, device=feat_f0.device)
-            f1u = f0u.clone()
-
-        # 5. fine matching                                                             [loftr.py:75]
-        self.fine_matching(f0u, f1u, data)
-        if self.expose_coarse_features:   # test / debugging tap, off by default: not a reference key
-            data["_feat_c0"], data["_feat_c1"] = state.x[: bs * L].view(bs, L, c), state.x[bs * L:].view(bs, S, c)
+        self._match_pairs(data, *self._backbone_pairs(data))
 
     @torch.no_grad()
     def extract_features(self, images, masks=None) -> "ImageFeatures":
         """Runs the configured backbone once on images [K, 1, H, W] (CUDA) -> ImageFeatures, a per-image feature bank
         for `match_features`.  masks: optional [K, H/8, W/8] padding masks (as forward's mask0 / mask1), stored with
         the bank.  Position encoding and the transformers are not applied: they depend on the pair."""
-        if self.training:
-            raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
+        _require_eval(self)
         _require_cuda(images, "images")
         if images.dim() != 4 or images.shape[1] != 1:
             raise ValueError(f"extract_features: images must be [K, 1, H, W] (got {tuple(images.shape)})")
@@ -735,9 +690,8 @@ class LoFTR(nn.Module):
         the outputs of a forward with no matches.  scale0 / scale1: optional [K0, 2] / [K1, 2] per-image scales of
         feats0 / feats1 (both or neither).  A bank is tied to the backbone weights it was extracted with: after
         load_state_dict, .to() or a parameter update it raises; extract again."""
-        if self.training:
-            raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
-        _lib.require_feature_bank(_lib.load())
+        _require_eval(self)
+        _lib.require(_lib.FEATURE_BANK_VERSION, "match_features")
         key = self._bank_key()
         dev = next(self.parameters()).device
         for name, f in (("feats0", feats0), ("feats1", feats1)):
@@ -765,8 +719,7 @@ class LoFTR(nn.Module):
                 work[name] = s.to(dev)[idx.long()]
         work.update({"bs": bs, "hw0_i": feats0.hw_i, "hw1_i": feats1.hw_i, "hw0_c": feats0.hw_c, "hw1_c": feats1.hw_c,
                      "hw0_f": feats0.hw_f, "hw1_f": feats1.hw_f})
-        state, L, S, c, m0, m1 = self._coarse_transformer(work, feats0.feat_c, feats1.feat_c, bs, idx0, idx1)
-        self._match_and_refine(work, state, feats0.feat_f, feats1.feat_f, bs, L, S, c, m0, m1, img_idx=(idx0, idx1))
+        self._match_pairs(work, feats0.feat_c, feats1.feat_c, feats0.feat_f, feats1.feat_f, img_idx=(idx0, idx1))
         out = {} if data is None else data
         out.update({k: v for k, v in work.items() if k not in ("mask0", "mask1", "scale0", "scale1")})
         return out
@@ -790,8 +743,7 @@ class LoFTR(nn.Module):
 
     def _bank_key(self):
         """What a feature bank depends on: the backbone implementation and its tensors' (data_ptr, _version)."""
-        tensors = list(self.backbone.parameters()) + list(self.backbone.buffers())
-        return (self.backbone_impl,) + _tensor_key(tensors)
+        return (self.backbone_impl,) + _weights_key(self.backbone)
 
     def _backbone(self, images):
         """The configured backbone on [N, 1, H, W] -> (feat_c, feat_f) as [N, C, h, w]; NHWC storage (channels-last
@@ -819,13 +771,7 @@ class LoFTR(nn.Module):
         overflows.
 
         Configurations whose output list depends on the data (match_coarse.thr < 0) raise ValueError."""
-        if self.training:
-            raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
-        if self.coarse_matching.thr < 0:
-            raise ValueError("forward_static needs match_coarse.thr >= 0: with thr < 0 the reference's mconf != 0 "
-                             "filter makes the output list depend on the data")
-        if capacity is not None and int(capacity) < 1:
-            raise ValueError(f"capacity must be a positive number of matches (got {capacity})")
+        _require_static(self, capacity, "forward_static")
         dev = None
         for k in ("image0", "image1", "mask0", "mask1", "scale0", "scale1"):
             if k not in data:
@@ -838,27 +784,11 @@ class LoFTR(nn.Module):
                 dev = t.device
             elif t.device != dev:
                 raise ValueError(f"forward_static: `{k}` is on {t.device}, image0 on {dev}")
-        state, feat_f0, feat_f1, bs, L, S, c, m0, m1 = self._coarse_features(data)
-        cap = int(capacity) if capacity is not None else self.coarse_matching.default_capacity(
-            bs, L, S, m0 is not None, self.coarse_matching.max_matches_per_pair)
+        self._match_pairs(data, *self._backbone_pairs(data), static=True, capacity=capacity)
 
-        # 3. coarse matching into capacity buffers; `count` stays on the device
-        count = self.coarse_matching.run_static(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1, cap)
-
-        # 4. fine-level refinement over the capacity layout, bounded on the device by `count`
-        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, bs, L, S, data, live=count)
-        ww = self.fine_preprocess.W ** 2
-        self.loftr_fine.run(fstate, cap, ww, ww, live=count)
-        f0u, f1u = fstate.x[: cap * ww].view(cap, ww, -1), fstate.x[cap * ww:].view(cap, ww, -1)
-
-        # 5. fine matching
-        self.fine_matching(f0u, f1u, data, live=count)
-        if self.expose_coarse_features:
-            data["_feat_c0"], data["_feat_c1"] = state.x[: bs * L].view(bs, L, c), state.x[bs * L:].view(bs, S, c)
-
-    def _coarse_features(self, data):
-        """Steps 1-2 of the forward (no host sync): backbone, position encoding and coarse transformer.
-        -> (coarse token state, feat_f0, feat_f1, n, L, S, C, mask0 u8, mask1 u8)."""
+    def _backbone_pairs(self, data):
+        """Step 1 of the forward (no host sync): the backbone on image0 / image1 -> (feat_c0, feat_c1, feat_f0,
+        feat_f1); writes bs and the image, coarse and fine sizes into `data`."""
         img0, img1 = data["image0"], data["image1"]
         bs = img0.size(0)
         data.update({"bs": bs, "hw0_i": img0.shape[2:], "hw1_i": img1.shape[2:]})
@@ -871,15 +801,17 @@ class LoFTR(nn.Module):
             (feat_c0, feat_f0), (feat_c1, feat_f1) = self._backbone(img0), self._backbone(img1)
         data.update({"hw0_c": feat_c0.shape[2:], "hw1_c": feat_c1.shape[2:],
                      "hw0_f": feat_f0.shape[2:], "hw1_f": feat_f1.shape[2:]})
-        state, L, S, c, m0, m1 = self._coarse_transformer(data, feat_c0, feat_c1, bs)
-        return state, feat_f0, feat_f1, bs, L, S, c, m0, m1
+        return feat_c0, feat_c1, feat_f0, feat_f1
 
-    def _coarse_transformer(self, data, feat_c0, feat_c1, bs, idx0=None, idx1=None):
-        """Step 2 of the forward (no host sync): position encoding, token layout and coarse transformer of `bs` pairs.
-        idx0 / idx1 (int32 [bs], both or neither): feat_c0 / feat_c1 are feature banks, read at image idx0[b] /
-        idx1[b] for pair b.  -> (coarse token state, L, S, C, mask0 u8, mask1 u8)."""
+    def _match_pairs(self, data, feat_c0, feat_c1, feat_f0, feat_f1, img_idx=None, static=False, capacity=None):
+        """Steps 2-5 of the forward for the data["bs"] pairs whose sizes `data` holds: position encoding and token
+        layout, coarse transformer, coarse matching, fine preprocess and transformer, fine matching.
+        img_idx: optional (idx0, idx1) int32 [bs]: the maps are then feature banks, read at image idx0[b] / idx1[b] for
+        pair b.  static: the match keys are buffers of `capacity` entries (None: the default capacity) and the fine
+        stage is bounded on the device by their count (CoarseMatching.run), so that nothing synchronises with the host."""
         # 2. position encoding + token layout + coarse transformer                     [loftr.py:58-64]
         lib = _lib.load()
+        bs = data["bs"]
         nhwc = self._tc_backbone is not None
         c = feat_c0.shape[1]
         (h0, w0), (h1, w1) = data["hw0_c"], data["hw1_c"]
@@ -887,6 +819,7 @@ class LoFTR(nn.Module):
         state = _TokenState(bs * L, bs * S, c, feat_c0.device)
         pe = self.pos_encoding.pe[0]
         st = _stream(feat_c0)
+        idx0, idx1 = (None, None) if img_idx is None else img_idx
         for feat, idx, h, w, row0 in ((feat_c0, idx0, h0, w0, 0), (feat_c1, idx1, h1, w1, bs * L)):
             feat = feat.float()
             feat = feat.permute(0, 2, 3, 1).contiguous() if nhwc else feat.contiguous()   # no copy in either case
@@ -905,16 +838,31 @@ class LoFTR(nn.Module):
             mask_all = torch.cat([m0, m1]).contiguous()
             m0, m1 = mask_all[: bs * L], mask_all[bs * L:]
         self.loftr_coarse.run(state, bs, L, S, mask_all)
-        return state, L, S, c, m0, m1
+
+        # 3. coarse matching                                                           [loftr.py:67]
+        live = self.coarse_matching.run(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1, static, capacity)
+
+        # 4. fine-level refinement over M windows: the match count, or the capacity    [loftr.py:70-72]
+        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, bs, L, S, data, live, img_idx)
+        m, ww = data["b_ids"].shape[0], self.fine_preprocess.W ** 2
+        if m:
+            self.loftr_fine.run(fstate, m, ww, ww, live=live)
+
+        # 5. fine matching                                                             [loftr.py:75]
+        self.fine_matching(*fstate.sides(m, ww, ww), data, live=live)
+        if self.expose_coarse_features:   # test / debugging tap, off by default: not a reference key
+            data["_feat_c0"], data["_feat_c1"] = state.sides(bs, L, S)
+
+    def _packed_caches(self):
+        """Every owner of a packed-weight cache: the caching submodules and the tensor-core backbone."""
+        caches = [m for m in self.modules() if isinstance(m, _PackedCache)]
+        return caches if self._tc_backbone is None else caches + [self._tc_backbone]
 
     def invalidate_packed(self):
         """Drop every packed-weight cache (fp16 hi/lo planes, folded BatchNorm): required after parameter writes
         that PyTorch cannot see (`.data` mutation); implied by load_state_dict / .to() / .cuda() / .float()."""
-        for m in self.modules():
-            if m is not self and hasattr(m, "invalidate_packed"):
-                m.invalidate_packed()
-        if self._tc_backbone is not None:
-            self._tc_backbone.invalidate_packed()
+        for m in self._packed_caches():
+            m.invalidate_packed()
 
     def _apply(self, fn, *args, **kwargs):
         self.invalidate_packed()
@@ -929,20 +877,21 @@ class LoFTR(nn.Module):
         return super().load_state_dict(state_dict, *args, **kwargs)
 
 
+def _require_static(model, capacity, what):
+    """Preconditions of the sync-free forward (`what`: the public entry point), checked before any launch."""
+    _require_eval(model)
+    if model.coarse_matching.thr < 0:
+        raise ValueError(f"{what} needs match_coarse.thr >= 0: with thr < 0 the reference's mconf != 0 filter makes "
+                         "the output list depend on the data")
+    if capacity is not None and int(capacity) < 1:
+        raise ValueError(f"capacity must be a positive number of matches (got {capacity})")
+
+
 def _weight_refs(model):
     """(packed-weight cache objects, parameters + buffers, their (data_ptr, _version) key) of `model`: everything a
     captured graph holds raw device pointers into."""
-    caches = [model.loftr_coarse._packed, model.loftr_fine._packed, model.fine_preprocess._packed]
-    if model._tc_backbone is not None:
-        caches.append(model._tc_backbone._packed)
-    tensors = list(model.parameters()) + list(model.buffers())
-    return caches, tensors, _tensor_key(tensors)
-
-
-def _tensor_key(tensors):
-    """(data_ptr, _version) of every tensor: changes when one is replaced, moved or modified in place (not through
-    `.data`)."""
-    return tuple((t.data_ptr(), t._version) for t in tensors)
+    caches = [m._packed for m in model._packed_caches()]
+    return caches, list(model.parameters()) + list(model.buffers()), _weights_key(model)
 
 
 class ImageFeatures:
@@ -983,13 +932,7 @@ class CapturedMatcher:
     _TRIMMED = ("b_ids", "i_ids", "j_ids", "gt_mask", "mconf", "mkpts0_c", "mkpts1_c", "mkpts1_f", "expec_f")
 
     def __init__(self, model, batch, hw0, hw1=None, masks=False, scales=False, capacity=None):
-        if model.training:
-            raise NotImplementedError("loftr_b200 builds the inference path only: call .eval()")
-        if model.coarse_matching.thr < 0:
-            raise ValueError("CapturedMatcher needs match_coarse.thr >= 0: with thr < 0 the reference's mconf != 0 "
-                             "filter makes the output list depend on the data")
-        if capacity is not None and int(capacity) < 1:
-            raise ValueError(f"capacity must be a positive number of matches (got {capacity})")
+        _require_static(model, capacity, "CapturedMatcher")
         dev = next(model.parameters()).device
         if dev.type != "cuda":
             raise ValueError("CapturedMatcher: the model must live on a CUDA (H100) device; call .cuda() first")

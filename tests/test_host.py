@@ -106,7 +106,7 @@ def test_model_with_packed_caches_deepcopies_and_pickles():
     arr = (_lib.LbEncoderLayerWeights * 2)()
     model.loftr_coarse._packed, model.loftr_coarse._packed_key = (arr, None, []), ("k",)
     model.fine_preprocess._packed, model.fine_preprocess._packed_key = {"x": arr}, ("k",)
-    model._tc_backbone._packed, model._tc_backbone._key = (_lib.LbBackboneWeights(), []), ("k",)
+    model._tc_backbone._packed, model._tc_backbone._packed_key = (_lib.LbBackboneWeights(), []), ("k",)
     c = copy.deepcopy(model)
     p = pickle.loads(pickle.dumps(model))
     for m in (c, p):
