@@ -6,11 +6,14 @@
 // shifted shared-memory descriptors over it; only the weights stream through the per-tap pipeline ring.
 //
 // Halo layout (wgmma no-swizzle K-major core matrices): [8-channel chunk][halo pixel (row-major, 18 wide)][16 bytes].
-// An m64 instruction covers output rows y = 0..7 of the tile's x-half mh; for tap (ky, kx) its 8-row group y is the
-// 8 consecutive halo pixels from (y + ky) * 18 + 8 * mh + kx -- one 128-byte core matrix -- so
-//   start = ((ky * 18) + 8 * mh + kx) * 16,   SBO = 18 * 16 (next y),   LBO = chunk stride (next 8 channels along K),
-// and k-step k of a 64-channel block starts 2k chunks further.  Row r of instruction mh is therefore tile pixel
-// (r / 8) * 16 + 8 * mh + r % 8; the accumulator is staged row-major by pixel, exactly as gemm_split_kernel stages it,
+// Consumer warpgroup h computes x-half h of the 8 x 16 tile (output rows y = 0..7, columns x = 8h..8h+7) over all
+// BLOCK_N channels: one m64nBLOCK_Nk16 instruction per product and k-step, so each A core matrix is read by one
+// warpgroup and a 196-channel output runs as a 200-wide tile (200 / 2 is no wgmma N).  For tap (ky, kx) the
+// instruction's 8-row group y is the 8 consecutive halo pixels from (y + ky) * 18 + 8 * h + kx -- one 128-byte core
+// matrix -- so
+//   start = ((ky * 18) + 8 * h + kx) * 16,   SBO = 18 * 16 (next y),   LBO = chunk stride (next 8 channels along K),
+// and k-step k of a 64-channel block starts 2k chunks further.  Row r of warpgroup h is therefore tile pixel
+// (r / 8) * 16 + 8 * h + r % 8; the accumulator is staged row-major by pixel, exactly as gemm_split_kernel stages it,
 // so the epilogue (EpiConv) is unchanged.
 //
 // Each halo plane is loaded as eight 8-channel boxes of a 4-D NHWC map whose channel extent is Cin: TMA zero-fills
@@ -41,7 +44,10 @@ static_assert(kHaloW * kHaloH * 16 <= kHaloChunkBytes && kHaloChunkBytes % 128 =
 
 // Shared memory: [weight ring | two halo slots (accumulator staging aliases both)][epilogue area][mbarriers].
 // A weight stage is one tap of a 64-channel block (kBK = 64, 128-byte swizzle rows) when three of them fit beside the
-// halo slots, else half a tap (kBK = 32, 64-byte swizzle rows): three or more stages in flight at every N.
+// halo slots, else half a tap (kBK = 32, 64-byte swizzle rows): three or more stages in flight at every N.  N = 200
+// gets four stages of 25,600 bytes because EpiConv<200> shares the residual transposer with the TMA-store staging
+// (EpiConv::kOwnXpose): its own transposer would take the fourth stage, and three stages made the 196-channel
+// layers 13-14 % slower on an H100 at 700 W.
 template <int BLOCK_N, int kEpiBytes>
 struct HaloSmem {
   static constexpr int kBarBytes = 256;
@@ -78,12 +84,11 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
                     const __grid_constant__ CUtensorMap tm_br_hi, const __grid_constant__ CUtensorMap tm_br_lo,
                     const GemmShape shape, const __grid_constant__ typename Epi::Params epi_params) {
   using S = HaloSmem<BLOCK_N, Epi::kSmemBytes>;
-  constexpr int kN = BLOCK_N / 2;
   constexpr int kBK = S::kBK;
   constexpr int kSubs = kBlockK / kBK;                       // weight stages per (tap, 64-channel block)
   constexpr int kRemBTile = BLOCK_N * kRemChannels * 2;      // per plane
   constexpr bool kStagingInRing = S::kAccBytes <= S::kRingBytes;   // N = 128: the halo slots stay free at the tile end
-  static_assert(kN % 8 == 0, "wgmma N must be a multiple of 8");
+  static_assert(BLOCK_N % 8 == 0 && BLOCK_N <= 256, "one wgmma spans the tile: N a multiple of 8, at most 256");
   static_assert(2 * kRemBTile <= S::kStageBytes && kRemBTile % 256 == 0, "remainder weight stage");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* ring = smem_raw;
@@ -209,10 +214,10 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
   } else {
     // ------------------------------------------------------------ consumer warpgroups: wgmma + epilogue
     const int ct = threadIdx.x - kEpiWarp0 * 32;
-    const int h = ct >> 7;
+    const int h = (warp - kEpiWarp0) >> 2;   // == ct >> 7, from the shuffled warp index: the compiler sees it uniform
     const int wt = ct & 127;
     Epi epi(epi_params, epi_smem, shape);
-    float acc[2][kN / 2];                           // x-half mh of the tile, this warpgroup's column half
+    float acc[BLOCK_N / 2];                         // x-half h of the tile, all BLOCK_N columns
     float* stg = reinterpret_cast<float*>(ring);
     const uint32_t ring_u32 = smem_u32(ring);
     const uint32_t halo_u32 = smem_u32(halo);
@@ -229,7 +234,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
       for (int nt = nt_begin; nt < nt_end; ++nt) {
         epi.prefetch(batch, mt * kBlockM, nt * BLOCK_N);
 #pragma unroll
-        for (int i = 0; i < kN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
+        for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
         int prev = -1;        // ring stage of the previous weight stage
         int prev_halo = -1;   // halo slot whose last tap was the previous weight stage, else -1
         for (int s = 0; s < n_steps; ++s) {
@@ -239,45 +244,35 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
           const int hi = halos + hh, slot = hi & 1;
           if (tap == 0) mbar_wait(&halo_full[slot], (hi >> 1) & 1);
           const int ky = tap / 3, kx = tap - ky * 3;
-          // halo pixel of row group y = 0 of x-half 0 for this tap
-          const uint32_t a_tap = halo_u32 + slot * kHaloSlotBytes + (ky * kHaloW + kx) * 16;
+          // halo pixel of row group y = 0 of x-half h for this tap
+          const uint32_t a_tap = halo_u32 + slot * kHaloSlotBytes + (ky * kHaloW + kx) * 16 + h * 8 * 16;
           const int subs = rem ? 1 : kSubs;
           for (int j = 0; j < subs; ++j) {
             mbar_wait(&full_bar[stage], phase);
             const uint32_t st = ring_u32 + stage * S::kStageBytes;
             wgmma_fence();
             if (rem) {
-              const uint32_t b_off = static_cast<uint32_t>(h * kN * kRemChannels * 2);
-              const uint64_t rb_hi = wgmma_desc_k_sw32(st + b_off);
-              const uint64_t rb_lo = wgmma_desc_k_sw32(st + kRemBTile + b_off);
-#pragma unroll
-              for (int mh = 0; mh < 2; ++mh) {
-                const uint32_t a = a_tap + mh * 8 * 16;
-                const uint64_t ra_hi = wgmma_desc_k_noswz(a, kHaloChunkBytes, kHaloW * 16);
-                const uint64_t ra_lo = wgmma_desc_k_noswz(a + kHaloPlaneBytes, kHaloChunkBytes, kHaloW * 16);
-                wgmma_f16<kN>(acc[mh], ra_hi, rb_hi, 1u);
-                wgmma_f16<kN>(acc[mh], ra_hi, rb_lo, 1u);
-                wgmma_f16<kN>(acc[mh], ra_lo, rb_hi, 1u);
-              }
+              const uint64_t rb_hi = wgmma_desc_k_sw32(st);
+              const uint64_t rb_lo = wgmma_desc_k_sw32(st + kRemBTile);
+              const uint64_t ra_hi = wgmma_desc_k_noswz(a_tap, kHaloChunkBytes, kHaloW * 16);
+              const uint64_t ra_lo = wgmma_desc_k_noswz(a_tap + kHaloPlaneBytes, kHaloChunkBytes, kHaloW * 16);
+              wgmma_f16<BLOCK_N>(acc, ra_hi, rb_hi, 1u);
+              wgmma_f16<BLOCK_N>(acc, ra_hi, rb_lo, 1u);
+              wgmma_f16<BLOCK_N>(acc, ra_lo, rb_hi, 1u);
             } else {
-              const uint32_t b_off = static_cast<uint32_t>(h * kN * kBK * 2);
-              const uint64_t db_hi = kBK == 64 ? wgmma_desc_k_sw128(st + b_off) : wgmma_desc_k_sw64(st + b_off);
-              const uint64_t db_lo =
-                  kBK == 64 ? wgmma_desc_k_sw128(st + S::kBTile + b_off) : wgmma_desc_k_sw64(st + S::kBTile + b_off);
+              const uint64_t db_hi = kBK == 64 ? wgmma_desc_k_sw128(st) : wgmma_desc_k_sw64(st);
+              const uint64_t db_lo = kBK == 64 ? wgmma_desc_k_sw128(st + S::kBTile) : wgmma_desc_k_sw64(st + S::kBTile);
+              const uint32_t a = a_tap + j * (kBK / kMmaK) * 2 * kHaloChunkBytes;
+              const uint64_t da_hi = wgmma_desc_k_noswz(a, kHaloChunkBytes, kHaloW * 16);
+              const uint64_t da_lo = wgmma_desc_k_noswz(a + kHaloPlaneBytes, kHaloChunkBytes, kHaloW * 16);
 #pragma unroll
-              for (int mh = 0; mh < 2; ++mh) {
-                const uint32_t a = a_tap + mh * 8 * 16 + j * (kBK / kMmaK) * 2 * kHaloChunkBytes;
-                const uint64_t da_hi = wgmma_desc_k_noswz(a, kHaloChunkBytes, kHaloW * 16);
-                const uint64_t da_lo = wgmma_desc_k_noswz(a + kHaloPlaneBytes, kHaloChunkBytes, kHaloW * 16);
-#pragma unroll
-                for (int k = 0; k < kBK / kMmaK; ++k) {
-                  // A: 16 channels = two chunks further; B: 32 bytes further inside the swizzle row (16-byte units)
-                  const uint64_t a_adv = static_cast<uint64_t>(k * 2 * kHaloChunkBytes / 16);
-                  const uint64_t b_adv = static_cast<uint64_t>(k * 2);
-                  wgmma_f16<kN>(acc[mh], da_hi + a_adv, db_hi + b_adv, 1u);
-                  wgmma_f16<kN>(acc[mh], da_hi + a_adv, db_lo + b_adv, 1u);
-                  wgmma_f16<kN>(acc[mh], da_lo + a_adv, db_hi + b_adv, 1u);
-                }
+              for (int k = 0; k < kBK / kMmaK; ++k) {
+                // A: 16 channels = two chunks further; B: 32 bytes further inside the swizzle row (16-byte units)
+                const uint64_t a_adv = static_cast<uint64_t>(k * 2 * kHaloChunkBytes / 16);
+                const uint64_t b_adv = static_cast<uint64_t>(k * 2);
+                wgmma_f16<BLOCK_N>(acc, da_hi + a_adv, db_hi + b_adv, 1u);
+                wgmma_f16<BLOCK_N>(acc, da_hi + a_adv, db_lo + b_adv, 1u);
+                wgmma_f16<BLOCK_N>(acc, da_lo + a_adv, db_hi + b_adv, 1u);
               }
             }
             wgmma_commit();
@@ -294,23 +289,19 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
         }
         halos += n_halo;
         wgmma_wait<0>();
-        wgmma_fence_regs(acc[0]);
-        wgmma_fence_regs(acc[1]);
+        wgmma_fence_regs(acc);
         mbar_arrive(&empty_bar[prev]);
         if (prev_halo >= 0) mbar_arrive(&halo_empty[prev_halo]);
-        // ---- stage the accumulator by tile pixel: row r of instruction mh is pixel (r / 8) * 16 + 8 * mh + r % 8
+        // ---- stage the accumulator by tile pixel: row r of warpgroup h is pixel (r / 8) * 16 + 8 * h + r % 8
         epi_group_sync();
         {
-          const int p0 = 32 * (wt >> 5) + ((wt & 31) >> 2);
-          const int c0 = h * kN + 2 * (wt & 3);
+          const int p0 = 32 * (wt >> 5) + 8 * h + ((wt & 31) >> 2);
+          const int c0 = 2 * (wt & 3);
 #pragma unroll
-          for (int mh = 0; mh < 2; ++mh) {
-#pragma unroll
-            for (int j = 0; j < kN / 8; ++j) {
-              float* p = stg + (p0 + 8 * mh) * S::kAccStride + c0 + 8 * j;
-              *reinterpret_cast<float2*>(p) = make_float2(acc[mh][4 * j], acc[mh][4 * j + 1]);
-              *reinterpret_cast<float2*>(p + 16 * S::kAccStride) = make_float2(acc[mh][4 * j + 2], acc[mh][4 * j + 3]);
-            }
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            float* p = stg + p0 * S::kAccStride + c0 + 8 * j;
+            *reinterpret_cast<float2*>(p) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(p + 16 * S::kAccStride) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
           }
         }
         epi_group_sync();

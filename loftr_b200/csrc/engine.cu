@@ -655,10 +655,16 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
 #define LB_CONV_CASE(BN)                                                                                              \
   {                                                                                                                   \
     if (r.up) LB_CONV_CASE_UP(BN, true, launch_conv<BN, true>)                                                        \
-    if (halo) LB_CONV_CASE_UP(BN, false, launch_conv_halo<BN>)                                                        \
     LB_CONV_CASE_UP(BN, false, launch_conv<BN, false>)                                                                \
   }
-  // output-channel tile: the smallest built N that covers Cout (196 -> 208: 13 x 16, no MMAs on 60 padding columns)
+  // output-channel tile: the smallest built N that covers Cout.  196 -> 200 in the halo kernel (one m64n200 wgmma per
+  // x-half); 208 in gemm_split_kernel, whose two column halves need N / 2 to be a wgmma N (104 = 13 x 8)
+  if (halo) {
+    if (w.cout <= 128) LB_CONV_CASE_UP(128, false, launch_conv_halo<128>)
+    if (w.cout <= 200) LB_CONV_CASE_UP(200, false, launch_conv_halo<200>)
+    if (w.cout <= 256) LB_CONV_CASE_UP(256, false, launch_conv_halo<256>)
+    return fail("convolutions with more than 256 output channels are not built");
+  }
   if (w.cout <= 128) LB_CONV_CASE(128)
   if (w.cout <= 208) LB_CONV_CASE(208)
   if (w.cout <= 256) LB_CONV_CASE(256)

@@ -2,12 +2,14 @@
 """Per-launch times of the backbone of one bench.py step (8 pairs = 16 images of 640x480 through lb_backbone_forward),
 taken with torch.profiler (CUDA activities) in a run of their own after warm-up:
     python tools/conv_bench.py [--batch 8] [--h 480] [--w 640] [--reps 5]
-One row per launch in execution order: median us over --reps profiled forwards, issued GFLOP (3 products x k-steps x
-N tile, from shapes), issued TFLOP/s, and the L2 -> shared-memory operand bytes of one launch, computed from shapes, for
+One row per launch in execution order: the output-channel tile N the launch ran with (read from the kernel's name),
+median us over --reps profiled forwards, issued GFLOP (3 products x k-steps x N tile, from shapes), issued TFLOP/s,
+and the L2 -> shared-memory operand bytes of one launch, computed from shapes, for
 the per-tap patch loads of gemm_split_kernel ("tap") and the once-per-channel-block halo of conv3x3_halo_kernel
 ("halo"; weights still per tap).  The halo column is filled for the stride-1 3x3 layers only."""
 import argparse
 import os
+import re
 import statistics
 import sys
 
@@ -32,9 +34,8 @@ LAYERS = [
     ("layer1_outconv2.3", 196, 128, 3, 1, 2)]
 
 
-def layer_counts(cin, cout, k, s, div, n, h, w):
-    """(issued GFLOP, per-tap bytes, halo bytes or None) of one launch."""
-    bn = 128 if cout <= 128 else 208 if cout <= 208 else 256
+def layer_counts(cin, cout, k, s, div, n, h, w, bn):
+    """(issued GFLOP, per-tap bytes, halo bytes or None) of one launch with output-channel tile bn."""
     cb, rem = (cin // 64, cin % 64) if cin > 64 and 0 < cin % 64 <= 16 else ((cin + 63) // 64, 0)
     hin, win = h // div, w // div
     ho, wo = (hin + 2 * (k // 2) - k) // s + 1, (win + 2 * (k // 2) - k) // s + 1
@@ -76,24 +77,27 @@ def main():
               and ("EpiConv" in e.name or "conv_stem" in e.name)]
         ev.sort(key=lambda e: e.time_range.start)
         per_rep.append([e.time_range.elapsed_us() for e in ev])
+        # output-channel tile of each EpiConv launch: the BLOCK_N template argument in the (de)mangled kernel name
+        tiles_n = [int(m.group(1)) for m in (re.search(r"EpiConv(?:<|ILi)(\d+)", e.name) for e in ev) if m]
     counts = {len(r) for r in per_rep}
-    if counts != {len(LAYERS) + 1}:
-        sys.exit(f"expected {len(LAYERS) + 1} backbone launches per forward, got {sorted(counts)}")
+    if counts != {len(LAYERS) + 1} or len(tiles_n) != len(LAYERS):
+        sys.exit(f"expected {len(LAYERS) + 1} backbone launches per forward ({len(LAYERS)} named EpiConv<N>), got "
+                 f"{sorted(counts)} ({len(tiles_n)})")
     us = [statistics.median(r[i] for r in per_rep) for i in range(len(LAYERS) + 1)]
     print(f"# {torch.cuda.get_device_name()}, {n} images {args.h}x{args.w}, median of {args.reps} profiled forwards")
-    print("| layer | us | issued GFLOP | issued TFLOP/s | L2->smem MB (tap) | L2->smem MB (halo) |")
-    print("|---|---|---|---|---|---|")
-    print(f"| stem 7x7 s2 | {us[0]:.0f} | - | - | - | - |")
+    print("| layer | N tile | us | issued GFLOP | issued TFLOP/s | L2->smem MB (tap) | L2->smem MB (halo) |")
+    print("|---|---|---|---|---|---|---|")
+    print(f"| stem 7x7 s2 | - | {us[0]:.0f} | - | - | - | - |")
     tot, tot_s1 = us[0], 0.0
-    for (name, cin, cout, k, s, div), t in zip(LAYERS, us[1:]):
-        gf, tb, hb = layer_counts(cin, cout, k, s, div, n, args.h, args.w)
+    for (name, cin, cout, k, s, div), bn, t in zip(LAYERS, tiles_n, us[1:]):
+        gf, tb, hb = layer_counts(cin, cout, k, s, div, n, args.h, args.w, bn)
         tot += t
         if hb is not None:
             tot_s1 += t
-        print(f"| {name} | {t:.0f} | {gf:.0f} | {gf / t * 1e3:.0f} | {tb / 1e6:.0f} | "
+        print(f"| {name} | {bn} | {t:.0f} | {gf:.0f} | {gf / t * 1e3:.0f} | {tb / 1e6:.0f} | "
               f"{'-' if hb is None else f'{hb / 1e6:.0f}'} |")
-    print(f"| **all launches** | **{tot:.0f}** | | | | |")
-    print(f"| **stride-1 3x3 only** | **{tot_s1:.0f}** | | | | |")
+    print(f"| **all launches** | | **{tot:.0f}** | | | | |")
+    print(f"| **stride-1 3x3 only** | | **{tot_s1:.0f}** | | | | |")
 
 
 if __name__ == "__main__":
