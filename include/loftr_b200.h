@@ -4,6 +4,8 @@
  * Every entry point replaces one `forward` of the reference (zju3dv/LoFTR, paths relative to the
  * reference root) and is what a binding from the reference side would call:
  *
+ *   lb_preprocess_images      <- read_megadepth_gray / read_scannet_gray    src/utils/dataset.py:94-125,141-157,
+ *                                (grey, resize, pad, / 255) + the 1/8 mask    src/datasets/megadepth.py:119-125
  *   lb_coarse_prep            <- PositionEncodingSine.forward + rearrange   src/loftr/utils/position_encoding.py:37-42,
  *                                                                           src/loftr/loftr.py:58-59
  *                                (lb_coarse_prep_indexed / lb_fine_preprocess_indexed: the same stages reading the
@@ -49,7 +51,8 @@ extern "C" {
 /* 101: device-count fields appended to LbTransformerState / LbFinePreprocessArgs / LbFineMatchArgs;
  * 102: full-attention layer kinds; 103: lb_selftest removed (no structure changes);
  * 104: lb_coarse_prep_indexed / lb_fine_preprocess_indexed (pairs read from a per-image feature bank);
- * 105: lb_coarse_match_capped (at most k matches per pair, chosen by confidence). */
+ * 105: lb_coarse_match_capped (at most k matches per pair, chosen by confidence);
+ * 106: lb_preprocess_images (uint8 images of any size -> the matcher's padded fp32 input and 1/8 mask). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -61,8 +64,8 @@ const char* lb_last_error(void);
 /* number of kernels this library has launched in this process (for bench.py's gpu_launches) */
 long long lb_launch_count(void);
 
-/* Optional per-launch CUDA-event timing of the tensor-core kernels and of the per-pair match cap (events recorded on
- * the launching stream around each kernel while enabled).  lb_timing_enable(1) clears old records and starts recording,
+/* Optional per-launch CUDA-event timing of the tensor-core kernels, the per-pair match cap and the image front end
+ * (events recorded on the launching stream around each kernel while enabled).  lb_timing_enable(1) clears old records and starts recording,
  * lb_timing_collect synchronises the recorded events and returns per-tag total milliseconds and launch counts
  * (arrays of lb_timing_num_tags() entries; names via lb_timing_tag_name).  Timed launches cannot be recorded into a
  * CUDA graph: while timing is enabled, a launch on a capturing stream fails. */
@@ -80,6 +83,29 @@ int lb_split_planes(const float* x, long rows, int cols, int ld_x, void* hi, voi
 int lb_gemm_split(const void* a_hi, const void* a_lo, long lda, long a_batch_stride, const void* b_hi,
                   const void* b_lo, long ldb, long b_batch_stride, float* out, long ldo, long o_batch_stride,
                   int batches, int M, int N, int K, void* stream);
+
+/* ---- image front end.  Replaces, for a whole batch in one launch, the per-image host work of the reference's dataset
+ * readers (src/utils/dataset.py: imread_gray's colour conversion :47-51, get_resized_wh / get_divisible_wh are the
+ * caller's, cv2.resize + pad_bottom_right + `/ 255` of read_megadepth_gray :94-125 and read_scannet_gray :141-157) and
+ * the 1/8 mask of src/datasets/megadepth.py:119-125.  One descriptor per image, in DEVICE memory. */
+typedef struct LbImageDesc {
+  const uint8_t* src;    /* device: pixel (y, x), channel c at src[y*row_stride_bytes + x*channels + c] */
+  int h, w;              /* source size, both >= 1 */
+  int row_stride_bytes;  /* >= w*channels: a cropped view or a row-padded decoder buffer needs no copy */
+  int channels;          /* 1 (grey) or 3 (interleaved colour) */
+  int r_index;           /* 3 channels: position of red, 0 = RGB, 2 = BGR (green is 1); ignored for 1 channel */
+  int h_new, w_new;      /* size after the resize, 1 <= h_new <= H, 1 <= w_new <= W */
+} LbImageDesc;
+
+/* Image i is converted to grey at source resolution (OpenCV's Y = (9798 R + 19235 G + 3735 B + 16384) >> 15), resized
+ * to h_new x w_new (bilinear, half-pixel centres, edge clamp, no antialiasing: cv2.resize INTER_LINEAR, except that
+ * the fp32 result is not rounded to a grey level), divided by 255 and written top-left into out[i] ([n_images, 1, H, W]
+ * fp32, 16-byte aligned); the rest of the canvas is 0.  With h_new == h and w_new == w, out is level / 255 exactly.
+ * mask: NULL, or [n_images, H/8, W/8] bytes, cell (Y, X) = (8Y < h_new && 8X < w_new).  H and W must be positive
+ * multiples of 8 and n_images at most 65535.  The descriptors are read on the device and not checked there: the caller
+ * guarantees the ranges above.  One launch (timing tag "preprocess"), no workspace, no atomics. */
+int lb_preprocess_images(const LbImageDesc* descs, int n_images, float* out, int H, int W, uint8_t* mask,
+                         void* stream);
 
 /* feat fp32 (NCHW [n_img, C, h, w], or NHWC [n_img, h, w, C] when nhwc != 0) + pe [C, pe_h, pe_w]
  * -> x_f32 [n_img*h*w, C], cat planes [rows, 2C] cols [0,C). */

@@ -49,6 +49,11 @@ class LbBackboneWeights(C.Structure):
                 ("l1_out2", LbConvWeights * 2)]
 
 
+class LbImageDesc(C.Structure):
+    _fields_ = [("src", c_void_p), ("h", c_int), ("w", c_int), ("row_stride_bytes", c_int), ("channels", c_int),
+                ("r_index", c_int), ("h_new", c_int), ("w_new", c_int)]
+
+
 class LbTransformerState(C.Structure):
     _fields_ = [("x_f32", c_void_p), ("cat_hi", c_void_p), ("cat_lo", c_void_p), ("mask", c_void_p),
                 ("n_groups", c_int), ("group_rows0", c_int), ("group_rows1", c_int), ("n_groups_live", c_void_p)]
@@ -109,6 +114,7 @@ SIGNATURES = {
     "lb_split_planes": (c_int, [c_void_p, c_long, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "lb_gemm_split": (c_int, [c_void_p, c_void_p, c_long, c_long, c_void_p, c_void_p, c_long, c_long, c_void_p,
                               c_long, c_long, c_int, c_int, c_int, c_int, c_void_p]),
+    "lb_preprocess_images": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "lb_coarse_prep": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                c_void_p, c_void_p, c_void_p]),
     "lb_coarse_prep_indexed": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
@@ -148,8 +154,10 @@ FULL_ATTENTION_VERSION = 102
 FEATURE_BANK_VERSION = 104
 # oldest library with the per-pair match cap (lb_coarse_match_capped)
 MATCH_CAP_VERSION = 105
+# oldest library with the image front end (lb_preprocess_images)
+PREPROCESS_VERSION = 106
 _SINCE = {"lb_coarse_prep_indexed": FEATURE_BANK_VERSION, "lb_fine_preprocess_indexed": FEATURE_BANK_VERSION,
-          "lb_coarse_match_capped": MATCH_CAP_VERSION}
+          "lb_coarse_match_capped": MATCH_CAP_VERSION, "lb_preprocess_images": PREPROCESS_VERSION}
 
 
 class LibraryMissing(RuntimeError):
@@ -208,7 +216,7 @@ def timing_enable(on: bool):
 
 
 def timing_collect() -> dict:
-    """-> {tag: (total_ms, launches)} for every kernel tag (tensor-core kernels, match cap) recorded since
+    """-> {tag: (total_ms, launches)} for every kernel tag (tensor-core kernels, match cap, image front end) recorded since
     timing_enable(True)."""
     lib = load()
     n = lib.lb_timing_num_tags()

@@ -56,13 +56,15 @@ static int fail(const char* fmt, ...) {
   } while (0)
 
 // ------------------------------------------------------------------------------------------------ timing hook
-// Optional per-launch CUDA-event timing of the tensor-core kernels (bench.py's roofline leg) and of the per-pair match
-// cap: events are recorded on the launching stream right around the kernel, and only while timing is enabled.
+// Optional per-launch CUDA-event timing of the tensor-core kernels (bench.py's roofline leg), of the per-pair match
+// cap and of the image front end: events are recorded on the launching stream right around the kernel, and only while timing is enabled.
 enum Tag { TAG_GEMM_TEST = 0, TAG_PROJ, TAG_MERGE_LN, TAG_MLP1, TAG_MLP2_LN, TAG_SCORE_LSE, TAG_SCORE_ARGMAX,
-           TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_FULL_ATTN, TAG_MATCH_CAP, TAG_COUNT };
+           TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_FULL_ATTN, TAG_MATCH_CAP, TAG_PREPROCESS,
+           TAG_COUNT };
 static const char* kTagNames[TAG_COUNT] = {"gemm_test", "proj_act", "merge_ln", "mlp1_relu", "mlp2_ln_res",
                                            "score_lse", "score_argmax", "fine_merge", "backbone_conv",
-                                           "tf_kv_proj_fused", "tf_q_attn_fused", "tf_full_attn", "match_cap"};
+                                           "tf_kv_proj_fused", "tf_q_attn_fused", "tf_full_attn", "match_cap",
+                                           "preprocess"};
 struct TimingRec {
   cudaEvent_t e0, e1;
   int tag;
@@ -933,7 +935,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
 
 extern "C" {
 
-int lb_version(void) { return 105; }
+int lb_version(void) { return 106; }
 int lb_block_k(void) { return kBlockK; }
 int lb_conv_layout(int cin, int* cin_blocks, int* rem_channels) {
   if (!cin_blocks || !rem_channels || cin <= 0) return fail("lb_conv_layout: bad arguments");
@@ -1009,6 +1011,28 @@ int lb_gemm_split(const void* a_hi, const void* a_lo, long lda, long a_batch_str
   using Epi = EpiActStore<128>;
   Epi::Params ep{0, nullptr, 1.f, om};
   return launch_gemm<128, Epi>(TAG_GEMM_TEST, A, B, batches, M, N, K, 0, ep, st);
+}
+
+int lb_preprocess_images(const LbImageDesc* descs, int n_images, float* out, int H, int W, uint8_t* mask,
+                         void* stream) {
+  if (H <= 0 || W <= 0 || H % 8 != 0 || W % 8 != 0)
+    return fail("lb_preprocess_images: canvas %dx%d must be positive and divisible by 8", H, W);
+  if (n_images < 0 || n_images > 65535) return fail("lb_preprocess_images: n_images=%d must be in [0, 65535]", n_images);
+  if (!descs || !out) return fail("lb_preprocess_images: descs and out are required");
+  if ((reinterpret_cast<uintptr_t>(out) & 15) != 0) return fail("lb_preprocess_images: out is not 16-byte aligned");
+  if (n_images == 0) return 0;
+  int sms;
+  DeviceGuard dev_guard;
+  LB_TRY(dev_guard.bind(out));
+  LB_TRY(device_check(&sms));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  dim3 grid(cdiv(W, kPreprocessBlockX * 4), cdiv(H, kPreprocessBlockY), n_images);
+  TimingRec rec{nullptr, nullptr, TAG_PREPROCESS};
+  LB_TRY(timing_begin(rec, st));
+  preprocess_images_kernel<<<grid, dim3(kPreprocessBlockX, kPreprocessBlockY), 0, st>>>(descs, out, H, W, mask);
+  LB_LAUNCHED();
+  LB_TRY(timing_end(rec, st));
+  return 0;
 }
 
 // n_out output images; with img_idx, output image b reads image img_idx[b] of feat

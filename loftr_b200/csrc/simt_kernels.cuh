@@ -4,6 +4,7 @@
 #pragma once
 #include <cuda_fp16.h>
 #include <cstdint>
+#include "../../include/loftr_b200.h"
 #include "epilogues.cuh"
 
 namespace lb {
@@ -76,6 +77,67 @@ __global__ void coarse_prep_kernel(const float* __restrict__ feat, int nhwc, con
       cat_lo[row * (2 * C) + c] = ll;
     }
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Image front end: uint8 source images of any size (grey, or interleaved RGB / BGR) -> the matcher's input
+// [n, 1, H, W] fp32 in [0, 1], each image resized to its (h_new, w_new), placed top-left in the H x W canvas and
+// zero-padded, plus the 1/8 padding mask.  = imread_gray's colour conversion, cv2.resize (INTER_LINEAR), pad_bottom_right
+// and `/ 255` of the reference (src/utils/dataset.py:47-51,94-125,141-157) and the mask subsampling of
+// src/datasets/megadepth.py:119-125.  HBM-bound: one pass, no shared memory, no atomics.
+//
+// Grey level of source pixel (y, x): the byte itself, or OpenCV's 15-bit fixed-point luma of an interleaved pixel.
+__device__ __forceinline__ float image_level(const LbImageDesc& d, int y, int x) {
+  const uint8_t* p = d.src + static_cast<long>(y) * d.row_stride_bytes + static_cast<long>(x) * d.channels;
+  if (d.channels == 1) return static_cast<float>(__ldg(p));
+  const int r = __ldg(p + d.r_index), g = __ldg(p + 1), b = __ldg(p + 2 - d.r_index);
+  return static_cast<float>((9798 * r + 19235 * g + 3735 * b + 16384) >> 15);
+}
+
+constexpr int kPreprocessBlockX = 32;   // threads along x, four output pixels each: a 128-pixel tile row
+constexpr int kPreprocessBlockY = 8;
+// grid (cdiv(W, 128), cdiv(H, 8), n); descs[img] describes image blockIdx.z.  Bilinear taps with half-pixel centres and
+// edge clamp.  The source coordinate is formed in fp64 (in fp32 its rounding at x ~ 1000 would move the weight by 1e-4,
+// i.e. the result by up to 1e-4 of full scale on a noisy image); the interpolation itself is fp32 on levels 0..255,
+// not rounded to a level, then a true division by 255.  With h_new == h and w_new == w both weights are exactly 0 and
+// the output is level / 255 bit for bit.  W is a multiple of 8, so a thread's four pixels lie in one row and its float4
+// store is aligned; mask cell (Y, X) is written by the thread that owns pixel (8Y, 8X).
+__global__ void __launch_bounds__(kPreprocessBlockX * kPreprocessBlockY)
+preprocess_images_kernel(const LbImageDesc* __restrict__ descs, float* __restrict__ out, int H, int W,
+                         uint8_t* __restrict__ mask) {
+  const int img = blockIdx.z;
+  const int x4 = (blockIdx.x * kPreprocessBlockX + threadIdx.x) * 4;
+  const int y = blockIdx.y * kPreprocessBlockY + threadIdx.y;
+  if (x4 >= W || y >= H) return;
+  const LbImageDesc d = descs[img];
+  const bool inside = y < d.h_new && x4 < d.w_new;
+  float v[4] = {0.f, 0.f, 0.f, 0.f};   // padding is exactly 0
+  if (inside) {
+    const double sy = (y + 0.5) * (static_cast<double>(d.h) / d.h_new) - 0.5;
+    const double sy0 = floor(sy);
+    const float fy = static_cast<float>(sy - sy0);
+    const int y0 = min(max(static_cast<int>(sy0), 0), d.h - 1);
+    const int y1 = min(max(static_cast<int>(sy0) + 1, 0), d.h - 1);
+    const double rx = static_cast<double>(d.w) / d.w_new;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int x = x4 + i;
+      if (x >= d.w_new) break;
+      const double sx = (x + 0.5) * rx - 0.5;
+      const double sx0 = floor(sx);
+      const float fx = static_cast<float>(sx - sx0);
+      const int x0 = min(max(static_cast<int>(sx0), 0), d.w - 1);
+      const int x1 = min(max(static_cast<int>(sx0) + 1, 0), d.w - 1);
+      const float a = image_level(d, y0, x0), b = image_level(d, y0, x1);
+      const float c = image_level(d, y1, x0), e = image_level(d, y1, x1);
+      const float top = a + fx * (b - a);
+      const float bot = c + fx * (e - c);
+      v[i] = (top + fy * (bot - top)) / 255.0f;
+    }
+  }
+  *reinterpret_cast<float4*>(out + (static_cast<long>(img) * H + y) * W + x4) = make_float4(v[0], v[1], v[2], v[3]);
+  if (mask && (y & 7) == 0 && (x4 & 7) == 0)
+    mask[(static_cast<long>(img) * (H >> 3) + (y >> 3)) * (W >> 3) + (x4 >> 3)] = inside ? 1 : 0;
 }
 
 // ------------------------------------------------------------------------------------------------
