@@ -19,6 +19,9 @@
  *   lb_fine_preprocess        <- FinePreprocess.forward                     src/loftr/loftr_module/fine_preprocess.py:29-59
  *   lb_fine_match             <- FineMatching.forward + get_fine_match      src/loftr/utils/fine_matching.py:15-74
  *
+ * lb_estimate_geometry has no counterpart in the reference: it fits a homography or a fundamental matrix to each
+ * pair's matches (batched RANSAC), the step callers otherwise run on the host after matching.
+ *
  * Conventions
  *   - All pointers are DEVICE pointers unless a parameter says "host".  No torch / C++ types cross this
  *     boundary; `stream` is a cudaStream_t passed as void*.
@@ -52,7 +55,8 @@ extern "C" {
  * 102: full-attention layer kinds; 103: lb_selftest removed (no structure changes);
  * 104: lb_coarse_prep_indexed / lb_fine_preprocess_indexed (pairs read from a per-image feature bank);
  * 105: lb_coarse_match_capped (at most k matches per pair, chosen by confidence);
- * 106: lb_preprocess_images (uint8 images of any size -> the matcher's padded fp32 input and 1/8 mask). */
+ * 106: lb_preprocess_images (uint8 images of any size -> the matcher's padded fp32 input and 1/8 mask);
+ * 107: lb_estimate_geometry (batched RANSAC homography / fundamental matrix per pair). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -64,8 +68,8 @@ const char* lb_last_error(void);
 /* number of kernels this library has launched in this process (for bench.py's gpu_launches) */
 long long lb_launch_count(void);
 
-/* Optional per-launch CUDA-event timing of the tensor-core kernels, the per-pair match cap and the image front end
- * (events recorded on the launching stream around each kernel while enabled).  lb_timing_enable(1) clears old records and starts recording,
+/* Optional per-launch CUDA-event timing of the tensor-core kernels, the per-pair match cap, the image front end and
+ * the geometry estimator (events recorded on the launching stream around each kernel while enabled).  lb_timing_enable(1) clears old records and starts recording,
  * lb_timing_collect synchronises the recorded events and returns per-tag total milliseconds and launch counts
  * (arrays of lb_timing_num_tags() entries; names via lb_timing_tag_name).  Timed launches cannot be recorded into a
  * CUDA graph: while timing is enabled, a launch on a capturing stream fails. */
@@ -105,6 +109,31 @@ typedef struct LbImageDesc {
  * multiples of 8 and n_images at most 65535.  The descriptors are read on the device and not checked there: the caller
  * guarantees the ranges above.  One launch (timing tag "preprocess"), no workspace, no atomics. */
 int lb_preprocess_images(const LbImageDesc* descs, int n_images, float* out, int H, int W, uint8_t* mask,
+                         void* stream);
+
+/* ---- two-view geometry.  Robust fit of one model per pair to matches in a padded layout: pts0 / pts1 [B, K, 2] fp32
+ * (x, y) pixels, 8-byte aligned; valid [B, K] bytes (non-zero: a match) or NULL (all K are matches).
+ * model LB_GEOMETRY_HOMOGRAPHY: x1 ~ H x0, 4-point normalised DLT hypotheses, symmetric transfer error (the mean of
+ * the squared forward and backward transfer distances); LB_GEOMETRY_FUNDAMENTAL: x1^T F x0 = 0, normalised 8-point
+ * hypotheses with rank 2 enforced, squared Sampson distance.  A match is an inlier when its error is below
+ * threshold^2 (threshold in pixels).
+ * Per pair: `iterations` hypotheses, hypothesis h drawn from Philox4x32-10 with counter (h, pair id, block, 0) and key
+ * seed (pair id: pair_ids[b], or b when pair_ids is NULL), so that a pair's result depends on its matches, its id, the
+ * seed and the budget only; degenerate samples are skipped; the best hypothesis has the most inliers, then the lowest
+ * MSAC cost (sum of min(error, threshold^2)), then the lowest index; the model is refitted by Hartley-normalised least
+ * squares on its inliers and the inliers are recomputed once.  All geometry in fp64.
+ * Outputs: model_out [B, 3, 3] fp32 (H scaled to H[2][2] = 1; F to unit Frobenius norm, largest entry positive), NaN
+ * when the pair has fewer valid matches than the sample size or only degenerate samples; mask_out [B, K] bytes (1:
+ * inlier of the returned model; padding and invalid entries 0); count_out [B] int32 (0 with a NaN model);
+ * best_out [B] (or NULL): the best hypothesis, -1 when none; samples_out [B, iterations, 4 or 8] (or NULL): every
+ * hypothesis' sample as columns of K, ascending, -1 when the pair is too small (a debugging output).
+ * Three launches, no host synchronisation (capturable in a CUDA graph), timing tag "geometry". */
+#define LB_GEOMETRY_HOMOGRAPHY 0
+#define LB_GEOMETRY_FUNDAMENTAL 1
+size_t lb_geometry_workspace_bytes(int B, int K, int iterations);
+int lb_estimate_geometry(const float* pts0, const float* pts1, const uint8_t* valid, const int* pair_ids, int B, int K,
+                         int model, float threshold, int iterations, unsigned long long seed, float* model_out,
+                         uint8_t* mask_out, int* count_out, int* best_out, int* samples_out, void* ws, size_t ws_bytes,
                          void* stream);
 
 /* feat fp32 (NCHW [n_img, C, h, w], or NHWC [n_img, h, w, C] when nhwc != 0) + pe [C, pe_h, pe_w]

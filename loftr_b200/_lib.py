@@ -115,6 +115,10 @@ SIGNATURES = {
     "lb_gemm_split": (c_int, [c_void_p, c_void_p, c_long, c_long, c_void_p, c_void_p, c_long, c_long, c_void_p,
                               c_long, c_long, c_int, c_int, c_int, c_int, c_void_p]),
     "lb_preprocess_images": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "lb_geometry_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "lb_estimate_geometry": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int,
+                                     C.c_ulonglong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_size_t, c_void_p]),
     "lb_coarse_prep": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                c_void_p, c_void_p, c_void_p]),
     "lb_coarse_prep_indexed": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
@@ -156,8 +160,13 @@ FEATURE_BANK_VERSION = 104
 MATCH_CAP_VERSION = 105
 # oldest library with the image front end (lb_preprocess_images)
 PREPROCESS_VERSION = 106
+# oldest library with the two-view geometry estimator (lb_estimate_geometry)
+GEOMETRY_VERSION = 107
+GEOMETRY_HOMOGRAPHY = 0
+GEOMETRY_FUNDAMENTAL = 1
 _SINCE = {"lb_coarse_prep_indexed": FEATURE_BANK_VERSION, "lb_fine_preprocess_indexed": FEATURE_BANK_VERSION,
-          "lb_coarse_match_capped": MATCH_CAP_VERSION, "lb_preprocess_images": PREPROCESS_VERSION}
+          "lb_coarse_match_capped": MATCH_CAP_VERSION, "lb_preprocess_images": PREPROCESS_VERSION,
+          "lb_geometry_workspace_bytes": GEOMETRY_VERSION, "lb_estimate_geometry": GEOMETRY_VERSION}
 
 
 class LibraryMissing(RuntimeError):
@@ -216,8 +225,8 @@ def timing_enable(on: bool):
 
 
 def timing_collect() -> dict:
-    """-> {tag: (total_ms, launches)} for every kernel tag (tensor-core kernels, match cap, image front end) recorded since
-    timing_enable(True)."""
+    """-> {tag: (total_ms, launches)} for every kernel tag (tensor-core kernels, match cap, image front end, geometry)
+    recorded since timing_enable(True)."""
     lib = load()
     n = lib.lb_timing_num_tags()
     ms = (C.c_double * n)()

@@ -5,6 +5,7 @@
 #include <cudaTypedefs.h>
 
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -22,6 +23,7 @@
 #include "full_attn.cuh"
 #include "stem_tc.cuh"
 #include "comm.cuh"
+#include "geometry.cuh"
 
 namespace lb {
 
@@ -57,14 +59,15 @@ static int fail(const char* fmt, ...) {
 
 // ------------------------------------------------------------------------------------------------ timing hook
 // Optional per-launch CUDA-event timing of the tensor-core kernels (bench.py's roofline leg), of the per-pair match
-// cap and of the image front end: events are recorded on the launching stream right around the kernel, and only while timing is enabled.
+// cap, of the image front end and of the geometry estimator (its three launches as one record): events are recorded on
+// the launching stream right around the kernels, and only while timing is enabled.
 enum Tag { TAG_GEMM_TEST = 0, TAG_PROJ, TAG_MERGE_LN, TAG_MLP1, TAG_MLP2_LN, TAG_SCORE_LSE, TAG_SCORE_ARGMAX,
            TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_FULL_ATTN, TAG_MATCH_CAP, TAG_PREPROCESS,
-           TAG_COUNT };
+           TAG_GEOMETRY, TAG_COUNT };
 static const char* kTagNames[TAG_COUNT] = {"gemm_test", "proj_act", "merge_ln", "mlp1_relu", "mlp2_ln_res",
                                            "score_lse", "score_argmax", "fine_merge", "backbone_conv",
                                            "tf_kv_proj_fused", "tf_q_attn_fused", "tf_full_attn", "match_cap",
-                                           "preprocess"};
+                                           "preprocess", "geometry"};
 struct TimingRec {
   cudaEvent_t e0, e1;
   int tag;
@@ -935,7 +938,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
 
 extern "C" {
 
-int lb_version(void) { return 106; }
+int lb_version(void) { return 107; }
 int lb_block_k(void) { return kBlockK; }
 int lb_conv_layout(int cin, int* cin_blocks, int* rem_channels) {
   if (!cin_blocks || !rem_channels || cin <= 0) return fail("lb_conv_layout: bad arguments");
@@ -1577,6 +1580,72 @@ int lb_epipolar_errors(const float* mkpts0_f, const float* mkpts1_f, const long 
   epipolar_error_kernel<<<cdiv(M, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(mkpts0_f, mkpts1_f, m_bids, M, n_pairs,
                                                                                       T_0to1, K0, K1, epi_errs);
   LB_LAUNCHED();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ two-view geometry
+static size_t geometry_ws_layout(int B, int K, int iterations, size_t* off_col, size_t* off_n, size_t* off_best) {
+  const size_t bk = static_cast<size_t>(B) * K;
+  const size_t n_tiles = static_cast<size_t>(cdiv(iterations, kGeoHypPerBlock));
+  *off_col = bk * sizeof(float4);
+  *off_n = *off_col + ((bk * sizeof(int) + 15) & ~size_t(15));
+  *off_best = *off_n + ((static_cast<size_t>(B) * sizeof(int) + 15) & ~size_t(15));
+  return *off_best + static_cast<size_t>(B) * n_tiles * sizeof(GeoBest);
+}
+
+size_t lb_geometry_workspace_bytes(int B, int K, int iterations) {
+  if (B <= 0 || K <= 0 || iterations <= 0) return 0;
+  size_t a, b, c;
+  return geometry_ws_layout(B, K, iterations, &a, &b, &c);
+}
+
+int lb_estimate_geometry(const float* pts0, const float* pts1, const uint8_t* valid, const int* pair_ids, int B, int K,
+                         int model, float threshold, int iterations, unsigned long long seed, float* model_out,
+                         uint8_t* mask_out, int* count_out, int* best_out, int* samples_out, void* ws, size_t ws_bytes,
+                         void* stream) {
+  if (model != LB_GEOMETRY_HOMOGRAPHY && model != LB_GEOMETRY_FUNDAMENTAL)
+    return fail("lb_estimate_geometry: unknown model %d", model);
+  const int s = model == LB_GEOMETRY_HOMOGRAPHY ? 4 : 8;
+  if (B < 0 || B > 65535) return fail("lb_estimate_geometry: B=%d must be in [0, 65535]", B);
+  if (K < s) return fail("lb_estimate_geometry: K=%d is below the minimal sample size %d", K, s);
+  if (!(threshold > 0.0f) || !std::isfinite(threshold))
+    return fail("lb_estimate_geometry: threshold must be a positive number of pixels");
+  if (iterations <= 0) return fail("lb_estimate_geometry: iterations=%d must be positive", iterations);
+  if (B == 0) return 0;
+  if (!pts0 || !pts1 || !model_out || !mask_out || !count_out || !ws)
+    return fail("lb_estimate_geometry: pts0, pts1, model_out, mask_out, count_out and ws are required");
+  if ((reinterpret_cast<uintptr_t>(pts0) & 7) || (reinterpret_cast<uintptr_t>(pts1) & 7) ||
+      (reinterpret_cast<uintptr_t>(ws) & 15))
+    return fail("lb_estimate_geometry: points must be 8-byte and the workspace 16-byte aligned");
+  size_t off_col, off_n, off_best;
+  const size_t need = geometry_ws_layout(B, K, iterations, &off_col, &off_n, &off_best);
+  if (ws_bytes < need) return fail("lb_estimate_geometry: workspace of %zu bytes, %zu needed", ws_bytes, need);
+  int sms;
+  DeviceGuard dev_guard;
+  LB_TRY(dev_guard.bind(model_out));
+  LB_TRY(device_check(&sms));
+  GeoParams p;
+  p.pts0 = pts0; p.pts1 = pts1; p.valid = valid; p.pair_ids = pair_ids;
+  p.B = B; p.K = K; p.model = model; p.iterations = iterations; p.n_tiles = cdiv(iterations, kGeoHypPerBlock);
+  p.seed = seed;
+  p.thr2 = static_cast<double>(threshold) * threshold;
+  char* w = static_cast<char*>(ws);
+  p.compact = reinterpret_cast<float4*>(w);
+  p.compact_col = reinterpret_cast<int*>(w + off_col);
+  p.n_valid = reinterpret_cast<int*>(w + off_n);
+  p.tile_best = reinterpret_cast<GeoBest*>(w + off_best);
+  p.model_out = model_out; p.mask_out = mask_out; p.count_out = count_out;
+  p.best_out = best_out; p.samples_out = samples_out;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  TimingRec rec{nullptr, nullptr, TAG_GEOMETRY};
+  LB_TRY(timing_begin(rec, st));
+  geometry_compact_kernel<<<B, kGeoRefitThreads, 0, st>>>(p);
+  LB_LAUNCHED();
+  geometry_score_kernel<<<dim3(p.n_tiles, B), kGeoHypPerBlock, 0, st>>>(p);
+  LB_LAUNCHED();
+  geometry_refit_kernel<<<B, kGeoRefitThreads, 0, st>>>(p);
+  LB_LAUNCHED();
+  LB_TRY(timing_end(rec, st));
   return 0;
 }
 

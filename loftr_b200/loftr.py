@@ -25,7 +25,7 @@ import numbers
 import torch
 import torch.nn as nn
 
-from . import _lib
+from . import _lib, geometry
 from .backbone import build_backbone
 
 _KIND = {("self", "linear"): _lib.LAYER_SELF, ("cross", "linear"): _lib.LAYER_CROSS,
@@ -680,7 +680,7 @@ class LoFTR(nn.Module):
         return ImageFeatures(feat_c, feat_f, masks, images.shape[2:], feat_c.shape[2:], feat_f.shape[2:], key)
 
     @torch.no_grad()
-    def match_features(self, feats0, idx0, feats1, idx1, scale0=None, scale1=None, data=None):
+    def match_features(self, feats0, idx0, feats1, idx1, scale0=None, scale1=None, data=None, estimate=None):
         """Matches pair b = (image idx0[b] of feats0, image idx1[b] of feats1) for every b of the pair list, from banks
         made by `extract_features` (feats1 may be feats0).  Writes into `data` (a new dict when None) and returns it:
         the keys, dtypes and values `forward` writes for the batch image0 = images idx0 of feats0, image1 = images
@@ -689,9 +689,23 @@ class LoFTR(nn.Module):
         idx0, idx1: int32 / int64 tensors [B] on the model's device, each index within its bank.  An empty list gives
         the outputs of a forward with no matches.  scale0 / scale1: optional [K0, 2] / [K1, 2] per-image scales of
         feats0 / feats1 (both or neither).  A bank is tied to the backbone weights it was extracted with: after
-        load_state_dict, .to() or a parameter update it raises; extract again."""
+        load_state_dict, .to() or a parameter update it raises; extract again.
+
+        estimate: None (the default: nothing else runs and no other key is written), "homography", "fundamental", or
+        a dict of `loftr_b200.estimate_geometry` options ("model", "threshold", "iterations", "seed").  The estimator
+        then fits that model to each pair's fine matches (mkpts0_f / mkpts1_f) on the GPU and adds
+        data["geom_model"] [B, 3, 3], data["geom_inliers"] [M] bool (one flag per match of the list) and
+        data["geom_num_inliers"] [B] int32; pair b's RNG key is b."""
         _require_eval(self)
         _lib.require(_lib.FEATURE_BANK_VERSION, "match_features")
+        geom = None
+        if estimate is not None:
+            opts = {"model": estimate} if isinstance(estimate, str) else estimate
+            if not isinstance(opts, dict) or not set(opts) <= {"model", "threshold", "iterations", "seed"}:
+                raise ValueError("match_features: estimate must be None, 'homography', 'fundamental' or a dict of "
+                                 "estimate_geometry options (model, threshold, iterations, seed)")
+            geom = dict(zip(("model", "threshold", "iterations", "seed"), geometry.check_options(**opts)))
+            _lib.require(_lib.GEOMETRY_VERSION, "match_features(estimate=...)")
         key = self._bank_key()
         dev = next(self.parameters()).device
         for name, f in (("feats0", feats0), ("feats1", feats1)):
@@ -720,6 +734,11 @@ class LoFTR(nn.Module):
         work.update({"bs": bs, "hw0_i": feats0.hw_i, "hw1_i": feats1.hw_i, "hw0_c": feats0.hw_c, "hw1_c": feats1.hw_c,
                      "hw0_f": feats0.hw_f, "hw1_f": feats1.hw_f})
         self._match_pairs(work, feats0.feat_c, feats1.feat_c, feats0.feat_f, feats1.feat_f, img_idx=(idx0, idx1))
+        if geom is not None:
+            (h0, w0), (h1, w1) = feats0.hw_c, feats1.hw_c
+            bound = CoarseMatching.default_capacity(1, h0 * w0, h1 * w1, feats0.mask is not None,
+                                                    self.coarse_matching.max_matches_per_pair)
+            geometry.estimate_on_matches(work, bs, bound, geom)
         out = {} if data is None else data
         out.update({k: v for k, v in work.items() if k not in ("mask0", "mask1", "scale0", "scale1")})
         return out
