@@ -26,9 +26,9 @@
 // (nine taps per halo, the next block's halo loading into the other slot meanwhile); the channel remainder
 // (Cin = 64 * cin_blocks + r, r <= 16) is a last 16-channel halo with one K = 16 step per tap.
 //
-// Warp roles, the epilogue contract, the accumulator staging over the dead ring / halo memory and the tile-end drain
-// are those of gemm_split_kernel.  Where the staging fits in the weight ring (N = 128) the next tile's first halos
-// load while the epilogue runs.
+// Warp roles, the epilogue contract, the set-up, the work split and the tile end (drain, accumulator staging over the
+// dead ring / halo memory, epilogue, hand-off) are gemm_split.cuh's shared pieces.  Where the staging fits in the
+// weight ring (N = 128) the next tile's first halos load while the epilogue runs.
 #pragma once
 #include "gemm_split.cuh"
 
@@ -51,15 +51,14 @@ static_assert(kHaloW * kHaloH * 16 <= kHaloChunkBytes && kHaloChunkBytes % 128 =
 template <int BLOCK_N, int kEpiBytes>
 struct HaloSmem {
   static constexpr int kBarBytes = 256;
-  static constexpr int kFree = 232448 - kBarBytes - kEpiBytes - 2 * kHaloSlotBytes;
+  static constexpr int kFree = kSmemLimit - kBarBytes - kEpiBytes - 2 * kHaloSlotBytes;
   static constexpr int kBK = kFree / (2 * BLOCK_N * kBlockK * 2) >= 3 ? kBlockK : kBlockK / 2;
   static constexpr int kBTile = BLOCK_N * kBK * 2;        // per plane
   static constexpr int kStageBytes = 2 * kBTile;
   static constexpr int kStages = kFree / kStageBytes < 6 ? kFree / kStageBytes : 6;
   static_assert(kStages >= 3, "the weight ring needs three stages");
   static constexpr int kRingBytes = kStages * kStageBytes;
-  static constexpr int kAccStride = BLOCK_N + 4;         // floats, as GemmSmem
-  static constexpr int kAccBytes = (kBlockM * kAccStride + 32) * 4;
+  static constexpr int kAccBytes = acc_bytes(BLOCK_N);
   static constexpr int kMainBytes = kRingBytes + 2 * kHaloSlotBytes;
   static_assert(kMainBytes >= kAccBytes && kMainBytes % 1024 == 0 && kRingBytes % 1024 == 0, "halo smem layout");
   static constexpr int kTotalBytes = kMainBytes + kEpiBytes + kBarBytes;
@@ -101,33 +100,14 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
   uint64_t* acc_free = halo_empty + 2;
   static_assert(Epi::kSmemBytes % 16 == 0, "epilogue area must keep the barriers aligned");
   static_assert((2 * S::kStages + 5) * 8 <= S::kBarBytes, "barrier area");
-  if ((smem_u32(smem_raw) & 1023u) != 0) asm volatile("trap;");
-
-  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
+  const int warp = persistent_setup<S::kStages>(smem_raw, &tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, full_bar, empty_bar,
+                                                acc_free, [&] {
+                                                  for (int s = 0; s < 2; ++s) {
+                                                    mbar_init(&halo_full[s], 1);
+                                                    mbar_init(&halo_empty[s], kEpiThreads);
+                                                  }
+                                                });
   const int lane = threadIdx.x & 31;
-
-  if (warp == kProducerWarp && lane == 0) {
-    tma_prefetch_desc(&tm_a_hi);
-    tma_prefetch_desc(&tm_a_lo);
-    tma_prefetch_desc(&tm_b_hi);
-    tma_prefetch_desc(&tm_b_lo);
-  }
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < S::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kEpiThreads);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&halo_full[s], 1);
-      mbar_init(&halo_empty[s], kEpiThreads);
-    }
-    mbar_init(acc_free, 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  // programmatic dependent launch, as in gemm_split_kernel
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
 
   const ConvGeom& g = shape.conv;
   const int n_halo = g.cin_blocks + (g.rem_groups > 0 ? 1 : 0);   // halos (channel blocks) per output tile
@@ -138,19 +118,14 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
   if (warp == kProducerWarp) {
     // ------------------------------------------------------------ TMA producer
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      RingPos<S::kStages> pos;
       uint32_t tiles = 0;
       int halos = 0;   // halo loads issued so far: load i goes to slot i & 1
       for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-        const int chunk = item % shape.n_chunks;
-        const int mt = (item / shape.n_chunks) % shape.m_tiles;
-        const int batch = item / (shape.n_chunks * shape.m_tiles);
-        const int ty = mt / g.tiles_w, tx = mt - ty * g.tiles_w;
+        const WorkItem w = work_item(shape, shape.m_tiles, item);
+        const int ty = w.mt / g.tiles_w, tx = w.mt - ty * g.tiles_w;
         const int x0 = tx * kConvTileW - 1, y0 = ty * kConvTileH - 1;
-        const int nt_begin = chunk * shape.tiles_per_chunk;
-        const int nt_end = min(nt_begin + shape.tiles_per_chunk, shape.n_tiles);
-        for (int nt = nt_begin; nt < nt_end; ++nt) {
+        for (int nt = w.nt_begin; nt < w.nt_end; ++nt) {
           // the previous tile's staged accumulator must be consumed before the ring (and, when the staging reaches
           // past the ring, the halo slots) is refilled
           bool staged = tiles > 0;
@@ -171,8 +146,8 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
             uint8_t* dst = halo + slot * kHaloSlotBytes;
             for (int c = 0; c < chunks; ++c) {
               const int ch = hh * kBlockK + 8 * c;
-              tma_load_4d(dst + c * kHaloChunkBytes, &tm_a_hi, fb, ch, x0, y0, batch);
-              tma_load_4d(dst + kHaloPlaneBytes + c * kHaloChunkBytes, &tm_a_lo, fb, ch, x0, y0, batch);
+              tma_load_4d(dst + c * kHaloChunkBytes, &tm_a_hi, fb, ch, x0, y0, w.batch);
+              tma_load_4d(dst + kHaloPlaneBytes + c * kHaloChunkBytes, &tm_a_lo, fb, ch, x0, y0, w.batch);
             }
           };
           // the halos needed first are issued before the weights (with kStagingInRing: while the previous tile's
@@ -187,9 +162,9 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
             // ---- the weights of (tap, hh): kSubs stages, or one 16-channel stage for the remainder
             for (int j = 0; j < (rem ? 1 : kSubs); ++j) {
               wait_staged();
-              mbar_wait(&empty_bar[stage], phase ^ 1);
-              uint8_t* st = ring + stage * S::kStageBytes;
-              uint64_t* fb = &full_bar[stage];
+              mbar_wait(&empty_bar[pos.stage], pos.phase ^ 1);
+              uint8_t* st = ring + pos.stage * S::kStageBytes;
+              uint64_t* fb = &full_bar[pos.stage];
               if (rem) {
                 mbar_arrive_expect_tx(fb, 2 * kRemBTile);
                 tma_load_3d(st, &tm_br_hi, fb, tap * kRemChannels, nt * BLOCK_N, 0);
@@ -201,10 +176,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
                 tma_load_3d(st, &tm_b_hi, fb, k0, nt * BLOCK_N, 0);
                 tma_load_3d(st + S::kBTile, &tm_b_lo, fb, k0, nt * BLOCK_N, 0);
               }
-              if (++stage == S::kStages) {
-                stage = 0;
-                phase ^= 1;
-              }
+              pos.advance();
             }
           }
           halos += n_halo;
@@ -215,24 +187,18 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
     // ------------------------------------------------------------ consumer warpgroups: wgmma + epilogue
     const int ct = threadIdx.x - kEpiWarp0 * 32;
     const int h = (warp - kEpiWarp0) >> 2;   // == ct >> 7, from the shuffled warp index: the compiler sees it uniform
-    const int wt = ct & 127;
     Epi epi(epi_params, epi_smem, shape);
     float acc[BLOCK_N / 2];                         // x-half h of the tile, all BLOCK_N columns
     float* stg = reinterpret_cast<float*>(ring);
     const uint32_t ring_u32 = smem_u32(ring);
     const uint32_t halo_u32 = smem_u32(halo);
-    int stage = 0;
-    uint32_t phase = 0;
+    RingPos<S::kStages> pos;
     int halos = 0;
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-      const int chunk = item % shape.n_chunks;
-      const int mt = (item / shape.n_chunks) % shape.m_tiles;
-      const int batch = item / (shape.n_chunks * shape.m_tiles);
-      const int nt_begin = chunk * shape.tiles_per_chunk;
-      const int nt_end = min(nt_begin + shape.tiles_per_chunk, shape.n_tiles);
-      epi.item_begin(batch, mt * kBlockM, chunk);
-      for (int nt = nt_begin; nt < nt_end; ++nt) {
-        epi.prefetch(batch, mt * kBlockM, nt * BLOCK_N);
+      const WorkItem w = work_item(shape, shape.m_tiles, item);
+      epi.item_begin(w.batch, w.mt * kBlockM, w.chunk);
+      for (int nt = w.nt_begin; nt < w.nt_end; ++nt) {
+        epi.prefetch(w.batch, w.mt * kBlockM, nt * BLOCK_N);
 #pragma unroll
         for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
         int prev = -1;        // ring stage of the previous weight stage
@@ -248,17 +214,15 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
           const uint32_t a_tap = halo_u32 + slot * kHaloSlotBytes + (ky * kHaloW + kx) * 16 + h * 8 * 16;
           const int subs = rem ? 1 : kSubs;
           for (int j = 0; j < subs; ++j) {
-            mbar_wait(&full_bar[stage], phase);
-            const uint32_t st = ring_u32 + stage * S::kStageBytes;
+            mbar_wait(&full_bar[pos.stage], pos.phase);
+            const uint32_t st = ring_u32 + pos.stage * S::kStageBytes;
             wgmma_fence();
             if (rem) {
               const uint64_t rb_hi = wgmma_desc_k_sw32(st);
               const uint64_t rb_lo = wgmma_desc_k_sw32(st + kRemBTile);
               const uint64_t ra_hi = wgmma_desc_k_noswz(a_tap, kHaloChunkBytes, kHaloW * 16);
               const uint64_t ra_lo = wgmma_desc_k_noswz(a_tap + kHaloPlaneBytes, kHaloChunkBytes, kHaloW * 16);
-              wgmma_f16<BLOCK_N>(acc, ra_hi, rb_hi, 1u);
-              wgmma_f16<BLOCK_N>(acc, ra_hi, rb_lo, 1u);
-              wgmma_f16<BLOCK_N>(acc, ra_lo, rb_hi, 1u);
+              wgmma_split<BLOCK_N>(acc, ra_hi, ra_lo, rb_hi, rb_lo);
             } else {
               const uint64_t db_hi = kBK == 64 ? wgmma_desc_k_sw128(st) : wgmma_desc_k_sw64(st);
               const uint64_t db_lo = kBK == 64 ? wgmma_desc_k_sw128(st + S::kBTile) : wgmma_desc_k_sw64(st + S::kBTile);
@@ -270,47 +234,30 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
                 // A: 16 channels = two chunks further; B: 32 bytes further inside the swizzle row (16-byte units)
                 const uint64_t a_adv = static_cast<uint64_t>(k * 2 * kHaloChunkBytes / 16);
                 const uint64_t b_adv = static_cast<uint64_t>(k * 2);
-                wgmma_f16<BLOCK_N>(acc, da_hi + a_adv, db_hi + b_adv, 1u);
-                wgmma_f16<BLOCK_N>(acc, da_hi + a_adv, db_lo + b_adv, 1u);
-                wgmma_f16<BLOCK_N>(acc, da_lo + a_adv, db_hi + b_adv, 1u);
+                wgmma_split<BLOCK_N>(acc, da_hi + a_adv, da_lo + a_adv, db_hi + b_adv, db_lo + b_adv);
               }
             }
             wgmma_commit();
             wgmma_wait<1>();   // the previous stage's MMAs are done: its weight slot (and halo, if last) may be refilled
             if (prev >= 0) mbar_arrive(&empty_bar[prev]);
             if (prev_halo >= 0) mbar_arrive(&halo_empty[prev_halo]);
-            prev = stage;
+            prev = pos.stage;
             prev_halo = (tap == kHaloTaps - 1 && j == subs - 1) ? slot : -1;
-            if (++stage == S::kStages) {
-              stage = 0;
-              phase ^= 1;
-            }
+            pos.advance();
           }
         }
         halos += n_halo;
-        wgmma_wait<0>();
-        wgmma_fence_regs(acc);
-        mbar_arrive(&empty_bar[prev]);
-        if (prev_halo >= 0) mbar_arrive(&halo_empty[prev_halo]);
-        // ---- stage the accumulator by tile pixel: row r of warpgroup h is pixel (r / 8) * 16 + 8 * h + r % 8
-        epi_group_sync();
-        {
-          const int p0 = 32 * (wt >> 5) + 8 * h + ((wt & 31) >> 2);
-          const int c0 = 2 * (wt & 3);
-#pragma unroll
-          for (int j = 0; j < BLOCK_N / 8; ++j) {
-            float* p = stg + p0 * S::kAccStride + c0 + 8 * j;
-            *reinterpret_cast<float2*>(p) = make_float2(acc[4 * j], acc[4 * j + 1]);
-            *reinterpret_cast<float2*>(p + 16 * S::kAccStride) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-          }
-        }
-        epi_group_sync();
-        epi.tile(smem_u32(stg + (ct & 127) * S::kAccStride), batch, mt * kBlockM, nt * BLOCK_N);
-        fence_proxy_async();   // staging reads / writes (generic proxy) before the next TMA writes into ring and halos
-        epi_group_sync();
-        if (ct == 0) mbar_arrive(acc_free);
+        // the accumulator is staged by tile pixel: row r of warpgroup h is pixel (r / 8) * 16 + 8 * h + r % 8
+        finish_tile<BLOCK_N>(
+            epi, acc,
+            [&] {
+              mbar_arrive(&empty_bar[prev]);
+              if (prev_halo >= 0) mbar_arrive(&halo_empty[prev_halo]);
+            },
+            [&] { stage_acc<BLOCK_N>(stg, acc_stride(BLOCK_N), acc, 8 * h, 16, 0); }, stg, ct, acc_free, w.batch,
+            w.mt * kBlockM, nt * BLOCK_N);
       }
-      epi.item_end(batch, mt * kBlockM, chunk);
+      epi.item_end(w.batch, w.mt * kBlockM, w.chunk);
     }
     tma_store_wait_all();
   }

@@ -179,107 +179,82 @@ static PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
   return fn;
 }
 
-// fp16 plane viewed as [batches][rows][K] with row stride ld and batch stride bs (elements);
-// box = 64 (K) x box_rows x 1, 128-byte swizzle, out-of-range elements read as zero.
+// One tiled tensor map over `rank` dims (innermost first) of fp16 or fp32 elements: byte strides of dims 1..rank-1,
+// box and element strides per dim (estr nullptr: all 1).  Out-of-range elements read as zero.
+static int encode_map(CUtensorMap* m, const char* what, const void* base, bool f32, int rank, const cuuint64_t* dims,
+                      const cuuint64_t* strides, const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapSwizzle swz,
+                      CUtensorMapL2promotion l2) {
+  auto enc = get_encode();
+  if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail("%s: base pointer not 16-byte aligned", what);
+  for (int i = 0; i + 1 < rank; ++i)
+    if (strides[i] % 16 != 0)
+      return fail("%s: stride of %llu bytes is not a multiple of 16", what, static_cast<unsigned long long>(strides[i]));
+  const cuuint32_t ones[4] = {1, 1, 1, 1};
+  CUresult r = enc(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank,
+                   const_cast<void*>(base), dims, strides, box, estr ? estr : ones, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
+                   l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (%s) failed with CUresult %d", what, static_cast<int>(r));
+  return 0;
+}
+static cuuint64_t u64(long v) { return static_cast<cuuint64_t>(v); }
+
+// fp16 plane viewed as [batches][rows][K] with row stride ld and batch stride bs (elements; 0 -> rows * ld);
+// box = box_k x box_rows x 1, swizzled rows of box_k elements.
 static CUtensorMapSwizzle swizzle_for(int box_k) {
   return box_k * 2 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : box_k * 2 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
 }
 static int make_map(CUtensorMap* m, const void* base, long K, long rows, long batches, long ld, long bs,
                     int box_rows, int box_k = kBlockK) {
-  auto enc = get_encode();
-  if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail("plane pointer not 16-byte aligned");
-  if ((ld * 2) % 16 != 0 || (bs * 2) % 16 != 0) return fail("plane strides must be multiples of 8 elements");
-  cuuint64_t dims[3] = {static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(rows), static_cast<cuuint64_t>(batches)};
-  cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld * 2), static_cast<cuuint64_t>((bs > 0 ? bs : rows * ld) * 2)};
-  cuuint32_t box[3] = {static_cast<cuuint32_t>(box_k), static_cast<cuuint32_t>(box_rows), 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(box_k),
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled failed with CUresult %d", static_cast<int>(r));
-  return 0;
+  const cuuint64_t dims[3] = {u64(K), u64(rows), u64(batches)};
+  const cuuint64_t strides[2] = {u64(ld * 2), u64((bs > 0 ? bs : rows * ld) * 2)};
+  const cuuint32_t box[3] = {static_cast<cuuint32_t>(box_k), static_cast<cuuint32_t>(box_rows), 1};
+  return encode_map(m, "plane", base, false, 3, dims, strides, box, nullptr, swizzle_for(box_k),
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
-// NHWC fp16 plane viewed as [N][H][W][C] (row stride ld elements); box = 64 channels x (16*stride) x (8*stride)
+// NHWC fp16 plane viewed as [N][H][W][C] (pixel stride ld elements); box = box_c channels x (16*stride) x (8*stride)
 // x 1 with element strides (1, stride, stride, 1): an 8 x 16 patch of (strided) pixels per load.
 static int make_map_nhwc(CUtensorMap* m, const void* base, int C, int W, int H, int N, long ld, int stride,
                          int box_c = kBlockK) {
-  auto enc = get_encode();
-  if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail("plane pointer not 16-byte aligned");
-  if ((ld * 2) % 16 != 0) return fail("NHWC channel stride must be a multiple of 8 elements (got %ld)", ld);
-  cuuint64_t dims[4] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H),
-                        static_cast<cuuint64_t>(N)};
-  cuuint64_t strides[3] = {static_cast<cuuint64_t>(ld * 2), static_cast<cuuint64_t>(ld * 2 * W),
-                           static_cast<cuuint64_t>(ld * 2 * W) * H};
-  cuuint32_t box[4] = {static_cast<cuuint32_t>(box_c), static_cast<cuuint32_t>(kConvTileW * stride),
-                       static_cast<cuuint32_t>(kConvTileH * stride), 1};
-  cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(box_c),
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (NHWC) failed with CUresult %d", static_cast<int>(r));
-  return 0;
+  const cuuint64_t dims[4] = {u64(C), u64(W), u64(H), u64(N)};
+  const cuuint64_t px = u64(ld * 2), strides[3] = {px, px * W, px * W * H};
+  const cuuint32_t box[4] = {static_cast<cuuint32_t>(box_c), static_cast<cuuint32_t>(kConvTileW * stride),
+                             static_cast<cuuint32_t>(kConvTileH * stride), 1};
+  const cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1};
+  return encode_map(m, "NHWC", base, false, 4, dims, strides, box, estr, swizzle_for(box_c),
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
 // NHWC fp16 plane [N][H][W][C] for conv3x3_halo_kernel: box = 8 channels x 18 x 10 pixels x 1, no swizzle (one
 // 8-channel chunk of a 10 x 18 halo).  The channel extent is C, so channels at or past C read as zeros.
 static int make_map_halo(CUtensorMap* m, const void* base, int C, int W, int H, int N, long ld) {
-  auto enc = get_encode();
-  if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail("plane pointer not 16-byte aligned");
-  if ((ld * 2) % 16 != 0) return fail("NHWC channel stride must be a multiple of 8 elements (got %ld)", ld);
-  cuuint64_t dims[4] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H),
-                        static_cast<cuuint64_t>(N)};
-  cuuint64_t strides[3] = {static_cast<cuuint64_t>(ld * 2), static_cast<cuuint64_t>(ld * 2 * W),
-                           static_cast<cuuint64_t>(ld * 2 * W) * H};
-  cuuint32_t box[4] = {8, static_cast<cuuint32_t>(kHaloW), static_cast<cuuint32_t>(kHaloH), 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (halo) failed with CUresult %d", static_cast<int>(r));
-  return 0;
+  const cuuint64_t dims[4] = {u64(C), u64(W), u64(H), u64(N)};
+  const cuuint64_t px = u64(ld * 2), strides[3] = {px, px * W, px * W * H};
+  const cuuint32_t box[4] = {8, static_cast<cuuint32_t>(kHaloW), static_cast<cuuint32_t>(kHaloH), 1};
+  return encode_map(m, "halo", base, false, 4, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_NONE,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
-// ---- output tensor maps for the TMA-store epilogues (epilogues.cuh OutMaps)
-// [batches][rows][cols] matrix (row stride ld, batch stride bs elements; bs = 0 -> rows * ld): box 32 x 32 x 1,
-// 64-byte swizzle for fp16 planes, 128-byte swizzle for fp32
+// ---- output tensor maps for the TMA-store epilogues (epilogues.cuh OutMaps): 64-byte swizzle for fp16 planes,
+// 128-byte swizzle for fp32
+static CUtensorMapSwizzle out_swizzle(bool f32) { return f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B; }
+// [batches][rows][cols] matrix (row stride ld, batch stride bs elements; bs = 0 -> rows * ld): box 32 x 32 x 1
 static int make_out_map(CUtensorMap* m, const void* base, bool f32, long cols, long rows, long batches, long ld, long bs) {
-  auto enc = get_encode();
-  if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
   const int esz = f32 ? 4 : 2;
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld * esz) % 16 != 0 || (bs * esz) % 16 != 0)
-    return fail("TMA-store output not 16-byte aligned");
-  cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows), static_cast<cuuint64_t>(batches)};
-  cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld * esz), static_cast<cuuint64_t>((bs > 0 ? bs : rows * ld) * esz)};
-  cuuint32_t box[3] = {32, 32, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims,
-                   strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                   CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (output) failed with CUresult %d", static_cast<int>(r));
-  return 0;
+  const cuuint64_t dims[3] = {u64(cols), u64(rows), u64(batches)};
+  const cuuint64_t strides[2] = {u64(ld * esz), u64((bs > 0 ? bs : rows * ld) * esz)};
+  const cuuint32_t box[3] = {32, 32, 1};
+  return encode_map(m, "output", base, f32, 3, dims, strides, box, nullptr, out_swizzle(f32),
+                    CU_TENSOR_MAP_L2_PROMOTION_NONE);
 }
 // NHWC [N][H][W][C] (pixel stride ld elements): box 32 channels x 16 x 2 pixels x 1 image
 static int make_out_map_nhwc(CUtensorMap* m, const void* base, bool f32, int C, int W, int H, int N, long ld) {
-  auto enc = get_encode();
-  if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
-  const int esz = f32 ? 4 : 2;
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld * esz) % 16 != 0) return fail("TMA-store NHWC output not 16-byte aligned");
-  cuuint64_t dims[4] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H), static_cast<cuuint64_t>(N)};
-  cuuint64_t strides[3] = {static_cast<cuuint64_t>(ld * esz), static_cast<cuuint64_t>(ld * esz) * W,
-                           static_cast<cuuint64_t>(ld * esz) * W * H};
-  cuuint32_t box[4] = {32, static_cast<cuuint32_t>(kConvTileW), 2, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims,
-                   strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                   CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (NHWC output) failed with CUresult %d", static_cast<int>(r));
-  return 0;
+  const cuuint64_t dims[4] = {u64(C), u64(W), u64(H), u64(N)};
+  const cuuint64_t px = u64(ld * (f32 ? 4 : 2)), strides[3] = {px, px * W, px * W * H};
+  const cuuint32_t box[4] = {32, static_cast<cuuint32_t>(kConvTileW), 2, 1};
+  return encode_map(m, "NHWC output", base, f32, 4, dims, strides, box, nullptr, out_swizzle(f32),
+                    CU_TENSOR_MAP_L2_PROMOTION_NONE);
 }
 // planes (+ optional fp32) of a [batches][rows][cols] output
 static int fill_out_maps(OutMaps* om, const void* hi, const void* lo, long ld_pl, const float* f32, long ld_f32, long cols,
@@ -350,7 +325,7 @@ static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const t
                       cudaStream_t st) {
   using S = GemmSmem<BN, Epi::kSmemBytes>;
   constexpr int smem_bytes = S::kRingBytes + S::kBarBytes + Epi::kSmemBytes;
-  static_assert(smem_bytes <= 232448, "shared memory budget exceeded");
+  static_assert(smem_bytes <= kSmemLimit, "shared memory budget exceeded");
   return launch_persistent<&gemm_split_kernel<BN, Epi>>(tag, s, smem_bytes, sms, st, maps.a_hi, maps.a_lo, maps.b_hi,
                                                           maps.b_lo, maps.ar_hi, maps.ar_lo, maps.br_hi, maps.br_lo, s, ep);
 }
@@ -408,6 +383,28 @@ static void conv_layout(int cin, int* cin_blocks, int* rem) {
     *rem = 0;
   }
 }
+// The implicit GEMM of convolution d with BN-wide n tiles (one per work item), and the output geometry its epilogue
+// reads.  *rem: the remainder channels per tap (0: none).
+template <int BN, class Params>
+static int conv_shape(const ConvDesc& d, const Planes& wgt_rem, GemmShape* s, Params* ep, int* rem) {
+  int cin_blocks = 0;
+  conv_layout(d.Cin, &cin_blocks, rem);
+  if (*rem && (!wgt_rem.hi || !wgt_rem.lo)) return fail("convolution with Cin=%d needs remainder weight planes", d.Cin);
+  const int taps = d.ksize * d.ksize;
+  const int tiles_h = (d.H_out + kConvTileH - 1) / kConvTileH;
+  const int tiles_w = (d.W_out + kConvTileW - 1) / kConvTileW;
+  const int m_tiles = tiles_h * tiles_w, n_tiles = (d.Cout + BN - 1) / BN;
+  const int rem_groups = *rem ? (taps + kRemTapsPerStage - 1) / kRemTapsPerStage : 0;
+  *s = GemmShape{d.N, m_tiles * kBlockM, d.Cout, taps * cin_blocks * kBlockK, /*b_batched=*/0, m_tiles, n_tiles,
+                 /*n_chunks=*/n_tiles, /*tiles_per_chunk=*/1,
+                 ConvGeom{1, tiles_w, d.stride, d.pad, d.ksize, cin_blocks, taps, taps * cin_blocks, rem_groups},
+                 /*live_count=*/nullptr, 0};
+  ep->H_out = d.H_out;
+  ep->W_out = d.W_out;
+  ep->tiles_w = tiles_w;
+  return 0;
+}
+
 template <int BN, bool kUpsample>
 static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_rem, const ConvDesc& d,
                        const typename EpiConv<BN, kUpsample>::Params& ep_in, cudaStream_t st) {
@@ -415,25 +412,9 @@ static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_re
   int sms = 0;
   LB_TRY(device_check(&sms));
   GemmShape s;
-  int cin_blocks = 0, rem = 0;
-  conv_layout(d.Cin, &cin_blocks, &rem);
-  const int taps = d.ksize * d.ksize;
-  const int tiles_h = (d.H_out + kConvTileH - 1) / kConvTileH;
-  const int tiles_w = (d.W_out + kConvTileW - 1) / kConvTileW;
-  s.batches = d.N;
-  s.M = tiles_h * tiles_w * kBlockM;
-  s.N = d.Cout;
-  s.K = taps * cin_blocks * kBlockK;
-  s.b_batched = 0;
-  s.m_tiles = tiles_h * tiles_w;
-  s.n_tiles = (d.Cout + BN - 1) / BN;
-  s.n_chunks = s.n_tiles;
-  s.tiles_per_chunk = 1;
-  const int rem_groups = rem ? (taps + kRemTapsPerStage - 1) / kRemTapsPerStage : 0;
-  s.conv = ConvGeom{1, tiles_w, d.stride, d.pad, d.ksize, cin_blocks, taps, taps * cin_blocks, rem_groups};
-  s.live_count = nullptr;
-  s.live_unit_rows = 0;
-  if (rem && (!wgt_rem.hi || !wgt_rem.lo)) return fail("convolution with Cin=%d needs remainder weight planes", d.Cin);
+  typename Epi::Params ep = ep_in;
+  int rem = 0;
+  LB_TRY(conv_shape<BN>(d, wgt_rem, &s, &ep, &rem));
   GemmMaps mp;
   LB_TRY(make_map_nhwc(&mp.a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride));
   LB_TRY(make_map_nhwc(&mp.a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride));
@@ -442,15 +423,11 @@ static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_re
   if (rem) {
     LB_TRY(make_map_nhwc(&mp.ar_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, kRemChannels));
     LB_TRY(make_map_nhwc(&mp.ar_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, kRemChannels));
-    LB_TRY(make_map(&mp.br_hi, wgt_rem.hi, taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
-    LB_TRY(make_map(&mp.br_lo, wgt_rem.lo, taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
+    LB_TRY(make_map(&mp.br_hi, wgt_rem.hi, s.conv.taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
+    LB_TRY(make_map(&mp.br_lo, wgt_rem.lo, s.conv.taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
   } else {
     mp.ar_hi = mp.a_hi; mp.ar_lo = mp.a_lo; mp.br_hi = mp.b_hi; mp.br_lo = mp.b_lo;
   }
-  typename Epi::Params ep = ep_in;
-  ep.H_out = d.H_out;
-  ep.W_out = d.W_out;
-  ep.tiles_w = tiles_w;
   return launch_raw<BN, Epi>(TAG_CONV, mp, s, ep, sms, st);
 }
 
@@ -460,46 +437,26 @@ static int launch_conv_halo(const Planes& in, const Planes& wgt, const Planes& w
                             const typename EpiConv<BN, false>::Params& ep_in, cudaStream_t st) {
   using Epi = EpiConv<BN, false>;
   using S = HaloSmem<BN, Epi::kSmemBytes>;
-  static_assert(S::kTotalBytes <= 232448, "shared memory budget exceeded");
+  static_assert(S::kTotalBytes <= kSmemLimit, "shared memory budget exceeded");
   int sms = 0;
   LB_TRY(device_check(&sms));
   if (d.ksize != 3 || d.stride != 1 || d.pad != 1) return fail("the halo convolution is built for 3x3, stride 1, pad 1");
-  int cin_blocks = 0, rem = 0;
-  conv_layout(d.Cin, &cin_blocks, &rem);
-  const int taps = kHaloTaps;
-  const int tiles_h = (d.H_out + kConvTileH - 1) / kConvTileH;
-  const int tiles_w = (d.W_out + kConvTileW - 1) / kConvTileW;
   GemmShape s;
-  s.batches = d.N;
-  s.M = tiles_h * tiles_w * kBlockM;
-  s.N = d.Cout;
-  s.K = taps * cin_blocks * kBlockK;
-  s.b_batched = 0;
-  s.m_tiles = tiles_h * tiles_w;
-  s.n_tiles = (d.Cout + BN - 1) / BN;
-  s.n_chunks = s.n_tiles;
-  s.tiles_per_chunk = 1;
-  const int rem_groups = rem ? (taps + kRemTapsPerStage - 1) / kRemTapsPerStage : 0;
-  s.conv = ConvGeom{1, tiles_w, 1, 1, 3, cin_blocks, taps, taps * cin_blocks, rem_groups};
-  s.live_count = nullptr;
-  s.live_unit_rows = 0;
-  if (rem && (!wgt_rem.hi || !wgt_rem.lo)) return fail("convolution with Cin=%d needs remainder weight planes", d.Cin);
+  typename Epi::Params ep = ep_in;
+  int rem = 0;
+  LB_TRY(conv_shape<BN>(d, wgt_rem, &s, &ep, &rem));
   CUtensorMap a_hi, a_lo, b_hi, b_lo, br_hi, br_lo;
   LB_TRY(make_map_halo(&a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld));
   LB_TRY(make_map_halo(&a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld));
   LB_TRY(make_map(&b_hi, wgt.hi, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
   LB_TRY(make_map(&b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
   if (rem) {
-    LB_TRY(make_map(&br_hi, wgt_rem.hi, taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
-    LB_TRY(make_map(&br_lo, wgt_rem.lo, taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
+    LB_TRY(make_map(&br_hi, wgt_rem.hi, kHaloTaps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
+    LB_TRY(make_map(&br_lo, wgt_rem.lo, kHaloTaps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
   } else {
     br_hi = b_hi;
     br_lo = b_lo;
   }
-  typename Epi::Params ep = ep_in;
-  ep.H_out = d.H_out;
-  ep.W_out = d.W_out;
-  ep.tiles_w = tiles_w;
   return launch_persistent<&conv3x3_halo_kernel<BN, Epi>>(TAG_CONV, s, S::kTotalBytes, sms, st, a_hi, a_lo, b_hi, b_lo,
                                                             br_hi, br_lo, s, ep);
 }

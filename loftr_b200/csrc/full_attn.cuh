@@ -111,21 +111,20 @@ full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid
       tma_load_3d(s_q, &tm_q_hi, q_bar, head * kFaD, qt * kFaRows, grp);
       tma_load_3d(s_q + kFwQPlane, &tm_q_lo, q_bar, head * kFaD, qt * kFaRows, grp);
     }
-    int stage = 0;
-    uint32_t phase = 0;
+    RingPos<kFwStages> pos;
     for (int kt = 0; kt < n_tiles; ++kt) {
-      mbar_wait(&empty_bar[stage], phase ^ 1);
+      mbar_wait(&empty_bar[pos.stage], pos.phase ^ 1);
       const int key0 = kt * kFaKeys;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int k = key0 + lane + 32 * h;
         const bool ok = k < p.Ls && (p.mask == nullptr || p.mask[srow0 + k] != 0);
-        s_bias[stage * kFaKeys + lane + 32 * h] = ok ? 0.f : -INFINITY;
+        s_bias[pos.stage * kFaKeys + lane + 32 * h] = ok ? 0.f : -INFINITY;
       }
       __syncwarp();
       if (lane == 0) {
-        uint8_t* st = s_ring + stage * kFwStage;
-        uint64_t* fb = &full_bar[stage];
+        uint8_t* st = s_ring + pos.stage * kFwStage;
+        uint64_t* fb = &full_bar[pos.stage];
         mbar_arrive_expect_tx(fb, kFwStage);
         tma_load_3d(st, &tm_kv_hi, fb, head * kFaD, key0, grp);
         tma_load_3d(st + kFwKvPlane, &tm_kv_lo, fb, head * kFaD, key0, grp);
@@ -133,10 +132,7 @@ full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid
         tma_load_3d(st + 3 * kFwKvPlane, &tm_kv_lo, fb, p.v_col0 + head * kFaD, key0, grp);
       }
       __syncwarp();
-      if (++stage == kFwStages) {
-        stage = 0;
-        phase ^= 1;
-      }
+      pos.advance();
     }
     return;
   }
@@ -151,11 +147,10 @@ full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid
   for (int i = 0; i < 16; ++i) o[i] = 0.f;
   float m_lo = -INFINITY, m_hi = -INFINITY, l_lo = 0.f, l_hi = 0.f;
   mbar_wait(q_bar, 0);
-  int stage = 0;
-  uint32_t phase = 0;
+  RingPos<kFwStages> pos;
   for (int kt = 0; kt < n_tiles; ++kt) {
-    mbar_wait(&full_bar[stage], phase);
-    const uint32_t st = smem_u32(s_ring + stage * kFwStage);
+    mbar_wait(&full_bar[pos.stage], pos.phase);
+    const uint32_t st = smem_u32(s_ring + pos.stage * kFwStage);
     float s[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) s[i] = 0.f;
@@ -165,16 +160,14 @@ full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid
       const uint64_t adv = static_cast<uint64_t>(kk * 2);   // 16 fp16 = 32 bytes along K inside the swizzle row
       const uint64_t ah = wgmma_desc_k_sw64(q_hi) + adv, al = wgmma_desc_k_sw64(q_lo) + adv;
       const uint64_t bh = wgmma_desc_k_sw64(st) + adv, bl = wgmma_desc_k_sw64(st + kFwKvPlane) + adv;
-      wgmma_f16<64>(s, ah, bh, 1u);
-      wgmma_f16<64>(s, ah, bl, 1u);
-      wgmma_f16<64>(s, al, bh, 1u);
+      wgmma_split<64>(s, ah, al, bh, bl);
     }
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs(s);
 
     // ---- scale, mask, online softmax: s[4j + 0..1] row g, s[4j + 2..3] row g + 8, columns 8j + 2t (+1)
-    const float* bias = s_bias + stage * kFaKeys;
+    const float* bias = s_bias + pos.stage * kFaKeys;
     float mx_lo = -INFINITY, mx_hi = -INFINITY;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -236,11 +229,8 @@ full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs(o);
-    mbar_arrive(&empty_bar[stage]);
-    if (++stage == kFwStages) {
-      stage = 0;
-      phase ^= 1;
-    }
+    mbar_arrive(&empty_bar[pos.stage]);
+    pos.advance();
   }
 
   // ---- epilogue: O / rowsum -> fp16 planes; padded queries and rows without a valid key write 0

@@ -92,23 +92,114 @@ struct EpiRowBound<Epi, decltype(void(Epi::kNoRowBound))> {
 // K-major operand tile descriptor of a k-block (128-byte swizzle rows).
 __device__ __forceinline__ uint64_t desc_k(uint32_t smem_addr) { return wgmma_desc_k_sw128(smem_addr); }
 
+// Dynamic shared memory a block may opt in to on the H100 (227 KB).
+constexpr int kSmemLimit = 232448;
+
+// Accumulator staging of the persistent kernels (gemm_split_kernel, conv3x3_halo_kernel): 128 rows of BLOCK_N + 4 fp32
+// over the dead ring.  A row stride of an odd multiple of 16 bytes keeps the epilogue's row-per-lane 16-byte reads free
+// of bank conflicts.  +32 floats: an epilogue's last 32-column group may run past N.
+__host__ __device__ constexpr int acc_stride(int block_n) { return block_n + 4; }   // floats
+__host__ __device__ constexpr int acc_bytes(int block_n) { return (kBlockM * acc_stride(block_n) + 32) * 4; }
+
 // Shared memory: [TMA ring | accumulator staging (aliased)][epilogue area][mbarriers].
-// The staging tile is 128 rows of BLOCK_N + 4 fp32: a row stride of an odd multiple of 16 bytes keeps the epilogue's
-// row-per-lane 16-byte reads free of bank conflicts.  +32 floats: an epilogue's last 32-column group may run past N.
 template <int BLOCK_N, int kEpiBytes = 0>
 struct GemmSmem {
   static constexpr int kATile = kBlockM * kBlockK * 2;          // 16 KB per plane
   static constexpr int kBTile = BLOCK_N * kBlockK * 2;          // per plane
   static constexpr int kStageBytes = 2 * kATile + 2 * kBTile;   // hi + lo of A and B
   static constexpr int kBarBytes = 256;
-  static constexpr int kAccStride = BLOCK_N + 4;                // floats
-  static constexpr int kAccBytes = (kBlockM * kAccStride + 32) * 4;
-  static constexpr int kFit = (232448 - kBarBytes - kEpiBytes) / kStageBytes;
+  static constexpr int kAccBytes = acc_bytes(BLOCK_N);
+  static constexpr int kFit = (kSmemLimit - kBarBytes - kEpiBytes) / kStageBytes;
   static constexpr int kWant = (192 * 1024) / kStageBytes;      // 2 (96 KB) / 3 (64 KB) / 4 (48 KB)
   static constexpr int kStages = kFit < kWant ? kFit : kWant;
   static_assert(kStages >= 2, "the TMA ring needs two stages");
   static constexpr int kRingBytes = kStages * kStageBytes > kAccBytes ? kStages * kStageBytes : kAccBytes;
 };
+
+// ---- pieces shared by the persistent kernels (gemm_split_kernel, conv3x3_halo_kernel)
+
+// Set-up: traps on a misaligned shared-memory base, prefetches the four main tensor-map descriptors, initialises the
+// ring barriers, the kernel's own barriers (init_more) and acc_free, then triggers the next grid and waits for the
+// previous one.  Returns the warp index broadcast from lane 0: provably warp-uniform, so the role branches on it are
+// not divergent paths.
+template <int kStages, class InitMore>
+__device__ __forceinline__ int persistent_setup(const uint8_t* smem_raw, const CUtensorMap* tm_a_hi,
+                                                const CUtensorMap* tm_a_lo, const CUtensorMap* tm_b_hi,
+                                                const CUtensorMap* tm_b_lo, uint64_t* full_bar, uint64_t* empty_bar,
+                                                uint64_t* acc_free, InitMore init_more) {
+  if ((smem_u32(smem_raw) & 1023u) != 0) asm volatile("trap;");
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  if (warp == kProducerWarp && lane == 0) {
+    tma_prefetch_desc(tm_a_hi);
+    tma_prefetch_desc(tm_a_lo);
+    tma_prefetch_desc(tm_b_hi);
+    tma_prefetch_desc(tm_b_lo);
+  }
+  if (warp == 0 && lane == 0) {
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], kEpiThreads);   // every consumer thread arrives (keeps the MMA window uniform)
+    }
+    init_more();
+    mbar_init(acc_free, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  // Programmatic dependent launch (engine.cu sets the launch attribute unless LOFTR_B200_PDL=0): the next kernel's CTAs
+  // take over SMs as ours exit and run their own set-up, while everything after this waits for the previous grid.
+  pdl_trigger();
+  pdl_wait();
+  return warp;
+}
+
+// Work item `item` = (batch, m tile, chunk of consecutive n tiles); items are strided over the persistent CTAs.
+struct WorkItem {
+  int batch, mt, chunk, nt_begin, nt_end;
+};
+__device__ __forceinline__ WorkItem work_item(const GemmShape& s, int m_tiles, int item) {
+  WorkItem w;
+  w.chunk = item % s.n_chunks;
+  w.mt = (item / s.n_chunks) % m_tiles;
+  w.batch = item / (s.n_chunks * m_tiles);
+  w.nt_begin = w.chunk * s.tiles_per_chunk;
+  w.nt_end = min(w.nt_begin + s.tiles_per_chunk, s.n_tiles);
+  return w;
+}
+
+// Stores an m64nN accumulator (wgmma_f16 fragment layout) row-major with a row stride of `stride` floats: thread t of
+// the warpgroup holds rows row0 + 2 step (t / 32) + (t % 32) / 4 and that + step, columns col0 + 8 j + 2 (t % 4) (+1).
+template <int N>
+__device__ __forceinline__ void stage_acc(float* stg, int stride, const float (&acc)[N / 2], int row0, int step,
+                                          int col0) {
+  const int t = threadIdx.x & 127;
+  const int r = 2 * step * (t >> 5) + ((t & 31) >> 2);
+  const int c = col0 + 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    float* p = stg + (row0 + r) * stride + c + 8 * j;
+    *reinterpret_cast<float2*>(p) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(p + step * stride) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  }
+}
+
+// Tile end of a consumer thread, after the tile's last wgmma_commit: drain the MMAs, release the ring slots they read
+// (release_ring), stage the accumulator over the ring (stage) once both warpgroups' MMAs are done with it, run the
+// epilogue on this thread's staged row and hand the ring back to the producer (acc_free).
+template <int BLOCK_N, class Epi, class Acc, class Release, class Stage>
+__device__ __forceinline__ void finish_tile(Epi& epi, Acc& acc, Release release_ring, Stage stage, const float* stg,
+                                            int ct, uint64_t* acc_free, int batch, int m0, int n0) {
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+  release_ring();
+  epi_group_sync();
+  stage();
+  epi_group_sync();
+  epi.tile(smem_u32(stg + (ct & 127) * acc_stride(BLOCK_N)), batch, m0, n0);
+  fence_proxy_async();   // staging reads / writes (generic proxy) before the next TMA writes over them
+  epi_group_sync();
+  if (ct == 0) mbar_arrive(acc_free);
+}
 
 // Epilogue contract (all methods are called by the 256 consumer threads only):
 //   struct Params;                               // trivially copyable, passed by value to the kernel
@@ -132,42 +223,18 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   static_assert(kN % 8 == 0, "wgmma N must be a multiple of 8");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // The swizzled tiles (ring, TMA-store staging) need a 1024-byte aligned base.  With no static shared memory the
-  // dynamic window starts 1024-aligned (checked below: a misaligned base traps instead of corrupting tiles); the
-  // pointers stay plain offsets of the __shared__ array -- through an integer round trip the compiler loses the
-  // address space and every epilogue smem access becomes a generic LD/ST.
+  // dynamic window starts 1024-aligned (checked in persistent_setup: a misaligned base traps instead of corrupting
+  // tiles); the pointers stay plain offsets of the __shared__ array -- through an integer round trip the compiler loses
+  // the address space and every epilogue smem access becomes a generic LD/ST.
   uint8_t* ring = smem_raw;
   uint8_t* epi_smem = smem_raw + S::kRingBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_raw + S::kRingBytes + Epi::kSmemBytes);
   uint64_t* empty_bar = full_bar + S::kStages;
   uint64_t* acc_free = empty_bar + S::kStages;
   static_assert(Epi::kSmemBytes % 16 == 0, "epilogue area must keep the barriers aligned");
-  if ((smem_u32(smem_raw) & 1023u) != 0) asm volatile("trap;");
-
-  // warp index broadcast from lane 0: provably warp-uniform, so the role branches below are not divergent paths
-  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
+  const int warp = persistent_setup<S::kStages>(smem_raw, &tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, full_bar, empty_bar,
+                                                acc_free, [] {});
   const int lane = threadIdx.x & 31;
-
-  if (warp == kProducerWarp && lane == 0) {
-    tma_prefetch_desc(&tm_a_hi);
-    tma_prefetch_desc(&tm_a_lo);
-    tma_prefetch_desc(&tm_b_hi);
-    tma_prefetch_desc(&tm_b_lo);
-  }
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < S::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kEpiThreads);   // every consumer thread arrives (keeps the MMA window uniform)
-    }
-    mbar_init(acc_free, 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  // Programmatic dependent launch (engine.cu sets the launch attribute unless LOFTR_B200_PDL=0; without it both
-  // instructions are no-ops): the NEXT kernel of the stream may be scheduled as soon as every CTA of this grid got
-  // here -- its CTAs take over SMs as ours exit and run their own set-up (barriers, descriptor prefetch) -- while
-  // everything below this line first waits until the PREVIOUS grid has completed and flushed.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
 
   // k-blocks of one output tile: K / 64 full blocks (+ the channel-remainder groups of a convolution)
   const int num_kb = shape.conv.enabled ? shape.conv.n_main + shape.conv.rem_groups : shape.K / kBlockK;
@@ -183,28 +250,22 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     const long live = min(static_cast<long>(max(*shape.live_count, 0)) * shape.live_unit_rows, static_cast<long>(shape.M));
     m_tiles = min(m_tiles, static_cast<int>((live + kBlockM - 1) / kBlockM));
   }
-  // work items (batch, m_tile, chunk), strided over the persistent CTAs
   const int total_items = shape.batches * m_tiles * shape.n_chunks;
 
   if (warp == kProducerWarp) {
     // ------------------------------------------------------------ TMA producer
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      RingPos<S::kStages> pos;
       uint32_t tiles = 0;
       for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-        const int chunk = item % shape.n_chunks;
-        const int mt = (item / shape.n_chunks) % m_tiles;
-        const int batch = item / (shape.n_chunks * m_tiles);
-        const int nt_begin = chunk * shape.tiles_per_chunk;
-        const int nt_end = min(nt_begin + shape.tiles_per_chunk, shape.n_tiles);
-        for (int nt = nt_begin; nt < nt_end; ++nt) {
+        const WorkItem w = work_item(shape, m_tiles, item);
+        for (int nt = w.nt_begin; nt < w.nt_end; ++nt) {
           if (tiles > 0) mbar_wait(acc_free, (tiles - 1) & 1);   // the previous tile's staged accumulator is consumed
           ++tiles;
           for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* st = ring + stage * S::kStageBytes;
-            uint64_t* fb = &full_bar[stage];
+            mbar_wait(&empty_bar[pos.stage], pos.phase ^ 1);
+            uint8_t* st = ring + pos.stage * S::kStageBytes;
+            uint64_t* fb = &full_bar[pos.stage];
             const bool rem_group = shape.conv.enabled && kb >= shape.conv.n_main;
             if (rem_group) {
               // ---- channel remainder: up to four taps, each a 16-channel box of A (hi, lo) and of the weights
@@ -212,7 +273,7 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
               const int rem_t0 = (kb - g.n_main) * kRemTapsPerStage;
               const int rem_nt = min(kRemTapsPerStage, g.taps - rem_t0);
               mbar_arrive_expect_tx(fb, static_cast<uint32_t>(rem_nt) * kTapBytes);
-              const int ty = mt / g.tiles_w, tx = mt - ty * g.tiles_w;
+              const int ty = w.mt / g.tiles_w, tx = w.mt - ty * g.tiles_w;
               for (int t = 0; t < rem_nt; ++t) {
                 const int tap = rem_t0 + t;
                 const int ky = tap / g.taps_w, kx = tap - ky * g.taps_w;
@@ -220,8 +281,8 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                 const int y = ty * kConvTileH * g.stride + ky - g.pad;
                 uint8_t* base = st + t * kTapBytes;
                 const int c0 = g.cin_blocks * kBlockK;
-                tma_load_4d(base, &tm_ar_hi, fb, c0, x, y, batch);
-                tma_load_4d(base + kRemATile, &tm_ar_lo, fb, c0, x, y, batch);
+                tma_load_4d(base, &tm_ar_hi, fb, c0, x, y, w.batch);
+                tma_load_4d(base + kRemATile, &tm_ar_lo, fb, c0, x, y, w.batch);
                 tma_load_3d(base + 2 * kRemATile, &tm_br_hi, fb, tap * kRemChannels, nt * BLOCK_N, 0);
                 tma_load_3d(base + 2 * kRemATile + kRemBTile, &tm_br_lo, fb, tap * kRemChannels, nt * BLOCK_N, 0);
               }
@@ -232,24 +293,21 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                 const ConvGeom& g = shape.conv;
                 const int tap = kb / g.cin_blocks, cb = kb - tap * g.cin_blocks;
                 const int ky = tap / g.taps_w, kx = tap - ky * g.taps_w;
-                const int ty = mt / g.tiles_w, tx = mt - ty * g.tiles_w;
+                const int ty = w.mt / g.tiles_w, tx = w.mt - ty * g.tiles_w;
                 const int x = tx * kConvTileW * g.stride + kx - g.pad;
                 const int y = ty * kConvTileH * g.stride + ky - g.pad;
-                tma_load_4d(st, &tm_a_hi, fb, cb * kBlockK, x, y, batch);
-                tma_load_4d(st + S::kATile, &tm_a_lo, fb, cb * kBlockK, x, y, batch);
+                tma_load_4d(st, &tm_a_hi, fb, cb * kBlockK, x, y, w.batch);
+                tma_load_4d(st + S::kATile, &tm_a_lo, fb, cb * kBlockK, x, y, w.batch);
               } else {
-                tma_load_3d(st, &tm_a_hi, fb, kb * kBlockK, mt * kBlockM, batch);
-                tma_load_3d(st + S::kATile, &tm_a_lo, fb, kb * kBlockK, mt * kBlockM, batch);
+                tma_load_3d(st, &tm_a_hi, fb, kb * kBlockK, w.mt * kBlockM, w.batch);
+                tma_load_3d(st + S::kATile, &tm_a_lo, fb, kb * kBlockK, w.mt * kBlockM, w.batch);
               }
               // ---- B
-              const int bb = shape.b_batched ? batch : 0;
+              const int bb = shape.b_batched ? w.batch : 0;
               tma_load_3d(st + 2 * S::kATile, &tm_b_hi, fb, kb * kBlockK, nt * BLOCK_N, bb);
               tma_load_3d(st + 2 * S::kATile + S::kBTile, &tm_b_lo, fb, kb * kBlockK, nt * BLOCK_N, bb);
             }
-            if (++stage == S::kStages) {
-              stage = 0;
-              phase ^= 1;
-            }
+            pos.advance();
           }
         }
       }
@@ -258,29 +316,23 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     // ------------------------------------------------------------ consumer warpgroups: wgmma + epilogue
     const int ct = threadIdx.x - kEpiWarp0 * 32;   // 0..255
     const int h = ct >> 7;                          // column half of the tile
-    const int wt = ct & 127;                        // thread within the warpgroup
     Epi epi(epi_params, epi_smem, shape);
     float acc[2][kN / 2];                           // rows [0, 64) and [64, 128) of this warpgroup's column half
     float* stg = reinterpret_cast<float*>(ring);
-    int stage = 0;
-    uint32_t phase = 0;
+    RingPos<S::kStages> pos;
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-      const int chunk = item % shape.n_chunks;
-      const int mt = (item / shape.n_chunks) % m_tiles;
-      const int batch = item / (shape.n_chunks * m_tiles);
-      const int nt_begin = chunk * shape.tiles_per_chunk;
-      const int nt_end = min(nt_begin + shape.tiles_per_chunk, shape.n_tiles);
-      epi.item_begin(batch, mt * kBlockM, chunk);
-      for (int nt = nt_begin; nt < nt_end; ++nt) {
-        epi.prefetch(batch, mt * kBlockM, nt * BLOCK_N);
+      const WorkItem w = work_item(shape, m_tiles, item);
+      epi.item_begin(w.batch, w.mt * kBlockM, w.chunk);
+      for (int nt = w.nt_begin; nt < w.nt_end; ++nt) {
+        epi.prefetch(w.batch, w.mt * kBlockM, nt * BLOCK_N);
         // a zeroed accumulator instead of a first MMA with scale-d = 0: the previous tile's values are dead after
         // staging, so the epilogue does not have to keep them in registers
 #pragma unroll
         for (int i = 0; i < kN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
         int prev = -1;
         for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          const uint32_t st = smem_u32(ring + stage * S::kStageBytes);
+          mbar_wait(&full_bar[pos.stage], pos.phase);
+          const uint32_t st = smem_u32(ring + pos.stage * S::kStageBytes);
           wgmma_fence();
           if (shape.conv.enabled && kb >= shape.conv.n_main) {
             // remainder group: one K = 16 step per tap, 32-byte swizzle rows (kb > 0 here: always accumulate)
@@ -296,9 +348,7 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                 const uint64_t ra_lo = wgmma_desc_k_sw32(base + kRemATile + a_off);
                 const uint64_t rb_hi = wgmma_desc_k_sw32(base + 2 * kRemATile + b_off);
                 const uint64_t rb_lo = wgmma_desc_k_sw32(base + 2 * kRemATile + kRemBTile + b_off);
-                wgmma_f16<kN>(acc[mh], ra_hi, rb_hi, 1u);
-                wgmma_f16<kN>(acc[mh], ra_hi, rb_lo, 1u);
-                wgmma_f16<kN>(acc[mh], ra_lo, rb_hi, 1u);
+                wgmma_split<kN>(acc[mh], ra_hi, ra_lo, rb_hi, rb_lo);
               }
             }
           } else {
@@ -314,47 +364,25 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
               for (int k = 0; k < kBlockK / kMmaK; ++k) {
                 // advance 16 fp16 = 32 bytes along K inside the swizzle row: +2 in 16-byte units
                 const uint64_t adv = static_cast<uint64_t>(k * 2);
-                wgmma_f16<kN>(acc[mh], da_hi + adv, db_hi + adv, 1u);
-                wgmma_f16<kN>(acc[mh], da_hi + adv, db_lo + adv, 1u);
-                wgmma_f16<kN>(acc[mh], da_lo + adv, db_hi + adv, 1u);
+                wgmma_split<kN>(acc[mh], da_hi + adv, da_lo + adv, db_hi + adv, db_lo + adv);
               }
             }
           }
           wgmma_commit();
           wgmma_wait<1>();   // the previous k-block's MMAs are done: its slot may be refilled
           if (prev >= 0) mbar_arrive(&empty_bar[prev]);
-          prev = stage;
-          if (++stage == S::kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
+          prev = pos.stage;
+          pos.advance();
         }
-        wgmma_wait<0>();
-        wgmma_fence_regs(acc[0]);
-        wgmma_fence_regs(acc[1]);
-        mbar_arrive(&empty_bar[prev]);
-        // ---- stage the accumulator (row-major) over the ring, once both warpgroups' MMAs have read it
-        epi_group_sync();
-        {
-          const int r0 = 16 * (wt >> 5) + ((wt & 31) >> 2);
-          const int c0 = h * kN + 2 * (wt & 3);
-#pragma unroll
-          for (int mh = 0; mh < 2; ++mh) {
-#pragma unroll
-            for (int j = 0; j < kN / 8; ++j) {
-              float* p = stg + (mh * 64 + r0) * S::kAccStride + c0 + 8 * j;
-              *reinterpret_cast<float2*>(p) = make_float2(acc[mh][4 * j], acc[mh][4 * j + 1]);
-              *reinterpret_cast<float2*>(p + 8 * S::kAccStride) = make_float2(acc[mh][4 * j + 2], acc[mh][4 * j + 3]);
-            }
-          }
-        }
-        epi_group_sync();
-        epi.tile(smem_u32(stg + (ct & 127) * S::kAccStride), batch, mt * kBlockM, nt * BLOCK_N);
-        fence_proxy_async();   // staging reads / writes (generic proxy) before the next TMA writes into the ring
-        epi_group_sync();
-        if (ct == 0) mbar_arrive(acc_free);
+        finish_tile<BLOCK_N>(
+            epi, acc, [&] { mbar_arrive(&empty_bar[prev]); },
+            [&] {
+              stage_acc<kN>(stg, acc_stride(BLOCK_N), acc[0], 0, 8, h * kN);
+              stage_acc<kN>(stg, acc_stride(BLOCK_N), acc[1], 64, 8, h * kN);
+            },
+            stg, ct, acc_free, w.batch, w.mt * kBlockM, nt * BLOCK_N);
       }
-      epi.item_end(batch, mt * kBlockM, chunk);
+      epi.item_end(w.batch, w.mt * kBlockM, w.chunk);
     }
     tma_store_wait_all();   // bulk stores issued by this thread (if any) have landed before the CTA may exit
   }

@@ -106,12 +106,11 @@ kv_gemm_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
 
   if (warp == 4) {
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      RingPos<kKvGemmStages> pos;
       for (int i = 0; i < nkb; ++i) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* st = smem + stage * kKvStageBytes;
-        uint64_t* fb = &full_bar[stage];
+        mbar_wait(&empty_bar[pos.stage], pos.phase ^ 1);
+        uint8_t* st = smem + pos.stage * kKvStageBytes;
+        uint64_t* fb = &full_bar[pos.stage];
         mbar_arrive_expect_tx(fb, kKvStageBytes);
         const int row0 = (kb0 + i) * 64;
 #pragma unroll
@@ -122,10 +121,7 @@ kv_gemm_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
           tma_load_3d(st + 2 * kKvTile + b * kKvBlock, &tm_hi, fb, cv, row0, image);
           tma_load_3d(st + 3 * kKvTile + b * kKvBlock, &tm_lo, fb, cv, row0, image);
         }
-        if (++stage == kKvGemmStages) {
-          stage = 0;
-          phase ^= 1;
-        }
+        pos.advance();
       }
     }
   } else {
@@ -136,11 +132,11 @@ kv_gemm_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
 #pragma unroll
     for (int i = 0; i < 8; ++i) ks[0][i] = ks[1][i] = 0.f;
     const uint64_t ones = wgmma_desc_ones(smem_u32(s_ones));
-    int stage = 0, prev = -1;
-    uint32_t phase = 0;
+    RingPos<kKvGemmStages> pos;
+    int prev = -1;
     for (int i = 0; i < nkb; ++i) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t st = smem_u32(smem + stage * kKvStageBytes);
+      mbar_wait(&full_bar[pos.stage], pos.phase);
+      const uint32_t st = smem_u32(smem + pos.stage * kKvStageBytes);
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
@@ -160,11 +156,8 @@ kv_gemm_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
       wgmma_commit();
       wgmma_wait<1>();   // the previous k-block's MMAs are done: its slot may be refilled
       if (prev >= 0) mbar_arrive(&empty_bar[prev]);
-      prev = stage;
-      if (++stage == kKvGemmStages) {
-        stage = 0;
-        phase ^= 1;
-      }
+      prev = pos.stage;
+      pos.advance();
     }
     wgmma_wait<0>();
     wgmma_fence_regs(acc[0]);

@@ -11,6 +11,13 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
+// ---------------------------------------------------------------- programmatic dependent launch
+// pdl_trigger: the next kernel of the stream, when launched with the PDL attribute, may be scheduled as soon as every
+// CTA of this grid got here, and run its own set-up while this grid is still working.  pdl_wait: everything after it
+// waits until the previous grid has completed and flushed.  Both are no-ops for an ordinary launch.
+__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -62,6 +69,19 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
+
+// Position in a ring of kStages mbarrier-guarded slots: the slot and the parity of its current phase.
+template <int kStages>
+struct RingPos {
+  int stage = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void advance() {
+    if (++stage == kStages) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+};
 
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -124,6 +144,11 @@ __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+template <int P, int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[P][R]) {
+#pragma unroll
+  for (int p = 0; p < P; ++p) wgmma_fence_regs(d[p]);
+}
 
 // D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 operands from shared memory (both K-major), fp32 accumulate.
 // Thread t of the warpgroup holds rows 16*(t/32) + (t%32)/4 (+8) and columns 8*j + 2*(t%4) (+1) of D.
@@ -178,6 +203,14 @@ __device__ __forceinline__ void wgmma_f16<256>(float (&d)[128], uint64_t desc_a,
       : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
+// Split-precision product D += A * B^T of A = a_hi + a_lo and B = b_hi + b_lo, as hi*hi + hi*lo + lo*hi in that order
+// (the dropped lo*lo term is <= 2^-22 relative).
+template <int N>
+__device__ __forceinline__ void wgmma_split(float (&d)[N / 2], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo) {
+  wgmma_f16<N>(d, a_hi, b_hi, 1u);
+  wgmma_f16<N>(d, a_hi, b_lo, 1u);
+  wgmma_f16<N>(d, a_lo, b_hi, 1u);
+}
 
 // ---------------------------------------------------------------- descriptors
 // Shared-memory matrix descriptor of a K-major operand tile stored as rows of 128 bytes (64 fp16) with the 128-byte

@@ -9,11 +9,6 @@
 
 namespace lb {
 
-// Programmatic dependent launch: lets a tensor-core kernel that follows on the stream (launched with the PDL attribute,
-// gemm_split.cuh) be scheduled and run its set-up while this grid is still working; it waits for this grid's completion
-// before it touches global memory.  A no-op when the next launch is an ordinary one.
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 // ------------------------------------------------------------------------------------------------
 // fp32 [rows, cols] (ld_x) -> fp16 hi/lo planes (ld_pl, column offset col0).  Weight packing and tests.
 __global__ void split_planes_kernel(const float* __restrict__ x, long rows, int cols, int ld_x,

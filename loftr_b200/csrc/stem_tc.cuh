@@ -30,7 +30,7 @@ constexpr int kStemPatchH = 2 * kConvTileH + 5;    // 21 input rows feed 8 outpu
 constexpr int kStemPatchW = 2 * kConvTileW + 5;    // 37
 constexpr int kStemPatchPitch = 40;
 constexpr int kStemATile = 128 * 128;              // [128 rows][64 fp16] = 16 KB per plane
-constexpr int kStemAccStride = 132;                // floats per staged accumulator row (conflict-free row reads)
+constexpr int kStemAccStride = acc_stride(128);    // floats per staged accumulator row (conflict-free row reads)
 constexpr int kStemSmemBytes = 2 * kStemATile      // A hi/lo
                                + 2 * kStemATile    // W hi/lo
                                + 128 * kStemAccStride * 4   // staged accumulator
@@ -42,7 +42,7 @@ __device__ __forceinline__ uint32_t stem_sw128(int row, int k) {   // byte offse
 }
 
 __global__ void __launch_bounds__(kStemThreads, 1) conv_stem7x7_tc_kernel(const __grid_constant__ StemTcParams p) {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // the first convolution may set up meanwhile
+  pdl_trigger();   // the first convolution may set up meanwhile
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) asm volatile("trap;");
   uint8_t* sA = smem;                                   // [hi|lo][16 KB]
@@ -87,7 +87,6 @@ __global__ void __launch_bounds__(kStemThreads, 1) conv_stem7x7_tc_kernel(const 
   const long tiles_per_img = static_cast<long>(p.tiles_w) * p.tiles_h;
   const long total = tiles_per_img * p.N;
   const int half = warp >> 2;                     // warpgroup = 64-channel half of the accumulator
-  const int wt = tid & 127;                       // thread within the warpgroup
   uint32_t* stage = sStage + warp * 1024;
 
   for (long t = blockIdx.x; t < total; t += gridDim.x) {
@@ -136,9 +135,7 @@ __global__ void __launch_bounds__(kStemThreads, 1) conv_stem7x7_tc_kernel(const 
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
           const uint64_t adv = static_cast<uint64_t>(k * 2);
-          wgmma_f16<64>(acc[mh], da_hi + adv, db_hi + adv, 1u);
-          wgmma_f16<64>(acc[mh], da_hi + adv, db_lo + adv, 1u);
-          wgmma_f16<64>(acc[mh], da_lo + adv, db_hi + adv, 1u);
+          wgmma_split<64>(acc[mh], da_hi + adv, da_lo + adv, db_hi + adv, db_lo + adv);
         }
       }
       wgmma_commit();
@@ -146,20 +143,9 @@ __global__ void __launch_bounds__(kStemThreads, 1) conv_stem7x7_tc_kernel(const 
       wgmma_fence_regs(acc[0]);
       wgmma_fence_regs(acc[1]);
     }
-    // (d) stage the accumulator row-major: thread holds rows 16 (wt/32) + (wt%32)/4 (+8, +64), columns 8 j + 2 (wt%4)
-    {
-      const int r0 = 16 * (wt >> 5) + ((wt & 31) >> 2);
-      const int c0 = half * 64 + 2 * (wt & 3);
-#pragma unroll
-      for (int mh = 0; mh < 2; ++mh) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float* q = sAcc + (mh * 64 + r0) * kStemAccStride + c0 + 8 * j;
-          *reinterpret_cast<float2*>(q) = make_float2(acc[mh][4 * j], acc[mh][4 * j + 1]);
-          *reinterpret_cast<float2*>(q + 8 * kStemAccStride) = make_float2(acc[mh][4 * j + 2], acc[mh][4 * j + 3]);
-        }
-      }
-    }
+    // (d) stage the accumulator row-major
+    stage_acc<64>(sAcc, kStemAccStride, acc[0], 0, 8, half * 64);
+    stage_acc<64>(sAcc, kStemAccStride, acc[1], 64, 8, half * 64);
     __syncthreads();
     // (e) epilogue: warp w drains pixel rows 32 (w%4) + lane, channel groups of its half
     const float* row = sAcc + ((warp & 3) * 32 + lane) * kStemAccStride;
