@@ -183,6 +183,15 @@ size_t lb_backbone_workspace_bytes(const LbBackboneWeights* w /*host*/, int N, i
 /* images [N,1,H,W] fp32 -> feat_c NHWC fp32 [N,H/8,W/8,block_dims[2]], feat_f NHWC fp32 [N,H/2,W/2,block_dims[0]] */
 int lb_backbone_forward(const LbBackboneWeights* w /*host*/, const float* images, int N, int H, int W,
                         float* feat_c_nhwc, float* feat_f_nhwc, void* ws, size_t ws_bytes, void* stream);
+/* The same network with single fp16 activations and one fp16 MMA per product (version 108; DESIGN.md §15).  The stem
+ * keeps its split product; every later convolution multiplies the stored fp16 activation by the hi weight planes
+ * (w_hi, wr_hi: fp16(w * 2^e) in the layout above) with fp32 accumulation, and the epilogue (x 2^-e, BatchNorm,
+ * residual, FPN upsample-add, activation) stores one fp16 plane, rounded to nearest even.  w_lo / wr_lo are ignored
+ * and may be NULL.  feat_c / feat_f are fp32 as above.  The workspace holds one plane per activation (about half of
+ * lb_backbone_workspace_bytes).  Separate entry points rather than a flag: DESIGN.md §12. */
+size_t lb_backbone_workspace_bytes_fp16(const LbBackboneWeights* w /*host*/, int N, int H, int W);
+int lb_backbone_forward_fp16(const LbBackboneWeights* w /*host*/, const float* images, int N, int H, int W,
+                             float* feat_c_nhwc, float* feat_f_nhwc, void* ws, size_t ws_bytes, void* stream);
 
 /* Weights of one LoFTREncoderLayer (state_dict names in comments), as fp16 planes of the [out, in] matrices.
  * Each weight matrix may be pre-scaled by a power of two 2^e before it is split (keeps the fp16 `lo` plane out of

@@ -126,6 +126,9 @@ SIGNATURES = {
     "lb_backbone_workspace_bytes": (c_size_t, [C.POINTER(LbBackboneWeights), c_int, c_int, c_int]),
     "lb_backbone_forward": (c_int, [C.POINTER(LbBackboneWeights), c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                                     c_void_p, c_size_t, c_void_p]),
+    "lb_backbone_workspace_bytes_fp16": (c_size_t, [C.POINTER(LbBackboneWeights), c_int, c_int, c_int]),
+    "lb_backbone_forward_fp16": (c_int, [C.POINTER(LbBackboneWeights), c_void_p, c_int, c_int, c_int, c_void_p,
+                                         c_void_p, c_void_p, c_size_t, c_void_p]),
     "lb_transformer_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "lb_transformer_forward": (c_int, [C.POINTER(LbEncoderLayerWeights), C.POINTER(c_int), c_int, c_int, c_int,
                                        C.POINTER(LbTransformerState), c_void_p, c_size_t, c_void_p]),
@@ -162,11 +165,14 @@ MATCH_CAP_VERSION = 105
 PREPROCESS_VERSION = 106
 # oldest library with the two-view geometry estimator (lb_estimate_geometry)
 GEOMETRY_VERSION = 107
+# oldest library with the single-pass fp16 backbone (lb_backbone_forward_fp16, backbone_impl="b200_fp16")
+BACKBONE_FP16_VERSION = 108
 GEOMETRY_HOMOGRAPHY = 0
 GEOMETRY_FUNDAMENTAL = 1
 _SINCE = {"lb_coarse_prep_indexed": FEATURE_BANK_VERSION, "lb_fine_preprocess_indexed": FEATURE_BANK_VERSION,
           "lb_coarse_match_capped": MATCH_CAP_VERSION, "lb_preprocess_images": PREPROCESS_VERSION,
-          "lb_geometry_workspace_bytes": GEOMETRY_VERSION, "lb_estimate_geometry": GEOMETRY_VERSION}
+          "lb_geometry_workspace_bytes": GEOMETRY_VERSION, "lb_estimate_geometry": GEOMETRY_VERSION,
+          "lb_backbone_workspace_bytes_fp16": BACKBONE_FP16_VERSION, "lb_backbone_forward_fp16": BACKBONE_FP16_VERSION}
 
 
 class LibraryMissing(RuntimeError):

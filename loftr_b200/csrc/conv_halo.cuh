@@ -38,7 +38,6 @@ constexpr int kHaloW = kConvTileW + 2;
 constexpr int kHaloH = kConvTileH + 2;
 constexpr int kHaloChunkBytes = 2944;                      // 180 pixels x 16 bytes = 2,880, 128-byte aligned
 constexpr int kHaloPlaneBytes = (kBlockK / 8) * kHaloChunkBytes;
-constexpr int kHaloSlotBytes = 2 * kHaloPlaneBytes;         // hi + lo planes of one channel block
 constexpr int kHaloTaps = 9;
 static_assert(kHaloW * kHaloH * 16 <= kHaloChunkBytes && kHaloChunkBytes % 128 == 0, "halo chunk layout");
 
@@ -48,13 +47,16 @@ static_assert(kHaloW * kHaloH * 16 <= kHaloChunkBytes && kHaloChunkBytes % 128 =
 // gets four stages of 25,600 bytes because EpiConv<200> shares the residual transposer with the TMA-store staging
 // (EpiConv::kOwnXpose): its own transposer would take the fourth stage, and three stages made the 196-channel
 // layers 13-14 % slower on an H100 at 700 W.
-template <int BLOCK_N, int kEpiBytes>
+// With single fp16 planes (kPlanes = 1: EpiConvF16) the halo slots and the weight stages are half as large and the same
+// rule gives kBK = 64 and 6 / 5 / 4 stages at N = 128 / 200 / 256 (two planes: 3 / 4 / 3).
+template <int BLOCK_N, int kEpiBytes, int kPlanes = 2>
 struct HaloSmem {
+  static constexpr int kHaloSlotBytes = kPlanes * kHaloPlaneBytes;   // hi (+ lo) planes of one channel block
   static constexpr int kBarBytes = 256;
   static constexpr int kFree = kSmemLimit - kBarBytes - kEpiBytes - 2 * kHaloSlotBytes;
-  static constexpr int kBK = kFree / (2 * BLOCK_N * kBlockK * 2) >= 3 ? kBlockK : kBlockK / 2;
+  static constexpr int kBK = kFree / (kPlanes * BLOCK_N * kBlockK * 2) >= 3 ? kBlockK : kBlockK / 2;
   static constexpr int kBTile = BLOCK_N * kBK * 2;        // per plane
-  static constexpr int kStageBytes = 2 * kBTile;
+  static constexpr int kStageBytes = kPlanes * kBTile;
   static constexpr int kStages = kFree / kStageBytes < 6 ? kFree / kStageBytes : 6;
   static_assert(kStages >= 3, "the weight ring needs three stages");
   static constexpr int kRingBytes = kStages * kStageBytes;
@@ -82,13 +84,15 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
                     const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
                     const __grid_constant__ CUtensorMap tm_br_hi, const __grid_constant__ CUtensorMap tm_br_lo,
                     const GemmShape shape, const __grid_constant__ typename Epi::Params epi_params) {
-  using S = HaloSmem<BLOCK_N, Epi::kSmemBytes>;
+  constexpr int kPlanes = EpiOperandPlanes<Epi>::value;   // 1: single fp16 planes, one MMA per k-step
+  using S = HaloSmem<BLOCK_N, Epi::kSmemBytes, kPlanes>;
+  constexpr int kHaloSlotBytes = S::kHaloSlotBytes;
   constexpr int kBK = S::kBK;
   constexpr int kSubs = kBlockK / kBK;                       // weight stages per (tap, 64-channel block)
   constexpr int kRemBTile = BLOCK_N * kRemChannels * 2;      // per plane
   constexpr bool kStagingInRing = S::kAccBytes <= S::kRingBytes;   // N = 128: the halo slots stay free at the tile end
   static_assert(BLOCK_N % 8 == 0 && BLOCK_N <= 256, "one wgmma spans the tile: N a multiple of 8, at most 256");
-  static_assert(2 * kRemBTile <= S::kStageBytes && kRemBTile % 256 == 0, "remainder weight stage");
+  static_assert(kPlanes * kRemBTile <= S::kStageBytes && kRemBTile % 256 == 0, "remainder weight stage");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* ring = smem_raw;
   uint8_t* halo = smem_raw + S::kRingBytes;
@@ -142,12 +146,13 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
             mbar_wait(&halo_empty[slot], ((hi >> 1) & 1) ^ 1);
             const int chunks = (hh == g.cin_blocks ? kRemChannels : kBlockK) / 8;
             uint64_t* fb = &halo_full[slot];
-            mbar_arrive_expect_tx(fb, static_cast<uint32_t>(chunks) * 2 * kHaloW * kHaloH * 16);
+            mbar_arrive_expect_tx(fb, static_cast<uint32_t>(chunks) * kPlanes * kHaloW * kHaloH * 16);
             uint8_t* dst = halo + slot * kHaloSlotBytes;
             for (int c = 0; c < chunks; ++c) {
               const int ch = hh * kBlockK + 8 * c;
               tma_load_4d(dst + c * kHaloChunkBytes, &tm_a_hi, fb, ch, x0, y0, w.batch);
-              tma_load_4d(dst + kHaloPlaneBytes + c * kHaloChunkBytes, &tm_a_lo, fb, ch, x0, y0, w.batch);
+              if constexpr (kPlanes == 2)
+                tma_load_4d(dst + kHaloPlaneBytes + c * kHaloChunkBytes, &tm_a_lo, fb, ch, x0, y0, w.batch);
             }
           };
           // the halos needed first are issued before the weights (with kStagingInRing: while the previous tile's
@@ -166,15 +171,15 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
               uint8_t* st = ring + pos.stage * S::kStageBytes;
               uint64_t* fb = &full_bar[pos.stage];
               if (rem) {
-                mbar_arrive_expect_tx(fb, 2 * kRemBTile);
+                mbar_arrive_expect_tx(fb, kPlanes * kRemBTile);
                 tma_load_3d(st, &tm_br_hi, fb, tap * kRemChannels, nt * BLOCK_N, 0);
-                tma_load_3d(st + kRemBTile, &tm_br_lo, fb, tap * kRemChannels, nt * BLOCK_N, 0);
+                if constexpr (kPlanes == 2) tma_load_3d(st + kRemBTile, &tm_br_lo, fb, tap * kRemChannels, nt * BLOCK_N, 0);
               } else {
                 // the main weight planes keep gemm_split_kernel's K layout: k-block (tap, cb) at (tap * cin_blocks + cb) * 64
                 const int k0 = (tap * g.cin_blocks + hh) * kBlockK + j * kBK;
                 mbar_arrive_expect_tx(fb, S::kStageBytes);
                 tma_load_3d(st, &tm_b_hi, fb, k0, nt * BLOCK_N, 0);
-                tma_load_3d(st + S::kBTile, &tm_b_lo, fb, k0, nt * BLOCK_N, 0);
+                if constexpr (kPlanes == 2) tma_load_3d(st + S::kBTile, &tm_b_lo, fb, k0, nt * BLOCK_N, 0);
               }
               pos.advance();
             }
@@ -222,7 +227,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
               const uint64_t rb_lo = wgmma_desc_k_sw32(st + kRemBTile);
               const uint64_t ra_hi = wgmma_desc_k_noswz(a_tap, kHaloChunkBytes, kHaloW * 16);
               const uint64_t ra_lo = wgmma_desc_k_noswz(a_tap + kHaloPlaneBytes, kHaloChunkBytes, kHaloW * 16);
-              wgmma_split<BLOCK_N>(acc, ra_hi, ra_lo, rb_hi, rb_lo);
+              wgmma_split<BLOCK_N, kPlanes>(acc, ra_hi, ra_lo, rb_hi, rb_lo);
             } else {
               const uint64_t db_hi = kBK == 64 ? wgmma_desc_k_sw128(st) : wgmma_desc_k_sw64(st);
               const uint64_t db_lo = kBK == 64 ? wgmma_desc_k_sw128(st + S::kBTile) : wgmma_desc_k_sw64(st + S::kBTile);
@@ -234,7 +239,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
                 // A: 16 channels = two chunks further; B: 32 bytes further inside the swizzle row (16-byte units)
                 const uint64_t a_adv = static_cast<uint64_t>(k * 2 * kHaloChunkBytes / 16);
                 const uint64_t b_adv = static_cast<uint64_t>(k * 2);
-                wgmma_split<BLOCK_N>(acc, da_hi + a_adv, da_lo + a_adv, db_hi + b_adv, db_lo + b_adv);
+                wgmma_split<BLOCK_N, kPlanes>(acc, da_hi + a_adv, da_lo + a_adv, db_hi + b_adv, db_lo + b_adv);
               }
             }
             wgmma_commit();

@@ -12,6 +12,7 @@
 #include <cstring>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/loftr_b200.h"
@@ -323,7 +324,7 @@ static int launch_persistent(int tag, const GemmShape& s, int smem_bytes, int sm
 template <int BN, class Epi>
 static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const typename Epi::Params& ep, int sms,
                       cudaStream_t st) {
-  using S = GemmSmem<BN, Epi::kSmemBytes>;
+  using S = GemmSmem<BN, Epi::kSmemBytes, EpiOperandPlanes<Epi>::value>;
   constexpr int smem_bytes = S::kRingBytes + S::kBarBytes + Epi::kSmemBytes;
   static_assert(smem_bytes <= kSmemLimit, "shared memory budget exceeded");
   return launch_persistent<&gemm_split_kernel<BN, Epi>>(tag, s, smem_bytes, sms, st, maps.a_hi, maps.a_lo, maps.b_hi,
@@ -384,12 +385,13 @@ static void conv_layout(int cin, int* cin_blocks, int* rem) {
   }
 }
 // The implicit GEMM of convolution d with BN-wide n tiles (one per work item), and the output geometry its epilogue
-// reads.  *rem: the remainder channels per tap (0: none).
+// reads.  *rem: the remainder channels per tap (0: none).  lo: the weights have lo planes (split precision).
 template <int BN, class Params>
-static int conv_shape(const ConvDesc& d, const Planes& wgt_rem, GemmShape* s, Params* ep, int* rem) {
+static int conv_shape(const ConvDesc& d, const Planes& wgt_rem, bool lo, GemmShape* s, Params* ep, int* rem) {
   int cin_blocks = 0;
   conv_layout(d.Cin, &cin_blocks, rem);
-  if (*rem && (!wgt_rem.hi || !wgt_rem.lo)) return fail("convolution with Cin=%d needs remainder weight planes", d.Cin);
+  if (*rem && (!wgt_rem.hi || (lo && !wgt_rem.lo)))
+    return fail("convolution with Cin=%d needs remainder weight planes", d.Cin);
   const int taps = d.ksize * d.ksize;
   const int tiles_h = (d.H_out + kConvTileH - 1) / kConvTileH;
   const int tiles_w = (d.W_out + kConvTileW - 1) / kConvTileW;
@@ -405,26 +407,34 @@ static int conv_shape(const ConvDesc& d, const Planes& wgt_rem, GemmShape* s, Pa
   return 0;
 }
 
-template <int BN, bool kUpsample>
+// Epi: EpiConv<BN, .> (hi / lo planes: operands, weights and outputs) or EpiConvF16<BN, .> (hi planes only; the lo
+// maps are copies of the hi ones and never loaded)
+template <int BN, class Epi>
 static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_rem, const ConvDesc& d,
-                       const typename EpiConv<BN, kUpsample>::Params& ep_in, cudaStream_t st) {
-  using Epi = EpiConv<BN, kUpsample>;
+                       const typename Epi::Params& ep_in, cudaStream_t st) {
+  constexpr bool kLo = EpiOperandPlanes<Epi>::value == 2;
   int sms = 0;
   LB_TRY(device_check(&sms));
   GemmShape s;
   typename Epi::Params ep = ep_in;
   int rem = 0;
-  LB_TRY(conv_shape<BN>(d, wgt_rem, &s, &ep, &rem));
+  LB_TRY(conv_shape<BN>(d, wgt_rem, kLo, &s, &ep, &rem));
   GemmMaps mp;
   LB_TRY(make_map_nhwc(&mp.a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride));
-  LB_TRY(make_map_nhwc(&mp.a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride));
   LB_TRY(make_map(&mp.b_hi, wgt.hi, s.K, d.Cout, 1, wgt.ld, 0, BN));
-  LB_TRY(make_map(&mp.b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN));
+  mp.a_lo = mp.a_hi; mp.b_lo = mp.b_hi;
+  if (kLo) {
+    LB_TRY(make_map_nhwc(&mp.a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride));
+    LB_TRY(make_map(&mp.b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN));
+  }
   if (rem) {
     LB_TRY(make_map_nhwc(&mp.ar_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, kRemChannels));
-    LB_TRY(make_map_nhwc(&mp.ar_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, kRemChannels));
     LB_TRY(make_map(&mp.br_hi, wgt_rem.hi, s.conv.taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
-    LB_TRY(make_map(&mp.br_lo, wgt_rem.lo, s.conv.taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
+    mp.ar_lo = mp.ar_hi; mp.br_lo = mp.br_hi;
+    if (kLo) {
+      LB_TRY(make_map_nhwc(&mp.ar_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, kRemChannels));
+      LB_TRY(make_map(&mp.br_lo, wgt_rem.lo, s.conv.taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
+    }
   } else {
     mp.ar_hi = mp.a_hi; mp.ar_lo = mp.a_lo; mp.br_hi = mp.b_hi; mp.br_lo = mp.b_lo;
   }
@@ -432,11 +442,11 @@ static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_re
 }
 
 // Stride-1 3x3 convolution through conv3x3_halo_kernel (same operands, weights and epilogue as launch_conv).
-template <int BN>
+template <int BN, class Epi>
 static int launch_conv_halo(const Planes& in, const Planes& wgt, const Planes& wgt_rem, const ConvDesc& d,
-                            const typename EpiConv<BN, false>::Params& ep_in, cudaStream_t st) {
-  using Epi = EpiConv<BN, false>;
-  using S = HaloSmem<BN, Epi::kSmemBytes>;
+                            const typename Epi::Params& ep_in, cudaStream_t st) {
+  constexpr bool kLo = EpiOperandPlanes<Epi>::value == 2;
+  using S = HaloSmem<BN, Epi::kSmemBytes, EpiOperandPlanes<Epi>::value>;
   static_assert(S::kTotalBytes <= kSmemLimit, "shared memory budget exceeded");
   int sms = 0;
   LB_TRY(device_check(&sms));
@@ -444,15 +454,20 @@ static int launch_conv_halo(const Planes& in, const Planes& wgt, const Planes& w
   GemmShape s;
   typename Epi::Params ep = ep_in;
   int rem = 0;
-  LB_TRY(conv_shape<BN>(d, wgt_rem, &s, &ep, &rem));
+  LB_TRY(conv_shape<BN>(d, wgt_rem, kLo, &s, &ep, &rem));
   CUtensorMap a_hi, a_lo, b_hi, b_lo, br_hi, br_lo;
   LB_TRY(make_map_halo(&a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld));
-  LB_TRY(make_map_halo(&a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld));
   LB_TRY(make_map(&b_hi, wgt.hi, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
-  LB_TRY(make_map(&b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
+  a_lo = a_hi;
+  b_lo = b_hi;
+  if (kLo) {
+    LB_TRY(make_map_halo(&a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld));
+    LB_TRY(make_map(&b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
+  }
   if (rem) {
     LB_TRY(make_map(&br_hi, wgt_rem.hi, kHaloTaps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
-    LB_TRY(make_map(&br_lo, wgt_rem.lo, kHaloTaps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
+    br_lo = br_hi;
+    if (kLo) LB_TRY(make_map(&br_lo, wgt_rem.lo, kHaloTaps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
   } else {
     br_hi = b_hi;
     br_lo = b_lo;
@@ -533,18 +548,19 @@ static int tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const Lb
 // ResNetFPN_8_2 forward (reference src/loftr/backbone/resnet_fpn.py:43-118) on tensor cores: every 3x3 / 1x1
 // convolution is an implicit GEMM through gemm_split_kernel<., EpiConv>, the stride-1 3x3 ones through
 // conv3x3_halo_kernel<., EpiConv> (BatchNorm, ReLU / LeakyReLU, residual add and the FPN upsample-add fused in the
-// epilogue); activations live as NHWC fp16 hi/lo planes.
+// epilogue); activations live as NHWC fp16 hi/lo planes.  The fp16 backbone (lb_backbone_forward_fp16) runs the same
+// network on single fp16 planes (planes = 1: lo == nullptr) with one MMA per product after the stem (EpiConvF16).
 struct BbBuf {
   __half* hi;
   __half* lo;
   int ld;
 };
 static inline int pad8(int c) { return (c + 7) & ~7; }
-static BbBuf bb_take(Bump& b, long pixels, int C) {
+static BbBuf bb_take(Bump& b, long pixels, int C, int planes) {
   BbBuf r;
   r.ld = pad8(C);
   r.hi = b.take<__half>(static_cast<size_t>(pixels) * r.ld);
-  r.lo = b.take<__half>(static_cast<size_t>(pixels) * r.ld);
+  r.lo = planes == 2 ? b.take<__half>(static_cast<size_t>(pixels) * r.ld) : nullptr;
   return r;
 }
 struct BbWs {
@@ -554,15 +570,16 @@ struct BbWs {
   BbBuf x2l, m2, x2o;                   // 1/4: d3, d3, d2
   BbBuf x1l, m1;                        // 1/2: d2, d2
 };
-static void carve_bb(Bump& b, BbWs& w, int N, int H, int W, int d1, int d2, int d3) {
+static void carve_bb(Bump& b, BbWs& w, int N, int H, int W, int d1, int d2, int d3, int planes) {
   const long p2 = static_cast<long>(N) * (H / 2) * (W / 2), p4 = static_cast<long>(N) * (H / 4) * (W / 4),
              p8 = static_cast<long>(N) * (H / 8) * (W / 8);
-  w.s0 = bb_take(b, p2, d1); w.t1 = bb_take(b, p2, d1); w.a1 = bb_take(b, p2, d1); w.x1 = bb_take(b, p2, d1);
-  w.t2 = bb_take(b, p4, d2); w.dn2 = bb_take(b, p4, d2); w.a2 = bb_take(b, p4, d2); w.x2 = bb_take(b, p4, d2);
-  w.t3 = bb_take(b, p8, d3); w.dn3 = bb_take(b, p8, d3); w.a3 = bb_take(b, p8, d3); w.x3 = bb_take(b, p8, d3);
-  w.x3o = bb_take(b, p8, d3);
-  w.x2l = bb_take(b, p4, d3); w.m2 = bb_take(b, p4, d3); w.x2o = bb_take(b, p4, d2);
-  w.x1l = bb_take(b, p2, d2); w.m1 = bb_take(b, p2, d2);
+  auto take = [&](long pixels, int C) { return bb_take(b, pixels, C, planes); };
+  w.s0 = take(p2, d1); w.t1 = take(p2, d1); w.a1 = take(p2, d1); w.x1 = take(p2, d1);
+  w.t2 = take(p4, d2); w.dn2 = take(p4, d2); w.a2 = take(p4, d2); w.x2 = take(p4, d2);
+  w.t3 = take(p8, d3); w.dn3 = take(p8, d3); w.a3 = take(p8, d3); w.x3 = take(p8, d3);
+  w.x3o = take(p8, d3);
+  w.x2l = take(p4, d3); w.m2 = take(p4, d3); w.x2o = take(p4, d2);
+  w.x1l = take(p2, d2); w.m1 = take(p2, d2);
 }
 
 struct ConvRun {
@@ -577,6 +594,8 @@ struct ConvRun {
   float* out_f32;
   int f32_ld;
 };
+// kPlanes = 2: the split-precision convolution (EpiConv); 1: single fp16 planes (EpiConvF16, w_lo / wr_lo unused)
+template <int kPlanes>
 static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
   const LbConvWeights& w = *r.w;
   ConvDesc d;
@@ -597,7 +616,7 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
   om.dims = 4;
   if (r.out) {
     LB_TRY(make_out_map_nhwc(&om.hi, r.out->hi, false, d.Cout, d.W_out, d.H_out, N, r.out->ld));
-    LB_TRY(make_out_map_nhwc(&om.lo, r.out->lo, false, d.Cout, d.W_out, d.H_out, N, r.out->ld));
+    if (kPlanes == 2) LB_TRY(make_out_map_nhwc(&om.lo, r.out->lo, false, d.Cout, d.W_out, d.H_out, N, r.out->ld));
     om.use |= 1;
   }
   if (r.out_f32) {
@@ -606,25 +625,28 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
   }
   // stride-1 3x3 convolutions (none of them carries the FPN upsample-add) load each input patch once per channel block
   const bool halo = w.ksize == 3 && w.stride == 1 && !r.up;
-#define LB_CONV_CASE_UP(BN, UP, ...)                                                                                  \
+  // the epilogue type of the tile width and FPN mode: it also selects the kernels' operand planes
+#define LB_CONV_EPI(BN, UP) std::conditional_t<kPlanes == 2, EpiConv<BN, UP>, EpiConvF16<BN, UP>>
+#define LB_CONV_CASE_UP(BN, UP, LAUNCH)                                                                               \
   {                                                                                                                   \
-    EpiConv<BN, UP>::Params ep{w.scale, w.shift, r.act, r.res ? r.res->hi : nullptr, r.res ? r.res->lo : nullptr,     \
-                               r.res ? r.res->ld : 0, r.up ? r.up->hi : nullptr, r.up ? r.up->lo : nullptr,          \
-                               r.up ? r.up->ld : 0, r.up_h, r.up_w, r.out ? r.out->hi : nullptr,                      \
-                               r.out ? r.out->lo : nullptr, r.out ? r.out->ld : 0, r.out_f32, r.f32_ld, 0, 0, 0, om}; \
-    return __VA_ARGS__(in, wg, wr, d, ep, st);                                                                        \
+    using Epi = LB_CONV_EPI(BN, UP);                                                                                  \
+    typename Epi::Params ep{w.scale, w.shift, r.act, r.res ? r.res->hi : nullptr, r.res ? r.res->lo : nullptr,        \
+                            r.res ? r.res->ld : 0, r.up ? r.up->hi : nullptr, r.up ? r.up->lo : nullptr,             \
+                            r.up ? r.up->ld : 0, r.up_h, r.up_w, r.out ? r.out->hi : nullptr,                         \
+                            r.out ? r.out->lo : nullptr, r.out ? r.out->ld : 0, r.out_f32, r.f32_ld, 0, 0, 0, om};    \
+    return LAUNCH<BN, Epi>(in, wg, wr, d, ep, st);                                                                    \
   }
 #define LB_CONV_CASE(BN)                                                                                              \
   {                                                                                                                   \
-    if (r.up) LB_CONV_CASE_UP(BN, true, launch_conv<BN, true>)                                                        \
-    LB_CONV_CASE_UP(BN, false, launch_conv<BN, false>)                                                                \
+    if (r.up) LB_CONV_CASE_UP(BN, true, launch_conv)                                                                  \
+    LB_CONV_CASE_UP(BN, false, launch_conv)                                                                           \
   }
   // output-channel tile: the smallest built N that covers Cout.  196 -> 200 in the halo kernel (one m64n200 wgmma per
   // x-half); 208 in gemm_split_kernel, whose two column halves need N / 2 to be a wgmma N (104 = 13 x 8)
   if (halo) {
-    if (w.cout <= 128) LB_CONV_CASE_UP(128, false, launch_conv_halo<128>)
-    if (w.cout <= 200) LB_CONV_CASE_UP(200, false, launch_conv_halo<200>)
-    if (w.cout <= 256) LB_CONV_CASE_UP(256, false, launch_conv_halo<256>)
+    if (w.cout <= 128) LB_CONV_CASE_UP(128, false, launch_conv_halo)
+    if (w.cout <= 200) LB_CONV_CASE_UP(200, false, launch_conv_halo)
+    if (w.cout <= 256) LB_CONV_CASE_UP(256, false, launch_conv_halo)
     return fail("convolutions with more than 256 output channels are not built");
   }
   if (w.cout <= 128) LB_CONV_CASE(128)
@@ -632,6 +654,7 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
   if (w.cout <= 256) LB_CONV_CASE(256)
 #undef LB_CONV_CASE
 #undef LB_CONV_CASE_UP
+#undef LB_CONV_EPI
   return fail("convolutions with more than 256 output channels are not built");
 }
 
@@ -895,7 +918,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
 
 extern "C" {
 
-int lb_version(void) { return 107; }
+int lb_version(void) { return 108; }
 int lb_block_k(void) { return kBlockK; }
 int lb_conv_layout(int cin, int* cin_blocks, int* rem_channels) {
   if (!cin_blocks || !rem_channels || cin <= 0) return fail("lb_conv_layout: bad arguments");
@@ -1088,15 +1111,20 @@ int lb_transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds
 }
 
 
-size_t lb_backbone_workspace_bytes(const LbBackboneWeights* w, int N, int H, int W) {
+}  // extern "C"
+
+// Workspace of the backbone with `planes` fp16 planes per activation
+static size_t backbone_workspace_bytes(const LbBackboneWeights* w, int N, int H, int W, int planes) {
   Bump b{nullptr, 0};
   BbWs ws;
-  carve_bb(b, ws, N, H, W, w->l1[0].cout, w->l2[0].cout, w->l3[0].cout);
+  carve_bb(b, ws, N, H, W, w->l1[0].cout, w->l2[0].cout, w->l3[0].cout, planes);
   return b.off + 256;
 }
 
-int lb_backbone_forward(const LbBackboneWeights* w, const float* images, int N, int H, int W, float* feat_c_nhwc,
-                        float* feat_f_nhwc, void* ws, size_t ws_bytes, void* stream) {
+// ResNetFPN_8_2 forward with split-precision (kPlanes = 2) or single fp16 (kPlanes = 1) activations and products
+template <int kPlanes>
+static int backbone_forward(const LbBackboneWeights* w, const float* images, int N, int H, int W, float* feat_c_nhwc,
+                            float* feat_f_nhwc, void* ws, size_t ws_bytes, void* stream) {
   int sms;
   if (N <= 0) return 0;
   DeviceGuard dev_guard;
@@ -1109,8 +1137,9 @@ int lb_backbone_forward(const LbBackboneWeights* w, const float* images, int N, 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   Bump b{static_cast<uint8_t*>(ws), ws_bytes};
   BbWs B;
-  carve_bb(b, B, N, H, W, d1, d2, d3);
-  if (!b.ok) return fail("backbone workspace too small: need %zu bytes", lb_backbone_workspace_bytes(w, N, H, W));
+  carve_bb(b, B, N, H, W, d1, d2, d3, kPlanes);
+  if (!b.ok)
+    return fail("backbone workspace too small: need %zu bytes", backbone_workspace_bytes(w, N, H, W, kPlanes));
   const int H2 = H / 2, W2 = W / 2, H4 = H / 4, W4 = W / 4, H8 = H / 8, W8 = W / 8;
 
   // stem: conv 7x7 s2 + BN + ReLU on the tensor cores, software im2col (stem_tc.cuh)  [resnet_fpn.py:101]
@@ -1122,18 +1151,19 @@ int lb_backbone_forward(const LbBackboneWeights* w, const float* images, int N, 
     sp.tiles_w = cdiv(W2, kConvTileW); sp.tiles_h = cdiv(H2, kConvTileH);
     sp.om.dims = 4;
     LB_TRY(make_out_map_nhwc(&sp.om.hi, B.s0.hi, false, 128, W2, H2, N, B.s0.ld));
-    LB_TRY(make_out_map_nhwc(&sp.om.lo, B.s0.lo, false, 128, W2, H2, N, B.s0.ld));
+    if (kPlanes == 2) LB_TRY(make_out_map_nhwc(&sp.om.lo, B.s0.lo, false, 128, W2, H2, N, B.s0.ld));
     sp.om.use = 1;
-    LB_TRY(set_max_dynamic_smem<&conv_stem7x7_tc_kernel>(kStemSmemBytes));
+    constexpr auto kStem = kPlanes == 2 ? &conv_stem7x7_tc_kernel : &conv_stem7x7_tc_fp16_kernel;
+    LB_TRY(set_max_dynamic_smem<kStem>(kStemSmemBytes));
     const long tiles = static_cast<long>(sp.tiles_w) * sp.tiles_h * N;
     const int grid = static_cast<int>(tiles < sms ? tiles : sms);
-    conv_stem7x7_tc_kernel<<<grid, kStemThreads, kStemSmemBytes, st>>>(sp);
+    kStem<<<grid, kStemThreads, kStemSmemBytes, st>>>(sp);
     LB_LAUNCHED();
   }
   auto conv = [&](const LbConvWeights& cw, const BbBuf& in, int hin, int win, int act, const BbBuf* res,
                   const BbBuf* up, int uph, int upw, const BbBuf* out, float* of32, int f32ld) -> int {
     ConvRun r{&cw, in, hin, win, act, res, up, uph, upw, out, of32, f32ld};
-    return run_conv(r, N, st);
+    return run_conv<kPlanes>(r, N, st);
   };
   // layer1 (1/2)                                                                    [resnet_fpn.py:102]
   LB_TRY(conv(w->l1[0], B.s0, H2, W2, 1, nullptr, nullptr, 0, 0, &B.t1, nullptr, 0));
@@ -1162,6 +1192,23 @@ int lb_backbone_forward(const LbBackboneWeights* w, const float* images, int N, 
   LB_TRY(conv(w->l1_out2[0], B.x1l, H2, W2, 2, nullptr, nullptr, 0, 0, &B.m1, nullptr, 0));
   LB_TRY(conv(w->l1_out2[1], B.m1, H2, W2, 0, nullptr, nullptr, 0, 0, nullptr, feat_f_nhwc, w->l1_out2[1].cout));
   return 0;
+}
+
+extern "C" {
+
+size_t lb_backbone_workspace_bytes(const LbBackboneWeights* w, int N, int H, int W) {
+  return backbone_workspace_bytes(w, N, H, W, 2);
+}
+int lb_backbone_forward(const LbBackboneWeights* w, const float* images, int N, int H, int W, float* feat_c_nhwc,
+                        float* feat_f_nhwc, void* ws, size_t ws_bytes, void* stream) {
+  return backbone_forward<2>(w, images, N, H, W, feat_c_nhwc, feat_f_nhwc, ws, ws_bytes, stream);
+}
+size_t lb_backbone_workspace_bytes_fp16(const LbBackboneWeights* w, int N, int H, int W) {
+  return backbone_workspace_bytes(w, N, H, W, 1);
+}
+int lb_backbone_forward_fp16(const LbBackboneWeights* w, const float* images, int N, int H, int W, float* feat_c_nhwc,
+                             float* feat_f_nhwc, void* ws, size_t ws_bytes, void* stream) {
+  return backbone_forward<1>(w, images, N, H, W, feat_c_nhwc, feat_f_nhwc, ws, ws_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ coarse matching

@@ -64,19 +64,32 @@ __device__ __forceinline__ void load_acc32(uint32_t acc_row, int col, float (&x)
                  : "memory");
 }
 
+// 32 values from fp16 hi (+ lo) planes; kPlanes = 1 reads the hi plane only (lp unused)
+template <int kPlanes = 2>
 __device__ __forceinline__ void load_planes32(const __half* hp, const __half* lp, float (&x)[32]) {
   const uint4* h4 = reinterpret_cast<const uint4*>(hp);
   const uint4* l4 = reinterpret_cast<const uint4*>(lp);
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    const uint4 a = h4[j], b = l4[j];
-    const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
+    const uint4 a = h4[j];
+    const uint32_t aw[4] = {a.x, a.y, a.z, a.w};
+    if constexpr (kPlanes == 2) {
+      const uint4 b = l4[j];
+      const uint32_t bw[4] = {b.x, b.y, b.z, b.w};
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&aw[k]));
-      const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&bw[k]));
-      x[j * 8 + 2 * k] = fh.x + fl.x;
-      x[j * 8 + 2 * k + 1] = fh.y + fl.y;
+      for (int k = 0; k < 4; ++k) {
+        const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&aw[k]));
+        const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&bw[k]));
+        x[j * 8 + 2 * k] = fh.x + fl.x;
+        x[j * 8 + 2 * k + 1] = fh.y + fl.y;
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&aw[k]));
+        x[j * 8 + 2 * k] = fh.x;
+        x[j * 8 + 2 * k + 1] = fh.y;
+      }
     }
   }
 }
@@ -139,7 +152,9 @@ __device__ __forceinline__ void warp_load_rows64(uint32_t* scr, const uint8_t* r
     w[4 * q] = v.x; w[4 * q + 1] = v.y; w[4 * q + 2] = v.z; w[4 * q + 3] = v.w;
   }
 }
-// 32 values of my row as fp16 hi/lo planes: hi_ptr / lo_ptr address (row, first column) or nullptr
+// 32 values of my row as fp16 hi/lo planes: hi_ptr / lo_ptr address (row, first column) or nullptr.  kPlanes = 1:
+// the hi plane only (round to nearest even; lo_ptr unused).
+template <int kPlanes = 2>
 __device__ __forceinline__ void warp_store_planes32(uint32_t* scr, __half* hi_ptr, __half* lo_ptr, const float (&x)[32]) {
   uint32_t h[16], l[16];
 #pragma unroll
@@ -147,7 +162,7 @@ __device__ __forceinline__ void warp_store_planes32(uint32_t* scr, __half* hi_pt
     split_f16x2(x[2 * j], x[2 * j + 1], h[j], l[j]);
   }
   warp_store_rows64(scr, reinterpret_cast<uint8_t*>(hi_ptr), h);
-  warp_store_rows64(scr, reinterpret_cast<uint8_t*>(lo_ptr), l);
+  if constexpr (kPlanes == 2) warp_store_rows64(scr, reinterpret_cast<uint8_t*>(lo_ptr), l);
 }
 __device__ __forceinline__ void warp_store_f32x32(uint32_t* scr, float* ptr, const float (&x)[32]) {
   uint32_t a[16], b[16];
@@ -161,7 +176,9 @@ __device__ __forceinline__ void warp_store_f32x32(uint32_t* scr, float* ptr, con
 }
 // 32 values of my row from fp16 hi/lo planes, in two steps: `issue` puts the lane's eight 16-byte global loads in flight
 // (rows lane/4 + 8i, 16-byte group lane%4), `finish` transposes them through the scratch into this lane's row.  An
-// epilogue can issue before it waits for / converts its accumulator group and finish afterwards.
+// epilogue can issue before it waits for / converts its accumulator group and finish afterwards.  kPlanes = 1: the hi
+// plane only (lo_ptr and vl unused).
+template <int kPlanes = 2>
 __device__ __forceinline__ void warp_issue_planes32(const __half* hi_ptr, const __half* lo_ptr, uint4 (&vh)[4], uint4 (&vl)[4]) {
   const int lane = threadIdx.x & 31;
   const int g = lane & 3;
@@ -169,19 +186,20 @@ __device__ __forceinline__ void warp_issue_planes32(const __half* hi_ptr, const 
   for (int i = 0; i < 4; ++i) {
     const int r = (lane >> 2) + 8 * i;
     const uint8_t* sh = shfl_ptr(reinterpret_cast<const uint8_t*>(hi_ptr), r);
-    const uint8_t* sl = shfl_ptr(reinterpret_cast<const uint8_t*>(lo_ptr), r);
+    const uint8_t* sl = kPlanes == 2 ? shfl_ptr(reinterpret_cast<const uint8_t*>(lo_ptr), r) : nullptr;
     vh[i] = make_uint4(0u, 0u, 0u, 0u);
     vl[i] = make_uint4(0u, 0u, 0u, 0u);
     if (sh) vh[i] = *reinterpret_cast<const uint4*>(sh + g * 16);
     if (sl) vl[i] = *reinterpret_cast<const uint4*>(sl + g * 16);
   }
 }
+template <int kPlanes = 2>
 __device__ __forceinline__ void warp_finish_planes32(uint32_t* scr, const uint4 (&vh)[4], const uint4 (&vl)[4], float (&x)[32]) {
   uint32_t h[16], l[16];
   const int lane = threadIdx.x & 31;
   const int g = lane & 3;
 #pragma unroll
-  for (int pass = 0; pass < 2; ++pass) {
+  for (int pass = 0; pass < kPlanes; ++pass) {
     __syncwarp();
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -202,9 +220,14 @@ __device__ __forceinline__ void warp_finish_planes32(uint32_t* scr, const uint4 
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&h[j]));
-    const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&l[j]));
-    x[2 * j] = fh.x + fl.x;
-    x[2 * j + 1] = fh.y + fl.y;
+    if constexpr (kPlanes == 2) {
+      const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&l[j]));
+      x[2 * j] = fh.x + fl.x;
+      x[2 * j + 1] = fh.y + fl.y;
+    } else {
+      x[2 * j] = fh.x;
+      x[2 * j + 1] = fh.y;
+    }
   }
 }
 __device__ __forceinline__ void warp_load_f32x32(uint32_t* scr, const float* ptr, float (&x)[32]) {
@@ -238,7 +261,9 @@ __device__ __forceinline__ void tma_store_box(const CUtensorMap* m, const void* 
   if (dims == 4) tma_store_4d(m, src, o.c0, o.c1, o.c2, o.c3);
   else tma_store_3d(m, src, o.c0, o.c1, o.c2);
 }
-// 32 values of my row -> fp16 hi/lo planes, box = 32 columns (64 B, 64-byte swizzle) x 32 rows
+// 32 values of my row -> fp16 hi/lo planes, box = 32 columns (64 B, 64-byte swizzle) x 32 rows.  kPlanes = 1: the hi
+// plane only (round to nearest even), through om.hi.
+template <int kPlanes = 2>
 __device__ __forceinline__ void warp_tma_store_planes32(uint32_t* stage, const OutMaps& om, const OutCoord& o, const float (&x)[32]) {
   const int lane = threadIdx.x & 31;
   uint32_t h[16], l[16];
@@ -252,13 +277,14 @@ __device__ __forceinline__ void warp_tma_store_planes32(uint32_t* stage, const O
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     *reinterpret_cast<uint4*>(stage + lane * 16 + ((q ^ sw) << 2)) = make_uint4(h[4 * q], h[4 * q + 1], h[4 * q + 2], h[4 * q + 3]);
-    *reinterpret_cast<uint4*>(stage + 512 + lane * 16 + ((q ^ sw) << 2)) = make_uint4(l[4 * q], l[4 * q + 1], l[4 * q + 2], l[4 * q + 3]);
+    if constexpr (kPlanes == 2)
+      *reinterpret_cast<uint4*>(stage + 512 + lane * 16 + ((q ^ sw) << 2)) = make_uint4(l[4 * q], l[4 * q + 1], l[4 * q + 2], l[4 * q + 3]);
   }
   fence_proxy_async();
   __syncwarp();
   if (lane == 0) {
     tma_store_box(&om.hi, stage, om.dims, o);
-    tma_store_box(&om.lo, stage + 512, om.dims, o);
+    if constexpr (kPlanes == 2) tma_store_box(&om.lo, stage + 512, om.dims, o);
     tma_store_commit();
   }
 }
@@ -643,9 +669,15 @@ struct EpiPlanes {
 // kUpsample selects the FPN merge at compile time.  false: every layer but the two FPN laterals, built without any
 // upsample code (leanest registers).  true: the two FPN lateral 1x1 convolutions; each thread gathers the four
 // bilinear neighbours of its pixel from the source planes in global memory (any shape).
-template <int BLOCK_N, bool kUpsample>
-struct EpiConv {
+//
+// kPlanes: 2 = split-precision activations (EpiConv): residual and upsample sources are read as hi + lo, outputs are
+// written as hi / lo planes, and the kernel's operands are hi / lo planes.  1 = single fp16 activations (EpiConvF16,
+// the fp16 backbone): the *_lo pointers and om.lo are unused, addends are read as their stored fp16 values, outputs are
+// rounded to nearest even into the hi plane, and the kernel runs one fp16 MMA per k-step (kOperandPlanes).
+template <int BLOCK_N, bool kUpsample, int kPlanes>
+struct EpiConvImpl {
   static constexpr bool kNoRowBound = true;      // backbone shapes are static: no device row bound (gemm_split.cuh)
+  static constexpr int kOperandPlanes = kPlanes;
   struct Params {
     const float* scale;   // [N]
     const float* shift;   // [N]
@@ -679,7 +711,7 @@ struct EpiConv {
   float* s_shift;
   uint32_t* scr;
   uint32_t* xscr;       // transposer scratch of the residual loads (== scr unless kOwnXpose)
-  __device__ EpiConv(const Params& p_, uint8_t* smem, const GemmShape& s_) : p(p_), s(s_), scr(epi_scratch(smem)) {
+  __device__ EpiConvImpl(const Params& p_, uint8_t* smem, const GemmShape& s_) : p(p_), s(s_), scr(epi_scratch(smem)) {
     s_scale = reinterpret_cast<float*>(smem + kEpiScratchBytes);
     s_shift = s_scale + kCols;
     xscr = kOwnXpose ? reinterpret_cast<uint32_t*>(smem + kXposeOffset + ((epi_tid() >> 5) << 11)) : scr;
@@ -714,7 +746,7 @@ struct EpiConv {
       const long pix = (static_cast<long>(batch) * p.H_out + y) * p.W_out + x;
       for (int c = c_lo; c < c_hi; c += 64) {
         prefetch_l2(p.res_hi + pix * p.res_ld + c);
-        prefetch_l2(p.res_lo + pix * p.res_ld + c);
+        if (kPlanes == 2) prefetch_l2(p.res_lo + pix * p.res_ld + c);
       }
     }
     if (kUpsample && p.up_hi) {
@@ -728,7 +760,7 @@ struct EpiConv {
       for (int q = 0; q < 4; ++q)
         for (int c = c_lo; c < c_hi; c += 64) {
           prefetch_l2(p.up_hi + u[q] + c);
-          prefetch_l2(p.up_lo + u[q] + c);
+          if (kPlanes == 2) prefetch_l2(p.up_lo + u[q] + c);
         }
     }
   }
@@ -776,7 +808,8 @@ struct EpiConv {
       const bool res_early = p.res_hi != nullptr && nvalid == 32;
       uint4 rh[4], rl[4];
       if (res_early)
-        warp_issue_planes32(ok ? p.res_hi + pix * p.res_ld + col : nullptr, ok ? p.res_lo + pix * p.res_ld + col : nullptr, rh, rl);
+        warp_issue_planes32<kPlanes>(ok ? p.res_hi + pix * p.res_ld + col : nullptr,
+                                     ok && kPlanes == 2 ? p.res_lo + pix * p.res_ld + col : nullptr, rh, rl);
       float v[32];
       load_acc32(acc_row, c * 32, v);
 #pragma unroll
@@ -786,7 +819,7 @@ struct EpiConv {
         if (p.res_hi) {
           if (p.om.use && !kOwnXpose) stage_quiesce();
           float r[32];
-          warp_finish_planes32(xscr, rh, rl, r);
+          warp_finish_planes32<kPlanes>(xscr, rh, rl, r);
 #pragma unroll
           for (int j = 0; j < 32; ++j) v[j] += r[j];
         }
@@ -796,14 +829,14 @@ struct EpiConv {
             const __half* uh = p.up_hi + col;
             const __half* ul = p.up_lo + col;
             float a[32], b[32];
-            load_planes32(uh + u00, ul + u00, a);
-            load_planes32(uh + u01, ul + u01, b);
+            load_planes32<kPlanes>(uh + u00, ul + u00, a);
+            load_planes32<kPlanes>(uh + u01, ul + u01, b);
             const float wy0 = 1.f - wy1, wx0 = 1.f - wx1;
             float top[32];
 #pragma unroll
             for (int j = 0; j < 32; ++j) top[j] = wx0 * a[j] + wx1 * b[j];
-            load_planes32(uh + u10, ul + u10, a);
-            load_planes32(uh + u11, ul + u11, b);
+            load_planes32<kPlanes>(uh + u10, ul + u10, a);
+            load_planes32<kPlanes>(uh + u11, ul + u11, b);
 #pragma unroll
             for (int j = 0; j < 32; ++j) v[j] += wy0 * top[j] + wy1 * (wx0 * a[j] + wx1 * b[j]);
           }
@@ -817,12 +850,14 @@ struct EpiConv {
           if (j >= nvalid) continue;
           if (p.res_hi) {
             const long o = pix * p.res_ld + col + j;
-            v[j] += __half2float(p.res_hi[o]) + __half2float(p.res_lo[o]);
+            v[j] += kPlanes == 2 ? __half2float(p.res_hi[o]) + __half2float(p.res_lo[o]) : __half2float(p.res_hi[o]);
           }
           if (kUpsample && p.up_hi) {
             const __half* uh = p.up_hi + col;
             const __half* ul = p.up_lo + col;
-            auto at = [&](long o) { return __half2float(uh[o + j]) + __half2float(ul[o + j]); };
+            auto at = [&](long o) {
+              return kPlanes == 2 ? __half2float(uh[o + j]) + __half2float(ul[o + j]) : __half2float(uh[o + j]);
+            };
             v[j] += wy0 * (wx0 * at(u00) + wx1 * at(u01)) + wy1 * (wx0 * at(u10) + wx1 * at(u11));
           }
         }
@@ -838,11 +873,12 @@ struct EpiConv {
       // outside the tensor are clipped by the map, so the TMA path also covers the channel tail and image borders
       const OutCoord oc{col, tx * kConvTileW, ty * kConvTileH + ((epi_tid() >> 5) & 3) * 2, batch};
       if (tma_f) warp_tma_store_f32x32(scr, p.om, oc, v);
-      if (tma_pl) warp_tma_store_planes32(scr, p.om, oc, v);
+      if (tma_pl) warp_tma_store_planes32<kPlanes>(scr, p.om, oc, v);
       if (nvalid == 32) {
         if (p.out_f32 && !tma_f) warp_store_f32x32(scr, ok ? p.out_f32 + pix * p.f32_ld + col : nullptr, v);
         if (p.out_hi && !tma_pl)
-          warp_store_planes32(scr, ok ? p.out_hi + pix * p.out_ld + col : nullptr, ok ? p.out_lo + pix * p.out_ld + col : nullptr, v);
+          warp_store_planes32<kPlanes>(scr, ok ? p.out_hi + pix * p.out_ld + col : nullptr,
+                                       ok && kPlanes == 2 ? p.out_lo + pix * p.out_ld + col : nullptr, v);
       } else if (ok && !(tma_pl || tma_f)) {
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
@@ -852,13 +888,23 @@ struct EpiConv {
             __half hh, ll;
             split_f16(v[j], hh, ll);
             p.out_hi[pix * p.out_ld + col + j] = hh;
-            p.out_lo[pix * p.out_ld + col + j] = ll;
+            if (kPlanes == 2) p.out_lo[pix * p.out_ld + col + j] = ll;
           }
         }
       }
     }
     if (s.n_tiles > 1) epi_bar_sync();  // s_scale / s_shift are rewritten by the next tile
   }
+};
+// The split-precision backbone's epilogue and its single-plane counterpart (two types, so that the split kernels keep
+// their instantiation names)
+template <int BLOCK_N, bool kUpsample>
+struct EpiConv : EpiConvImpl<BLOCK_N, kUpsample, 2> {
+  using EpiConvImpl<BLOCK_N, kUpsample, 2>::EpiConvImpl;
+};
+template <int BLOCK_N, bool kUpsample>
+struct EpiConvF16 : EpiConvImpl<BLOCK_N, kUpsample, 1> {
+  using EpiConvImpl<BLOCK_N, kUpsample, 1>::EpiConvImpl;
 };
 
 // ------------------------------------------------------------------------------------------------

@@ -89,6 +89,20 @@ struct EpiRowBound<Epi, decltype(void(Epi::kNoRowBound))> {
   static constexpr bool value = !Epi::kNoRowBound;
 };
 
+// Operand planes of a tensor-core kernel, declared by its epilogue: 2 (the default) = split precision, hi and lo planes
+// of A and B and three MMAs per k-step; an epilogue that declares `static constexpr int kOperandPlanes = 1;` runs the
+// kernel on single fp16 planes with one MMA per k-step (the fp16 backbone, EpiConvF16).  The ring then carries the hi
+// planes only and every stage is half as large.
+template <class Epi, class = void>
+struct EpiOperandPlanes {
+  static constexpr int value = 2;
+};
+template <class Epi>
+struct EpiOperandPlanes<Epi, decltype(void(Epi::kOperandPlanes))> {
+  static constexpr int value = Epi::kOperandPlanes;
+  static_assert(value == 1 || value == 2, "operands are one or two fp16 planes");
+};
+
 // K-major operand tile descriptor of a k-block (128-byte swizzle rows).
 __device__ __forceinline__ uint64_t desc_k(uint32_t smem_addr) { return wgmma_desc_k_sw128(smem_addr); }
 
@@ -102,15 +116,17 @@ __host__ __device__ constexpr int acc_stride(int block_n) { return block_n + 4; 
 __host__ __device__ constexpr int acc_bytes(int block_n) { return (kBlockM * acc_stride(block_n) + 32) * 4; }
 
 // Shared memory: [TMA ring | accumulator staging (aliased)][epilogue area][mbarriers].
-template <int BLOCK_N, int kEpiBytes = 0>
+// The ring aims at 192 KB whatever the operand planes: with one plane the stages are half as large and twice as many
+// are in flight (N = 128 / 208 / 256: 6 / 4 / 4 stages beside EpiConvF16, against 3 / 2 / 2 with two planes).
+template <int BLOCK_N, int kEpiBytes = 0, int kPlanes = 2>
 struct GemmSmem {
   static constexpr int kATile = kBlockM * kBlockK * 2;          // 16 KB per plane
   static constexpr int kBTile = BLOCK_N * kBlockK * 2;          // per plane
-  static constexpr int kStageBytes = 2 * kATile + 2 * kBTile;   // hi + lo of A and B
+  static constexpr int kStageBytes = kPlanes * (kATile + kBTile);   // hi (+ lo) of A and B
   static constexpr int kBarBytes = 256;
   static constexpr int kAccBytes = acc_bytes(BLOCK_N);
   static constexpr int kFit = (kSmemLimit - kBarBytes - kEpiBytes) / kStageBytes;
-  static constexpr int kWant = (192 * 1024) / kStageBytes;      // 2 (96 KB) / 3 (64 KB) / 4 (48 KB)
+  static constexpr int kWant = (192 * 1024) / kStageBytes;      // two planes: 2 (96 KB) / 3 (64 KB) / 4 (48 KB)
   static constexpr int kStages = kFit < kWant ? kFit : kWant;
   static_assert(kStages >= 2, "the TMA ring needs two stages");
   static constexpr int kRingBytes = kStages * kStageBytes > kAccBytes ? kStages * kStageBytes : kAccBytes;
@@ -218,7 +234,8 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                   const __grid_constant__ CUtensorMap tm_ar_hi, const __grid_constant__ CUtensorMap tm_ar_lo,
                   const __grid_constant__ CUtensorMap tm_br_hi, const __grid_constant__ CUtensorMap tm_br_lo,
                   const GemmShape shape, const __grid_constant__ typename Epi::Params epi_params) {
-  using S = GemmSmem<BLOCK_N, Epi::kSmemBytes>;
+  constexpr int kPlanes = EpiOperandPlanes<Epi>::value;   // 1: single fp16 planes, one MMA per k-step
+  using S = GemmSmem<BLOCK_N, Epi::kSmemBytes, kPlanes>;
   constexpr int kN = BLOCK_N / 2;   // columns per consumer warpgroup
   static_assert(kN % 8 == 0, "wgmma N must be a multiple of 8");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -238,10 +255,10 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
 
   // k-blocks of one output tile: K / 64 full blocks (+ the channel-remainder groups of a convolution)
   const int num_kb = shape.conv.enabled ? shape.conv.n_main + shape.conv.rem_groups : shape.K / kBlockK;
-  constexpr int kTapBytes = S::kStageBytes / kRemTapsPerStage;   // one tap of a remainder group: A_hi A_lo B_hi B_lo
+  constexpr int kTapBytes = S::kStageBytes / kRemTapsPerStage;   // one tap of a remainder group: A_hi (A_lo) B_hi (B_lo)
   constexpr int kRemATile = kBlockM * kRemChannels * 2;           // 4 KB
   constexpr int kRemBTile = S::kBTile / (kBlockK / kRemChannels);
-  static_assert(kTapBytes == 2 * kRemATile + 2 * kRemBTile && kTapBytes % 256 == 0 && kRemBTile % 256 == 0,
+  static_assert(kTapBytes == kPlanes * (kRemATile + kRemBTile) && kTapBytes % 256 == 0 && kRemBTile % 256 == 0,
                 "remainder group layout");
   // m tiles per batch: all of them, or those that hold live rows.  The count is written by an earlier kernel of the
   // stream, so it is read only here, after griddepcontrol.wait; producer and consumers read the same value.
@@ -282,9 +299,10 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                 uint8_t* base = st + t * kTapBytes;
                 const int c0 = g.cin_blocks * kBlockK;
                 tma_load_4d(base, &tm_ar_hi, fb, c0, x, y, w.batch);
-                tma_load_4d(base + kRemATile, &tm_ar_lo, fb, c0, x, y, w.batch);
-                tma_load_3d(base + 2 * kRemATile, &tm_br_hi, fb, tap * kRemChannels, nt * BLOCK_N, 0);
-                tma_load_3d(base + 2 * kRemATile + kRemBTile, &tm_br_lo, fb, tap * kRemChannels, nt * BLOCK_N, 0);
+                if constexpr (kPlanes == 2) tma_load_4d(base + kRemATile, &tm_ar_lo, fb, c0, x, y, w.batch);
+                tma_load_3d(base + kPlanes * kRemATile, &tm_br_hi, fb, tap * kRemChannels, nt * BLOCK_N, 0);
+                if constexpr (kPlanes == 2)
+                  tma_load_3d(base + 2 * kRemATile + kRemBTile, &tm_br_lo, fb, tap * kRemChannels, nt * BLOCK_N, 0);
               }
             } else {
               mbar_arrive_expect_tx(fb, S::kStageBytes);
@@ -297,15 +315,16 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                 const int x = tx * kConvTileW * g.stride + kx - g.pad;
                 const int y = ty * kConvTileH * g.stride + ky - g.pad;
                 tma_load_4d(st, &tm_a_hi, fb, cb * kBlockK, x, y, w.batch);
-                tma_load_4d(st + S::kATile, &tm_a_lo, fb, cb * kBlockK, x, y, w.batch);
+                if constexpr (kPlanes == 2) tma_load_4d(st + S::kATile, &tm_a_lo, fb, cb * kBlockK, x, y, w.batch);
               } else {
                 tma_load_3d(st, &tm_a_hi, fb, kb * kBlockK, w.mt * kBlockM, w.batch);
-                tma_load_3d(st + S::kATile, &tm_a_lo, fb, kb * kBlockK, w.mt * kBlockM, w.batch);
+                if constexpr (kPlanes == 2) tma_load_3d(st + S::kATile, &tm_a_lo, fb, kb * kBlockK, w.mt * kBlockM, w.batch);
               }
               // ---- B
               const int bb = shape.b_batched ? w.batch : 0;
-              tma_load_3d(st + 2 * S::kATile, &tm_b_hi, fb, kb * kBlockK, nt * BLOCK_N, bb);
-              tma_load_3d(st + 2 * S::kATile + S::kBTile, &tm_b_lo, fb, kb * kBlockK, nt * BLOCK_N, bb);
+              tma_load_3d(st + kPlanes * S::kATile, &tm_b_hi, fb, kb * kBlockK, nt * BLOCK_N, bb);
+              if constexpr (kPlanes == 2)
+                tma_load_3d(st + 2 * S::kATile + S::kBTile, &tm_b_lo, fb, kb * kBlockK, nt * BLOCK_N, bb);
             }
             pos.advance();
           }
@@ -346,9 +365,9 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                 const uint32_t a_off = static_cast<uint32_t>(mh * 64 * kRemChannels * 2);
                 const uint64_t ra_hi = wgmma_desc_k_sw32(base + a_off);
                 const uint64_t ra_lo = wgmma_desc_k_sw32(base + kRemATile + a_off);
-                const uint64_t rb_hi = wgmma_desc_k_sw32(base + 2 * kRemATile + b_off);
+                const uint64_t rb_hi = wgmma_desc_k_sw32(base + kPlanes * kRemATile + b_off);
                 const uint64_t rb_lo = wgmma_desc_k_sw32(base + 2 * kRemATile + kRemBTile + b_off);
-                wgmma_split<kN>(acc[mh], ra_hi, ra_lo, rb_hi, rb_lo);
+                wgmma_split<kN, kPlanes>(acc[mh], ra_hi, ra_lo, rb_hi, rb_lo);
               }
             }
           } else {
@@ -358,13 +377,13 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
               const uint32_t a_off = static_cast<uint32_t>(mh * 64 * kBlockK * 2);
               const uint64_t da_hi = desc_k(st + a_off);
               const uint64_t da_lo = desc_k(st + S::kATile + a_off);
-              const uint64_t db_hi = desc_k(st + 2 * S::kATile + b_off);
+              const uint64_t db_hi = desc_k(st + kPlanes * S::kATile + b_off);
               const uint64_t db_lo = desc_k(st + 2 * S::kATile + S::kBTile + b_off);
 #pragma unroll
               for (int k = 0; k < kBlockK / kMmaK; ++k) {
                 // advance 16 fp16 = 32 bytes along K inside the swizzle row: +2 in 16-byte units
                 const uint64_t adv = static_cast<uint64_t>(k * 2);
-                wgmma_split<kN>(acc[mh], da_hi + adv, da_lo + adv, db_hi + adv, db_lo + adv);
+                wgmma_split<kN, kPlanes>(acc[mh], da_hi + adv, da_lo + adv, db_hi + adv, db_lo + adv);
               }
             }
           }

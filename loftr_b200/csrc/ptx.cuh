@@ -204,12 +204,16 @@ __device__ __forceinline__ void wgmma_f16<256>(float (&d)[128], uint64_t desc_a,
 }
 
 // Split-precision product D += A * B^T of A = a_hi + a_lo and B = b_hi + b_lo, as hi*hi + hi*lo + lo*hi in that order
-// (the dropped lo*lo term is <= 2^-22 relative).
-template <int N>
+// (the dropped lo*lo term is <= 2^-22 relative).  kPlanes = 1: the operands are single fp16 planes and the product is
+// the one hi*hi MMA (a_lo / b_lo are not read).
+template <int N, int kPlanes = 2>
 __device__ __forceinline__ void wgmma_split(float (&d)[N / 2], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo) {
+  static_assert(kPlanes == 1 || kPlanes == 2, "operands are one or two fp16 planes");
   wgmma_f16<N>(d, a_hi, b_hi, 1u);
-  wgmma_f16<N>(d, a_hi, b_lo, 1u);
-  wgmma_f16<N>(d, a_lo, b_hi, 1u);
+  if constexpr (kPlanes == 2) {
+    wgmma_f16<N>(d, a_hi, b_lo, 1u);
+    wgmma_f16<N>(d, a_lo, b_hi, 1u);
+  }
 }
 
 // ---------------------------------------------------------------- descriptors

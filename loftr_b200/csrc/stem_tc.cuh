@@ -9,7 +9,8 @@
 // half (rows 0-63 and 64-127 x 4 k-steps x (hi*hi + hi*lo + lo*hi)).  The accumulator is staged row-major in shared
 // memory and all 8 warps run the epilogue (BN + ReLU + split, TMA store of 2 x 16 pixel x 32 channel boxes).  The
 // weights (128 x 49 fp32) are scaled by a power of two, split and swizzled into shared memory once per CTA.  One
-// persistent CTA per SM, 256 threads.
+// persistent CTA per SM, 256 threads.  conv_stem7x7_tc_fp16_kernel is the same kernel for the fp16 backbone: the
+// product stays split, only the output is one fp16 plane (rounded to nearest even, om.hi).
 #pragma once
 #include "epilogues.cuh"
 
@@ -21,7 +22,8 @@ struct StemTcParams {
   const float* wt;      // conv1.weight transposed [49][128]
   const float* scale;   // folded bn1 [128]
   const float* shift;
-  OutMaps om;           // NHWC planes [N, H/2, W/2, 128]: 4-D TMA-store maps (box 32 ch x 16 x 2 px)
+  OutMaps om;           // NHWC planes [N, H/2, W/2, 128]: 4-D TMA-store maps (box 32 ch x 16 x 2 px); om.lo unused
+                        // by the fp16 kernel
   int tiles_w, tiles_h; // 16- / 8-pixel tiles of the output grid
 };
 
@@ -41,7 +43,9 @@ __device__ __forceinline__ uint32_t stem_sw128(int row, int k) {   // byte offse
   return static_cast<uint32_t>(row * 128 + ((((k >> 3) ^ (row & 7)) << 4) | ((k & 7) << 1)));
 }
 
-__global__ void __launch_bounds__(kStemThreads, 1) conv_stem7x7_tc_kernel(const __grid_constant__ StemTcParams p) {
+// kOutPlanes: 2 = hi / lo output planes, 1 = the hi plane only
+template <int kOutPlanes>
+__device__ __forceinline__ void conv_stem7x7_tc(const StemTcParams& p) {
   pdl_trigger();   // the first convolution may set up meanwhile
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) asm volatile("trap;");
@@ -160,11 +164,19 @@ __global__ void __launch_bounds__(kStemThreads, 1) conv_stem7x7_tc_kernel(const 
         x[j + 2] = fmaxf(fmaf(v.z, sScale[c * 32 + j + 2], sShift[c * 32 + j + 2]), 0.f);
         x[j + 3] = fmaxf(fmaf(v.w, sScale[c * 32 + j + 3], sShift[c * 32 + j + 3]), 0.f);
       }
-      warp_tma_store_planes32(stage, p.om, OutCoord{c * 32, tx * kConvTileW, ty * kConvTileH + (warp & 3) * 2, n}, x);
+      warp_tma_store_planes32<kOutPlanes>(stage, p.om, OutCoord{c * 32, tx * kConvTileW, ty * kConvTileH + (warp & 3) * 2, n},
+                                          x);
     }
     __syncthreads();   // the staged accumulator and the operand tile are rewritten by the next tile
   }
   tma_store_wait_all();
+}
+
+__global__ void __launch_bounds__(kStemThreads, 1) conv_stem7x7_tc_kernel(const __grid_constant__ StemTcParams p) {
+  conv_stem7x7_tc<2>(p);
+}
+__global__ void __launch_bounds__(kStemThreads, 1) conv_stem7x7_tc_fp16_kernel(const __grid_constant__ StemTcParams p) {
+  conv_stem7x7_tc<1>(p);
 }
 
 }  // namespace lb

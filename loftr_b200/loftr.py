@@ -5,7 +5,8 @@ Same constructor argument (the lower-case config dict), same sub-module and para
 mutates `data` with the reference's output keys.  Everything runs in the hand-written sm_90a kernels behind the
 C ABI of include/loftr_b200.h: the ResNet-FPN backbone as implicit-GEMM convolutions on the tensor cores
 (`backbone_impl="b200"`, the default for the shipped ResNetFPN_8_2 shape; `"torch"` keeps the PyTorch/cuDNN fp32
-forward, which is closer to fp64 -- DESIGN.md §10), then position encoding, coarse transformer, coarse
+forward, which is closer to fp64 -- DESIGN.md §10; `"b200_fp16"` is the opt-in single-pass fp16 variant, faster and
+less accurate -- DESIGN.md §15), then position encoding, coarse transformer, coarse
 matching, fine windows, fine transformer and fine matching.
 There is no fallback path: without the built library / an H100 the forward raises.
 
@@ -91,14 +92,19 @@ def _require_cuda(t: torch.Tensor, name: str):
                            "no CPU implementation")
 
 
+def weight_exponent(w: torch.Tensor) -> int:
+    """The power-of-two exponent e of `split_weight`: max|w| * 2^e ~ 2^12, clamped to [-24, 24]."""
+    amax = float(w.abs().max())
+    e = 0 if amax == 0.0 else int(math.floor(math.log2(4096.0 / amax)))
+    return max(min(e, 24), -24)
+
+
 def split_weight(w: torch.Tensor):
     """Weight matrix -> (hi, lo, acc_scale): planes of w * 2^e with e chosen so that max|w| * 2^e ~ 2^12, and
     acc_scale = 2^-e for the epilogue.  Power-of-two scaling is exact; it moves the `lo` residuals of typical
     (small) weights out of fp16's subnormal range, where they would only carry ~1e-6 relative accuracy."""
     w = w.detach().float().contiguous()
-    amax = float(w.abs().max())
-    e = 0 if amax == 0.0 else int(math.floor(math.log2(4096.0 / amax)))
-    e = max(min(e, 24), -24)
+    e = weight_exponent(w)
     hi, lo = split_planes((w * (2.0 ** e)).contiguous())
     return hi, lo, 2.0 ** (-e)
 
@@ -122,10 +128,21 @@ class TensorCoreBackbone(_PackedCache):
     """ResNetFPN_8_2 forward through `lb_backbone_forward` (implicit-GEMM convolutions on wgmma).  Holds no
     parameters of its own: it packs the weights of the PyTorch `ResNetFPN` module it wraps (BatchNorm folded
     with its running statistics = eval mode), lazily and again whenever a parameter or buffer changes.  It is not a
-    submodule, so `LoFTR` drops its cache on `_apply` / `load_state_dict`."""
+    submodule, so `LoFTR` drops its cache on `_apply` / `load_state_dict`.
 
-    def __init__(self, torch_backbone):
+    precision: "split" (hi/lo planes, three MMAs per product: the parity path) or "fp16" (`lb_backbone_forward_fp16`:
+    single fp16 activations and one MMA per product after the stem; only the hi weight planes fp16(w * 2^e) are
+    packed, DESIGN.md §15)."""
+
+    PRECISIONS = ("split", "fp16")
+
+    def __init__(self, torch_backbone, precision="split"):
+        if precision not in self.PRECISIONS:
+            raise ValueError(f"TensorCoreBackbone: precision must be one of {self.PRECISIONS} (got {precision!r})")
+        if precision == "fp16":
+            _lib.require(_lib.BACKBONE_FP16_VERSION, 'the fp16 backbone (backbone_impl="b200_fp16")')
         self.m = torch_backbone
+        self.precision = precision
 
     def _packed_source(self):
         return self.m
@@ -161,16 +178,23 @@ class TensorCoreBackbone(_PackedCache):
             wr[:, :, :rem.value] = wt[:, :, cmain:]
             planes.append(wr.reshape(cout, k * k * 16))
         # one power-of-two scale for both plane sets (they feed the same accumulator)
-        hi, lo, acc_scale = split_weight(torch.cat(planes, 1))
+        wcat = torch.cat(planes, 1)
+        if self.precision == "fp16":
+            # the hi plane of split_weight, fp16(w * 2^e) rounded to nearest even (the scaling is exact); no lo plane
+            e = weight_exponent(wcat)
+            hi, lo, acc_scale = (wcat * (2.0 ** e)).half(), None, 2.0 ** (-e)
+        else:
+            hi, lo, acc_scale = split_weight(wcat)
         nmain = k * k * cmain
-        hi_m, lo_m = hi[:, :nmain].contiguous(), lo[:, :nmain].contiguous()
+        part = lambda t, cols: None if t is None else t[:, cols].contiguous()
+        hi_m, lo_m = part(hi, slice(0, nmain)), part(lo, slice(0, nmain))
         hi_r = lo_r = None
         if rem.value:
-            hi_r, lo_r = hi[:, nmain:].contiguous(), lo[:, nmain:].contiguous()
+            hi_r, lo_r = part(hi, slice(nmain, None)), part(lo, slice(nmain, None))
         scale, shift = self._fold(bn, cout, w.device)
         scale = (scale * acc_scale).contiguous()   # y = acc * (2^-e * bn_scale) + bn_shift
         keep += [hi_m, lo_m, hi_r, lo_r, scale, shift]
-        return _lib.LbConvWeights(hi_m.data_ptr(), lo_m.data_ptr(), _lib.ptr(hi_r), _lib.ptr(lo_r), scale.data_ptr(),
+        return _lib.LbConvWeights(hi_m.data_ptr(), _lib.ptr(lo_m), _lib.ptr(hi_r), _lib.ptr(lo_r), scale.data_ptr(),
                                   shift.data_ptr(), cin, cout, k, conv.stride[0])
 
     def _build(self):
@@ -208,10 +232,13 @@ class TensorCoreBackbone(_PackedCache):
         c3, c1 = self.m.layer3_outconv.out_channels, self.m.layer1_outconv2[3].out_channels
         feat_c = torch.empty(n, h // 8, wd // 8, c3, dtype=torch.float32, device=images.device)
         feat_f = torch.empty(n, h // 2, wd // 2, c1, dtype=torch.float32, device=images.device)
-        nbytes = lib.lb_backbone_workspace_bytes(C.byref(w), n, h, wd)
+        fp16 = self.precision == "fp16"
+        ws_bytes = lib.lb_backbone_workspace_bytes_fp16 if fp16 else lib.lb_backbone_workspace_bytes
+        forward = lib.lb_backbone_forward_fp16 if fp16 else lib.lb_backbone_forward
+        nbytes = ws_bytes(C.byref(w), n, h, wd)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=images.device)
-        _lib.check(lib.lb_backbone_forward(C.byref(w), images.data_ptr(), n, h, wd, feat_c.data_ptr(),
-                                           feat_f.data_ptr(), ws.data_ptr(), nbytes, _stream(images)))
+        _lib.check(forward(C.byref(w), images.data_ptr(), n, h, wd, feat_c.data_ptr(), feat_f.data_ptr(), ws.data_ptr(),
+                           nbytes, _stream(images)))
         return feat_c, feat_f
 
 
@@ -616,7 +643,10 @@ class LoFTR(nn.Module):
     def __init__(self, config, backbone_impl="auto"):
         """backbone_impl: "torch" keeps the PyTorch/cuDNN ResNet-FPN forward (the north_star default scope);
         "b200" runs it as implicit-GEMM convolutions on the tensor cores (SURVEY.md §8(f) rank 1); "auto" picks
-        "b200" whenever the configured backbone is the supported ResNetFPN_8_2 shape.  Both are GPU paths."""
+        "b200" whenever the configured backbone is the supported ResNetFPN_8_2 shape.  "b200_fp16" (opt-in, never
+        picked by "auto") runs the same convolutions with single fp16 activations and one fp16 MMA per product: faster,
+        but it does not meet the reference-parity target (DESIGN.md §10, §15); the transformers and matching stay
+        split-precision.  All are GPU paths."""
         super().__init__()
         self.config = config
         # the kernels are built for the shipped shapes; anything else must fail here, not at the first forward
@@ -636,12 +666,15 @@ class LoFTR(nn.Module):
         self.backbone = build_backbone(config)
         if backbone_impl == "auto":
             backbone_impl = "b200" if TensorCoreBackbone.supported(self.backbone) else "torch"
-        if backbone_impl not in ("torch", "b200"):
+        if backbone_impl not in ("torch", "b200", "b200_fp16"):
             raise ValueError(backbone_impl)
-        if backbone_impl == "b200" and not TensorCoreBackbone.supported(self.backbone):
+        if backbone_impl != "torch" and not TensorCoreBackbone.supported(self.backbone):
             raise ValueError("the tensor-core backbone is built for ResNetFPN_8_2 with initial_dim 128, dims <= 256")
         self.backbone_impl = backbone_impl
-        self._tc_backbone = TensorCoreBackbone(self.backbone) if backbone_impl == "b200" else None
+        self._tc_backbone = None
+        if backbone_impl != "torch":
+            precision = "fp16" if backbone_impl == "b200_fp16" else "split"
+            self._tc_backbone = TensorCoreBackbone(self.backbone, precision=precision)
         self.pos_encoding = PositionEncodingSine(config["coarse"]["d_model"],
                                                  temp_bug_fix=config["coarse"]["temp_bug_fix"])
         self.loftr_coarse = LocalFeatureTransformer(config["coarse"])
