@@ -515,7 +515,7 @@ struct TfWs {
   __half* att_lo;
   __half* h_hi;     // [R, 2C]
   __half* h_lo;
-  float* kv;        // [2*n_groups, H, D*D + D]
+  float* kv;        // coarse only: [2*n_groups, H, D*D + D]
   float* kv_part;   // coarse only: [2*n_groups, max(m_tiles, kKvSplits), H, per] (K^T V split partials)
 };
 // kv_gemm_kernel sums K^T V over at most max(m_tiles, kKvSplits) row splits per group.  That bound sizes kv_part here
@@ -531,7 +531,7 @@ static void carve_tf(Bump& b, TfWs& w, int C, int H, long R, int n_groups, bool 
   w.att_lo = b.take<__half>(static_cast<size_t>(R) * C);
   w.h_hi = b.take<__half>(static_cast<size_t>(R) * 2 * C);
   w.h_lo = b.take<__half>(static_cast<size_t>(R) * 2 * C);
-  w.kv = b.take<float>(static_cast<size_t>(2) * n_groups * H * (D * D + D));
+  w.kv = coarse ? b.take<float>(static_cast<size_t>(2) * n_groups * H * (D * D + D)) : nullptr;
   const size_t tiles = static_cast<size_t>((max_group_rows + kBlockM - 1) / kBlockM);
   const size_t parts = tiles > static_cast<size_t>(kKvSplits) ? tiles : static_cast<size_t>(kKvSplits);
   w.kv_part = coarse ? b.take<float>(static_cast<size_t>(2) * n_groups * H * parts * (D * D + D)) : nullptr;
@@ -856,21 +856,15 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
       window_full_attn_kernel<16, 8, 32><<<grid, 256, 0, stream>>>(w.qkv, 3 * C, 0, C, 2 * C, x_base, s_base,
                                                                    x_group_rows, n_groups_x, mask, w.att_hi, w.att_lo,
                                                                    C, live, live_cap);
-    } else if (x_group_rows == s_group_rows) {
+    } else {
       // linear attention, one kernel per pass: KV stays in shared memory      [linear_attention.py:43-46]
       const int grid = n_groups_x < 3 * sms ? n_groups_x : 3 * sms;   // 3 resident blocks per SM (60 KB, <= 85 registers)
-      const int wa_smem = (H * (D * D + D) + 4 * x_group_rows * C) * static_cast<int>(sizeof(float));
+      const int wa_smem = (H * (D * D + D) + 4 * s_group_rows * C) * static_cast<int>(sizeof(float));
       LB_TRY((set_max_dynamic_smem<&window_attn_kernel<16, 8>>(
           (8 * (16 * 16 + 16) + 4 * 32 * 128) * static_cast<int>(sizeof(float)))));   // largest (32-row) window
       window_attn_kernel<16, 8><<<grid, 256, wa_smem, stream>>>(w.qkv, 3 * C, 0, C, 2 * C, x_base, s_base, x_group_rows,
-                                                                n_groups_x, 1e-6f, w.att_hi, w.att_lo, C, live, live_cap);
-    } else {
-      // linear attention between windows of different sizes (a cross pass of the standalone fine transformer): KV and
-      // Ksum per source window through HBM, then one 32-row block per query window   [linear_attention.py:43-46]
-      kv_window_kernel<16, 8><<<n_groups_s, 256, 0, stream>>>(w.qkv, 3 * C, C, 2 * C, s_base, s_group_rows, w.kv);
-      LB_LAUNCHED();
-      attn_apply_kernel<16, 8><<<dim3(n_groups_x, 1), 256, 0, stream>>>(w.qkv, 3 * C, 0, x_base, x_group_rows, 32,
-                                                                        w.kv, 1e-6f, w.att_hi, w.att_lo, C);
+                                                                s_group_rows, n_groups_x, 1e-6f, w.att_hi, w.att_lo, C,
+                                                                live, live_cap);
     }
     LB_LAUNCHED();
   }

@@ -157,121 +157,17 @@ __global__ void kv_tile_merge_kernel(const float* __restrict__ part, int nparts,
   kv[i] = acc;
 }
 
-// Window variant for the fine transformer (group = one window of at most 32 rows, D = 16, H = 8): one block per
-// window, all heads; writes kv directly.  Only the cross pass between windows of different sizes uses it (with
-// attn_apply_kernel<16, 8>); equal windows run window_attn_kernel.
-template <int D, int H>
-__global__ void __launch_bounds__(256) kv_window_kernel(const float* __restrict__ qkv, int ld, int k_col0,
-                                                        int v_col0, long row_base, int rows_per_group,
-                                                        float* __restrict__ kv) {
-  static_assert(D == 16 && H == 8, "fine head layout");
-  constexpr int C = D * H;  // 128
-  constexpr int MAXR = 32;
-  __shared__ __align__(16) float sK[MAXR][C];
-  __shared__ __align__(16) float sV[MAXR][C];
-  const int g = blockIdx.x;
-  const int tid = threadIdx.x;
-  for (int i = tid; i < rows_per_group * (C / 4); i += 256) {
-    const int s = i / (C / 4), c4 = (i % (C / 4)) * 4;
-    const float* rowp = qkv + (row_base + static_cast<long>(g) * rows_per_group + s) * ld;
-    *reinterpret_cast<float4*>(&sK[s][c4]) = *reinterpret_cast<const float4*>(rowp + k_col0 + c4);
-    *reinterpret_cast<float4*>(&sV[s][c4]) = *reinterpret_cast<const float4*>(rowp + v_col0 + c4);
-  }
-  __syncthreads();
-  const int hd = tid >> 5;          // 0..7
-  const int d = (tid & 31) >> 1;    // 0..15
-  const int v0 = (tid & 1) * 8;     // 0 or 8
-  float acc[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-  float ks = 0.f;
-  for (int s = 0; s < rows_per_group; ++s) {
-    const float k = sK[s][hd * D + d];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j] = fmaf(k, sV[s][hd * D + v0 + j], acc[j]);
-    ks += k;
-  }
-  float* out = kv + (static_cast<long>(g) * H + hd) * (D * D + D);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) out[d * D + v0 + j] = acc[j];
-  if ((tid & 1) == 0) out[D * D + d] = ks;
-}
-
 // ------------------------------------------------------------------------------------------------
-// Linear attention, query side (reference linear_attention.py:45-46):
+// Fine (window) linear attention (reference linear_attention.py:43-46 on the [M, 25, 128] window sequences of
+// fine_preprocess.py), one kernel per pass:
 //   out[r,h,:] = (Q[r,h,:] . KV[g,h]) / (Q[r,h,:] . Ksum[g,h] + eps)
-// written as fp16 planes = the A operand of the merge projection.  One warp per head, lanes = rows.
-template <int D, int H>
-__global__ void __launch_bounds__(32 * H) attn_apply_kernel(const float* __restrict__ qkv, int ld, int q_col0,
-                                                            long x_row_base, int rows_per_group,
-                                                            int rows_per_block, const float* __restrict__ kv,
-                                                            float eps, __half* __restrict__ att_hi,
-                                                            __half* __restrict__ att_lo, int ld_att) {
-  constexpr int PER = D * D + D;
-  __shared__ __align__(16) float sKV[H][PER];
-  const int g = blockIdx.x;
-  const int r_begin = blockIdx.y * rows_per_block;
-  const int r_end = min(r_begin + rows_per_block, rows_per_group);
-  const int hd = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  {
-    const float* src = kv + static_cast<long>(g) * H * PER;
-    float* dst = &sKV[0][0];
-    for (int i = threadIdx.x; i < H * PER; i += 32 * H) dst[i] = src[i];
-  }
-  __syncthreads();
-  const float* kvh = sKV[hd];
-  for (int r0 = r_begin; r0 < r_end; r0 += 32) {
-    const int r = r0 + lane;
-    if (r < r_end) {
-      const long row = x_row_base + static_cast<long>(g) * rows_per_group + r;
-      float q[D];
-      const float4* qp = reinterpret_cast<const float4*>(qkv + row * ld + q_col0 + hd * D);
-#pragma unroll
-      for (int j = 0; j < D / 4; ++j) {
-        const float4 t = qp[j];
-        q[4 * j] = t.x; q[4 * j + 1] = t.y; q[4 * j + 2] = t.z; q[4 * j + 3] = t.w;
-      }
-      float zden = eps;
-#pragma unroll
-      for (int d = 0; d < D; ++d) zden = fmaf(q[d], kvh[D * D + d], zden);
-      const float z = 1.f / zden;
-      __half* hp = att_hi + row * ld_att + hd * D;
-      __half* lp = att_lo + row * ld_att + hd * D;
-#pragma unroll
-      for (int v8 = 0; v8 < D; v8 += 8) {
-        float o[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = 0.f;
-#pragma unroll
-        for (int d = 0; d < D; ++d) {
-          const float4 a = *reinterpret_cast<const float4*>(&kvh[d * D + v8]);
-          const float4 b = *reinterpret_cast<const float4*>(&kvh[d * D + v8 + 4]);
-          o[0] = fmaf(q[d], a.x, o[0]); o[1] = fmaf(q[d], a.y, o[1]);
-          o[2] = fmaf(q[d], a.z, o[2]); o[3] = fmaf(q[d], a.w, o[3]);
-          o[4] = fmaf(q[d], b.x, o[4]); o[5] = fmaf(q[d], b.y, o[5]);
-          o[6] = fmaf(q[d], b.z, o[6]); o[7] = fmaf(q[d], b.w, o[7]);
-        }
-        uint32_t hw[4], lw[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          split_f16x2(o[2 * j] * z, o[2 * j + 1] * z, hw[j], lw[j]);
-        }
-        *reinterpret_cast<uint4*>(hp + v8) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-        *reinterpret_cast<uint4*>(lp + v8) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-      }
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Fine (window) linear attention in ONE kernel: kv_window_kernel + attn_apply_kernel<16, 8> back to back per window
-// (reference linear_attention.py:43-46 on the [M, 25, 128] window sequences of fine_preprocess.py).  One block takes
-// windows g, g + gridDim.x, ...; KV[h] = K_h^T V_h and Ksum_h are built in shared memory (never in HBM) and warp h /
-// lane r applies them to query row r.  The kernel is latency-bound on the q/k/v reads (ncu: 34 % of the samples wait
-// on them), so the NEXT window's K / V rows travel global -> shared with cp.async into the other half of a double
-// buffer and its query row into registers while the current window is computed.  Same summation order as the
-// two-kernel path: bit-identical output.  Dynamic shared memory: 2 x 2 x rows x 512 B + 8.7 KB (60 KB for 25 rows).
+// written as fp16 planes = the A operand of the merge projection.  Query window g has x_rows rows and source window g
+// s_rows rows (both <= 32; they differ in a cross pass of the standalone fine transformer with L != S).  One block
+// takes windows g, g + gridDim.x, ...; KV[h] = K_h^T V_h and Ksum_h over the s_rows source rows are built in shared
+// memory (never in HBM) and warp h / lane r applies them to query row r.  The kernel is latency-bound on the q/k/v
+// reads (ncu: 34 % of the samples wait on them), so the NEXT window's K / V rows travel global -> shared with cp.async
+// into the other half of a double buffer and its query row into registers while the current window is computed.
+// Dynamic shared memory: 2 x 2 x s_rows x 512 B + 8.7 KB (60 KB for 25 rows).
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }
@@ -282,7 +178,7 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 template <int D, int H>
 __global__ void __launch_bounds__(32 * H, 3) window_attn_kernel(const float* __restrict__ qkv, int ld, int q_col0, int k_col0,
                                                                 int v_col0, long x_row_base, long s_row_base,
-                                                                int rows_per_group, int n_groups, float eps,
+                                                                int x_rows, int s_rows, int n_groups, float eps,
                                                                 __half* __restrict__ att_hi, __half* __restrict__ att_lo,
                                                                 int ld_att, const int* __restrict__ live, int live_cap) {
   pdl_trigger();
@@ -291,25 +187,25 @@ __global__ void __launch_bounds__(32 * H, 3) window_attn_kernel(const float* __r
   constexpr int PER = D * D + D;
   extern __shared__ __align__(16) float wa_smem[];
   float* sKV = wa_smem;                                   // [H][PER]
-  float* sKVbuf = wa_smem + H * PER;                      // [2][K | V][rows][C]
-  const int buf_floats = 2 * rows_per_group * C;
+  float* sKVbuf = wa_smem + H * PER;                      // [2][K | V][s_rows][C]
+  const int buf_floats = 2 * s_rows * C;
   const int tid = threadIdx.x;
   const int hd = tid >> 5, lane = tid & 31;
-  const bool has_row = lane < rows_per_group;
+  const bool has_row = lane < x_rows;
 
   auto issue = [&](int g, int b) {   // K / V rows of window g -> buffer b
     float* dK = sKVbuf + b * buf_floats;
-    float* dV = dK + rows_per_group * C;
-    for (int i = tid; i < rows_per_group * (C / 4); i += 32 * H) {
+    float* dV = dK + s_rows * C;
+    for (int i = tid; i < s_rows * (C / 4); i += 32 * H) {
       const int r = i / (C / 4), c4 = (i % (C / 4)) * 4;
-      const float* rowp = qkv + (s_row_base + static_cast<long>(g) * rows_per_group + r) * ld;
+      const float* rowp = qkv + (s_row_base + static_cast<long>(g) * s_rows + r) * ld;
       cp_async16(dK + r * C + c4, rowp + k_col0 + c4);
       cp_async16(dV + r * C + c4, rowp + v_col0 + c4);
     }
   };
   auto load_q = [&](int g, float (&q)[D]) {
     const float4* qp = reinterpret_cast<const float4*>(
-        qkv + (x_row_base + static_cast<long>(g) * rows_per_group + lane) * ld + q_col0 + hd * D);
+        qkv + (x_row_base + static_cast<long>(g) * x_rows + lane) * ld + q_col0 + hd * D);
 #pragma unroll
     for (int j = 0; j < D / 4; ++j) {
       const float4 t = qp[j];
@@ -350,15 +246,15 @@ __global__ void __launch_bounds__(32 * H, 3) window_attn_kernel(const float* __r
     cp_async_wait<1>();      // this thread's copies of window g have landed ...
     __syncthreads();         // ... and everybody else's
     const float* sK = sKVbuf + b * buf_floats;
-    const float* sV = sK + rows_per_group * C;
-    // KV[hd][d][v0..v0+7] and Ksum[hd][d] over the window's rows
+    const float* sV = sK + s_rows * C;
+    // KV[hd][d][v0..v0+7] and Ksum[hd][d] over the source window's rows
     {
       const int d = lane >> 1, v0 = (lane & 1) * 8;
       float acc[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[j] = 0.f;
       float ks = 0.f;
-      for (int r = 0; r < rows_per_group; ++r) {
+      for (int r = 0; r < s_rows; ++r) {
         const float k = sK[r * C + hd * D + d];
         const float4 a = *reinterpret_cast<const float4*>(&sV[r * C + hd * D + v0]);
         const float4 c = *reinterpret_cast<const float4*>(&sV[r * C + hd * D + v0 + 4]);
@@ -375,7 +271,7 @@ __global__ void __launch_bounds__(32 * H, 3) window_attn_kernel(const float* __r
     // message row = (q . KV) / (q . Ksum + eps) -> fp16 planes
     if (has_row) {
       const float* kvh = sKV + hd * PER;
-      const long xrow = x_row_base + static_cast<long>(g) * rows_per_group + lane;
+      const long xrow = x_row_base + static_cast<long>(g) * x_rows + lane;
       float zden = eps;
 #pragma unroll
       for (int d = 0; d < D; ++d) zden = fmaf(q[d], kvh[D * D + d], zden);

@@ -817,10 +817,10 @@ class LoFTR(nn.Module):
         refined: the fine stage reads the count on the device.
 
         capacity: defaults to the exact bound of the coarse stage, n*min(L, S) (n*L with masks), or n*min(k, that
-        per-pair bound) with match_coarse.max_matches_per_pair = k.  The fine stage keeps about 5 KB of state per window
-        row, i.e. about 256 KB per match of capacity (about 10 GB at batch 8 640x480 without k): a smaller capacity
-        trades that memory for the risk of overflow, which stays visible in num_matches.  A capacity of n*k never
-        overflows.
+        per-pair bound) with match_coarse.max_matches_per_pair = k.  The fine stage keeps about 4.8 KB of state per
+        window row, i.e. about 240 KB per match of capacity (about 9.4 GB at batch 8 640x480 without k): a smaller
+        capacity trades that memory for the risk of overflow, which stays visible in num_matches.  A capacity of n*k
+        never overflows.
 
         Configurations whose output list depends on the data (match_coarse.thr < 0) raise ValueError."""
         _require_static(self, capacity, "forward_static")

@@ -1,10 +1,11 @@
 """Record the exact output bits of the whole matcher (tests/golden/matcher_bits.npz) for
 tests/test_matcher_bits_gpu.py: the SHA-256 of every tensor output of `matcher(batch)` for each case of MATCHER_CASES, of the
-live prefix of every `forward_static` output, and of `lb_gemm_split` at N = 128 and 256; the outputs of FULL are stored
-in full as well.  Between them the cases launch every tensor-core kernel instantiation of the library (the backbone's
-convolutions, every GEMM epilogue of the transformers and of both coarse matchings, the linear and full attention
-kernels).  A change that only restructures kernel code must keep these bits; a change to any summation order must
-regenerate them (and say so).  Needs an H100; LOFTR_B200_LIB selects the build that defines the reference bits.
+live prefix of every `forward_static` output, of `lb_gemm_split` at N = 128 and 256, and of the standalone fine
+transformer between windows of different sizes (FINE_TF_CASES); the outputs of FULL are stored in full as well.
+Between them the cases launch every tensor-core kernel instantiation of the library (the backbone's convolutions,
+every GEMM epilogue of the transformers and of both coarse matchings, the linear and full attention kernels).  A
+change that only restructures kernel code must keep these bits; a change to any summation order must regenerate them
+(and say so).  Needs an H100; LOFTR_B200_LIB selects the build that defines the reference bits.
 
     LOFTR_B200_LIB=<variant> python tests/golden/make_golden_matcher_bits.py [OUT.npz]
 """
@@ -49,6 +50,12 @@ MATCHER_CASES = {
                                   "valid1": [(112, 128), (96, 144)], "match_type": "sinkhorn"}, "static"),
 }
 GEMM_CASES = {"gemm_n128": (2, 300, 128, 256), "gemm_n256": (1, 1000, 256, 128)}   # (batches, M, N, K)
+# model.loftr_fine(f0, f1[, mask0, mask1]) with the shipped ["self", "cross"] linear layers on windows of L and S rows:
+# the cross layer pairs windows of different sizes.  450 windows per side: more than one window per block of the
+# window kernel (at most 3 blocks per SM).  name -> (L, S, padding masks)
+FINE_TF_CASES = {f"fine_tf_{l}x{s}{'_masked' if m else ''}": (l, s, m)
+                 for l, s in ((25, 16), (16, 25), (32, 9)) for m in (False, True)}
+FINE_TF_WINDOWS = 450
 FULL = "ds_thr0"   # stored in full as well
 # keys of forward_static whose first dimension is the match capacity: only the live prefix is defined
 _LIST_KEYS = ("b_ids", "i_ids", "j_ids", "m_bids", "gt_mask", "mconf", "mkpts0_c", "mkpts1_c", "mkpts0_f", "mkpts1_f",
@@ -114,11 +121,31 @@ def gemm_output(name):
     return {"out": out}
 
 
+def fine_tf_output(name):
+    """-> the two outputs of the fine transformer of the ds_thr0 model at FINE_TF_CASES[name] on seeded features (and
+    masks that pad every window to its size after a valid prefix of at least one row)."""
+    l, s, masked = FINE_TF_CASES[name]
+    model = _model(_C["ds_thr0"], False)
+    rs = np.random.RandomState(7)
+    n = FINE_TF_WINDOWS
+    f0 = torch.from_numpy(rs.standard_normal((n, l, 128)).astype(np.float32)).to(DEV)
+    f1 = torch.from_numpy(rs.standard_normal((n, s, 128)).astype(np.float32)).to(DEV)
+    masks = ()
+    if masked:
+        masks = tuple(torch.from_numpy(np.arange(rows)[None, :] < rs.randint(1, rows + 1, size=(n, 1))).to(DEV)
+                      for rows in (l, s))
+    g0, g1 = model.loftr_fine(f0, f1, *masks)
+    torch.cuda.synchronize()
+    return {"feat0": g0, "feat1": g1}
+
+
 def outputs(name):
-    return gemm_output(name) if name in GEMM_CASES else matcher_outputs(name)
+    if name in GEMM_CASES:
+        return gemm_output(name)
+    return fine_tf_output(name) if name in FINE_TF_CASES else matcher_outputs(name)
 
 
-NAMES = list(MATCHER_CASES) + list(GEMM_CASES)
+NAMES = list(MATCHER_CASES) + list(GEMM_CASES) + list(FINE_TF_CASES)
 
 
 def main():

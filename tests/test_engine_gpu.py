@@ -56,7 +56,7 @@ def test_transformer_matches_oracle(cfgname):
     model, cfg, _ = util.build_model(case, DEV)
     rs = np.random.RandomState(3)
     if cfgname.startswith("fine_windows"):
-        # unequal: the cross layer pairs 25-row with 16-row windows (kv_window_kernel + attn_apply_kernel<16, 8>)
+        # unequal: the cross layer pairs 25-row with 16-row windows (window_attn_kernel with x_rows != s_rows)
         tf, tcfg = model.loftr_fine, cfg["fine"]
         n, l, s, c = (37, 25, 16, 128) if cfgname == "fine_windows_unequal" else (37, 25, 25, 128)
         m0 = m1 = None

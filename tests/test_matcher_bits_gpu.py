@@ -3,8 +3,9 @@
 The cases launch every tensor-core kernel instantiation: the backbone's convolutions (gemm_split_kernel's convolution
 mode, conv3x3_halo_kernel, the stem), the transformers' GEMMs with linear (kv_gemm_kernel) and full
 (full_attn_wgmma_kernel) attention, both coarse matchings with and without the Sinkhorn prefilter, masked unequal-size
-pairs, return_conf_matrix, the static path and the lb_gemm_split hook.  Every kernel is deterministic, so every output
-must keep its bits, not merely stay within a tolerance."""
+pairs, return_conf_matrix, the static path and the lb_gemm_split hook.  Further cases run the standalone fine
+transformer's linear attention between windows of different sizes, with and without padding masks.  Every kernel is
+deterministic, so every output must keep its bits, not merely stay within a tolerance."""
 import os
 
 import numpy as np

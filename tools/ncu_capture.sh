@@ -12,7 +12,7 @@ timeout 600 $NCU --metrics gpu__time_duration.sum --csv --log-file gpurun_out/${
   python tools/profile_step.py > gpurun_out/${tag}_launches.out 2>&1
 FULL="--set full --import-source on"
 # first self layer + first cross pass of the coarse transformer (every kernel kind once or twice)
-timeout 900 $NCU $FULL -k regex:"EpiActStore|EpiLayerNorm|EpiPlanes|EpiKv|EpiAttn|kv_partial|attn_apply|kv_merge|kv_tile_merge|coarse_prep" -c "${NCU_TF_COUNT:-16}" \
+timeout 900 $NCU $FULL -k regex:"EpiActStore|EpiLayerNorm|EpiPlanes|EpiKv|EpiAttn|kv_tile_merge|coarse_prep" -c "${NCU_TF_COUNT:-16}" \
   -f -o gpurun_out/${tag}_tf python tools/profile_step.py > gpurun_out/${tag}_tf.out 2>&1
 timeout 900 $NCU $FULL -k regex:"EpiConv|stem" -c 23 -f -o gpurun_out/${tag}_conv python tools/profile_step.py \
   > gpurun_out/${tag}_conv.out 2>&1
