@@ -283,7 +283,7 @@ struct Planes {
 
 // ------------------------------------------------------------------------------------------------ GEMM launch
 struct GemmMaps {
-  CUtensorMap a_hi, a_lo, b_hi, b_lo;      // 64-element k-blocks
+  CUtensorMap a_hi, a_lo, b_hi, b_lo;      // boxes one ring stage deep along K (GemmSmem::kBK)
   CUtensorMap ar_hi, ar_lo, br_hi, br_lo;  // convolution channel remainder (16-element boxes); copies of the above if unused
 };
 
@@ -356,12 +356,13 @@ static int launch_gemm(int tag, const Planes& A, const Planes& B, int batches, i
   s.live_count = live;
   s.live_unit_rows = live_unit_rows;
 
+  constexpr int kBK = GemmSmem<BN, Epi::kSmemBytes, EpiOperandPlanes<Epi>::value>::kBK;
   GemmMaps mp;
-  LB_TRY(make_map(&mp.a_hi, A.hi, K, M, batches, A.ld, A.batch_stride, kBlockM));
-  LB_TRY(make_map(&mp.a_lo, A.lo, K, M, batches, A.ld, A.batch_stride, kBlockM));
+  LB_TRY(make_map(&mp.a_hi, A.hi, K, M, batches, A.ld, A.batch_stride, kBlockM, kBK));
+  LB_TRY(make_map(&mp.a_lo, A.lo, K, M, batches, A.ld, A.batch_stride, kBlockM, kBK));
   const int bb = s.b_batched ? batches : 1;
-  LB_TRY(make_map(&mp.b_hi, B.hi, K, N, bb, B.ld, B.batch_stride, BN));
-  LB_TRY(make_map(&mp.b_lo, B.lo, K, N, bb, B.ld, B.batch_stride, BN));
+  LB_TRY(make_map(&mp.b_hi, B.hi, K, N, bb, B.ld, B.batch_stride, BN, kBK));
+  LB_TRY(make_map(&mp.b_lo, B.lo, K, N, bb, B.ld, B.batch_stride, BN, kBK));
   mp.ar_hi = mp.a_hi; mp.ar_lo = mp.a_lo; mp.br_hi = mp.b_hi; mp.br_lo = mp.b_lo;
   return launch_raw<BN, Epi>(tag, mp, s, ep, sms, st);
 }
@@ -386,8 +387,10 @@ static void conv_layout(int cin, int* cin_blocks, int* rem) {
 }
 // The implicit GEMM of convolution d with BN-wide n tiles (one per work item), and the output geometry its epilogue
 // reads.  *rem: the remainder channels per tap (0: none).  lo: the weights have lo planes (split precision).
+// rem_taps_per_group: taps of one remainder group (ConvGeom::rem_groups).
 template <int BN, class Params>
-static int conv_shape(const ConvDesc& d, const Planes& wgt_rem, bool lo, GemmShape* s, Params* ep, int* rem) {
+static int conv_shape(const ConvDesc& d, const Planes& wgt_rem, bool lo, int rem_taps_per_group, GemmShape* s,
+                      Params* ep, int* rem) {
   int cin_blocks = 0;
   conv_layout(d.Cin, &cin_blocks, rem);
   if (*rem && (!wgt_rem.hi || (lo && !wgt_rem.lo)))
@@ -396,7 +399,7 @@ static int conv_shape(const ConvDesc& d, const Planes& wgt_rem, bool lo, GemmSha
   const int tiles_h = (d.H_out + kConvTileH - 1) / kConvTileH;
   const int tiles_w = (d.W_out + kConvTileW - 1) / kConvTileW;
   const int m_tiles = tiles_h * tiles_w, n_tiles = (d.Cout + BN - 1) / BN;
-  const int rem_groups = *rem ? (taps + kRemTapsPerStage - 1) / kRemTapsPerStage : 0;
+  const int rem_groups = *rem ? (taps + rem_taps_per_group - 1) / rem_taps_per_group : 0;
   *s = GemmShape{d.N, m_tiles * kBlockM, d.Cout, taps * cin_blocks * kBlockK, /*b_batched=*/0, m_tiles, n_tiles,
                  /*n_chunks=*/n_tiles, /*tiles_per_chunk=*/1,
                  ConvGeom{1, tiles_w, d.stride, d.pad, d.ksize, cin_blocks, taps, taps * cin_blocks, rem_groups},
@@ -413,19 +416,20 @@ template <int BN, class Epi>
 static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_rem, const ConvDesc& d,
                        const typename Epi::Params& ep_in, cudaStream_t st) {
   constexpr bool kLo = EpiOperandPlanes<Epi>::value == 2;
+  using S = GemmSmem<BN, Epi::kSmemBytes, EpiOperandPlanes<Epi>::value>;
   int sms = 0;
   LB_TRY(device_check(&sms));
   GemmShape s;
   typename Epi::Params ep = ep_in;
   int rem = 0;
-  LB_TRY(conv_shape<BN>(d, wgt_rem, kLo, &s, &ep, &rem));
+  LB_TRY(conv_shape<BN>(d, wgt_rem, kLo, S::kRemTapsPerStage, &s, &ep, &rem));
   GemmMaps mp;
-  LB_TRY(make_map_nhwc(&mp.a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride));
-  LB_TRY(make_map(&mp.b_hi, wgt.hi, s.K, d.Cout, 1, wgt.ld, 0, BN));
+  LB_TRY(make_map_nhwc(&mp.a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, S::kBK));
+  LB_TRY(make_map(&mp.b_hi, wgt.hi, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
   mp.a_lo = mp.a_hi; mp.b_lo = mp.b_hi;
   if (kLo) {
-    LB_TRY(make_map_nhwc(&mp.a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride));
-    LB_TRY(make_map(&mp.b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN));
+    LB_TRY(make_map_nhwc(&mp.a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, S::kBK));
+    LB_TRY(make_map(&mp.b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
   }
   if (rem) {
     LB_TRY(make_map_nhwc(&mp.ar_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, kRemChannels));
@@ -454,7 +458,7 @@ static int launch_conv_halo(const Planes& in, const Planes& wgt, const Planes& w
   GemmShape s;
   typename Epi::Params ep = ep_in;
   int rem = 0;
-  LB_TRY(conv_shape<BN>(d, wgt_rem, kLo, &s, &ep, &rem));
+  LB_TRY(conv_shape<BN>(d, wgt_rem, kLo, kHaloTaps, &s, &ep, &rem));   // the remainder is one 16-channel halo
   CUtensorMap a_hi, a_lo, b_hi, b_lo, br_hi, br_lo;
   LB_TRY(make_map_halo(&a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld));
   LB_TRY(make_map(&b_hi, wgt.hi, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));

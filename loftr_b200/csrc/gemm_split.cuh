@@ -16,9 +16,13 @@
 //   warps 0-7  : two consumer warpgroups.  Warpgroup h issues the wgmma of the tile's column half h (M = 128 as two
 //                m64 instructions, N = BLOCK_N / 2, K = 16), stages its fp32 accumulator in shared memory (row-major,
 //                padded rows) and then runs the epilogue on it: thread t owns accumulator row t%128 and column half
-//                t/128.  The staging area aliases the TMA ring, so the producer starts the next tile's loads only
-//                once the epilogue has released it.
-//   warp 8     : TMA producer    (global -> 128B-swizzled smem ring, 4 tiles per stage)
+//                t/128.  The staging area aliases the GemmSmem::kAccStages consecutive ring stages the tile consumed
+//                last (GemmSmem::staging_first), so the producer loads the next tile into the other stages while the
+//                epilogue runs and waits for the epilogue's release (acc_free) only before it writes a staged one.
+//   warp 8     : TMA producer    (global -> swizzled smem ring; a stage holds the A and B tiles, hi and lo planes)
+// A ring stage holds GemmSmem::kBK of K: 32 (64-byte swizzle rows) with two planes, 64 (128-byte swizzle rows) with one,
+// so a stage is as large either way and 4-6 stages are in flight.  The k16 MMAs run in the same k order at any stage
+// depth, so the stage depth does not change a bit of the result.
 // Everything between the first wgmma of a tile and its last wait_group is warpgroup-uniform (no per-lane branches,
 // every consumer thread arrives on the ring's empty barriers): otherwise ptxas serialises the asynchronous MMAs.
 #pragma once
@@ -27,7 +31,7 @@
 namespace lb {
 
 constexpr int kBlockM = 128;
-constexpr int kBlockK = 64;   // k-block of one pipeline stage: 64 fp16 = one 128-byte swizzle row
+constexpr int kBlockK = 64;   // granularity of K (and of a convolution's channel blocks): 64 fp16 = one 128-byte row
 constexpr int kMmaK = 16;
 constexpr int kGemmThreads = 288;
 constexpr int kEpiThreads = 256;  // two epilogue warpgroups: rows x {left, right} half of the tile's columns
@@ -43,10 +47,9 @@ constexpr int kConvTileH = 8;
 constexpr int kConvTileW = 16;
 // Channel remainder (Cin = 64*cin_blocks + r, 0 < r <= 16, e.g. 196 = 3*64 + 4): instead of a fourth, 94 % empty
 // 64-channel block per tap, the r channels of every tap travel as 16-channel boxes (32-byte swizzle rows, one K = 16
-// MMA step per tap); four taps share one pipeline stage ("remainder group").  K-steps per output for a 3x3 / Cin = 196
-// convolution: 9*3*4 + 9 = 117 instead of 9*4*4 = 144.
+// MMA step per tap); GemmSmem::kRemTapsPerStage taps (2 with two planes, 4 with one) share one pipeline stage
+// ("remainder group").  K-steps per output for a 3x3 / Cin = 196 convolution: 9*3*4 + 9 = 117 instead of 9*4*4 = 144.
 constexpr int kRemChannels = 16;
-constexpr int kRemTapsPerStage = 4;
 struct ConvGeom {
   int enabled;     // 0: plain GEMM (3-D maps)
   int tiles_w;     // spatial tiles per tile row; m_tile = ty * tiles_w + tx
@@ -56,7 +59,7 @@ struct ConvGeom {
   int cin_blocks;  // full 64-channel blocks per tap
   int taps;        // kernel taps (ksize^2)
   int n_main;      // taps * cin_blocks k-blocks of 64 channels
-  int rem_groups;  // 0, or ceil(taps / 4) remainder groups that follow the main k-blocks
+  int rem_groups;  // 0, or the remainder groups (ceil(taps / kRemTapsPerStage)) that follow the main k-blocks
 };
 
 struct GemmShape {
@@ -103,8 +106,13 @@ struct EpiOperandPlanes<Epi, decltype(void(Epi::kOperandPlanes))> {
   static_assert(value == 1 || value == 2, "operands are one or two fp16 planes");
 };
 
-// K-major operand tile descriptor of a k-block (128-byte swizzle rows).
-__device__ __forceinline__ uint64_t desc_k(uint32_t smem_addr) { return wgmma_desc_k_sw128(smem_addr); }
+// K-major operand tile descriptor of a ring stage holding kBK of K: rows of 128 bytes (kBK = 64, 128-byte swizzle) or
+// 64 bytes (kBK = 32, 64-byte swizzle).
+template <int kBK>
+__device__ __forceinline__ uint64_t desc_k(uint32_t smem_addr) {
+  static_assert(kBK == 32 || kBK == 64, "a stage holds 32 or 64 of K");
+  return kBK == 64 ? wgmma_desc_k_sw128(smem_addr) : wgmma_desc_k_sw64(smem_addr);
+}
 
 // Dynamic shared memory a block may opt in to on the H100 (227 KB).
 constexpr int kSmemLimit = 232448;
@@ -115,21 +123,44 @@ constexpr int kSmemLimit = 232448;
 __host__ __device__ constexpr int acc_stride(int block_n) { return block_n + 4; }   // floats
 __host__ __device__ constexpr int acc_bytes(int block_n) { return (kBlockM * acc_stride(block_n) + 32) * 4; }
 
-// Shared memory: [TMA ring | accumulator staging (aliased)][epilogue area][mbarriers].
-// The ring aims at 192 KB whatever the operand planes: with one plane the stages are half as large and twice as many
-// are in flight (N = 128 / 208 / 256: 6 / 4 / 4 stages beside EpiConvF16, against 3 / 2 / 2 with two planes).
+// Shared memory: [TMA ring (the accumulator staging aliases kAccStages consecutive stages)][epilogue area][mbarriers].
+// A stage holds kBK of K: 32 with two planes (64-byte swizzle rows), 64 with one, so the stages are as large either way
+// and the ring of about 192 KB holds 6 / 4 / 4 of them at N = 128 / 208 / 256 (32 / 42 / 48 KB each).  The staged
+// accumulator (acc_bytes) covers 3 of them at every N, which leaves 3 / 1 / 1 stages to the producer while the
+// epilogue runs.
 template <int BLOCK_N, int kEpiBytes = 0, int kPlanes = 2>
 struct GemmSmem {
-  static constexpr int kATile = kBlockM * kBlockK * 2;          // 16 KB per plane
-  static constexpr int kBTile = BLOCK_N * kBlockK * 2;          // per plane
+  static constexpr int kBK = kPlanes == 2 ? kBlockK / 2 : kBlockK;
+  static constexpr int kATile = kBlockM * kBK * 2;              // per plane
+  static constexpr int kBTile = BLOCK_N * kBK * 2;              // per plane
   static constexpr int kStageBytes = kPlanes * (kATile + kBTile);   // hi (+ lo) of A and B
   static constexpr int kBarBytes = 256;
   static constexpr int kAccBytes = acc_bytes(BLOCK_N);
   static constexpr int kFit = (kSmemLimit - kBarBytes - kEpiBytes) / kStageBytes;
-  static constexpr int kWant = (192 * 1024) / kStageBytes;      // two planes: 2 (96 KB) / 3 (64 KB) / 4 (48 KB)
+  static constexpr int kWant = (192 * 1024) / kStageBytes;
   static constexpr int kStages = kFit < kWant ? kFit : kWant;
-  static_assert(kStages >= 2, "the TMA ring needs two stages");
-  static constexpr int kRingBytes = kStages * kStageBytes > kAccBytes ? kStages * kStageBytes : kAccBytes;
+  static constexpr int kRingBytes = kStages * kStageBytes;
+  static constexpr int kAccStages = (kAccBytes + kStageBytes - 1) / kStageBytes;   // stages the staging covers
+  static_assert(kAccStages < kStages, "the ring needs a stage beside the staged accumulator");
+  static_assert((2 * kStages + 1) * 8 <= kBarBytes, "barrier area");
+  // channel remainder: one tap = a 16-channel box of A and of B per plane; kBK / 16 taps per stage
+  static constexpr int kRemATile = kBlockM * kRemChannels * 2;   // 4 KB
+  static constexpr int kRemBTile = BLOCK_N * kRemChannels * 2;
+  static constexpr int kTapBytes = kPlanes * (kRemATile + kRemBTile);
+  static constexpr int kRemTapsPerStage = kStageBytes / kTapBytes;
+  static_assert(kRemTapsPerStage * kTapBytes == kStageBytes && kTapBytes % 256 == 0 && kRemBTile % 256 == 0,
+                "remainder group layout");
+
+  // First ring stage of the staged accumulator of a tile whose last k-stage was in ring stage `last`: the kAccStages
+  // stages that end at `last`, so the stages that follow it in ring order (where the next tile's loads go) stay free.
+  // When those would wrap around the ring's end, the last kAccStages stages of the ring, the farthest from last + 1.
+  // Producer and consumers both place the staging with this function.
+  __host__ __device__ static constexpr int staging_first(int last) {
+    return last >= kAccStages - 1 ? last - kAccStages + 1 : kStages - kAccStages;
+  }
+  __host__ __device__ static constexpr bool staged_over(int first, int stage) {
+    return stage >= first && stage < first + kAccStages;
+  }
 };
 
 // ---- pieces shared by the persistent kernels (gemm_split_kernel, conv3x3_halo_kernel)
@@ -200,8 +231,11 @@ __device__ __forceinline__ void stage_acc(float* stg, int stride, const float (&
 }
 
 // Tile end of a consumer thread, after the tile's last wgmma_commit: drain the MMAs, release the ring slots they read
-// (release_ring), stage the accumulator over the ring (stage) once both warpgroups' MMAs are done with it, run the
-// epilogue on this thread's staged row and hand the ring back to the producer (acc_free).
+// (release_ring), stage the accumulator at `stg` (stage) once both warpgroups' MMAs are done with the ring, run the
+// epilogue on this thread's staged row and hand the staging memory back to the producer (acc_free).  `stg` must be
+// memory the producer does not write before acc_free: gemm_split_kernel's producer keeps off the kAccStages ring stages
+// from GemmSmem::staging_first until then, conv3x3_halo_kernel's off its whole weight ring (and the halo slots when the
+// staging reaches into them).
 template <int BLOCK_N, class Epi, class Acc, class Release, class Stage>
 __device__ __forceinline__ void finish_tile(Epi& epi, Acc& acc, Release release_ring, Stage stage, const float* stg,
                                             int ct, uint64_t* acc_free, int batch, int m0, int n0) {
@@ -253,13 +287,16 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
                                                 acc_free, [] {});
   const int lane = threadIdx.x & 31;
 
-  // k-blocks of one output tile: K / 64 full blocks (+ the channel-remainder groups of a convolution)
-  const int num_kb = shape.conv.enabled ? shape.conv.n_main + shape.conv.rem_groups : shape.K / kBlockK;
-  constexpr int kTapBytes = S::kStageBytes / kRemTapsPerStage;   // one tap of a remainder group: A_hi (A_lo) B_hi (B_lo)
-  constexpr int kRemATile = kBlockM * kRemChannels * 2;           // 4 KB
-  constexpr int kRemBTile = S::kBTile / (kBlockK / kRemChannels);
-  static_assert(kTapBytes == kPlanes * (kRemATile + kRemBTile) && kTapBytes % 256 == 0 && kRemBTile % 256 == 0,
-                "remainder group layout");
+  // k-stages (ring stages) of one output tile: K / kBK (+ the channel-remainder groups of a convolution).  A stage of
+  // the main loop is part j of k-block ks / kSubs (64 of K: a convolution's (tap, 64-channel block)), K offset ks * kBK.
+  constexpr int kBK = S::kBK;
+  constexpr int kSubs = kBlockK / kBK;
+  const int n_main = shape.conv.enabled ? shape.conv.n_main * kSubs : shape.K / kBK;
+  const int num_ks = n_main + (shape.conv.enabled ? shape.conv.rem_groups : 0);
+  constexpr int kTapBytes = S::kTapBytes;   // one tap of a remainder group: A_hi (A_lo) B_hi (B_lo)
+  constexpr int kRemATile = S::kRemATile;
+  constexpr int kRemBTile = S::kRemBTile;
+  constexpr int kRemTapsPerStage = S::kRemTapsPerStage;
   // m tiles per batch: all of them, or those that hold live rows.  The count is written by an earlier kernel of the
   // stream, so it is read only here, after griddepcontrol.wait; producer and consumers read the same value.
   int m_tiles = shape.m_tiles;
@@ -274,20 +311,28 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     if (lane == 0) {
       RingPos<S::kStages> pos;
       uint32_t tiles = 0;
+      int staged = -1;   // first ring stage of the previous tile's staged accumulator until acc_free is waited on
       for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
         const WorkItem w = work_item(shape, m_tiles, item);
         for (int nt = w.nt_begin; nt < w.nt_end; ++nt) {
-          if (tiles > 0) mbar_wait(acc_free, (tiles - 1) & 1);   // the previous tile's staged accumulator is consumed
-          ++tiles;
-          for (int kb = 0; kb < num_kb; ++kb) {
+          int last = 0;
+          for (int ks = 0; ks < num_ks; ++ks) {
+            // The previous tile's epilogue must release its staging before a stage under it is refilled.  The wait
+            // comes at the latest before this tile's last load: the consumers cannot finish this tile before it, so
+            // acc_free never runs two phases ahead of the parity waited on.
+            if (staged >= 0 && (S::staged_over(staged, pos.stage) || ks == num_ks - 1)) {
+              mbar_wait(acc_free, (tiles - 1) & 1);
+              staged = -1;
+            }
             mbar_wait(&empty_bar[pos.stage], pos.phase ^ 1);
             uint8_t* st = ring + pos.stage * S::kStageBytes;
             uint64_t* fb = &full_bar[pos.stage];
-            const bool rem_group = shape.conv.enabled && kb >= shape.conv.n_main;
+            const bool rem_group = ks >= n_main;
             if (rem_group) {
-              // ---- channel remainder: up to four taps, each a 16-channel box of A (hi, lo) and of the weights
+              // ---- channel remainder: up to kRemTapsPerStage taps, each a 16-channel box of A (hi, lo) and of the
+              // weights
               const ConvGeom& g = shape.conv;
-              const int rem_t0 = (kb - g.n_main) * kRemTapsPerStage;
+              const int rem_t0 = (ks - n_main) * kRemTapsPerStage;
               const int rem_nt = min(kRemTapsPerStage, g.taps - rem_t0);
               mbar_arrive_expect_tx(fb, static_cast<uint32_t>(rem_nt) * kTapBytes);
               const int ty = w.mt / g.tiles_w, tx = w.mt - ty * g.tiles_w;
@@ -307,27 +352,33 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             } else {
               mbar_arrive_expect_tx(fb, S::kStageBytes);
               // ---- A: 128 rows (or an 8 x 16 pixel patch shifted by the tap)
+              const int k0 = ks * kBK;
               if (shape.conv.enabled) {
                 const ConvGeom& g = shape.conv;
+                const int kb = ks / kSubs;
                 const int tap = kb / g.cin_blocks, cb = kb - tap * g.cin_blocks;
                 const int ky = tap / g.taps_w, kx = tap - ky * g.taps_w;
                 const int ty = w.mt / g.tiles_w, tx = w.mt - ty * g.tiles_w;
                 const int x = tx * kConvTileW * g.stride + kx - g.pad;
                 const int y = ty * kConvTileH * g.stride + ky - g.pad;
-                tma_load_4d(st, &tm_a_hi, fb, cb * kBlockK, x, y, w.batch);
-                if constexpr (kPlanes == 2) tma_load_4d(st + S::kATile, &tm_a_lo, fb, cb * kBlockK, x, y, w.batch);
+                const int c0 = cb * kBlockK + (ks - kb * kSubs) * kBK;
+                tma_load_4d(st, &tm_a_hi, fb, c0, x, y, w.batch);
+                if constexpr (kPlanes == 2) tma_load_4d(st + S::kATile, &tm_a_lo, fb, c0, x, y, w.batch);
               } else {
-                tma_load_3d(st, &tm_a_hi, fb, kb * kBlockK, w.mt * kBlockM, w.batch);
-                if constexpr (kPlanes == 2) tma_load_3d(st + S::kATile, &tm_a_lo, fb, kb * kBlockK, w.mt * kBlockM, w.batch);
+                tma_load_3d(st, &tm_a_hi, fb, k0, w.mt * kBlockM, w.batch);
+                if constexpr (kPlanes == 2) tma_load_3d(st + S::kATile, &tm_a_lo, fb, k0, w.mt * kBlockM, w.batch);
               }
-              // ---- B
+              // ---- B (a convolution's weight planes hold k-block (tap, cb) at (tap * cin_blocks + cb) * 64)
               const int bb = shape.b_batched ? w.batch : 0;
-              tma_load_3d(st + kPlanes * S::kATile, &tm_b_hi, fb, kb * kBlockK, nt * BLOCK_N, bb);
+              tma_load_3d(st + kPlanes * S::kATile, &tm_b_hi, fb, k0, nt * BLOCK_N, bb);
               if constexpr (kPlanes == 2)
-                tma_load_3d(st + 2 * S::kATile + S::kBTile, &tm_b_lo, fb, kb * kBlockK, nt * BLOCK_N, bb);
+                tma_load_3d(st + 2 * S::kATile + S::kBTile, &tm_b_lo, fb, k0, nt * BLOCK_N, bb);
             }
+            last = pos.stage;
             pos.advance();
           }
+          staged = S::staging_first(last);
+          ++tiles;
         }
       }
     }
@@ -337,7 +388,6 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     const int h = ct >> 7;                          // column half of the tile
     Epi epi(epi_params, epi_smem, shape);
     float acc[2][kN / 2];                           // rows [0, 64) and [64, 128) of this warpgroup's column half
-    float* stg = reinterpret_cast<float*>(ring);
     RingPos<S::kStages> pos;
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
       const WorkItem w = work_item(shape, m_tiles, item);
@@ -349,13 +399,13 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
 #pragma unroll
         for (int i = 0; i < kN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
         int prev = -1;
-        for (int kb = 0; kb < num_kb; ++kb) {
+        for (int ks = 0; ks < num_ks; ++ks) {
           mbar_wait(&full_bar[pos.stage], pos.phase);
           const uint32_t st = smem_u32(ring + pos.stage * S::kStageBytes);
           wgmma_fence();
-          if (shape.conv.enabled && kb >= shape.conv.n_main) {
-            // remainder group: one K = 16 step per tap, 32-byte swizzle rows (kb > 0 here: always accumulate)
-            const int rem_t0 = (kb - shape.conv.n_main) * kRemTapsPerStage;
+          if (ks >= n_main) {
+            // remainder group: one K = 16 step per tap, 32-byte swizzle rows (ks > 0 here: always accumulate)
+            const int rem_t0 = (ks - n_main) * kRemTapsPerStage;
             const int rem_nt = min(kRemTapsPerStage, shape.conv.taps - rem_t0);
             for (int t = 0; t < rem_nt; ++t) {
               const uint32_t base = st + t * kTapBytes;
@@ -371,16 +421,16 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
               }
             }
           } else {
-            const uint32_t b_off = static_cast<uint32_t>(h * kN * kBlockK * 2);
+            const uint32_t b_off = static_cast<uint32_t>(h * kN * kBK * 2);
 #pragma unroll
             for (int mh = 0; mh < 2; ++mh) {
-              const uint32_t a_off = static_cast<uint32_t>(mh * 64 * kBlockK * 2);
-              const uint64_t da_hi = desc_k(st + a_off);
-              const uint64_t da_lo = desc_k(st + S::kATile + a_off);
-              const uint64_t db_hi = desc_k(st + kPlanes * S::kATile + b_off);
-              const uint64_t db_lo = desc_k(st + 2 * S::kATile + S::kBTile + b_off);
+              const uint32_t a_off = static_cast<uint32_t>(mh * 64 * kBK * 2);
+              const uint64_t da_hi = desc_k<kBK>(st + a_off);
+              const uint64_t da_lo = desc_k<kBK>(st + S::kATile + a_off);
+              const uint64_t db_hi = desc_k<kBK>(st + kPlanes * S::kATile + b_off);
+              const uint64_t db_lo = desc_k<kBK>(st + 2 * S::kATile + S::kBTile + b_off);
 #pragma unroll
-              for (int k = 0; k < kBlockK / kMmaK; ++k) {
+              for (int k = 0; k < kBK / kMmaK; ++k) {
                 // advance 16 fp16 = 32 bytes along K inside the swizzle row: +2 in 16-byte units
                 const uint64_t adv = static_cast<uint64_t>(k * 2);
                 wgmma_split<kN, kPlanes>(acc[mh], da_hi + adv, da_lo + adv, db_hi + adv, db_lo + adv);
@@ -388,11 +438,12 @@ gemm_split_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
             }
           }
           wgmma_commit();
-          wgmma_wait<1>();   // the previous k-block's MMAs are done: its slot may be refilled
+          wgmma_wait<1>();   // the previous k-stage's MMAs are done: its slot may be refilled
           if (prev >= 0) mbar_arrive(&empty_bar[prev]);
           prev = pos.stage;
           pos.advance();
         }
+        float* stg = reinterpret_cast<float*>(ring + S::staging_first(prev) * S::kStageBytes);
         finish_tile<BLOCK_N>(
             epi, acc, [&] { mbar_arrive(&empty_bar[prev]); },
             [&] {
