@@ -149,9 +149,11 @@ class TensorCoreBackbone(_PackedCache):
 
     @staticmethod
     def supported(torch_backbone) -> bool:
+        # feat_c is stored through an fp32 NHWC tensor map, whose row stride (4 * d3 bytes) must be a multiple of 16
         m = torch_backbone
+        d3 = m.layer3[0].conv1.out_channels
         return getattr(m, "depth", 0) == 3 and m.conv1.out_channels == 128 and m.layer1[0].conv1.out_channels == 128 \
-            and max(m.layer2[0].conv1.out_channels, m.layer3[0].conv1.out_channels) <= 256
+            and max(m.layer2[0].conv1.out_channels, d3) <= 256 and d3 % 4 == 0
 
     @staticmethod
     def _fold(bn, cout, device):
@@ -669,7 +671,8 @@ class LoFTR(nn.Module):
         if backbone_impl not in ("torch", "b200", "b200_fp16"):
             raise ValueError(backbone_impl)
         if backbone_impl != "torch" and not TensorCoreBackbone.supported(self.backbone):
-            raise ValueError("the tensor-core backbone is built for ResNetFPN_8_2 with initial_dim 128, dims <= 256")
+            raise ValueError("the tensor-core backbone is built for ResNetFPN_8_2 with initial_dim 128, dims <= 256 and "
+                             "a layer3 width divisible by 4")
         self.backbone_impl = backbone_impl
         self._tc_backbone = None
         if backbone_impl != "torch":
