@@ -56,7 +56,9 @@ extern "C" {
  * 104: lb_coarse_prep_indexed / lb_fine_preprocess_indexed (pairs read from a per-image feature bank);
  * 105: lb_coarse_match_capped (at most k matches per pair, chosen by confidence);
  * 106: lb_preprocess_images (uint8 images of any size -> the matcher's padded fp32 input and 1/8 mask);
- * 107: lb_estimate_geometry (batched RANSAC homography / fundamental matrix per pair). */
+ * 107: lb_estimate_geometry (batched RANSAC homography / fundamental matrix per pair);
+ * 108: lb_backbone_workspace_bytes_fp16 / lb_backbone_forward_fp16 (single-pass fp16 backbone);
+ * 109: lb_transformer_forward_fp16 / lb_coarse_match_fp16 (single-pass fp16 transformers and coarse matching). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -233,6 +235,15 @@ size_t lb_transformer_workspace_bytes(int d_model, int nhead, int n_groups, int 
 int lb_transformer_forward(const LbEncoderLayerWeights* layers /*host*/, const int* kinds /*host*/, int n_layers,
                            int d_model, int nhead, const LbTransformerState* st /*host*/, void* ws,
                            size_t ws_bytes, void* stream);
+/* The same layers with one fp16 MMA per tensor-core product (version 109; DESIGN.md §16): every projection, merge and
+ * MLP product, K^T V / Ksum of the coarse linear attention and S = Q K^T, P V of the coarse full attention multiply the
+ * hi planes of their operands only (P rounded once to fp16), with fp32 accumulation.  Epilogues, LayerNorm, residuals
+ * (read as hi + lo), masks, the stored hi / lo planes, the fp32 window-attention kernels and the workspace
+ * (lb_transformer_workspace_bytes) are those of lb_transformer_forward.  The *_lo weight planes are not read and may
+ * be NULL. */
+int lb_transformer_forward_fp16(const LbEncoderLayerWeights* layers /*host*/, const int* kinds /*host*/, int n_layers,
+                                int d_model, int nhead, const LbTransformerState* st /*host*/, void* ws,
+                                size_t ws_bytes, void* stream);
 
 typedef struct LbCoarseMatchArgs {
   const void* f0_hi;   /* planes of feat_c0 [n_pairs*L, >=C] */
@@ -273,6 +284,12 @@ int lb_coarse_match(const LbCoarseMatchArgs* args /*host*/, void* ws, size_t ws_
  * affected.  One more launch than lb_coarse_match (timing tag "match_cap"); same workspace. */
 int lb_coarse_match_capped(const LbCoarseMatchArgs* args /*host*/, int max_per_pair, void* ws, size_t ws_bytes,
                            void* stream);
+/* Coarse matching with the score matrix computed as hi(f0) . hi(f1), one fp16 MMA per product (version 109;
+ * DESIGN.md §16), in every pass (log-sum-exp, Sinkhorn iterations, arg-maxima, prefilter, conf_matrix), so all passes
+ * see the same logits.  f0_lo / f1_lo are not read and may be NULL.  max_per_pair: 0 = no cap (as lb_coarse_match),
+ * >= 1 as lb_coarse_match_capped; negative values are an error.  Same workspace. */
+int lb_coarse_match_fp16(const LbCoarseMatchArgs* args /*host*/, int max_per_pair, void* ws, size_t ws_bytes,
+                         void* stream);
 
 typedef struct LbFinePreprocessArgs {
   const float* feat_f0;   /* fine maps, any strides (elements): index = n*sn + c*sc + y*sh + x*sw */

@@ -132,9 +132,12 @@ SIGNATURES = {
     "lb_transformer_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "lb_transformer_forward": (c_int, [C.POINTER(LbEncoderLayerWeights), C.POINTER(c_int), c_int, c_int, c_int,
                                        C.POINTER(LbTransformerState), c_void_p, c_size_t, c_void_p]),
+    "lb_transformer_forward_fp16": (c_int, [C.POINTER(LbEncoderLayerWeights), C.POINTER(c_int), c_int, c_int, c_int,
+                                            C.POINTER(LbTransformerState), c_void_p, c_size_t, c_void_p]),
     "lb_coarse_match_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "lb_coarse_match": (c_int, [C.POINTER(LbCoarseMatchArgs), c_void_p, c_size_t, c_void_p]),
     "lb_coarse_match_capped": (c_int, [C.POINTER(LbCoarseMatchArgs), c_int, c_void_p, c_size_t, c_void_p]),
+    "lb_coarse_match_fp16": (c_int, [C.POINTER(LbCoarseMatchArgs), c_int, c_void_p, c_size_t, c_void_p]),
     "lb_fine_preprocess_workspace_bytes": (c_size_t, [c_long, c_int, c_int]),
     "lb_fine_preprocess": (c_int, [C.POINTER(LbFinePreprocessArgs), c_void_p, c_size_t, c_void_p]),
     "lb_fine_preprocess_indexed": (c_int, [C.POINTER(LbFinePreprocessArgs), c_void_p, c_void_p, c_void_p, c_size_t,
@@ -167,12 +170,15 @@ PREPROCESS_VERSION = 106
 GEOMETRY_VERSION = 107
 # oldest library with the single-pass fp16 backbone (lb_backbone_forward_fp16, backbone_impl="b200_fp16")
 BACKBONE_FP16_VERSION = 108
+# oldest library with the single-pass fp16 transformers and coarse matching (match_precision="fp16")
+MATCH_FP16_VERSION = 109
 GEOMETRY_HOMOGRAPHY = 0
 GEOMETRY_FUNDAMENTAL = 1
 _SINCE = {"lb_coarse_prep_indexed": FEATURE_BANK_VERSION, "lb_fine_preprocess_indexed": FEATURE_BANK_VERSION,
           "lb_coarse_match_capped": MATCH_CAP_VERSION, "lb_preprocess_images": PREPROCESS_VERSION,
           "lb_geometry_workspace_bytes": GEOMETRY_VERSION, "lb_estimate_geometry": GEOMETRY_VERSION,
-          "lb_backbone_workspace_bytes_fp16": BACKBONE_FP16_VERSION, "lb_backbone_forward_fp16": BACKBONE_FP16_VERSION}
+          "lb_backbone_workspace_bytes_fp16": BACKBONE_FP16_VERSION, "lb_backbone_forward_fp16": BACKBONE_FP16_VERSION,
+          "lb_transformer_forward_fp16": MATCH_FP16_VERSION, "lb_coarse_match_fp16": MATCH_FP16_VERSION}
 
 
 class LibraryMissing(RuntimeError):

@@ -356,13 +356,17 @@ static int launch_gemm(int tag, const Planes& A, const Planes& B, int batches, i
   s.live_count = live;
   s.live_unit_rows = live_unit_rows;
 
+  // one operand plane: the lo maps are copies of the hi ones and never loaded (A.lo / B.lo may be null)
+  constexpr bool kLo = EpiOperandPlanes<Epi>::value == 2;
   constexpr int kBK = GemmSmem<BN, Epi::kSmemBytes, EpiOperandPlanes<Epi>::value>::kBK;
   GemmMaps mp;
   LB_TRY(make_map(&mp.a_hi, A.hi, K, M, batches, A.ld, A.batch_stride, kBlockM, kBK));
-  LB_TRY(make_map(&mp.a_lo, A.lo, K, M, batches, A.ld, A.batch_stride, kBlockM, kBK));
+  mp.a_lo = mp.a_hi;
+  if (kLo) LB_TRY(make_map(&mp.a_lo, A.lo, K, M, batches, A.ld, A.batch_stride, kBlockM, kBK));
   const int bb = s.b_batched ? batches : 1;
   LB_TRY(make_map(&mp.b_hi, B.hi, K, N, bb, B.ld, B.batch_stride, BN, kBK));
-  LB_TRY(make_map(&mp.b_lo, B.lo, K, N, bb, B.ld, B.batch_stride, BN, kBK));
+  mp.b_lo = mp.b_hi;
+  if (kLo) LB_TRY(make_map(&mp.b_lo, B.lo, K, N, bb, B.ld, B.batch_stride, BN, kBK));
   mp.ar_hi = mp.a_hi; mp.ar_lo = mp.a_lo; mp.br_hi = mp.b_hi; mp.br_lo = mp.b_lo;
   return launch_raw<BN, Epi>(tag, mp, s, ep, sms, st);
 }
@@ -527,6 +531,12 @@ struct TfWs {
 // formula changes the output bits.
 constexpr int kKvSplits = 8;
 
+// Operand planes of the transformer and score-matrix products: 2 = split precision (hi*hi + hi*lo + lo*hi), 1 = the hi
+// planes only, one fp16 MMA per product (match_precision "fp16": lb_transformer_forward_fp16 / lb_coarse_match_fp16,
+// DESIGN.md §16).  The epilogues are the same; only the kernels' main loops read and multiply less.
+template <class Epi, int kP>
+using Operands = std::conditional_t<kP == 2, Epi, EpiF16Operands<Epi>>;
+
 static void carve_tf(Bump& b, TfWs& w, int C, int H, long R, int n_groups, bool coarse, int max_group_rows) {
   const int D = C / H;
   // fp32 q|k|v of the fine (window) transformer; the coarse projections write planes
@@ -541,7 +551,7 @@ static void carve_tf(Bump& b, TfWs& w, int C, int H, long R, int n_groups, bool 
   w.kv_part = coarse ? b.take<float>(static_cast<size_t>(2) * n_groups * H * parts * (D * D + D)) : nullptr;
 }
 
-template <int BN>
+template <int BN, int kP>
 static int tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st, const TfWs& w,
                          long x_base, long x_rows, int x_group_rows, long s_base, long s_rows, int s_group_rows,
                          int n_groups_x, bool self_pass, bool write_f32, cudaStream_t stream, const int* live,
@@ -671,7 +681,7 @@ using namespace lb;
 // Projections carry no feature map and no row zeroing: masks act inside the attention (key weight 0, padded query 0).
 // Q goes to the att planes [R, C] (overwritten in place by the message), K|V to the MLP hidden planes [R, 2C], which
 // are dead at this point of the layer; full_attn_wgmma_kernel (full_attn.cuh) reads both through tensor maps.
-template <int BN>
+template <int BN, int kP>
 static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st,
                                     const TfWs& w, long x_base, long x_rows, int x_group_rows, long s_base,
                                     long s_rows, int s_group_rows, int n_groups_x, bool self_pass, cudaStream_t stream) {
@@ -685,7 +695,7 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
   const __half* wq_lo = static_cast<const __half*>(lw.wqkv_lo);
   const long wkv_off = static_cast<long>(C) * C;   // k_proj, v_proj rows of wqkv
   {
-    using Epi = EpiPlanes<BN>;
+    using Epi = Operands<EpiPlanes<BN>, kP>;
     Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, 0};
     Planes B{wq_hi, wq_lo, C, 0};
     typename Epi::Params ep{0, nullptr, 1, lw.s_qkv, {}};
@@ -693,7 +703,7 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
     LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, 1, static_cast<int>(x_rows), C, C, 0, ep, stream)));
   }
   {
-    using Epi = EpiPlanes<BN>;
+    using Epi = Operands<EpiPlanes<BN>, kP>;
     Planes A{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, 0};
     Planes B{wq_hi + wkv_off, wq_lo + wkv_off, C, 0};
     typename Epi::Params ep{0, nullptr, 1, lw.s_qkv, {}};
@@ -703,10 +713,15 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
   const long qbs = static_cast<long>(x_group_rows) * C, kvbs = static_cast<long>(s_group_rows) * ldc;
   CUtensorMap tq_hi, tq_lo, tkv_hi, tkv_lo;
   LB_TRY(make_map(&tq_hi, w.att_hi + x_base * C, C, x_group_rows, n_groups_x, C, qbs, kFaRows, kFaD));
-  LB_TRY(make_map(&tq_lo, w.att_lo + x_base * C, C, x_group_rows, n_groups_x, C, qbs, kFaRows, kFaD));
   LB_TRY(make_map(&tkv_hi, w.h_hi + s_base * ldc, 2 * C, s_group_rows, n_groups_s, ldc, kvbs, kFaKeys, kFaD));
-  LB_TRY(make_map(&tkv_lo, w.h_lo + s_base * ldc, 2 * C, s_group_rows, n_groups_s, ldc, kvbs, kFaKeys, kFaD));
-  LB_TRY(set_max_dynamic_smem<&full_attn_wgmma_kernel>(kFwSmem));
+  tq_lo = tq_hi;
+  tkv_lo = tkv_hi;
+  if (kP == 2) {
+    LB_TRY(make_map(&tq_lo, w.att_lo + x_base * C, C, x_group_rows, n_groups_x, C, qbs, kFaRows, kFaD));
+    LB_TRY(make_map(&tkv_lo, w.h_lo + s_base * ldc, 2 * C, s_group_rows, n_groups_s, ldc, kvbs, kFaKeys, kFaD));
+  }
+  constexpr auto kernel = kP == 2 ? &full_attn_wgmma_kernel : &full_attn_wgmma_fp16_kernel;
+  LB_TRY(set_max_dynamic_smem<kernel>(fw_smem_bytes(kP)));
   FullAttnWgParams wp;
   wp.Lx = x_group_rows;
   wp.Ls = s_group_rows;
@@ -721,7 +736,7 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
   const dim3 grid(cdiv(x_group_rows, kFaRows), H, n_groups_x);
   TimingRec rec{nullptr, nullptr, TAG_FULL_ATTN};
   LB_TRY(timing_begin(rec, stream));
-  full_attn_wgmma_kernel<<<grid, kFwThreads, kFwSmem, stream>>>(tq_hi, tq_lo, tkv_hi, tkv_lo, wp);
+  kernel<<<grid, kFwThreads, fw_smem_bytes(kP), stream>>>(tq_hi, tq_lo, tkv_hi, tkv_lo, wp);
   LB_LAUNCHED();
   LB_TRY(timing_end(rec, stream));
   return 0;
@@ -731,10 +746,11 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
 // writes K = elu(k)+1 and V as planes, kv_gemm_kernel reduces them to K^T V and Ksum on the tensor cores, and the q
 // projection applies the attention in its epilogue; q, k, v never reach HBM.
 //                                                   [transformer.py:47-50, linear_attention.py:31-46]
+template <int kP>
 static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st,
                                       const TfWs& w, long x_base, int x_group_rows, long s_base, int s_group_rows,
                                       int n_groups_x, int n_groups_s, cudaStream_t stream) {
-  if (!lw.wkv_hi || !lw.wkv_lo)
+  if (!lw.wkv_hi || (kP == 2 && !lw.wkv_lo))
     return fail("linear attention of the coarse transformer needs the fused k|v weight planes (wkv_hi / wkv_lo)");
   const int D = C / H;
   const int per = D * D + D;
@@ -747,7 +763,7 @@ static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, in
   __half* kvp_hi = w.h_hi + s_base * ldc;   // the MLP hidden planes [R, 2C] are free at this point of the layer
   __half* kvp_lo = w.h_lo + s_base * ldc;
   {
-    using Epi = EpiKvProj<256>;
+    using Epi = Operands<EpiKvProj<256>, kP>;
     Planes A{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, static_cast<long>(s_group_rows) * ldc};
     Planes B{lw.wkv_hi, lw.wkv_lo, C, 0};
     typename Epi::Params ep;
@@ -759,7 +775,9 @@ static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, in
   {
     CUtensorMap tm_hi, tm_lo;
     LB_TRY(make_map(&tm_hi, kvp_hi, 2 * C, s_group_rows, n_groups_s, ldc, static_cast<long>(s_group_rows) * ldc, 64, 64));
-    LB_TRY(make_map(&tm_lo, kvp_lo, 2 * C, s_group_rows, n_groups_s, ldc, static_cast<long>(s_group_rows) * ldc, 64, 64));
+    tm_lo = tm_hi;
+    if (kP == 2)
+      LB_TRY(make_map(&tm_lo, kvp_lo, 2 * C, s_group_rows, n_groups_s, ldc, static_cast<long>(s_group_rows) * ldc, 64, 64));
     const int kb_total = cdiv(s_group_rows, 64);
     const int m_tiles_s = cdiv(s_group_rows, kBlockM);
     const int parts_cap = m_tiles_s > kKvSplits ? m_tiles_s : kKvSplits;   // capacity of kv_part (see kKvSplits)
@@ -769,16 +787,17 @@ static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, in
     if (splits > parts_cap) splits = parts_cap;
     const int kb_per = cdiv(kb_total, splits);
     splits = cdiv(kb_total, kb_per);
-    LB_TRY(set_max_dynamic_smem<&kv_gemm_kernel>(kKvGemmSmem));
+    constexpr auto kernel = kP == 2 ? &kv_gemm_kernel : &kv_gemm_fp16_kernel;
+    LB_TRY(set_max_dynamic_smem<kernel>(kv_gemm_smem(kP)));
     KvGemmParams kp{w.kv_part, kb_total, kb_per, splits};
-    kv_gemm_kernel<<<dim3(splits, 2, n_groups_s), kKvGemmThreads, kKvGemmSmem, stream>>>(tm_hi, tm_lo, kp);
+    kernel<<<dim3(splits, 2, n_groups_s), kKvGemmThreads, kv_gemm_smem(kP), stream>>>(tm_hi, tm_lo, kp);
     LB_LAUNCHED();
     const long total = static_cast<long>(n_groups_s) * H * per;
     kv_tile_merge_kernel<<<cdiv(total, 256), 256, 0, stream>>>(w.kv_part, splits, H * per, w.kv, total);
     LB_LAUNCHED();
   }
   {
-    using Epi = EpiAttn<256, 32>;
+    using Epi = Operands<EpiAttn<256, 32>, kP>;
     Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, static_cast<long>(x_group_rows) * ldc};
     Planes B{lw.wqkv_hi, lw.wqkv_lo, C, 0};
     typename Epi::Params ep{mask ? mask + x_base : nullptr, lw.s_qkv, w.kv, 1e-6f, w.att_hi + x_base * C,
@@ -790,7 +809,7 @@ static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, in
 
 // Runs one encoder-layer call `x <- layer(x, source)` for the row range x (queries) / s (source).
 // self_pass: x range == source range (q, k, v in one projection launch).
-template <int BN>
+template <int BN, int kP>
 static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st,
                              const TfWs& w, long x_base, long x_rows, int x_group_rows, long s_base, long s_rows,
                              int s_group_rows, int n_groups_x, bool self_pass, bool write_f32, cudaStream_t stream,
@@ -815,11 +834,11 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
 
   // 1-3. attention message -> att planes [x rows, C]
   if (D == 32 && !full) {
-    LB_TRY(tf_linear_attention_coarse(lw, C, H, st, w, x_base, x_group_rows, s_base, s_group_rows, n_groups_x,
+    LB_TRY(tf_linear_attention_coarse<kP>(lw, C, H, st, w, x_base, x_group_rows, s_base, s_group_rows, n_groups_x,
                                       n_groups_s, stream));
   } else if (D == 32) {
-    LB_TRY(tf_full_attention_coarse<BN>(lw, C, H, st, w, x_base, x_rows, x_group_rows, s_base, s_rows, s_group_rows,
-                                        n_groups_x, self_pass, stream));
+    LB_TRY((tf_full_attention_coarse<BN, kP>(lw, C, H, st, w, x_base, x_rows, x_group_rows, s_base, s_rows, s_group_rows,
+                                        n_groups_x, self_pass, stream)));
   } else {
     // windows of the fine transformer (D = 16, H = 8): the window kernels give every query / source row one lane
     if (x_group_rows > 32 || s_group_rows > 32)
@@ -830,7 +849,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
     //                                                                 [transformer.py:47-49, linear_attention.py:31-39]
     const int elu_self = full ? 0 : 2 * C, elu_q = full ? 0 : C, elu_kv = full ? 0 : C;
     const uint8_t* pmask = full ? nullptr : mask;
-    using Epi = EpiActStore<BN>;
+    using Epi = Operands<EpiActStore<BN>, kP>;
     if (self_pass) {
       Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, xbs};
       Planes B{lw.wqkv_hi, lw.wqkv_lo, C, 0};
@@ -874,7 +893,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   }
   // 4. merge + norm1 -> cat[:, C:2C]                            [transformer.py:51-52]
   {
-    using Epi = EpiLayerNorm<BN>;
+    using Epi = Operands<EpiLayerNorm<BN>, kP>;
     Planes A{w.att_hi + x_base * C, w.att_lo + x_base * C, C, xbs_a};
     Planes B{lw.wm_hi, lw.wm_lo, C, 0};
     OutMaps om;
@@ -887,7 +906,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   }
   // 5. mlp[0] + ReLU on cat([x, message]) -> h planes           [transformer.py:55, mlp 22-26]
   {
-    using Epi = EpiPlanes<BN>;
+    using Epi = Operands<EpiPlanes<BN>, kP>;
     Planes A{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, xbs};
     Planes B{lw.w1_hi, lw.w1_lo, 2 * C, 0};
     typename Epi::Params ep{1, nullptr, 1, lw.s_1, {}};
@@ -898,7 +917,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   // The residual stream lives in the fp16 planes (x = hi + lo, exact to 2^-22 relative): no fp32 master copy is read
   // or written between layers.
   {
-    using Epi = EpiLayerNorm<BN>;
+    using Epi = Operands<EpiLayerNorm<BN>, kP>;
     Planes A{w.h_hi + x_base * ldc, w.h_lo + x_base * ldc, ldc, xbs};
     Planes B{lw.w2_hi, lw.w2_lo, 2 * C, 0};
     float* xf = write_f32 ? st.x_f32 + x_base * C : nullptr;
@@ -916,7 +935,7 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
 
 extern "C" {
 
-int lb_version(void) { return 108; }
+int lb_version(void) { return 109; }
 int lb_block_k(void) { return kBlockK; }
 int lb_conv_layout(int cin, int* cin_blocks, int* rem_channels) {
   if (!cin_blocks || !rem_channels || cin <= 0) return fail("lb_conv_layout: bad arguments");
@@ -1054,8 +1073,12 @@ size_t lb_transformer_workspace_bytes(int d_model, int nhead, int n_groups, int 
   return b.off + 256;
 }
 
-int lb_transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds, int n_layers, int d_model,
-                           int nhead, const LbTransformerState* st, void* ws, size_t ws_bytes, void* stream) {
+}  // extern "C"
+
+// kP: operand planes of every tensor-core product (Operands)
+template <int kP>
+static int transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds, int n_layers, int d_model,
+                               int nhead, const LbTransformerState* st, void* ws, size_t ws_bytes, void* stream) {
   int sms;
   if (st->n_groups <= 0) return 0;
   DeviceGuard dev_guard;
@@ -1083,10 +1106,10 @@ int lb_transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds
     const int kind = kinds[l];
     const bool full = kind == LB_LAYER_SELF_FULL || kind == LB_LAYER_CROSS_FULL;
     auto pass = [&](long xb, long xr, int xg, long sb, long sr, int sg, int ng, bool self_pass) -> int {
-      return coarse ? tf_layer_pass<256>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s, nullptr, 0,
-                                         full)
-                    : tf_layer_pass<128>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s, live,
-                                         st->n_groups, full);
+      return coarse ? tf_layer_pass<256, kP>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s, nullptr,
+                                             0, full)
+                    : tf_layer_pass<128, kP>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s, live,
+                                             st->n_groups, full);
     };
     if (kind == LB_LAYER_SELF || kind == LB_LAYER_SELF_FULL) {
       // feat0 = layer(feat0, feat0); feat1 = layer(feat1, feat1)  [transformer.py:93-94]; same weights,
@@ -1108,6 +1131,17 @@ int lb_transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds
   return 0;
 }
 
+extern "C" {
+
+int lb_transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds, int n_layers, int d_model,
+                           int nhead, const LbTransformerState* st, void* ws, size_t ws_bytes, void* stream) {
+  return transformer_forward<2>(layers, kinds, n_layers, d_model, nhead, st, ws, ws_bytes, stream);
+}
+
+int lb_transformer_forward_fp16(const LbEncoderLayerWeights* layers, const int* kinds, int n_layers, int d_model,
+                                int nhead, const LbTransformerState* st, void* ws, size_t ws_bytes, void* stream) {
+  return transformer_forward<1>(layers, kinds, n_layers, d_model, nhead, st, ws, ws_bytes, stream);
+}
 
 }  // extern "C"
 
@@ -1261,7 +1295,11 @@ size_t lb_coarse_match_workspace_bytes(int n_pairs, int L, int S) {
   return b.off + 256;
 }
 
-// max_per_pair: 0 = every match; otherwise each pair keeps its max_per_pair most confident matches (match_cap_kernel)
+}  // extern "C"
+
+// max_per_pair: 0 = every match; otherwise each pair keeps its max_per_pair most confident matches (match_cap_kernel).
+// kP: operand planes of the score products (Operands); every pass recomputes the same logits.
+template <int kP>
 static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, size_t ws_bytes, void* stream) {
   int sms;
   DeviceGuard dev_guard;
@@ -1321,8 +1359,8 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
       ct = w.col_t;
       rt = w.row_t;
     }
-    using Epi = EpiScoreLse<BN, true, true>;
-    Epi::Params ep{scale, ct, rt, w.row_part, w.col_part};
+    using Epi = Operands<EpiScoreLse<BN, true, true>, kP>;
+    typename Epi::Params ep{scale, ct, rt, w.row_part, w.col_part};
     LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, n, L, S, C, chunks, ep, st)));
     // row_t = -rowLSE, col_t = -colLSE (kNegBig on padded entries)              [coarse_matching.py:119]
     lse_merge_kernel<<<cdiv(nl, TB), TB, 0, st>>>(w.row_part, n_chunks, nl, 0.f, nullptr, nullptr, L, a->mask0, w.row_t);
@@ -1354,8 +1392,8 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
     for (int it = 0; it < a->skh_iters; ++it) {
       // u_i = log_mu_i - LSE_j(Z_ij + v_j), j over S real columns + the dustbin column   [superglue.py:146]
       {
-        using Epi = EpiScoreLse<BN, true, false>;
-        Epi::Params ep{scale, w.col_t, nullptr, w.row_part, w.col_part};
+        using Epi = Operands<EpiScoreLse<BN, true, false>, kP>;
+        typename Epi::Params ep{scale, w.col_t, nullptr, w.row_part, w.col_part};
         LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, n, L, S, C, chunks, ep, st)));
         lse_merge_kernel<<<cdiv(nl, TB), TB, 0, st>>>(w.row_part, n_chunks, nl, norm, a->bin_score, w.bin_v, L,
                                                       a->mask0, w.row_u);
@@ -1368,8 +1406,8 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
       LB_LAUNCHED();
       // v_j = log_nu_j - LSE_i(Z_ij + u_i), i over L real rows + the dustbin row            [superglue.py:147]
       {
-        using Epi = EpiScoreLse<BN, false, true>;
-        Epi::Params ep{scale, nullptr, w.row_t, w.row_part, w.col_part};
+        using Epi = Operands<EpiScoreLse<BN, false, true>, kP>;
+        typename Epi::Params ep{scale, nullptr, w.row_t, w.row_part, w.col_part};
         LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, n, L, S, C, chunks, ep, st)));
         lse_merge_kernel<<<cdiv(ns, TB), TB, 0, st>>>(w.col_part, m_tiles, ns, norm, a->bin_score, w.bin_u, S,
                                                       a->mask1, w.col_v);
@@ -1392,8 +1430,8 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
   const uint8_t* col_dead = nullptr;
   const int passes = (a->match_type == LB_MATCH_SINKHORN && a->skh_prefilter) ? 2 : 1;
   for (int pass = 0; pass < passes; ++pass) {
-    using Epi = EpiScoreArgmax<BN>;
-    Epi::Params ep{scale, alpha, w.col_t, w.row_t, w.row_apart, w.col_apart};
+    using Epi = Operands<EpiScoreArgmax<BN>, kP>;
+    typename Epi::Params ep{scale, alpha, w.col_t, w.row_t, w.row_apart, w.col_apart};
     LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_ARGMAX, A, B, n, L, S, C, chunks, ep, st)));
     argmax_merge_kernel<<<cdiv(nl, TB), TB, 0, st>>>(w.row_apart, n_chunks, nl, w.row_key, w.row_arg);
     LB_LAUNCHED();
@@ -1415,9 +1453,9 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
   }
 
   if (a->conf_matrix) {   // opt-in materialisation of data['conf_matrix']         [coarse_matching.py:145]
-    using Epi = EpiConfStore<BN>;
+    using Epi = Operands<EpiConfStore<BN>, kP>;
     // row_t / col_t hold -LSE (dual-softmax) or the Sinkhorn potentials, with padded / prefiltered entries disabled
-    Epi::Params ep{scale, alpha, conf_bias, w.row_t, w.col_t, a->conf_matrix};
+    typename Epi::Params ep{scale, alpha, conf_bias, w.row_t, w.col_t, a->conf_matrix};
     LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_ARGMAX, A, B, n, L, S, C, 0, ep, st)));
   }
 
@@ -1458,13 +1496,20 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
   return 0;
 }
 
+extern "C" {
+
 int lb_coarse_match(const LbCoarseMatchArgs* a, void* ws, size_t ws_bytes, void* stream) {
-  return coarse_match(a, 0, ws, ws_bytes, stream);
+  return coarse_match<2>(a, 0, ws, ws_bytes, stream);
 }
 
 int lb_coarse_match_capped(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, size_t ws_bytes, void* stream) {
   if (max_per_pair < 1) return fail("lb_coarse_match_capped: max_per_pair must be at least 1 (got %d)", max_per_pair);
-  return coarse_match(a, max_per_pair, ws, ws_bytes, stream);
+  return coarse_match<2>(a, max_per_pair, ws, ws_bytes, stream);
+}
+
+int lb_coarse_match_fp16(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, size_t ws_bytes, void* stream) {
+  if (max_per_pair < 0) return fail("lb_coarse_match_fp16: max_per_pair must be 0 (no cap) or at least 1 (got %d)", max_per_pair);
+  return coarse_match<1>(a, max_per_pair, ws, ws_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ fine level

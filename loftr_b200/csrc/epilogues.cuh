@@ -1340,4 +1340,15 @@ struct EpiScoreArgmax {
   }
 };
 
+// ------------------------------------------------------------------------------------------------
+// An epilogue of the transformers or the score matrix on a kernel with single fp16 operand planes (match_precision
+// "fp16", DESIGN.md §16): the kernel reads the hi planes of A and B only and issues one MMA per k-step.  These
+// epilogues do not depend on the operand planes -- they still store hi and lo planes and read residuals as hi + lo --
+// so one wrapper serves all of them and the split instantiations keep their names.
+template <class Epi>
+struct EpiF16Operands : Epi {
+  using Epi::Epi;
+  static constexpr int kOperandPlanes = 1;
+};
+
 }  // namespace lb

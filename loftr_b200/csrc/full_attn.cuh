@@ -18,6 +18,10 @@
 //
 // Q is read from the same planes the message is written to: every CTA reads only its own (rows, head) block, before it
 // writes that block.  Deterministic: no atomics, fixed reduction order.
+//
+// full_attn_wgmma_fp16_kernel (match_precision "fp16", DESIGN.md §16) is the same kernel on the hi planes only:
+// S = hi(Q) hi(K)^T, P rounded once to fp16, O += fp16(P) hi(V), one MMA each; Q and every ring stage are half as
+// large, with the same 3 stages.
 #pragma once
 #include <cuda_fp16.h>
 #include <cstdint>
@@ -34,8 +38,11 @@ constexpr int kFwStages = 3;
 constexpr int kFwThreads = 288;                       // warps 0-7 consumers, warp 8 producer
 constexpr int kFwQPlane = kFaRows * 64;               // 128 rows x 64 B
 constexpr int kFwKvPlane = kFaKeys * 64;              // 64 keys x 64 B
-constexpr int kFwStage = 4 * kFwKvPlane;              // K hi, K lo, V hi, V lo
-constexpr int kFwSmem = 2 * kFwQPlane + kFwStages * kFwStage + kFwStages * kFaKeys * 4 + 2 * kFwStages * 8 + 8 + 1024;
+// a stage holds K hi (K lo) V hi (V lo)
+__host__ __device__ constexpr int fw_stage_bytes(int planes) { return 2 * planes * kFwKvPlane; }
+__host__ __device__ constexpr int fw_smem_bytes(int planes) {
+  return planes * kFwQPlane + kFwStages * fw_stage_bytes(planes) + kFwStages * kFaKeys * 4 + 2 * kFwStages * 8 + 8 + 1024;
+}
 
 // D[64 x 32] += A[64 x 16] (registers, fp16x2) * B, B MN-major in shared memory (imm-trans-b = 1)
 __device__ __forceinline__ void wgmma_rs_n32_tb(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b) {
@@ -68,16 +75,18 @@ struct FullAttnWgParams {
   float scale_log2;
 };
 
-// tm_q_hi/lo: Q planes as [groups][Lx][C], box (32, 128); tm_kv_hi/lo: K|V planes as [groups][Ls][2C], box (32, 64)
-__global__ void __launch_bounds__(kFwThreads, 1)
-full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_constant__ CUtensorMap tm_q_lo,
-                       const __grid_constant__ CUtensorMap tm_kv_hi, const __grid_constant__ CUtensorMap tm_kv_lo,
-                       const FullAttnWgParams p) {
+// tm_q_hi/lo: Q planes as [groups][Lx][C], box (32, 128); tm_kv_hi/lo: K|V planes as [groups][Ls][2C], box (32, 64).
+// kPlanes = 1: the lo maps are not read (the message is still written as hi / lo planes).
+template <int kPlanes>
+__device__ __forceinline__ void full_attn_wgmma(const CUtensorMap& tm_q_hi, const CUtensorMap& tm_q_lo,
+                                                const CUtensorMap& tm_kv_hi, const CUtensorMap& tm_kv_lo,
+                                                const FullAttnWgParams& p) {
+  constexpr int kFwStage = fw_stage_bytes(kPlanes);
   pdl_trigger();
   extern __shared__ __align__(1024) uint8_t fw_smem[];
   uint8_t* smem = fw_smem + ((1024u - (smem_u32(fw_smem) & 1023u)) & 1023u);
-  uint8_t* s_q = smem;                                              // [hi | lo][128][64 B]
-  uint8_t* s_ring = smem + 2 * kFwQPlane;                           // [stage][K hi, K lo, V hi, V lo][64][64 B]
+  uint8_t* s_q = smem;                                              // [hi (| lo)][128][64 B]
+  uint8_t* s_ring = smem + kPlanes * kFwQPlane;                     // [stage][K hi, (K lo,) V hi, (V lo)][64][64 B]
   float* s_bias = reinterpret_cast<float*>(s_ring + kFwStages * kFwStage);   // [stage][64]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_bias + kFwStages * kFaKeys);
   uint64_t* empty_bar = full_bar + kFwStages;
@@ -107,9 +116,9 @@ full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid
   if (warp == 8) {
     // ---- producer: Q once, then the K / V ring; the key bias of a tile is written before its barrier arrives
     if (lane == 0) {
-      mbar_arrive_expect_tx(q_bar, 2 * kFwQPlane);
+      mbar_arrive_expect_tx(q_bar, kPlanes * kFwQPlane);
       tma_load_3d(s_q, &tm_q_hi, q_bar, head * kFaD, qt * kFaRows, grp);
-      tma_load_3d(s_q + kFwQPlane, &tm_q_lo, q_bar, head * kFaD, qt * kFaRows, grp);
+      if constexpr (kPlanes == 2) tma_load_3d(s_q + kFwQPlane, &tm_q_lo, q_bar, head * kFaD, qt * kFaRows, grp);
     }
     RingPos<kFwStages> pos;
     for (int kt = 0; kt < n_tiles; ++kt) {
@@ -127,9 +136,9 @@ full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid
         uint64_t* fb = &full_bar[pos.stage];
         mbar_arrive_expect_tx(fb, kFwStage);
         tma_load_3d(st, &tm_kv_hi, fb, head * kFaD, key0, grp);
-        tma_load_3d(st + kFwKvPlane, &tm_kv_lo, fb, head * kFaD, key0, grp);
-        tma_load_3d(st + 2 * kFwKvPlane, &tm_kv_hi, fb, p.v_col0 + head * kFaD, key0, grp);
-        tma_load_3d(st + 3 * kFwKvPlane, &tm_kv_lo, fb, p.v_col0 + head * kFaD, key0, grp);
+        if constexpr (kPlanes == 2) tma_load_3d(st + kFwKvPlane, &tm_kv_lo, fb, head * kFaD, key0, grp);
+        tma_load_3d(st + kPlanes * kFwKvPlane, &tm_kv_hi, fb, p.v_col0 + head * kFaD, key0, grp);
+        if constexpr (kPlanes == 2) tma_load_3d(st + 3 * kFwKvPlane, &tm_kv_lo, fb, p.v_col0 + head * kFaD, key0, grp);
       }
       __syncwarp();
       pos.advance();
@@ -160,7 +169,7 @@ full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid
       const uint64_t adv = static_cast<uint64_t>(kk * 2);   // 16 fp16 = 32 bytes along K inside the swizzle row
       const uint64_t ah = wgmma_desc_k_sw64(q_hi) + adv, al = wgmma_desc_k_sw64(q_lo) + adv;
       const uint64_t bh = wgmma_desc_k_sw64(st) + adv, bl = wgmma_desc_k_sw64(st + kFwKvPlane) + adv;
-      wgmma_split<64>(s, ah, al, bh, bl);
+      wgmma_split<64, kPlanes>(s, ah, al, bh, bl);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -220,11 +229,13 @@ full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
       const uint32_t off = static_cast<uint32_t>(kk * 16 * 64);
-      const uint64_t vh = wgmma_desc_mn_sw64(st + 2 * kFwKvPlane + off);
+      const uint64_t vh = wgmma_desc_mn_sw64(st + kPlanes * kFwKvPlane + off);
       const uint64_t vl = wgmma_desc_mn_sw64(st + 3 * kFwKvPlane + off);
       wgmma_rs_n32_tb(o, ph[kk], vh);
-      wgmma_rs_n32_tb(o, ph[kk], vl);
-      wgmma_rs_n32_tb(o, pl[kk], vh);
+      if constexpr (kPlanes == 2) {
+        wgmma_rs_n32_tb(o, ph[kk], vl);
+        wgmma_rs_n32_tb(o, pl[kk], vh);
+      }
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -254,6 +265,19 @@ full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid
       *reinterpret_cast<uint32_t*>(p.o_lo + off + n * 8) = lo;
     }
   }
+}
+
+__global__ void __launch_bounds__(kFwThreads, 1)
+full_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_constant__ CUtensorMap tm_q_lo,
+                       const __grid_constant__ CUtensorMap tm_kv_hi, const __grid_constant__ CUtensorMap tm_kv_lo,
+                       const FullAttnWgParams p) {
+  full_attn_wgmma<2>(tm_q_hi, tm_q_lo, tm_kv_hi, tm_kv_lo, p);
+}
+__global__ void __launch_bounds__(kFwThreads, 1)
+full_attn_wgmma_fp16_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_constant__ CUtensorMap tm_q_lo,
+                            const __grid_constant__ CUtensorMap tm_kv_hi, const __grid_constant__ CUtensorMap tm_kv_lo,
+                            const FullAttnWgParams p) {
+  full_attn_wgmma<1>(tm_q_hi, tm_q_lo, tm_kv_hi, tm_kv_lo, p);
 }
 
 }  // namespace lb

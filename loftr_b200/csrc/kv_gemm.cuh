@@ -11,7 +11,8 @@
 // One CTA per (k-split, head quartet, image), one consumer warpgroup and one TMA warp.  Only the four diagonal
 // 32 x 32 blocks of the quartet's 128 x 128 product are attention state, so the warpgroup computes two m64n64 blocks
 // (heads 0-1 x their v, heads 2-3 x their v) and stores them as one partial per (image, split, head).  Split
-// precision as everywhere: hi*hi + hi*lo + lo*hi into one fp32 register accumulator.
+// precision as everywhere: hi*hi + hi*lo + lo*hi into one fp32 register accumulator.  kv_gemm_fp16_kernel
+// (match_precision "fp16", DESIGN.md §16) loads the hi planes only, issues hi*hi and takes Ksum from hi.
 //
 // Ksum = K^T 1 (`K.sum(dim=1)`, linear_attention.py:44) rides along: N = 16 MMAs multiply the K planes with a block of
 // ones (1 KB of fp16 1.0 in shared memory -- with every element equal, any descriptor that stays inside the block is a
@@ -32,9 +33,12 @@ constexpr int kKvGemmThreads = 160;                 // warps 0-3 wgmma + epilogu
 constexpr int kKvGemmStages = 3;
 constexpr int kKvBlock = 64 * 128;                  // one TMA box: 64 k-rows x 128 bytes
 constexpr int kKvTile = 2 * kKvBlock;               // 128 d (or v) x 64 k-rows per plane: 16 KB
-constexpr int kKvStageBytes = 4 * kKvTile;          // A hi, A lo, B hi, B lo
 constexpr int kKvOnesBytes = 1024;
-constexpr int kKvGemmSmem = kKvGemmStages * kKvStageBytes + kKvOnesBytes + 256;
+// a stage holds A hi (A lo) B hi (B lo): 2 * kPlanes tiles
+__host__ __device__ constexpr int kv_stage_bytes(int planes) { return 2 * planes * kKvTile; }
+__host__ __device__ constexpr int kv_gemm_smem(int planes) {
+  return kKvGemmStages * kv_stage_bytes(planes) + kKvOnesBytes + 256;
+}
 
 // D[64 x 64] += A^T B with both operands MN-major (transposed) in shared memory
 __device__ __forceinline__ void wgmma_f16_n64_tt(float (&d)[32], uint64_t desc_a, uint64_t desc_b) {
@@ -75,9 +79,10 @@ __device__ __forceinline__ uint64_t wgmma_desc_ones(uint32_t smem_addr) {
 }
 
 // tm_hi / tm_lo: the K|V planes [images][rows][512] with box (64 columns, 64 rows, 1); columns as the projection emits
-// them: [K of heads 0-3 | V of heads 0-3 | K of heads 4-7 | V of heads 4-7]
-__global__ void __launch_bounds__(kKvGemmThreads, 1)
-kv_gemm_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, const KvGemmParams p) {
+// them: [K of heads 0-3 | V of heads 0-3 | K of heads 4-7 | V of heads 4-7].  kPlanes = 1: tm_lo is not read.
+template <int kPlanes>
+__device__ __forceinline__ void kv_gemm(const CUtensorMap& tm_hi, const CUtensorMap& tm_lo, const KvGemmParams& p) {
+  constexpr int kKvStageBytes = kv_stage_bytes(kPlanes);
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) asm volatile("trap;");
   uint8_t* s_ones = smem + kKvGemmStages * kKvStageBytes;
@@ -117,9 +122,9 @@ kv_gemm_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
         for (int b = 0; b < 2; ++b) {
           const int ck = quartet * 256 + b * 64, cv = quartet * 256 + 128 + b * 64;
           tma_load_3d(st + b * kKvBlock, &tm_hi, fb, ck, row0, image);
-          tma_load_3d(st + kKvTile + b * kKvBlock, &tm_lo, fb, ck, row0, image);
-          tma_load_3d(st + 2 * kKvTile + b * kKvBlock, &tm_hi, fb, cv, row0, image);
-          tma_load_3d(st + 3 * kKvTile + b * kKvBlock, &tm_lo, fb, cv, row0, image);
+          if constexpr (kPlanes == 2) tma_load_3d(st + kKvTile + b * kKvBlock, &tm_lo, fb, ck, row0, image);
+          tma_load_3d(st + kPlanes * kKvTile + b * kKvBlock, &tm_hi, fb, cv, row0, image);
+          if constexpr (kPlanes == 2) tma_load_3d(st + 3 * kKvTile + b * kKvBlock, &tm_lo, fb, cv, row0, image);
         }
         pos.advance();
       }
@@ -145,12 +150,14 @@ kv_gemm_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
         for (int mh = 0; mh < 2; ++mh) {
           const uint32_t blk = off + static_cast<uint32_t>(mh * kKvBlock);
           const uint64_t a_hi = wgmma_desc_mn_sw128(st + blk), a_lo = wgmma_desc_mn_sw128(st + kKvTile + blk);
-          const uint64_t b_hi = wgmma_desc_mn_sw128(st + 2 * kKvTile + blk), b_lo = wgmma_desc_mn_sw128(st + 3 * kKvTile + blk);
+          const uint64_t b_hi = wgmma_desc_mn_sw128(st + kPlanes * kKvTile + blk), b_lo = wgmma_desc_mn_sw128(st + 3 * kKvTile + blk);
           wgmma_f16_n64_tt(acc[mh], a_hi, b_hi);
-          wgmma_f16_n64_tt(acc[mh], a_hi, b_lo);
-          wgmma_f16_n64_tt(acc[mh], a_lo, b_hi);
+          if constexpr (kPlanes == 2) {
+            wgmma_f16_n64_tt(acc[mh], a_hi, b_lo);
+            wgmma_f16_n64_tt(acc[mh], a_lo, b_hi);
+          }
           wgmma_f16_n16_tn(ks[mh], a_hi, ones);
-          wgmma_f16_n16_tn(ks[mh], a_lo, ones);
+          if constexpr (kPlanes == 2) wgmma_f16_n16_tn(ks[mh], a_lo, ones);
         }
       }
       wgmma_commit();
@@ -185,6 +192,16 @@ kv_gemm_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(kKvGemmThreads, 1)
+kv_gemm_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo, const KvGemmParams p) {
+  kv_gemm<2>(tm_hi, tm_lo, p);
+}
+__global__ void __launch_bounds__(kKvGemmThreads, 1)
+kv_gemm_fp16_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
+                    const KvGemmParams p) {
+  kv_gemm<1>(tm_hi, tm_lo, p);
 }
 
 }  // namespace lb

@@ -7,7 +7,8 @@ C ABI of include/loftr_b200.h: the ResNet-FPN backbone as implicit-GEMM convolut
 (`backbone_impl="b200"`, the default for the shipped ResNetFPN_8_2 shape; `"torch"` keeps the PyTorch/cuDNN fp32
 forward, which is closer to fp64 -- DESIGN.md §10; `"b200_fp16"` is the opt-in single-pass fp16 variant, faster and
 less accurate -- DESIGN.md §15), then position encoding, coarse transformer, coarse
-matching, fine windows, fine transformer and fine matching.
+matching, fine windows, fine transformer and fine matching (`match_precision="fp16"`: the opt-in single-pass fp16
+products for the transformers and the coarse score matrix -- DESIGN.md §16).
 There is no fallback path: without the built library / an H100 the forward raises.
 
 Packed-weight caches.  The kernels read fp16 hi/lo planes packed lazily from the parameters.  The caches are
@@ -32,6 +33,17 @@ from .backbone import build_backbone
 _KIND = {("self", "linear"): _lib.LAYER_SELF, ("cross", "linear"): _lib.LAYER_CROSS,
          ("self", "full"): _lib.LAYER_SELF_FULL, ("cross", "full"): _lib.LAYER_CROSS_FULL}
 ATTENTIONS = ("linear", "full")   # reference config: coarse.attention / fine.attention, options ['linear', 'full']
+# operand precision of the transformers' and the coarse score matrix's tensor-core products: "split" (hi/lo planes,
+# three MMAs per product: the parity path) or "fp16" (the hi planes only, one MMA per product; DESIGN.md §16)
+MATCH_PRECISIONS = ("split", "fp16")
+
+
+def _check_match_precision(precision, who):
+    if isinstance(precision, str) and precision in MATCH_PRECISIONS:
+        if precision == "fp16":
+            _lib.require(_lib.MATCH_FP16_VERSION, f'{who}="fp16"')
+        return precision
+    raise ValueError(f"{who} must be one of {MATCH_PRECISIONS} (got {precision!r})")
 
 
 def _stream(ref=None):
@@ -306,10 +318,14 @@ class _TokenState:
 
 
 class LocalFeatureTransformer(_PackedCache, nn.Module):
-    """Interleaved self/cross encoder with linear or full (softmax) attention (reference transformer.py:61-101)."""
+    """Interleaved self/cross encoder with linear or full (softmax) attention (reference transformer.py:61-101).
 
-    def __init__(self, config):
+    precision (read-only after construction): "split" or "fp16" (`lb_transformer_forward_fp16`: every tensor-core
+    product reads the hi planes only; the same packed weights and token state, DESIGN.md §16)."""
+
+    def __init__(self, config, precision="split"):
         super().__init__()
+        self._precision = _check_match_precision(precision, "LocalFeatureTransformer: precision")
         self.config = config
         self.d_model = config["d_model"]
         self.nhead = config["nhead"]
@@ -319,6 +335,10 @@ class LocalFeatureTransformer(_PackedCache, nn.Module):
         for p in self.parameters():
             if p.dim() > 1:
                 nn.init.xavier_uniform_(p)
+
+    @property
+    def precision(self):
+        return self._precision
 
     # -- weight packing: fp16 hi/lo planes of the [out, in] matrices
     def _build(self):
@@ -362,8 +382,9 @@ class LocalFeatureTransformer(_PackedCache, nn.Module):
         arr, kinds, _ = self._pack()
         nbytes = lib.lb_transformer_workspace_bytes(self.d_model, self.nhead, n_groups, group_rows0, group_rows1)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=state.x.device)
-        _lib.check(lib.lb_transformer_forward(arr, kinds, len(self.layers), self.d_model, self.nhead, C.byref(st),
-                                              ws.data_ptr(), nbytes, _stream(state.x)))
+        fwd = lib.lb_transformer_forward_fp16 if self._precision == "fp16" else lib.lb_transformer_forward
+        _lib.check(fwd(arr, kinds, len(self.layers), self.d_model, self.nhead, C.byref(st), ws.data_ptr(), nbytes,
+                       _stream(state.x)))
 
     @torch.no_grad()
     def forward(self, feat0, feat1, mask0=None, mask1=None):
@@ -390,10 +411,14 @@ class CoarseMatching(nn.Module):
     config["max_matches_per_pair"] (optional, not a reference key): None or absent keeps every match; an int k >= 1
     keeps, within each pair, the k matches with the largest mconf (a tie at the k-th value goes to the smaller row
     index i), selected on the device before the fine stage.  The list stays in ascending (b, i) order.  The attribute
-    `max_matches_per_pair` may be changed later; it is validated the same way."""
+    `max_matches_per_pair` may be changed later; it is validated the same way.
 
-    def __init__(self, config):
+    precision (read-only after construction): "split" or "fp16" (`lb_coarse_match_fp16`: every pass computes the score
+    matrix from the hi planes of the features, one MMA per product; DESIGN.md §16)."""
+
+    def __init__(self, config, precision="split"):
         super().__init__()
+        self._precision = _check_match_precision(precision, "CoarseMatching: precision")
         self.config = config
         self.max_matches_per_pair = config.get("max_matches_per_pair")
         self.thr = config["thr"]
@@ -409,6 +434,10 @@ class CoarseMatching(nn.Module):
             self.skh_prefilter = config["skh_prefilter"]
         else:
             raise NotImplementedError()
+
+    @property
+    def precision(self):
+        return self._precision
 
     @property
     def max_matches_per_pair(self):
@@ -481,7 +510,10 @@ class CoarseMatching(nn.Module):
             a.conf_matrix = conf.data_ptr()
         nbytes = lib.lb_coarse_match_workspace_bytes(n, L, S)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        if k is None:
+        if self._precision == "fp16":   # 0: no cap
+            _lib.check(lib.lb_coarse_match_fp16(C.byref(a), 0 if k is None else min(k, L), ws.data_ptr(), nbytes,
+                                                _stream(hi)))
+        elif k is None:
             _lib.check(lib.lb_coarse_match(C.byref(a), ws.data_ptr(), nbytes, _stream(hi)))
         else:   # k >= L keeps every match; min() keeps the argument within a C int
             _lib.check(lib.lb_coarse_match_capped(C.byref(a), min(k, L), ws.data_ptr(), nbytes, _stream(hi)))
@@ -642,14 +674,19 @@ class FineMatching(nn.Module):
 class LoFTR(nn.Module):
     """Top-level matcher (reference loftr.py:12-81)."""
 
-    def __init__(self, config, backbone_impl="auto"):
+    def __init__(self, config, backbone_impl="auto", match_precision="split"):
         """backbone_impl: "torch" keeps the PyTorch/cuDNN ResNet-FPN forward (the north_star default scope);
         "b200" runs it as implicit-GEMM convolutions on the tensor cores (SURVEY.md §8(f) rank 1); "auto" picks
         "b200" whenever the configured backbone is the supported ResNetFPN_8_2 shape.  "b200_fp16" (opt-in, never
         picked by "auto") runs the same convolutions with single fp16 activations and one fp16 MMA per product: faster,
-        but it does not meet the reference-parity target (DESIGN.md §10, §15); the transformers and matching stay
-        split-precision.  All are GPU paths."""
+        but it does not meet the reference-parity target (DESIGN.md §10, §15).  All are GPU paths.
+
+        match_precision: "split" (the default) computes every tensor-core product of the coarse and fine transformers
+        and of the coarse score matrix from hi/lo planes; "fp16" (opt-in) from the hi planes only, one fp16 MMA per
+        product: faster, but it does not meet the reference-parity target either (DESIGN.md §16).  Independent of
+        backbone_impl, and fixed at construction (read-only attribute `match_precision`)."""
         super().__init__()
+        self._match_precision = _check_match_precision(match_precision, "LoFTR: match_precision")
         self.config = config
         # the kernels are built for the shipped shapes; anything else must fail here, not at the first forward
         cc, fc = config["coarse"], config["fine"]
@@ -680,11 +717,15 @@ class LoFTR(nn.Module):
             self._tc_backbone = TensorCoreBackbone(self.backbone, precision=precision)
         self.pos_encoding = PositionEncodingSine(config["coarse"]["d_model"],
                                                  temp_bug_fix=config["coarse"]["temp_bug_fix"])
-        self.loftr_coarse = LocalFeatureTransformer(config["coarse"])
-        self.coarse_matching = CoarseMatching(config["match_coarse"])
+        self.loftr_coarse = LocalFeatureTransformer(config["coarse"], precision=match_precision)
+        self.coarse_matching = CoarseMatching(config["match_coarse"], precision=match_precision)
         self.fine_preprocess = FinePreprocess(config)
-        self.loftr_fine = LocalFeatureTransformer(config["fine"])
+        self.loftr_fine = LocalFeatureTransformer(config["fine"], precision=match_precision)
         self.fine_matching = FineMatching()
+
+    @property
+    def match_precision(self):
+        return self._match_precision
 
     @torch.no_grad()
     def forward(self, data):

@@ -1,0 +1,187 @@
+"""CPU checks of the single-pass fp16 matching mode (`match_precision="fp16"`, DESIGN.md §16): the float64 emulation
+(tests/match_fp16_ref.py) against ref64 with rounding off and on hand cases with it on, and the Python API (constructor
+values, read-only attributes, the library version gate, the C entry points' argument check)."""
+import copy
+import ctypes as C
+
+import pytest
+import torch
+
+import loftr_b200
+import match_fp16_ref as M
+import ref64
+from loftr_b200 import _lib
+from loftr_b200.loftr import CoarseMatching, LocalFeatureTransformer
+
+F64 = torch.float64
+TINY = 2.0 ** -12    # below half an fp16 ulp of values in [1, 2): rounds away
+
+
+def _layers(d_model, attention, n_layers=2, seed=0):
+    torch.manual_seed(seed)
+    cfg = {"d_model": d_model, "nhead": 8, "layer_names": ["self", "cross"][:n_layers], "attention": attention}
+    return cfg, ref64.layer_weights(LocalFeatureTransformer(cfg))
+
+
+def _masks(n, L, S):
+    m0 = torch.ones(n, L, dtype=torch.bool)
+    m1 = torch.ones(n, S, dtype=torch.bool)
+    m0[0, L - 3:] = False
+    m1[-1, S - 5:] = False
+    return m0, m1
+
+
+# ------------------------------------------------------------------------------------------------ emulation = ref64
+@pytest.mark.parametrize("d_model,attention", [(256, "linear"), (256, "full"), (128, "linear"), (128, "full")])
+@pytest.mark.parametrize("masked", [False, True])
+def test_identity_rounding_is_ref64_transformer(d_model, attention, masked):
+    cfg, layers = _layers(d_model, attention)
+    n, L, S = 2, 25 if d_model == 128 else 37, 25 if d_model == 128 else 29
+    f0 = torch.randn(n, L, d_model, dtype=F64)
+    f1 = torch.randn(n, S, d_model, dtype=F64)
+    m0, m1 = _masks(n, L, S) if masked else (None, None)
+    got = M.transformer(f0, f1, layers, cfg["layer_names"], 8, m0, m1, attention, rounding=False)
+    ref = ref64.transformer(f0, f1, layers, cfg["layer_names"], 8, m0, m1, attention)
+    for g, r in zip(got, ref):
+        assert torch.allclose(g, r, rtol=0, atol=1e-12), (g - r).abs().max()
+
+
+@pytest.mark.parametrize("match_type", ["dual_softmax", "sinkhorn"])
+def test_identity_rounding_is_ref64_conf_matrix(match_type):
+    mc = dict(loftr_b200.get_cfg("indoor_ds")["match_coarse"], match_type=match_type, skh_iters=3, skh_prefilter=False)
+    f0, f1 = torch.randn(2, 30, 256, dtype=F64) * 4, torch.randn(2, 21, 256, dtype=F64) * 4
+    m0, m1 = _masks(2, 30, 21)
+    bs = torch.tensor(1.0, dtype=F64)
+    got = M.conf_matrix(f0, f1, mc, m0, m1, bs, rounding=False)
+    assert torch.equal(got, ref64.conf_matrix(f0, f1, mc, m0, m1, bs))
+    assert not torch.equal(M.conf_matrix(f0, f1, mc, m0, m1, bs), got)
+
+
+# ------------------------------------------------------------------------------------------------ hand cases
+def test_roundings_of_one_value():
+    x = torch.tensor([1.0 + TINY, 1.0 + 2.0 ** -10, 1.0 / 3.0], dtype=F64)
+    assert M.r16(x).tolist() == [1.0, 1.0 + 2.0 ** -10, float(torch.tensor(1.0 / 3.0).half())]
+    assert torch.equal(M.r16(x, rounding=False), x)
+    w = torch.tensor([1e-3 / 3.0], dtype=F64)    # e = 21: fp16(w * 2^21) keeps 11 bits of w whatever its magnitude
+    assert M.w16(w, 21).item() == float(torch.tensor(1e-3 / 3.0 * 2.0 ** 21).half()) * 2.0 ** -21
+    assert abs(M.w16(w, 21).item() / w.item() - 1) < 2.0 ** -11 and M.w16(w, 21).item() != w.item()
+
+
+def test_linear_attention_rounds_k_and_v():
+    # K = elu(k)+1 = 1 + TINY and V = 1 + TINY round to 1: the rounded message equals the one of K = V = 1
+    q = torch.randn(1, 5, 2, 4, dtype=F64)
+    k = torch.full((1, 7, 2, 4), TINY, dtype=F64)
+    v = torch.full((1, 7, 2, 4), 1.0 + TINY, dtype=F64)
+    exact1 = M.linear_attention(q, torch.zeros_like(k), torch.ones_like(v), rounding=False)
+    assert torch.allclose(M.linear_attention(q, k, v), exact1, rtol=1e-15, atol=0)
+    assert not torch.allclose(M.linear_attention(q, k, v, rounding=False), exact1, rtol=1e-6, atol=0)
+
+
+def test_full_attention_rounds_q_k_v_and_p():
+    q = torch.full((1, 3, 1, 32), 1.0 + TINY, dtype=F64)
+    k = torch.full((1, 4, 1, 32), 1.0 + TINY, dtype=F64)
+    v = torch.arange(4, dtype=F64).view(1, 4, 1, 1).expand(1, 4, 1, 32) * (1.0 + TINY)
+    one = M.full_attention(torch.ones_like(q), torch.ones_like(k), v.half().double(), rounding=False)
+    assert torch.allclose(M.full_attention(q, k, v), one, rtol=1e-15, atol=0)   # equal logits: mean of fp16(V)
+    # P = exp(S / sqrt(D) - rowmax) is rounded in P V, not in the row sum
+    a = 2.0 ** -4
+    qq = torch.zeros(1, 1, 1, 32, dtype=F64)
+    qq[..., 0] = 1.0
+    kk = torch.zeros(1, 2, 1, 32, dtype=F64)
+    kk[0, 1, 0, 0] = a
+    vv = torch.cat([torch.ones(1, 1, 1, 32), torch.full((1, 1, 1, 32), 2.0)], 1).double()
+    p0 = torch.exp(torch.tensor(-a / 32 ** 0.5, dtype=F64))
+    assert M.r16(p0) != p0
+    want = (M.r16(p0) * 1.0 + 2.0) / (p0 + 1.0)
+    assert torch.allclose(M.full_attention(qq, kk, vv), torch.full((1, 1, 1, 32), want.item(), dtype=F64), rtol=1e-15,
+                          atol=0)
+    assert not torch.allclose(M.full_attention(qq, kk, vv, rounding=False), torch.full((1, 1, 1, 32), want.item(),
+                                                                                       dtype=F64), rtol=1e-9, atol=0)
+
+
+def test_encoder_layer_rounds_activations_and_weights_but_not_the_residual():
+    cfg, layers = _layers(256, "linear", n_layers=1, seed=3)
+    w = layers[0]
+    x0 = (torch.randn(1, 9, 256, dtype=F64) + 3.0).half().double()        # fp16 values in about [1, 6]
+    x = x0 * (1.0 + TINY / 8)                                            # rounds back to x0 everywhere it is an operand
+    out0, out = M.encoder_layer(x0, x0, w, 8), M.encoder_layer(x, x, w, 8)
+    assert torch.allclose(out - x, out0 - x0, rtol=0, atol=1e-12)        # only the exact residual sees the change
+    exact = M.encoder_layer(x, x, w, 8, rounding=False) - M.encoder_layer(x0, x0, w, 8, rounding=False)
+    assert (exact - (x - x0)).abs().max() > 1e-7
+    # weights within a fraction of an fp16 ulp of their hi plane give the same layer
+    e = M.layer_exponents(w)
+    keys = {"q_proj.weight": "qkv", "k_proj.weight": "qkv", "v_proj.weight": "qkv", "merge.weight": "merge",
+            "mlp.0.weight": "mlp0", "mlp.2.weight": "mlp2"}
+    w_hi = dict(w, **{k: M.w16(w[k], e[g]) for k, g in keys.items()})
+    w_near = dict(w_hi, **{k: w_hi[k] * (1.0 + TINY / 4) for k in keys})
+    assert M.layer_exponents(w_near) == e
+    assert torch.equal(M.encoder_layer(x0, x0, w_near, 8), M.encoder_layer(x0, x0, w_hi, 8))
+    assert not torch.equal(M.encoder_layer(x0, x0, w_near, 8, rounding=False),
+                           M.encoder_layer(x0, x0, w_hi, 8, rounding=False))
+
+
+def test_score_matrix_rounds_both_features():
+    mc = loftr_b200.get_cfg("indoor_ds")["match_coarse"]
+    f0 = (torch.randn(1, 6, 256, dtype=F64) + 2).half().double()
+    f1 = (torch.randn(1, 5, 256, dtype=F64) + 2).half().double()
+    near = M.conf_matrix(f0 * (1 + TINY / 8), f1 * (1 - TINY / 8), mc)
+    assert torch.equal(near, M.conf_matrix(f0, f1, mc))
+    assert not torch.equal(M.conf_matrix(f0 * (1 + TINY / 8), f1, mc, rounding=False), M.conf_matrix(f0, f1, mc))
+
+
+# ------------------------------------------------------------------------------------------------ Python API
+def test_constructor_modes():
+    cfg = loftr_b200.get_cfg("indoor_ds")
+    assert loftr_b200.LoFTR(cfg).match_precision == "split"       # the default is unchanged
+    for backbone in ("b200", "b200_fp16"):
+        for prec in ("split", "fp16"):
+            m = loftr_b200.LoFTR(cfg, backbone_impl=backbone, match_precision=prec)
+            assert m.backbone_impl == backbone and m.match_precision == prec
+            assert m.loftr_coarse.precision == m.loftr_fine.precision == m.coarse_matching.precision == prec
+    m = loftr_b200.LoFTR(cfg, match_precision="fp16")
+    assert m.backbone_impl == "b200"                               # "auto" does not follow match_precision
+    assert set(m.state_dict()) == set(loftr_b200.LoFTR(cfg).state_dict())
+    for obj, attr in ((m, "match_precision"), (m.loftr_coarse, "precision"), (m.coarse_matching, "precision")):
+        with pytest.raises(AttributeError):
+            setattr(obj, attr, "split")
+    assert LocalFeatureTransformer(cfg["coarse"], precision="fp16").precision == "fp16"
+    assert CoarseMatching(cfg["match_coarse"], precision="fp16").precision == "fp16"
+
+
+@pytest.mark.parametrize("bad", ["FP16", "bf16", "fp32", "", None, 16, ["fp16"]])
+def test_bad_precisions_are_rejected(bad):
+    cfg = loftr_b200.get_cfg("indoor_ds")
+    with pytest.raises(ValueError, match="match_precision"):
+        loftr_b200.LoFTR(cfg, match_precision=bad)
+    with pytest.raises(ValueError, match="precision"):
+        LocalFeatureTransformer(cfg["coarse"], precision=bad)
+    with pytest.raises(ValueError, match="precision"):
+        CoarseMatching(cfg["match_coarse"], precision=bad)
+
+
+def test_fp16_matching_refuses_an_older_library(monkeypatch):
+    class OldLib:
+        def lb_version(self):
+            return 108
+
+    monkeypatch.setattr(_lib, "load", lambda: OldLib())
+    assert _lib.MATCH_FP16_VERSION == 109
+    cfg = loftr_b200.get_cfg("indoor_ds")
+    with pytest.raises(RuntimeError, match=r"match_precision.*version 109 or newer.*is version 108"):
+        loftr_b200.LoFTR(cfg, match_precision="fp16")
+    for make in (lambda: LocalFeatureTransformer(cfg["fine"], precision="fp16"),
+                 lambda: CoarseMatching(cfg["match_coarse"], precision="fp16")):
+        with pytest.raises(RuntimeError, match=r"version 109 or newer.*is version 108"):
+            make()
+    loftr_b200.LoFTR(copy.deepcopy(cfg), backbone_impl="b200_fp16")   # the split matching needs nothing new
+
+
+def test_fp16_entry_points_are_bound_and_check_k():
+    lib = _lib.load()
+    assert lib.lb_version() == _lib.MATCH_FP16_VERSION
+    for name in ("lb_transformer_forward_fp16", "lb_coarse_match_fp16"):
+        assert _lib.SIGNATURES[name][1] == getattr(lib, name).argtypes
+    a = _lib.LbCoarseMatchArgs()
+    for k in (-1, -7):
+        assert lib.lb_coarse_match_fp16(C.byref(a), k, None, 0, None) != 0
+        assert b"max_per_pair must be 0" in lib.lb_last_error()
