@@ -48,6 +48,7 @@ def test_backbone_halo_convs_match_fp64(shape):
     for got, ex, name in ((got_c, ex_c, "coarse"), (got_f, ex_f, "fine")):
         scale = ex.abs().max().item()
         err = (got.permute(0, 3, 1, 2).double() - ex).abs().max().item()
+        util.record(f"backbone_halo_{name}_{n}x{h}x{w}", {"err_over_scale": err / scale, "scale": scale})
         assert err <= 1e-4 * scale, f"{name}: {err:.3e} (scale {scale:.3e})"
 
 

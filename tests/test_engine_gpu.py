@@ -355,10 +355,13 @@ def test_tensor_core_backbone_matches_torch(shape):
         err_ours = (got.permute(0, 3, 1, 2).double() - ex).abs().max().item()
         err_torch = (ref.double() - ex).abs().max().item()
         util.record(f"backbone_{name}_{n}x{h}x{w}", {"err_ours_vs_fp64": err_ours, "err_torch_fp32_vs_fp64": err_torch,
-                                                      "scale": scale})
+                                                      "scale": scale, "err_over_scale": err_ours / scale})
         # The tensor-core path (fp16 hi/lo operand planes, three MMAs per product) is less accurate than cuDNN's
-        # fp32 FMA chain, and the error compounds over the ~20 convolutions.  It stays well inside what the matcher
-        # tolerances need (end-to-end mconf rel err < 1e-3, see parity_stats); bound it so regressions are caught.
+        # fp32 FMA chain, and the error compounds over the ~20 convolutions: 1-6e-5 of the scale on an H100 80GB HBM3
+        # (700 W), above the 1e-5 parity budget of DESIGN.md §2, because every 3x3 stage loses up to ~12x the fp32
+        # error to the tensor cores' truncating accumulation (tests/test_backbone_stages_gpu.py holds each stage to
+        # its own bound).  It stays well inside what the matcher tolerances need (end-to-end mconf rel err < 1e-3,
+        # see parity_stats); bound it so regressions are caught.
         assert err_ours <= 1e-4 * scale, f"{name}: {err_ours:.3e} (torch fp32: {err_torch:.3e}, scale {scale:.3e})"
 
 
