@@ -101,6 +101,47 @@ def linear_attention(q, k, v, q_mask=None, kv_mask=None, eps=1e-6):
     return np.ascontiguousarray(out.transpose(0, 2, 1, 3)).astype(F32)
 
 
+def full_attention(q, k, v, q_mask=None, kv_mask=None):
+    """FullAttention.forward (linear_attention.py:56-81), dropout off.  q [N,L,H,D], k/v [N,S,H,D] -> [N,L,H,D].
+    A = softmax(Q K^T / sqrt(D)) over s with -inf logits where !(q_mask[l] & kv_mask[s]); values are not masked.
+    Row-blocked so that L x S x H never exists at once.
+
+    Masked rows: the reference gives every logit of a padded query row -inf, so its softmax (and, through the values
+    of the next layer, every row after it) is NaN.  The engine and this oracle give such a row, and a row without any
+    valid key, a zero message instead; valid rows equal the reference wherever it is finite."""
+    n, L, H, D = q.shape
+    qh = np.ascontiguousarray(q.transpose(0, 2, 1, 3)).astype(F32)          # [N,H,L,D]
+    kh = np.ascontiguousarray(k.transpose(0, 2, 3, 1)).astype(F32)          # [N,H,D,S]
+    vh = np.ascontiguousarray(v.transpose(0, 2, 1, 3)).astype(F32)          # [N,H,S,D]
+    temp = F32(1.0 / D ** 0.5)                                              # :77
+    out = np.zeros((n, H, L, D), F32)
+    for b in range(n):
+        kbias = None
+        if kv_mask is not None:
+            kbias = np.where(np.asarray(kv_mask[b]).astype(bool), F32(0), F32(-np.inf)).astype(F32)
+
+        def body(lo, hi, b=b, kbias=kbias):
+            qk = qh[b, :, lo:hi] @ kh[b]                                     # einsum nlhd,nshd->nlsh  :70
+            if kbias is not None:
+                qk = qk + kbias[None, None, :]                               # masked_fill(-inf)  :72-73
+            z = temp * qk
+            m = z.max(axis=-1, keepdims=True)
+            m = np.where(np.isfinite(m), m, F32(0))
+            e = np.exp(z - m)
+            ssum = e.sum(axis=-1, keepdims=True)
+            a = np.where(ssum > 0, e / np.where(ssum > 0, ssum, F32(1)), F32(0))   # softmax(dim=2)  :78
+            o = a @ vh[b]                                                    # einsum nlsh,nshd->nlhd  :81
+            if q_mask is not None:
+                o = o * np.asarray(q_mask[b, lo:hi]).astype(F32)[None, :, None]
+            out[b, :, lo:hi] = o
+
+        _blocked(body, L, 256)
+    return np.ascontiguousarray(out.transpose(0, 2, 1, 3)).astype(F32)
+
+
+ATTENTION = {"linear": linear_attention, "full": full_attention}   # transformer.py:21
+
+
 def layer_norm(x, g, b, eps=1e-5):
     """nn.LayerNorm over the last axis (biased variance), float32."""
     out = np.empty(x.shape, F32)
@@ -117,15 +158,15 @@ def layer_norm(x, g, b, eps=1e-5):
     return out
 
 
-def encoder_layer(x, source, w, nhead, x_mask=None, source_mask=None):
-    """LoFTREncoderLayer.forward (transformer.py:35-58).  `w` maps the layer's state_dict suffixes
-    ('q_proj.weight', ..., 'norm2.bias') to arrays ([out, in] for Linear)."""
+def encoder_layer(x, source, w, nhead, x_mask=None, source_mask=None, attention="linear"):
+    """LoFTREncoderLayer.forward (transformer.py:35-58) with attention 'linear' or 'full'.  `w` maps the layer's
+    state_dict suffixes ('q_proj.weight', ..., 'norm2.bias') to arrays ([out, in] for Linear)."""
     bs, _, c = x.shape
     dim = c // nhead
     q = (x @ w["q_proj.weight"].T).reshape(bs, -1, nhead, dim)          # :47
     k = (source @ w["k_proj.weight"].T).reshape(bs, -1, nhead, dim)     # :48
     v = (source @ w["v_proj.weight"].T).reshape(bs, -1, nhead, dim)     # :49
-    msg = linear_attention(q, k, v, x_mask, source_mask)                # :50
+    msg = ATTENTION[attention](q, k, v, x_mask, source_mask)            # :50
     msg = msg.reshape(bs, -1, nhead * dim) @ w["merge.weight"].T        # :51
     msg = layer_norm(msg, w["norm1.weight"], w["norm1.bias"])           # :52
     h = np.concatenate([x, msg], axis=2) @ w["mlp.0.weight"].T          # :55
@@ -135,16 +176,17 @@ def encoder_layer(x, source, w, nhead, x_mask=None, source_mask=None):
     return (x + msg).astype(F32)                                        # :58
 
 
-def local_feature_transformer(feat0, feat1, layers, layer_names, nhead, mask0=None, mask1=None):
-    """LocalFeatureTransformer.forward (transformer.py:80-101): interleaved self / cross layers;
-    in a cross layer feat1 attends to the already updated feat0 (:96-97)."""
+def local_feature_transformer(feat0, feat1, layers, layer_names, nhead, mask0=None, mask1=None, attention="linear"):
+    """LocalFeatureTransformer.forward (transformer.py:80-101): interleaved self / cross layers, one attention kind
+    for every layer; in a cross layer feat1 attends to the already updated feat0 (:96-97)."""
+    a = attention
     for w, name in zip(layers, layer_names):
         if name == "self":
-            feat0 = encoder_layer(feat0, feat0, w, nhead, mask0, mask0)
-            feat1 = encoder_layer(feat1, feat1, w, nhead, mask1, mask1)
+            feat0 = encoder_layer(feat0, feat0, w, nhead, mask0, mask0, a)
+            feat1 = encoder_layer(feat1, feat1, w, nhead, mask1, mask1, a)
         elif name == "cross":
-            feat0 = encoder_layer(feat0, feat1, w, nhead, mask0, mask1)
-            feat1 = encoder_layer(feat1, feat0, w, nhead, mask1, mask0)
+            feat0 = encoder_layer(feat0, feat1, w, nhead, mask0, mask1, a)
+            feat1 = encoder_layer(feat1, feat0, w, nhead, mask1, mask0, a)
         else:
             raise KeyError(name)
     return feat0, feat1
@@ -383,7 +425,8 @@ def split_layers(state, prefix, n_layers):
 def hot_path(feat_c0, feat_c1, feat_f0, feat_f1, state, cfg, hw0_i, hw1_i, mask0=None, mask1=None, scale0=None,
              scale1=None):
     """Backbone outputs (NCHW) -> every key LoFTR.forward writes after the backbone.  `cfg` is the
-    reference's lower-case config dict; `state` the state_dict as numpy arrays."""
+    reference's lower-case config dict (cfg['coarse' | 'fine']['attention']: 'linear' when absent); `state` the
+    state_dict as numpy arrays."""
     n = feat_c0.shape[0]
     hw0_c, hw1_c = feat_c0.shape[2:], feat_c1.shape[2:]
     hw0_f, hw1_f = feat_f0.shape[2:], feat_f1.shape[2:]
@@ -394,7 +437,8 @@ def hot_path(feat_c0, feat_c1, feat_f0, feat_f1, state, cfg, hw0_i, hw1_i, mask0
     m0 = mask0.reshape(n, -1) if mask0 is not None else None
     m1 = mask1.reshape(n, -1) if mask1 is not None else None
     layers = split_layers(state, "loftr_coarse", len(cc["layer_names"]))
-    x0, x1 = local_feature_transformer(x0, x1, layers, cc["layer_names"], cc["nhead"], m0, m1)
+    x0, x1 = local_feature_transformer(x0, x1, layers, cc["layer_names"], cc["nhead"], m0, m1,
+                                       cc.get("attention", "linear"))
     mc = cfg["match_coarse"]
     bin_score = state.get("coarse_matching.bin_score")
     out = coarse_matching(x0, x1, mc, hw0_i, hw0_c, hw1_c, mask0, mask1, scale0, scale1, bin_score)
@@ -407,7 +451,8 @@ def hot_path(feat_c0, feat_c1, feat_f0, feat_f1, state, cfg, hw0_i, hw1_i, mask0
     if f0.shape[0] != 0:
         fc = cfg["fine"]
         flayers = split_layers(state, "loftr_fine", len(fc["layer_names"]))
-        f0, f1 = local_feature_transformer(f0, f1, flayers, fc["layer_names"], fc["nhead"])
+        f0, f1 = local_feature_transformer(f0, f1, flayers, fc["layer_names"], fc["nhead"],
+                                           attention=fc.get("attention", "linear"))
     out.update(fine_matching(f0, f1, out["mkpts0_c"], out["mkpts1_c"], out["b_ids"], hw0_i, hw0_f, scale1))
     out.update({"feat_c0": x0, "feat_c1": x1, "feat_f0_unfold": f0, "feat_f1_unfold": f1,
                 "hw0_c": tuple(hw0_c), "hw1_c": tuple(hw1_c), "hw0_f": tuple(hw0_f), "hw1_f": tuple(hw1_f)})

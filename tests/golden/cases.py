@@ -47,6 +47,8 @@ def build_cfg(case):
     cfg["match_coarse"]["skh_prefilter"] = case.get("prefilter", False)
     cfg["match_coarse"]["border_rm"] = case.get("border_rm", 2)
     cfg["coarse"]["temp_bug_fix"] = case.get("temp_bug_fix", True)
+    cfg["coarse"]["attention"] = case.get("coarse_attention", "linear")
+    cfg["fine"]["attention"] = case.get("fine_attention", "linear")
     return cfg
 
 

@@ -5,8 +5,6 @@ from __future__ import annotations
 
 import numpy as np
 
-from cases import build_cfg
-
 # 96 x 128 images: L = S = 192 coarse tokens, so the last 128-query tile of the coarse kernel is partial
 FULL_CASES = [
     {"name": "full_ds_thr0", "n": 2, "hw0": (96, 128), "hw1": (96, 128), "thr": 0.0, "images": "smooth",
@@ -21,7 +19,7 @@ FULL_CASES = [
      "coarse_attention": "full", "fine_attention": "full"},
 ]
 
-# Full-size parity cases of the GPU tests against the oracle (tests/full_oracle.oracle_forward_per_pair; precomputable
+# Full-size parity cases of the GPU tests against the oracle (tests/util.oracle_forward_per_pair; precomputable
 # on CPU with tools/precompute_oracle.py into the git-ignored tests/_oracle_cache/)
 FULL_BASELINE_CASES = {
     "full_b2_640x480": {"name": "full_b2_640x480", "n": 2, "hw0": (480, 640), "hw1": (480, 640), "thr": 0.0,
@@ -34,13 +32,6 @@ FULL_BASELINE_CASES = {
 # One reference FullAttention call with padding masks and finite inputs (valid rows pin the masked convention)
 FA_MODULE_CASE = {"name": "fa_masked_module", "n": 2, "L": 150, "S": 131, "H": 8, "D": 32,
                   "valid_l": [150, 97], "valid_s": [101, 131]}
-
-
-def build_full_cfg(case):
-    cfg = build_cfg(case)
-    cfg["coarse"]["attention"] = case.get("coarse_attention", "linear")
-    cfg["fine"]["attention"] = case.get("fine_attention", "linear")
-    return cfg
 
 
 def build_fa_module_inputs(case=FA_MODULE_CASE):

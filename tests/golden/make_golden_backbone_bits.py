@@ -13,7 +13,6 @@ import os
 import sys
 
 import numpy as np
-import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
@@ -37,15 +36,12 @@ def digest(t):
 
 def backbone_bits(shape, dev="cuda:0"):
     """-> (feat_c, feat_f) of lb_backbone_forward on the test weights and a seeded image batch of `shape`."""
+    import backbone_ref as B
     import util
     from cases import CASES
-    from test_conv_halo_gpu import _forward
     from loftr_b200.loftr import TensorCoreBackbone
-    n, h, w = shape
     model, _, _ = util.build_model(dict(CASES[0]), dev)
-    rs = np.random.RandomState(SEED)
-    img = torch.from_numpy(rs.uniform(0, 1, (n, 1, h, w)).astype(np.float32)).to(dev)
-    return _forward(TensorCoreBackbone(model.backbone), img, 0)
+    return B.backbone_forward(TensorCoreBackbone(model.backbone), B.image(shape, SEED, dev))[1:]
 
 
 def main():

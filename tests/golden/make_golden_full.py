@@ -17,7 +17,7 @@ sys.path.insert(0, HERE)
 
 from oracle import ref_import  # noqa: E402
 import make_golden  # noqa: E402
-from full_cases import FA_MODULE_CASE, FULL_CASES, build_fa_module_inputs, build_full_cfg  # noqa: E402
+from full_cases import FA_MODULE_CASE, FULL_CASES, build_fa_module_inputs  # noqa: E402
 
 
 def run_fa_module_case(case):
@@ -32,7 +32,6 @@ def run_fa_module_case(case):
 def main():
     ref = ref_import.load_reference()
     torch.set_num_threads(8)
-    make_golden.build_cfg = build_full_cfg   # run_case builds the model from the case's config
     for case in FULL_CASES:
         out = make_golden.run_case(ref, case)
         path = os.path.join(HERE, case["name"] + ".npz")

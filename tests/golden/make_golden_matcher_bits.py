@@ -68,12 +68,12 @@ def digest(t):
 
 
 def _model(case, conf):
-    """LoFTR with the RandomState weights of weights.py (as util.build_model), the attention kinds of full_cases and the
-    case's block_dims; conf: return_conf_matrix."""
+    """LoFTR with the RandomState weights of weights.py (as util.build_model), the case's attention kinds and
+    block_dims; conf: return_conf_matrix."""
     import loftr_b200
     import weights as W
-    from full_cases import build_full_cfg
-    cfg = build_full_cfg(case)
+    from cases import build_cfg
+    cfg = build_cfg(case)
     cfg["match_coarse"]["return_conf_matrix"] = conf
     cfg["resnetfpn"]["block_dims"] = list(case.get("block_dims", cfg["resnetfpn"]["block_dims"]))
     model = loftr_b200.LoFTR(cfg).eval()

@@ -7,7 +7,19 @@ the reference root).  Pinned against the reference's own float64 outputs by test
 Conventions that differ from the reference:
 - full attention gives a padded query row, and a row without any valid key, a zero message (the reference gives NaN;
   DESIGN.md §5).  Linear attention yields zero for both by construction.
-"""
+
+With `fp16=True` the transformer and score-matrix stages emulate the single-pass fp16 matching mode
+(`match_precision="fp16"`, lb_transformer_forward_fp16 / lb_coarse_match_fp16; DESIGN.md §16): every tensor-core
+product multiplies the hi planes of its operands and accumulates exactly.
+- an activation operand is fp16(x) (round to nearest even) of the value the split path stores as hi + lo;
+- a weight operand is fp16(w * 2^e) * 2^-e, with e = `weight_exponent` of the packed matrix (q|k|v share the exponent
+  of their concatenation, as in `LocalFeatureTransformer._build`);
+- coarse linear attention: K^T V and Ksum from fp16(K) and fp16(V), K = elu(k)+1 and V masked; Q stays exact;
+- coarse full attention: S = fp16(Q) fp16(K)^T, P = exp(S / sqrt(D) - rowmax) rounded once to fp16 in the product
+  with fp16(V), the row sum taken from the unrounded P;
+- the fine (window) attention stays exact: the window kernels run in fp32 on the fp32 projections;
+- score matrix: fp16(feat_c0) . fp16(feat_c1), shared by every pass.
+Epilogues, LayerNorm, residuals, masks and everything after the score matrix are exact."""
 from __future__ import annotations
 
 import math
@@ -25,9 +37,28 @@ def f64(x, device=None):
     return t.to(device=device if device is not None else t.device, dtype=F64)
 
 
+def r16(t, rounding=True):
+    """fp16 round to nearest even (the hi plane), back in t's dtype"""
+    return t.half().to(t.dtype) if rounding else t
+
+
+def w16(w, e, rounding=True):
+    """hi weight plane fp16(w * 2^e) as a value: fp16(w * 2^e) * 2^-e."""
+    return (w * 2.0 ** e).half().double() * 2.0 ** (-e) if rounding else w
+
+
+def layer_exponents(w):
+    """weight_exponent of each packed matrix of one layer (`w`: a layer_weights dict)."""
+    from loftr_b200.loftr import weight_exponent
+    qkv = torch.cat([w["q_proj.weight"], w["k_proj.weight"], w["v_proj.weight"]], 0).float()
+    return {"qkv": weight_exponent(qkv), "merge": weight_exponent(w["merge.weight"].float()),
+            "mlp0": weight_exponent(w["mlp.0.weight"].float()), "mlp2": weight_exponent(w["mlp.2.weight"].float())}
+
+
 # ------------------------------------------------------------------------------------------------ transformer
-def linear_attention(q, k, v, q_mask=None, kv_mask=None, eps=1e-6):
-    """LinearAttention.forward (linear_attention.py:20-47).  q [N,L,H,D], k / v [N,S,H,D]."""
+def linear_attention(q, k, v, q_mask=None, kv_mask=None, eps=1e-6, fp16=False):
+    """LinearAttention.forward (linear_attention.py:20-47).  q [N,L,H,D], k / v [N,S,H,D].  fp16: K and V rounded for
+    K^T V and Ksum (kv_gemm_fp16_kernel)."""
     Q = F.elu(q) + 1                                                    # :31-32
     K = F.elu(k) + 1
     if q_mask is not None:                                              # :35-39
@@ -35,6 +66,7 @@ def linear_attention(q, k, v, q_mask=None, kv_mask=None, eps=1e-6):
     if kv_mask is not None:
         K = K * kv_mask[:, :, None, None].to(F64)
         v = v * kv_mask[:, :, None, None].to(F64)
+    K, v = r16(K, fp16), r16(v, fp16)
     v_length = v.shape[1]
     v = v / v_length                                                    # :41-42
     KV = torch.einsum("nshd,nshv->nhdv", K, v)                          # :43
@@ -42,34 +74,44 @@ def linear_attention(q, k, v, q_mask=None, kv_mask=None, eps=1e-6):
     return torch.einsum("nlhd,nhdv,nlh->nlhv", Q, KV, Z) * v_length    # :45
 
 
-def full_attention(q, k, v, q_mask=None, kv_mask=None, block=1024):
-    """FullAttention.forward (linear_attention.py:56-81), query-blocked, with the zero-message convention."""
+def full_attention(q, k, v, q_mask=None, kv_mask=None, block=1024, fp16=False):
+    """FullAttention.forward (linear_attention.py:56-81), query-blocked, with the zero-message convention.  fp16: Q, K,
+    V rounded and P rounded once in P V, not in the row sum (full_attn_wgmma_fp16_kernel)."""
+    q, k, v = r16(q, fp16), r16(k, fp16), r16(v, fp16)
     n, L, H, D = q.shape
     out = torch.zeros(n, L, H, D, dtype=F64, device=q.device)
     for lo in range(0, L, block):
         hi = min(lo + block, L)
-        qk = torch.einsum("nlhd,nshd->nlsh", q[:, lo:hi], k)           # :69
+        s = torch.einsum("nlhd,nshd->nlsh", q[:, lo:hi], k) / math.sqrt(D)   # :69, :74
         if kv_mask is not None:                                         # :70-71
             ok = q_mask[:, lo:hi, None, None] & kv_mask[:, None, :, None]
-            qk = qk.masked_fill(~ok, float("-inf"))
-        a = torch.softmax(qk / math.sqrt(D), dim=2)                     # :74-75
-        a = torch.nan_to_num(a, nan=0.0)                                # rows without a valid logit: zero message
-        out[:, lo:hi] = torch.einsum("nlsh,nshd->nlhd", a, v)           # :79
+            s = s.masked_fill(~ok, float("-inf"))
+        m = s.amax(dim=2, keepdim=True)                                 # softmax over s  :74-75
+        p = torch.exp(s - torch.where(torch.isinf(m), torch.zeros_like(m), m))
+        den = p.sum(dim=2)[..., None]                                   # [n, l, h, 1]; 0: no valid key
+        num = torch.einsum("nlsh,nshd->nlhd", r16(p, fp16), v)         # :79
+        out[:, lo:hi] = torch.where(den > 0, num / den.clamp_min(1e-300), torch.zeros_like(num))
     return out
 
 
-def encoder_layer(x, source, w, nhead, x_mask=None, source_mask=None, attention="linear"):
-    """LoFTREncoderLayer.forward (transformer.py:35-58).  `w`: the layer's state_dict suffixes -> float64 tensors."""
+def encoder_layer(x, source, w, nhead, x_mask=None, source_mask=None, attention="linear", fp16=False):
+    """LoFTREncoderLayer.forward (transformer.py:35-58).  `w`: the layer's state_dict suffixes -> float64 tensors.
+    fp16: every projection, merge and MLP product on fp16 operands; the attention is rounded for the coarse
+    transformer (head dim 32) and exact for the fine (window) transformer."""
     bs, _, c = x.shape
     dim = c // nhead
-    q = (x @ w["q_proj.weight"].T).view(bs, -1, nhead, dim)             # :47
-    k = (source @ w["k_proj.weight"].T).view(bs, -1, nhead, dim)        # :48
-    v = (source @ w["v_proj.weight"].T).view(bs, -1, nhead, dim)        # :49
+    e = layer_exponents(w) if fp16 else {}
+    wt = lambda name, group: w16(w[name], e[group]) if fp16 else w[name]
+    xh, sh = r16(x, fp16), r16(source, fp16)
+    q = (xh @ wt("q_proj.weight", "qkv").T).view(bs, -1, nhead, dim)   # :47
+    k = (sh @ wt("k_proj.weight", "qkv").T).view(bs, -1, nhead, dim)   # :48
+    v = (sh @ wt("v_proj.weight", "qkv").T).view(bs, -1, nhead, dim)   # :49
     att = linear_attention if attention == "linear" else full_attention
-    msg = att(q, k, v, x_mask, source_mask)                             # :50
-    msg = msg.reshape(bs, -1, c) @ w["merge.weight"].T                  # :51
+    msg = att(q, k, v, x_mask, source_mask, fp16=fp16 and dim == 32)   # :50
+    msg = r16(msg.reshape(bs, -1, c), fp16) @ wt("merge.weight", "merge").T   # :51
     msg = F.layer_norm(msg, (c,), w["norm1.weight"], w["norm1.bias"])   # :52
-    msg = torch.relu(torch.cat([x, msg], 2) @ w["mlp.0.weight"].T) @ w["mlp.2.weight"].T   # :55
+    h = torch.relu(r16(torch.cat([x, msg], 2), fp16) @ wt("mlp.0.weight", "mlp0").T)   # :55
+    msg = r16(h, fp16) @ wt("mlp.2.weight", "mlp2").T
     msg = F.layer_norm(msg, (c,), w["norm2.weight"], w["norm2.bias"])   # :56
     return x + msg                                                      # :58
 
@@ -84,15 +126,16 @@ def layer_weights(tf_module, device=None):
     return out
 
 
-def transformer(feat0, feat1, layers, layer_names, nhead, mask0=None, mask1=None, attention="linear"):
+def transformer(feat0, feat1, layers, layer_names, nhead, mask0=None, mask1=None, attention="linear", fp16=False):
     """LocalFeatureTransformer.forward (transformer.py:80-101): feat1 attends to the updated feat0 (:96-97)."""
+    a = attention
     for w, name in zip(layers, layer_names):
         if name == "self":
-            feat0 = encoder_layer(feat0, feat0, w, nhead, mask0, mask0, attention)
-            feat1 = encoder_layer(feat1, feat1, w, nhead, mask1, mask1, attention)
+            feat0 = encoder_layer(feat0, feat0, w, nhead, mask0, mask0, a, fp16)
+            feat1 = encoder_layer(feat1, feat1, w, nhead, mask1, mask1, a, fp16)
         elif name == "cross":
-            feat0 = encoder_layer(feat0, feat1, w, nhead, mask0, mask1, attention)
-            feat1 = encoder_layer(feat1, feat0, w, nhead, mask1, mask0, attention)
+            feat0 = encoder_layer(feat0, feat1, w, nhead, mask0, mask1, a, fp16)
+            feat1 = encoder_layer(feat1, feat0, w, nhead, mask1, mask0, a, fp16)
         else:
             raise KeyError(name)
     return feat0, feat1
@@ -116,8 +159,10 @@ def log_optimal_transport(scores, alpha, iters):
     return couplings + u[:, :, None] + v[:, None, :] - norm                                    # :148,169
 
 
-def conf_matrix(feat_c0, feat_c1, mc, mask_c0=None, mask_c1=None, bin_score=None):
-    """CoarseMatching.forward up to conf_matrix (coarse_matching.py:103-143).  feat [N, L|S, C]; masks bool [N, L|S]."""
+def conf_matrix(feat_c0, feat_c1, mc, mask_c0=None, mask_c1=None, bin_score=None, fp16=False):
+    """CoarseMatching.forward up to conf_matrix (coarse_matching.py:103-143).  feat [N, L|S, C]; masks bool [N, L|S].
+    fp16: the product of the rounded features; the scale 1/sqrt(C) (and 1/T) applies to the exact product."""
+    feat_c0, feat_c1 = r16(feat_c0, fp16), r16(feat_c1, fp16)
     c = feat_c0.shape[-1]
     f0, f1 = feat_c0 / c ** 0.5, feat_c1 / c ** 0.5                                         # :106-107
     pad = None if mask_c0 is None else ~(mask_c0[..., None] & mask_c1[:, None])

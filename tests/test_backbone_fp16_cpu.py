@@ -8,8 +8,8 @@ import pytest
 import torch
 
 import loftr_b200
+import backbone_ref as B
 import util
-from backbone_fp16_ref import backbone_fp16_ref
 from cases import CASES
 from loftr_b200 import _lib
 from loftr_b200.loftr import TensorCoreBackbone, weight_exponent
@@ -26,7 +26,7 @@ def test_emulation_without_rounding_is_the_float64_module():
     img = torch.from_numpy(rs.uniform(0, 1, (2, 1, 32, 48)).astype(np.float32))
     with torch.no_grad():
         ex_c, ex_f = copy.deepcopy(m).double()(img.double())
-        got_c, got_f = backbone_fp16_ref(m, img, rounding=False)
+        got_c, got_f = B.forward_f64(m, img, fp16=False)
     for got, ex in ((got_c, ex_c), (got_f, ex_f)):
         assert got.shape == ex.shape
         assert (got - ex).abs().max().item() <= 1e-12 * ex.abs().max().item()
@@ -39,7 +39,7 @@ def test_emulation_rounds_like_fp16():
     img = torch.from_numpy(rs.uniform(0, 1, (1, 1, 32, 32)).astype(np.float32))
     with torch.no_grad():
         ex_c, ex_f = copy.deepcopy(m).double()(img.double())
-        got_c, got_f = backbone_fp16_ref(m, img)
+        got_c, got_f = B.forward_f64(m, img)
     for got, ex in ((got_c, ex_c), (got_f, ex_f)):
         rel = (got - ex).abs().max().item() / ex.abs().max().item()
         assert 1e-5 < rel < 3e-2, rel

@@ -1,26 +1,24 @@
 """The fp16 backbone (`backbone_impl="b200_fp16"`, lb_backbone_forward_fp16) on the GPU.
 
 Per output map, the error against the float64 module is held to twice the error of the float64 emulation of the same
-semantics (tests/backbone_fp16_ref.py) plus 1e-6 of the map's scale: the kernels' fp32 accumulation order is the
+semantics (tests/backbone_ref.py) plus 1e-6 of the map's scale: the kernels' fp32 accumulation order is the
 only difference from the emulation.  Bits do not depend on the workspace's padding, on repetition or on the batch, and
 the whole matcher runs unchanged on top of the new backbone."""
 import copy
-import ctypes as C
 
 import numpy as np
 import pytest
 import torch
 
+import backbone_ref as B
 import loftr_b200
 import util
-from backbone_fp16_ref import backbone_fp16_ref
 from cases import BASELINE_CASES, CASES, build_inputs
+from match_cap_ref import LIST_KEYS
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 _CASE = {c["name"]: c for c in CASES}
-_LIST_KEYS = ["b_ids", "i_ids", "j_ids", "m_bids", "gt_mask", "mconf", "mkpts0_c", "mkpts1_c", "mkpts0_f", "mkpts1_f",
-              "expec_f"]
 
 
 def _tc(model):
@@ -28,37 +26,14 @@ def _tc(model):
     return TensorCoreBackbone(model.backbone, precision="fp16")
 
 
-def _forward(tc, img, fill=0):
-    """lb_backbone_forward_fp16 with a workspace pre-filled with byte `fill` (0xFF: every fp16 is NaN)."""
-    from loftr_b200 import _lib
-    from loftr_b200.loftr import _stream
-    lib = _lib.load()
-    w, _ = tc._pack()
-    n, _, h, wd = img.shape
-    feat_c = torch.empty(n, h // 8, wd // 8, 256, dtype=torch.float32, device=DEV)
-    feat_f = torch.empty(n, h // 2, wd // 2, 128, dtype=torch.float32, device=DEV)
-    nbytes = lib.lb_backbone_workspace_bytes_fp16(C.byref(w), n, h, wd)
-    ws = torch.full((nbytes,), fill, dtype=torch.uint8, device=DEV)
-    _lib.check(lib.lb_backbone_forward_fp16(C.byref(w), img.data_ptr(), n, h, wd, feat_c.data_ptr(),
-                                            feat_f.data_ptr(), ws.data_ptr(), nbytes, _stream(img)))
-    torch.cuda.synchronize()
-    return feat_c, feat_f
-
-
-def _image(shape, seed):
-    n, h, w = shape
-    rs = np.random.RandomState(seed)
-    return torch.from_numpy(rs.uniform(0, 1, (n, 1, h, w)).astype(np.float32)).to(DEV)
-
-
 @pytest.mark.parametrize("shape", [(1, 16, 16), (16, 136, 200), (1, 88, 72), (1, 480, 640)])
 def test_fp16_backbone_error_is_that_of_its_semantics(shape):
     model, _, _ = util.build_model(dict(CASES[0]), DEV)
-    img = _image(shape, 21)
+    img = B.image(shape, 21)
     with torch.no_grad():
         ex = copy.deepcopy(model.backbone).double()(img.double())
-        emu = backbone_fp16_ref(model.backbone, img)
-    got = _forward(_tc(model), img)
+        emu = B.forward_f64(model.backbone, img)
+    got = B.backbone_forward(_tc(model), img)[1:]
     stats = {}
     for g, e, x, name in zip(got, emu, ex, ("coarse", "fine")):
         g = g.permute(0, 3, 1, 2).double()
@@ -97,43 +72,28 @@ def test_fp16_backbone_ignores_channel_padding_and_repeats_bitwise():
     the bits of a zeroed one, and a repeated run gives the same bits."""
     model, _, _ = util.build_model(dict(CASES[0]), DEV)
     tc = _tc(model)
-    img = _image((2, 96, 136), 12)
-    zc, zf = _forward(tc, img, 0)
-    nc, nf = _forward(tc, img, 0xFF)
+    img = B.image((2, 96, 136), 12)
+    _, zc, zf = B.backbone_forward(tc, img, 0)
+    _, nc, nf = B.backbone_forward(tc, img, 0xFF)
     assert torch.isfinite(nc).all() and torch.isfinite(nf).all()
     assert torch.equal(zc, nc) and torch.equal(zf, nf)
-    rc, rf = _forward(tc, img, 0)
+    _, rc, rf = B.backbone_forward(tc, img, 0)
     assert torch.equal(zc, rc) and torch.equal(zf, rf)
 
 
 def test_fp16_backbone_image_alone_equals_image_in_batch():
     model, _, _ = util.build_model(dict(CASES[0]), DEV)
     tc = _tc(model)
-    batch = _image((16, 136, 200), 13)
-    bc, bf = _forward(tc, batch)
+    batch = B.image((16, 136, 200), 13)
+    _, bc, bf = B.backbone_forward(tc, batch)
     for i in (0, 7, 15):
-        c, f = _forward(tc, batch[i:i + 1].contiguous())
+        _, c, f = B.backbone_forward(tc, batch[i:i + 1].contiguous())
         assert torch.equal(c[0], bc[i]) and torch.equal(f[0], bf[i]), i
 
 
 # ---------------------------------------------------------------------------------------------- end to end
 def _model(case, backbone_impl="b200_fp16"):
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
-    model, cfg, _ = util.build_model(case, "cpu")
-    m2 = loftr_b200.LoFTR(cfg, backbone_impl=backbone_impl).eval()
-    m2.load_state_dict(model.state_dict())
-    return m2.to(DEV)
-
-
-def _inputs(case):
-    return {k: torch.from_numpy(np.ascontiguousarray(v)).to(DEV) for k, v in build_inputs(case).items()}
-
-
-def _eager(model, inp):
-    data = dict(inp)
-    model(data)
-    return data
+    return util.build_model(case, DEV, backbone_impl)[0]
 
 
 @pytest.mark.parametrize("name", ["ds_thr0", "ds_masked_scaled", "ds_unequal", "ds_empty", "ot_thr0"])
@@ -141,10 +101,10 @@ def test_fp16_matcher_runs_every_path(name):
     """matcher(batch), forward_static and CapturedMatcher with the fp16 backbone: the split mode's keys, dtypes and
     (b, i) order; the static and captured outputs equal the eager forward bit for bit."""
     case = _CASE[name]
-    inp = _inputs(case)
+    inp = util.device_inputs(case)
     model = _model(case)
-    got = _eager(model, inp)
-    ref = _eager(_model(case, "b200"), inp)
+    got = util.eager(model, inp)
+    ref = util.eager(_model(case, "b200"), inp)
     assert list(got) == list(ref)
     for k, v in ref.items():
         if torch.is_tensor(v):
@@ -157,7 +117,7 @@ def test_fp16_matcher_runs_every_path(name):
     st = dict(inp)
     model.forward_static(st)
     assert int(st["num_matches"].item()) == m
-    for k in _LIST_KEYS:
+    for k in LIST_KEYS:
         assert torch.equal(st[k][:m], got[k]), f"forward_static {k}"
     masked = "mask0" in inp
     cm = loftr_b200.CapturedMatcher(model, case["n"], case["hw0"], case["hw1"], masks=masked, scales="scale0" in inp)
@@ -198,9 +158,9 @@ def test_fp16_agreement_with_split_backbone_at_8x640x480():
     """Recorded, not gated: with random weights the coarse logits reach 70-105 (SURVEY.md hard part 1), which
     exaggerates the effect of fp16 features on the match list.  No trained checkpoint is available here."""
     case = BASELINE_CASES["b8"]
-    inp = _inputs(case)
-    got = _eager(_model(case), inp)
-    ref = _eager(_model(case, "b200"), inp)
+    inp = util.device_inputs(case)
+    got = util.eager(_model(case), inp)
+    ref = util.eager(_model(case, "b200"), inp)
     kg = {k: n for n, k in enumerate(zip(*(got[x].tolist() for x in ("b_ids", "i_ids", "j_ids"))))}
     kr = {k: n for n, k in enumerate(zip(*(ref[x].tolist() for x in ("b_ids", "i_ids", "j_ids"))))}
     common = sorted(set(kg) & set(kr))

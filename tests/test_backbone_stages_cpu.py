@@ -1,5 +1,5 @@
 """CPU side of tests/test_backbone_stages_gpu.py: the workspace mirror against the library's workspace size, and the
-stage rules against the float64 emulation of the split path (tests/backbone_stage_ref.py) with and without defects.
+stage rules against the float64 emulation of the split path (tests/backbone_ref.py) with and without defects.
 
 The split rule must pass the clean emulation and fail each defect -- hi*lo or lo*hi product dropped, lo plane of the
 output not stored, the remainder channels of a 196-channel input multiplied hi*hi only -- by at least 10x, judged
@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 import torch
 
-import backbone_stage_ref as S
+import backbone_ref as S
 from loftr_b200 import _lib
 from loftr_b200.loftr import TensorCoreBackbone
 
@@ -24,7 +24,7 @@ DEFECT_STAGES = ["l2.2", "l2.3", "l3.down", "l2_out", "l1_out2.0"]
 
 @pytest.mark.parametrize("d2,d3", S.GRID_WIDTHS)
 def test_workspace_mirror_matches_the_library(d2, d3):
-    """carve_bb's layout as tests/backbone_stage_ref.py mirrors it sums to the library's workspace size - 256"""
+    """carve_bb's layout as tests/backbone_ref.py mirrors it sums to the library's workspace size - 256"""
     m = S.make_backbone(d2, d3, "cpu")
     w, _ = TensorCoreBackbone(m, precision="fp16")._build()   # the workspace size reads only the layer widths
     lib = _lib.load()
@@ -45,14 +45,10 @@ def _emulated(precision):
         if precision == "split":
             y = S.split_stage(m, steps, bufs.__getitem__)
         else:
-            y = S.run_stage(m, steps, bufs.__getitem__, torch.float64, "fp16", store=_r16)
-            y = y if steps[-1][6] == "feat_f" else _r16(y)
+            y = S.run_stage(m, steps, bufs.__getitem__, torch.float64, "fp16", store=S.r16)
+            y = y if steps[-1][6] == "feat_f" else S.r16(y)
         bufs[steps[-1][6]] = y
     return m, bufs
-
-
-def _r16(t):
-    return t.half().to(t.dtype)
 
 
 @pytest.mark.parametrize("stage", DEFECT_STAGES)
@@ -80,13 +76,13 @@ def test_fp16_rule_needs_its_accumulation_term():
         for name, _, steps in S.STAGES:
             if steps[-1][6] == "feat_f":
                 continue
-            ref = S.run_stage(m, steps, bufs.__getitem__, torch.float64, "fp16", store=_r16)
-            oracle = S.run_stage(m, steps, bufs.__getitem__, torch.float32, "fp16", store=_r16)
-            ok, stats = S.fp16_rule(_r16(oracle).double(), ref, oracle)
+            ref = S.run_stage(m, steps, bufs.__getitem__, torch.float64, "fp16", store=S.r16)
+            oracle = S.run_stage(m, steps, bufs.__getitem__, torch.float32, "fp16", store=S.r16)
+            ok, stats = S.fp16_rule(S.r16(oracle).double(), ref, oracle)
             assert ok, (name, stats)
             worst_ulps = max(worst_ulps, stats["max_ulps"])
             # an fp16 store that truncates instead of rounding to nearest differs at far more than 1 % of the values
-            r16 = _r16(ref)
+            r16 = S.r16(ref)
             trunc = torch.where(r16.abs() > ref.abs(), r16 - torch.sign(r16) * S.fp16_ulp(r16), r16)
             assert not S.fp16_rule(trunc, ref, oracle)[0], name
     assert worst_ulps > 1

@@ -1,7 +1,7 @@
 """Every stage of the tensor-core backbone against float64, from the kernels' own stored inputs.
 
 One forward of lb_backbone_forward (split) or lb_backbone_forward_fp16 runs into a workspace the test allocates; the
-mirror of `carve_bb` in tests/backbone_stage_ref.py then reads every activation back, and each stage (one convolution,
+mirror of `carve_bb` in tests/backbone_ref.py then reads every activation back, and each stage (one convolution,
 or two where the first one's output is overwritten later: t1, t2, t3) is recomputed from the inputs the kernels stored,
 residual and upsample addends included.  So a stage's error is its own, and a failure names its layer and kernel
 class: the stem (conv_stem7x7_tc), the halo convolution (conv3x3_halo_kernel: every stride-1 3x3), the implicit GEMM
@@ -21,19 +21,16 @@ Rules (DESIGN.md §2, §15):
   emulation of the kernel.
 - fp16 path, the fp32 maps feat_c and feat_f: the split rule, with the fp16 operands as the exact operands.
 - fp16 path, a chain of two convolutions: the split rule with 2^-11 (one fp16 rounding) as the storage term.
-The 3x3 stages are a listed finding (FINDING_STAGES in tests/backbone_stage_ref.py): 16x the oracle's error instead of 4x.
+The 3x3 stages are a listed finding (FINDING_STAGES in tests/backbone_ref.py): 16x the oracle's error instead of 4x.
 
 The grid covers a 1 x 1 map at 1/8 (upsampled from one pixel), partial 8 x 16 tiles at every level with three images
 (a halo leaking across images shows at their borders), one-row and one-column images, multi-tile CTA sequences and the
 benchmark size, at the shipped widths and at three of test_backbone_widths_gpu.WIDTHS (channel remainders,
 zero-padded last channel blocks, Cout on both sides of 128 and 200).  Every stage's ratio to its bound is recorded."""
-import ctypes as C
-
-import numpy as np
 import pytest
 import torch
 
-import backbone_stage_ref as S
+import backbone_ref as S
 import util
 
 pytestmark = pytest.mark.gpu
@@ -42,29 +39,6 @@ DEV = "cuda:0"
 SHAPES = S.GRID_SHAPES
 # (d2, d3): the shipped ResNetFPN_8_2 widths (d1 = 128 always) and three of test_backbone_widths_gpu.WIDTHS
 WIDTHS = S.GRID_WIDTHS
-
-
-def _forward(tc, img):
-    """TensorCoreBackbone.__call__ into a workspace of our own -> (workspace bytes, feat_c, feat_f) NCHW"""
-    from loftr_b200 import _lib
-    from loftr_b200.loftr import _stream
-    lib = _lib.load()
-    w, _ = tc._pack()
-    n, _, h, wd = img.shape
-    fp16 = tc.precision == "fp16"
-    workspace_bytes = lib.lb_backbone_workspace_bytes_fp16 if fp16 else lib.lb_backbone_workspace_bytes
-    forward = lib.lb_backbone_forward_fp16 if fp16 else lib.lb_backbone_forward
-    feat_c = torch.empty(n, h // 8, wd // 8, tc.m.layer3_outconv.out_channels, dtype=torch.float32, device=DEV)
-    feat_f = torch.empty(n, h // 2, wd // 2, 128, dtype=torch.float32, device=DEV)
-    ws = torch.zeros(workspace_bytes(C.byref(w), n, h, wd), dtype=torch.uint8, device=DEV)
-    _lib.check(forward(C.byref(w), img.data_ptr(), n, h, wd, feat_c.data_ptr(), feat_f.data_ptr(), ws.data_ptr(),
-                       ws.numel(), _stream(img)))
-    torch.cuda.synchronize()
-    return ws, feat_c.permute(0, 3, 1, 2).double(), feat_f.permute(0, 3, 1, 2).double()
-
-
-def _r16(t):
-    return t.half().to(t.dtype)
 
 
 @pytest.mark.parametrize("precision", ["split", "fp16"])
@@ -76,13 +50,13 @@ def test_backbone_stages_match_fp64(shape, d2, d3, precision):
     torch.backends.cuda.matmul.allow_tf32 = False
     n, h, w = shape
     m = S.make_backbone(d2, d3, DEV)
-    rs = np.random.RandomState(d2 + d3 + h + w)
-    img = torch.from_numpy(rs.uniform(0, 1, (n, 1, h, w)).astype(np.float32)).to(DEV)
+    img = S.image(shape, d2 + d3 + h + w)
     fp16 = precision == "fp16"
-    ws, feat_c, feat_f = _forward(TensorCoreBackbone(m, precision=precision), img)
+    ws, feat_c, feat_f = S.backbone_forward(TensorCoreBackbone(m, precision=precision), img)
     layout, total = S.workspace_layout(n, h, w, (128, d2, d3), 1 if fp16 else 2)
-    assert total + 256 == ws.numel(), "tests/backbone_stage_ref.py no longer mirrors carve_bb"
-    stored = {"image": img.double(), "feat_c": feat_c, "feat_f": feat_f}
+    assert total + 256 == ws.numel(), "tests/backbone_ref.py no longer mirrors carve_bb"
+    stored = {"image": img.double(), "feat_c": feat_c.permute(0, 3, 1, 2).double(),
+              "feat_f": feat_f.permute(0, 3, 1, 2).double()}
 
     def get(name):
         if name not in stored:
@@ -94,8 +68,8 @@ def test_backbone_stages_match_fp64(shape, d2, d3, precision):
     tag = "backbone_stage_%s_%dx%d_%dx%dx%d" % (precision, d2, d3, n, h, w)
     with torch.no_grad():
         for name, cls, steps in S.STAGES:
-            ref = S.run_stage(m, steps, get, torch.float64, weights, store=_r16 if fp16 else None)
-            oracle = S.run_stage(m, steps, get, torch.float32, weights, store=_r16 if fp16 else None)
+            ref = S.run_stage(m, steps, get, torch.float64, weights, store=S.r16 if fp16 else None)
+            oracle = S.run_stage(m, steps, get, torch.float32, weights, store=S.r16 if fp16 else None)
             out = steps[-1][6]
             checks = [(out, get(out))] if out != "feat_f" else []
             if out in S.FP32_OUTPUTS:

@@ -11,16 +11,13 @@ tests/test_pipeline_coverage_cpu.py checks that these categories stay covered.
 Bounds: the split path is held to 1e-4 of each output map's scale (test_backbone_halo_convs_match_fp64), the fp16 path
 to twice the error of its float64 emulation plus 1e-6 of the scale (test_fp16_backbone_error_is_that_of_its_semantics)."""
 import copy
-import ctypes as C
 
-import numpy as np
 import pytest
 import torch
 
+import backbone_ref as B
 import loftr_b200
 import util
-import weights as W
-from backbone_fp16_ref import backbone_fp16_ref
 
 DEV = "cuda:0"
 gpu = pytest.mark.gpu
@@ -35,52 +32,18 @@ SHAPES = [(1, 16, 16), (2, 88, 72)]
 PADDED = [(81, 208), (193, 80), (209, 64)]
 
 
-def _backbone(d2, d3, device=DEV):
-    from loftr_b200.backbone import ResNetFPN
-    m = ResNetFPN(128, [128, d2, d3]).eval()
-    shapes = {k: tuple(v.shape) for k, v in m.state_dict().items()}
-    m.load_state_dict({k: torch.from_numpy(v) for k, v in W.make_state(shapes, seed=d2 * 1000 + d3).items()})
-    return m.to(device)
-
-
-def _image(shape, seed):
-    n, h, w = shape
-    rs = np.random.RandomState(seed)
-    return torch.from_numpy(rs.uniform(0, 1, (n, 1, h, w)).astype(np.float32)).to(DEV)
-
-
-def _forward(tc, img, fill=0):
-    """TensorCoreBackbone.__call__ with a workspace pre-filled with byte `fill` (0xFF: every fp16 is NaN)."""
-    from loftr_b200 import _lib
-    from loftr_b200.loftr import _stream
-    lib = _lib.load()
-    w, _ = tc._pack()
-    n, _, h, wd = img.shape
-    fp16 = tc.precision == "fp16"
-    workspace_bytes = lib.lb_backbone_workspace_bytes_fp16 if fp16 else lib.lb_backbone_workspace_bytes
-    forward = lib.lb_backbone_forward_fp16 if fp16 else lib.lb_backbone_forward
-    feat_c = torch.empty(n, h // 8, wd // 8, tc.m.layer3_outconv.out_channels, dtype=torch.float32, device=DEV)
-    feat_f = torch.empty(n, h // 2, wd // 2, 128, dtype=torch.float32, device=DEV)
-    nbytes = workspace_bytes(C.byref(w), n, h, wd)
-    ws = torch.full((nbytes,), fill, dtype=torch.uint8, device=DEV)
-    _lib.check(forward(C.byref(w), img.data_ptr(), n, h, wd, feat_c.data_ptr(), feat_f.data_ptr(), ws.data_ptr(),
-                       nbytes, _stream(img)))
-    torch.cuda.synchronize()
-    return feat_c, feat_f
-
-
 @gpu
 @pytest.mark.parametrize("d2,d3,shape", [(*d, s) for d in WIDTHS for s in SHAPES] + [(*d, (8, 136, 200)) for d in BATCH8])
 def test_backbone_widths_match_fp64(d2, d3, shape):
     from loftr_b200.loftr import TensorCoreBackbone
-    m = _backbone(d2, d3)
+    m = B.make_backbone(d2, d3, DEV)
     assert TensorCoreBackbone.supported(m)
-    img = _image(shape, d2 + d3)
+    img = B.image(shape, d2 + d3)
     with torch.no_grad():
         ex = copy.deepcopy(m).double()(img.double())
-        emu = backbone_fp16_ref(m, img)
-    split = _forward(TensorCoreBackbone(m), img)
-    fp16 = _forward(TensorCoreBackbone(m, precision="fp16"), img)
+        emu = B.forward_f64(m, img)
+    split = B.backbone_forward(TensorCoreBackbone(m), img)[1:]
+    fp16 = B.backbone_forward(TensorCoreBackbone(m, precision="fp16"), img)[1:]
     stats, failed = {}, []
     for name, g_split, g_fp16, x, e in zip(("coarse", "fine"), split, fp16, ex, emu):
         scale = x.abs().max().item()
@@ -104,14 +67,14 @@ def test_backbone_widths_ignore_padding_and_batch_position(d2, d3, precision):
     """The channels between a layer's width and its padded row stride are never written: a NaN-filled workspace gives
     the bits of a zeroed one.  An image alone gives the bits it gets inside a batch."""
     from loftr_b200.loftr import TensorCoreBackbone
-    tc = TensorCoreBackbone(_backbone(d2, d3), precision=precision)
-    batch = _image((3, 88, 72), 7)
-    zc, zf = _forward(tc, batch, 0)
-    nc, nf = _forward(tc, batch, 0xFF)
+    tc = TensorCoreBackbone(B.make_backbone(d2, d3, DEV), precision=precision)
+    batch = B.image((3, 88, 72), 7)
+    _, zc, zf = B.backbone_forward(tc, batch, 0)
+    _, nc, nf = B.backbone_forward(tc, batch, 0xFF)
     assert torch.isfinite(zc).all() and torch.isfinite(zf).all()
     assert torch.equal(zc, nc) and torch.equal(zf, nf)
     for i in (0, 2):
-        c, f = _forward(tc, batch[i:i + 1].contiguous(), 0xFF)
+        _, c, f = B.backbone_forward(tc, batch[i:i + 1].contiguous(), 0xFF)
         assert torch.equal(c[0], zc[i]) and torch.equal(f[0], zf[i]), i
 
 
@@ -121,10 +84,10 @@ def test_coarse_width_not_divisible_by_4_cannot_run(d3):
     """feat_c is stored as fp32 NHWC rows of d3 values through a TMA map, whose row stride must be a multiple of 16
     bytes: d3 % 4 != 0 fails there, which is why `supported()` refuses such widths."""
     from loftr_b200.loftr import TensorCoreBackbone
-    m = _backbone(196, d3)
+    m = B.make_backbone(196, d3, DEV)
     assert not TensorCoreBackbone.supported(m)
     with pytest.raises(RuntimeError, match="not a multiple of 16"):
-        _forward(TensorCoreBackbone(m), _image((1, 16, 16), 3))
+        B.backbone_forward(TensorCoreBackbone(m), B.image((1, 16, 16), 3))
 
 
 @pytest.mark.parametrize("d3", [130, 201])

@@ -3,13 +3,12 @@ lb_backbone_forward: every layer class of the network -- Cin 128 / 196 / 256 wit
 remainder, Cout tiles 128 / 208 / 256, BatchNorm, residual and FPN paths -- against the float64 PyTorch module, at
 batch 1 and 16 and at sizes whose 1/2, 1/4 and 1/8 grids are not multiples of the 8 x 16 output tile (a 16 x 16
 image leaves 2 x 2 pixels at 1/8: the halo is mostly zero fill)."""
-import ctypes as C
 import copy
 
-import numpy as np
 import pytest
 import torch
 
+import backbone_ref as B
 import util
 from cases import CASES
 
@@ -17,34 +16,16 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 
 
-def _forward(tc, img, fill):
-    """TensorCoreBackbone.__call__ with a workspace pre-filled with byte `fill` (0xFF: every fp16 is NaN)."""
-    from loftr_b200 import _lib
-    from loftr_b200.loftr import _stream
-    lib = _lib.load()
-    w, _ = tc._pack()
-    n, _, h, wd = img.shape
-    feat_c = torch.empty(n, h // 8, wd // 8, 256, dtype=torch.float32, device=DEV)
-    feat_f = torch.empty(n, h // 2, wd // 2, 128, dtype=torch.float32, device=DEV)
-    nbytes = lib.lb_backbone_workspace_bytes(C.byref(w), n, h, wd)
-    ws = torch.full((nbytes,), fill, dtype=torch.uint8, device=DEV)
-    _lib.check(lib.lb_backbone_forward(C.byref(w), img.data_ptr(), n, h, wd, feat_c.data_ptr(), feat_f.data_ptr(),
-                                       ws.data_ptr(), nbytes, _stream(img)))
-    torch.cuda.synchronize()
-    return feat_c, feat_f
-
-
 @pytest.mark.parametrize("shape", [(1, 16, 16), (16, 136, 200), (1, 88, 72)])
 def test_backbone_halo_convs_match_fp64(shape):
     from loftr_b200.loftr import TensorCoreBackbone
     n, h, w = shape
     model, _, _ = util.build_model(dict(CASES[0]), DEV)
-    rs = np.random.RandomState(11)
-    img = torch.from_numpy(rs.uniform(0, 1, (n, 1, h, w)).astype(np.float32)).to(DEV)
+    img = B.image(shape, 11)
     with torch.no_grad():
         ex_c, ex_f = copy.deepcopy(model.backbone).double()(img.double())
     tc = TensorCoreBackbone(model.backbone)
-    got_c, got_f = _forward(tc, img, 0)
+    _, got_c, got_f = B.backbone_forward(tc, img)
     for got, ex, name in ((got_c, ex_c, "coarse"), (got_f, ex_f, "fine")):
         scale = ex.abs().max().item()
         err = (got.permute(0, 3, 1, 2).double() - ex).abs().max().item()
@@ -57,10 +38,9 @@ def test_backbone_ignores_channel_padding():
     workspace full of NaN must give the same bits as a zeroed one: the padding never reaches an MMA."""
     from loftr_b200.loftr import TensorCoreBackbone
     model, _, _ = util.build_model(dict(CASES[0]), DEV)
-    rs = np.random.RandomState(12)
-    img = torch.from_numpy(rs.uniform(0, 1, (2, 1, 96, 136)).astype(np.float32)).to(DEV)
+    img = B.image((2, 96, 136), 12)
     tc = TensorCoreBackbone(model.backbone)
-    zc, zf = _forward(tc, img, 0)
-    nc, nf = _forward(tc, img, 0xFF)
+    _, zc, zf = B.backbone_forward(tc, img, 0)
+    _, nc, nf = B.backbone_forward(tc, img, 0xFF)
     assert torch.isfinite(nc).all() and torch.isfinite(nf).all()
     assert torch.equal(zc, nc) and torch.equal(zf, nf)

@@ -2,41 +2,19 @@
 model's configuration surface and the library-version guard of the binding."""
 import numpy as np
 import pytest
-import torch
 
-import full_oracle as FO
 import loftr_b200
 import util
-from full_cases import FA_MODULE_CASE, FULL_CASES, build_fa_module_inputs, build_full_cfg
+from full_cases import FA_MODULE_CASE, FULL_CASES, build_fa_module_inputs
 from loftr_b200 import _lib
 from loftr_b200.loftr import LocalFeatureTransformer, LoFTREncoderLayer
-
-
-def _oracle_forward(case):
-    """PyTorch backbone + tests/full_oracle.hot_path (util.oracle_forward with the case's attention kinds)."""
-    import weights as W
-    cfg = build_full_cfg(case)
-    model = loftr_b200.LoFTR(cfg).eval()
-    shapes = {k: tuple(v.shape) for k, v in model.state_dict().items()}
-    state = W.make_state(shapes, seed=case.get("wseed", 0))
-    model.load_state_dict({k: torch.from_numpy(v) for k, v in state.items()})
-    inp = util.build_inputs(case)
-    with torch.no_grad():
-        i0, i1 = torch.from_numpy(inp["image0"]), torch.from_numpy(inp["image1"])
-        if i0.shape == i1.shape:
-            fc, ff = model.backbone(torch.cat([i0, i1], 0))
-            (c0, c1), (f0, f1) = fc.split(i0.shape[0]), ff.split(i0.shape[0])
-        else:
-            (c0, f0), (c1, f1) = model.backbone(i0), model.backbone(i1)
-    npf = lambda t: t.float().numpy()
-    return FO.hot_path(npf(c0), npf(c1), npf(f0), npf(f1), state, cfg, inp["image0"].shape[2:], inp["image1"].shape[2:],
-                       inp.get("mask0"), inp.get("mask1"), inp.get("scale0"), inp.get("scale1"))
+from oracle import loftr_oracle as O
 
 
 @pytest.mark.parametrize("case", FULL_CASES, ids=[c["name"] for c in FULL_CASES])
 def test_full_oracle_matches_reference(case):
     gold = util.load_golden(case["name"])
-    out = _oracle_forward(case)
+    out = util.oracle_forward(case)
     np.testing.assert_allclose(out["feat_c0"][:, ::7, ::5], gold["feat_c0_s"], rtol=2e-4, atol=2e-4)
     np.testing.assert_allclose(out["feat_c1"][:, ::7, ::5], gold["feat_c1_s"], rtol=2e-4, atol=2e-4)
     stats = util.compare_matches(out, gold, gold, conf_rtol=1e-3, px_tol=0.05, label=case["name"])
@@ -53,7 +31,7 @@ def test_full_attention_masked_module_convention():
     """Valid rows equal the reference's FullAttention; the reference's padded rows are NaN, ours are 0."""
     gold = util.load_golden(FA_MODULE_CASE["name"])
     q, k, v, qm, km = build_fa_module_inputs()
-    out = FO.full_attention(q, k, v, qm, km)
+    out = O.full_attention(q, k, v, qm, km)
     assert np.isfinite(out).all()
     assert np.isnan(gold["out"][~qm]).all()          # what the convention replaces
     np.testing.assert_allclose(out[qm], gold["out"][qm], rtol=1e-5, atol=1e-6)
@@ -61,8 +39,8 @@ def test_full_attention_masked_module_convention():
     # a row whose keys are all masked gets a zero message too; unmasked calls are a plain softmax
     km0 = km.copy()
     km0[0] = False
-    assert (FO.full_attention(q, k, v, qm, km0)[0] == 0).all()
-    plain = FO.full_attention(q[:1, :5], k[:1], v[:1])
+    assert (O.full_attention(q, k, v, qm, km0)[0] == 0).all()
+    plain = O.full_attention(q[:1, :5], k[:1], v[:1])
     s = np.einsum("lhd,shd->lhs", q[0, :5].astype(np.float64), k[0].astype(np.float64)) / np.sqrt(q.shape[-1])
     a = np.exp(s - s.max(-1, keepdims=True))
     a /= a.sum(-1, keepdims=True)

@@ -215,14 +215,13 @@ def kv_splits(n_groups, rows, sms):
 
 
 def _tf_check(name, tf, attention, f0, f1, m0=None, m1=None):
-    import full_oracle as FO
     lw = R.layer_weights(tf, DEV)
     names, nhead = tf.layer_names, tf.nhead
     t = lambda m: None if m is None else _t(m)
     g0, g1 = tf(_t(f0), _t(f1), t(m0), t(m1))
     r0, r1 = R.transformer(R.f64(f0, DEV), R.f64(f1, DEV), lw, names, nhead, t(m0), t(m1), attention)
     ow = [{k: _np(v).astype(np.float32) for k, v in w.items()} for w in lw]
-    o0, o1 = FO.local_feature_transformer(f0, f1, ow, names, nhead, m0, m1, attention)
+    o0, o1 = O.local_feature_transformer(f0, f1, ow, names, nhead, m0, m1, attention)
     finding = RATIO_FINDINGS.get(name)
     errs = [_bound(name + "_feat0", g0, r0, o0, finding=finding), _bound(name + "_feat1", g1, r1, o1, finding=finding)]
     return errs

@@ -8,9 +8,8 @@ import pytest
 import torch
 
 import loftr_b200
-import weights as W
+import util
 from cases import BASELINE_CASES, CASES, CM_CASES, build_cfg, build_cm_inputs, build_inputs
-from full_cases import build_full_cfg
 from loftr_b200 import _lib
 from match_cap_ref import LIST_KEYS, apply_cap, capped_rows, per_pair_counts
 
@@ -37,21 +36,6 @@ GRID = {
     # n = 1 at the largest size (L = 19,200)
     "n1_1280x960": BASELINE_CASES["sweep960"],
 }
-
-
-def _model(case, backbone_impl="auto"):
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
-    model = loftr_b200.LoFTR(build_full_cfg(case), backbone_impl=backbone_impl).eval()
-    shapes = {k: tuple(v.shape) for k, v in model.state_dict().items()}
-    model.load_state_dict({k: torch.from_numpy(v) for k, v in W.make_state(shapes, seed=case.get("wseed", 0)).items()})
-    return model.to(DEV)
-
-
-def _inputs(case, seed=None):
-    if seed is not None:
-        case = dict(case, iseed=seed)
-    return {k: torch.from_numpy(np.ascontiguousarray(v)).to(DEV) for k, v in build_inputs(case).items()}
 
 
 def _eager(model, inp, k="keep"):
@@ -86,8 +70,8 @@ def _k_values(counts, L):
 @pytest.mark.parametrize("name", list(GRID))
 def test_cap_selects_the_most_confident_rows(name):
     case = GRID[name]
-    model = _model(case)
-    inp = _inputs(case)
+    model, _, _ = util.build_model(case, DEV)
+    inp = util.device_inputs(case)
     lib = _lib.load()
     _eager(model, inp, None)   # the first call also packs the weights
     n0 = lib.lb_launch_count()
@@ -124,9 +108,9 @@ def test_cap_selects_the_most_confident_rows(name):
 def test_ties_at_the_kth_value_go_to_the_smaller_row():
     """At a tiny softmax temperature most mutual matches score exactly 1.0 in fp32."""
     case = dict(_SMALL, name="ties")
-    model = _model(case)
+    model, _, _ = util.build_model(case, DEV)
     model.coarse_matching.temperature = 1e-4
-    inp = _inputs(case)
+    inp = util.device_inputs(case)
     uncapped = _eager(model, inp, None)
     b_ids, conf, i_ids = uncapped["b_ids"], uncapped["mconf"], uncapped["i_ids"]
     above = [int(((b_ids == b) & (conf > 1.0)).sum()) for b in range(case["n"])]
@@ -147,8 +131,8 @@ def test_ties_at_the_kth_value_go_to_the_smaller_row():
 
 def test_captured_matcher_with_a_cap():
     case = BASELINE_CASES["b8"]
-    model = _model(case)
-    batches = [_inputs(case, seed) for seed in (1, 2)]
+    model, _, _ = util.build_model(case, DEV)
+    batches = [util.device_inputs(case, seed) for seed in (1, 2)]
     model.coarse_matching.max_matches_per_pair = 300
     cm = loftr_b200.CapturedMatcher(model, case["n"], case["hw0"])
     assert cm.capacity == 8 * 300
@@ -184,7 +168,7 @@ def test_captured_matcher_with_a_cap():
 
 def test_match_features_equals_capped_matcher_batch():
     """Tensor-core backbone: the bank path and matcher(batch) on the stacked pairs agree bit for bit under a cap."""
-    model = _model(dict(_SMALL, name="bank"), backbone_impl="b200")
+    model, _, _ = util.build_model(dict(_SMALL, name="bank"), DEV, "b200")
     inp = build_inputs({"n": 3, "hw0": (480, 640), "hw1": (480, 640), "images": "smooth", "iseed": 1})
     imgs = torch.from_numpy(np.concatenate([inp["image0"], inp["image1"]])).to(DEV)
     bank = model.extract_features(imgs)

@@ -1,5 +1,5 @@
 """CPU checks of the single-pass fp16 matching mode (`match_precision="fp16"`, DESIGN.md §16): the float64 emulation
-(tests/match_fp16_ref.py) against ref64 with rounding off and on hand cases with it on, and the Python API (constructor
+(`fp16=True` of tests/ref64.py) on hand cases, and the Python API (constructor
 values, read-only attributes, the library version gate, the C entry points' argument check)."""
 import copy
 import ctypes as C
@@ -8,8 +8,7 @@ import pytest
 import torch
 
 import loftr_b200
-import match_fp16_ref as M
-import ref64
+import ref64 as R
 from loftr_b200 import _lib
 from loftr_b200.loftr import CoarseMatching, LocalFeatureTransformer
 
@@ -20,51 +19,17 @@ TINY = 2.0 ** -12    # below half an fp16 ulp of values in [1, 2): rounds away
 def _layers(d_model, attention, n_layers=2, seed=0):
     torch.manual_seed(seed)
     cfg = {"d_model": d_model, "nhead": 8, "layer_names": ["self", "cross"][:n_layers], "attention": attention}
-    return cfg, ref64.layer_weights(LocalFeatureTransformer(cfg))
-
-
-def _masks(n, L, S):
-    m0 = torch.ones(n, L, dtype=torch.bool)
-    m1 = torch.ones(n, S, dtype=torch.bool)
-    m0[0, L - 3:] = False
-    m1[-1, S - 5:] = False
-    return m0, m1
-
-
-# ------------------------------------------------------------------------------------------------ emulation = ref64
-@pytest.mark.parametrize("d_model,attention", [(256, "linear"), (256, "full"), (128, "linear"), (128, "full")])
-@pytest.mark.parametrize("masked", [False, True])
-def test_identity_rounding_is_ref64_transformer(d_model, attention, masked):
-    cfg, layers = _layers(d_model, attention)
-    n, L, S = 2, 25 if d_model == 128 else 37, 25 if d_model == 128 else 29
-    f0 = torch.randn(n, L, d_model, dtype=F64)
-    f1 = torch.randn(n, S, d_model, dtype=F64)
-    m0, m1 = _masks(n, L, S) if masked else (None, None)
-    got = M.transformer(f0, f1, layers, cfg["layer_names"], 8, m0, m1, attention, rounding=False)
-    ref = ref64.transformer(f0, f1, layers, cfg["layer_names"], 8, m0, m1, attention)
-    for g, r in zip(got, ref):
-        assert torch.allclose(g, r, rtol=0, atol=1e-12), (g - r).abs().max()
-
-
-@pytest.mark.parametrize("match_type", ["dual_softmax", "sinkhorn"])
-def test_identity_rounding_is_ref64_conf_matrix(match_type):
-    mc = dict(loftr_b200.get_cfg("indoor_ds")["match_coarse"], match_type=match_type, skh_iters=3, skh_prefilter=False)
-    f0, f1 = torch.randn(2, 30, 256, dtype=F64) * 4, torch.randn(2, 21, 256, dtype=F64) * 4
-    m0, m1 = _masks(2, 30, 21)
-    bs = torch.tensor(1.0, dtype=F64)
-    got = M.conf_matrix(f0, f1, mc, m0, m1, bs, rounding=False)
-    assert torch.equal(got, ref64.conf_matrix(f0, f1, mc, m0, m1, bs))
-    assert not torch.equal(M.conf_matrix(f0, f1, mc, m0, m1, bs), got)
+    return cfg, R.layer_weights(LocalFeatureTransformer(cfg))
 
 
 # ------------------------------------------------------------------------------------------------ hand cases
 def test_roundings_of_one_value():
     x = torch.tensor([1.0 + TINY, 1.0 + 2.0 ** -10, 1.0 / 3.0], dtype=F64)
-    assert M.r16(x).tolist() == [1.0, 1.0 + 2.0 ** -10, float(torch.tensor(1.0 / 3.0).half())]
-    assert torch.equal(M.r16(x, rounding=False), x)
+    assert R.r16(x).tolist() == [1.0, 1.0 + 2.0 ** -10, float(torch.tensor(1.0 / 3.0).half())]
+    assert torch.equal(R.r16(x, False), x)
     w = torch.tensor([1e-3 / 3.0], dtype=F64)    # e = 21: fp16(w * 2^21) keeps 11 bits of w whatever its magnitude
-    assert M.w16(w, 21).item() == float(torch.tensor(1e-3 / 3.0 * 2.0 ** 21).half()) * 2.0 ** -21
-    assert abs(M.w16(w, 21).item() / w.item() - 1) < 2.0 ** -11 and M.w16(w, 21).item() != w.item()
+    assert R.w16(w, 21).item() == float(torch.tensor(1e-3 / 3.0 * 2.0 ** 21).half()) * 2.0 ** -21
+    assert abs(R.w16(w, 21).item() / w.item() - 1) < 2.0 ** -11 and R.w16(w, 21).item() != w.item()
 
 
 def test_linear_attention_rounds_k_and_v():
@@ -72,17 +37,17 @@ def test_linear_attention_rounds_k_and_v():
     q = torch.randn(1, 5, 2, 4, dtype=F64)
     k = torch.full((1, 7, 2, 4), TINY, dtype=F64)
     v = torch.full((1, 7, 2, 4), 1.0 + TINY, dtype=F64)
-    exact1 = M.linear_attention(q, torch.zeros_like(k), torch.ones_like(v), rounding=False)
-    assert torch.allclose(M.linear_attention(q, k, v), exact1, rtol=1e-15, atol=0)
-    assert not torch.allclose(M.linear_attention(q, k, v, rounding=False), exact1, rtol=1e-6, atol=0)
+    exact1 = R.linear_attention(q, torch.zeros_like(k), torch.ones_like(v))
+    assert torch.allclose(R.linear_attention(q, k, v, fp16=True), exact1, rtol=1e-15, atol=0)
+    assert not torch.allclose(R.linear_attention(q, k, v), exact1, rtol=1e-6, atol=0)
 
 
 def test_full_attention_rounds_q_k_v_and_p():
     q = torch.full((1, 3, 1, 32), 1.0 + TINY, dtype=F64)
     k = torch.full((1, 4, 1, 32), 1.0 + TINY, dtype=F64)
     v = torch.arange(4, dtype=F64).view(1, 4, 1, 1).expand(1, 4, 1, 32) * (1.0 + TINY)
-    one = M.full_attention(torch.ones_like(q), torch.ones_like(k), v.half().double(), rounding=False)
-    assert torch.allclose(M.full_attention(q, k, v), one, rtol=1e-15, atol=0)   # equal logits: mean of fp16(V)
+    one = R.full_attention(torch.ones_like(q), torch.ones_like(k), v.half().double())
+    assert torch.allclose(R.full_attention(q, k, v, fp16=True), one, rtol=1e-15, atol=0)   # equal logits: mean fp16(V)
     # P = exp(S / sqrt(D) - rowmax) is rounded in P V, not in the row sum
     a = 2.0 ** -4
     qq = torch.zeros(1, 1, 1, 32, dtype=F64)
@@ -91,11 +56,11 @@ def test_full_attention_rounds_q_k_v_and_p():
     kk[0, 1, 0, 0] = a
     vv = torch.cat([torch.ones(1, 1, 1, 32), torch.full((1, 1, 1, 32), 2.0)], 1).double()
     p0 = torch.exp(torch.tensor(-a / 32 ** 0.5, dtype=F64))
-    assert M.r16(p0) != p0
-    want = (M.r16(p0) * 1.0 + 2.0) / (p0 + 1.0)
-    assert torch.allclose(M.full_attention(qq, kk, vv), torch.full((1, 1, 1, 32), want.item(), dtype=F64), rtol=1e-15,
-                          atol=0)
-    assert not torch.allclose(M.full_attention(qq, kk, vv, rounding=False), torch.full((1, 1, 1, 32), want.item(),
+    assert R.r16(p0) != p0
+    want = (R.r16(p0) * 1.0 + 2.0) / (p0 + 1.0)
+    assert torch.allclose(R.full_attention(qq, kk, vv, fp16=True), torch.full((1, 1, 1, 32), want.item(), dtype=F64),
+                          rtol=1e-15, atol=0)
+    assert not torch.allclose(R.full_attention(qq, kk, vv), torch.full((1, 1, 1, 32), want.item(),
                                                                                        dtype=F64), rtol=1e-9, atol=0)
 
 
@@ -104,29 +69,28 @@ def test_encoder_layer_rounds_activations_and_weights_but_not_the_residual():
     w = layers[0]
     x0 = (torch.randn(1, 9, 256, dtype=F64) + 3.0).half().double()        # fp16 values in about [1, 6]
     x = x0 * (1.0 + TINY / 8)                                            # rounds back to x0 everywhere it is an operand
-    out0, out = M.encoder_layer(x0, x0, w, 8), M.encoder_layer(x, x, w, 8)
+    out0, out = R.encoder_layer(x0, x0, w, 8, fp16=True), R.encoder_layer(x, x, w, 8, fp16=True)
     assert torch.allclose(out - x, out0 - x0, rtol=0, atol=1e-12)        # only the exact residual sees the change
-    exact = M.encoder_layer(x, x, w, 8, rounding=False) - M.encoder_layer(x0, x0, w, 8, rounding=False)
+    exact = R.encoder_layer(x, x, w, 8) - R.encoder_layer(x0, x0, w, 8)
     assert (exact - (x - x0)).abs().max() > 1e-7
     # weights within a fraction of an fp16 ulp of their hi plane give the same layer
-    e = M.layer_exponents(w)
+    e = R.layer_exponents(w)
     keys = {"q_proj.weight": "qkv", "k_proj.weight": "qkv", "v_proj.weight": "qkv", "merge.weight": "merge",
             "mlp.0.weight": "mlp0", "mlp.2.weight": "mlp2"}
-    w_hi = dict(w, **{k: M.w16(w[k], e[g]) for k, g in keys.items()})
+    w_hi = dict(w, **{k: R.w16(w[k], e[g]) for k, g in keys.items()})
     w_near = dict(w_hi, **{k: w_hi[k] * (1.0 + TINY / 4) for k in keys})
-    assert M.layer_exponents(w_near) == e
-    assert torch.equal(M.encoder_layer(x0, x0, w_near, 8), M.encoder_layer(x0, x0, w_hi, 8))
-    assert not torch.equal(M.encoder_layer(x0, x0, w_near, 8, rounding=False),
-                           M.encoder_layer(x0, x0, w_hi, 8, rounding=False))
+    assert R.layer_exponents(w_near) == e
+    assert torch.equal(R.encoder_layer(x0, x0, w_near, 8, fp16=True), R.encoder_layer(x0, x0, w_hi, 8, fp16=True))
+    assert not torch.equal(R.encoder_layer(x0, x0, w_near, 8), R.encoder_layer(x0, x0, w_hi, 8))
 
 
 def test_score_matrix_rounds_both_features():
     mc = loftr_b200.get_cfg("indoor_ds")["match_coarse"]
     f0 = (torch.randn(1, 6, 256, dtype=F64) + 2).half().double()
     f1 = (torch.randn(1, 5, 256, dtype=F64) + 2).half().double()
-    near = M.conf_matrix(f0 * (1 + TINY / 8), f1 * (1 - TINY / 8), mc)
-    assert torch.equal(near, M.conf_matrix(f0, f1, mc))
-    assert not torch.equal(M.conf_matrix(f0 * (1 + TINY / 8), f1, mc, rounding=False), M.conf_matrix(f0, f1, mc))
+    near = R.conf_matrix(f0 * (1 + TINY / 8), f1 * (1 - TINY / 8), mc, fp16=True)
+    assert torch.equal(near, R.conf_matrix(f0, f1, mc, fp16=True))
+    assert not torch.equal(R.conf_matrix(f0 * (1 + TINY / 8), f1, mc), R.conf_matrix(f0, f1, mc, fp16=True))
 
 
 # ------------------------------------------------------------------------------------------------ Python API

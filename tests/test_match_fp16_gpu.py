@@ -2,7 +2,7 @@
 the GPU.
 
 Per output, the error against float64 (ref64) is held to twice the error of the float64 emulation of the same
-semantics (tests/match_fp16_ref.py) plus 1e-6 of the output's scale, as for the fp16 backbone.  The coarse match list
+semantics (ref64 with fp16=True) plus 1e-6 of the output's scale, as for the fp16 backbone.  The coarse match list
 follows the emulation's by the match-list rule of DESIGN.md §5 with the emulation in place of fp64.  Every public path
 runs unchanged on top, bit for bit against the eager forward, and the bits do not depend on the workspace's contents
 or on repetition."""
@@ -14,12 +14,9 @@ import torch
 
 import loftr_b200
 import loftr_b200.loftr as L
-import match_fp16_ref as M
 import ref64
 import util
-import weights as W
 from cases import BASELINE_CASES, CASES, build_cfg, build_inputs
-from full_cases import build_full_cfg
 from loftr_b200 import _lib
 from match_cap_ref import LIST_KEYS, apply_cap, capped_rows
 
@@ -86,7 +83,7 @@ def test_coarse_transformer_error_is_that_of_its_semantics(attention, masked):
     got = _run(tf, f0, f1, mask)
     x0, x1 = f0.double(), f1.double()
     exact = ref64.transformer(x0, x1, layers, cfg["layer_names"], 8, m0, m1, attention)
-    emu = M.transformer(x0, x1, layers, cfg["layer_names"], 8, m0, m1, attention)
+    emu = ref64.transformer(x0, x1, layers, cfg["layer_names"], 8, m0, m1, attention, fp16=True)
     stats = {}
     for name, gg, e, x in zip(("feat0", "feat1"), got, emu, exact):
         _bound(name, gg, e, x, stats)
@@ -107,7 +104,7 @@ def test_fine_transformer_error_is_that_of_its_semantics(ww, attention, live):
     k = n if live is None else live
     x0, x1 = f0[:k].double(), f1[:k].double()
     exact = ref64.transformer(x0, x1, layers, cfg["layer_names"], 8, attention=attention)
-    emu = M.transformer(x0, x1, layers, cfg["layer_names"], 8, attention=attention)
+    emu = ref64.transformer(x0, x1, layers, cfg["layer_names"], 8, attention=attention, fp16=True)
     stats = {}
     for name, gg, e, x in zip(("feat0", "feat1"), got, emu, exact):
         _bound(name, gg[:k], e, x, stats)
@@ -165,7 +162,7 @@ def test_conf_matrix_and_match_list_follow_the_emulation(match_type, masked):
     fm0 = None if m0 is None else m0.flatten(-2)
     fm1 = None if m1 is None else m1.flatten(-2)
     exact = ref64.conf_matrix(f0.double(), f1.double(), mc, fm0, fm1, bs)
-    emu = M.conf_matrix(f0.double(), f1.double(), mc, fm0, fm1, bs)
+    emu = ref64.conf_matrix(f0.double(), f1.double(), mc, fm0, fm1, bs, fp16=True)
     got = data["conf_matrix"]
     if masked:   # cells whose row and column are both padding: 0 in the engine (DESIGN.md §5)
         valid = (fm0[:, :, None] | fm1[:, None, :]).double()
@@ -210,22 +207,7 @@ def test_coarse_match_bits_do_not_depend_on_the_workspace_and_the_cap_keeps_rows
 
 # ---------------------------------------------------------------------------------------------- end to end
 def _model(case, backbone_impl="b200", match_precision="fp16"):
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
-    model = loftr_b200.LoFTR(build_full_cfg(case), backbone_impl=backbone_impl, match_precision=match_precision).eval()
-    shapes = {k: tuple(v.shape) for k, v in model.state_dict().items()}
-    model.load_state_dict({k: torch.from_numpy(v) for k, v in W.make_state(shapes, seed=case.get("wseed", 0)).items()})
-    return model.to(DEV)
-
-
-def _inputs(case):
-    return {k: torch.from_numpy(np.ascontiguousarray(v)).to(DEV) for k, v in build_inputs(case).items()}
-
-
-def _eager(model, inp):
-    data = dict(inp)
-    model(data)
-    return data
+    return util.build_model(case, DEV, backbone_impl, match_precision)[0]
 
 
 @pytest.mark.parametrize("name", ["ds_thr0", "ds_masked_scaled", "ds_unequal", "ds_empty", "ot_thr0"])
@@ -234,10 +216,10 @@ def test_fp16_matching_runs_every_path(name):
     dtypes and (b, i) order; static, captured and repeated outputs equal the eager forward bit for bit; a capped run
     equals the selected rows of the uncapped one."""
     case = _CASE[name]
-    inp = _inputs(case)
+    inp = util.device_inputs(case)
     model = _model(case)
-    got = _eager(model, inp)
-    ref = _eager(_model(case, match_precision="split"), inp)
+    got = util.eager(model, inp)
+    ref = util.eager(_model(case, match_precision="split"), inp)
     assert list(got) == list(ref)
     for k, v in ref.items():
         if torch.is_tensor(v):
@@ -247,7 +229,7 @@ def test_fp16_matching_runs_every_path(name):
     m = got["b_ids"].shape[0]
     if name == "ds_empty":
         assert m == 0
-    again = _eager(model, inp)
+    again = util.eager(model, inp)
     for k, v in got.items():
         if torch.is_tensor(v):
             assert torch.equal(again[k], v), f"repeat {k}"
@@ -266,7 +248,7 @@ def test_fp16_matching_runs_every_path(name):
     if m:
         k = max(1, m // (2 * case["n"]))
         model.coarse_matching.max_matches_per_pair = k
-        capped = _eager(model, inp)
+        capped = util.eager(model, inp)
         sel = apply_cap(got, k)
         for key in LIST_KEYS:
             assert torch.equal(capped[key], sel[key]), f"cap {k}: {key}"
@@ -298,9 +280,9 @@ def test_fp16_matching_agreement_with_split_at_8x640x480(backbone):
     """Recorded, not gated: with random weights the coarse logits reach 70-105 (SURVEY.md hard part 1), which
     exaggerates the effect of fp16 products on the match list.  No trained checkpoint is available here."""
     case = BASELINE_CASES["b8"]
-    inp = _inputs(case)
-    got = _eager(_model(case, backbone), inp)
-    ref = _eager(_model(case, backbone, "split"), inp)
+    inp = util.device_inputs(case)
+    got = util.eager(_model(case, backbone), inp)
+    ref = util.eager(_model(case, backbone, "split"), inp)
     kg = {k: n for n, k in enumerate(zip(*(got[x].tolist() for x in ("b_ids", "i_ids", "j_ids"))))}
     kr = {k: n for n, k in enumerate(zip(*(ref[x].tolist() for x in ("b_ids", "i_ids", "j_ids"))))}
     common = sorted(set(kg) & set(kr))

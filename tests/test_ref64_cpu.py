@@ -10,7 +10,7 @@ import ref64 as R
 import util
 from cases import CASES, CM_CASES, build_cfg, build_cm_inputs, build_inputs
 from edge_cases import EDGE_CASES, build_edge_cfg
-from full_cases import FULL_CASES, build_full_cfg
+from full_cases import FULL_CASES
 
 
 def _np(t):
@@ -86,7 +86,7 @@ def test_ref64_edge_configs_match_reference_f64(case):
 def test_ref64_full_attention_matches_reference(case):
     """Full attention: the float64 keys exactly, and the fp32 taps at the tolerance of the fp32 oracle's tests."""
     gold = util.load_golden(case["name"])
-    out = _model_f64_forward(case, build_full_cfg(case))
+    out = _model_f64_forward(case, build_cfg(case))
     _check_f64_keys(out, gold)
     np.testing.assert_allclose(_np(out["feat_c0"])[:, ::7, ::5], gold["feat_c0_s"], rtol=2e-4, atol=2e-4)
     np.testing.assert_allclose(_np(out["feat_c1"])[:, ::7, ::5], gold["feat_c1_s"], rtol=2e-4, atol=2e-4)

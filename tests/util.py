@@ -1,4 +1,5 @@
-"""Shared helpers of the parity tests."""
+"""Shared helpers of the parity tests: the model with the test weights, the numpy oracle's forward (whole batch and per
+pair, cached), the match-list rule, and the GPU matcher harness (device inputs, eager forward, static = eager)."""
 from __future__ import annotations
 
 import os
@@ -8,19 +9,24 @@ import torch
 
 import weights as W
 from cases import build_cfg, build_cm_inputs, build_inputs  # noqa: F401
+from match_cap_ref import LIST_KEYS
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+DEV = "cuda:0"
 
 
 def load_golden(name):
     return dict(np.load(os.path.join(GOLDEN, name + ".npz")))
 
 
-def build_model(case, device="cpu"):
-    """loftr_b200.LoFTR with the deterministic RandomState weights of tests/golden/weights.py."""
+def build_model(case, device="cpu", backbone_impl="auto", match_precision="split"):
+    """loftr_b200.LoFTR with the case's configuration (attention kinds included), the deterministic RandomState weights
+    of tests/golden/weights.py and TF32 off (torch's fp32 products stay fp32) -> (model on `device`, cfg, state)."""
     import loftr_b200
+    torch.backends.cudnn.allow_tf32 = False
+    torch.backends.cuda.matmul.allow_tf32 = False
     cfg = build_cfg(case)
-    model = loftr_b200.LoFTR(cfg).eval()
+    model = loftr_b200.LoFTR(cfg, backbone_impl=backbone_impl, match_precision=match_precision).eval()
     shapes = {k: tuple(v.shape) for k, v in model.state_dict().items()}
     state = W.make_state(shapes, seed=case.get("wseed", 0))
     if "bin_score" in case and "coarse_matching.bin_score" in state:
@@ -29,23 +35,53 @@ def build_model(case, device="cpu"):
     return model.to(device), cfg, state
 
 
-def oracle_forward(case, backbone_device="cpu"):
-    """PyTorch backbone (the part that stays PyTorch) + numpy oracle for everything after it."""
-    from oracle import loftr_oracle as O
-    model, cfg, state = build_model(case, backbone_device)
-    inp = build_inputs(case)
+def device_inputs(case, seed=None):
+    """The case's input batch (image seed `seed` instead of the case's) as tensors on the GPU"""
+    if seed is not None:
+        case = dict(case, iseed=seed)
+    return {k: torch.from_numpy(np.ascontiguousarray(v)).to(DEV) for k, v in build_inputs(case).items()}
+
+
+def eager(model, inp):
+    """model(batch) on a copy of `inp` -> the batch dict with every output"""
+    data = dict(inp)
+    model(data)
+    return data
+
+
+def assert_static_equals_eager(st, eager, label):
+    """The live prefix of every list output of forward_static / CapturedMatcher equals the eager forward bit for bit,
+    with the eager dtypes and sizes, within the capacity, and mkpts0_f aliases mkpts0_c as in the eager forward."""
+    m = int(st["num_matches"].item())
+    assert m == eager["b_ids"].shape[0], f"{label}: count {m} vs eager {eager['b_ids'].shape[0]}"
+    assert m <= st["b_ids"].shape[0]
+    for k in LIST_KEYS:
+        assert st[k].dtype == eager[k].dtype, (label, k)
+        assert torch.equal(st[k][:m], eager[k]), f"{label}: {k} differs from the eager forward"
+    assert st["mkpts0_f"] is st["mkpts0_c"]
+    for k in ("bs", "hw0_i", "hw1_i", "hw0_c", "hw1_c", "hw0_f", "hw1_f", "W"):
+        assert st[k] == eager[k], (label, k)
+
+
+def _backbone(model, i0, i1):
+    """PyTorch backbone of one batch (both images in one pass when their sizes agree) -> c0, c1, f0, f1 float32 numpy"""
     with torch.no_grad():
-        i0 = torch.from_numpy(inp["image0"]).to(backbone_device)
-        i1 = torch.from_numpy(inp["image1"]).to(backbone_device)
         if i0.shape == i1.shape:
             fc, ff = model.backbone(torch.cat([i0, i1], 0))
             (c0, c1), (f0, f1) = fc.split(i0.shape[0]), ff.split(i0.shape[0])
         else:
             (c0, f0), (c1, f1) = model.backbone(i0), model.backbone(i1)
-    npf = lambda t: t.float().cpu().numpy()
-    out = O.hot_path(npf(c0), npf(c1), npf(f0), npf(f1), state, cfg, inp["image0"].shape[2:], inp["image1"].shape[2:],
-                     inp.get("mask0"), inp.get("mask1"), inp.get("scale0"), inp.get("scale1"))
-    return out
+    return [t.float().cpu().numpy() for t in (c0, c1, f0, f1)]
+
+
+def oracle_forward(case, backbone_device="cpu"):
+    """PyTorch backbone (the part that stays PyTorch) + numpy oracle for everything after it."""
+    from oracle import loftr_oracle as O
+    model, cfg, state = build_model(case, backbone_device)
+    inp = build_inputs(case)
+    c0, c1, f0, f1 = _backbone(model, *(torch.from_numpy(inp[k]).to(backbone_device) for k in ("image0", "image1")))
+    return O.hot_path(c0, c1, f0, f1, state, cfg, inp["image0"].shape[2:], inp["image1"].shape[2:],
+                      inp.get("mask0"), inp.get("mask1"), inp.get("scale0"), inp.get("scale1"))
 
 
 def near_tie_top2_f64(x0, x1, mc_cfg, m0=None, m1=None, block=2048):
@@ -98,8 +134,8 @@ def _cache_key(case, adjudicate):
     import json
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     h = hashlib.sha1(json.dumps([case, bool(adjudicate)], sort_keys=True, default=str).encode())
-    for rel in ("oracle/loftr_oracle.py", "tests/golden/weights.py", "tests/golden/cases.py", "loftr_b200/backbone.py",
-                "loftr_b200/config.py"):
+    for rel in ("oracle/loftr_oracle.py", "tests/util.py", "tests/golden/weights.py", "tests/golden/cases.py",
+                "tests/golden/full_cases.py", "loftr_b200/backbone.py", "loftr_b200/config.py"):
         h.update(open(os.path.join(root, rel), "rb").read())
     return h.hexdigest()[:20]
 
@@ -132,18 +168,8 @@ def _oracle_forward_per_pair(case, backbone_device="cpu", adjudicate=True):
     from oracle import loftr_oracle as O
     model, cfg, state = build_model(case, backbone_device)
     inp = build_inputs(case)
-    n = inp["image0"].shape[0]
-    feats = []
-    with torch.no_grad():
-        for b in range(n):
-            i0 = torch.from_numpy(inp["image0"][b:b + 1]).to(backbone_device)
-            i1 = torch.from_numpy(inp["image1"][b:b + 1]).to(backbone_device)
-            if i0.shape == i1.shape:
-                fc, ff = model.backbone(torch.cat([i0, i1], 0))
-                (c0, c1), (f0, f1) = fc.split(1), ff.split(1)
-            else:
-                (c0, f0), (c1, f1) = model.backbone(i0), model.backbone(i1)
-            feats.append([t.float().cpu().numpy() for t in (c0, c1, f0, f1)])
+    feats = [_backbone(model, *(torch.from_numpy(inp[k][b:b + 1]).to(backbone_device) for k in ("image0", "image1")))
+             for b in range(inp["image0"].shape[0])]
     keys = ["b_ids", "i_ids", "j_ids", "mconf", "mkpts0_c", "mkpts1_c", "mkpts0_f", "mkpts1_f"]
     parts = {k: [] for k in keys}
     rows, cols, fc0 = [], [], []

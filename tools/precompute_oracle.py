@@ -14,15 +14,10 @@ for p in (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tests", "golden
     sys.path.insert(0, p)
 import util  # noqa: E402
 from cases import BASELINE_CASES  # noqa: E402
-
-import full_oracle  # noqa: E402
 from full_cases import FULL_BASELINE_CASES  # noqa: E402
 
-names = sys.argv[1:] or list(BASELINE_CASES) + list(FULL_BASELINE_CASES)
-for name in names:
+cases = {**BASELINE_CASES, **FULL_BASELINE_CASES}   # the second: full (softmax) attention, test_full_attention_gpu.py
+for name in sys.argv[1:] or list(cases):
     t0 = time.time()
-    if name in FULL_BASELINE_CASES:   # full (softmax) attention cases of tests/test_full_attention_gpu.py
-        res, gold = full_oracle.oracle_forward_per_pair(FULL_BASELINE_CASES[name])
-    else:
-        res, gold = util.oracle_forward_per_pair(BASELINE_CASES[name], "cpu", adjudicate=name != "b8thr")
+    res, gold = util.oracle_forward_per_pair(cases[name], "cpu", adjudicate=name != "b8thr")
     print(f"{name}: {len(res['b_ids'])} matches, adjudication stats: {gold is not None}, {time.time() - t0:.0f} s", flush=True)
