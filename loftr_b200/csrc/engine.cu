@@ -13,6 +13,7 @@
 #include <mutex>
 #include <string>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/loftr_b200.h"
@@ -52,18 +53,14 @@ static int fail(const char* fmt, ...) {
     if (r__ != 0) return r__; \
   } while (0)
 
-#define LB_LAUNCHED()                 \
-  do {                                \
-    g_launches.fetch_add(1);          \
-    LB_CUDA(cudaGetLastError());      \
-  } while (0)
+static inline int cdiv(long a, long b) { return static_cast<int>((a + b - 1) / b); }
 
 // ------------------------------------------------------------------------------------------------ timing hook
 // Optional per-launch CUDA-event timing of the tensor-core kernels (bench.py's roofline leg), of the per-pair match
 // cap, of the image front end and of the geometry estimator (its three launches as one record): events are recorded on
-// the launching stream right around the kernels, and only while timing is enabled.
-enum Tag { TAG_GEMM_TEST = 0, TAG_PROJ, TAG_MERGE_LN, TAG_MLP1, TAG_MLP2_LN, TAG_SCORE_LSE, TAG_SCORE_ARGMAX,
-           TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_FULL_ATTN, TAG_MATCH_CAP, TAG_PREPROCESS,
+// the launching stream right around the kernels, and only while timing is enabled.  TAG_NONE: not timed.
+enum Tag { TAG_NONE = -1, TAG_GEMM_TEST = 0, TAG_PROJ, TAG_MERGE_LN, TAG_MLP1, TAG_MLP2_LN, TAG_SCORE_LSE,
+           TAG_SCORE_ARGMAX, TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_FULL_ATTN, TAG_MATCH_CAP, TAG_PREPROCESS,
            TAG_GEOMETRY, TAG_COUNT };
 static const char* kTagNames[TAG_COUNT] = {"gemm_test", "proj_act", "merge_ln", "mlp1_relu", "mlp2_ln_res",
                                            "score_lse", "score_argmax", "fine_merge", "backbone_conv",
@@ -76,26 +73,57 @@ struct TimingRec {
 static bool g_timing = false;
 static std::vector<TimingRec> g_recs;
 static std::mutex g_timing_mu;
-// Around a launch on `st`: events are only created and recorded while timing is enabled.
-static int timing_begin(TimingRec& rec, cudaStream_t st) {
-  if (!g_timing) return 0;
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  cudaError_t e = cudaStreamIsCapturing(st, &cs);
-  if (e != cudaSuccess) return fail("cudaStreamIsCapturing failed: %s", cudaGetErrorString(e));
-  if (cs != cudaStreamCaptureStatusNone)
-    return fail("kernel timing is enabled (lb_timing_enable) but the stream is being captured into a CUDA graph: "
-                "timing events cannot be recorded into a graph; disable timing before capture");
-  if (cudaEventCreate(&rec.e0) != cudaSuccess || cudaEventCreate(&rec.e1) != cudaSuccess ||
-      cudaEventRecord(rec.e0, st) != cudaSuccess)
-    return fail("timing event set-up failed");
-  return 0;
-}
-static int timing_end(const TimingRec& rec, cudaStream_t st) {
-  if (!g_timing) return 0;
-  if (cudaEventRecord(rec.e1, st) != cudaSuccess) return fail("timing event record failed");
-  std::lock_guard<std::mutex> lk(g_timing_mu);
-  g_recs.push_back(rec);
-  return 0;
+// One timing record over the launches issued on `st` between begin() and end(); events are only created and recorded
+// while timing is enabled, and never for TAG_NONE.
+struct TimedRange {
+  TimingRec rec{nullptr, nullptr, TAG_NONE};
+  cudaStream_t st = nullptr;
+  int begin(int tag, cudaStream_t stream) {
+    if (!g_timing || tag == TAG_NONE) return 0;
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    cudaError_t e = cudaStreamIsCapturing(stream, &cs);
+    if (e != cudaSuccess) return fail("cudaStreamIsCapturing failed: %s", cudaGetErrorString(e));
+    if (cs != cudaStreamCaptureStatusNone)
+      return fail("kernel timing is enabled (lb_timing_enable) but the stream is being captured into a CUDA graph: "
+                  "timing events cannot be recorded into a graph; disable timing before capture");
+    if (cudaEventCreate(&rec.e0) != cudaSuccess || cudaEventCreate(&rec.e1) != cudaSuccess ||
+        cudaEventRecord(rec.e0, stream) != cudaSuccess)
+      return fail("timing event set-up failed");
+    rec.tag = tag;
+    st = stream;
+    return 0;
+  }
+  int end() {
+    if (rec.tag == TAG_NONE) return 0;
+    if (cudaEventRecord(rec.e1, st) != cudaSuccess) return fail("timing event record failed");
+    std::lock_guard<std::mutex> lk(g_timing_mu);
+    g_recs.push_back(rec);
+    return 0;
+  }
+};
+
+// Every kernel launch: `kern` over grid x block with `smem` bytes of dynamic shared memory on `st`, counted by
+// lb_launch_count() and, with a tag, timed as one record.  kPdl: programmatic dependent launch (the kernel's set-up
+// overlaps the previous kernel's tail).
+template <bool kPdl = false, class... Params, class... Args>
+static int launch(int tag, void (*kern)(Params...), dim3 grid, dim3 block, int smem, cudaStream_t st, Args&&... args) {
+  TimedRange t;
+  LB_TRY(t.begin(tag, st));
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = kPdl ? 1 : 0;
+  cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);   // its error is returned and cleared by cudaGetLastError
+  g_launches.fetch_add(1);
+  LB_CUDA(cudaGetLastError());
+  return t.end();
 }
 
 // The library carries its own (static) CUDA runtime, whose notion of "current device" is independent of the
@@ -103,11 +131,11 @@ static int timing_end(const TimingRec& rec, cudaStream_t st) {
 // buffers it was given -- otherwise a process working on cuda:1 would launch on device 0 through the legacy
 // default stream.
 // The previous device of the calling thread is restored when the entry point returns (RAII), so a caller whose
-// current device differs from the buffers' device is left undisturbed.
+// current device differs from the buffers' device is left undisturbed.  Binding also checks that the device is an
+// sm_90 one and gives its SM count (`sms`).
 constexpr int kMaxDevices = 64;
-struct DeviceGuard {
-  int prev = -1;
-  bool switched = false;
+struct DeviceScope {
+  int sms = 0;
   int bind(const void* dev_ptr) {
     if (!dev_ptr) return fail("null device pointer");
     cudaPointerAttributes attr;
@@ -118,38 +146,38 @@ struct DeviceGuard {
     }
     if (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged)
       return fail("expected a CUDA device pointer; loftr_b200 has no CPU fallback");
+    return bind_device(attr.device);
+  }
+  int bind_device(int device) {
     LB_CUDA(cudaGetDevice(&prev));
-    if (prev != attr.device) {
-      LB_CUDA(cudaSetDevice(attr.device));
+    if (prev != device) {
+      LB_CUDA(cudaSetDevice(device));
       switched = true;
     }
+    if (device < 0 || device >= kMaxDevices) return fail("device index %d out of range", device);
+    static std::mutex mu;
+    static int count[kMaxDevices] = {0};
+    std::lock_guard<std::mutex> lk(mu);
+    if (count[device] == 0) {
+      cudaDeviceProp prop;
+      cudaError_t e = cudaGetDeviceProperties(&prop, device);
+      if (e != cudaSuccess) return fail("cudaGetDeviceProperties: %s", cudaGetErrorString(e));
+      if (prop.major != 9 || prop.minor != 0)
+        return fail("loftr_b200 requires an sm_90 (H100) device, found sm_%d%d; there is no fallback", prop.major,
+                    prop.minor);
+      count[device] = prop.multiProcessorCount;
+    }
+    sms = count[device];
     return 0;
   }
-  ~DeviceGuard() {
+  ~DeviceScope() {
     if (switched) cudaSetDevice(prev);
   }
-};
 
-static int device_check(int* sm_count) {
-  static std::mutex mu;
-  static int sms[kMaxDevices] = {0};
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return fail("no CUDA device: %s", cudaGetErrorString(e));
-  if (dev < 0 || dev >= kMaxDevices) return fail("device index %d out of range", dev);
-  std::lock_guard<std::mutex> lk(mu);
-  if (sms[dev] == 0) {
-    cudaDeviceProp prop;
-    e = cudaGetDeviceProperties(&prop, dev);
-    if (e != cudaSuccess) return fail("cudaGetDeviceProperties: %s", cudaGetErrorString(e));
-    if (prop.major != 9 || prop.minor != 0)
-      return fail("loftr_b200 requires an sm_90 (H100) device, found sm_%d%d; there is no fallback", prop.major,
-                  prop.minor);
-    sms[dev] = prop.multiProcessorCount;
-  }
-  *sm_count = sms[dev];
-  return 0;
-}
+ private:
+  int prev = -1;
+  bool switched = false;
+};
 
 // Allows `Kernel` up to `bytes` of dynamic shared memory on the current device (needed above 48 KB); the attribute is
 // set on the first launch per device.
@@ -257,18 +285,43 @@ static int make_out_map_nhwc(CUtensorMap* m, const void* base, bool f32, int C, 
   return encode_map(m, "NHWC output", base, f32, 4, dims, strides, box, nullptr, out_swizzle(f32),
                     CU_TENSOR_MAP_L2_PROMOTION_NONE);
 }
+
+// The map `make` builds over the hi plane and, for data held as two planes, the one over the lo plane.  With one plane
+// the lo map is a copy of the hi map, which the kernels never read (lo may be null).
+template <auto make, class... Args>
+static int map_planes(int planes, CUtensorMap* m_hi, CUtensorMap* m_lo, const void* hi, const void* lo, Args... args) {
+  LB_TRY(make(m_hi, hi, args...));
+  if (planes == 2) return make(m_lo, lo, args...);
+  *m_lo = *m_hi;
+  return 0;
+}
+
 // planes (+ optional fp32) of a [batches][rows][cols] output
 static int fill_out_maps(OutMaps* om, const void* hi, const void* lo, long ld_pl, const float* f32, long ld_f32, long cols,
                          long rows, long batches) {
   memset(om, 0, sizeof(*om));
   om->dims = 3;
   if (hi) {
-    LB_TRY(make_out_map(&om->hi, hi, false, cols, rows, batches, ld_pl, 0));
-    LB_TRY(make_out_map(&om->lo, lo, false, cols, rows, batches, ld_pl, 0));
+    LB_TRY(map_planes<make_out_map>(2, &om->hi, &om->lo, hi, lo, false, cols, rows, batches, ld_pl, 0L));
     om->use |= 1;
   }
   if (f32) {
     LB_TRY(make_out_map(&om->f32, f32, true, cols, rows, batches, ld_f32, 0));
+    om->use |= 2;
+  }
+  return 0;
+}
+// `planes` fp16 planes (+ optional fp32) of an NHWC [N][H][W][C] output
+static int fill_out_maps_nhwc(OutMaps* om, int planes, const void* hi, const void* lo, long ld_pl, const float* f32,
+                              long ld_f32, int C, int W, int H, int N) {
+  memset(om, 0, sizeof(*om));
+  om->dims = 4;
+  if (hi) {
+    LB_TRY(map_planes<make_out_map_nhwc>(planes, &om->hi, &om->lo, hi, lo, false, C, W, H, N, ld_pl));
+    om->use |= 1;
+  }
+  if (f32) {
+    LB_TRY(make_out_map_nhwc(&om->f32, f32, true, C, W, H, N, ld_f32));
     om->use |= 2;
   }
   return 0;
@@ -293,32 +346,14 @@ static int launch_persistent(int tag, const GemmShape& s, int smem_bytes, int sm
   LB_TRY(set_max_dynamic_smem<kern>(smem_bytes));
   const long items = static_cast<long>(s.batches) * s.m_tiles * s.n_chunks;
   const int grid = static_cast<int>(items < sms ? items : sms);
-  TimingRec rec{nullptr, nullptr, tag};
-  LB_TRY(timing_begin(rec, st));
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = smem_bytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  cfg.attrs = attr;
-  cfg.numAttrs = 0;
   // programmatic dependent launch of the tensor-core kernels (gemm_split.cuh): the next kernel's set-up overlaps this
   // one's tail.  LOFTR_B200_PDL=0 disables it.
-  static int pdl = -1;
-  if (pdl < 0) {
+  static const bool pdl = [] {
     const char* e = getenv("LOFTR_B200_PDL");
-    pdl = e ? (atoi(e) != 0 ? 1 : 0) : 1;
-  }
-  if (pdl) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.numAttrs = 1;
-  }
-  LB_CUDA(cudaLaunchKernelEx(&cfg, kern, args...));
-  LB_LAUNCHED();
-  return timing_end(rec, st);
+    return !e || atoi(e) != 0;
+  }();
+  return pdl ? launch<true>(tag, kern, grid, kGemmThreads, smem_bytes, st, args...)
+             : launch<false>(tag, kern, grid, kGemmThreads, smem_bytes, st, args...);
 }
 
 template <int BN, class Epi>
@@ -331,51 +366,52 @@ static int launch_raw(int tag, const GemmMaps& maps, const GemmShape& s, const t
                                                           maps.b_lo, maps.ar_hi, maps.ar_lo, maps.br_hi, maps.br_lo, s, ep);
 }
 
-// live / live_unit_rows: optional device bound on the rows of every batch (GemmShape::live_count)
-template <int BN, class Epi>
-static int launch_gemm(int tag, const Planes& A, const Planes& B, int batches, int M, int N, int K, int n_chunks,
-                       const typename Epi::Params& ep, cudaStream_t st, const int* live = nullptr,
-                       int live_unit_rows = 0) {
-  int sms = 0;
-  LB_TRY(device_check(&sms));
-  if (K % kBlockK != 0 || K <= 0) return fail("K=%d must be a positive multiple of %d", K, kBlockK);
-  if (M <= 0 || N <= 0 || batches <= 0) return 0;  // nothing to do
-  if (live && !EpiRowBound<Epi>::value) return fail("this GEMM epilogue is built without a device row bound");
+// The work split of `batches` M x N x K products in BN-wide n tiles: each work item sweeps one chunk of n tiles, with
+// the n tiles split into n_chunks chunks (0: one tile per chunk).  b_batched: B holds one matrix per batch.
+// live / live_unit_rows: optional device bound on the rows of every batch (GemmShape::live_count).
+template <int BN>
+static GemmShape gemm_shape(int batches, int M, int N, int K, bool b_batched = false, int n_chunks = 0,
+                            const int* live = nullptr, int live_unit_rows = 0) {
   GemmShape s;
   s.batches = batches;
   s.M = M;
   s.N = N;
   s.K = K;
-  s.b_batched = B.batch_stride > 0 ? 1 : 0;
-  s.m_tiles = (M + kBlockM - 1) / kBlockM;
-  s.n_tiles = (N + BN - 1) / BN;
+  s.b_batched = b_batched ? 1 : 0;
+  s.m_tiles = cdiv(M, kBlockM);
+  s.n_tiles = cdiv(N, BN);
   if (n_chunks <= 0 || n_chunks > s.n_tiles) n_chunks = s.n_tiles;
-  s.tiles_per_chunk = (s.n_tiles + n_chunks - 1) / n_chunks;
-  s.n_chunks = (s.n_tiles + s.tiles_per_chunk - 1) / s.tiles_per_chunk;
+  s.tiles_per_chunk = n_chunks > 0 ? cdiv(s.n_tiles, n_chunks) : 1;   // no n tiles: nothing is launched
+  s.n_chunks = cdiv(s.n_tiles, s.tiles_per_chunk);
   s.conv = ConvGeom{0, 0, 0, 0, 0, 0, 0, 0, 0};
   s.live_count = live;
   s.live_unit_rows = live_unit_rows;
+  return s;
+}
 
-  // one operand plane: the lo maps are copies of the hi ones and never loaded (A.lo / B.lo may be null)
-  constexpr bool kLo = EpiOperandPlanes<Epi>::value == 2;
-  constexpr int kBK = GemmSmem<BN, Epi::kSmemBytes, EpiOperandPlanes<Epi>::value>::kBK;
+template <int BN, class Epi>
+static int launch_gemm(int tag, const Planes& A, const Planes& B, const GemmShape& s, const typename Epi::Params& ep,
+                       int sms, cudaStream_t st) {
+  if (s.K % kBlockK != 0 || s.K <= 0) return fail("K=%d must be a positive multiple of %d", s.K, kBlockK);
+  if (s.M <= 0 || s.N <= 0 || s.batches <= 0) return 0;  // nothing to do
+  if (s.live_count && !EpiRowBound<Epi>::value) return fail("this GEMM epilogue is built without a device row bound");
+  constexpr int kP = EpiOperandPlanes<Epi>::value;
+  constexpr int kBK = GemmSmem<BN, Epi::kSmemBytes, kP>::kBK;
   GemmMaps mp;
-  LB_TRY(make_map(&mp.a_hi, A.hi, K, M, batches, A.ld, A.batch_stride, kBlockM, kBK));
-  mp.a_lo = mp.a_hi;
-  if (kLo) LB_TRY(make_map(&mp.a_lo, A.lo, K, M, batches, A.ld, A.batch_stride, kBlockM, kBK));
-  const int bb = s.b_batched ? batches : 1;
-  LB_TRY(make_map(&mp.b_hi, B.hi, K, N, bb, B.ld, B.batch_stride, BN, kBK));
-  mp.b_lo = mp.b_hi;
-  if (kLo) LB_TRY(make_map(&mp.b_lo, B.lo, K, N, bb, B.ld, B.batch_stride, BN, kBK));
+  LB_TRY(map_planes<make_map>(kP, &mp.a_hi, &mp.a_lo, A.hi, A.lo, s.K, s.M, s.batches, A.ld, A.batch_stride, kBlockM,
+                              kBK));
+  const int bb = s.b_batched ? s.batches : 1;
+  LB_TRY(map_planes<make_map>(kP, &mp.b_hi, &mp.b_lo, B.hi, B.lo, s.K, s.N, bb, B.ld, B.batch_stride, BN, kBK));
   mp.ar_hi = mp.a_hi; mp.ar_lo = mp.a_lo; mp.br_hi = mp.b_hi; mp.br_lo = mp.b_lo;
   return launch_raw<BN, Epi>(tag, mp, s, ep, sms, st);
 }
 
 // Implicit-GEMM convolution launch: in = NHWC planes [N, H_in, W_in, ld_in] with Cin valid channels; weights =
 // main planes [Cout, taps * cin_blocks * 64] (+ remainder planes [Cout, taps * 16], see lb_conv_layout); out pixel
-// grid H_out x W_out.
+// grid H_out x W_out; cin_blocks / rem: the K layout of conv_layout.
 struct ConvDesc {
   int N, H_in, W_in, Cin, H_out, W_out, Cout, ksize, stride, pad;
+  int cin_blocks, rem;
 };
 // K layout of a convolution's implicit GEMM: `cin_blocks` 64-channel blocks per tap, plus `rem` (<= 16) remainder
 // channels per tap that travel as 16-channel boxes (gemm_split.cuh ConvGeom).
@@ -390,23 +426,21 @@ static void conv_layout(int cin, int* cin_blocks, int* rem) {
   }
 }
 // The implicit GEMM of convolution d with BN-wide n tiles (one per work item), and the output geometry its epilogue
-// reads.  *rem: the remainder channels per tap (0: none).  lo: the weights have lo planes (split precision).
-// rem_taps_per_group: taps of one remainder group (ConvGeom::rem_groups).
+// reads.  lo: the weights have lo planes (split precision).  rem_taps_per_group: taps of one remainder group
+// (ConvGeom::rem_groups).
 template <int BN, class Params>
 static int conv_shape(const ConvDesc& d, const Planes& wgt_rem, bool lo, int rem_taps_per_group, GemmShape* s,
-                      Params* ep, int* rem) {
-  int cin_blocks = 0;
-  conv_layout(d.Cin, &cin_blocks, rem);
-  if (*rem && (!wgt_rem.hi || (lo && !wgt_rem.lo)))
+                      Params* ep) {
+  if (d.rem && (!wgt_rem.hi || (lo && !wgt_rem.lo)))
     return fail("convolution with Cin=%d needs remainder weight planes", d.Cin);
   const int taps = d.ksize * d.ksize;
   const int tiles_h = (d.H_out + kConvTileH - 1) / kConvTileH;
   const int tiles_w = (d.W_out + kConvTileW - 1) / kConvTileW;
   const int m_tiles = tiles_h * tiles_w, n_tiles = (d.Cout + BN - 1) / BN;
-  const int rem_groups = *rem ? (taps + rem_taps_per_group - 1) / rem_taps_per_group : 0;
-  *s = GemmShape{d.N, m_tiles * kBlockM, d.Cout, taps * cin_blocks * kBlockK, /*b_batched=*/0, m_tiles, n_tiles,
+  const int rem_groups = d.rem ? (taps + rem_taps_per_group - 1) / rem_taps_per_group : 0;
+  *s = GemmShape{d.N, m_tiles * kBlockM, d.Cout, taps * d.cin_blocks * kBlockK, /*b_batched=*/0, m_tiles, n_tiles,
                  /*n_chunks=*/n_tiles, /*tiles_per_chunk=*/1,
-                 ConvGeom{1, tiles_w, d.stride, d.pad, d.ksize, cin_blocks, taps, taps * cin_blocks, rem_groups},
+                 ConvGeom{1, tiles_w, d.stride, d.pad, d.ksize, d.cin_blocks, taps, taps * d.cin_blocks, rem_groups},
                  /*live_count=*/nullptr, 0};
   ep->H_out = d.H_out;
   ep->W_out = d.W_out;
@@ -418,31 +452,21 @@ static int conv_shape(const ConvDesc& d, const Planes& wgt_rem, bool lo, int rem
 // maps are copies of the hi ones and never loaded)
 template <int BN, class Epi>
 static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_rem, const ConvDesc& d,
-                       const typename Epi::Params& ep_in, cudaStream_t st) {
-  constexpr bool kLo = EpiOperandPlanes<Epi>::value == 2;
-  using S = GemmSmem<BN, Epi::kSmemBytes, EpiOperandPlanes<Epi>::value>;
-  int sms = 0;
-  LB_TRY(device_check(&sms));
+                       const typename Epi::Params& ep_in, int sms, cudaStream_t st) {
+  constexpr int kP = EpiOperandPlanes<Epi>::value;
+  using S = GemmSmem<BN, Epi::kSmemBytes, kP>;
   GemmShape s;
   typename Epi::Params ep = ep_in;
-  int rem = 0;
-  LB_TRY(conv_shape<BN>(d, wgt_rem, kLo, S::kRemTapsPerStage, &s, &ep, &rem));
+  LB_TRY(conv_shape<BN>(d, wgt_rem, kP == 2, S::kRemTapsPerStage, &s, &ep));
   GemmMaps mp;
-  LB_TRY(make_map_nhwc(&mp.a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, S::kBK));
-  LB_TRY(make_map(&mp.b_hi, wgt.hi, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
-  mp.a_lo = mp.a_hi; mp.b_lo = mp.b_hi;
-  if (kLo) {
-    LB_TRY(make_map_nhwc(&mp.a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, S::kBK));
-    LB_TRY(make_map(&mp.b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
-  }
-  if (rem) {
-    LB_TRY(make_map_nhwc(&mp.ar_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, kRemChannels));
-    LB_TRY(make_map(&mp.br_hi, wgt_rem.hi, s.conv.taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
-    mp.ar_lo = mp.ar_hi; mp.br_lo = mp.br_hi;
-    if (kLo) {
-      LB_TRY(make_map_nhwc(&mp.ar_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride, kRemChannels));
-      LB_TRY(make_map(&mp.br_lo, wgt_rem.lo, s.conv.taps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
-    }
+  LB_TRY(map_planes<make_map_nhwc>(kP, &mp.a_hi, &mp.a_lo, in.hi, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld, d.stride,
+                                   S::kBK));
+  LB_TRY(map_planes<make_map>(kP, &mp.b_hi, &mp.b_lo, wgt.hi, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
+  if (d.rem) {
+    LB_TRY(map_planes<make_map_nhwc>(kP, &mp.ar_hi, &mp.ar_lo, in.hi, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld,
+                                     d.stride, kRemChannels));
+    LB_TRY(map_planes<make_map>(kP, &mp.br_hi, &mp.br_lo, wgt_rem.hi, wgt_rem.lo, s.conv.taps * kRemChannels, d.Cout,
+                                1, wgt_rem.ld, 0, BN, kRemChannels));
   } else {
     mp.ar_hi = mp.a_hi; mp.ar_lo = mp.a_lo; mp.br_hi = mp.b_hi; mp.br_lo = mp.b_lo;
   }
@@ -452,30 +476,20 @@ static int launch_conv(const Planes& in, const Planes& wgt, const Planes& wgt_re
 // Stride-1 3x3 convolution through conv3x3_halo_kernel (same operands, weights and epilogue as launch_conv).
 template <int BN, class Epi>
 static int launch_conv_halo(const Planes& in, const Planes& wgt, const Planes& wgt_rem, const ConvDesc& d,
-                            const typename Epi::Params& ep_in, cudaStream_t st) {
-  constexpr bool kLo = EpiOperandPlanes<Epi>::value == 2;
-  using S = HaloSmem<BN, Epi::kSmemBytes, EpiOperandPlanes<Epi>::value>;
+                            const typename Epi::Params& ep_in, int sms, cudaStream_t st) {
+  constexpr int kP = EpiOperandPlanes<Epi>::value;
+  using S = HaloSmem<BN, Epi::kSmemBytes, kP>;
   static_assert(S::kTotalBytes <= kSmemLimit, "shared memory budget exceeded");
-  int sms = 0;
-  LB_TRY(device_check(&sms));
   if (d.ksize != 3 || d.stride != 1 || d.pad != 1) return fail("the halo convolution is built for 3x3, stride 1, pad 1");
   GemmShape s;
   typename Epi::Params ep = ep_in;
-  int rem = 0;
-  LB_TRY(conv_shape<BN>(d, wgt_rem, kLo, kHaloTaps, &s, &ep, &rem));   // the remainder is one 16-channel halo
+  LB_TRY(conv_shape<BN>(d, wgt_rem, kP == 2, kHaloTaps, &s, &ep));   // the remainder is one 16-channel halo
   CUtensorMap a_hi, a_lo, b_hi, b_lo, br_hi, br_lo;
-  LB_TRY(make_map_halo(&a_hi, in.hi, d.Cin, d.W_in, d.H_in, d.N, in.ld));
-  LB_TRY(make_map(&b_hi, wgt.hi, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
-  a_lo = a_hi;
-  b_lo = b_hi;
-  if (kLo) {
-    LB_TRY(make_map_halo(&a_lo, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld));
-    LB_TRY(make_map(&b_lo, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
-  }
-  if (rem) {
-    LB_TRY(make_map(&br_hi, wgt_rem.hi, kHaloTaps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
-    br_lo = br_hi;
-    if (kLo) LB_TRY(make_map(&br_lo, wgt_rem.lo, kHaloTaps * kRemChannels, d.Cout, 1, wgt_rem.ld, 0, BN, kRemChannels));
+  LB_TRY(map_planes<make_map_halo>(kP, &a_hi, &a_lo, in.hi, in.lo, d.Cin, d.W_in, d.H_in, d.N, in.ld));
+  LB_TRY(map_planes<make_map>(kP, &b_hi, &b_lo, wgt.hi, wgt.lo, s.K, d.Cout, 1, wgt.ld, 0, BN, S::kBK));
+  if (d.rem) {
+    LB_TRY(map_planes<make_map>(kP, &br_hi, &br_lo, wgt_rem.hi, wgt_rem.lo, kHaloTaps * kRemChannels, d.Cout, 1,
+                                wgt_rem.ld, 0, BN, kRemChannels));
   } else {
     br_hi = b_hi;
     br_lo = b_lo;
@@ -514,8 +528,6 @@ struct Bump {
   }
 };
 
-static inline int cdiv(long a, long b) { return static_cast<int>((a + b - 1) / b); }
-
 // ------------------------------------------------------------------------------------------------ transformer
 struct TfWs {
   float* qkv;       // fine only: [R, 3C]
@@ -524,12 +536,28 @@ struct TfWs {
   __half* h_hi;     // [R, 2C]
   __half* h_lo;
   float* kv;        // coarse only: [2*n_groups, H, D*D + D]
-  float* kv_part;   // coarse only: [2*n_groups, max(m_tiles, kKvSplits), H, per] (K^T V split partials)
+  float* kv_part;   // coarse only: [2*n_groups, KvSplits::parts, H, per] (K^T V split partials)
 };
-// kv_gemm_kernel sums K^T V over at most max(m_tiles, kKvSplits) row splits per group.  That bound sizes kv_part here
-// and caps `splits` in tf_linear_attention_coarse; `splits` fixes the summation order of K^T V, so changing either
-// formula changes the output bits.
+// The row splits over which kv_gemm_kernel sums K^T V for n_groups groups of group_rows rows on `sms` SMs (64-row
+// blocks, kb_per of them per split).  parts = max(m_tiles, kKvSplits) bounds `splits` on every device and sizes
+// TfWs::kv_part; the workspace size needs only `parts` and passes sms = 0.  `splits` fixes the summation order of
+// K^T V, so changing this plan changes the output bits.
 constexpr int kKvSplits = 8;
+struct KvSplits {
+  int parts, kb_total, kb_per, splits;
+};
+static KvSplits kv_splits(int group_rows, int n_groups, int sms) {
+  const int m_tiles = cdiv(group_rows, kBlockM);
+  KvSplits k{m_tiles > kKvSplits ? m_tiles : kKvSplits, cdiv(group_rows, 64), 0, 0};
+  if (sms <= 0) return k;
+  int splits = sms / (2 * n_groups);
+  if (splits < 1) splits = 1;
+  if (splits > k.kb_total) splits = k.kb_total;
+  if (splits > k.parts) splits = k.parts;
+  k.kb_per = cdiv(k.kb_total, splits);
+  k.splits = cdiv(k.kb_total, k.kb_per);
+  return k;
+}
 
 // Operand planes of the transformer and score-matrix products: 2 = split precision (hi*hi + hi*lo + lo*hi), 1 = the hi
 // planes only, one fp16 MMA per product (match_precision "fp16": lb_transformer_forward_fp16 / lb_coarse_match_fp16,
@@ -546,17 +574,9 @@ static void carve_tf(Bump& b, TfWs& w, int C, int H, long R, int n_groups, bool 
   w.h_hi = b.take<__half>(static_cast<size_t>(R) * 2 * C);
   w.h_lo = b.take<__half>(static_cast<size_t>(R) * 2 * C);
   w.kv = coarse ? b.take<float>(static_cast<size_t>(2) * n_groups * H * (D * D + D)) : nullptr;
-  const size_t tiles = static_cast<size_t>((max_group_rows + kBlockM - 1) / kBlockM);
-  const size_t parts = tiles > static_cast<size_t>(kKvSplits) ? tiles : static_cast<size_t>(kKvSplits);
+  const size_t parts = static_cast<size_t>(kv_splits(max_group_rows, n_groups, 0).parts);
   w.kv_part = coarse ? b.take<float>(static_cast<size_t>(2) * n_groups * H * parts * (D * D + D)) : nullptr;
 }
-
-template <int BN, int kP>
-static int tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st, const TfWs& w,
-                         long x_base, long x_rows, int x_group_rows, long s_base, long s_rows, int s_group_rows,
-                         int n_groups_x, bool self_pass, bool write_f32, cudaStream_t stream, const int* live,
-                         int live_cap, bool full);
-
 
 // ------------------------------------------------------------------------------------------------ backbone
 // ResNetFPN_8_2 forward (reference src/loftr/backbone/resnet_fpn.py:43-118) on tensor cores: every 3x3 / 1x1
@@ -608,9 +628,41 @@ struct ConvRun {
   float* out_f32;
   int f32_ld;
 };
+// The kernel of a convolution and its output-channel tile BN.  Stride-1 3x3 convolutions (none of them carries the FPN
+// upsample-add) run conv3x3_halo_kernel, which loads each input patch once per channel block; the others the implicit
+// GEMM.  BN is the smallest built N that covers Cout: 196 -> 200 in the halo kernel (one m64n200 wgmma per x-half);
+// 208 in gemm_split_kernel, whose two column halves need N / 2 to be a wgmma N (104 = 13 x 8).  0: none is built.
+struct ConvKernel {
+  bool halo;
+  int bn;
+};
+static ConvKernel conv_kernel(const LbConvWeights& w, bool up) {
+  const bool halo = w.ksize == 3 && w.stride == 1 && !up;
+  const int mid = halo ? 200 : 208;
+  return {halo, w.cout <= 128 ? 128 : w.cout <= mid ? mid : w.cout <= 256 ? 256 : 0};
+}
+
+// One convolution on the kernel and tile conv_kernel picked; the epilogue type of the tile width and FPN mode also
+// selects the kernels' operand planes.
+template <int kPlanes, bool kHalo, int BN, bool kUp>
+static int launch_conv_on(const ConvRun& r, const ConvDesc& d, const OutMaps& om, int sms, cudaStream_t st) {
+  using Epi = std::conditional_t<kPlanes == 2, EpiConv<BN, kUp>, EpiConvF16<BN, kUp>>;
+  const LbConvWeights& w = *r.w;
+  const int taps = w.ksize * w.ksize;
+  const Planes in{r.in.hi, r.in.lo, r.in.ld, 0};
+  const Planes wg{w.w_hi, w.w_lo, static_cast<long>(taps) * d.cin_blocks * kBlockK, 0};
+  const Planes wr{w.wr_hi, w.wr_lo, static_cast<long>(taps) * kRemChannels, 0};
+  typename Epi::Params ep{w.scale, w.shift, r.act, r.res ? r.res->hi : nullptr, r.res ? r.res->lo : nullptr,
+                          r.res ? r.res->ld : 0, r.up ? r.up->hi : nullptr, r.up ? r.up->lo : nullptr,
+                          r.up ? r.up->ld : 0, r.up_h, r.up_w, r.out ? r.out->hi : nullptr,
+                          r.out ? r.out->lo : nullptr, r.out ? r.out->ld : 0, r.out_f32, r.f32_ld, 0, 0, 0, om};
+  if constexpr (kHalo) return launch_conv_halo<BN, Epi>(in, wg, wr, d, ep, sms, st);
+  else return launch_conv<BN, Epi>(in, wg, wr, d, ep, sms, st);
+}
+
 // kPlanes = 2: the split-precision convolution (EpiConv); 1: single fp16 planes (EpiConvF16, w_lo / wr_lo unused)
 template <int kPlanes>
-static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
+static int run_conv(const ConvRun& r, int N, int sms, cudaStream_t st) {
   const LbConvWeights& w = *r.w;
   ConvDesc d;
   d.N = N; d.H_in = r.H_in; d.W_in = r.W_in; d.Cin = w.cin;
@@ -618,57 +670,31 @@ static int run_conv(const ConvRun& r, int N, cudaStream_t st) {
   d.H_out = (r.H_in + 2 * d.pad - w.ksize) / w.stride + 1;
   d.W_out = (r.W_in + 2 * d.pad - w.ksize) / w.stride + 1;
   d.Cout = w.cout;
-  int cin_blocks = 0, rem = 0;
-  conv_layout(w.cin, &cin_blocks, &rem);
-  const int taps = w.ksize * w.ksize;
-  Planes in{r.in.hi, r.in.lo, r.in.ld, 0};
-  Planes wg{w.w_hi, w.w_lo, static_cast<long>(taps) * cin_blocks * kBlockK, 0};
-  Planes wr{w.wr_hi, w.wr_lo, static_cast<long>(taps) * kRemChannels, 0};
+  conv_layout(w.cin, &d.cin_blocks, &d.rem);
   // NHWC output maps of the TMA-store epilogue (planes and / or fp32 feature map)
   OutMaps om;
-  memset(&om, 0, sizeof(om));
-  om.dims = 4;
-  if (r.out) {
-    LB_TRY(make_out_map_nhwc(&om.hi, r.out->hi, false, d.Cout, d.W_out, d.H_out, N, r.out->ld));
-    if (kPlanes == 2) LB_TRY(make_out_map_nhwc(&om.lo, r.out->lo, false, d.Cout, d.W_out, d.H_out, N, r.out->ld));
-    om.use |= 1;
+  LB_TRY(fill_out_maps_nhwc(&om, kPlanes, r.out ? r.out->hi : nullptr, r.out ? r.out->lo : nullptr,
+                            r.out ? r.out->ld : 0, r.out_f32, r.f32_ld, d.Cout, d.W_out, d.H_out, N));
+  const ConvKernel k = conv_kernel(w, r.up != nullptr);
+  if (k.halo) {
+    switch (k.bn) {
+      case 128: return launch_conv_on<kPlanes, true, 128, false>(r, d, om, sms, st);
+      case 200: return launch_conv_on<kPlanes, true, 200, false>(r, d, om, sms, st);
+      case 256: return launch_conv_on<kPlanes, true, 256, false>(r, d, om, sms, st);
+    }
+  } else if (r.up) {
+    switch (k.bn) {
+      case 128: return launch_conv_on<kPlanes, false, 128, true>(r, d, om, sms, st);
+      case 208: return launch_conv_on<kPlanes, false, 208, true>(r, d, om, sms, st);
+      case 256: return launch_conv_on<kPlanes, false, 256, true>(r, d, om, sms, st);
+    }
+  } else {
+    switch (k.bn) {
+      case 128: return launch_conv_on<kPlanes, false, 128, false>(r, d, om, sms, st);
+      case 208: return launch_conv_on<kPlanes, false, 208, false>(r, d, om, sms, st);
+      case 256: return launch_conv_on<kPlanes, false, 256, false>(r, d, om, sms, st);
+    }
   }
-  if (r.out_f32) {
-    LB_TRY(make_out_map_nhwc(&om.f32, r.out_f32, true, d.Cout, d.W_out, d.H_out, N, r.f32_ld));
-    om.use |= 2;
-  }
-  // stride-1 3x3 convolutions (none of them carries the FPN upsample-add) load each input patch once per channel block
-  const bool halo = w.ksize == 3 && w.stride == 1 && !r.up;
-  // the epilogue type of the tile width and FPN mode: it also selects the kernels' operand planes
-#define LB_CONV_EPI(BN, UP) std::conditional_t<kPlanes == 2, EpiConv<BN, UP>, EpiConvF16<BN, UP>>
-#define LB_CONV_CASE_UP(BN, UP, LAUNCH)                                                                               \
-  {                                                                                                                   \
-    using Epi = LB_CONV_EPI(BN, UP);                                                                                  \
-    typename Epi::Params ep{w.scale, w.shift, r.act, r.res ? r.res->hi : nullptr, r.res ? r.res->lo : nullptr,        \
-                            r.res ? r.res->ld : 0, r.up ? r.up->hi : nullptr, r.up ? r.up->lo : nullptr,             \
-                            r.up ? r.up->ld : 0, r.up_h, r.up_w, r.out ? r.out->hi : nullptr,                         \
-                            r.out ? r.out->lo : nullptr, r.out ? r.out->ld : 0, r.out_f32, r.f32_ld, 0, 0, 0, om};    \
-    return LAUNCH<BN, Epi>(in, wg, wr, d, ep, st);                                                                    \
-  }
-#define LB_CONV_CASE(BN)                                                                                              \
-  {                                                                                                                   \
-    if (r.up) LB_CONV_CASE_UP(BN, true, launch_conv)                                                                  \
-    LB_CONV_CASE_UP(BN, false, launch_conv)                                                                           \
-  }
-  // output-channel tile: the smallest built N that covers Cout.  196 -> 200 in the halo kernel (one m64n200 wgmma per
-  // x-half); 208 in gemm_split_kernel, whose two column halves need N / 2 to be a wgmma N (104 = 13 x 8)
-  if (halo) {
-    if (w.cout <= 128) LB_CONV_CASE_UP(128, false, launch_conv_halo)
-    if (w.cout <= 200) LB_CONV_CASE_UP(200, false, launch_conv_halo)
-    if (w.cout <= 256) LB_CONV_CASE_UP(256, false, launch_conv_halo)
-    return fail("convolutions with more than 256 output channels are not built");
-  }
-  if (w.cout <= 128) LB_CONV_CASE(128)
-  if (w.cout <= 208) LB_CONV_CASE(208)
-  if (w.cout <= 256) LB_CONV_CASE(256)
-#undef LB_CONV_CASE
-#undef LB_CONV_CASE_UP
-#undef LB_CONV_EPI
   return fail("convolutions with more than 256 output channels are not built");
 }
 
@@ -684,7 +710,8 @@ using namespace lb;
 template <int BN, int kP>
 static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st,
                                     const TfWs& w, long x_base, long x_rows, int x_group_rows, long s_base,
-                                    long s_rows, int s_group_rows, int n_groups_x, bool self_pass, cudaStream_t stream) {
+                                    long s_rows, int s_group_rows, int n_groups_x, bool self_pass, int sms,
+                                    cudaStream_t stream) {
   const long ldc = 2L * C;
   const __half* cat_hi = static_cast<const __half*>(st.cat_hi);
   const __half* cat_lo = static_cast<const __half*>(st.cat_lo);
@@ -700,7 +727,7 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
     Planes B{wq_hi, wq_lo, C, 0};
     typename Epi::Params ep{0, nullptr, 1, lw.s_qkv, {}};
     LB_TRY(fill_out_maps(&ep.om, w.att_hi + x_base * C, w.att_lo + x_base * C, C, nullptr, 0, C, x_rows, 1));
-    LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, 1, static_cast<int>(x_rows), C, C, 0, ep, stream)));
+    LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, gemm_shape<BN>(1, static_cast<int>(x_rows), C, C), ep, sms, stream)));
   }
   {
     using Epi = Operands<EpiPlanes<BN>, kP>;
@@ -708,18 +735,15 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
     Planes B{wq_hi + wkv_off, wq_lo + wkv_off, C, 0};
     typename Epi::Params ep{0, nullptr, 1, lw.s_qkv, {}};
     LB_TRY(fill_out_maps(&ep.om, w.h_hi + s_base * ldc, w.h_lo + s_base * ldc, ldc, nullptr, 0, 2 * C, s_rows, 1));
-    LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, 1, static_cast<int>(s_rows), 2 * C, C, 0, ep, stream)));
+    LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, gemm_shape<BN>(1, static_cast<int>(s_rows), 2 * C, C), ep, sms,
+                                 stream)));
   }
   const long qbs = static_cast<long>(x_group_rows) * C, kvbs = static_cast<long>(s_group_rows) * ldc;
   CUtensorMap tq_hi, tq_lo, tkv_hi, tkv_lo;
-  LB_TRY(make_map(&tq_hi, w.att_hi + x_base * C, C, x_group_rows, n_groups_x, C, qbs, kFaRows, kFaD));
-  LB_TRY(make_map(&tkv_hi, w.h_hi + s_base * ldc, 2 * C, s_group_rows, n_groups_s, ldc, kvbs, kFaKeys, kFaD));
-  tq_lo = tq_hi;
-  tkv_lo = tkv_hi;
-  if (kP == 2) {
-    LB_TRY(make_map(&tq_lo, w.att_lo + x_base * C, C, x_group_rows, n_groups_x, C, qbs, kFaRows, kFaD));
-    LB_TRY(make_map(&tkv_lo, w.h_lo + s_base * ldc, 2 * C, s_group_rows, n_groups_s, ldc, kvbs, kFaKeys, kFaD));
-  }
+  LB_TRY(map_planes<make_map>(kP, &tq_hi, &tq_lo, w.att_hi + x_base * C, w.att_lo + x_base * C, C, x_group_rows,
+                              n_groups_x, C, qbs, kFaRows, kFaD));
+  LB_TRY(map_planes<make_map>(kP, &tkv_hi, &tkv_lo, w.h_hi + s_base * ldc, w.h_lo + s_base * ldc, 2 * C, s_group_rows,
+                              n_groups_s, ldc, kvbs, kFaKeys, kFaD));
   constexpr auto kernel = kP == 2 ? &full_attn_wgmma_kernel : &full_attn_wgmma_fp16_kernel;
   LB_TRY(set_max_dynamic_smem<kernel>(fw_smem_bytes(kP)));
   FullAttnWgParams wp;
@@ -734,12 +758,7 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
   wp.ld_o = C;
   wp.scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(kFaD));
   const dim3 grid(cdiv(x_group_rows, kFaRows), H, n_groups_x);
-  TimingRec rec{nullptr, nullptr, TAG_FULL_ATTN};
-  LB_TRY(timing_begin(rec, stream));
-  kernel<<<grid, kFwThreads, fw_smem_bytes(kP), stream>>>(tq_hi, tq_lo, tkv_hi, tkv_lo, wp);
-  LB_LAUNCHED();
-  LB_TRY(timing_end(rec, stream));
-  return 0;
+  return launch(TAG_FULL_ATTN, kernel, grid, kFwThreads, fw_smem_bytes(kP), stream, tq_hi, tq_lo, tkv_hi, tkv_lo, wp);
 }
 
 // Steps 1-3 of a coarse (D = 32) encoder-layer call with linear attention (SURVEY.md §2a G1/G2): the k|v projection
@@ -749,7 +768,7 @@ static int tf_full_attention_coarse(const LbEncoderLayerWeights& lw, int C, int 
 template <int kP>
 static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st,
                                       const TfWs& w, long x_base, int x_group_rows, long s_base, int s_group_rows,
-                                      int n_groups_x, int n_groups_s, cudaStream_t stream) {
+                                      int n_groups_x, int n_groups_s, int sms, cudaStream_t stream) {
   if (!lw.wkv_hi || (kP == 2 && !lw.wkv_lo))
     return fail("linear attention of the coarse transformer needs the fused k|v weight planes (wkv_hi / wkv_lo)");
   const int D = C / H;
@@ -758,8 +777,6 @@ static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, in
   const __half* cat_hi = static_cast<const __half*>(st.cat_hi);
   const __half* cat_lo = static_cast<const __half*>(st.cat_lo);
   const uint8_t* mask = st.mask;
-  int sms = 0;
-  LB_TRY(device_check(&sms));
   __half* kvp_hi = w.h_hi + s_base * ldc;   // the MLP hidden planes [R, 2C] are free at this point of the layer
   __half* kvp_lo = w.h_lo + s_base * ldc;
   {
@@ -770,31 +787,21 @@ static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, in
     ep.rowmask = mask ? mask + s_base : nullptr;
     ep.acc_scale = lw.s_qkv;
     LB_TRY(fill_out_maps(&ep.om, kvp_hi, kvp_lo, ldc, nullptr, 0, 2 * C, s_group_rows, n_groups_s));
-    LB_TRY((launch_gemm<256, Epi>(TAG_KV, A, B, n_groups_s, s_group_rows, 2 * C, C, 0, ep, stream)));
+    LB_TRY((launch_gemm<256, Epi>(TAG_KV, A, B, gemm_shape<256>(n_groups_s, s_group_rows, 2 * C, C), ep, sms, stream)));
   }
   {
     CUtensorMap tm_hi, tm_lo;
-    LB_TRY(make_map(&tm_hi, kvp_hi, 2 * C, s_group_rows, n_groups_s, ldc, static_cast<long>(s_group_rows) * ldc, 64, 64));
-    tm_lo = tm_hi;
-    if (kP == 2)
-      LB_TRY(make_map(&tm_lo, kvp_lo, 2 * C, s_group_rows, n_groups_s, ldc, static_cast<long>(s_group_rows) * ldc, 64, 64));
-    const int kb_total = cdiv(s_group_rows, 64);
-    const int m_tiles_s = cdiv(s_group_rows, kBlockM);
-    const int parts_cap = m_tiles_s > kKvSplits ? m_tiles_s : kKvSplits;   // capacity of kv_part (see kKvSplits)
-    int splits = sms / (2 * n_groups_s);
-    if (splits < 1) splits = 1;
-    if (splits > kb_total) splits = kb_total;
-    if (splits > parts_cap) splits = parts_cap;
-    const int kb_per = cdiv(kb_total, splits);
-    splits = cdiv(kb_total, kb_per);
+    LB_TRY(map_planes<make_map>(kP, &tm_hi, &tm_lo, kvp_hi, kvp_lo, 2 * C, s_group_rows, n_groups_s, ldc,
+                                static_cast<long>(s_group_rows) * ldc, 64, 64));
+    const KvSplits ks = kv_splits(s_group_rows, n_groups_s, sms);
     constexpr auto kernel = kP == 2 ? &kv_gemm_kernel : &kv_gemm_fp16_kernel;
     LB_TRY(set_max_dynamic_smem<kernel>(kv_gemm_smem(kP)));
-    KvGemmParams kp{w.kv_part, kb_total, kb_per, splits};
-    kernel<<<dim3(splits, 2, n_groups_s), kKvGemmThreads, kv_gemm_smem(kP), stream>>>(tm_hi, tm_lo, kp);
-    LB_LAUNCHED();
+    KvGemmParams kp{w.kv_part, ks.kb_total, ks.kb_per, ks.splits};
+    LB_TRY(launch(TAG_NONE, kernel, dim3(ks.splits, 2, n_groups_s), kKvGemmThreads, kv_gemm_smem(kP), stream, tm_hi,
+                  tm_lo, kp));
     const long total = static_cast<long>(n_groups_s) * H * per;
-    kv_tile_merge_kernel<<<cdiv(total, 256), 256, 0, stream>>>(w.kv_part, splits, H * per, w.kv, total);
-    LB_LAUNCHED();
+    LB_TRY(launch(TAG_NONE, kv_tile_merge_kernel, cdiv(total, 256), 256, 0, stream, w.kv_part, ks.splits, H * per, w.kv,
+                  total));
   }
   {
     using Epi = Operands<EpiAttn<256, 32>, kP>;
@@ -802,7 +809,7 @@ static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, in
     Planes B{lw.wqkv_hi, lw.wqkv_lo, C, 0};
     typename Epi::Params ep{mask ? mask + x_base : nullptr, lw.s_qkv, w.kv, 1e-6f, w.att_hi + x_base * C,
                             w.att_lo + x_base * C, C};
-    LB_TRY((launch_gemm<256, Epi>(TAG_QATTN, A, B, n_groups_x, x_group_rows, C, C, 0, ep, stream)));
+    LB_TRY((launch_gemm<256, Epi>(TAG_QATTN, A, B, gemm_shape<256>(n_groups_x, x_group_rows, C, C), ep, sms, stream)));
   }
   return 0;
 }
@@ -810,10 +817,10 @@ static int tf_linear_attention_coarse(const LbEncoderLayerWeights& lw, int C, in
 // Runs one encoder-layer call `x <- layer(x, source)` for the row range x (queries) / s (source).
 // self_pass: x range == source range (q, k, v in one projection launch).
 template <int BN, int kP>
-static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st,
-                             const TfWs& w, long x_base, long x_rows, int x_group_rows, long s_base, long s_rows,
-                             int s_group_rows, int n_groups_x, bool self_pass, bool write_f32, cudaStream_t stream,
-                             const int* live, int live_cap, bool full) {
+static int tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const LbTransformerState& st, const TfWs& w,
+                         long x_base, long x_rows, int x_group_rows, long s_base, long s_rows, int s_group_rows,
+                         int n_groups_x, bool self_pass, bool write_f32, int sms, cudaStream_t stream, const int* live,
+                         int live_cap, bool full) {
   const int D = C / H;
   const long ldc = 2L * C;
   const __half* cat_hi = static_cast<const __half*>(st.cat_hi);
@@ -835,10 +842,10 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
   // 1-3. attention message -> att planes [x rows, C]
   if (D == 32 && !full) {
     LB_TRY(tf_linear_attention_coarse<kP>(lw, C, H, st, w, x_base, x_group_rows, s_base, s_group_rows, n_groups_x,
-                                      n_groups_s, stream));
+                                      n_groups_s, sms, stream));
   } else if (D == 32) {
     LB_TRY((tf_full_attention_coarse<BN, kP>(lw, C, H, st, w, x_base, x_rows, x_group_rows, s_base, s_rows, s_group_rows,
-                                        n_groups_x, self_pass, stream)));
+                                        n_groups_x, self_pass, sms, stream)));
   } else {
     // windows of the fine transformer (D = 16, H = 8): the window kernels give every query / source row one lane
     if (x_group_rows > 32 || s_group_rows > 32)
@@ -856,7 +863,8 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
       OutMaps om;
       LB_TRY(fill_out_maps(&om, nullptr, nullptr, 0, w.qkv + x_base * 3 * C, 3 * C, 3 * C, xM, xb));
       typename Epi::Params ep{elu_self, pmask ? pmask + x_base : nullptr, lw.s_qkv, om};
-      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, xb, xM, 3 * C, C, 0, ep, stream, live, x_group_rows)));
+      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, A, B, gemm_shape<BN>(xb, xM, 3 * C, C, false, 0, live, x_group_rows), ep,
+                                   sms, stream)));
     } else {
       Planes Aq{cat_hi + x_base * ldc, cat_lo + x_base * ldc, ldc, xbs};
       Planes Bq{lw.wqkv_hi, lw.wqkv_lo, C, 0};
@@ -864,32 +872,29 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
       LB_TRY(fill_out_maps(&omq, nullptr, nullptr, 0, w.qkv + x_base * 3 * C, 3 * C, C, xM, xb));
       LB_TRY(fill_out_maps(&omk, nullptr, nullptr, 0, w.qkv + s_base * 3 * C + C, 3 * C, 2 * C, sM, sb));
       typename Epi::Params eq{elu_q, pmask ? pmask + x_base : nullptr, lw.s_qkv, omq};
-      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Aq, Bq, xb, xM, C, C, 0, eq, stream, live, x_group_rows)));
+      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Aq, Bq, gemm_shape<BN>(xb, xM, C, C, false, 0, live, x_group_rows), eq,
+                                   sms, stream)));
       Planes Ak{cat_hi + s_base * ldc, cat_lo + s_base * ldc, ldc, sbs};
       Planes Bk{static_cast<const __half*>(lw.wqkv_hi) + static_cast<long>(C) * C,
                 static_cast<const __half*>(lw.wqkv_lo) + static_cast<long>(C) * C, C, 0};
       typename Epi::Params ek{elu_kv, pmask ? pmask + s_base : nullptr, lw.s_qkv, omk};
-      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Ak, Bk, sb, sM, 2 * C, C, 0, ek, stream, live, s_group_rows)));
+      LB_TRY((launch_gemm<BN, Epi>(TAG_PROJ, Ak, Bk, gemm_shape<BN>(sb, sM, 2 * C, C, false, 0, live, s_group_rows), ek,
+                                   sms, stream)));
     }
-    int sms = 0;
-    LB_TRY(device_check(&sms));
     if (full) {
       // full (softmax) attention of the windows, exact fp32                      [linear_attention.py:56-81]
       const int grid = n_groups_x < 4 * sms ? n_groups_x : 4 * sms;
-      window_full_attn_kernel<16, 8, 32><<<grid, 256, 0, stream>>>(w.qkv, 3 * C, 0, C, 2 * C, x_base, s_base,
-                                                                   x_group_rows, n_groups_x, mask, w.att_hi, w.att_lo,
-                                                                   C, live, live_cap);
+      LB_TRY(launch(TAG_NONE, window_full_attn_kernel<16, 8, 32>, grid, 256, 0, stream, w.qkv, 3 * C, 0, C, 2 * C,
+                    x_base, s_base, x_group_rows, n_groups_x, mask, w.att_hi, w.att_lo, C, live, live_cap));
     } else {
       // linear attention, one kernel per pass: KV stays in shared memory      [linear_attention.py:43-46]
       const int grid = n_groups_x < 3 * sms ? n_groups_x : 3 * sms;   // 3 resident blocks per SM (60 KB, <= 85 registers)
       const int wa_smem = (H * (D * D + D) + 4 * s_group_rows * C) * static_cast<int>(sizeof(float));
       LB_TRY((set_max_dynamic_smem<&window_attn_kernel<16, 8>>(
           (8 * (16 * 16 + 16) + 4 * 32 * 128) * static_cast<int>(sizeof(float)))));   // largest (32-row) window
-      window_attn_kernel<16, 8><<<grid, 256, wa_smem, stream>>>(w.qkv, 3 * C, 0, C, 2 * C, x_base, s_base, x_group_rows,
-                                                                s_group_rows, n_groups_x, 1e-6f, w.att_hi, w.att_lo, C,
-                                                                live, live_cap);
+      LB_TRY(launch(TAG_NONE, window_attn_kernel<16, 8>, grid, 256, wa_smem, stream, w.qkv, 3 * C, 0, C, 2 * C, x_base,
+                    s_base, x_group_rows, s_group_rows, n_groups_x, 1e-6f, w.att_hi, w.att_lo, C, live, live_cap));
     }
-    LB_LAUNCHED();
   }
   // 4. merge + norm1 -> cat[:, C:2C]                            [transformer.py:51-52]
   {
@@ -902,7 +907,8 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
     typename Epi::Params ep{lw.ln1_g, lw.ln1_b, 1e-5f, nullptr, 0, nullptr, nullptr, 0, nullptr, 0,
                             static_cast<__half*>(st.cat_hi) + x_base * ldc,
                             static_cast<__half*>(st.cat_lo) + x_base * ldc, static_cast<int>(ldc), C, lw.s_m, om};
-    LB_TRY((launch_gemm<BN, Epi>(TAG_MERGE_LN, A, B, xb, xM, C, C, 0, ep, stream, live, x_group_rows)));
+    LB_TRY((launch_gemm<BN, Epi>(TAG_MERGE_LN, A, B, gemm_shape<BN>(xb, xM, C, C, false, 0, live, x_group_rows), ep,
+                                 sms, stream)));
   }
   // 5. mlp[0] + ReLU on cat([x, message]) -> h planes           [transformer.py:55, mlp 22-26]
   {
@@ -911,7 +917,8 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
     Planes B{lw.w1_hi, lw.w1_lo, 2 * C, 0};
     typename Epi::Params ep{1, nullptr, 1, lw.s_1, {}};
     LB_TRY(fill_out_maps(&ep.om, w.h_hi + x_base * ldc, w.h_lo + x_base * ldc, ldc, nullptr, 0, 2 * C, xM, xb));
-    LB_TRY((launch_gemm<BN, Epi>(TAG_MLP1, A, B, xb, xM, 2 * C, 2 * C, 0, ep, stream, live, x_group_rows)));
+    LB_TRY((launch_gemm<BN, Epi>(TAG_MLP1, A, B, gemm_shape<BN>(xb, xM, 2 * C, 2 * C, false, 0, live, x_group_rows), ep,
+                                 sms, stream)));
   }
   // 6. mlp[2] + norm2 + residual -> cat[:, 0:C] (and x_f32 after the last layer)   [transformer.py:55-58]
   // The residual stream lives in the fp16 planes (x = hi + lo, exact to 2^-22 relative): no fp32 master copy is read
@@ -928,7 +935,8 @@ static int lb::tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, cons
                             static_cast<int>(ldc), xf, C,
                             static_cast<__half*>(st.cat_hi) + x_base * ldc,
                             static_cast<__half*>(st.cat_lo) + x_base * ldc, static_cast<int>(ldc), 0, lw.s_2, om};
-    LB_TRY((launch_gemm<BN, Epi>(TAG_MLP2_LN, A, B, xb, xM, C, 2 * C, 0, ep, stream, live, x_group_rows)));
+    LB_TRY((launch_gemm<BN, Epi>(TAG_MLP2_LN, A, B, gemm_shape<BN>(xb, xM, C, 2 * C, false, 0, live, x_group_rows), ep,
+                                 sms, stream)));
   }
   return 0;
 }
@@ -978,24 +986,20 @@ int lb_timing_collect(double* total_ms, long long* counts, int n) {
 int lb_split_planes(const float* x, long rows, int cols, int ld_x, void* hi, void* lo, int ld_pl, int col0,
                     void* stream) {
   if (rows <= 0 || cols <= 0) return 0;
-  int sms;
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(x));
-  LB_TRY(device_check(&sms));
+  DeviceScope dev;
+  LB_TRY(dev.bind(x));
   const long total = rows * cols;
   const int grid = static_cast<int>(total / 256 + 1 < 4096 ? total / 256 + 1 : 4096);
-  split_planes_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      x, rows, cols, ld_x, static_cast<__half*>(hi), static_cast<__half*>(lo), ld_pl, col0);
-  LB_LAUNCHED();
-  return 0;
+  return launch(TAG_NONE, split_planes_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream), x, rows, cols, ld_x,
+                static_cast<__half*>(hi), static_cast<__half*>(lo), ld_pl, col0);
 }
 
 int lb_gemm_split(const void* a_hi, const void* a_lo, long lda, long a_batch_stride, const void* b_hi,
                   const void* b_lo, long ldb, long b_batch_stride, float* out, long ldo, long o_batch_stride,
                   int batches, int M, int N, int K, void* stream) {
   if (N % 32 != 0) return fail("lb_gemm_split: N must be a multiple of 32");
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(out));
+  DeviceScope dev;
+  LB_TRY(dev.bind(out));
   if (batches > 1 && o_batch_stride != static_cast<long>(M) * ldo)
     return fail("lb_gemm_split: output batches must be densely stacked (o_batch_stride == M*ldo)");
   Planes A{a_hi, a_lo, lda, batches > 1 ? a_batch_stride : 0};
@@ -1006,11 +1010,13 @@ int lb_gemm_split(const void* a_hi, const void* a_lo, long lda, long a_batch_str
   if (N % 256 == 0 || N > 128) {
     using Epi = EpiActStore<256>;
     Epi::Params ep{0, nullptr, 1.f, om};
-    return launch_gemm<256, Epi>(TAG_GEMM_TEST, A, B, batches, M, N, K, 0, ep, st);
+    return launch_gemm<256, Epi>(TAG_GEMM_TEST, A, B, gemm_shape<256>(batches, M, N, K, b_batch_stride > 0), ep,
+                                 dev.sms, st);
   }
   using Epi = EpiActStore<128>;
   Epi::Params ep{0, nullptr, 1.f, om};
-  return launch_gemm<128, Epi>(TAG_GEMM_TEST, A, B, batches, M, N, K, 0, ep, st);
+  return launch_gemm<128, Epi>(TAG_GEMM_TEST, A, B, gemm_shape<128>(batches, M, N, K, b_batch_stride > 0), ep, dev.sms,
+                               st);
 }
 
 int lb_preprocess_images(const LbImageDesc* descs, int n_images, float* out, int H, int W, uint8_t* mask,
@@ -1021,37 +1027,24 @@ int lb_preprocess_images(const LbImageDesc* descs, int n_images, float* out, int
   if (!descs || !out) return fail("lb_preprocess_images: descs and out are required");
   if ((reinterpret_cast<uintptr_t>(out) & 15) != 0) return fail("lb_preprocess_images: out is not 16-byte aligned");
   if (n_images == 0) return 0;
-  int sms;
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(out));
-  LB_TRY(device_check(&sms));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  DeviceScope dev;
+  LB_TRY(dev.bind(out));
   dim3 grid(cdiv(W, kPreprocessBlockX * 4), cdiv(H, kPreprocessBlockY), n_images);
-  TimingRec rec{nullptr, nullptr, TAG_PREPROCESS};
-  LB_TRY(timing_begin(rec, st));
-  preprocess_images_kernel<<<grid, dim3(kPreprocessBlockX, kPreprocessBlockY), 0, st>>>(descs, out, H, W, mask);
-  LB_LAUNCHED();
-  LB_TRY(timing_end(rec, st));
-  return 0;
+  return launch(TAG_PREPROCESS, preprocess_images_kernel, grid, dim3(kPreprocessBlockX, kPreprocessBlockY), 0,
+                static_cast<cudaStream_t>(stream), descs, out, H, W, mask);
 }
 
 // n_out output images; with img_idx, output image b reads image img_idx[b] of feat
 static int coarse_prep(const float* feat, int nhwc, const float* pe, const int* img_idx, int n_out, int C, int h,
                        int w, int pe_h, int pe_w, float* x_f32, void* cat_hi, void* cat_lo, void* stream) {
-  int sms;
   if (n_out <= 0) return 0;
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(x_f32));
-  LB_TRY(device_check(&sms));
+  DeviceScope dev;
+  LB_TRY(dev.bind(x_f32));
   if (h > pe_h || w > pe_w) return fail("feature map %dx%d exceeds the position-encoding table %dx%d", h, w, pe_h, pe_w);
   dim3 grid(cdiv(static_cast<long>(h) * w, 32), cdiv(C, 32), n_out);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  __half* hi = static_cast<__half*>(cat_hi);
-  __half* lo = static_cast<__half*>(cat_lo);
-  if (img_idx) coarse_prep_kernel<true><<<grid, dim3(32, 8), 0, st>>>(feat, nhwc, pe, C, h, w, pe_h, pe_w, x_f32, hi, lo, img_idx);
-  else coarse_prep_kernel<false><<<grid, dim3(32, 8), 0, st>>>(feat, nhwc, pe, C, h, w, pe_h, pe_w, x_f32, hi, lo, nullptr);
-  LB_LAUNCHED();
-  return 0;
+  return launch(TAG_NONE, img_idx ? coarse_prep_kernel<true> : coarse_prep_kernel<false>, grid, dim3(32, 8), 0,
+                static_cast<cudaStream_t>(stream), feat, nhwc, pe, C, h, w, pe_h, pe_w, x_f32,
+                static_cast<__half*>(cat_hi), static_cast<__half*>(cat_lo), img_idx);
 }
 
 int lb_coarse_prep(const float* feat, int nhwc, const float* pe, int n_img, int C, int h, int w, int pe_h, int pe_w,
@@ -1079,11 +1072,9 @@ size_t lb_transformer_workspace_bytes(int d_model, int nhead, int n_groups, int 
 template <int kP>
 static int transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds, int n_layers, int d_model,
                                int nhead, const LbTransformerState* st, void* ws, size_t ws_bytes, void* stream) {
-  int sms;
   if (st->n_groups <= 0) return 0;
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(st->x_f32));
-  LB_TRY(device_check(&sms));
+  DeviceScope dev;
+  LB_TRY(dev.bind(st->x_f32));
   const int C = d_model, H = nhead;
   const bool coarse = (C == 256 && H == 8);
   const bool fine = (C == 128 && H == 8);
@@ -1106,10 +1097,10 @@ static int transformer_forward(const LbEncoderLayerWeights* layers, const int* k
     const int kind = kinds[l];
     const bool full = kind == LB_LAYER_SELF_FULL || kind == LB_LAYER_CROSS_FULL;
     auto pass = [&](long xb, long xr, int xg, long sb, long sr, int sg, int ng, bool self_pass) -> int {
-      return coarse ? tf_layer_pass<256, kP>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s, nullptr,
-                                             0, full)
-                    : tf_layer_pass<128, kP>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, s, live,
-                                             st->n_groups, full);
+      return coarse ? tf_layer_pass<256, kP>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, dev.sms, s,
+                                             nullptr, 0, full)
+                    : tf_layer_pass<128, kP>(lw, C, H, *st, w, xb, xr, xg, sb, sr, sg, ng, self_pass, last, dev.sms, s,
+                                             live, st->n_groups, full);
     };
     if (kind == LB_LAYER_SELF || kind == LB_LAYER_SELF_FULL) {
       // feat0 = layer(feat0, feat0); feat1 = layer(feat1, feat1)  [transformer.py:93-94]; same weights,
@@ -1157,11 +1148,10 @@ static size_t backbone_workspace_bytes(const LbBackboneWeights* w, int N, int H,
 template <int kPlanes>
 static int backbone_forward(const LbBackboneWeights* w, const float* images, int N, int H, int W, float* feat_c_nhwc,
                             float* feat_f_nhwc, void* ws, size_t ws_bytes, void* stream) {
-  int sms;
   if (N <= 0) return 0;
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(images));
-  LB_TRY(device_check(&sms));
+  DeviceScope dev;
+  LB_TRY(dev.bind(images));
+  const int sms = dev.sms;
   if (H % 8 != 0 || W % 8 != 0) return fail("image size %dx%d must be divisible by 8", H, W);
   if (!ws) return fail("workspace pointer is null");
   const int d1 = w->l1[0].cout, d2 = w->l2[0].cout, d3 = w->l3[0].cout;
@@ -1181,21 +1171,17 @@ static int backbone_forward(const LbBackboneWeights* w, const float* images, int
     sp.img = images; sp.N = N; sp.H = H; sp.W = W;
     sp.wt = w->stem_wt; sp.scale = w->stem_scale; sp.shift = w->stem_shift;
     sp.tiles_w = cdiv(W2, kConvTileW); sp.tiles_h = cdiv(H2, kConvTileH);
-    sp.om.dims = 4;
-    LB_TRY(make_out_map_nhwc(&sp.om.hi, B.s0.hi, false, 128, W2, H2, N, B.s0.ld));
-    if (kPlanes == 2) LB_TRY(make_out_map_nhwc(&sp.om.lo, B.s0.lo, false, 128, W2, H2, N, B.s0.ld));
-    sp.om.use = 1;
+    LB_TRY(fill_out_maps_nhwc(&sp.om, kPlanes, B.s0.hi, B.s0.lo, B.s0.ld, nullptr, 0, 128, W2, H2, N));
     constexpr auto kStem = kPlanes == 2 ? &conv_stem7x7_tc_kernel : &conv_stem7x7_tc_fp16_kernel;
     LB_TRY(set_max_dynamic_smem<kStem>(kStemSmemBytes));
     const long tiles = static_cast<long>(sp.tiles_w) * sp.tiles_h * N;
     const int grid = static_cast<int>(tiles < sms ? tiles : sms);
-    kStem<<<grid, kStemThreads, kStemSmemBytes, st>>>(sp);
-    LB_LAUNCHED();
+    LB_TRY(launch(TAG_NONE, kStem, grid, kStemThreads, kStemSmemBytes, st, sp));
   }
   auto conv = [&](const LbConvWeights& cw, const BbBuf& in, int hin, int win, int act, const BbBuf* res,
                   const BbBuf* up, int uph, int upw, const BbBuf* out, float* of32, int f32ld) -> int {
     ConvRun r{&cw, in, hin, win, act, res, up, uph, upw, out, of32, f32ld};
-    return run_conv<kPlanes>(r, N, st);
+    return run_conv<kPlanes>(r, N, sms, st);
   };
   // layer1 (1/2)                                                                    [resnet_fpn.py:102]
   LB_TRY(conv(w->l1[0], B.s0, H2, W2, 1, nullptr, nullptr, 0, 0, &B.t1, nullptr, 0));
@@ -1301,10 +1287,8 @@ size_t lb_coarse_match_workspace_bytes(int n_pairs, int L, int S) {
 // kP: operand planes of the score products (Operands); every pass recomputes the same logits.
 template <int kP>
 static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, size_t ws_bytes, void* stream) {
-  int sms;
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(a->count));
-  LB_TRY(device_check(&sms));
+  DeviceScope dev;
+  LB_TRY(dev.bind(a->count));
   const int n = a->n_pairs, L = a->L, S = a->S, C = a->C;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (n <= 0) {
@@ -1320,24 +1304,20 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
   carve_cm(b, w, n, L, S);
   if (!b.ok) return fail("coarse-match workspace too small: need %zu bytes", lb_coarse_match_workspace_bytes(n, L, S));
 
+  // the score products: row partials per chunk of n tiles (score.n_chunks), column partials per m tile
   constexpr int BN = 256;
   const long nl = static_cast<long>(n) * L, ns = static_cast<long>(n) * S;
-  const int m_tiles = (L + kBlockM - 1) / kBlockM;
-  const int n_tiles = (S + BN - 1) / BN;
-  int chunks = pick_chunks(n * m_tiles, n_tiles, sms);
+  int chunks = pick_chunks(n * cdiv(L, kBlockM), cdiv(S, BN), dev.sms);
   if (chunks > kMaxChunks) chunks = kMaxChunks;
-  // launch_gemm re-derives (tiles_per_chunk, n_chunks) from this request; mirror it to size the merges
-  const int tpc = (n_tiles + chunks - 1) / chunks;
-  const int n_chunks = (n_tiles + tpc - 1) / tpc;
+  const GemmShape score = gemm_shape<BN>(n, L, S, C, /*b_batched=*/true, chunks);
+  const int n_chunks = score.n_chunks, m_tiles = score.m_tiles;
 
   Planes A{a->f0_hi, a->f0_lo, a->ld, static_cast<long>(L) * a->ld};
   Planes B{a->f1_hi, a->f1_lo, a->ld, static_cast<long>(S) * a->ld};
   const bool masked = a->mask0 != nullptr;
   if (masked) {
-    mask_extent_kernel<<<n, 128, 0, st>>>(a->mask0, a->h0c, a->w0c, w.ext0);
-    LB_LAUNCHED();
-    mask_extent_kernel<<<n, 128, 0, st>>>(a->mask1, a->h1c, a->w1c, w.ext1);
-    LB_LAUNCHED();
+    LB_TRY(launch(TAG_NONE, mask_extent_kernel, n, 128, 0, st, a->mask0, a->h0c, a->w0c, w.ext0));
+    LB_TRY(launch(TAG_NONE, mask_extent_kernel, n, 128, 0, st, a->mask1, a->h1c, a->w1c, w.ext1));
   }
   const int TB = 256;
   float conf_bias = 0.f;
@@ -1352,21 +1332,19 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
     const float* ct = nullptr;
     const float* rt = nullptr;
     if (masked) {  // padded rows / columns leave every normaliser      [coarse_matching.py:115-118]
-      mask_term_kernel<<<cdiv(ns, TB), TB, 0, st>>>(nullptr, a->mask1, nullptr, ns, w.col_t);
-      LB_LAUNCHED();
-      mask_term_kernel<<<cdiv(nl, TB), TB, 0, st>>>(nullptr, a->mask0, nullptr, nl, w.row_t);
-      LB_LAUNCHED();
+      LB_TRY(launch(TAG_NONE, mask_term_kernel, cdiv(ns, TB), TB, 0, st, nullptr, a->mask1, nullptr, ns, w.col_t));
+      LB_TRY(launch(TAG_NONE, mask_term_kernel, cdiv(nl, TB), TB, 0, st, nullptr, a->mask0, nullptr, nl, w.row_t));
       ct = w.col_t;
       rt = w.row_t;
     }
     using Epi = Operands<EpiScoreLse<BN, true, true>, kP>;
     typename Epi::Params ep{scale, ct, rt, w.row_part, w.col_part};
-    LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, n, L, S, C, chunks, ep, st)));
+    LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, score, ep, dev.sms, st)));
     // row_t = -rowLSE, col_t = -colLSE (kNegBig on padded entries)              [coarse_matching.py:119]
-    lse_merge_kernel<<<cdiv(nl, TB), TB, 0, st>>>(w.row_part, n_chunks, nl, 0.f, nullptr, nullptr, L, a->mask0, w.row_t);
-    LB_LAUNCHED();
-    lse_merge_kernel<<<cdiv(ns, TB), TB, 0, st>>>(w.col_part, m_tiles, ns, 0.f, nullptr, nullptr, S, a->mask1, w.col_t);
-    LB_LAUNCHED();
+    LB_TRY(launch(TAG_NONE, lse_merge_kernel, cdiv(nl, TB), TB, 0, st, w.row_part, n_chunks, nl, 0.f, nullptr, nullptr,
+                  L, a->mask0, w.row_t));
+    LB_TRY(launch(TAG_NONE, lse_merge_kernel, cdiv(ns, TB), TB, 0, st, w.col_part, m_tiles, ns, 0.f, nullptr, nullptr,
+                  S, a->mask1, w.col_t));
     rowterm_for_conf = w.row_t;
   } else if (a->match_type == LB_MATCH_SINKHORN) {
     // sim = <f0, f1> / C ; log-domain Sinkhorn with dustbins              [coarse_matching.py:121-131]
@@ -1377,46 +1355,35 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
     const float log_mu_bin = logf(static_cast<float>(S)) + norm;  // dustbin row mass   [superglue.py:161]
     const float log_nu_bin = logf(static_cast<float>(L)) + norm;  // dustbin column mass [superglue.py:162]
     // v = 0 (kNegBig on padded columns for the masked variant), bin_v = 0
-    mask_term_kernel<<<cdiv(ns, TB), TB, 0, st>>>(nullptr, a->mask1, nullptr, ns, w.col_t);
-    LB_LAUNCHED();
-    fill_kernel<<<cdiv(ns, TB), TB, 0, st>>>(w.col_v, 0.f, ns);
-    LB_LAUNCHED();
-    fill_kernel<<<cdiv(n, TB), TB, 0, st>>>(w.bin_v, 0.f, n);
-    LB_LAUNCHED();
-    fill_kernel<<<cdiv(nl, TB), TB, 0, st>>>(w.row_u, 0.f, nl);   // u = 0 (only observable with skh_iters == 0)
-    LB_LAUNCHED();
-    fill_kernel<<<cdiv(n, TB), TB, 0, st>>>(w.bin_u, 0.f, n);
-    LB_LAUNCHED();
-    mask_term_kernel<<<cdiv(nl, TB), TB, 0, st>>>(nullptr, a->mask0, nullptr, nl, w.row_t);
-    LB_LAUNCHED();
+    LB_TRY(launch(TAG_NONE, mask_term_kernel, cdiv(ns, TB), TB, 0, st, nullptr, a->mask1, nullptr, ns, w.col_t));
+    LB_TRY(launch(TAG_NONE, fill_kernel, cdiv(ns, TB), TB, 0, st, w.col_v, 0.f, ns));
+    LB_TRY(launch(TAG_NONE, fill_kernel, cdiv(n, TB), TB, 0, st, w.bin_v, 0.f, n));
+    // u = 0 (only observable with skh_iters == 0)
+    LB_TRY(launch(TAG_NONE, fill_kernel, cdiv(nl, TB), TB, 0, st, w.row_u, 0.f, nl));
+    LB_TRY(launch(TAG_NONE, fill_kernel, cdiv(n, TB), TB, 0, st, w.bin_u, 0.f, n));
+    LB_TRY(launch(TAG_NONE, mask_term_kernel, cdiv(nl, TB), TB, 0, st, nullptr, a->mask0, nullptr, nl, w.row_t));
     for (int it = 0; it < a->skh_iters; ++it) {
       // u_i = log_mu_i - LSE_j(Z_ij + v_j), j over S real columns + the dustbin column   [superglue.py:146]
       {
         using Epi = Operands<EpiScoreLse<BN, true, false>, kP>;
         typename Epi::Params ep{scale, w.col_t, nullptr, w.row_part, w.col_part};
-        LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, n, L, S, C, chunks, ep, st)));
-        lse_merge_kernel<<<cdiv(nl, TB), TB, 0, st>>>(w.row_part, n_chunks, nl, norm, a->bin_score, w.bin_v, L,
-                                                      a->mask0, w.row_u);
-        LB_LAUNCHED();
+        LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, score, ep, dev.sms, st)));
+        LB_TRY(launch(TAG_NONE, lse_merge_kernel, cdiv(nl, TB), TB, 0, st, w.row_part, n_chunks, nl, norm, a->bin_score,
+                      w.bin_v, L, a->mask0, w.row_u));
       }
       // dustbin row: u_L = log_mu_L - LSE_j(bin + v_j, bin + bin_v)                         [superglue.py:146]
-      bin_lse_kernel<<<n, 256, 0, st>>>(w.col_v, S, a->bin_score, w.bin_v, log_mu_bin, w.bin_u);
-      LB_LAUNCHED();
-      mask_term_kernel<<<cdiv(nl, TB), TB, 0, st>>>(w.row_u, a->mask0, nullptr, nl, w.row_t);
-      LB_LAUNCHED();
+      LB_TRY(launch(TAG_NONE, bin_lse_kernel, n, 256, 0, st, w.col_v, S, a->bin_score, w.bin_v, log_mu_bin, w.bin_u));
+      LB_TRY(launch(TAG_NONE, mask_term_kernel, cdiv(nl, TB), TB, 0, st, w.row_u, a->mask0, nullptr, nl, w.row_t));
       // v_j = log_nu_j - LSE_i(Z_ij + u_i), i over L real rows + the dustbin row            [superglue.py:147]
       {
         using Epi = Operands<EpiScoreLse<BN, false, true>, kP>;
         typename Epi::Params ep{scale, nullptr, w.row_t, w.row_part, w.col_part};
-        LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, n, L, S, C, chunks, ep, st)));
-        lse_merge_kernel<<<cdiv(ns, TB), TB, 0, st>>>(w.col_part, m_tiles, ns, norm, a->bin_score, w.bin_u, S,
-                                                      a->mask1, w.col_v);
-        LB_LAUNCHED();
+        LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, score, ep, dev.sms, st)));
+        LB_TRY(launch(TAG_NONE, lse_merge_kernel, cdiv(ns, TB), TB, 0, st, w.col_part, m_tiles, ns, norm, a->bin_score,
+                      w.bin_u, S, a->mask1, w.col_v));
       }
-      bin_lse_kernel<<<n, 256, 0, st>>>(w.row_u, L, a->bin_score, w.bin_u, log_nu_bin, w.bin_v);
-      LB_LAUNCHED();
-      mask_term_kernel<<<cdiv(ns, TB), TB, 0, st>>>(w.col_v, a->mask1, nullptr, ns, w.col_t);
-      LB_LAUNCHED();
+      LB_TRY(launch(TAG_NONE, bin_lse_kernel, n, 256, 0, st, w.row_u, L, a->bin_score, w.bin_u, log_nu_bin, w.bin_v));
+      LB_TRY(launch(TAG_NONE, mask_term_kernel, cdiv(ns, TB), TB, 0, st, w.col_v, a->mask1, nullptr, ns, w.col_t));
     }
     // assignment = exp(Z + u + v - norm)                                      [superglue.py:148,168-169]
     conf_bias = -norm;
@@ -1432,21 +1399,19 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
   for (int pass = 0; pass < passes; ++pass) {
     using Epi = Operands<EpiScoreArgmax<BN>, kP>;
     typename Epi::Params ep{scale, alpha, w.col_t, w.row_t, w.row_apart, w.col_apart};
-    LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_ARGMAX, A, B, n, L, S, C, chunks, ep, st)));
-    argmax_merge_kernel<<<cdiv(nl, TB), TB, 0, st>>>(w.row_apart, n_chunks, nl, w.row_key, w.row_arg);
-    LB_LAUNCHED();
-    argmax_merge_kernel<<<cdiv(ns, TB), TB, 0, st>>>(w.col_apart, m_tiles, ns, w.col_key, w.col_arg);
-    LB_LAUNCHED();
+    LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_ARGMAX, A, B, score, ep, dev.sms, st)));
+    LB_TRY(launch(TAG_NONE, argmax_merge_kernel, cdiv(nl, TB), TB, 0, st, w.row_apart, n_chunks, nl, w.row_key,
+                  w.row_arg));
+    LB_TRY(launch(TAG_NONE, argmax_merge_kernel, cdiv(ns, TB), TB, 0, st, w.col_apart, m_tiles, ns, w.col_key,
+                  w.col_arg));
     if (passes == 2 && pass == 0) {
       // prefilter: rows / columns whose best partner is the dustbin are zeroed  [coarse_matching.py:136-140]
-      ot_dead_kernel<<<cdiv(nl, TB), TB, 0, st>>>(w.row_key, a->bin_score, w.bin_v, L, nl, w.row_dead);
-      LB_LAUNCHED();
-      ot_dead_kernel<<<cdiv(ns, TB), TB, 0, st>>>(w.col_key, a->bin_score, w.bin_u, S, ns, w.col_dead);
-      LB_LAUNCHED();
-      mask_term_kernel<<<cdiv(nl, TB), TB, 0, st>>>(w.row_u, a->mask0, w.row_dead, nl, w.row_t);
-      LB_LAUNCHED();
-      mask_term_kernel<<<cdiv(ns, TB), TB, 0, st>>>(w.col_v, a->mask1, w.col_dead, ns, w.col_t);
-      LB_LAUNCHED();
+      LB_TRY(launch(TAG_NONE, ot_dead_kernel, cdiv(nl, TB), TB, 0, st, w.row_key, a->bin_score, w.bin_v, L, nl,
+                    w.row_dead));
+      LB_TRY(launch(TAG_NONE, ot_dead_kernel, cdiv(ns, TB), TB, 0, st, w.col_key, a->bin_score, w.bin_u, S, ns,
+                    w.col_dead));
+      LB_TRY(launch(TAG_NONE, mask_term_kernel, cdiv(nl, TB), TB, 0, st, w.row_u, a->mask0, w.row_dead, nl, w.row_t));
+      LB_TRY(launch(TAG_NONE, mask_term_kernel, cdiv(ns, TB), TB, 0, st, w.col_v, a->mask1, w.col_dead, ns, w.col_t));
       row_dead = w.row_dead;
       col_dead = w.col_dead;
     }
@@ -1456,7 +1421,8 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
     using Epi = Operands<EpiConfStore<BN>, kP>;
     // row_t / col_t hold -LSE (dual-softmax) or the Sinkhorn potentials, with padded / prefiltered entries disabled
     typename Epi::Params ep{scale, alpha, conf_bias, w.row_t, w.col_t, a->conf_matrix};
-    LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_ARGMAX, A, B, n, L, S, C, 0, ep, st)));
+    LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_ARGMAX, A, B, gemm_shape<BN>(n, L, S, C, /*b_batched=*/true), ep, dev.sms,
+                                 st)));
   }
 
   SelectParams sp;
@@ -1471,14 +1437,9 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
   sp.ext0 = masked ? w.ext0 : nullptr; sp.ext1 = masked ? w.ext1 : nullptr;
   sp.row_dead = row_dead; sp.col_dead = col_dead;
   sp.flag = w.flag; sp.conf = w.conf;
-  match_flag_kernel<<<cdiv(nl, TB), TB, 0, st>>>(sp);
-  LB_LAUNCHED();
+  LB_TRY(launch(TAG_NONE, match_flag_kernel, cdiv(nl, TB), TB, 0, st, sp));
   if (max_per_pair > 0) {
-    TimingRec rec{nullptr, nullptr, TAG_MATCH_CAP};
-    LB_TRY(timing_begin(rec, st));
-    match_cap_kernel<<<n, kCapBlock, 0, st>>>(w.flag, w.conf, L, max_per_pair);
-    LB_LAUNCHED();
-    LB_TRY(timing_end(rec, st));
+    LB_TRY(launch(TAG_MATCH_CAP, match_cap_kernel, n, kCapBlock, 0, st, w.flag, w.conf, L, max_per_pair));
   }
 
   CompactParams cp;
@@ -1489,10 +1450,8 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
   cp.b_ids = a->b_ids; cp.i_ids = a->i_ids; cp.j_ids = a->j_ids;
   cp.mconf = a->mconf; cp.mkpts0 = a->mkpts0_c; cp.mkpts1 = a->mkpts1_c; cp.count = a->count;
   const int cblocks = cdiv(nl, kCompactBlock);
-  match_count_kernel<<<cblocks, kCompactBlock, 0, st>>>(w.flag, nl, w.blk_counts);
-  LB_LAUNCHED();
-  match_scatter_kernel<<<cblocks, kCompactBlock, 0, st>>>(cp, w.blk_counts);
-  LB_LAUNCHED();
+  LB_TRY(launch(TAG_NONE, match_count_kernel, cblocks, kCompactBlock, 0, st, w.flag, nl, w.blk_counts));
+  LB_TRY(launch(TAG_NONE, match_scatter_kernel, cblocks, kCompactBlock, 0, st, cp, w.blk_counts));
   return 0;
 }
 
@@ -1513,32 +1472,39 @@ int lb_coarse_match_fp16(const LbCoarseMatchArgs* a, int max_per_pair, void* ws,
 }
 
 // ------------------------------------------------------------------------------------------------ fine level
+struct FpWs {
+  __half* win_hi;   // [2*M*W*W, Cf] gathered windows
+  __half* win_lo;
+  float* gbias;     // [2*M, Cf] per-window bias of the merge
+};
+static void carve_fp(Bump& b, FpWs& w, long M, int W, int Cf) {
+  const size_t rows = static_cast<size_t>(2) * M * W * W;
+  w.win_hi = b.take<__half>(rows * Cf);
+  w.win_lo = b.take<__half>(rows * Cf);
+  w.gbias = b.take<float>(static_cast<size_t>(2) * M * Cf);
+}
+
 size_t lb_fine_preprocess_workspace_bytes(long M, int W, int Cf) {
   Bump b{nullptr, 0};
-  const size_t rows = static_cast<size_t>(2) * M * W * W;
-  b.take<__half>(rows * Cf);
-  b.take<__half>(rows * Cf);
-  b.take<float>(static_cast<size_t>(2) * M * Cf);
+  FpWs w;
+  carve_fp(b, w, M, W, Cf);
   return b.off + 256;
 }
 
 // img_idx0 / img_idx1: NULL, or pair b's windows are read from image img_idx0[b] of feat_f0 / img_idx1[b] of feat_f1
 static int fine_preprocess(const LbFinePreprocessArgs* a, const int* img_idx0, const int* img_idx1, void* ws,
                            size_t ws_bytes, void* stream) {
-  int sms;
   if (a->M <= 0) return 0;
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(a->x_f32));
-  LB_TRY(device_check(&sms));
+  DeviceScope dev;
+  LB_TRY(dev.bind(a->x_f32));
   if (a->Cf != 128 || a->Cc > 256) return fail("fine preprocess built for Cf=128, Cc<=256 (got %d, %d)", a->Cf, a->Cc);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int WW = a->W * a->W;
   const long rows = 2 * a->M * WW;
   if (!ws) return fail("workspace pointer is null");
   Bump b{static_cast<uint8_t*>(ws), ws_bytes};
-  __half* win_hi = b.take<__half>(static_cast<size_t>(rows) * a->Cf);
-  __half* win_lo = b.take<__half>(static_cast<size_t>(rows) * a->Cf);
-  float* gbias = b.take<float>(static_cast<size_t>(2) * a->M * a->Cf);
+  FpWs w;
+  carve_fp(b, w, a->M, a->W, a->Cf);
   if (!b.ok) return fail("fine-preprocess workspace too small");
 
   FineGatherParams g;
@@ -1548,21 +1514,16 @@ static int fine_preprocess(const LbFinePreprocessArgs* a, const int* img_idx0, c
   g.Hf0 = a->Hf0; g.Wf0 = a->Wf0; g.Hf1 = a->Hf1; g.Wf1 = a->Wf1;
   g.w0c = a->w0c; g.w1c = a->w1c; g.stride = a->stride; g.W = a->W; g.Cf = a->Cf; g.M = a->M;
   g.b_ids = a->b_ids; g.i_ids = a->i_ids; g.j_ids = a->j_ids;
-  g.out_hi = win_hi; g.out_lo = win_lo; g.ld = a->Cf;
+  g.out_hi = w.win_hi; g.out_lo = w.win_lo; g.ld = a->Cf;
   g.live = a->M_live;
   g.img_idx0 = img_idx0; g.img_idx1 = img_idx1;
   const bool vec8 = a->sc0 == 1 && a->sc1 == 1 && a->Cf % 8 == 0 && g.ld % 8 == 0 && a->sw0 % 4 == 0 && a->sw1 % 4 == 0 &&
                     a->sh0 % 4 == 0 && a->sh1 % 4 == 0 && a->sn0 % 4 == 0 && a->sn1 % 4 == 0 &&
                     (reinterpret_cast<uintptr_t>(a->feat_f0) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->feat_f1) & 15) == 0;
   const unsigned wins = static_cast<unsigned>(2 * a->M);
-  if (img_idx0) {
-    if (vec8) fine_gather_vec8_kernel<true><<<wins, 256, 0, st>>>(g);
-    else fine_gather_kernel<true><<<wins, 256, 0, st>>>(g);
-  } else {
-    if (vec8) fine_gather_vec8_kernel<false><<<wins, 256, 0, st>>>(g);
-    else fine_gather_kernel<false><<<wins, 256, 0, st>>>(g);
-  }
-  LB_LAUNCHED();
+  const auto gather = img_idx0 ? (vec8 ? fine_gather_vec8_kernel<true> : fine_gather_kernel<true>)
+                               : (vec8 ? fine_gather_vec8_kernel<false> : fine_gather_kernel<false>);
+  LB_TRY(launch(TAG_NONE, gather, wins, 256, 0, st, g));
 
   FineBiasParams fb;
   fb.feat_c = a->feat_c;
@@ -1570,21 +1531,22 @@ static int fine_preprocess(const LbFinePreprocessArgs* a, const int* img_idx0, c
   fb.L = a->L; fb.S = a->S; fb.Cc = a->Cc; fb.Cf = a->Cf; fb.M = a->M;
   fb.b_ids = a->b_ids; fb.i_ids = a->i_ids; fb.j_ids = a->j_ids;
   fb.WdT = a->down_wt; fb.bd = a->down_b; fb.Wm2T = a->merge_w2t; fb.bm = a->merge_b;
-  fb.gbias = gbias;
+  fb.gbias = w.gbias;
   fb.live = a->M_live;
-  fine_bias_kernel<<<static_cast<unsigned>(cdiv(2 * a->M, kFineBiasWin)), 128, 0, st>>>(fb);
-  LB_LAUNCHED();
+  LB_TRY(launch(TAG_NONE, fine_bias_kernel, static_cast<unsigned>(cdiv(2 * a->M, kFineBiasWin)), 128, 0, st, fb));
 
   // merge_feat over [window | coarse] = window @ Wm[:, :Cf]^T + per-window bias     [fine_preprocess.py:52-56]
   // With a device bound each side is one GEMM batch of M*WW rows (M = capacity) with its own live prefix.
   using Epi = EpiPlanes<128>;
   const int nb = a->M_live ? 2 : 1;
   const long rows_b = rows / nb;
-  Planes A{win_hi, win_lo, a->Cf, nb > 1 ? rows_b * a->Cf : 0};
+  Planes A{w.win_hi, w.win_lo, a->Cf, nb > 1 ? rows_b * a->Cf : 0};
   Planes B{a->merge_w_hi, a->merge_w_lo, a->Cf, 0};
-  Epi::Params ep{0, gbias, WW, a->merge_acc_scale, {}};
+  Epi::Params ep{0, w.gbias, WW, a->merge_acc_scale, {}};
   LB_TRY(fill_out_maps(&ep.om, a->cat_hi, a->cat_lo, 2 * a->Cf, a->x_f32, a->Cf, a->Cf, rows_b, nb));
-  return launch_gemm<128, Epi>(TAG_FINE_MERGE, A, B, nb, static_cast<int>(rows_b), a->Cf, a->Cf, 0, ep, st, a->M_live, WW);
+  return launch_gemm<128, Epi>(TAG_FINE_MERGE, A, B,
+                               gemm_shape<128>(nb, static_cast<int>(rows_b), a->Cf, a->Cf, false, 0, a->M_live, WW),
+                               ep, dev.sms, st);
 }
 
 int lb_fine_preprocess(const LbFinePreprocessArgs* a, void* ws, size_t ws_bytes, void* stream) {
@@ -1598,11 +1560,9 @@ int lb_fine_preprocess_indexed(const LbFinePreprocessArgs* a, const int* img_idx
 }
 
 int lb_fine_match(const LbFineMatchArgs* a, void* stream) {
-  int sms;
   if (a->M <= 0) return 0;
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(a->expec_f));
-  LB_TRY(device_check(&sms));
+  DeviceScope dev;
+  LB_TRY(dev.bind(a->expec_f));
   if (a->W * a->W > 32) return fail("fine window %dx%d exceeds one warp", a->W, a->W);
   FineMatchParams p;
   p.f0 = a->f0; p.f1 = a->f1; p.W = a->W; p.C = a->C; p.M = a->M;
@@ -1610,24 +1570,19 @@ int lb_fine_match(const LbFineMatchArgs* a, void* stream) {
   p.mkpts1_c = a->mkpts1_c; p.expec_f = a->expec_f; p.mkpts1_f = a->mkpts1_f;
   p.live = a->M_live;
   const int warps_per_block = 8;
-  fine_match_kernel<<<cdiv(a->M, warps_per_block), warps_per_block * 32, 0, static_cast<cudaStream_t>(stream)>>>(p);
-  LB_LAUNCHED();
-  return 0;
+  return launch(TAG_NONE, fine_match_kernel, cdiv(a->M, warps_per_block), warps_per_block * 32, 0,
+                static_cast<cudaStream_t>(stream), p);
 }
 
 // ------------------------------------------------------------------------------------------------ evaluation
 int lb_epipolar_errors(const float* mkpts0_f, const float* mkpts1_f, const long long* m_bids, long M, int n_pairs,
                        const float* T_0to1, const float* K0, const float* K1, float* epi_errs, void* stream) {
   if (M <= 0) return 0;
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(epi_errs));
-  int sms;
-  LB_TRY(device_check(&sms));
+  DeviceScope dev;
+  LB_TRY(dev.bind(epi_errs));
   if (!mkpts0_f || !mkpts1_f || !m_bids || !T_0to1 || !K0 || !K1) return fail("lb_epipolar_errors: null input");
-  epipolar_error_kernel<<<cdiv(M, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(mkpts0_f, mkpts1_f, m_bids, M, n_pairs,
-                                                                                      T_0to1, K0, K1, epi_errs);
-  LB_LAUNCHED();
-  return 0;
+  return launch(TAG_NONE, epipolar_error_kernel, cdiv(M, 256), 256, 0, static_cast<cudaStream_t>(stream), mkpts0_f,
+                mkpts1_f, m_bids, M, n_pairs, T_0to1, K0, K1, epi_errs);
 }
 
 // ------------------------------------------------------------------------------------------------ two-view geometry
@@ -1667,10 +1622,8 @@ int lb_estimate_geometry(const float* pts0, const float* pts1, const uint8_t* va
   size_t off_col, off_n, off_best;
   const size_t need = geometry_ws_layout(B, K, iterations, &off_col, &off_n, &off_best);
   if (ws_bytes < need) return fail("lb_estimate_geometry: workspace of %zu bytes, %zu needed", ws_bytes, need);
-  int sms;
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(model_out));
-  LB_TRY(device_check(&sms));
+  DeviceScope dev;
+  LB_TRY(dev.bind(model_out));
   GeoParams p;
   p.pts0 = pts0; p.pts1 = pts1; p.valid = valid; p.pair_ids = pair_ids;
   p.B = B; p.K = K; p.model = model; p.iterations = iterations; p.n_tiles = cdiv(iterations, kGeoHypPerBlock);
@@ -1684,16 +1637,12 @@ int lb_estimate_geometry(const float* pts0, const float* pts1, const uint8_t* va
   p.model_out = model_out; p.mask_out = mask_out; p.count_out = count_out;
   p.best_out = best_out; p.samples_out = samples_out;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  TimingRec rec{nullptr, nullptr, TAG_GEOMETRY};
-  LB_TRY(timing_begin(rec, st));
-  geometry_compact_kernel<<<B, kGeoRefitThreads, 0, st>>>(p);
-  LB_LAUNCHED();
-  geometry_score_kernel<<<dim3(p.n_tiles, B), kGeoHypPerBlock, 0, st>>>(p);
-  LB_LAUNCHED();
-  geometry_refit_kernel<<<B, kGeoRefitThreads, 0, st>>>(p);
-  LB_LAUNCHED();
-  LB_TRY(timing_end(rec, st));
-  return 0;
+  TimedRange timed;   // the three launches are one record
+  LB_TRY(timed.begin(TAG_GEOMETRY, st));
+  LB_TRY(launch(TAG_NONE, geometry_compact_kernel, B, kGeoRefitThreads, 0, st, p));
+  LB_TRY(launch(TAG_NONE, geometry_score_kernel, dim3(p.n_tiles, B), kGeoHypPerBlock, 0, st, p));
+  LB_TRY(launch(TAG_NONE, geometry_refit_kernel, B, kGeoRefitThreads, 0, st, p));
+  return timed.end();
 }
 
 // ------------------------------------------------------------------------------------------------ multi-GPU
@@ -1711,20 +1660,12 @@ int lb_comm_init(const char* id_bytes, int rank, int world, int device, const ch
   if (!id_bytes || !comm_out || world <= 0 || rank < 0 || rank >= world) return fail("lb_comm_init: bad arguments");
   NcclApi* api = nccl_api(nccl_lib_path);
   if (!api) return fail("NCCL library not found (dlopen of libnccl.so.2 failed; set LOFTR_B200_NCCL_LIB)");
-  int prev = -1;
-  LB_CUDA(cudaGetDevice(&prev));
-  LB_CUDA(cudaSetDevice(device));
-  int sms;
-  int rc0 = device_check(&sms);
-  if (rc0) {
-    cudaSetDevice(prev);
-    return rc0;
-  }
+  DeviceScope dev;
+  LB_TRY(dev.bind_device(device));
   NcclApi::UniqueId id;
   memcpy(id.internal, id_bytes, LB_NCCL_UNIQUE_ID_BYTES);
   void* nccl = nullptr;
   const int rc = api->CommInitRank(&nccl, world, id, rank);
-  cudaSetDevice(prev);
   if (rc != 0) return fail("ncclCommInitRank failed: %s", api->GetErrorString ? api->GetErrorString(rc) : "?");
   *comm_out = new LbComm{nccl, rank, world, device};
   return 0;
@@ -1741,22 +1682,20 @@ int lb_comm_destroy(void* comm) {
 
 int lb_pack_matches(const float* mkpts0_f, const float* mkpts1_f, const float* mconf, const long long* m_bids,
                     long count, int pair_offset, float* wire, long capacity, void* stream) {
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(wire));
+  DeviceScope dev;
+  LB_TRY(dev.bind(wire));
   if (count > capacity) return fail("lb_pack_matches: %ld matches exceed the wire capacity %ld", count, capacity);
   if (count > 0 && (!mkpts0_f || !mkpts1_f || !mconf || !m_bids)) return fail("lb_pack_matches: null input");
   const long n = count > 0 ? count : 1;
-  pack_matches_kernel<<<cdiv(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(mkpts0_f, mkpts1_f, mconf, m_bids, count,
-                                                                                    pair_offset, wire, capacity);
-  LB_LAUNCHED();
-  return 0;
+  return launch(TAG_NONE, pack_matches_kernel, cdiv(n, 256), 256, 0, static_cast<cudaStream_t>(stream), mkpts0_f,
+                mkpts1_f, mconf, m_bids, count, pair_offset, wire, capacity);
 }
 
 int lb_allgather_matches(void* comm, const float* wire_send, float* wire_recv, long capacity, void* stream) {
   if (!comm) return fail("lb_allgather_matches: null communicator");
   LbComm* c = static_cast<LbComm*>(comm);
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(wire_recv));
+  DeviceScope dev;
+  LB_TRY(dev.bind(wire_recv));
   NcclApi* api = nccl_api(nullptr);
   if (!api) return fail("NCCL library not loaded");
   const size_t count = static_cast<size_t>(1 + capacity) * kWireCols;
@@ -1767,14 +1706,12 @@ int lb_allgather_matches(void* comm, const float* wire_send, float* wire_recv, l
 
 int lb_unpack_matches(const float* wire_recv, int world, long capacity, float* mkpts0_f, float* mkpts1_f, float* mconf,
                       long long* m_bids, long out_capacity, int* counts_out, void* stream) {
-  DeviceGuard dev_guard;
-  LB_TRY(dev_guard.bind(wire_recv));
+  DeviceScope dev;
+  LB_TRY(dev.bind(wire_recv));
   if (world <= 0 || capacity < 0) return fail("lb_unpack_matches: bad arguments");
   const long n = capacity > 0 ? capacity : 1;
-  unpack_matches_kernel<<<dim3(cdiv(n, 256), world), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      wire_recv, world, capacity, mkpts0_f, mkpts1_f, mconf, m_bids, out_capacity, counts_out);
-  LB_LAUNCHED();
-  return 0;
+  return launch(TAG_NONE, unpack_matches_kernel, dim3(cdiv(n, 256), world), 256, 0, static_cast<cudaStream_t>(stream),
+                wire_recv, world, capacity, mkpts0_f, mkpts1_f, mconf, m_bids, out_capacity, counts_out);
 }
 
 }  // extern "C"

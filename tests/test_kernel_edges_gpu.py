@@ -90,7 +90,7 @@ def _model(W=5, coarse="linear", fine="linear", device=DEV):
 
 # ------------------------------------------------------------------------------------------------ coarse matching
 def cm_launch(n, L, S, sms):
-    """Mirror of lb_coarse_match's chunking (engine.cu pick_chunks, kMaxChunks, the tpc / n_chunks mirror)."""
+    """Mirror of lb_coarse_match's chunking (engine.cu pick_chunks, kMaxChunks, gemm_shape's tpc / n_chunks)."""
     m_tiles, n_tiles = _cdiv(L, BLOCK_M), _cdiv(S, SCORE_BN)
     raw = 1
     while n * m_tiles * raw < 40 * sms and raw < n_tiles:
@@ -207,7 +207,7 @@ def test_conf_matrix_multi_chunk_vs_f64(match_type):
 
 # ------------------------------------------------------------------------------------------------ transformers
 def kv_splits(n_groups, rows, sms):
-    """Mirror of the split-K count of kv_gemm_kernel (engine.cu tf_linear_attention_coarse)."""
+    """Mirror of the split-K count of kv_gemm_kernel (engine.cu kv_splits)."""
     kb_total = _cdiv(rows, 64)
     parts_cap = max(_cdiv(rows, BLOCK_M), KV_SPLITS)
     s = min(max(sms // (2 * n_groups), 1), kb_total, parts_cap)
