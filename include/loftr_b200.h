@@ -58,7 +58,8 @@ extern "C" {
  * 106: lb_preprocess_images (uint8 images of any size -> the matcher's padded fp32 input and 1/8 mask);
  * 107: lb_estimate_geometry (batched RANSAC homography / fundamental matrix per pair);
  * 108: lb_backbone_workspace_bytes_fp16 / lb_backbone_forward_fp16 (single-pass fp16 backbone);
- * 109: lb_transformer_forward_fp16 / lb_coarse_match_fp16 (single-pass fp16 transformers and coarse matching). */
+ * 109: lb_transformer_forward_fp16 / lb_coarse_match_fp16 (single-pass fp16 transformers and coarse matching);
+ * 110: lb_gemm_fp16 (test hook of the contraction core on single fp16 planes). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -89,6 +90,11 @@ int lb_split_planes(const float* x, long rows, int cols, int ld_x, void* hi, voi
 int lb_gemm_split(const void* a_hi, const void* a_lo, long lda, long a_batch_stride, const void* b_hi,
                   const void* b_lo, long ldb, long b_batch_stride, float* out, long ldo, long o_batch_stride,
                   int batches, int M, int N, int K, void* stream);
+/* The same product on the hi planes only, one fp16 MMA per k-step with fp32 accumulation (version 110): the kernels of
+ * match_precision "fp16" (DESIGN.md §16).  Same arguments as lb_gemm_split; a_lo and b_lo are not read and may be NULL. */
+int lb_gemm_fp16(const void* a_hi, const void* a_lo, long lda, long a_batch_stride, const void* b_hi,
+                 const void* b_lo, long ldb, long b_batch_stride, float* out, long ldo, long o_batch_stride,
+                 int batches, int M, int N, int K, void* stream);
 
 /* ---- image front end.  Replaces, for a whole batch in one launch, the per-image host work of the reference's dataset
  * readers (src/utils/dataset.py: imread_gray's colour conversion :47-51, get_resized_wh / get_divisible_wh are the

@@ -114,6 +114,8 @@ SIGNATURES = {
     "lb_split_planes": (c_int, [c_void_p, c_long, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "lb_gemm_split": (c_int, [c_void_p, c_void_p, c_long, c_long, c_void_p, c_void_p, c_long, c_long, c_void_p,
                               c_long, c_long, c_int, c_int, c_int, c_int, c_void_p]),
+    "lb_gemm_fp16": (c_int, [c_void_p, c_void_p, c_long, c_long, c_void_p, c_void_p, c_long, c_long, c_void_p,
+                             c_long, c_long, c_int, c_int, c_int, c_int, c_void_p]),
     "lb_preprocess_images": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "lb_geometry_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "lb_estimate_geometry": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int,
@@ -172,13 +174,16 @@ GEOMETRY_VERSION = 107
 BACKBONE_FP16_VERSION = 108
 # oldest library with the single-pass fp16 transformers and coarse matching (match_precision="fp16")
 MATCH_FP16_VERSION = 109
+# oldest library with the contraction core's single-plane test hook (lb_gemm_fp16)
+GEMM_FP16_VERSION = 110
 GEOMETRY_HOMOGRAPHY = 0
 GEOMETRY_FUNDAMENTAL = 1
 _SINCE = {"lb_coarse_prep_indexed": FEATURE_BANK_VERSION, "lb_fine_preprocess_indexed": FEATURE_BANK_VERSION,
           "lb_coarse_match_capped": MATCH_CAP_VERSION, "lb_preprocess_images": PREPROCESS_VERSION,
           "lb_geometry_workspace_bytes": GEOMETRY_VERSION, "lb_estimate_geometry": GEOMETRY_VERSION,
           "lb_backbone_workspace_bytes_fp16": BACKBONE_FP16_VERSION, "lb_backbone_forward_fp16": BACKBONE_FP16_VERSION,
-          "lb_transformer_forward_fp16": MATCH_FP16_VERSION, "lb_coarse_match_fp16": MATCH_FP16_VERSION}
+          "lb_transformer_forward_fp16": MATCH_FP16_VERSION, "lb_coarse_match_fp16": MATCH_FP16_VERSION,
+          "lb_gemm_fp16": GEMM_FP16_VERSION}
 
 
 class LibraryMissing(RuntimeError):

@@ -941,9 +941,37 @@ static int tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const Lb
   return 0;
 }
 
+// The test hooks of the contraction core: gemm_split_kernel<BN, Operands<EpiActStore<BN>, kP>> at BN 256 / 128, the
+// instantiations the transformers run (kP = 1 reads the hi planes only: a_lo / b_lo may be null).
+template <int kP>
+static int gemm_test(const char* who, const void* a_hi, const void* a_lo, long lda, long a_batch_stride,
+                     const void* b_hi, const void* b_lo, long ldb, long b_batch_stride, float* out, long ldo,
+                     long o_batch_stride, int batches, int M, int N, int K, void* stream) {
+  if (N % 32 != 0) return fail("%s: N must be a multiple of 32", who);
+  DeviceScope dev;
+  LB_TRY(dev.bind(out));
+  if (batches > 1 && o_batch_stride != static_cast<long>(M) * ldo)
+    return fail("%s: output batches must be densely stacked (o_batch_stride == M*ldo)", who);
+  Planes A{a_hi, a_lo, lda, batches > 1 ? a_batch_stride : 0};
+  Planes B{b_hi, b_lo, ldb, b_batch_stride};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  OutMaps om;
+  LB_TRY(fill_out_maps(&om, nullptr, nullptr, 0, out, ldo, N, M, batches));
+  if (N % 256 == 0 || N > 128) {
+    using Epi = Operands<EpiActStore<256>, kP>;
+    typename Epi::Params ep{0, nullptr, 1.f, om};
+    return launch_gemm<256, Epi>(TAG_GEMM_TEST, A, B, gemm_shape<256>(batches, M, N, K, b_batch_stride > 0), ep,
+                                 dev.sms, st);
+  }
+  using Epi = Operands<EpiActStore<128>, kP>;
+  typename Epi::Params ep{0, nullptr, 1.f, om};
+  return launch_gemm<128, Epi>(TAG_GEMM_TEST, A, B, gemm_shape<128>(batches, M, N, K, b_batch_stride > 0), ep, dev.sms,
+                               st);
+}
+
 extern "C" {
 
-int lb_version(void) { return 109; }
+int lb_version(void) { return 110; }
 int lb_block_k(void) { return kBlockK; }
 int lb_conv_layout(int cin, int* cin_blocks, int* rem_channels) {
   if (!cin_blocks || !rem_channels || cin <= 0) return fail("lb_conv_layout: bad arguments");
@@ -997,26 +1025,15 @@ int lb_split_planes(const float* x, long rows, int cols, int ld_x, void* hi, voi
 int lb_gemm_split(const void* a_hi, const void* a_lo, long lda, long a_batch_stride, const void* b_hi,
                   const void* b_lo, long ldb, long b_batch_stride, float* out, long ldo, long o_batch_stride,
                   int batches, int M, int N, int K, void* stream) {
-  if (N % 32 != 0) return fail("lb_gemm_split: N must be a multiple of 32");
-  DeviceScope dev;
-  LB_TRY(dev.bind(out));
-  if (batches > 1 && o_batch_stride != static_cast<long>(M) * ldo)
-    return fail("lb_gemm_split: output batches must be densely stacked (o_batch_stride == M*ldo)");
-  Planes A{a_hi, a_lo, lda, batches > 1 ? a_batch_stride : 0};
-  Planes B{b_hi, b_lo, ldb, b_batch_stride};
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  OutMaps om;
-  LB_TRY(fill_out_maps(&om, nullptr, nullptr, 0, out, ldo, N, M, batches));
-  if (N % 256 == 0 || N > 128) {
-    using Epi = EpiActStore<256>;
-    Epi::Params ep{0, nullptr, 1.f, om};
-    return launch_gemm<256, Epi>(TAG_GEMM_TEST, A, B, gemm_shape<256>(batches, M, N, K, b_batch_stride > 0), ep,
-                                 dev.sms, st);
-  }
-  using Epi = EpiActStore<128>;
-  Epi::Params ep{0, nullptr, 1.f, om};
-  return launch_gemm<128, Epi>(TAG_GEMM_TEST, A, B, gemm_shape<128>(batches, M, N, K, b_batch_stride > 0), ep, dev.sms,
-                               st);
+  return gemm_test<2>("lb_gemm_split", a_hi, a_lo, lda, a_batch_stride, b_hi, b_lo, ldb, b_batch_stride, out, ldo,
+                      o_batch_stride, batches, M, N, K, stream);
+}
+
+int lb_gemm_fp16(const void* a_hi, const void* a_lo, long lda, long a_batch_stride, const void* b_hi,
+                 const void* b_lo, long ldb, long b_batch_stride, float* out, long ldo, long o_batch_stride,
+                 int batches, int M, int N, int K, void* stream) {
+  return gemm_test<1>("lb_gemm_fp16", a_hi, a_lo, lda, a_batch_stride, b_hi, b_lo, ldb, b_batch_stride, out, ldo,
+                      o_batch_stride, batches, M, N, K, stream);
 }
 
 int lb_preprocess_images(const LbImageDesc* descs, int n_images, float* out, int H, int W, uint8_t* mask,

@@ -10,7 +10,9 @@ Conventions that differ from the reference:
 
 With `fp16=True` the transformer and score-matrix stages emulate the single-pass fp16 matching mode
 (`match_precision="fp16"`, lb_transformer_forward_fp16 / lb_coarse_match_fp16; DESIGN.md §16): every tensor-core
-product multiplies the hi planes of its operands and accumulates exactly.
+product multiplies the hi planes of its operands and accumulates exactly.  The emulation keeps the dtype of its
+inputs: run on float32 tensors (inputs and `layer_weights(..., dtype=torch.float32)`), the same code is the fp32 oracle
+of the fp16 semantics, whose distance from the float64 run measures what fp32 accumulation alone costs.
 - an activation operand is fp16(x) (round to nearest even) of the value the split path stores as hi + lo;
 - a weight operand is fp16(w * 2^e) * 2^-e, with e = `weight_exponent` of the packed matrix (q|k|v share the exponent
   of their concatenation, as in `LocalFeatureTransformer._build`);
@@ -29,6 +31,12 @@ import torch.nn.functional as F
 
 F64 = torch.float64
 INF = 1e9  # coarse_matching.py:6
+# Defects the fp16 emulation can be run with, so that tests/test_match_fp16_rule_cpu.py can show that the accuracy rule
+# of the fp16 kernels sees each of them.  Empty everywhere else.
+#   residual_hi   the residual read as hi only          p_row_sum     P rounded to fp16 in the row sum too
+#   ksum_exact    Ksum taken from the unrounded K       merge_block   K block [64, 128) of the merge product dropped
+#   key_tile      source keys [64, 128) treated as valid in the attention
+DEFECTS = frozenset()
 
 
 def f64(x, device=None):
@@ -43,8 +51,8 @@ def r16(t, rounding=True):
 
 
 def w16(w, e, rounding=True):
-    """hi weight plane fp16(w * 2^e) as a value: fp16(w * 2^e) * 2^-e."""
-    return (w * 2.0 ** e).half().double() * 2.0 ** (-e) if rounding else w
+    """hi weight plane fp16(w * 2^e) as a value in w's dtype: fp16(w * 2^e) * 2^-e."""
+    return (w * 2.0 ** e).half().to(w.dtype) * 2.0 ** (-e) if rounding else w
 
 
 def layer_exponents(w):
@@ -62,15 +70,17 @@ def linear_attention(q, k, v, q_mask=None, kv_mask=None, eps=1e-6, fp16=False):
     Q = F.elu(q) + 1                                                    # :31-32
     K = F.elu(k) + 1
     if q_mask is not None:                                              # :35-39
-        Q = Q * q_mask[:, :, None, None].to(F64)
+        Q = Q * q_mask[:, :, None, None].to(Q.dtype)
     if kv_mask is not None:
-        K = K * kv_mask[:, :, None, None].to(F64)
-        v = v * kv_mask[:, :, None, None].to(F64)
+        K = K * kv_mask[:, :, None, None].to(K.dtype)
+        v = v * kv_mask[:, :, None, None].to(v.dtype)
+    Ksum = K.sum(dim=1) if fp16 and "ksum_exact" in DEFECTS else None
     K, v = r16(K, fp16), r16(v, fp16)
+    Ksum = K.sum(dim=1) if Ksum is None else Ksum
     v_length = v.shape[1]
     v = v / v_length                                                    # :41-42
     KV = torch.einsum("nshd,nshv->nhdv", K, v)                          # :43
-    Z = 1 / (torch.einsum("nlhd,nhd->nlh", Q, K.sum(dim=1)) + eps)     # :44
+    Z = 1 / (torch.einsum("nlhd,nhd->nlh", Q, Ksum) + eps)             # :44
     return torch.einsum("nlhd,nhdv,nlh->nlhv", Q, KV, Z) * v_length    # :45
 
 
@@ -79,7 +89,7 @@ def full_attention(q, k, v, q_mask=None, kv_mask=None, block=1024, fp16=False):
     V rounded and P rounded once in P V, not in the row sum (full_attn_wgmma_fp16_kernel)."""
     q, k, v = r16(q, fp16), r16(k, fp16), r16(v, fp16)
     n, L, H, D = q.shape
-    out = torch.zeros(n, L, H, D, dtype=F64, device=q.device)
+    out = torch.zeros(n, L, H, D, dtype=q.dtype, device=q.device)
     for lo in range(0, L, block):
         hi = min(lo + block, L)
         s = torch.einsum("nlhd,nshd->nlsh", q[:, lo:hi], k) / math.sqrt(D)   # :69, :74
@@ -88,7 +98,7 @@ def full_attention(q, k, v, q_mask=None, kv_mask=None, block=1024, fp16=False):
             s = s.masked_fill(~ok, float("-inf"))
         m = s.amax(dim=2, keepdim=True)                                 # softmax over s  :74-75
         p = torch.exp(s - torch.where(torch.isinf(m), torch.zeros_like(m), m))
-        den = p.sum(dim=2)[..., None]                                   # [n, l, h, 1]; 0: no valid key
+        den = r16(p, fp16 and "p_row_sum" in DEFECTS).sum(dim=2)[..., None]   # [n, l, h, 1]; 0: no valid key
         num = torch.einsum("nlsh,nshd->nlhd", r16(p, fp16), v)         # :79
         out[:, lo:hi] = torch.where(den > 0, num / den.clamp_min(1e-300), torch.zeros_like(num))
     return out
@@ -107,22 +117,29 @@ def encoder_layer(x, source, w, nhead, x_mask=None, source_mask=None, attention=
     k = (sh @ wt("k_proj.weight", "qkv").T).view(bs, -1, nhead, dim)   # :48
     v = (sh @ wt("v_proj.weight", "qkv").T).view(bs, -1, nhead, dim)   # :49
     att = linear_attention if attention == "linear" else full_attention
+    if fp16 and "key_tile" in DEFECTS and source_mask is not None:
+        source_mask = source_mask.clone()
+        source_mask[:, 64:128] = True
     msg = att(q, k, v, x_mask, source_mask, fp16=fp16 and dim == 32)   # :50
-    msg = r16(msg.reshape(bs, -1, c), fp16) @ wt("merge.weight", "merge").T   # :51
+    msg = r16(msg.reshape(bs, -1, c), fp16)
+    if fp16 and "merge_block" in DEFECTS:
+        msg = torch.cat([msg[..., :64], torch.zeros_like(msg[..., 64:128]), msg[..., 128:]], -1)
+    msg = msg @ wt("merge.weight", "merge").T                           # :51
     msg = F.layer_norm(msg, (c,), w["norm1.weight"], w["norm1.bias"])   # :52
     h = torch.relu(r16(torch.cat([x, msg], 2), fp16) @ wt("mlp.0.weight", "mlp0").T)   # :55
     msg = r16(h, fp16) @ wt("mlp.2.weight", "mlp2").T
     msg = F.layer_norm(msg, (c,), w["norm2.weight"], w["norm2.bias"])   # :56
-    return x + msg                                                      # :58
+    return (r16(x) if fp16 and "residual_hi" in DEFECTS else x) + msg  # :58
 
 
-def layer_weights(tf_module, device=None):
-    """float64 per-layer weight dicts of a loftr_b200 LocalFeatureTransformer (same names as the reference)."""
+def layer_weights(tf_module, device=None, dtype=F64):
+    """float64 (or `dtype`) per-layer weight dicts of a loftr_b200 LocalFeatureTransformer (same names as the
+    reference)."""
     sd = tf_module.state_dict()
     out = []
     for i in range(len(tf_module.layers)):
         pre = f"layers.{i}."
-        out.append({k[len(pre):]: f64(v, device) for k, v in sd.items() if k.startswith(pre)})
+        out.append({k[len(pre):]: f64(v, device).to(dtype) for k, v in sd.items() if k.startswith(pre)})
     return out
 
 

@@ -140,11 +140,13 @@ def test_fp16_matching_refuses_an_older_library(monkeypatch):
     loftr_b200.LoFTR(copy.deepcopy(cfg), backbone_impl="b200_fp16")   # the split matching needs nothing new
 
 
-def test_fp16_entry_points_are_bound_and_check_k():
+def test_fp16_entry_points_and_the_gemm_hook_are_bound_and_check_arguments():
     lib = _lib.load()
-    assert lib.lb_version() == _lib.MATCH_FP16_VERSION
-    for name in ("lb_transformer_forward_fp16", "lb_coarse_match_fp16"):
+    assert lib.lb_version() == _lib.GEMM_FP16_VERSION > _lib.MATCH_FP16_VERSION
+    for name in ("lb_transformer_forward_fp16", "lb_coarse_match_fp16", "lb_gemm_fp16"):
         assert _lib.SIGNATURES[name][1] == getattr(lib, name).argtypes
+    assert lib.lb_gemm_fp16(None, None, 64, 0, None, None, 64, 0, None, 80, 0, 1, 128, 80, 64, None) != 0
+    assert b"lb_gemm_fp16: N must be a multiple of 32" in lib.lb_last_error()
     a = _lib.LbCoarseMatchArgs()
     for k in (-1, -7):
         assert lib.lb_coarse_match_fp16(C.byref(a), k, None, 0, None) != 0

@@ -1,7 +1,7 @@
-"""What tests/test_gemm_pipeline_gpu.py and tests/test_backbone_widths_gpu.py reach, replayed on the CPU from the ring
-constants of the sources (read with regular expressions) and a mirror of engine.cu's conv_layout.  These tests fail
-when a change to the kernels' shared-memory budget or to those files' cases leaves the tile hand-off or the
-convolution layouts they were written for uncovered."""
+"""What tests/test_gemm_pipeline_gpu.py, tests/test_gemm_pipeline_fp16_gpu.py and tests/test_backbone_widths_gpu.py
+reach, replayed on the CPU from the ring constants of the sources (read with regular expressions) and a mirror of
+engine.cu's conv_layout.  These tests fail when a change to the kernels' shared-memory budget or to those files' cases
+leaves the tile hand-off or the convolution layouts they were written for uncovered."""
 import collections
 import os
 import re
@@ -10,6 +10,7 @@ import pytest
 import torch
 
 import test_backbone_widths_gpu as widths
+import test_gemm_pipeline_fp16_gpu as pipeline16
 import test_gemm_pipeline_gpu as pipeline
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -42,15 +43,15 @@ OWN_XPOSE = _int(r"kSmemBytes = kXposeOffset \+ \(kOwnXpose \? ([^:]+) :", "epil
 TAPS = 9
 
 
-def gemm_ring(bn, epi_bytes):
-    """GemmSmem<bn, epi_bytes> with hi and lo planes: (K per stage, ring stages, stages under the staged accumulator,
-    remainder taps per stage)."""
-    bk = BLOCK_K // 2
-    stage = 2 * (BLOCK_M + bn) * bk * 2
+def gemm_ring(bn, epi_bytes, planes=2):
+    """GemmSmem<bn, epi_bytes, planes> (hi and lo planes, or hi only): (K per stage, ring stages, stages under the
+    staged accumulator, remainder taps per stage)."""
+    bk = BLOCK_K // planes
+    stage = planes * (BLOCK_M + bn) * bk * 2
     stages = min((SMEM_LIMIT - BAR_BYTES - epi_bytes) // stage, RING_WANT // stage)
     acc_stages = -(-((BLOCK_M * (bn + ACC_PAD) + ACC_TAIL) * 4) // stage)
     assert acc_stages < stages
-    return bk, stages, acc_stages, stage // (2 * (BLOCK_M + bn) * REM_CHANNELS * 2)
+    return bk, stages, acc_stages, stage // (planes * (BLOCK_M + bn) * REM_CHANNELS * 2)
 
 
 def conv_epi_bytes(bn, upsample):
@@ -85,10 +86,10 @@ def test_conv_layout_mirror_matches_the_library():
         assert (cb.value, rem.value) == conv_layout(cin), cin
 
 
-def gemm_schedule(n, k, batches, rem, sms):
-    """Per CTA of one lb_gemm_split launch: a list of (last ring stage, staging wraps, next tile's first load lands in
-    a staged stage) for each of its tiles."""
-    bk, ring, acc, _ = gemm_ring(pipeline.block_n(n), EPI_SCRATCH)
+def gemm_schedule(n, k, batches, rem, sms, planes=2):
+    """Per CTA of one lb_gemm_split (planes = 2) or lb_gemm_fp16 (planes = 1) launch: a list of (last ring stage,
+    staging wraps, next tile's first load lands in a staged stage) for each of its tiles."""
+    bk, ring, acc, _ = gemm_ring(pipeline.block_n(n), EPI_SCRATCH, planes)
     _, _, items = pipeline.launch_shape(n, batches, rem, sms)
     grid = min(items, sms)
     stages = k // bk
@@ -104,13 +105,22 @@ def gemm_schedule(n, k, batches, rem, sms):
     return ctas
 
 
-def test_gemm_ring_is_the_one_the_table_describes():
-    """lb_gemm_split's epilogue (EpiActStore) takes kEpiScratchBytes, and its rings are those of the table in
-    tests/test_gemm_pipeline_gpu.py: 32 of K per stage, 4 / 6 stages at BLOCK_N 256 / 128, 3 under the staging."""
+def test_gemm_rings_are_the_ones_the_tables_describe():
+    """lb_gemm_split's and lb_gemm_fp16's epilogue (EpiActStore, with EpiF16Operands adding nothing but the plane
+    count) takes kEpiScratchBytes, and its rings are those of the tables in tests/test_gemm_pipeline_gpu.py and
+    tests/test_gemm_pipeline_fp16_gpu.py: 32 / 64 of K per stage with two planes / one, 4 / 6 stages at BLOCK_N
+    256 / 128, 3 under the staging."""
     m = re.search(r"struct EpiActStore \{.*?kSmemBytes = (\w+);", SRC["epilogues.cuh"], re.S)
     assert m and m.group(1) == "kEpiScratchBytes"
-    assert re.search(r"using Epi = EpiActStore<256>;", SRC["engine.cu"])
+    m = re.search(r"struct EpiF16Operands : Epi \{(.*?)\};", SRC["epilogues.cuh"], re.S)
+    assert m and m.group(1).split() == ["using", "Epi::Epi;", "static", "constexpr", "int", "kOperandPlanes", "=", "1;"]
+    m = re.search(r"static int gemm_test\(.*?\n\}\n", SRC["engine.cu"], re.S)
+    assert m, "gemm_test not found in engine.cu"
+    assert re.findall(r"using Epi = Operands<EpiActStore<(\d+)>, kP>;", m.group(0)) == ["256", "128"]
+    assert re.search(r"int lb_gemm_split\([^{]*\{\s*return gemm_test<2>\(", SRC["engine.cu"])
+    assert re.search(r"int lb_gemm_fp16\([^{]*\{\s*return gemm_test<1>\(", SRC["engine.cu"])
     assert [gemm_ring(bn, EPI_SCRATCH)[:3] for bn in (256, 128)] == [(32, 4, 3), (32, 6, 3)]
+    assert [gemm_ring(bn, EPI_SCRATCH, 1)[:3] for bn in (256, 128)] == [(64, 4, 3), (64, 6, 3)]
 
 
 @pytest.mark.parametrize("sms", [114, 132])
@@ -127,6 +137,33 @@ def test_gemm_pipeline_launches_reach_the_tile_hand_off(sms):
         k64 |= k == 64
     assert wraps and no_wraps and staged_first_load and k64
     assert {pipeline.block_n(n) for n, *_ in pipeline.CASES} == {128, 256}
+
+
+@pytest.mark.parametrize("sms", [114, 132])
+def test_gemm_fp16_pipeline_launches_reach_the_tile_hand_off(sms):
+    """The one-plane ring at both column tiles: staging that wraps and that does not, 1- and 2-stage tiles (fewer than
+    the 3 the staging covers), and at BLOCK_N 256 a next tile whose first load lands in the staging.  At BLOCK_N 128
+    (ring 6, staging 3) no ring position can stage the next tile's first load."""
+    seen = {bn: collections.Counter() for bn in (128, 256)}
+    for n, k, batches, rem, _, _ in pipeline16.CASES:
+        ctas = gemm_schedule(n, k, batches, rem, sms, planes=1)
+        counts = {len(t) for t in ctas}
+        assert len(ctas) == sms and counts == {3, 4}, (n, k, batches, counts)
+        c = seen[pipeline.block_n(n)]
+        tiles = [t for cta in ctas for t in cta]
+        c["wrap"] += sum(w for _, w, _ in tiles)
+        c["no_wrap"] += sum(not w for _, w, _ in tiles)
+        c["staged_first_load"] += sum(s for cta in ctas for _, _, s in cta[:-1])
+        c[f"stages_{k // BLOCK_K}"] += 1
+    for bn, c in seen.items():
+        assert c["wrap"] and c["no_wrap"] and c["stages_1"] and c["stages_2"], (bn, c)
+    assert seen[256]["staged_first_load"]
+    _, ring, acc, _ = gemm_ring(128, EPI_SCRATCH, 1)
+    for last in range(ring):
+        first = last - acc + 1 if last >= acc - 1 else ring - acc
+        assert not first <= (last + 1) % ring < first + acc
+    assert {k for n, k, *_ in pipeline16.CASES if pipeline.block_n(n) == 256} == {64, 128, 192, 256, 320, 512}
+    assert {k for n, k, *_ in pipeline16.CASES if pipeline.block_n(n) == 128} == {64, 128, 192, 384}
 
 
 Conv = collections.namedtuple("Conv", "kind cin cout cin_blocks rem halos tap_major bn stages ring")
