@@ -6,9 +6,9 @@ one process on the same seeded weights (indoor_ds, thr 0) and images:
              as in tools/pair_list_bench.py.
 A 256 MiB buffer is written before every timed call (untimed; flushes the 50 MB L2); calls are timed with CUDA events
 and reported as min / median / max over --reps.  Then, in a pass of its own, every backbone launch of a 16-image
-forward of each mode under torch.profiler (median us over 5 forwards) with its algorithmic TFLOP/s (2 * pixels * Cout *
-Cin * k^2; in fp16 mode each product is one MMA, so issued = algorithmic), and the workspace bytes of each mode.  Prints
-a Markdown layer table and one JSON line with the GPU name and power limit (read-only nvidia-smi query).
+forward of each mode under the profiler (tools/conv_bench.py's launch_us: median us over 5 forwards) with its
+algorithmic TFLOP/s (2 * pixels * Cout * Cin * k^2; in fp16 mode each product is one MMA, so issued = algorithmic), and
+the workspace bytes of each mode.  Prints a Markdown layer table and one JSON line with the GPU name and power limit.
 
     python tools/backbone_fp16_bench.py [--reps 5] [--warmup 1]
 """
@@ -17,19 +17,17 @@ import ctypes as C
 import itertools
 import json
 import os
-import statistics
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import torch  # noqa: E402
 
 import loftr_b200  # noqa: E402
-from conv_bench import LAYERS  # noqa: E402
+from conv_bench import LAYERS, launch_us  # noqa: E402
 from loftr_b200 import _lib  # noqa: E402
-from pair_list_bench import gpu_info, stats  # noqa: E402
+from measure import gpu_label, require_gpu, stats, timed  # noqa: E402
 
 N_IMAGES, H, W, BATCH = 16, 480, 640, 8
 MODES = ("b200", "b200_fp16")
@@ -44,29 +42,12 @@ def layer_gflop(n, h, w):
     return out
 
 
-def launch_us(tc, img, reps=5):
-    """Median us of every backbone launch (stem first) over `reps` profiled forwards."""
-    per_rep = []
-    for _ in range(reps):
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            tc(img)
-            torch.cuda.synchronize()
-        ev = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
-                     and ("EpiConv" in e.name or "conv_stem" in e.name)), key=lambda e: e.time_range.start)
-        per_rep.append([e.time_range.elapsed_us() for e in ev])
-    if {len(r) for r in per_rep} != {len(LAYERS) + 1}:
-        sys.exit(f"expected {len(LAYERS) + 1} backbone launches per forward, got {sorted({len(r) for r in per_rep})}")
-    return [statistics.median(r[i] for r in per_rep) for i in range(len(LAYERS) + 1)]
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=1)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("backbone_fp16_bench: no CUDA device (this measurement needs an H100)")
-    dev = torch.device("cuda:0")
+    dev = require_gpu("backbone_fp16_bench")
     torch.manual_seed(0)
     cfg = loftr_b200.get_cfg("indoor_ds", thr=0.0)
     models = {"b200": loftr_b200.LoFTR(cfg, backbone_impl="b200").eval()}
@@ -79,16 +60,6 @@ def main():
     batches = [(pairs[s:s + BATCH, 0].contiguous(), pairs[s:s + BATCH, 1].contiguous())
                for s in range(0, len(pairs), BATCH)]
     step = {"image0": images[:BATCH], "image1": images[BATCH:]}
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-
-    def timed(fn):
-        flush.zero_()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        out = fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return out, e0.elapsed_time(e1)
 
     def one_rep(model):
         bank, t_ext = timed(lambda: model.extract_features(images))
@@ -117,16 +88,13 @@ def main():
     us, ws_bytes = {}, {}
     for mode in MODES:
         tc = models[mode]._tc_backbone
-        for _ in range(3):
-            tc(images)
-        torch.cuda.synchronize()
-        us[mode] = launch_us(tc, images)
+        us[mode], _ = launch_us(tc, images)
         w, _ = tc._pack()
         lib = _lib.load()
         fn = lib.lb_backbone_workspace_bytes_fp16 if mode == "b200_fp16" else lib.lb_backbone_workspace_bytes
         ws_bytes[mode] = int(fn(C.byref(w), N_IMAGES, H, W))
 
-    info = gpu_info()
+    info = gpu_label()
     print(f"# {info['gpu']} at {info['power_limit']}, {N_IMAGES} images {H}x{W}, median of 5 profiled forwards")
     print("| layer | GFLOP | split us | split TFLOP/s | fp16 us | fp16 TFLOP/s | speed-up |")
     print("|---|---|---|---|---|---|---|")

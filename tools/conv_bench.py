@@ -18,6 +18,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import loftr_b200  # noqa: E402
 from loftr_b200.loftr import TensorCoreBackbone  # noqa: E402
+from measure import gpu_label, require_gpu  # noqa: E402
 
 # (name, Cin, Cout, ksize, stride, input-grid divisor) in lb_backbone_forward's launch order after the stem
 LAYERS = [
@@ -51,6 +52,25 @@ def layer_counts(cin, cout, k, s, div, n, h, w, bn):
     return gflop, tap_bytes, halo
 
 
+def launch_us(tc, img, reps=5):
+    """Median us of every backbone launch of `tc(img)` (stem first) over `reps` profiled forwards after 3 warm-up
+    forwards, and the kernel names of those launches."""
+    for _ in range(3):
+        tc(img)
+    torch.cuda.synchronize()
+    per_rep = []
+    for _ in range(reps):
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            tc(img)
+            torch.cuda.synchronize()
+        ev = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
+                     and ("EpiConv" in e.name or "conv_stem" in e.name)), key=lambda e: e.time_range.start)
+        per_rep.append([e.time_range.elapsed_us() for e in ev])
+    if {len(r) for r in per_rep} != {len(LAYERS) + 1}:
+        sys.exit(f"expected {len(LAYERS) + 1} backbone launches per forward, got {sorted({len(r) for r in per_rep})}")
+    return [statistics.median(r[i] for r in per_rep) for i in range(len(LAYERS) + 1)], [e.name for e in ev]
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=8, help="image pairs (2x as many images)")
@@ -58,33 +78,20 @@ def main():
     ap.add_argument("--w", type=int, default=640)
     ap.add_argument("--reps", type=int, default=5)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("conv_bench.py needs a CUDA device")
+    require_gpu("conv_bench")
     torch.manual_seed(0)
     model = loftr_b200.LoFTR(loftr_b200.get_cfg("indoor_ds", thr=0.0)).eval().cuda()
     tc = TensorCoreBackbone(model.backbone)
     n = 2 * args.batch
     img = torch.rand(n, 1, args.h, args.w, generator=torch.Generator().manual_seed(1000)).cuda()
-    for _ in range(3):
-        tc(img)
-    torch.cuda.synchronize()
-    per_rep = []
-    for _ in range(args.reps):
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            tc(img)
-            torch.cuda.synchronize()
-        ev = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
-              and ("EpiConv" in e.name or "conv_stem" in e.name)]
-        ev.sort(key=lambda e: e.time_range.start)
-        per_rep.append([e.time_range.elapsed_us() for e in ev])
-        # output-channel tile of each EpiConv launch: the BLOCK_N template argument in the (de)mangled kernel name
-        tiles_n = [int(m.group(1)) for m in (re.search(r"EpiConv(?:<|ILi)(\d+)", e.name) for e in ev) if m]
-    counts = {len(r) for r in per_rep}
-    if counts != {len(LAYERS) + 1} or len(tiles_n) != len(LAYERS):
-        sys.exit(f"expected {len(LAYERS) + 1} backbone launches per forward ({len(LAYERS)} named EpiConv<N>), got "
-                 f"{sorted(counts)} ({len(tiles_n)})")
-    us = [statistics.median(r[i] for r in per_rep) for i in range(len(LAYERS) + 1)]
-    print(f"# {torch.cuda.get_device_name()}, {n} images {args.h}x{args.w}, median of {args.reps} profiled forwards")
+    us, names = launch_us(tc, img, args.reps)
+    # output-channel tile of each EpiConv launch: the BLOCK_N template argument in the (de)mangled kernel name
+    tiles_n = [int(m.group(1)) for m in (re.search(r"EpiConv(?:<|ILi)(\d+)", name) for name in names) if m]
+    if len(tiles_n) != len(LAYERS):
+        sys.exit(f"expected {len(LAYERS)} launches named EpiConv<N> per forward, got {len(tiles_n)}")
+    info = gpu_label()
+    print(f"# {info['gpu']} at {info['power_limit']}, {n} images {args.h}x{args.w}, median of {args.reps} profiled "
+          "forwards")
     print("| layer | N tile | us | issued GFLOP | issued TFLOP/s | L2->smem MB (tap) | L2->smem MB (halo) |")
     print("|---|---|---|---|---|---|---|")
     print(f"| stem 7x7 s2 | - | {us[0]:.0f} | - | - | - | - |")

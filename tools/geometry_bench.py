@@ -8,14 +8,13 @@ a fixed seed with 30 % outliers, the default budget of 2048 hypotheses and a 3 p
   opencv        host clock around cv2.findHomography / cv2.findFundamentalMat (RANSAC, 3 px, 2048 iterations) over
                 the B pairs one after the other, on host arrays; absent when cv2 cannot be imported.
 Reported: ms (min / median / max over --steps), the estimator's share of the matcher's median, the GPU name and power
-limit (read-only nvidia-smi query).  Prints one JSON line per workload; fails without a CUDA device.
+limit.  Prints one JSON line per workload; fails without a CUDA device.
 
     python tools/geometry_bench.py [--steps 20] [--warmup 3]
 """
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -27,26 +26,12 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 import loftr_b200  # noqa: E402
+from measure import alternate, gpu_label, require_gpu, stats  # noqa: E402
 
 BATCHES = (1, 8, 32)
 KS = (512, 2048)
 MODELS = ("homography", "fundamental")
 ITERATIONS, THRESHOLD = 2048, 3.0
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], check=True,
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = [s.strip() for s in out.split(",")]
-        return {"gpu": name, "power_limit": power}
-    except Exception as e:
-        return {"gpu": torch.cuda.get_device_name(0), "power_limit": f"unavailable ({type(e).__name__})"}
-
-
-def stats(v, nd=3):
-    v = sorted(v)
-    return {"min": round(v[0], nd), "median": round(v[len(v) // 2], nd), "max": round(v[-1], nd)}
 
 
 def scenes(rs, model, B, K, outliers=0.3):
@@ -71,21 +56,6 @@ def scenes(rs, model, B, K, outliers=0.3):
     return p0.astype(np.float32), p1.astype(np.float32)
 
 
-def time_cuda(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    ms = []
-    for _ in range(steps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        e1.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    return ms
-
-
 def matcher():
     import weights as W
     torch.backends.cudnn.allow_tf32 = False
@@ -105,13 +75,12 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("geometry_bench: no CUDA device (the numbers are GPU timings; there is no CPU fallback)")
+    require_gpu("geometry_bench")
     try:
         import cv2
     except ImportError:
         cv2 = None
-    info = gpu_info()
+    info = gpu_label()
     model, bank = matcher()
     rs = np.random.RandomState(0)
     for B in BATCHES:
@@ -121,12 +90,14 @@ def main():
             model.coarse_matching.max_matches_per_pair = K
             out = model.match_features(bank, i0, bank, i1)
             per_pair = torch.bincount(out["m_bids"], minlength=B).float().mean().item()
-            t_match = time_cuda(lambda: model.match_features(bank, i0, bank, i1), args.steps, args.warmup)
+            t_match = alternate({"matcher": lambda: model.match_features(bank, i0, bank, i1)}, args.steps, args.warmup,
+                                flush=False)[0]["matcher"]
             for name in MODELS:
                 a0, a1 = scenes(rs, name, B, K)
                 p0, p1 = torch.from_numpy(a0).cuda(), torch.from_numpy(a1).cuda()
-                t_est = time_cuda(lambda: loftr_b200.estimate_geometry(p0, p1, model=name, threshold=THRESHOLD,
-                                                                      iterations=ITERATIONS), args.steps, args.warmup)
+                t_est = alternate({"estimator": lambda: loftr_b200.estimate_geometry(
+                    p0, p1, model=name, threshold=THRESHOLD, iterations=ITERATIONS)}, args.steps, args.warmup,
+                    flush=False)[0]["estimator"]
                 row = {"workload": f"B{B}_K{K}_{name}", "B": B, "K": K, "model": name, "iterations": ITERATIONS,
                        "estimator_ms": stats(t_est), "matcher_ms": stats(t_match),
                        "matcher_matches_per_pair": round(per_pair, 1),

@@ -2,14 +2,13 @@
 process.  Per workload: GPU ms per step (CUDA events), host wall ms per step (ending in a device synchronise), library
 kernel launches per step (enqueued by the host; a graph replay enqueues none) and whether both produced bit-identical
 outputs.  indoor_ds at thr 0 with seeded weights and uniform-random images, as in bench.py.  Prints one JSON line with
-the GPU name and power limit (read-only nvidia-smi query).
+the GPU name and power limit.
 
     python tools/graph_bench.py [--steps 20] [--warmup 3]
 """
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -20,19 +19,10 @@ import torch  # noqa: E402
 
 import loftr_b200  # noqa: E402
 from loftr_b200 import _lib  # noqa: E402
+from measure import gpu_label, require_gpu, stats, timed  # noqa: E402
 
 WORKLOADS = [(1, 240, 320), (1, 480, 640), (1, 960, 1280), (8, 480, 640)]   # (batch, H, W)
 KEYS = ["b_ids", "i_ids", "j_ids", "mconf", "mkpts0_c", "mkpts1_c", "mkpts0_f", "mkpts1_f", "expec_f", "gt_mask"]
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], check=True,
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = [s.strip() for s in out.split(",")]
-        return {"gpu": name, "power_limit": power}
-    except Exception as e:   # the numbers stay valid; say where the label is missing
-        return {"gpu": torch.cuda.get_device_name(0), "power_limit": f"unavailable ({type(e).__name__})"}
 
 
 def run(batch, h, w, steps, warmup, dev):
@@ -54,33 +44,29 @@ def run(batch, h, w, steps, warmup, dev):
         cm(d)
         return d
 
-    stats = {}
+    runs = {}
     for name, fn in (("eager", eager), ("graph", captured)):
         for _ in range(warmup):
             fn()
-        stats[name] = {"gpu_ms": [], "wall_ms": [], "launches": []}
+        runs[name] = {"gpu_ms": [], "wall_ms": [], "launches": []}
     torch.cuda.synchronize()
     last = {}
     for _ in range(steps):
-        for name, fn in (("eager", eager), ("graph", captured)):   # alternate: both see the same clocks
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        # alternate by hand: the wall clock and the launch count of each step are measured around the event pair
+        for name, fn in (("eager", eager), ("graph", captured)):
             n0 = lib.lb_launch_count()
             t0 = time.perf_counter()
-            e0.record()
-            last[name] = fn()
-            e1.record()
-            torch.cuda.synchronize()
+            last[name], gpu_ms = timed(fn, flush=False)
             t1 = time.perf_counter()
-            stats[name]["gpu_ms"].append(e0.elapsed_time(e1))
-            stats[name]["wall_ms"].append((t1 - t0) * 1e3)
-            stats[name]["launches"].append(lib.lb_launch_count() - n0)
+            runs[name]["gpu_ms"].append(gpu_ms)
+            runs[name]["wall_ms"].append((t1 - t0) * 1e3)
+            runs[name]["launches"].append(lib.lb_launch_count() - n0)
     equal = all(torch.equal(last["eager"][k], last["graph"][k]) for k in KEYS)
-    med = lambda v: sorted(v)[len(v) // 2]
     res = {"batch": batch, "hw": [h, w], "matches": int(last["eager"]["b_ids"].shape[0]),
            "capacity": cm.capacity, "outputs_equal": equal}
-    for name, s in stats.items():
-        res[name] = {"gpu_ms_median": round(med(s["gpu_ms"]), 3), "wall_ms_median": round(med(s["wall_ms"]), 3),
-                     "lib_launches_per_step": med(s["launches"])}
+    for name, s in runs.items():
+        res[name] = {"gpu_ms_median": stats(s["gpu_ms"])["median"], "wall_ms_median": stats(s["wall_ms"])["median"],
+                     "lib_launches_per_step": stats(s["launches"])["median"]}
     res["wall_speedup"] = round(res["eager"]["wall_ms_median"] / res["graph"]["wall_ms_median"], 3)
     del cm, model
     torch.cuda.empty_cache()
@@ -92,10 +78,8 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("graph_bench: no CUDA device (this measurement needs an H100)")
-    dev = torch.device("cuda:0")
-    out = {"tool": "graph_bench", "steps": args.steps, **gpu_info(),
+    dev = require_gpu("graph_bench")
+    out = {"tool": "graph_bench", "steps": args.steps, **gpu_label(),
            "workloads": [run(b, h, w, args.steps, args.warmup, dev) for b, h, w in WORKLOADS]}
     print(json.dumps(out))
 

@@ -10,14 +10,13 @@ and k:
   matches_per_pair    before (k = none) and after the cap (min / mean / max over the pairs);
   captured_capacity   the default capacity of `CapturedMatcher`, and the peak device memory
                       (torch.cuda.max_memory_allocated) of its construction and one replay, and of one eager step.
-Prints one JSON line with the GPU name and power limit (read-only nvidia-smi query).
+Prints one JSON line with the GPU name and power limit.
 
     python tools/match_cap_bench.py [--steps 10] [--warmup 2]
 """
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -26,7 +25,7 @@ sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
 import loftr_b200  # noqa: E402
-from loftr_b200 import _lib  # noqa: E402
+from measure import alternate, gpu_label, require_gpu, stats, tag_ms  # noqa: E402
 
 CAPS = [None, 256, 1024]
 # (name, config, batch, H, W, valid (h, w) of image0 / image1 per pair or None)
@@ -36,21 +35,6 @@ WORKLOADS = [
     ("4x832x832_masked", "outdoor_ds", 4, 832, 832,
      ([(832, 624), (832, 832), (560, 832), (704, 768)], [(640, 832), (768, 832), (832, 832), (832, 616)])),
 ]
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], check=True,
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = [s.strip() for s in out.split(",")]
-        return {"gpu": name, "power_limit": power}
-    except Exception as e:   # the numbers stay valid; say where the label is missing
-        return {"gpu": torch.cuda.get_device_name(0), "power_limit": f"unavailable ({type(e).__name__})"}
-
-
-def stats(v, nd=3):
-    v = sorted(v)
-    return {"min": round(v[0], nd), "median": round(v[len(v) // 2], nd), "max": round(v[-1], nd)}
 
 
 def inputs(batch, h, w, valid, dev):
@@ -71,7 +55,6 @@ def run(name, cfg_name, batch, h, w, valid, steps, warmup, dev):
     torch.manual_seed(0)
     model = loftr_b200.LoFTR(loftr_b200.get_cfg(cfg_name, thr=0.0)).eval().to(dev)
     inp = inputs(batch, h, w, valid, dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     cmatch = model.coarse_matching
 
     def step(k):
@@ -80,30 +63,11 @@ def run(name, cfg_name, batch, h, w, valid, steps, warmup, dev):
         model(d)
         return d
 
-    for _ in range(warmup):
-        for k in CAPS:
-            step(k)
-    step_ms = {k: [] for k in CAPS}
-    last = {}
-    for _ in range(steps):
-        for k in CAPS:   # alternate: every k sees the same clocks and neighbours
-            flush.zero_()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            last[k] = step(k)
-            e1.record()
-            torch.cuda.synchronize()
-            step_ms[k].append(e0.elapsed_time(e1))
+    step_ms, last = alternate({k: (lambda k=k: step(k)) for k in CAPS}, steps, warmup)
 
     kernel = {}
-    for k in CAPS:   # kernel timing in a pass of its own (events around the tagged launches slow the host)
-        _lib.timing_enable(True)
-        for _ in range(3):
-            flush.zero_()
-            step(k)
-        torch.cuda.synchronize()
-        tags = _lib.timing_collect()
-        _lib.timing_enable(False)
+    for k in CAPS:
+        tags = tag_ms(lambda: step(k), runs=3, flush=True)
         cap_ms, cap_n = tags.get("match_cap", (0.0, 0))
         score_ms = tags.get("score_lse", (0.0, 0))[0] + tags.get("score_argmax", (0.0, 0))[0]
         kernel[k] = {"match_cap_ms_per_step": round(cap_ms / 3, 4), "match_cap_launches_per_step": cap_n / 3,
@@ -139,7 +103,7 @@ def run(name, cfg_name, batch, h, w, valid, steps, warmup, dev):
         res["caps"]["none" if k is None else str(k)] = {"step_ms": stats(step_ms[k]),
                                                          "matches_per_pair": per_pair(last[k]), **kernel[k],
                                                          **memory[k]}
-    del model, last, flush
+    del model, last
     torch.cuda.empty_cache()
     return res
 
@@ -149,10 +113,8 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=2)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("match_cap_bench: no CUDA device (this measurement needs an H100)")
-    dev = torch.device("cuda:0")
-    out = {"tool": "match_cap_bench", "steps": args.steps, **gpu_info(),
+    dev = require_gpu("match_cap_bench")
+    out = {"tool": "match_cap_bench", "steps": args.steps, **gpu_label(),
            "l2": "256 MiB buffer written before every timed step",
            "workloads": [run(*w, args.steps, args.warmup, dev) for w in WORKLOADS]}
     print(json.dumps(out))

@@ -8,7 +8,7 @@ one process on the same seeded weights and images.  Workloads (`matcher(batch)` 
 A 256 MiB buffer is written before every timed call (untimed; flushes the 50 MB L2); steps are timed with CUDA events
 after --warmup untimed rounds and reported as min / median / max over --reps.  Then, in a pass of its own, the
 per-tag kernel ms of one step of each workload and mode (lb_timing_*, CUDA events around every tagged launch).  Prints
-one JSON line with the GPU name and power limit (read-only nvidia-smi query).
+one JSON line with the GPU name and power limit.
 
     python tools/match_fp16_bench.py [--reps 7] [--warmup 2]
 """
@@ -19,13 +19,11 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import torch  # noqa: E402
 
 import loftr_b200  # noqa: E402
-from loftr_b200 import _lib  # noqa: E402
-from pair_list_bench import gpu_info, stats  # noqa: E402
+from measure import alternate, gpu_label, require_gpu, stats, tag_ms  # noqa: E402
 
 TAGS = ("proj_act", "tf_kv_proj_fused", "tf_q_attn_fused", "merge_ln", "mlp1_relu", "mlp2_ln_res", "tf_full_attn",
         "score_lse", "score_argmax")
@@ -49,11 +47,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--only", default="", help="comma-separated workload names (default: all)")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("match_fp16_bench: no CUDA device (this measurement needs an H100)")
-    dev = torch.device("cuda:0")
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-    out = {"tool": "match_fp16_bench", **gpu_info(), "reps": args.reps, "warmup": args.warmup,
+    dev = require_gpu("match_fp16_bench")
+    out = {"tool": "match_fp16_bench", **gpu_label(), "reps": args.reps, "warmup": args.warmup,
            "l2": "256 MiB buffer written before every timed call"}
     for name, (cfg, n, (h, w), modes) in workloads().items():
         if args.only and name not in args.only.split(","):
@@ -71,29 +66,15 @@ def main():
 
         def run(model):
             d = dict(step)
-            flush.zero_()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
             model(d)
-            e1.record()
-            torch.cuda.synchronize()
-            return e0.elapsed_time(e1), int(d["b_ids"].shape[0])
+            return d
 
-        for _ in range(args.warmup):
-            for m in models.values():
-                run(m)
-        times = {k: [] for k in models}
-        matches = {}
-        for _ in range(args.reps):   # alternate: every mode sees the same clocks and neighbours
-            for k, m in models.items():
-                t, matches[k] = run(m)
-                times[k].append(t)
+        arms = {k: (lambda m=m: run(m)) for k, m in models.items()}
+        times, last = alternate(arms, args.reps, args.warmup)
+        matches = {k: int(d["b_ids"].shape[0]) for k, d in last.items()}
         tags = {}
-        for k, m in models.items():
-            _lib.timing_enable(True)
-            run(m)
-            rec = _lib.timing_collect()
-            _lib.timing_enable(False)
+        for k, fn in arms.items():
+            rec = tag_ms(fn, flush=True)
             tags[k] = {t: round(rec[t][0], 3) for t in TAGS if rec.get(t, (0, 0))[1]}
         out[name] = {"batch": n, "hw": [h, w], "match_type": cfg["match_coarse"]["match_type"],
                      "attention": cfg["coarse"]["attention"], "step_ms": {k: stats(v) for k, v in times.items()},

@@ -9,7 +9,7 @@ A 256 MiB buffer is written before every step (untimed; flushes the 50 MB L2) an
 Reported: ms per step (min / median / max over steps), ms and pairs/s per list (min / median / max over repetitions),
 the share of the plain step spent in the backbone's convolutions (`backbone_conv` kernel timing tag, from a separate
 profiled pass; the 7x7 stem is not tagged), and whether both produced bit-identical outputs for every batch.  Prints
-one JSON line with the GPU name and power limit (read-only nvidia-smi query).
+one JSON line with the GPU name and power limit.
 
     python tools/pair_list_bench.py [--reps 5] [--warmup 1]
 """
@@ -17,7 +17,6 @@ import argparse
 import itertools
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -26,26 +25,11 @@ sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
 import loftr_b200  # noqa: E402
-from loftr_b200 import _lib  # noqa: E402
+from measure import gpu_label, require_gpu, stats, tag_ms, timed  # noqa: E402
 
 N_IMAGES, H, W, BATCH = 16, 480, 640, 8
 KEYS = ["b_ids", "i_ids", "j_ids", "gt_mask", "m_bids", "mconf", "mkpts0_c", "mkpts1_c", "mkpts0_f", "mkpts1_f",
         "expec_f"]
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], check=True,
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = [s.strip() for s in out.split(",")]
-        return {"gpu": name, "power_limit": power}
-    except Exception as e:   # the numbers stay valid; say where the label is missing
-        return {"gpu": torch.cuda.get_device_name(0), "power_limit": f"unavailable ({type(e).__name__})"}
-
-
-def stats(v):
-    v = sorted(v)
-    return {"min": round(v[0], 3), "median": round(v[len(v) // 2], 3), "max": round(v[-1], 3)}
 
 
 def main():
@@ -53,9 +37,7 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=1)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("pair_list_bench: no CUDA device (this measurement needs an H100)")
-    dev = torch.device("cuda:0")
+    dev = require_gpu("pair_list_bench")
     torch.manual_seed(0)
     model = loftr_b200.LoFTR(loftr_b200.get_cfg("indoor_ds", thr=0.0)).eval().to(dev)
     g = torch.Generator().manual_seed(1000)
@@ -63,16 +45,6 @@ def main():
     pairs = torch.tensor(list(itertools.combinations(range(N_IMAGES), 2)), device=dev)
     batches = [(pairs[s:s + BATCH, 0].contiguous(), pairs[s:s + BATCH, 1].contiguous())
                for s in range(0, len(pairs), BATCH)]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-
-    def timed(fn):
-        flush.zero_()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        out = fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return out, e0.elapsed_time(e1)
 
     def plain_step(i0, i1):
         d = {"image0": images[i0], "image1": images[i1]}
@@ -116,14 +88,12 @@ def main():
         del p_out, b_out
 
     # backbone share of the plain step: per-launch events around the tagged kernels, in a pass of its own
-    _lib.timing_enable(True)
-    _, prof_ms = run_plain()
-    tags = _lib.timing_collect()
-    _lib.timing_enable(False)
+    prof_ms = []
+    tags = tag_ms(lambda: prof_ms.extend(run_plain()[1]))
     conv_ms = tags.get("backbone_conv", (0.0, 0))[0]
 
     n_pairs = len(pairs)
-    res = {"tool": "pair_list_bench", **gpu_info(), "images": N_IMAGES, "hw": [H, W], "pairs": n_pairs,
+    res = {"tool": "pair_list_bench", **gpu_label(), "images": N_IMAGES, "hw": [H, W], "pairs": n_pairs,
            "batch": BATCH, "reps": args.reps, "matches_per_list": matches, "outputs_identical": bool(identical),
            "plain_ms_per_step": stats(plain_ms), "bank_match_ms_per_step": stats(bank_ms),
            "bank_extract_ms": stats(extract_ms),

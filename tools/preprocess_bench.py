@@ -8,14 +8,13 @@ square-padded (MegaDepth style), uniform-random pixels from a fixed seed.  Arms,
 Reported: ms per batch (host clock around a device synchronise; min / median / max), the kernel's own time from the
 `preprocess` timing tag in a pass of its own (a 256 MiB buffer written before every launch), the bytes the kernel
 reads and writes computed from the shapes (`kernel_bytes`), the resulting GB/s next to the 3.35 TB/s HBM3 data-sheet figure (the kernel is HBM-bound; the share is of a figure for a 700 W card), and
-the GPU name and power limit (read-only nvidia-smi query).  Prints one JSON line; fails without a CUDA device.
+the GPU name and power limit.  Prints one JSON line; fails without a CUDA device.
 
     python tools/preprocess_bench.py [--steps 20] [--warmup 3]
 """
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -26,7 +25,7 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 import loftr_b200  # noqa: E402
-from loftr_b200 import _lib  # noqa: E402
+from measure import gpu_label, require_gpu, stats, tag_ms  # noqa: E402
 
 HBM_DATASHEET_GBPS = 3350.0
 # (name, frames, (h, w), resize, pad_to)
@@ -34,21 +33,6 @@ WORKLOADS = [
     ("16x968x1296_to_480x640", 16, (968, 1296), (640, 480), None),
     ("8x1200x1600_to_832_square", 8, (1200, 1600), 832, "square"),
 ]
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], check=True,
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = [s.strip() for s in out.split(",")]
-        return {"gpu": name, "power_limit": power}
-    except Exception as e:   # the numbers stay valid; say where the label is missing
-        return {"gpu": torch.cuda.get_device_name(0), "power_limit": f"unavailable ({type(e).__name__})"}
-
-
-def stats(v, nd=3):
-    v = sorted(v)
-    return {"min": round(v[0], nd), "median": round(v[len(v) // 2], nd), "max": round(v[-1], nd)}
 
 
 def kernel_bytes(n, h, w, h_new, w_new, H, W, masked):
@@ -106,14 +90,9 @@ def run(name, n, hw, resize, pad_to, steps, warmup, dev):
             ms[k].append((time.perf_counter() - t0) * 1e3)
 
     dev_frames = pinned_u8.to(dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-    _lib.timing_enable(True)
-    for _ in range(steps):
-        flush.zero_()   # the frames would otherwise stay in the 50 MB L2 from one launch to the next
-        loftr_b200.prepare_images(dev_frames, resize=resize, pad_to=pad_to)
-    torch.cuda.synchronize()
-    k_ms, k_n = _lib.timing_collect()["preprocess"]
-    _lib.timing_enable(False)
+    # flushed: the frames would otherwise stay in the 50 MB L2 from one launch to the next
+    k_ms, k_n = tag_ms(lambda: loftr_b200.prepare_images(dev_frames, resize=resize, pad_to=pad_to), runs=steps,
+                       flush=True)["preprocess"]
     kernel_ms = k_ms / k_n
     nbytes = kernel_bytes(n, h, w, h_new, w_new, H, W, pad_to is not None)
     gbps = nbytes / (kernel_ms * 1e-3) / 1e9
@@ -133,10 +112,8 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("preprocess_bench: no CUDA device (this measurement needs an H100)")
-    dev = torch.device("cuda:0")
-    out = {"tool": "preprocess_bench", "steps": args.steps, **gpu_info(), "bound": "HBM",
+    dev = require_gpu("preprocess_bench")
+    out = {"tool": "preprocess_bench", "steps": args.steps, **gpu_label(), "bound": "HBM",
            "hbm_datasheet_gbps": HBM_DATASHEET_GBPS,
            "workloads": [run(*w, args.steps, args.warmup, dev) for w in WORKLOADS]}
     print(json.dumps(out))
