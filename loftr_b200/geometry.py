@@ -49,9 +49,11 @@ def estimate_geometry(points0, points1, valid=None, model="homography", threshol
     first count[b] entries of row b are matches).  K must be at least the minimal sample (4 for H, 8 for F).
     threshold: inlier threshold in pixels, on the symmetric transfer error for H (the root of the mean of the squared
     forward and backward transfer distances) and on the Sampson distance for F.  iterations: hypotheses per pair (a
-    fixed budget: there is no adaptive early stop).  seed and pair_ids (int [B], default 0..B-1) key the random
-    samples: a pair's result depends only on its own valid matches, its id, the seed and the budget, never on its
-    neighbours in the batch or on where its padding lies.
+    fixed budget: there is no adaptive early stop).  seed and pair_ids (int32 / int64 [B], default 0..B-1) key the
+    random samples: a pair's result depends only on its own valid matches, its id, the seed and the budget, never on
+    its neighbours in the batch or on where its padding lies.  The samples are keyed by the id modulo 2**32 (the
+    counter word is 32 bits wide), so ids that differ by a multiple of 2**32, such as -1 and 2**32 - 1, draw the same
+    samples.
 
     -> (model [B, 3, 3] float32, inlier_mask [B, K] bool, num_inliers [B] int32).  H is scaled to H[2, 2] = 1, F to
     unit Frobenius norm with its largest-magnitude entry positive.  A pair with fewer valid matches than the minimal

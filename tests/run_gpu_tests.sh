@@ -1,10 +1,10 @@
 #!/bin/bash
-# Run the GPU parity tests function by function in separate processes (a device-side trap poisons the CUDA
+# Run every gpu-marked test function by function in separate processes (a device-side trap poisons the CUDA
 # context of its process), keeping the log under gpurun_out/.  Optional argument: an egrep filter on test names.
 mkdir -p gpurun_out
 cd "$(dirname "$0")/.."
 filter="${1:-.}"
-mapfile -t groups < <(python -m pytest tests/test_*gpu*.py --collect-only -q -m gpu -p no:cacheprovider 2>/dev/null \
+mapfile -t groups < <(python -m pytest tests/test_*.py --collect-only -q -m gpu -p no:cacheprovider 2>/dev/null \
   | grep "::" | sed 's/\[.*//' | sort -u | grep -E "$filter")
 rc=0
 : > gpurun_out/gpu_tests.log

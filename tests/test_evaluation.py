@@ -143,3 +143,24 @@ def test_evaluation_pipeline_on_matcher_output():
                "epi_errs": [data["epi_errs"].cpu().numpy()[bids == b] for b in range(2)]}
     agg = E.aggregate_metrics(metrics)
     assert set(agg) == {"auc@5", "auc@10", "auc@20", "prec@5e-04"} and all(0.0 <= v <= 1.0 for v in agg.values())
+
+
+# ------------------------------------------------------------------------------------------------ epipolar rule
+def test_fp32_oracle_meets_the_epipolar_rule():
+    """The per-match rule of tests/epipolar_ref.py puts a plain fp32 evaluation within a few 2^-24 of float64 on every
+    scene of tests/test_evaluation_edges_gpu.py, and rejects normalising x by fy and y by fx by orders of magnitude."""
+    import epipolar_ref as R
+    scenes = [make_scene_batch(s, 3) for s in (0, 1, 7)] + [R.outdoor_scene(3), R.forward_scene(4),
+                                                             R.rotation_scene(5), R.sized_scene(6, 257)]
+    for i, sc in enumerate(scenes):
+        r, scale = R.terms(sc)
+        with np.errstate(all="ignore"):
+            o = R.oracle32(sc)
+        assert np.isnan(o[np.isnan(r)]).all() and np.isfinite(o[~np.isnan(r)]).all(), i
+        assert np.nanmax(R.rule_error(o, r, scale)) <= 4 * R.ULP, i
+        swapped = {k: v.copy() for k, v in sc.items()}
+        for k in ("K0", "K1"):
+            swapped[k][:, 0, 0], swapped[k][:, 1, 1] = sc[k][:, 1, 1], sc[k][:, 0, 0]
+        if i != 5:      # the pure-rotation scene has a single translating pair with fx == fy
+            with np.errstate(all="ignore"):
+                assert np.nanmax(R.rule_error(R.oracle32(swapped), r, scale)) > 1e3 * R.ULP, i

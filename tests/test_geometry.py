@@ -1,289 +1,20 @@
 """Robust two-view geometry (`loftr_b200.estimate_geometry`, `match_features(..., estimate=...)`).
 
-The file carries a float64 NumPy implementation of the same estimator: the same Philox4x32-10 sample draw, the same
-minimal solvers (4-point normalised DLT with h33 = 1; normalised 8-point with rank 2), the same errors (symmetric
-transfer, Sampson), the same MSAC ranking and the same Hartley-normalised least-squares refit.  The GPU runs the
-geometry in fp64 too, so on identical samples the winning hypothesis must agree exactly and the refitted model to
-rounding.  Synthetic scenes with known H / F check accuracy; the CPU tests check the reference and the host-side
-validation and run without a GPU."""
+tests/geometry_ref.py carries a float64 NumPy implementation of the same estimator (sample draw, minimal solvers,
+errors, MSAC ranking, refit).  The GPU runs the geometry in fp64 too, so on identical samples the winning hypothesis
+must agree exactly and the refitted model to rounding.  Synthetic scenes with known H / F check accuracy; the CPU tests
+check the reference, its mirror of the library's workspace and the host-side validation, and run without a GPU.
+tests/test_geometry_edges_gpu.py checks the kernels' intermediate results at their launch boundaries."""
 import numpy as np
 import pytest
 import torch
 
 import loftr_b200
+from geometry_ref import (S, STAGE, STAGING_THR, draw_samples, errors, model_dist, pad_batch, philox4x32_10, project_h,
+                          ransac_ref, scene, solve_f8, solve_h4, staging_case, tile_ranking, ws_layout)
 from loftr_b200 import geometry
 
 DEV = "cuda:0"
-S = {"homography": 4, "fundamental": 8}
-
-
-# ---------------------------------------------------------------------------------------------- NumPy reference
-def philox4x32_10(ctr, key):
-    """ctr [..., 4] uint32, key (k0, k1) -> [..., 4] uint32 (Random123's Philox4x32-10)."""
-    c = [ctr[..., i].astype(np.uint64) for i in range(4)]
-    k0, k1 = np.uint64(key[0]), np.uint64(key[1])
-    m32 = np.uint64(0xFFFFFFFF)
-    for _ in range(10):
-        p0 = np.uint64(0xD2511F53) * c[0]
-        p1 = np.uint64(0xCD9E8D57) * c[2]
-        c = [(p1 >> np.uint64(32)) ^ c[1] ^ k0, p1 & m32, (p0 >> np.uint64(32)) ^ c[3] ^ k1, p0 & m32]
-        k0 = (k0 + np.uint64(0x9E3779B9)) & m32
-        k1 = (k1 + np.uint64(0xBB67AE85)) & m32
-    return np.stack(c, -1).astype(np.uint32)
-
-
-def draw_samples(seed, pair_id, n, s, iterations):
-    """[iterations, s] ascending indices in [0, n): the kernel's draw (header of lb_estimate_geometry)."""
-    hyp = np.arange(iterations, dtype=np.uint64)
-    words = []
-    for blk in range(2):
-        ctr = np.stack([hyp, np.full_like(hyp, pair_id), np.full_like(hyp, blk), np.zeros_like(hyp)], -1)
-        words.append(philox4x32_10(ctr, (seed & 0xFFFFFFFF, seed >> 32)))
-    w = np.concatenate(words, -1).astype(np.uint64)
-    out = np.empty((iterations, s), np.int64)
-    for h in range(iterations):
-        chosen = []
-        for j in range(s):
-            r = int((int(w[h, j]) * (n - j)) >> 32)
-            for c in chosen:            # ascending
-                if r >= c:
-                    r += 1
-            chosen.append(r)
-            chosen.sort()
-        out[h] = chosen
-    return out
-
-
-def norm_t(p):
-    """Hartley normalisation [.., n, 2] -> (s, -s cx, -s cy) or None when the points coincide."""
-    n = p.shape[-2]
-    sx, sy = p[..., 0].sum(-1), p[..., 1].sum(-1)
-    sq = (p ** 2).sum((-1, -2))
-    cx, cy = sx / n, sy / n
-    d2 = sq / n - (cx * cx + cy * cy)
-    ok = d2 > 1e-24 * (sq / n) + 1e-300
-    s = np.sqrt(2.0 / np.where(ok, d2, 1.0))
-    return np.stack([s, -s * cx, -s * cy], -1), ok
-
-
-def denormalise(model, mn, t0, t1):
-    T0 = np.zeros(t0.shape[:-1] + (3, 3))
-    T0[..., 0, 0] = T0[..., 1, 1] = t0[..., 0]
-    T0[..., 0, 2], T0[..., 1, 2], T0[..., 2, 2] = t0[..., 1], t0[..., 2], 1
-    T1 = np.zeros_like(T0)
-    T1[..., 0, 0] = T1[..., 1, 1] = t1[..., 0]
-    T1[..., 0, 2], T1[..., 1, 2], T1[..., 2, 2] = t1[..., 1], t1[..., 2], 1
-    if model == "homography":
-        return np.linalg.inv(T1) @ mn @ T0
-    return np.swapaxes(T1, -1, -2) @ mn @ T0
-
-
-def rank2(f):
-    _, v = np.linalg.eigh(np.swapaxes(f, -1, -2) @ f)
-    v0 = v[..., :, 0:1]
-    return f - (f @ v0) @ np.swapaxes(v0, -1, -2)
-
-
-def apply(t, p):
-    return p * t[..., None, 0:1] + t[..., None, 1:3]
-
-
-def solve_h4(p0, p1):
-    """[..., 4, 2] -> (H [..., 3, 3], ok)."""
-    t0, ok0 = norm_t(p0)
-    t1, ok1 = norm_t(p1)
-    u, u2 = apply(t0, p0), apply(t1, p1)
-    ok = ok0 & ok1
-    for q in (u, u2):
-        for a, b, c in ((0, 1, 2), (0, 1, 3), (0, 2, 3), (1, 2, 3)):
-            d1, d2 = q[..., b, :] - q[..., a, :], q[..., c, :] - q[..., a, :]
-            ok &= np.abs(d1[..., 0] * d2[..., 1] - d1[..., 1] * d2[..., 0]) >= 1e-5
-    A = np.zeros(p0.shape[:-2] + (8, 9))
-    x, y, x2, y2 = u[..., 0], u[..., 1], u2[..., 0], u2[..., 1]
-    A[..., 0::2, 0], A[..., 0::2, 1], A[..., 0::2, 2] = x, y, 1
-    A[..., 0::2, 6], A[..., 0::2, 7], A[..., 0::2, 8] = -x * x2, -y * x2, x2
-    A[..., 1::2, 3], A[..., 1::2, 4], A[..., 1::2, 5] = x, y, 1
-    A[..., 1::2, 6], A[..., 1::2, 7], A[..., 1::2, 8] = -x * y2, -y * y2, y2
-    idx = np.arange(A.shape[0])
-    for c in range(8):                         # Gaussian elimination, partial pivoting (first maximum)
-        piv = c + np.argmax(np.abs(A[:, c:, c]), axis=1)
-        ok &= np.abs(A[idx, piv, c]) >= 1e-10
-        rc, rp = A[idx, c].copy(), A[idx, piv].copy()
-        A[idx, c], A[idx, piv] = rp, rc
-        pc = np.where(ok, A[:, c, c], 1.0)
-        f = A[:, c + 1:, c] / pc[:, None]
-        A[:, c + 1:, :] -= f[..., None] * A[:, c:c + 1, :]
-    hn = np.ones(A.shape[:1] + (9,))
-    for c in range(7, -1, -1):
-        s = A[:, c, 8] - (A[:, c, c + 1:8] * hn[:, c + 1:8]).sum(-1)
-        hn[:, c] = s / np.where(ok, A[:, c, c], 1.0)
-    with np.errstate(all="ignore"):
-        h = denormalise("homography", hn.reshape(-1, 3, 3), t0, t1)
-        inv_ok = np.isfinite(h).all((-1, -2)) & (np.linalg.det(np.where(np.isfinite(h), h, 0)) != 0)
-    return h, ok & inv_ok
-
-
-def f_rows(u, u2):
-    x, y, x2, y2 = u[..., 0], u[..., 1], u2[..., 0], u2[..., 1]
-    return np.stack([x2 * x, x2 * y, x2, y2 * x, y2 * y, y2, x, y, np.ones_like(x)], -1)
-
-
-def h_rows(u, u2):
-    x, y, x2, y2 = u[..., 0], u[..., 1], u2[..., 0], u2[..., 1]
-    z, o = np.zeros_like(x), np.ones_like(x)
-    a = np.stack([-x, -y, -o, z, z, z, x2 * x, x2 * y, x2], -1)
-    b = np.stack([z, z, z, -x, -y, -o, y2 * x, y2 * y, y2], -1)
-    return np.concatenate([a, b], -2)
-
-
-def solve_system(model, m, t0, t1, need_rank):
-    w, v = np.linalg.eigh(m)
-    ok = w[..., 1] > 1e-12 * w[..., -1] if need_rank else np.ones(w.shape[:-1], bool)
-    mn = v[..., :, 0].reshape(v.shape[:-2] + (3, 3))
-    if model == "fundamental":
-        mn = rank2(mn)
-    out = denormalise(model, mn, t0, t1)
-    return out, ok & np.isfinite(out).all((-1, -2))
-
-
-def solve_f8(p0, p1):
-    t0, ok0 = norm_t(p0)
-    t1, ok1 = norm_t(p1)
-    a = f_rows(apply(t0, p0), apply(t1, p1))
-    f, ok = solve_system("fundamental", np.swapaxes(a, -1, -2) @ a, t0, t1, True)
-    return f, ok & ok0 & ok1
-
-
-def errors(model, m, p0, p1):
-    """m [..., 3, 3], p [n, 2] -> squared pixel errors [..., n] (inf / NaN: never an inlier)."""
-    x0, y0, x1, y1 = p0[:, 0], p0[:, 1], p1[:, 0], p1[:, 1]
-    m = m[..., None, :, :]
-    with np.errstate(all="ignore"):
-        if model == "homography":
-            mi = np.linalg.inv(m)
-            pw = m[..., 2, 0] * x0 + m[..., 2, 1] * y0 + m[..., 2, 2]
-            px = (m[..., 0, 0] * x0 + m[..., 0, 1] * y0 + m[..., 0, 2]) / pw - x1
-            py = (m[..., 1, 0] * x0 + m[..., 1, 1] * y0 + m[..., 1, 2]) / pw - y1
-            qw = mi[..., 2, 0] * x1 + mi[..., 2, 1] * y1 + mi[..., 2, 2]
-            qx = (mi[..., 0, 0] * x1 + mi[..., 0, 1] * y1 + mi[..., 0, 2]) / qw - x0
-            qy = (mi[..., 1, 0] * x1 + mi[..., 1, 1] * y1 + mi[..., 1, 2]) / qw - y0
-            return 0.5 * (px * px + py * py + qx * qx + qy * qy)
-        f0 = m[..., 0, 0] * x0 + m[..., 0, 1] * y0 + m[..., 0, 2]
-        f1 = m[..., 1, 0] * x0 + m[..., 1, 1] * y0 + m[..., 1, 2]
-        f2 = m[..., 2, 0] * x0 + m[..., 2, 1] * y0 + m[..., 2, 2]
-        g0 = m[..., 0, 0] * x1 + m[..., 1, 0] * y1 + m[..., 2, 0]
-        g1 = m[..., 0, 1] * x1 + m[..., 1, 1] * y1 + m[..., 2, 1]
-        e = x1 * f0 + y1 * f1 + f2
-        return e * e / (f0 * f0 + f1 * f1 + g0 * g0 + g1 * g1)
-
-
-def output_scale(model, m):
-    nrm = np.linalg.norm(m)
-    flat = m.reshape(-1)
-    d = nrm if flat[np.argmax(np.abs(flat))] >= 0 else -nrm
-    if model == "homography" and abs(m[2, 2]) > 1e-12 * nrm:
-        d = m[2, 2]
-    return m / d
-
-
-def ransac_ref(p0, p1, model, thr, iterations, seed=0, pair_id=0):
-    """One pair's compacted matches [n, 2] -> dict(best, model [3, 3] (NaN when none), mask [n], count, samples)."""
-    p0, p1 = np.asarray(p0, np.float64), np.asarray(p1, np.float64)
-    n, s, t2 = len(p0), S[model], float(np.float32(thr)) ** 2
-    none = {"best": -1, "model": np.full((3, 3), np.nan), "mask": np.zeros(n, bool), "count": 0, "samples": None}
-    if n < s:
-        return none
-    samples = draw_samples(seed, pair_id, n, s, iterations)
-    m, ok = (solve_h4 if model == "homography" else solve_f8)(p0[samples], p1[samples])
-    e = errors(model, np.where(ok[:, None, None], m, np.eye(3)), p0, p1)   # degenerate: placeholder, not ranked
-    inl = e < t2
-    cnt = np.where(ok, inl.sum(1), -1)
-    cost = np.where(inl, e, 0).sum(1) + (n - inl.sum(1)) * t2
-    if not ok.any():
-        return dict(none, samples=samples)
-    order = np.lexsort((np.arange(iterations), cost, -cnt))
-    best = int(order[0])
-    mdl = m[best]
-    inl = errors(model, mdl, p0, p1) < t2
-    if inl.sum() >= s:
-        t0, ok0 = norm_t(p0[inl])
-        t1, ok1 = norm_t(p1[inl])
-        if ok0 and ok1:
-            u, u2 = apply(t0, p0[inl]), apply(t1, p1[inl])
-            a = h_rows(u, u2) if model == "homography" else f_rows(u, u2)
-            r, rok = solve_system(model, a.T @ a, t0, t1, False)
-            if rok and (model == "fundamental" or np.linalg.det(r) != 0):
-                mdl = r
-    mask = errors(model, mdl, p0, p1) < t2
-    return {"best": best, "model": output_scale(model, mdl), "mask": mask, "count": int(mask.sum()),
-            "samples": samples}
-
-
-# ---------------------------------------------------------------------------------------------- synthetic scenes
-def random_h(rs):
-    return np.array([[1 + rs.uniform(-.2, .2), rs.uniform(-.2, .2), rs.uniform(-60, 60)],
-                     [rs.uniform(-.2, .2), 1 + rs.uniform(-.2, .2), rs.uniform(-60, 60)],
-                     [rs.uniform(-3e-4, 3e-4), rs.uniform(-3e-4, 3e-4), 1.0]])
-
-
-def project_h(h, p):
-    q = p @ h[:, :2].T + h[:, 2]
-    return q[:, :2] / q[:, 2:]
-
-
-def rot(rs, deg):
-    ax = rs.standard_normal(3)
-    ax /= np.linalg.norm(ax)
-    a = np.deg2rad(deg)
-    k = np.array([[0, -ax[2], ax[1]], [ax[2], 0, -ax[0]], [-ax[1], ax[0], 0]])
-    return np.eye(3) + np.sin(a) * k + (1 - np.cos(a)) * k @ k
-
-
-def scene(rs, model, n, outlier_ratio, sigma=0.5, w=640, h=480):
-    """-> p0, p1 [n, 2] float32, is_inlier [n], ground-truth model, noise-free (p0, p1) of the inliers."""
-    n_out = int(round(outlier_ratio * n))
-    if model == "homography":
-        gt = random_h(rs)
-        p0 = rs.uniform((0, 0), (w, h), (n, 2))
-        clean1 = project_h(gt, p0)
-    else:
-        kk = np.array([[500.0, 0, w / 2], [0, 500.0, h / 2], [0, 0, 1]])
-        r, t = rot(rs, 8.0), np.array([1.0, rs.uniform(-.3, .3), rs.uniform(-.3, .3)])
-        X = np.stack([rs.uniform(-4, 4, n), rs.uniform(-3, 3, n), rs.uniform(6, 14, n)], 1)
-        x0 = X @ kk.T
-        p0 = x0[:, :2] / x0[:, 2:]
-        x1 = (X @ r.T + t) @ kk.T
-        clean1 = x1[:, :2] / x1[:, 2:]
-        tx = np.array([[0, -t[2], t[1]], [t[2], 0, -t[0]], [-t[1], t[0], 0]])
-        ki = np.linalg.inv(kk)
-        gt = ki.T @ tx @ r @ ki
-    clean0 = p0.copy()
-    p1 = clean1 + sigma * rs.standard_normal((n, 2))
-    p0 = p0 + sigma * rs.standard_normal((n, 2))
-    inl = np.ones(n, bool)
-    out = rs.permutation(n)[:n_out]
-    inl[out] = False
-    p1[out] = rs.uniform((0, 0), (w, h), (n_out, 2))
-    return p0.astype(np.float32), p1.astype(np.float32), inl, gt, (clean0[inl], clean1[inl])
-
-
-def pad_batch(pairs, K, rs=None):
-    """[(p0, p1)] -> padded [B, K, 2] arrays and a bool mask; with rs the valid entries go to random columns."""
-    B = len(pairs)
-    P0, P1 = np.full((B, K, 2), 7.0, np.float32), np.full((B, K, 2), -3.0, np.float32)   # junk in the padding
-    V = np.zeros((B, K), bool)
-    cols = []
-    for b, (a, c) in enumerate(pairs):
-        col = np.sort(rs.permutation(K)[:len(a)]) if rs is not None else np.arange(len(a))
-        P0[b, col], P1[b, col], V[b, col] = a, c, True
-        cols.append(col)
-    return P0, P1, V, cols
-
-
-def model_dist(a, b):
-    """Distance of two 3x3 models up to scale and sign."""
-    a, b = a / np.linalg.norm(a), b / np.linalg.norm(b)
-    return min(np.abs(a - b).max(), np.abs(a + b).max())
 
 
 def gpu(*arrays):
@@ -351,6 +82,35 @@ def test_host_validation_without_gpu():
             geometry.check_options(iterations=bad)
     with pytest.raises(ValueError, match="seed"):
         geometry.check_options(seed=-1)
+
+
+def test_workspace_layout_mirror_matches_the_library():
+    """ws_layout (how tests/test_geometry_edges_gpu.py reads the kernels' intermediate results back) is the library's
+    geometry_ws_layout; the size query needs no device."""
+    from loftr_b200 import _lib
+    lib = _lib.load()
+    for B in (0, 1, 3, 65535):
+        for K in (4, 8, 255, 257, 19200):
+            for it in (1, 63, 64, 65, 129, 2048):
+                assert lib.lb_geometry_workspace_bytes(B, K, it) == ws_layout(B, K, it)["total"], (B, K, it)
+    lay = ws_layout(3, 5, 65)
+    assert (lay["compact_col"], lay["n_valid"], lay["tile_best"], lay["n_tiles"]) == (240, 304, 320, 2)
+
+
+@pytest.mark.parametrize("model", list(S))
+def test_staging_cases_bite_on_the_reference(model):
+    """The staging grid of test_geometry_edges_gpu.py would catch a scoring loop that stops after its first round of
+    STAGE matches (another winner from n = 2048 on) or skips a partial last round (another tile count whenever one
+    exists: at n = 1025 the lone match of round 2 is an inlier)."""
+    for n in (1025, 2048, 2049, 4100):
+        p0, p1, it, seed = staging_case(model, n)
+        full = tile_ranking(p0, p1, model, STAGING_THR, it, seed)
+        win = lambda r: r[2][np.lexsort((r[2], r[1], -r[0]))[0]]
+        if n >= 2 * STAGE:
+            assert win(full) != win(tile_ranking(p0, p1, model, STAGING_THR, it, seed, upto=STAGE)), n
+        if n % STAGE:
+            partial = tile_ranking(p0, p1, model, STAGING_THR, it, seed, upto=n - n % STAGE)
+            assert (partial[0] != full[0]).any(), n
 
 
 # ---------------------------------------------------------------------------------------------- GPU tests
