@@ -59,7 +59,9 @@ extern "C" {
  * 107: lb_estimate_geometry (batched RANSAC homography / fundamental matrix per pair);
  * 108: lb_backbone_workspace_bytes_fp16 / lb_backbone_forward_fp16 (single-pass fp16 backbone);
  * 109: lb_transformer_forward_fp16 / lb_coarse_match_fp16 (single-pass fp16 transformers and coarse matching);
- * 110: lb_gemm_fp16 (test hook of the contraction core on single fp16 planes). */
+ * 110: lb_gemm_fp16 (test hook of the contraction core on single fp16 planes).
+ * Entries added without a version step (a caller finds them by name: a build that lacks one does not export it):
+ * lb_coarse_query / lb_fine_preprocess_centres (matching caller-given image0 points). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -297,6 +299,39 @@ int lb_coarse_match_capped(const LbCoarseMatchArgs* args /*host*/, int max_per_p
 int lb_coarse_match_fp16(const LbCoarseMatchArgs* args /*host*/, int max_per_pair, void* ws, size_t ws_bytes,
                          void* stream);
 
+/* Caller-given image0 points of every pair (found by name, see lb_version; LoFTR.match_points, DESIGN.md §17).  A separate structure, not
+ * new fields of LbCoarseMatchArgs: DESIGN.md §12.  Outputs are per query, q = b*Q + k. */
+typedef struct LbCoarseQueryArgs {
+  int Q;                  /* queries per pair */
+  const float* points0;   /* [n_pairs, Q, 2] (x, y) f32: image0 pixels, or source pixels when args->scale0 is given */
+  const uint8_t* valid0;  /* optional [n_pairs, Q]: 0 = not a query */
+  int H0, W0;             /* image0 size (hw0_i) */
+  int Hf0, Wf0;           /* fine map of image0 (hw0_f) */
+  int stride;             /* fine pixels per coarse cell (hw0_f / hw0_c) */
+  float fine_scale;       /* image pixels per fine pixel (hw0_i / hw0_f) */
+  long long* i_ids;       /* [n_pairs*Q] the query's cell in image0, -1 when it is not inside */
+  long long* j_ids;       /* [n_pairs*Q] the row arg-max of that cell in image1, -1 when not inside */
+  float* conf;            /* [n_pairs*Q] mconf's expression for (b, i, j); 0 when not inside */
+  uint8_t* mutual;        /* [n_pairs*Q] i is the column arg-max of j */
+  uint8_t* valid;         /* [n_pairs*Q] the forward would keep (b, i, j) before any per-pair cap */
+  uint8_t* inside;        /* [n_pairs*Q] the query was answered */
+  int* centres;           /* [2, n_pairs*Q, 2] fine-map (x, y) centres of the image0 / image1 windows */
+  long long* win_ids;     /* [3, n_pairs*Q] (b, i, j) for lb_fine_preprocess_centres / lb_fine_match: i = j = 0 when
+                           * the query is not inside, so every id is in range */
+  float* pts0_f;          /* [n_pairs*Q, 2] fine-grid image0 point (source pixels); NaN when not inside */
+  float* pts1_c;          /* [n_pairs*Q, 2] image1 window centre (source pixels): mkpts1_c of lb_fine_match */
+} LbCoarseQueryArgs;
+
+/* The coarse stage of lb_coarse_match (operand_planes 2) or lb_coarse_match_fp16 (1), answered for the points of
+ * `query` instead of as a match list.  A query is inside when valid0 allows it, its point (divided by scale0) is finite
+ * and in [0, W0 - 1] x [0, H0 - 1], its cell cx = clamp(floor(x / img_scale + 0.5)) (and y) is unmasked, and the row
+ * of that cell has a valid column.  Fine centres: f0 = clamp(floor(p / fine_scale + 0.5)) on the fine map, f1 =
+ * stride * (jx, jy) + f0 - stride * (cx, cy).  The match-list outputs of `args` (capacity, b_ids .. count) are not
+ * read or written; conf_matrix is written when given.  Same workspace as lb_coarse_match; one more launch after its
+ * flag pass (timing tag "match_query"), no per-pair cap and no compaction. */
+int lb_coarse_query(const LbCoarseMatchArgs* args /*host*/, const LbCoarseQueryArgs* query /*host*/,
+                    int operand_planes, void* ws, size_t ws_bytes, void* stream);
+
 typedef struct LbFinePreprocessArgs {
   const float* feat_f0;   /* fine maps, any strides (elements): index = n*sn + c*sc + y*sh + x*sw */
   const float* feat_f1;
@@ -335,6 +370,12 @@ int lb_fine_preprocess(const LbFinePreprocessArgs* args /*host*/, void* ws, size
  * img_idx0[b] of feat_f0 and image img_idx1[b] of feat_f1 (device ints [n_pairs], each in range of its bank; sn0 / sn1
  * step from one bank image to the next).  feat_c stays pair-major.  Same workspace as lb_fine_preprocess. */
 int lb_fine_preprocess_indexed(const LbFinePreprocessArgs* args /*host*/, const int* img_idx0, const int* img_idx1,
+                               void* ws, size_t ws_bytes, void* stream);
+/* lb_fine_preprocess with the window centres read from `centres` ([2, M, 2] fine-map (x, y) of side 0 then side 1,
+ * as lb_coarse_query writes them) instead of stride * (the cell of i_ids / j_ids) (found by name).  Windows m with
+ * inside[m] == 0 are gathered as zeros; b_ids / i_ids / j_ids still select the image and the coarse-feature bias and
+ * must be in range for every m.  M_live must be NULL.  Same workspace as lb_fine_preprocess. */
+int lb_fine_preprocess_centres(const LbFinePreprocessArgs* args /*host*/, const int* centres, const uint8_t* inside,
                                void* ws, size_t ws_bytes, void* stream);
 
 typedef struct LbFineMatchArgs {

@@ -75,6 +75,15 @@ class LbCoarseMatchArgs(C.Structure):
     ]
 
 
+class LbCoarseQueryArgs(C.Structure):
+    _fields_ = [
+        ("Q", c_int), ("points0", c_void_p), ("valid0", c_void_p), ("H0", c_int), ("W0", c_int),
+        ("Hf0", c_int), ("Wf0", c_int), ("stride", c_int), ("fine_scale", c_float),
+        ("i_ids", c_void_p), ("j_ids", c_void_p), ("conf", c_void_p), ("mutual", c_void_p), ("valid", c_void_p),
+        ("inside", c_void_p), ("centres", c_void_p), ("win_ids", c_void_p), ("pts0_f", c_void_p), ("pts1_c", c_void_p),
+    ]
+
+
 class LbFinePreprocessArgs(C.Structure):
     _fields_ = [
         ("feat_f0", c_void_p), ("feat_f1", c_void_p),
@@ -140,9 +149,13 @@ SIGNATURES = {
     "lb_coarse_match": (c_int, [C.POINTER(LbCoarseMatchArgs), c_void_p, c_size_t, c_void_p]),
     "lb_coarse_match_capped": (c_int, [C.POINTER(LbCoarseMatchArgs), c_int, c_void_p, c_size_t, c_void_p]),
     "lb_coarse_match_fp16": (c_int, [C.POINTER(LbCoarseMatchArgs), c_int, c_void_p, c_size_t, c_void_p]),
+    "lb_coarse_query": (c_int, [C.POINTER(LbCoarseMatchArgs), C.POINTER(LbCoarseQueryArgs), c_int, c_void_p, c_size_t,
+                                c_void_p]),
     "lb_fine_preprocess_workspace_bytes": (c_size_t, [c_long, c_int, c_int]),
     "lb_fine_preprocess": (c_int, [C.POINTER(LbFinePreprocessArgs), c_void_p, c_size_t, c_void_p]),
     "lb_fine_preprocess_indexed": (c_int, [C.POINTER(LbFinePreprocessArgs), c_void_p, c_void_p, c_void_p, c_size_t,
+                                           c_void_p]),
+    "lb_fine_preprocess_centres": (c_int, [C.POINTER(LbFinePreprocessArgs), c_void_p, c_void_p, c_void_p, c_size_t,
                                            c_void_p]),
     "lb_fine_match": (c_int, [C.POINTER(LbFineMatchArgs), c_void_p]),
     "lb_epipolar_errors": (c_int, [c_void_p, c_void_p, c_void_p, c_long, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -176,6 +189,10 @@ BACKBONE_FP16_VERSION = 108
 MATCH_FP16_VERSION = 109
 # oldest library with the contraction core's single-plane test hook (lb_gemm_fp16)
 GEMM_FP16_VERSION = 110
+# entries that came without a version step: `load()` binds each one the library exports, and `require_entries` stops
+# the paths that need one the library lacks
+POINTS_ENTRIES = ("lb_coarse_query", "lb_fine_preprocess_centres")   # LoFTR.match_points
+_OPTIONAL = set(POINTS_ENTRIES)
 GEOMETRY_HOMOGRAPHY = 0
 GEOMETRY_FUNDAMENTAL = 1
 _SINCE = {"lb_coarse_prep_indexed": FEATURE_BANK_VERSION, "lb_fine_preprocess_indexed": FEATURE_BANK_VERSION,
@@ -208,8 +225,8 @@ def load():
         raise LibraryMissing(f"{LIB_PATH} is version {lib.lb_version()}, older than the binding ({MIN_VERSION}): "
                              "rebuild it with `make`")
     for name, (res, args) in SIGNATURES.items():
-        if lib.lb_version() < _SINCE.get(name, 0):
-            continue             # not in this older build; `require` stops its callers
+        if lib.lb_version() < _SINCE.get(name, 0) or (name in _OPTIONAL and not hasattr(lib, name)):
+            continue             # not in this build; `require` / `require_entries` stop its callers
         fn = getattr(lib, name)  # AttributeError if the library does not export a declared symbol
         fn.restype = res
         fn.argtypes = args
@@ -224,6 +241,16 @@ def require(version: int, what: str):
     if v < version:
         raise RuntimeError(f"loftr_b200: {what} needs library version {version} or newer, but {LIB_PATH} is version "
                            f"{v}: rebuild it with `make`")
+
+
+def require_entries(names, what: str):
+    """Raise unless the library exports every entry of `names`, naming `what`, the first missing entry and the
+    library's version."""
+    lib = load()
+    missing = [n for n in names if not hasattr(lib, n)]
+    if missing:
+        raise RuntimeError(f"loftr_b200: {what} needs {missing[0]}, which {LIB_PATH} (version {lib.lb_version()}) does "
+                           "not export: rebuild it with `make`")
 
 
 def check(rc: int):
@@ -242,8 +269,8 @@ def timing_enable(on: bool):
 
 
 def timing_collect() -> dict:
-    """-> {tag: (total_ms, launches)} for every kernel tag (tensor-core kernels, match cap, image front end, geometry)
-    recorded since timing_enable(True)."""
+    """-> {tag: (total_ms, launches)} for every kernel tag (tensor-core kernels, match cap, point queries, image front
+    end, geometry) recorded since timing_enable(True)."""
     lib = load()
     n = lib.lb_timing_num_tags()
     ms = (C.c_double * n)()

@@ -57,15 +57,16 @@ static inline int cdiv(long a, long b) { return static_cast<int>((a + b - 1) / b
 
 // ------------------------------------------------------------------------------------------------ timing hook
 // Optional per-launch CUDA-event timing of the tensor-core kernels (bench.py's roofline leg), of the per-pair match
-// cap, of the image front end and of the geometry estimator (its three launches as one record): events are recorded on
-// the launching stream right around the kernels, and only while timing is enabled.  TAG_NONE: not timed.
+// cap, of the point queries, of the image front end and of the geometry estimator (its three launches as one record):
+// events are recorded on the launching stream right around the kernels, and only while timing is enabled.  TAG_NONE:
+// not timed.
 enum Tag { TAG_NONE = -1, TAG_GEMM_TEST = 0, TAG_PROJ, TAG_MERGE_LN, TAG_MLP1, TAG_MLP2_LN, TAG_SCORE_LSE,
            TAG_SCORE_ARGMAX, TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_FULL_ATTN, TAG_MATCH_CAP, TAG_PREPROCESS,
-           TAG_GEOMETRY, TAG_COUNT };
+           TAG_GEOMETRY, TAG_MATCH_QUERY, TAG_COUNT };
 static const char* kTagNames[TAG_COUNT] = {"gemm_test", "proj_act", "merge_ln", "mlp1_relu", "mlp2_ln_res",
                                            "score_lse", "score_argmax", "fine_merge", "backbone_conv",
                                            "tf_kv_proj_fused", "tf_q_attn_fused", "tf_full_attn", "match_cap",
-                                           "preprocess", "geometry"};
+                                           "preprocess", "geometry", "match_query"};
 struct TimingRec {
   cudaEvent_t e0, e1;
   int tag;
@@ -1300,24 +1301,19 @@ size_t lb_coarse_match_workspace_bytes(int n_pairs, int L, int S) {
 
 }  // extern "C"
 
-// max_per_pair: 0 = every match; otherwise each pair keeps its max_per_pair most confident matches (match_cap_kernel).
+// The coarse quantities of every row of every pair (n_pairs > 0), shared by lb_coarse_match* and lb_coarse_query: the
+// score passes, the Sinkhorn iterations and prefilter, the optional conf_matrix, and match_flag_kernel's flag / conf.
+// On return `w` holds them in the workspace and `sp` describes them.
 // kP: operand planes of the score products (Operands); every pass recomputes the same logits.
 template <int kP>
-static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, size_t ws_bytes, void* stream) {
-  DeviceScope dev;
-  LB_TRY(dev.bind(a->count));
+static int coarse_rows(const LbCoarseMatchArgs* a, const DeviceScope& dev, void* ws, size_t ws_bytes, cudaStream_t st,
+                       CmWs& w, SelectParams& sp) {
   const int n = a->n_pairs, L = a->L, S = a->S, C = a->C;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (n <= 0) {
-    LB_CUDA(cudaMemsetAsync(a->count, 0, sizeof(int), st));
-    return 0;
-  }
   if (L != a->h0c * a->w0c || S != a->h1c * a->w1c) return fail("L/S do not match the coarse grid sizes");
   if (C % kBlockK != 0) return fail("C=%d must be a multiple of %d", C, kBlockK);
   if ((a->mask0 == nullptr) != (a->mask1 == nullptr)) return fail("mask0 and mask1 must be given together");
   if (!ws) return fail("workspace pointer is null");
   Bump b{static_cast<uint8_t*>(ws), ws_bytes};
-  CmWs w;
   carve_cm(b, w, n, L, S);
   if (!b.ok) return fail("coarse-match workspace too small: need %zu bytes", lb_coarse_match_workspace_bytes(n, L, S));
 
@@ -1442,7 +1438,6 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
                                  st)));
   }
 
-  SelectParams sp;
   sp.n_pairs = n; sp.L = L; sp.S = S;
   sp.h0c = a->h0c; sp.w0c = a->w0c; sp.h1c = a->h1c; sp.w1c = a->w1c;
   sp.border = a->border_rm;
@@ -1454,7 +1449,24 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
   sp.ext0 = masked ? w.ext0 : nullptr; sp.ext1 = masked ? w.ext1 : nullptr;
   sp.row_dead = row_dead; sp.col_dead = col_dead;
   sp.flag = w.flag; sp.conf = w.conf;
-  LB_TRY(launch(TAG_NONE, match_flag_kernel, cdiv(nl, TB), TB, 0, st, sp));
+  return launch(TAG_NONE, match_flag_kernel, cdiv(nl, TB), TB, 0, st, sp);
+}
+
+// max_per_pair: 0 = every match; otherwise each pair keeps its max_per_pair most confident matches (match_cap_kernel).
+template <int kP>
+static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, size_t ws_bytes, void* stream) {
+  DeviceScope dev;
+  LB_TRY(dev.bind(a->count));
+  const int n = a->n_pairs, L = a->L, S = a->S;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (n <= 0) {
+    LB_CUDA(cudaMemsetAsync(a->count, 0, sizeof(int), st));
+    return 0;
+  }
+  CmWs w;
+  SelectParams sp;
+  LB_TRY(coarse_rows<kP>(a, dev, ws, ws_bytes, st, w, sp));
+  const long nl = static_cast<long>(n) * L;
   if (max_per_pair > 0) {
     LB_TRY(launch(TAG_MATCH_CAP, match_cap_kernel, n, kCapBlock, 0, st, w.flag, w.conf, L, max_per_pair));
   }
@@ -1488,6 +1500,39 @@ int lb_coarse_match_fp16(const LbCoarseMatchArgs* a, int max_per_pair, void* ws,
   return coarse_match<1>(a, max_per_pair, ws, ws_bytes, stream);
 }
 
+int lb_coarse_query(const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, int operand_planes, void* ws,
+                    size_t ws_bytes, void* stream) {
+  if (operand_planes != 1 && operand_planes != 2)
+    return fail("lb_coarse_query: operand_planes must be 1 (fp16) or 2 (split) (got %d)", operand_planes);
+  if (q->Q <= 0 || a->n_pairs <= 0) return 0;
+  DeviceScope dev;
+  LB_TRY(dev.bind(q->i_ids));
+  if (!q->points0) return fail("lb_coarse_query: points0 is null");
+  if (q->stride <= 0 || q->fine_scale <= 0.f || q->Hf0 <= 0 || q->Wf0 <= 0)
+    return fail("lb_coarse_query: bad fine grid (stride %d, fine_scale %g, %d x %d)", q->stride, q->fine_scale, q->Hf0,
+                q->Wf0);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CmWs w;
+  SelectParams sp;
+  LB_TRY(operand_planes == 2 ? coarse_rows<2>(a, dev, ws, ws_bytes, st, w, sp)
+                             : coarse_rows<1>(a, dev, ws, ws_bytes, st, w, sp));
+  QueryParams qp;
+  qp.n_pairs = a->n_pairs; qp.Q = q->Q; qp.L = a->L; qp.S = a->S;
+  qp.h0c = a->h0c; qp.w0c = a->w0c; qp.w1c = a->w1c;
+  qp.H0 = q->H0; qp.W0 = q->W0; qp.Hf0 = q->Hf0; qp.Wf0 = q->Wf0;
+  qp.stride = q->stride; qp.s_c = a->img_scale; qp.s_f = q->fine_scale;
+  qp.conf_bias = sp.conf_bias;
+  qp.points0 = q->points0; qp.valid0 = q->valid0;
+  qp.scale0 = a->scale0; qp.scale1 = a->scale1; qp.mask0 = a->mask0;
+  qp.row_key = sp.row_key; qp.row_arg = sp.row_arg; qp.col_arg = sp.col_arg; qp.rowterm = sp.rowterm;
+  qp.flag = sp.flag;
+  qp.i_ids = q->i_ids; qp.j_ids = q->j_ids; qp.conf = q->conf;
+  qp.mutual = q->mutual; qp.valid = q->valid; qp.inside = q->inside;
+  qp.centres = q->centres; qp.win = q->win_ids; qp.pts0_f = q->pts0_f; qp.pts1_c = q->pts1_c;
+  const long nq = static_cast<long>(a->n_pairs) * q->Q;
+  return launch(TAG_MATCH_QUERY, coarse_query_kernel, cdiv(nq, 256), 256, 0, st, qp);
+}
+
 // ------------------------------------------------------------------------------------------------ fine level
 struct FpWs {
   __half* win_hi;   // [2*M*W*W, Cf] gathered windows
@@ -1508,9 +1553,10 @@ size_t lb_fine_preprocess_workspace_bytes(long M, int W, int Cf) {
   return b.off + 256;
 }
 
-// img_idx0 / img_idx1: NULL, or pair b's windows are read from image img_idx0[b] of feat_f0 / img_idx1[b] of feat_f1
-static int fine_preprocess(const LbFinePreprocessArgs* a, const int* img_idx0, const int* img_idx1, void* ws,
-                           size_t ws_bytes, void* stream) {
+// img_idx0 / img_idx1: NULL, or pair b's windows are read from image img_idx0[b] of feat_f0 / img_idx1[b] of feat_f1.
+// centres / inside: NULL, or the window centres come from the centre table (lb_fine_preprocess_centres).
+static int fine_preprocess(const LbFinePreprocessArgs* a, const int* img_idx0, const int* img_idx1, const int* centres,
+                           const uint8_t* inside, void* ws, size_t ws_bytes, void* stream) {
   if (a->M <= 0) return 0;
   DeviceScope dev;
   LB_TRY(dev.bind(a->x_f32));
@@ -1534,12 +1580,14 @@ static int fine_preprocess(const LbFinePreprocessArgs* a, const int* img_idx0, c
   g.out_hi = w.win_hi; g.out_lo = w.win_lo; g.ld = a->Cf;
   g.live = a->M_live;
   g.img_idx0 = img_idx0; g.img_idx1 = img_idx1;
+  g.centres = centres; g.inside = inside;
   const bool vec8 = a->sc0 == 1 && a->sc1 == 1 && a->Cf % 8 == 0 && g.ld % 8 == 0 && a->sw0 % 4 == 0 && a->sw1 % 4 == 0 &&
                     a->sh0 % 4 == 0 && a->sh1 % 4 == 0 && a->sn0 % 4 == 0 && a->sn1 % 4 == 0 &&
                     (reinterpret_cast<uintptr_t>(a->feat_f0) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->feat_f1) & 15) == 0;
   const unsigned wins = static_cast<unsigned>(2 * a->M);
-  const auto gather = img_idx0 ? (vec8 ? fine_gather_vec8_kernel<true> : fine_gather_kernel<true>)
-                               : (vec8 ? fine_gather_vec8_kernel<false> : fine_gather_kernel<false>);
+  const auto gather = centres    ? (vec8 ? fine_gather_vec8_kernel<false, true> : fine_gather_kernel<false, true>)
+                      : img_idx0 ? (vec8 ? fine_gather_vec8_kernel<true> : fine_gather_kernel<true>)
+                                 : (vec8 ? fine_gather_vec8_kernel<false> : fine_gather_kernel<false>);
   LB_TRY(launch(TAG_NONE, gather, wins, 256, 0, st, g));
 
   FineBiasParams fb;
@@ -1567,13 +1615,20 @@ static int fine_preprocess(const LbFinePreprocessArgs* a, const int* img_idx0, c
 }
 
 int lb_fine_preprocess(const LbFinePreprocessArgs* a, void* ws, size_t ws_bytes, void* stream) {
-  return fine_preprocess(a, nullptr, nullptr, ws, ws_bytes, stream);
+  return fine_preprocess(a, nullptr, nullptr, nullptr, nullptr, ws, ws_bytes, stream);
 }
 
 int lb_fine_preprocess_indexed(const LbFinePreprocessArgs* a, const int* img_idx0, const int* img_idx1, void* ws,
                                size_t ws_bytes, void* stream) {
   if (a->M > 0 && (!img_idx0 || !img_idx1)) return fail("lb_fine_preprocess_indexed: img_idx0 and img_idx1 are required");
-  return fine_preprocess(a, img_idx0, img_idx1, ws, ws_bytes, stream);
+  return fine_preprocess(a, img_idx0, img_idx1, nullptr, nullptr, ws, ws_bytes, stream);
+}
+
+int lb_fine_preprocess_centres(const LbFinePreprocessArgs* a, const int* centres, const uint8_t* inside, void* ws,
+                               size_t ws_bytes, void* stream) {
+  if (a->M > 0 && (!centres || !inside)) return fail("lb_fine_preprocess_centres: centres and inside are required");
+  if (a->M_live) return fail("lb_fine_preprocess_centres: M_live is not supported (every query has a window)");
+  return fine_preprocess(a, nullptr, nullptr, centres, inside, ws, ws_bytes, stream);
 }
 
 int lb_fine_match(const LbFineMatchArgs* a, void* stream) {

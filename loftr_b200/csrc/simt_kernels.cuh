@@ -528,6 +528,95 @@ __global__ void match_flag_kernel(const SelectParams p) {
   p.conf[gi] = conf;
 }
 
+// Caller-given image0 points -> the coarse answer of each (LoFTR.match_points, DESIGN.md §17): the cell i nearest to
+// the point, its row arg-max j, conf and flags as match_flag_kernel computes them for row i, and the fine window
+// centres of both images.  One thread per query; queries that are not inside get NaN points, conf 0, no flags,
+// ids -1 and fine-stage ids (win) 0, so no later kernel reads through an invalid index.
+struct QueryParams {
+  int n_pairs, Q, L, S;
+  int h0c, w0c, w1c;
+  int H0, W0;               // image0 (network pixels)
+  int Hf0, Wf0;             // fine map of image0
+  int stride;               // fine pixels per coarse cell
+  float s_c, s_f;           // image pixels per coarse / fine pixel
+  float conf_bias;
+  const float* points0;     // [n*Q, 2] (x, y), source pixels when scale0 is given
+  const uint8_t* valid0;    // optional [n*Q]
+  const float* scale0;      // optional [n, 2]
+  const float* scale1;
+  const uint8_t* mask0;     // optional [n*L]
+  const float* row_key;     // [n*L]
+  const int* row_arg;
+  const int* col_arg;       // [n*S]
+  const float* rowterm;
+  const uint8_t* flag;      // [n*L] match_flag_kernel's test
+  long long* i_ids;         // [n*Q]
+  long long* j_ids;
+  float* conf;
+  uint8_t* mutual;
+  uint8_t* valid;
+  uint8_t* inside;
+  int* centres;             // [2, n*Q, 2] fine-map (x, y) of the image0 / image1 window centres
+  long long* win;           // [3, n*Q] (b, i, j) read by the fine stage
+  float* pts0_f;            // [n*Q, 2]
+  float* pts1_c;
+};
+__global__ void coarse_query_kernel(const QueryParams p) {
+  const long q = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x;
+  const long nq = static_cast<long>(p.n_pairs) * p.Q;
+  if (q >= nq) return;
+  const int b = static_cast<int>(q / p.Q);
+  float sx0 = 1.f, sy0 = 1.f, sx1 = 1.f, sy1 = 1.f;
+  if (p.scale0) { sx0 = p.scale0[2 * b]; sy0 = p.scale0[2 * b + 1]; sx1 = p.scale1[2 * b]; sy1 = p.scale1[2 * b + 1]; }
+  float px = p.points0[2 * q], py = p.points0[2 * q + 1];
+  if (p.scale0) { px = px / sx0; py = py / sy0; }
+  // the comparisons are false for NaN, so a NaN coordinate fails here
+  bool in = (!p.valid0 || p.valid0[q]) && px >= 0.f && px <= static_cast<float>(p.W0 - 1) && py >= 0.f &&
+            py <= static_cast<float>(p.H0 - 1);
+  int i = 0, j = 0, cx = 0, cy = 0;
+  long gi = 0;
+  if (in) {
+    cx = min(max(static_cast<int>(floorf(px / p.s_c + 0.5f)), 0), p.w0c - 1);
+    cy = min(max(static_cast<int>(floorf(py / p.s_c + 0.5f)), 0), p.h0c - 1);
+    i = cy * p.w0c + cx;
+    gi = static_cast<long>(b) * p.L + i;
+    if (p.mask0 && !p.mask0[gi]) in = false;
+  }
+  if (in) {
+    j = p.row_arg[gi];
+    in = j >= 0 && j < p.S && p.row_key[gi] > -1.0e29f;   // a row without any valid column has no answer
+  }
+  const long nq2 = 2 * nq;
+  if (!in) {
+    const float nan = __int_as_float(0x7fffffff);
+    p.i_ids[q] = -1; p.j_ids[q] = -1;
+    p.conf[q] = 0.f;
+    p.mutual[q] = 0; p.valid[q] = 0; p.inside[q] = 0;
+    p.centres[2 * q] = 0; p.centres[2 * q + 1] = 0; p.centres[2 * (nq + q)] = 0; p.centres[2 * (nq + q) + 1] = 0;
+    p.win[q] = b; p.win[nq + q] = 0; p.win[nq2 + q] = 0;
+    p.pts0_f[2 * q] = nan; p.pts0_f[2 * q + 1] = nan;
+    p.pts1_c[2 * q] = nan; p.pts1_c[2 * q + 1] = nan;
+    return;
+  }
+  const int fx0 = min(max(static_cast<int>(floorf(px / p.s_f + 0.5f)), 0), p.Wf0 - 1);
+  const int fy0 = min(max(static_cast<int>(floorf(py / p.s_f + 0.5f)), 0), p.Hf0 - 1);
+  const int jy = j / p.w1c, jx = j - jy * p.w1c;
+  const int fx1 = p.stride * jx + (fx0 - p.stride * cx);
+  const int fy1 = p.stride * jy + (fy0 - p.stride * cy);
+  p.i_ids[q] = i; p.j_ids[q] = j;
+  p.conf[q] = expf(p.row_key[gi] + p.rowterm[gi] + p.conf_bias);   // match_flag_kernel's conf
+  p.mutual[q] = p.col_arg[static_cast<long>(b) * p.S + j] == i ? 1 : 0;
+  p.valid[q] = p.flag[gi];
+  p.inside[q] = 1;
+  p.centres[2 * q] = fx0; p.centres[2 * q + 1] = fy0;
+  p.centres[2 * (nq + q)] = fx1; p.centres[2 * (nq + q) + 1] = fy1;
+  p.win[q] = b; p.win[nq + q] = i; p.win[nq2 + q] = j;
+  p.pts0_f[2 * q] = static_cast<float>(fx0) * p.s_f * sx0;
+  p.pts0_f[2 * q + 1] = static_cast<float>(fy0) * p.s_f * sy0;
+  p.pts1_c[2 * q] = static_cast<float>(fx1) * p.s_f * sx1;
+  p.pts1_c[2 * q + 1] = static_cast<float>(fy1) * p.s_f * sy1;
+}
+
 // Ordered stream compaction (ascending (b, i) like torch.where, coarse_matching.py:194) + coarse
 // keypoints (coarse_matching.py:241-250).
 struct CompactParams {
@@ -791,13 +880,36 @@ struct FineGatherParams {
   const int* live;  // optional device count: windows m >= min(*live, M) of each side are skipped (M = capacity)
   const int* img_idx0;  // kIndexed: pair b reads image img_idx0[b] of feat0 / img_idx1[b] of feat1
   const int* img_idx1;
+  const int* centres;   // kCentres: [2, M, 2] fine-map (x, y) window centres of side 0 / side 1
+  const uint8_t* inside;  // kCentres: [M]; windows m with inside[m] == 0 are written as zeros
 };
 // Image of `feat0` / `feat1` that pair b's side-`side` windows are read from.
 template <bool kIndexed>
 __device__ __forceinline__ int fine_gather_image(const FineGatherParams& p, int side, int b) {
   return kIndexed ? (side ? p.img_idx1 : p.img_idx0)[b] : b;
 }
-template <bool kIndexed>
+// Window m's centre on side `side` is (step * cx, step * cy) on the fine map: step = stride and (cx, cy) the coarse
+// cell of i_ids / j_ids, or (kCentres) step = 1 and (cx, cy) read from the centre table.  `answered` is false for a
+// kCentres window whose query is not inside.
+template <bool kCentres>
+__device__ __forceinline__ void fine_gather_centre(const FineGatherParams& p, int side, long m, int& cx, int& cy,
+                                                   int& step, bool& answered) {
+  if (kCentres) {
+    const int* c = p.centres + 2 * (side * p.M + m);
+    cx = c[0];
+    cy = c[1];
+    step = 1;
+    answered = p.inside[m] != 0;
+  } else {
+    const int idx = static_cast<int>(side ? p.j_ids[m] : p.i_ids[m]);
+    const int wc = side ? p.w1c : p.w0c;
+    cy = idx / wc;
+    cx = idx - cy * wc;
+    step = p.stride;
+    answered = true;
+  }
+}
+template <bool kIndexed, bool kCentres = false>
 __global__ void fine_gather_kernel(const FineGatherParams p) {
   const int WW = p.W * p.W;
   const long win = blockIdx.x;             // 0 .. 2M-1
@@ -805,9 +917,9 @@ __global__ void fine_gather_kernel(const FineGatherParams p) {
   const long m = side ? win - p.M : win;
   if (p.live != nullptr && m >= *p.live) return;
   const int img = fine_gather_image<kIndexed>(p, side, static_cast<int>(p.b_ids[m]));
-  const int idx = static_cast<int>(side ? p.j_ids[m] : p.i_ids[m]);
-  const int wc = side ? p.w1c : p.w0c;
-  const int cy = idx / wc, cx = idx - cy * wc;
+  int cx, cy, step;
+  bool answered;
+  fine_gather_centre<kCentres>(p, side, m, cx, cy, step, answered);
   const float* feat = side ? p.feat1 : p.feat0;
   const long sn = side ? p.sn1 : p.sn0, sc = side ? p.sc1 : p.sc0, sh = side ? p.sh1 : p.sh0,
              sw = side ? p.sw1 : p.sw0;
@@ -815,10 +927,10 @@ __global__ void fine_gather_kernel(const FineGatherParams p) {
   for (int e = threadIdx.x; e < WW * p.Cf; e += blockDim.x) {
     const int k = e / p.Cf, c = e - k * p.Cf;
     const int ky = k / p.W, kx = k - ky * p.W;
-    const int y = p.stride * cy - p.W / 2 + ky;
-    const int x = p.stride * cx - p.W / 2 + kx;
+    const int y = step * cy - p.W / 2 + ky;
+    const int x = step * cx - p.W / 2 + kx;
     float v = 0.f;
-    if (y >= 0 && y < Hf && x >= 0 && x < Wf) v = feat[img * sn + c * sc + y * sh + x * sw];
+    if (answered && y >= 0 && y < Hf && x >= 0 && x < Wf) v = feat[img * sn + c * sc + y * sh + x * sw];
     __half hh, ll;
     split_f16(v, hh, ll);
     const long row = win * WW + k;
@@ -829,7 +941,7 @@ __global__ void fine_gather_kernel(const FineGatherParams p) {
 
 // Channel-contiguous (NHWC, sc == 1) maps with Cf % 8 == 0: one thread moves 8 channels of one window position --
 // two 16-byte loads, packed split, one 16-byte store per plane (the element-wise kernel above issues 2-byte stores).
-template <bool kIndexed>
+template <bool kIndexed, bool kCentres = false>
 __global__ void __launch_bounds__(256) fine_gather_vec8_kernel(const FineGatherParams p) {
   const int WW = p.W * p.W;
   const int c8n = p.Cf >> 3;
@@ -838,19 +950,19 @@ __global__ void __launch_bounds__(256) fine_gather_vec8_kernel(const FineGatherP
   const long m = side ? win - p.M : win;
   if (p.live != nullptr && m >= *p.live) return;
   const int img = fine_gather_image<kIndexed>(p, side, static_cast<int>(p.b_ids[m]));
-  const int idx = static_cast<int>(side ? p.j_ids[m] : p.i_ids[m]);
-  const int wc = side ? p.w1c : p.w0c;
-  const int cy = idx / wc, cx = idx - cy * wc;
+  int cx, cy, step;
+  bool answered;
+  fine_gather_centre<kCentres>(p, side, m, cx, cy, step, answered);
   const float* feat = side ? p.feat1 : p.feat0;
   const long sn = side ? p.sn1 : p.sn0, sh = side ? p.sh1 : p.sh0, sw = side ? p.sw1 : p.sw0;
   const int Hf = side ? p.Hf1 : p.Hf0, Wf = side ? p.Wf1 : p.Wf0;
   for (int e = threadIdx.x; e < WW * c8n; e += blockDim.x) {
     const int k = e / c8n, c = (e - k * c8n) << 3;
     const int ky = k / p.W, kx = k - ky * p.W;
-    const int y = p.stride * cy - p.W / 2 + ky;
-    const int x = p.stride * cx - p.W / 2 + kx;
+    const int y = step * cy - p.W / 2 + ky;
+    const int x = step * cx - p.W / 2 + kx;
     float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
-    if (y >= 0 && y < Hf && x >= 0 && x < Wf) {
+    if (answered && y >= 0 && y < Hf && x >= 0 && x < Wf) {
       const float4* src = reinterpret_cast<const float4*>(feat + img * sn + y * sh + x * sw + c);
       v0 = src[0];
       v1 = src[1];

@@ -480,27 +480,7 @@ class CoarseMatching(nn.Module):
         mk0 = torch.empty(cap, 2, dtype=torch.float32, device=dev)
         mk1 = torch.empty(cap, 2, dtype=torch.float32, device=dev)
         count = torch.zeros(1, dtype=torch.int32, device=dev)
-        a = _lib.LbCoarseMatchArgs()
-        esz = hi.element_size()
-        a.f0_hi, a.f0_lo = hi.data_ptr(), lo.data_ptr()
-        a.f1_hi, a.f1_lo = hi.data_ptr() + n * L * ld * esz, lo.data_ptr() + n * L * ld * esz
-        a.ld, a.n_pairs, a.L, a.S, a.C = ld, n, L, S, c
-        (a.h0c, a.w0c), (a.h1c, a.w1c) = data["hw0_c"], data["hw1_c"]
-        a.match_type = _lib.MATCH_DUAL_SOFTMAX if self.match_type == "dual_softmax" else _lib.MATCH_SINKHORN
-        a.temperature = float(getattr(self, "temperature", 1.0))
-        a.thr, a.border_rm = float(self.thr), int(self.border_rm)
-        keep = []
-        if self.match_type == "sinkhorn":
-            bs = self.bin_score.detach().float().reshape(1).contiguous()
-            keep.append(bs)
-            a.bin_score, a.skh_iters, a.skh_prefilter = bs.data_ptr(), int(self.skh_iters), int(bool(self.skh_prefilter))
-        a.mask0, a.mask1 = _lib.ptr(mask_u8_0), _lib.ptr(mask_u8_1)
-        a.img_scale = data["hw0_i"][0] / data["hw0_c"][0]
-        if "scale0" in data:
-            s0 = data["scale0"].to(dev, torch.float32).contiguous()
-            s1 = data["scale1"].to(dev, torch.float32).contiguous()
-            keep += [s0, s1]
-            a.scale0, a.scale1 = s0.data_ptr(), s1.data_ptr()
+        a, keep = self._args(hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1)
         a.capacity = cap
         a.b_ids, a.i_ids, a.j_ids = b_ids.data_ptr(), i_ids.data_ptr(), j_ids.data_ptr()
         a.mconf, a.mkpts0_c, a.mkpts1_c, a.count = mconf.data_ptr(), mk0.data_ptr(), mk1.data_ptr(), count.data_ptr()
@@ -537,6 +517,76 @@ class CoarseMatching(nn.Module):
             data["num_matches"] = count
             return count
         return None
+
+    def _args(self, hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1):
+        """LbCoarseMatchArgs of the coarse stage without its match-list outputs -> (args, tensors it points into)."""
+        dev = hi.device
+        a = _lib.LbCoarseMatchArgs()
+        esz = hi.element_size()
+        a.f0_hi, a.f0_lo = hi.data_ptr(), lo.data_ptr()
+        a.f1_hi, a.f1_lo = hi.data_ptr() + n * L * ld * esz, lo.data_ptr() + n * L * ld * esz
+        a.ld, a.n_pairs, a.L, a.S, a.C = ld, n, L, S, c
+        (a.h0c, a.w0c), (a.h1c, a.w1c) = data["hw0_c"], data["hw1_c"]
+        a.match_type = _lib.MATCH_DUAL_SOFTMAX if self.match_type == "dual_softmax" else _lib.MATCH_SINKHORN
+        a.temperature = float(getattr(self, "temperature", 1.0))
+        a.thr, a.border_rm = float(self.thr), int(self.border_rm)
+        keep = []
+        if self.match_type == "sinkhorn":
+            bs = self.bin_score.detach().float().reshape(1).contiguous()
+            keep.append(bs)
+            a.bin_score, a.skh_iters, a.skh_prefilter = bs.data_ptr(), int(self.skh_iters), int(bool(self.skh_prefilter))
+        a.mask0, a.mask1 = _lib.ptr(mask_u8_0), _lib.ptr(mask_u8_1)
+        a.img_scale = data["hw0_i"][0] / data["hw0_c"][0]
+        if "scale0" in data:
+            s0 = data["scale0"].to(dev, torch.float32).contiguous()
+            s1 = data["scale1"].to(dev, torch.float32).contiguous()
+            keep += [s0, s1]
+            a.scale0, a.scale1 = s0.data_ptr(), s1.data_ptr()
+        return a, keep
+
+    def query(self, hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1, points0, valid0=None):
+        """The coarse stage for caller-given image0 points (LoFTR.match_points, DESIGN.md §17): planes as `run`,
+        points0 [n, Q, 2] f32 and valid0 (None or bool [n, Q]) on the device, validated by the caller.  No host sync.
+        -> dict of the per-query outputs (q_i_ids, q_j_ids, qconf, qmutual, qvalid, qinside [n, Q]; qpts0_f, qpts1_c
+        [n, Q, 2]) and of what the fine stage reads: "centres" int32 [2, n*Q, 2] and "win_ids" int64 [3, n*Q].
+        The per-pair cap (max_matches_per_pair) is not applied."""
+        _require_eval(self)
+        _lib.require_entries(_lib.POINTS_ENTRIES, "match_points")
+        lib = _lib.load()
+        dev = hi.device
+        q = points0.shape[1]
+        nq = n * q
+        out = {"q_i_ids": torch.empty(n, q, dtype=torch.int64, device=dev),
+               "q_j_ids": torch.empty(n, q, dtype=torch.int64, device=dev),
+               "qconf": torch.empty(n, q, dtype=torch.float32, device=dev),
+               "qmutual": torch.empty(n, q, dtype=torch.bool, device=dev),
+               "qvalid": torch.empty(n, q, dtype=torch.bool, device=dev),
+               "qinside": torch.empty(n, q, dtype=torch.bool, device=dev),
+               "qpts0_f": torch.empty(n, q, 2, dtype=torch.float32, device=dev),
+               "qpts1_c": torch.empty(n, q, 2, dtype=torch.float32, device=dev),
+               "centres": torch.empty(2, nq, 2, dtype=torch.int32, device=dev),
+               "win_ids": torch.empty(3, nq, dtype=torch.int64, device=dev)}
+        a, keep = self._args(hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1)
+        qa = _lib.LbCoarseQueryArgs()
+        points0 = points0.contiguous()
+        keep.append(points0)
+        qa.Q, qa.points0 = q, points0.data_ptr()
+        if valid0 is not None:
+            valid0 = valid0.contiguous().view(torch.uint8)
+            keep.append(valid0)
+            qa.valid0 = valid0.data_ptr()
+        (qa.H0, qa.W0), (qa.Hf0, qa.Wf0) = data["hw0_i"], data["hw0_f"]
+        qa.stride = data["hw0_f"][0] // data["hw0_c"][0]
+        qa.fine_scale = data["hw0_i"][0] / data["hw0_f"][0]
+        qa.i_ids, qa.j_ids, qa.conf = out["q_i_ids"].data_ptr(), out["q_j_ids"].data_ptr(), out["qconf"].data_ptr()
+        qa.mutual, qa.valid, qa.inside = (out[k].data_ptr() for k in ("qmutual", "qvalid", "qinside"))
+        qa.centres, qa.win_ids = out["centres"].data_ptr(), out["win_ids"].data_ptr()
+        qa.pts0_f, qa.pts1_c = out["qpts0_f"].data_ptr(), out["qpts1_c"].data_ptr()
+        nbytes = lib.lb_coarse_match_workspace_bytes(n, L, S)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _lib.check(lib.lb_coarse_query(C.byref(a), C.byref(qa), 1 if self._precision == "fp16" else 2, ws.data_ptr(),
+                                       nbytes, _stream(hi)))
+        return out
 
     @torch.no_grad()
     def forward(self, feat_c0, feat_c1, data, mask_c0=None, mask_c1=None):
@@ -579,13 +629,15 @@ class FinePreprocess(_PackedCache, nn.Module):
                 "bm": self.merge_feat.bias.detach().float().contiguous(),
                 "wm_hi": hi, "wm_lo": lo, "wm_scale": msc}
 
-    def run(self, feat_f0, feat_f1, feat_c_all, n, L, S, data, live=None, img_idx=None):
+    def run(self, feat_f0, feat_f1, feat_c_all, n, L, S, data, live=None, img_idx=None, centres=None):
         """-> _TokenState of the fine transformer (rows: side, match, window position); with M == 0 it has no rows
         and nothing is launched.  M is the length of data["b_ids"].
         `live`: int32 device count; the match keys of `data` are then capacity buffers and only windows below the
         count are gathered (rows keep the capacity layout side*cap*WW + m*WW + k).
         `img_idx`: (idx0, idx1) int32 device tensors [n]: feat_f0 / feat_f1 are then feature banks and pair b's
-        windows are read from their images idx0[b] / idx1[b]."""
+        windows are read from their images idx0[b] / idx1[b].
+        `centres`: (centres, inside) of CoarseMatching.query: the windows are centred on the fine pixels of the int32
+        table [2, M, 2] rather than on the cells of i_ids / j_ids, and windows m with inside[m] false are zeros."""
         lib = _lib.load()
         W = self.W
         stride = data["hw0_f"][0] // data["hw0_c"][0]
@@ -614,7 +666,10 @@ class FinePreprocess(_PackedCache, nn.Module):
         a.M_live = _lib.ptr(live)
         nbytes = lib.lb_fine_preprocess_workspace_bytes(m, W, cf)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        if img_idx is None:
+        if centres is not None:
+            _lib.check(lib.lb_fine_preprocess_centres(C.byref(a), centres[0].data_ptr(), centres[1].data_ptr(),
+                                                      ws.data_ptr(), nbytes, _stream(feat_f0)))
+        elif img_idx is None:
             _lib.check(lib.lb_fine_preprocess(C.byref(a), ws.data_ptr(), nbytes, _stream(feat_f0)))
         else:
             _lib.check(lib.lb_fine_preprocess_indexed(C.byref(a), img_idx[0].data_ptr(), img_idx[1].data_ptr(),
@@ -882,6 +937,54 @@ class LoFTR(nn.Module):
                 raise ValueError(f"forward_static: `{k}` is on {t.device}, image0 on {dev}")
         self._match_pairs(data, *self._backbone_pairs(data), static=True, capacity=capacity)
 
+    @torch.no_grad()
+    def match_points(self, data, points0, valid0=None):
+        """Refines caller-given image0 points to image1 through the coarse and fine stages (DESIGN.md §17).
+
+        data: forward's inputs (image0 / image1, optional mask0 / mask1 and scale0 / scale1), all on the device.
+        points0: float32 [N, Q, 2] (x, y) in image0 pixels, or in source pixels when scale0 is given (as mkpts0_f).
+        valid0: optional bool [N, Q]; false marks a slot that is not a query.
+
+        Writes qpts0_f (the query snapped to the fine grid), qpts1_c (centre of the image1 search window), qpts1_f (the
+        refined correspondence), all [N, Q, 2] f32 in source pixels; qexpec_f [N, Q, 3] (as expec_f); qconf [N, Q]
+        (mconf's expression for the chosen cell pair); q_i_ids / q_j_ids [N, Q] int64 (the query's cell and its best
+        cell in image1, -1: none); qmutual, qvalid (the forward would keep the pair, before any per-pair cap) and
+        qinside (the query was answered) [N, Q] bool.  A query that is not inside has NaN points and qexpec_f, qconf 0,
+        false flags and ids -1.  Nothing of forward's match list is written.
+
+        Each query's outputs depend only on its own point, pair and images.  A query at a forward match's mkpts0_c gets
+        that match's j_ids, mconf, mkpts1_c, mkpts1_f and expec_f bit for bit.  Shapes are fixed by [N, Q] and there is
+        no host synchronisation, so the call can be captured by `torch.cuda.graph` after one eager call."""
+        _require_eval(self)
+        _lib.require_entries(_lib.POINTS_ENTRIES, "match_points")
+        _check_points(data, points0, valid0)
+        n, q = points0.shape[:2]
+        dev = points0.device
+        if q == 0:
+            data.update(_query_outputs(n, 0, dev))
+            return
+        feat_c0, feat_c1, feat_f0, feat_f1 = self._backbone_pairs(data)
+        c = feat_c0.shape[1]
+        (h0, w0), (h1, w1) = data["hw0_c"], data["hw1_c"]
+        L, S = h0 * w0, h1 * w1
+        state, m0, m1 = self._coarse_tokens(data, feat_c0, feat_c1)
+        out = self.coarse_matching.query(state.cat_hi, state.cat_lo, 2 * c, n, L, S, c, data, m0, m1, points0, valid0)
+        centres, win = out.pop("centres"), out.pop("win_ids")
+        inside = out["qinside"].reshape(-1)
+        # the fine stage reads the windows as a match list of N*Q entries: (b, i, j) = win_ids, mkpts1_c = qpts1_c
+        work = {k: data[k] for k in ("bs", "hw0_i", "hw1_i", "hw0_c", "hw1_c", "hw0_f", "hw1_f", "scale0", "scale1")
+                if k in data}
+        work.update({"b_ids": win[0], "i_ids": win[1], "j_ids": win[2], "mkpts0_c": out["qpts0_f"].view(-1, 2),
+                     "mkpts1_c": out["qpts1_c"].view(-1, 2)})
+        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, n, L, S, work,
+                                          centres=(centres, inside))
+        ww = self.fine_preprocess.W ** 2
+        self.loftr_fine.run(fstate, n * q, ww, ww)
+        self.fine_matching(*fstate.sides(n * q, ww, ww), work)
+        out["qpts1_f"] = work["mkpts1_f"].view(n, q, 2)
+        out["qexpec_f"] = work["expec_f"].view(n, q, 3).masked_fill_(~out["qinside"][..., None], float("nan"))
+        data.update(out)
+
     def _backbone_pairs(self, data):
         """Step 1 of the forward (no host sync): the backbone on image0 / image1 -> (feat_c0, feat_c1, feat_f0,
         feat_f1); writes bs and the image, coarse and fine sizes into `data`."""
@@ -905,6 +1008,28 @@ class LoFTR(nn.Module):
         img_idx: optional (idx0, idx1) int32 [bs]: the maps are then feature banks, read at image idx0[b] / idx1[b] for
         pair b.  static: the match keys are buffers of `capacity` entries (None: the default capacity) and the fine
         stage is bounded on the device by their count (CoarseMatching.run), so that nothing synchronises with the host."""
+        bs, c = data["bs"], feat_c0.shape[1]
+        (h0, w0), (h1, w1) = data["hw0_c"], data["hw1_c"]
+        L, S = h0 * w0, h1 * w1
+        state, m0, m1 = self._coarse_tokens(data, feat_c0, feat_c1, img_idx)
+
+        # 3. coarse matching                                                           [loftr.py:67]
+        live = self.coarse_matching.run(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1, static, capacity)
+
+        # 4. fine-level refinement over M windows: the match count, or the capacity    [loftr.py:70-72]
+        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, bs, L, S, data, live, img_idx)
+        m, ww = data["b_ids"].shape[0], self.fine_preprocess.W ** 2
+        if m:
+            self.loftr_fine.run(fstate, m, ww, ww, live=live)
+
+        # 5. fine matching                                                             [loftr.py:75]
+        self.fine_matching(*fstate.sides(m, ww, ww), data, live=live)
+        if self.expose_coarse_features:   # test / debugging tap, off by default: not a reference key
+            data["_feat_c0"], data["_feat_c1"] = state.sides(bs, L, S)
+
+    def _coarse_tokens(self, data, feat_c0, feat_c1, img_idx=None):
+        """Step 2 of the forward: position encoding, token layout and coarse transformer (img_idx as in
+        `_match_pairs`) -> (token state, flattened uint8 mask0, mask1 views or None)."""
         # 2. position encoding + token layout + coarse transformer                     [loftr.py:58-64]
         lib = _lib.load()
         bs = data["bs"]
@@ -934,20 +1059,7 @@ class LoFTR(nn.Module):
             mask_all = torch.cat([m0, m1]).contiguous()
             m0, m1 = mask_all[: bs * L], mask_all[bs * L:]
         self.loftr_coarse.run(state, bs, L, S, mask_all)
-
-        # 3. coarse matching                                                           [loftr.py:67]
-        live = self.coarse_matching.run(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1, static, capacity)
-
-        # 4. fine-level refinement over M windows: the match count, or the capacity    [loftr.py:70-72]
-        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, bs, L, S, data, live, img_idx)
-        m, ww = data["b_ids"].shape[0], self.fine_preprocess.W ** 2
-        if m:
-            self.loftr_fine.run(fstate, m, ww, ww, live=live)
-
-        # 5. fine matching                                                             [loftr.py:75]
-        self.fine_matching(*fstate.sides(m, ww, ww), data, live=live)
-        if self.expose_coarse_features:   # test / debugging tap, off by default: not a reference key
-            data["_feat_c0"], data["_feat_c1"] = state.sides(bs, L, S)
+        return state, m0, m1
 
     def _packed_caches(self):
         """Every owner of a packed-weight cache: the caching submodules and the tensor-core backbone."""
@@ -981,6 +1093,48 @@ def _require_static(model, capacity, what):
                          "the output list depend on the data")
     if capacity is not None and int(capacity) < 1:
         raise ValueError(f"capacity must be a positive number of matches (got {capacity})")
+
+
+_QUERY_KEYS = {"qpts0_f": (torch.float32, 2), "qpts1_c": (torch.float32, 2), "qpts1_f": (torch.float32, 2),
+               "qexpec_f": (torch.float32, 3), "qconf": (torch.float32, 0), "q_i_ids": (torch.int64, 0),
+               "q_j_ids": (torch.int64, 0), "qmutual": (torch.bool, 0), "qvalid": (torch.bool, 0),
+               "qinside": (torch.bool, 0)}
+
+
+def _query_outputs(n, q, dev):
+    """Empty output tensors of LoFTR.match_points for [n, q] queries."""
+    return {k: torch.empty(n, q, *((d,) if d else ()), dtype=t, device=dev) for k, (t, d) in _QUERY_KEYS.items()}
+
+
+def _check_points(data, points0, valid0):
+    """Host-side validation of LoFTR.match_points' arguments, before any launch: shapes and dtypes first, then that
+    everything is on image0's CUDA device."""
+    for k in ("image0", "image1"):
+        if k not in data:
+            raise ValueError(f"match_points: data must hold `{k}`")
+    if ("scale0" in data) != ("scale1" in data):
+        raise ValueError("match_points: give scale0 and scale1 together")
+    if ("mask0" in data) != ("mask1" in data):
+        raise ValueError("match_points: give mask0 and mask1 together")
+    n = data["image0"].shape[0]
+    if not torch.is_tensor(points0) or points0.dtype != torch.float32:
+        raise TypeError("match_points: points0 must be a float32 tensor (got "
+                        f"{points0.dtype if torch.is_tensor(points0) else type(points0).__name__})")
+    if points0.dim() != 3 or points0.shape[0] != n or points0.shape[2] != 2:
+        raise ValueError(f"match_points: points0 must be [N, Q, 2] with N = {n} pairs (got {tuple(points0.shape)})")
+    if valid0 is not None:
+        if not torch.is_tensor(valid0) or valid0.dtype != torch.bool:
+            raise TypeError("match_points: valid0 must be a bool tensor")
+        if tuple(valid0.shape) != tuple(points0.shape[:2]):
+            raise ValueError(f"match_points: valid0 must be [N, Q] = {tuple(points0.shape[:2])} (got "
+                             f"{tuple(valid0.shape)})")
+    dev = data["image0"].device
+    named = [(k, data[k]) for k in ("image0", "image1", "mask0", "mask1", "scale0", "scale1") if k in data]
+    for k, t in named + [("points0", points0)] + ([("valid0", valid0)] if valid0 is not None else []):
+        if not torch.is_tensor(t) or not t.is_cuda:
+            raise ValueError(f"match_points: `{k}` must be a CUDA tensor")
+        if t.device != dev:
+            raise ValueError(f"match_points: `{k}` is on {t.device}, image0 on {dev}")
 
 
 def _weight_refs(model):
