@@ -438,6 +438,8 @@ static int conv_shape(const ConvDesc& d, const Planes& wgt_rem, bool lo, int rem
   const int tiles_h = (d.H_out + kConvTileH - 1) / kConvTileH;
   const int tiles_w = (d.W_out + kConvTileW - 1) / kConvTileW;
   const int m_tiles = tiles_h * tiles_w, n_tiles = (d.Cout + BN - 1) / BN;
+  if (n_tiles != 1)   // EpiConvImpl stages the folded BatchNorm of one n-tile per CTA
+    return fail("convolution with Cout=%d needs one %d-wide n-tile, got %d", d.Cout, BN, n_tiles);
   const int rem_groups = d.rem ? (taps + rem_taps_per_group - 1) / rem_taps_per_group : 0;
   *s = GemmShape{d.N, m_tiles * kBlockM, d.Cout, taps * d.cin_blocks * kBlockK, /*b_batched=*/0, m_tiles, n_tiles,
                  /*n_chunks=*/n_tiles, /*tiles_per_chunk=*/1,
@@ -625,7 +627,7 @@ struct ConvRun {
   const BbBuf* res;
   const BbBuf* up;
   int up_h, up_w;
-  const BbBuf* out;
+  const BbBuf* out;     // outputs (planes and / or fp32): run_conv builds the epilogue's store maps over them
   float* out_f32;
   int f32_ld;
 };
@@ -655,8 +657,7 @@ static int launch_conv_on(const ConvRun& r, const ConvDesc& d, const OutMaps& om
   const Planes wr{w.wr_hi, w.wr_lo, static_cast<long>(taps) * kRemChannels, 0};
   typename Epi::Params ep{w.scale, w.shift, r.act, r.res ? r.res->hi : nullptr, r.res ? r.res->lo : nullptr,
                           r.res ? r.res->ld : 0, r.up ? r.up->hi : nullptr, r.up ? r.up->lo : nullptr,
-                          r.up ? r.up->ld : 0, r.up_h, r.up_w, r.out ? r.out->hi : nullptr,
-                          r.out ? r.out->lo : nullptr, r.out ? r.out->ld : 0, r.out_f32, r.f32_ld, 0, 0, 0, om};
+                          r.up ? r.up->ld : 0, r.up_h, r.up_w, 0, 0, 0, om};
   if constexpr (kHalo) return launch_conv_halo<BN, Epi>(in, wg, wr, d, ep, sms, st);
   else return launch_conv<BN, Epi>(in, wg, wr, d, ep, sms, st);
 }
@@ -902,12 +903,9 @@ static int tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const Lb
     using Epi = Operands<EpiLayerNorm<BN>, kP>;
     Planes A{w.att_hi + x_base * C, w.att_lo + x_base * C, C, xbs_a};
     Planes B{lw.wm_hi, lw.wm_lo, C, 0};
-    OutMaps om;
-    LB_TRY(fill_out_maps(&om, static_cast<__half*>(st.cat_hi) + x_base * ldc + C, static_cast<__half*>(st.cat_lo) + x_base * ldc + C,
-                         ldc, nullptr, 0, C, xM, xb));
-    typename Epi::Params ep{lw.ln1_g, lw.ln1_b, 1e-5f, nullptr, 0, nullptr, nullptr, 0, nullptr, 0,
-                            static_cast<__half*>(st.cat_hi) + x_base * ldc,
-                            static_cast<__half*>(st.cat_lo) + x_base * ldc, static_cast<int>(ldc), C, lw.s_m, om};
+    typename Epi::Params ep{lw.ln1_g, lw.ln1_b, 1e-5f, nullptr, nullptr, 0, lw.s_m, {}};
+    LB_TRY(fill_out_maps(&ep.om, static_cast<__half*>(st.cat_hi) + x_base * ldc + C,
+                         static_cast<__half*>(st.cat_lo) + x_base * ldc + C, ldc, nullptr, 0, C, xM, xb));
     LB_TRY((launch_gemm<BN, Epi>(TAG_MERGE_LN, A, B, gemm_shape<BN>(xb, xM, C, C, false, 0, live, x_group_rows), ep,
                                  sms, stream)));
   }
@@ -929,13 +927,10 @@ static int tf_layer_pass(const LbEncoderLayerWeights& lw, int C, int H, const Lb
     Planes A{w.h_hi + x_base * ldc, w.h_lo + x_base * ldc, ldc, xbs};
     Planes B{lw.w2_hi, lw.w2_lo, 2 * C, 0};
     float* xf = write_f32 ? st.x_f32 + x_base * C : nullptr;
-    OutMaps om;
-    LB_TRY(fill_out_maps(&om, static_cast<__half*>(st.cat_hi) + x_base * ldc, static_cast<__half*>(st.cat_lo) + x_base * ldc, ldc, xf,
-                         C, C, xM, xb));
-    typename Epi::Params ep{lw.ln2_g, lw.ln2_b, 1e-5f, nullptr, 0, cat_hi + x_base * ldc, cat_lo + x_base * ldc,
-                            static_cast<int>(ldc), xf, C,
-                            static_cast<__half*>(st.cat_hi) + x_base * ldc,
-                            static_cast<__half*>(st.cat_lo) + x_base * ldc, static_cast<int>(ldc), 0, lw.s_2, om};
+    typename Epi::Params ep{lw.ln2_g, lw.ln2_b, 1e-5f, cat_hi + x_base * ldc, cat_lo + x_base * ldc,
+                            static_cast<int>(ldc), lw.s_2, {}};
+    LB_TRY(fill_out_maps(&ep.om, static_cast<__half*>(st.cat_hi) + x_base * ldc,
+                         static_cast<__half*>(st.cat_lo) + x_base * ldc, ldc, xf, C, C, xM, xb));
     LB_TRY((launch_gemm<BN, Epi>(TAG_MLP2_LN, A, B, gemm_shape<BN>(xb, xM, C, 2 * C, false, 0, live, x_group_rows), ep,
                                  sms, stream)));
   }

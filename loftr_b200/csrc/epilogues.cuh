@@ -96,15 +96,16 @@ __device__ __forceinline__ void load_planes32(const __half* hp, const __half* lp
 
 
 // ------------------------------------------------------------------------------------------------
-// Coalesced epilogue I/O.  An epilogue thread owns one accumulator ROW, so a warp-wide 16-byte store of "my row's
+// Coalesced residual loads.  An epilogue thread owns one accumulator ROW, so a warp-wide 16-byte load of "my row's
 // next 16 bytes" touches 32 different cache lines (32 sectors per request: the L1 tag stage, not DRAM, becomes the
-// limiter -- l1tex at 70-75 % in the round-1 ncu captures).  These helpers transpose a [32 rows x 64 B] block through
-// a 2 KB per-warp shared-memory scratch (XOR-swizzled, bank-conflict free both ways) so that every global access
-// instruction covers 8 rows x 64 contiguous bytes.  Rows are addressed by a per-lane pointer (lane = row; nullptr =
-// row not stored / read as zero), so the same code serves row-major matrices and NHWC pixel rows.
+// limiter -- l1tex at 70-75 % in the round-1 ncu captures).  warp_issue_planes32 / warp_finish_planes32 read a
+// [32 rows x 64 B] block with every global load covering 8 rows x 64 contiguous bytes and transpose it into the owning
+// lanes through a 2 KB per-warp shared-memory scratch (XOR-swizzled, bank-conflict free both ways).  Rows are addressed
+// by a per-lane pointer (lane = row; nullptr = row read as zero), so the same code serves row-major matrices and NHWC
+// pixel rows.  Outputs leave through TMA stores (below).
 // Per-warp 4 KB staging tile at the START of the epilogue area (1024-byte aligned): a [32 rows x 128 B] fp32 block or
 // two [32 rows x 64 B] plane blocks (hi at +0, lo at +2048) for TMA stores; its first 2 KB double as the transposer
-// scratch of the coalesced load / store helpers below.
+// scratch of the residual loads.
 constexpr int kEpiScratchBytes = 8 * 4096;   // 8 epilogue warps x 4 KB
 __device__ __forceinline__ uint32_t* epi_scratch(uint8_t* base) {
   return reinterpret_cast<uint32_t*>(base + ((epi_tid() >> 5) << 12));
@@ -113,66 +114,6 @@ template <class T>
 __device__ __forceinline__ T* shfl_ptr(T* p, int src_lane) {
   const unsigned long long v = __shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(p), src_lane);
   return reinterpret_cast<T*>(v);
-}
-// w[16]: 64 bytes of this lane's row -> *(row_ptr + 0..63) for every lane with row_ptr != nullptr
-__device__ __forceinline__ void warp_store_rows64(uint32_t* scr, uint8_t* row_ptr, const uint32_t (&w)[16]) {
-  const int lane = threadIdx.x & 31;
-  __syncwarp();
-#pragma unroll
-  for (int q = 0; q < 4; ++q)
-    *reinterpret_cast<uint4*>(scr + lane * 16 + ((q ^ ((lane >> 1) & 3)) << 2)) =
-        make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
-  __syncwarp();
-  const int g = lane & 3;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = (lane >> 2) + 8 * i;
-    uint8_t* dst = shfl_ptr(row_ptr, r);
-    const uint4 v = *reinterpret_cast<const uint4*>(scr + r * 16 + ((g ^ ((r >> 1) & 3)) << 2));
-    if (dst) *reinterpret_cast<uint4*>(dst + g * 16) = v;
-  }
-}
-// inverse: 64 bytes at row_ptr (zeros for nullptr) -> w[16] of the owning lane
-__device__ __forceinline__ void warp_load_rows64(uint32_t* scr, const uint8_t* row_ptr, uint32_t (&w)[16]) {
-  const int lane = threadIdx.x & 31;
-  const int g = lane & 3;
-  __syncwarp();
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = (lane >> 2) + 8 * i;
-    const uint8_t* src = shfl_ptr(row_ptr, r);
-    uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (src) v = *reinterpret_cast<const uint4*>(src + g * 16);
-    *reinterpret_cast<uint4*>(scr + r * 16 + ((g ^ ((r >> 1) & 3)) << 2)) = v;
-  }
-  __syncwarp();
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const uint4 v = *reinterpret_cast<const uint4*>(scr + lane * 16 + ((q ^ ((lane >> 1) & 3)) << 2));
-    w[4 * q] = v.x; w[4 * q + 1] = v.y; w[4 * q + 2] = v.z; w[4 * q + 3] = v.w;
-  }
-}
-// 32 values of my row as fp16 hi/lo planes: hi_ptr / lo_ptr address (row, first column) or nullptr.  kPlanes = 1:
-// the hi plane only (round to nearest even; lo_ptr unused).
-template <int kPlanes = 2>
-__device__ __forceinline__ void warp_store_planes32(uint32_t* scr, __half* hi_ptr, __half* lo_ptr, const float (&x)[32]) {
-  uint32_t h[16], l[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    split_f16x2(x[2 * j], x[2 * j + 1], h[j], l[j]);
-  }
-  warp_store_rows64(scr, reinterpret_cast<uint8_t*>(hi_ptr), h);
-  if constexpr (kPlanes == 2) warp_store_rows64(scr, reinterpret_cast<uint8_t*>(lo_ptr), l);
-}
-__device__ __forceinline__ void warp_store_f32x32(uint32_t* scr, float* ptr, const float (&x)[32]) {
-  uint32_t a[16], b[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    a[j] = __float_as_uint(x[j]);
-    b[j] = __float_as_uint(x[16 + j]);
-  }
-  warp_store_rows64(scr, reinterpret_cast<uint8_t*>(ptr), a);
-  warp_store_rows64(scr, ptr ? reinterpret_cast<uint8_t*>(ptr) + 64 : nullptr, b);
 }
 // 32 values of my row from fp16 hi/lo planes, in two steps: `issue` puts the lane's eight 16-byte global loads in flight
 // (rows lane/4 + 8i, 16-byte group lane%4), `finish` transposes them through the scratch into this lane's row.  An
@@ -230,16 +171,6 @@ __device__ __forceinline__ void warp_finish_planes32(uint32_t* scr, const uint4 
     }
   }
 }
-__device__ __forceinline__ void warp_load_f32x32(uint32_t* scr, const float* ptr, float (&x)[32]) {
-  uint32_t a[16], b[16];
-  warp_load_rows64(scr, reinterpret_cast<const uint8_t*>(ptr), a);
-  warp_load_rows64(scr, ptr ? reinterpret_cast<const uint8_t*>(ptr) + 64 : nullptr, b);
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    x[j] = __uint_as_float(a[j]);
-    x[16 + j] = __uint_as_float(b[j]);
-  }
-}
 
 
 // ------------------------------------------------------------------------------------------------
@@ -249,9 +180,7 @@ __device__ __forceinline__ void warp_load_f32x32(uint32_t* scr, const float* ptr
 // tile is reused only after the engine has read the previous block (wait_group.read).
 struct OutMaps {            // filled on the host (engine.cu make_out_map_*) for the outputs an epilogue writes
   CUtensorMap hi, lo, f32;
-  int use;                  // bit 0: planes map set, bit 1: fp32 map set.  The host always sets the bits of the outputs
-                            // it passes; EpiLayerNorm and EpiConv keep pointer stores for a clear bit because without
-                            // that code ptxas allocates their registers worse (more spills in EpiConv<256, 0>)
+  int use;                  // bit 0: planes map set, bit 1: fp32 map set; an epilogue writes exactly the outputs set here
   int dims;                 // 3: (col, row, batch) coordinates;  4: NHWC (channel, x, y, image) coordinates
 };
 struct OutCoord {           // where this warp's 32-row block goes
@@ -459,19 +388,11 @@ struct EpiLayerNorm {
     const float* gamma;
     const float* beta;
     float eps;
-    const float* residual;  // optional fp32 residual [rows, ld_res]
-    int ld_res;
     const __half* res_hi;   // optional residual as fp16 planes [rows, ld_res_pl] (x = hi + lo, exact to 2^-22): the
     const __half* res_lo;   // residual stream then needs no fp32 master copy between layers
     int ld_res_pl;
-    float* out_f32;         // optional [rows, ld_f32]
-    int ld_f32;
-    __half* out_hi;         // optional planes [rows, ld_pl], written at column offset pl_col0
-    __half* out_lo;
-    int ld_pl;
-    int pl_col0;
     float acc_scale;        // 2^-e of the weight planes
-    OutMaps om;             // TMA-store maps of (out_hi, out_lo) [based at column pl_col0] and out_f32
+    OutMaps om;             // TMA-store maps of the outputs: om.use bit 0 = fp16 planes, bit 1 = fp32 (either or both)
   };
   // gamma / beta are read through the read-only cache (2 KB, L1-resident): the shared memory goes to the staging tiles
   static constexpr int kSmemBytes = kEpiScratchBytes + 2 * 128 * 8 + 128 * 4;
@@ -495,9 +416,6 @@ struct EpiLayerNorm {
         prefetch_l2(p.res_hi + grow * p.ld_res_pl + c0 + c);
         prefetch_l2(p.res_lo + grow * p.ld_res_pl + c0 + c);
       }
-    }
-    if (p.residual) {
-      for (int c = 0; c < BLOCK_N / 2; c += 32) prefetch_l2(p.residual + grow * p.ld_res + c0 + c);
     }
   }
   // the two threads that share a row (column halves) exchange their partial (sum, sum of squares) through smem
@@ -566,33 +484,17 @@ struct EpiLayerNorm {
         x[4 * j4 + 2] = (x[4 * j4 + 2] * p.acc_scale - mean) * rstd * g4.z + b4.z;
         x[4 * j4 + 3] = (x[4 * j4 + 3] * p.acc_scale - mean) * rstd * g4.w + b4.w;
       }
-      // warp-cooperative (coalesced) residual loads and stores: every lane takes part, invalid rows pass nullptr
-      if (p.om.use && (p.residual || p.res_hi)) stage_quiesce();
-      if (p.residual) {
-        float r[32];
-        warp_load_f32x32(scr, row_ok ? p.residual + grow * p.ld_res + c * 32 : nullptr, r);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] += r[j];
-      }
+      // the residual rows pass through the warp's staging tile: every lane takes part, invalid rows read zeros
       if (p.res_hi) {
+        stage_quiesce();
         float r[32];
         warp_finish_planes32(scr, rh, rl, r);
 #pragma unroll
         for (int j = 0; j < 32; ++j) x[j] += r[j];
       }
       const OutCoord oc{c * 32, m0 + ((epi_tid() >> 5) & 3) * 32, batch, 0};
-      if (p.out_f32) {
-        if (p.om.use & 2) warp_tma_store_f32x32(scr, p.om, oc, x);
-        else warp_store_f32x32(scr, row_ok ? p.out_f32 + grow * p.ld_f32 + c * 32 : nullptr, x);
-      }
-      if (p.out_hi) {
-        if (p.om.use & 1) {
-          warp_tma_store_planes32(scr, p.om, oc, x);
-        } else {
-          const long off = grow * p.ld_pl + p.pl_col0 + c * 32;
-          warp_store_planes32(scr, row_ok ? p.out_hi + off : nullptr, row_ok ? p.out_lo + off : nullptr, x);
-        }
-      }
+      if (p.om.use & 2) warp_tma_store_f32x32(scr, p.om, oc, x);
+      if (p.om.use & 1) warp_tma_store_planes32(scr, p.om, oc, x);
     }
   }
 };
@@ -688,13 +590,9 @@ struct EpiConvImpl {
     const __half* up_hi;  // optional x2-upsample source planes [batches, up_h, up_w, up_ld]
     const __half* up_lo;
     int up_ld, up_h, up_w;
-    __half* out_hi;       // optional NHWC planes [batches*H*W, out_ld]
-    __half* out_lo;
-    int out_ld;
-    float* out_f32;       // optional NHWC fp32 [batches*H*W, f32_ld]
-    int f32_ld;
     int H_out, W_out, tiles_w;
-    OutMaps om;           // NHWC TMA-store maps (channel, x, y, image): box 32 channels x 16 x 2 pixels
+    OutMaps om;           // NHWC TMA-store maps of the outputs (channel, x, y, image): box 32 channels x 16 x 2 pixels;
+                          // om.use bit 0 = fp16 planes, bit 1 = fp32 (either or both)
   };
   static constexpr int kChunks = (BLOCK_N + 31) / 32;        // 32-column groups of the tile (the last may be partial)
   static constexpr int kChunksHalf0 = (kChunks + 1) / 2;     // column half 0 takes the first ones
@@ -715,17 +613,12 @@ struct EpiConvImpl {
     s_scale = reinterpret_cast<float*>(smem + kEpiScratchBytes);
     s_shift = s_scale + kCols;
     xscr = kOwnXpose ? reinterpret_cast<uint32_t*>(smem + kXposeOffset + ((epi_tid() >> 5) << 11)) : scr;
-    if (s.n_tiles == 1) {   // every layer of the backbone: one n-tile -> the folded BatchNorm is staged once per CTA
-      stage_affine(0);
-      epi_bar_sync();
-    }
-  }
-  __device__ void stage_affine(int n0) {
+    // one n-tile covers every output channel (conv_shape checks it): the folded BatchNorm is staged once per CTA
     for (int j = epi_tid(); j < kCols; j += kEpiThreads) {
-      const int c = n0 + j;
-      s_scale[j] = c < s.N ? p.scale[c] : 0.f;
-      s_shift[j] = c < s.N ? p.shift[c] : 0.f;
+      s_scale[j] = j < s.N ? p.scale[j] : 0.f;
+      s_shift[j] = j < s.N ? p.shift[j] : 0.f;
     }
+    epi_bar_sync();
   }
   __device__ void item_begin(int, int, int) {}
   __device__ void item_end(int, int, int) {}
@@ -765,10 +658,6 @@ struct EpiConvImpl {
     }
   }
   __device__ void tile(uint32_t acc_row, int batch, int m0, int n0) {
-    if (s.n_tiles > 1) {
-      stage_affine(n0);
-      epi_bar_sync();
-    }
     const int row = epi_row();
     const int mt = m0 / kBlockM;
     const int ty = mt / p.tiles_w, tx = mt - ty * p.tiles_w;
@@ -798,7 +687,7 @@ struct EpiConvImpl {
     const int c_end = epi_half() == 0 ? kChunksHalf0 : kChunks;
     // launch parameters read once per tile (inside the chunk loop each constant-bank load was an exposed latency)
     const int act = p.act;
-    const bool tma_pl = p.out_hi && (p.om.use & 1), tma_f = p.out_f32 && (p.om.use & 2);
+    const bool tma_pl = p.om.use & 1, tma_f = p.om.use & 2;
 #pragma unroll 1
     for (int c = c_begin; c < c_end; ++c) {
       const int col = n0 + c * 32;
@@ -815,9 +704,9 @@ struct EpiConvImpl {
 #pragma unroll
       for (int j = 0; j < 32; ++j) v[j] = fmaf(v[j], s_scale[c * 32 + j], s_shift[c * 32 + j]);
       if (nvalid == 32) {
-        // full 32-channel group: warp-cooperative (coalesced) loads / stores, pixels outside the image pass nullptr
+        // full 32-channel group: warp-cooperative (coalesced) residual loads, pixels outside the image pass nullptr
         if (p.res_hi) {
-          if (p.om.use && !kOwnXpose) stage_quiesce();
+          if (!kOwnXpose) stage_quiesce();
           float r[32];
           warp_finish_planes32<kPlanes>(xscr, rh, rl, r);
 #pragma unroll
@@ -842,7 +731,7 @@ struct EpiConvImpl {
           }
         }
       } else if (ok) {
-        // channel tail (e.g. 196 = 6*32 + 4): scalar path.  Fully unrolled with a predicate: a run-time trip count
+        // channel tail (e.g. 196 = 6*32 + 4): scalar reads.  Fully unrolled with a predicate: a run-time trip count
         // would index v[] dynamically and push the whole array through local memory (LDL/STL in every chunk)
         const float wy0 = 1.f - wy1, wx0 = 1.f - wx1;
 #pragma unroll
@@ -874,26 +763,7 @@ struct EpiConvImpl {
       const OutCoord oc{col, tx * kConvTileW, ty * kConvTileH + ((epi_tid() >> 5) & 3) * 2, batch};
       if (tma_f) warp_tma_store_f32x32(scr, p.om, oc, v);
       if (tma_pl) warp_tma_store_planes32<kPlanes>(scr, p.om, oc, v);
-      if (nvalid == 32) {
-        if (p.out_f32 && !tma_f) warp_store_f32x32(scr, ok ? p.out_f32 + pix * p.f32_ld + col : nullptr, v);
-        if (p.out_hi && !tma_pl)
-          warp_store_planes32<kPlanes>(scr, ok ? p.out_hi + pix * p.out_ld + col : nullptr,
-                                       ok && kPlanes == 2 ? p.out_lo + pix * p.out_ld + col : nullptr, v);
-      } else if (ok && !(tma_pl || tma_f)) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          if (j >= nvalid) continue;
-          if (p.out_f32) p.out_f32[pix * p.f32_ld + col + j] = v[j];
-          if (p.out_hi) {
-            __half hh, ll;
-            split_f16(v[j], hh, ll);
-            p.out_hi[pix * p.out_ld + col + j] = hh;
-            if (kPlanes == 2) p.out_lo[pix * p.out_ld + col + j] = ll;
-          }
-        }
-      }
     }
-    if (s.n_tiles > 1) epi_bar_sync();  // s_scale / s_shift are rewritten by the next tile
   }
 };
 // The split-precision backbone's epilogue and its single-plane counterpart (two types, so that the split kernels keep
