@@ -61,7 +61,8 @@ extern "C" {
  * 109: lb_transformer_forward_fp16 / lb_coarse_match_fp16 (single-pass fp16 transformers and coarse matching);
  * 110: lb_gemm_fp16 (test hook of the contraction core on single fp16 planes).
  * Entries added without a version step (a caller finds them by name: a build that lacks one does not export it):
- * lb_coarse_query / lb_fine_preprocess_centres (matching caller-given image0 points). */
+ * lb_coarse_query / lb_fine_preprocess_centres (matching caller-given image0 points);
+ * lb_coarse_match_guided (coarse matching restricted to a band around a homography or fundamental matrix). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -298,6 +299,28 @@ int lb_coarse_match_capped(const LbCoarseMatchArgs* args /*host*/, int max_per_p
  * >= 1 as lb_coarse_match_capped; negative values are an error.  Same workspace. */
 int lb_coarse_match_fp16(const LbCoarseMatchArgs* args /*host*/, int max_per_pair, void* ws, size_t ws_bytes,
                          void* stream);
+
+/* Guided coarse matching (found by name, see lb_version; DESIGN.md §18).  A separate structure, not new fields of LbCoarseMatchArgs:
+ * DESIGN.md §12. */
+#define LB_GUIDE_HOMOGRAPHY 0
+#define LB_GUIDE_FUNDAMENTAL 1
+typedef struct LbCoarseGuide {
+  int kind;            /* LB_GUIDE_* */
+  const float* model;  /* [n_pairs][9] f32, device: row-major 3x3 T per pair, in the coordinates of mkpts0_c / mkpts1_c
+                        * (source pixels when scale0 / scale1 are given); a pair whose T has a non-finite entry is
+                        * unguided */
+  float radius;        /* finite, > 0: pixels of image1's output coordinates */
+} LbCoarseGuide;
+/* lb_coarse_match / lb_coarse_match_capped (fp16 = 0) or lb_coarse_match_fp16 (fp16 = 1) with every score entry of an
+ * inadmissible cell pair left out of the normalisers (the reference's -1e9 fill) and given conf 0 before the
+ * threshold, border and mutual-nearest tests, in the dual-softmax and the Sinkhorn branch; conf_matrix is 0 there too.
+ * Cell pair (i, j) of pair b is admissible when p0 = mkpts0_c(i), p1 = mkpts1_c(j) satisfy, in fp32:
+ *   LB_GUIDE_FUNDAMENTAL  l = T (p0, 1):  |l . (p1, 1)| <= radius * sqrt(l0^2 + l1^2)  (l0 = l1 = 0: none)
+ *   LB_GUIDE_HOMOGRAPHY   q = T (p0, 1):  q2 != 0 and |q01 / q2 - p1| <= radius
+ * max_per_pair: 0 = no cap, >= 1 as lb_coarse_match_capped.  Errors: a NULL guide or model, an unknown kind, a radius
+ * that is not finite and positive.  Same workspace as lb_coarse_match. */
+int lb_coarse_match_guided(const LbCoarseMatchArgs* args /*host*/, const LbCoarseGuide* guide /*host*/,
+                           int max_per_pair, int fp16, void* ws, size_t ws_bytes, void* stream);
 
 /* Caller-given image0 points of every pair (found by name, see lb_version; LoFTR.match_points, DESIGN.md §17).  A separate structure, not
  * new fields of LbCoarseMatchArgs: DESIGN.md §12.  Outputs are per query, q = b*Q + k. */

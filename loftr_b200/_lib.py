@@ -84,6 +84,10 @@ class LbCoarseQueryArgs(C.Structure):
     ]
 
 
+class LbCoarseGuide(C.Structure):
+    _fields_ = [("kind", c_int), ("model", c_void_p), ("radius", c_float)]
+
+
 class LbFinePreprocessArgs(C.Structure):
     _fields_ = [
         ("feat_f0", c_void_p), ("feat_f1", c_void_p),
@@ -149,6 +153,8 @@ SIGNATURES = {
     "lb_coarse_match": (c_int, [C.POINTER(LbCoarseMatchArgs), c_void_p, c_size_t, c_void_p]),
     "lb_coarse_match_capped": (c_int, [C.POINTER(LbCoarseMatchArgs), c_int, c_void_p, c_size_t, c_void_p]),
     "lb_coarse_match_fp16": (c_int, [C.POINTER(LbCoarseMatchArgs), c_int, c_void_p, c_size_t, c_void_p]),
+    "lb_coarse_match_guided": (c_int, [C.POINTER(LbCoarseMatchArgs), C.POINTER(LbCoarseGuide), c_int, c_int, c_void_p,
+                                       c_size_t, c_void_p]),
     "lb_coarse_query": (c_int, [C.POINTER(LbCoarseMatchArgs), C.POINTER(LbCoarseQueryArgs), c_int, c_void_p, c_size_t,
                                 c_void_p]),
     "lb_fine_preprocess_workspace_bytes": (c_size_t, [c_long, c_int, c_int]),
@@ -192,9 +198,12 @@ GEMM_FP16_VERSION = 110
 # entries that came without a version step: `load()` binds each one the library exports, and `require_entries` stops
 # the paths that need one the library lacks
 POINTS_ENTRIES = ("lb_coarse_query", "lb_fine_preprocess_centres")   # LoFTR.match_points
-_OPTIONAL = set(POINTS_ENTRIES)
+GUIDE_ENTRIES = ("lb_coarse_match_guided",)   # data["guide"] / match_features(guide=...), DESIGN.md §18
+_OPTIONAL = set(POINTS_ENTRIES) | set(GUIDE_ENTRIES)
 GEOMETRY_HOMOGRAPHY = 0
 GEOMETRY_FUNDAMENTAL = 1
+GUIDE_HOMOGRAPHY = 0
+GUIDE_FUNDAMENTAL = 1
 _SINCE = {"lb_coarse_prep_indexed": FEATURE_BANK_VERSION, "lb_fine_preprocess_indexed": FEATURE_BANK_VERSION,
           "lb_coarse_match_capped": MATCH_CAP_VERSION, "lb_preprocess_images": PREPROCESS_VERSION,
           "lb_geometry_workspace_bytes": GEOMETRY_VERSION, "lb_estimate_geometry": GEOMETRY_VERSION,

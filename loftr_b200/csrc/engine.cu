@@ -1300,9 +1300,19 @@ size_t lb_coarse_match_workspace_bytes(int n_pairs, int L, int S) {
 // score passes, the Sinkhorn iterations and prefilter, the optional conf_matrix, and match_flag_kernel's flag / conf.
 // On return `w` holds them in the workspace and `sp` describes them.
 // kP: operand planes of the score products (Operands); every pass recomputes the same logits.
-template <int kP>
-static int coarse_rows(const LbCoarseMatchArgs* a, const DeviceScope& dev, void* ws, size_t ws_bytes, cudaStream_t st,
-                       CmWs& w, SelectParams& sp) {
+// kG: guided (DESIGN.md §18): every score pass and the conf_matrix take the guided epilogue, with `guide` beside its
+// arguments; the passes between them and match_flag_kernel are the same launches.
+template <bool kG, class Plain, class Guided>
+using GuideSel = std::conditional_t<kG, Guided, Plain>;
+template <class Epi>
+static typename Epi::Params epi_params(const typename Epi::Args& args, const GuideParams* guide) {
+  if constexpr (std::is_same_v<typename Epi::Params, typename Epi::Args>) return args;
+  else return typename Epi::Params{args, *guide};
+}
+
+template <int kP, bool kG>
+static int coarse_rows(const LbCoarseMatchArgs* a, const GuideParams* guide, const DeviceScope& dev, void* ws,
+                       size_t ws_bytes, cudaStream_t st, CmWs& w, SelectParams& sp) {
   const int n = a->n_pairs, L = a->L, S = a->S, C = a->C;
   if (L != a->h0c * a->w0c || S != a->h1c * a->w1c) return fail("L/S do not match the coarse grid sizes");
   if (C % kBlockK != 0) return fail("C=%d must be a multiple of %d", C, kBlockK);
@@ -1345,8 +1355,8 @@ static int coarse_rows(const LbCoarseMatchArgs* a, const DeviceScope& dev, void*
       ct = w.col_t;
       rt = w.row_t;
     }
-    using Epi = Operands<EpiScoreLse<BN, true, true>, kP>;
-    typename Epi::Params ep{scale, ct, rt, w.row_part, w.col_part};
+    using Epi = Operands<GuideSel<kG, EpiScoreLse<BN, true, true>, EpiScoreLseGuided<BN, true, true>>, kP>;
+    const auto ep = epi_params<Epi>({scale, ct, rt, w.row_part, w.col_part}, guide);
     LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, score, ep, dev.sms, st)));
     // row_t = -rowLSE, col_t = -colLSE (kNegBig on padded entries)              [coarse_matching.py:119]
     LB_TRY(launch(TAG_NONE, lse_merge_kernel, cdiv(nl, TB), TB, 0, st, w.row_part, n_chunks, nl, 0.f, nullptr, nullptr,
@@ -1373,8 +1383,8 @@ static int coarse_rows(const LbCoarseMatchArgs* a, const DeviceScope& dev, void*
     for (int it = 0; it < a->skh_iters; ++it) {
       // u_i = log_mu_i - LSE_j(Z_ij + v_j), j over S real columns + the dustbin column   [superglue.py:146]
       {
-        using Epi = Operands<EpiScoreLse<BN, true, false>, kP>;
-        typename Epi::Params ep{scale, w.col_t, nullptr, w.row_part, w.col_part};
+        using Epi = Operands<GuideSel<kG, EpiScoreLse<BN, true, false>, EpiScoreLseGuided<BN, true, false>>, kP>;
+        const auto ep = epi_params<Epi>({scale, w.col_t, nullptr, w.row_part, w.col_part}, guide);
         LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, score, ep, dev.sms, st)));
         LB_TRY(launch(TAG_NONE, lse_merge_kernel, cdiv(nl, TB), TB, 0, st, w.row_part, n_chunks, nl, norm, a->bin_score,
                       w.bin_v, L, a->mask0, w.row_u));
@@ -1384,8 +1394,8 @@ static int coarse_rows(const LbCoarseMatchArgs* a, const DeviceScope& dev, void*
       LB_TRY(launch(TAG_NONE, mask_term_kernel, cdiv(nl, TB), TB, 0, st, w.row_u, a->mask0, nullptr, nl, w.row_t));
       // v_j = log_nu_j - LSE_i(Z_ij + u_i), i over L real rows + the dustbin row            [superglue.py:147]
       {
-        using Epi = Operands<EpiScoreLse<BN, false, true>, kP>;
-        typename Epi::Params ep{scale, nullptr, w.row_t, w.row_part, w.col_part};
+        using Epi = Operands<GuideSel<kG, EpiScoreLse<BN, false, true>, EpiScoreLseGuided<BN, false, true>>, kP>;
+        const auto ep = epi_params<Epi>({scale, nullptr, w.row_t, w.row_part, w.col_part}, guide);
         LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_LSE, A, B, score, ep, dev.sms, st)));
         LB_TRY(launch(TAG_NONE, lse_merge_kernel, cdiv(ns, TB), TB, 0, st, w.col_part, m_tiles, ns, norm, a->bin_score,
                       w.bin_u, S, a->mask1, w.col_v));
@@ -1405,8 +1415,8 @@ static int coarse_rows(const LbCoarseMatchArgs* a, const DeviceScope& dev, void*
   const uint8_t* col_dead = nullptr;
   const int passes = (a->match_type == LB_MATCH_SINKHORN && a->skh_prefilter) ? 2 : 1;
   for (int pass = 0; pass < passes; ++pass) {
-    using Epi = Operands<EpiScoreArgmax<BN>, kP>;
-    typename Epi::Params ep{scale, alpha, w.col_t, w.row_t, w.row_apart, w.col_apart};
+    using Epi = Operands<GuideSel<kG, EpiScoreArgmax<BN>, EpiScoreArgmaxGuided<BN>>, kP>;
+    const auto ep = epi_params<Epi>({scale, alpha, w.col_t, w.row_t, w.row_apart, w.col_apart}, guide);
     LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_ARGMAX, A, B, score, ep, dev.sms, st)));
     LB_TRY(launch(TAG_NONE, argmax_merge_kernel, cdiv(nl, TB), TB, 0, st, w.row_apart, n_chunks, nl, w.row_key,
                   w.row_arg));
@@ -1426,9 +1436,9 @@ static int coarse_rows(const LbCoarseMatchArgs* a, const DeviceScope& dev, void*
   }
 
   if (a->conf_matrix) {   // opt-in materialisation of data['conf_matrix']         [coarse_matching.py:145]
-    using Epi = Operands<EpiConfStore<BN>, kP>;
+    using Epi = Operands<GuideSel<kG, EpiConfStore<BN>, EpiConfStoreGuided<BN>>, kP>;
     // row_t / col_t hold -LSE (dual-softmax) or the Sinkhorn potentials, with padded / prefiltered entries disabled
-    typename Epi::Params ep{scale, alpha, conf_bias, w.row_t, w.col_t, a->conf_matrix};
+    const auto ep = epi_params<Epi>({scale, alpha, conf_bias, w.row_t, w.col_t, a->conf_matrix}, guide);
     LB_TRY((launch_gemm<BN, Epi>(TAG_SCORE_ARGMAX, A, B, gemm_shape<BN>(n, L, S, C, /*b_batched=*/true), ep, dev.sms,
                                  st)));
   }
@@ -1448,8 +1458,10 @@ static int coarse_rows(const LbCoarseMatchArgs* a, const DeviceScope& dev, void*
 }
 
 // max_per_pair: 0 = every match; otherwise each pair keeps its max_per_pair most confident matches (match_cap_kernel).
+// guide: NULL, or the guide of lb_coarse_match_guided.
 template <int kP>
-static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, size_t ws_bytes, void* stream) {
+static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, const GuideParams* guide, void* ws,
+                        size_t ws_bytes, void* stream) {
   DeviceScope dev;
   LB_TRY(dev.bind(a->count));
   const int n = a->n_pairs, L = a->L, S = a->S;
@@ -1460,7 +1472,8 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
   }
   CmWs w;
   SelectParams sp;
-  LB_TRY(coarse_rows<kP>(a, dev, ws, ws_bytes, st, w, sp));
+  LB_TRY((guide ? coarse_rows<kP, true>(a, guide, dev, ws, ws_bytes, st, w, sp)
+                : coarse_rows<kP, false>(a, nullptr, dev, ws, ws_bytes, st, w, sp)));
   const long nl = static_cast<long>(n) * L;
   if (max_per_pair > 0) {
     LB_TRY(launch(TAG_MATCH_CAP, match_cap_kernel, n, kCapBlock, 0, st, w.flag, w.conf, L, max_per_pair));
@@ -1482,17 +1495,32 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, 
 extern "C" {
 
 int lb_coarse_match(const LbCoarseMatchArgs* a, void* ws, size_t ws_bytes, void* stream) {
-  return coarse_match<2>(a, 0, ws, ws_bytes, stream);
+  return coarse_match<2>(a, 0, nullptr, ws, ws_bytes, stream);
 }
 
 int lb_coarse_match_capped(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, size_t ws_bytes, void* stream) {
   if (max_per_pair < 1) return fail("lb_coarse_match_capped: max_per_pair must be at least 1 (got %d)", max_per_pair);
-  return coarse_match<2>(a, max_per_pair, ws, ws_bytes, stream);
+  return coarse_match<2>(a, max_per_pair, nullptr, ws, ws_bytes, stream);
 }
 
 int lb_coarse_match_fp16(const LbCoarseMatchArgs* a, int max_per_pair, void* ws, size_t ws_bytes, void* stream) {
   if (max_per_pair < 0) return fail("lb_coarse_match_fp16: max_per_pair must be 0 (no cap) or at least 1 (got %d)", max_per_pair);
-  return coarse_match<1>(a, max_per_pair, ws, ws_bytes, stream);
+  return coarse_match<1>(a, max_per_pair, nullptr, ws, ws_bytes, stream);
+}
+
+int lb_coarse_match_guided(const LbCoarseMatchArgs* a, const LbCoarseGuide* g, int max_per_pair, int fp16, void* ws,
+                           size_t ws_bytes, void* stream) {
+  if (!g || !g->model) return fail("lb_coarse_match_guided: the guide model is null");
+  if (g->kind != LB_GUIDE_HOMOGRAPHY && g->kind != LB_GUIDE_FUNDAMENTAL)
+    return fail("lb_coarse_match_guided: unknown guide kind %d", g->kind);
+  if (!std::isfinite(g->radius) || !(g->radius > 0.f))
+    return fail("lb_coarse_match_guided: the radius must be finite and positive (got %g)", g->radius);
+  if (max_per_pair < 0)
+    return fail("lb_coarse_match_guided: max_per_pair must be 0 (no cap) or at least 1 (got %d)", max_per_pair);
+  if (fp16 != 0 && fp16 != 1) return fail("lb_coarse_match_guided: fp16 must be 0 (split) or 1 (got %d)", fp16);
+  const GuideParams gp{g->kind, g->model, g->radius, a->img_scale, a->scale0, a->scale1, a->w0c, a->w1c};
+  return fp16 ? coarse_match<1>(a, max_per_pair, &gp, ws, ws_bytes, stream)
+              : coarse_match<2>(a, max_per_pair, &gp, ws, ws_bytes, stream);
 }
 
 int lb_coarse_query(const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, int operand_planes, void* ws,
@@ -1509,8 +1537,8 @@ int lb_coarse_query(const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, int 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CmWs w;
   SelectParams sp;
-  LB_TRY(operand_planes == 2 ? coarse_rows<2>(a, dev, ws, ws_bytes, st, w, sp)
-                             : coarse_rows<1>(a, dev, ws, ws_bytes, st, w, sp));
+  LB_TRY((operand_planes == 2 ? coarse_rows<2, false>(a, nullptr, dev, ws, ws_bytes, st, w, sp)
+                              : coarse_rows<1, false>(a, nullptr, dev, ws, ws_bytes, st, w, sp)));
   QueryParams qp;
   qp.n_pairs = a->n_pairs; qp.Q = q->Q; qp.L = a->L; qp.S = a->S;
   qp.h0c = a->h0c; qp.w0c = a->w0c; qp.w1c = a->w1c;

@@ -3,6 +3,9 @@
 // elementwise / row-wise work that the reference runs as separate eager kernels.
 #pragma once
 #include <cuda_fp16.h>
+
+#include <type_traits>
+
 #include "gemm_split.cuh"
 
 namespace lb {
@@ -861,6 +864,111 @@ __device__ __forceinline__ float f32_unordered(uint32_t u) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// Guided coarse matching (DESIGN.md §18): cell pair (i, j) of pair b is admissible when the coarse keypoints
+// p0 = mkpts0_c(i) and p1 = mkpts1_c(j) agree with the pair's 3x3 model T (output coordinates, row-major):
+//   fundamental  l = T (p0, 1);  |(l0*x1 + l1*y1) + l2| <= r * sqrt(l0*l0 + l1*l1);  l0 = l1 = 0 admits nothing
+//   homography   q = T (p0, 1);  q2 != 0 and (q0/q2 - x1)^2 + (q1/q2 - y1)^2 <= r*r
+// with T (p0, 1)_k = (T_k0*x0 + T_k1*y0) + T_k2.  Every operation is a separately rounded fp32 one (no FMA
+// contraction), so a float32 oracle evaluates the same predicate bit for bit.  A model with a non-finite entry admits
+// every cell pair.  Inadmissible entries take the kNegBig route of padded ones in every pass.
+constexpr int kGuideHomography = 0;    // LB_GUIDE_HOMOGRAPHY
+constexpr int kGuideFundamental = 1;   // LB_GUIDE_FUNDAMENTAL
+struct GuideParams {
+  int kind;
+  const float* model;    // [batches][9]
+  float radius;
+  float img_scale;       // coarse keypoints as mkpts0_c / mkpts1_c: cell corner * img_scale (* scale0 / scale1)
+  const float* scale0;   // optional [batches][2]
+  const float* scale1;
+  int w0c, w1c;
+};
+// An epilogue's launch arguments with the guide beside them (the guided instantiations' Params)
+template <class Args>
+struct WithGuide : Args {
+  GuideParams guide;
+};
+
+// coarse keypoint of `cell` on a grid `w` cells wide, in the expression of match_scatter_kernel
+__device__ __forceinline__ float2 guide_point(int cell, int w, float img_scale, const float* sc, int batch) {
+  float sx = img_scale, sy = img_scale;
+  if (sc) {
+    sx = __fmul_rn(img_scale, sc[2 * batch]);
+    sy = __fmul_rn(img_scale, sc[2 * batch + 1]);
+  }
+  return make_float2(__fmul_rn(static_cast<float>(cell % w), sx), __fmul_rn(static_cast<float>(cell / w), sy));
+}
+
+// Per-row part of the predicate.  fundamental: the line (a, b, c) and t = r * |(a, b)|; homography: the transferred
+// point (a, b) and t = r * r.  Column bits are (test & keep) | force.
+struct GuideRow {
+  float a, b, c, t;
+  uint32_t keep;    // 0: the row admits nothing
+  uint32_t force;   // ~0u: the row admits everything (unguided pair, or a row past the tile's end)
+};
+__device__ __forceinline__ GuideRow guide_row(const GuideParams& g, int batch, int row, bool row_ok) {
+  GuideRow gr{0.f, 0.f, 0.f, 0.f, 0u, ~0u};
+  if (!row_ok) return gr;
+  const float* T = g.model + 9L * batch;
+  float m[9];
+  bool finite = true;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) {
+    m[k] = __ldg(T + k);
+    finite = finite && isfinite(m[k]);
+  }
+  if (!finite) return gr;
+  const float2 p = guide_point(row, g.w0c, g.img_scale, g.scale0, batch);
+  float v[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+    v[k] = __fadd_rn(__fadd_rn(__fmul_rn(m[3 * k], p.x), __fmul_rn(m[3 * k + 1], p.y)), m[3 * k + 2]);
+  gr.force = 0u;
+  gr.keep = ~0u;
+  if (g.kind == kGuideFundamental) {
+    gr.a = v[0];
+    gr.b = v[1];
+    gr.c = v[2];
+    gr.t = __fmul_rn(g.radius, __fsqrt_rn(__fadd_rn(__fmul_rn(v[0], v[0]), __fmul_rn(v[1], v[1]))));
+    if (v[0] == 0.f && v[1] == 0.f) gr.keep = 0u;
+  } else {
+    if (v[2] == 0.f) {
+      gr.keep = 0u;
+    } else {
+      gr.a = __fdiv_rn(v[0], v[2]);
+      gr.b = __fdiv_rn(v[1], v[2]);
+    }
+    gr.t = __fmul_rn(g.radius, g.radius);
+  }
+  return gr;
+}
+// Admissibility of this row against 32 consecutive columns (p1: their keypoints, staged in shared memory): bit j
+__device__ __forceinline__ uint32_t guide_mask32(int kind, const GuideRow& gr, const float2* p1) {
+  uint32_t m = 0u;
+  if (kind == kGuideFundamental) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const float2 q = p1[j];
+      const float e = __fadd_rn(__fadd_rn(__fmul_rn(gr.a, q.x), __fmul_rn(gr.b, q.y)), gr.c);
+      m |= (fabsf(e) <= gr.t ? 1u : 0u) << j;
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const float2 q = p1[j];
+      const float dx = __fsub_rn(gr.a, q.x), dy = __fsub_rn(gr.b, q.y);
+      m |= (__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) <= gr.t ? 1u : 0u) << j;
+    }
+  }
+  return (m & gr.keep) | gr.force;
+}
+// x where column j of the mask is admissible, kNegBig elsewhere; the identity when unguided
+template <bool kGuided>
+__device__ __forceinline__ float guide_sel(uint32_t adm, int j, float x) {
+  if constexpr (kGuided) return ((adm >> j) & 1u) ? x : kNegBig;
+  return x;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Pass 1 of the fused coarse matching: z = acc * scale is one 128 x BLOCK_N tile of the similarity
 // matrix (reference coarse_matching.py:109-110 / 122).  Emits log-sum-exp partials
 //   rows:    (max, sum) over this work item's columns of  z[i,j] + colterm[j]
@@ -869,30 +977,36 @@ __device__ __forceinline__ float f32_unordered(uint32_t u) {
 // dual-softmax (coarse_matching.py:119); with the Sinkhorn potentials they are one half-iteration of
 // log_sinkhorn_iterations (third_party superglue.py:141-148).  Masked / out-of-range entries carry
 // the term kNegBig and therefore vanish from every sum (coarse_matching.py:115-118 fills -1e9).
-template <int BLOCK_N, bool kRows, bool kCols>
-struct EpiScoreLse {
-  struct Params {
+// kGuided: inadmissible entries (guide_mask32) vanish the same way; EpiScoreLse / EpiScoreLseGuided below.
+template <int BLOCK_N, bool kRows, bool kCols, bool kGuided>
+struct EpiScoreLseImpl {
+  struct Args {
     float scale;
     const float* colterm;   // optional [batches*N]; nullptr -> 0
     const float* rowterm;   // optional [batches*M]
     float2* row_part;       // [n_chunks][batches*M]
     float2* col_part;       // [m_tiles][batches*N]
   };
+  using Params = std::conditional_t<kGuided, WithGuide<Args>, Args>;
   // colterm staging + per-warp-row-quarter column partials + per-warp column-max broadcast + row merge
-  static constexpr int kSmemBytes = BLOCK_N * 4 + 4 * BLOCK_N * 8 + 8 * 32 * 4 + 128 * 8;
+  // (+ the tile's image1 keypoints when guided)
+  static constexpr int kGuideOffset = BLOCK_N * 4 + 4 * BLOCK_N * 8 + 8 * 32 * 4 + 128 * 8;
+  static constexpr int kSmemBytes = kGuideOffset + (kGuided ? BLOCK_N * 8 : 0);
   const Params& p;
   const GemmShape& s;
   float* s_ct;       // [BLOCK_N]
   float2* s_cpart;   // [4][BLOCK_N]
   float* s_cmax;     // [8][32]
   float2* s_rmerge;  // [128]
+  float2* s_p1;      // [BLOCK_N] guided only
   float row_m, row_l;
 
-  __device__ EpiScoreLse(const Params& p_, uint8_t* smem, const GemmShape& s_) : p(p_), s(s_) {
+  __device__ EpiScoreLseImpl(const Params& p_, uint8_t* smem, const GemmShape& s_) : p(p_), s(s_) {
     s_ct = reinterpret_cast<float*>(smem);
     s_cpart = reinterpret_cast<float2*>(smem + BLOCK_N * 4);
     s_cmax = reinterpret_cast<float*>(smem + BLOCK_N * 4 + 4 * BLOCK_N * 8);
     s_rmerge = reinterpret_cast<float2*>(smem + BLOCK_N * 4 + 4 * BLOCK_N * 8 + 8 * 32 * 4);
+    s_p1 = reinterpret_cast<float2*>(smem + kGuideOffset);
   }
   __device__ void prefetch(int, int, int) {}
   __device__ void item_begin(int, int, int) {
@@ -930,9 +1044,12 @@ struct EpiScoreLse {
       float ct = kNegBig;
       if (col < s.N) ct = p.colterm ? p.colterm[static_cast<long>(batch) * s.N + col] : 0.f;
       s_ct[j] = ct;
+      if constexpr (kGuided) s_p1[j] = guide_point(col, p.guide.w1c, p.guide.img_scale, p.guide.scale1, batch);
     }
     float rt = kNegBig;
     if (r < s.M) rt = p.rowterm ? p.rowterm[static_cast<long>(batch) * s.M + r] : 0.f;
+    GuideRow gr{};
+    if constexpr (kGuided) gr = guide_row(p.guide, batch, r, r < s.M);
     epi_bar_sync();
 
     const int c_begin = epi_half() * (BLOCK_N / 64);
@@ -940,6 +1057,7 @@ struct EpiScoreLse {
     // e = exp(z - g) with g the maximum of the warp's 32 x 32 block; a (g, sum) pair is a valid partial for both
     // directions.  If any row or column of the block sits more than ~69 nats below g (its sum would lose
     // significant terms to fp32 underflow) the whole block falls back to the per-row / per-column references.
+    // Guided, only a wholly admissible block takes it.
     const bool shared_ref = kRows && kCols && p.colterm == nullptr && p.rowterm == nullptr;
 #pragma unroll 1
     for (int c = c_begin; c < c_begin + BLOCK_N / 64; ++c) {
@@ -948,8 +1066,11 @@ struct EpiScoreLse {
       load_acc32(acc_row, c * 32, z);
 #pragma unroll
       for (int j = 0; j < 32; ++j) z[j] *= p.scale;
+      uint32_t adm = ~0u;
+      if constexpr (kGuided) adm = guide_mask32(p.guide.kind, gr, s_p1 + c * 32);
 
-      if (kRows && kCols && shared_ref && n0 + c * 32 + 32 <= s.N) {   // warp-uniform condition
+      if (kRows && kCols && shared_ref && n0 + c * 32 + 32 <= s.N &&
+          (!kGuided || __all_sync(0xffffffffu, adm == ~0u))) {   // warp-uniform condition
         const bool row_valid = r < s.M;
         float cm = kNegBig;
 #pragma unroll
@@ -980,11 +1101,11 @@ struct EpiScoreLse {
       if (kRows) {
         float cm = kNegBig;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) cm = fmaxf(cm, z[j] + s_ct[c * 32 + j]);
+        for (int j = 0; j < 32; ++j) cm = fmaxf(cm, guide_sel<kGuided>(adm, j, z[j] + s_ct[c * 32 + j]));
         const float m_new = fmaxf(row_m, cm);
         float acc = 0.f;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) acc += exp_fast(z[j] + s_ct[c * 32 + j] - m_new);
+        for (int j = 0; j < 32; ++j) acc += exp_fast(guide_sel<kGuided>(adm, j, z[j] + s_ct[c * 32 + j]) - m_new);
         row_l = row_l * exp_fast(row_m - m_new) + acc;
         row_m = m_new;
       }
@@ -992,7 +1113,7 @@ struct EpiScoreLse {
         float v[32];
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
-          z[j] += rt;
+          z[j] = guide_sel<kGuided>(adm, j, z[j] + rt);
           v[j] = z[j];
         }
         const float cmax = warp_transpose_reduce(v, OpMaxF());  // lane j: max of column c*32+j
@@ -1028,26 +1149,38 @@ struct EpiScoreLse {
     epi_bar_sync();  // s_ct / s_cpart are reused by the next tile
   }
 };
+// Two types, so that the unguided kernels keep their instantiation names
+template <int BLOCK_N, bool kRows, bool kCols>
+struct EpiScoreLse : EpiScoreLseImpl<BLOCK_N, kRows, kCols, false> {
+  using EpiScoreLseImpl<BLOCK_N, kRows, kCols, false>::EpiScoreLseImpl;
+};
+template <int BLOCK_N, bool kRows, bool kCols>
+struct EpiScoreLseGuided : EpiScoreLseImpl<BLOCK_N, kRows, kCols, true> {
+  using EpiScoreLseImpl<BLOCK_N, kRows, kCols, true>::EpiScoreLseImpl;
+};
 
 // ------------------------------------------------------------------------------------------------
 // Optional materialisation of the confidence matrix (reference `data['conf_matrix']`, coarse_matching.py:145;
 // its only consumer is the training loss, so the engine writes it on request only):
 //   conf[i,j] = exp(alpha*z[i,j] + rowterm[i] + colterm[j] + bias), 0 where a term is disabled (padded /
-//   prefiltered rows and columns).  HBM-bound: 4*L*S bytes per pair.
-template <int BLOCK_N>
-struct EpiConfStore {
-  struct Params {
+//   prefiltered rows and columns).  HBM-bound: 4*L*S bytes per pair.  kGuided: 0 outside the guide's band as well.
+template <int BLOCK_N, bool kGuided>
+struct EpiConfStoreImpl {
+  struct Args {
     float scale, alpha, bias;
     const float* rowterm;  // [batches*M]
     const float* colterm;  // [batches*N]
     float* out;            // [batches, M, N]
   };
-  static constexpr int kSmemBytes = BLOCK_N * 4;
+  using Params = std::conditional_t<kGuided, WithGuide<Args>, Args>;
+  static constexpr int kSmemBytes = BLOCK_N * 4 + (kGuided ? BLOCK_N * 8 : 0);   // colterm (+ image1 keypoints)
   const Params& p;
   const GemmShape& s;
   float* s_ct;
-  __device__ EpiConfStore(const Params& p_, uint8_t* smem, const GemmShape& s_) : p(p_), s(s_) {
+  float2* s_p1;   // guided only
+  __device__ EpiConfStoreImpl(const Params& p_, uint8_t* smem, const GemmShape& s_) : p(p_), s(s_) {
     s_ct = reinterpret_cast<float*>(smem);
+    s_p1 = reinterpret_cast<float2*>(smem + BLOCK_N * 4);
   }
   __device__ void item_begin(int, int, int) {}
   __device__ void item_end(int, int, int) {}
@@ -1057,11 +1190,14 @@ struct EpiConfStore {
     for (int j = t; j < BLOCK_N; j += kEpiThreads) {
       const int col = n0 + j;
       s_ct[j] = (col < s.N) ? p.colterm[static_cast<long>(batch) * s.N + col] : kNegBig;
+      if constexpr (kGuided) s_p1[j] = guide_point(col, p.guide.w1c, p.guide.img_scale, p.guide.scale1, batch);
     }
     const int r = m0 + epi_row();
     const bool row_ok = r < s.M;
     const float rt = row_ok ? p.rowterm[static_cast<long>(batch) * s.M + r] : kNegBig;
     const float sa = p.scale * p.alpha;
+    GuideRow gr{};
+    if constexpr (kGuided) gr = guide_row(p.guide, batch, r, row_ok);
     epi_bar_sync();
     float* orow = p.out + (static_cast<long>(batch) * s.M + r) * s.N;
     const int c_begin = epi_half() * (BLOCK_N / 64);
@@ -1071,10 +1207,12 @@ struct EpiConfStore {
       if (col >= s.N) break;
       float z[32];
       load_acc32(acc_row, c * 32, z);
+      uint32_t adm = ~0u;
+      if constexpr (kGuided) adm = guide_mask32(p.guide.kind, gr, s_p1 + c * 32);
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const float ct = s_ct[c * 32 + j];
-        z[j] = (rt > -1.0e29f && ct > -1.0e29f) ? expf(z[j] * sa + rt + ct + p.bias) : 0.f;
+        z[j] = (rt > -1.0e29f && ct > -1.0e29f && ((adm >> j) & 1u)) ? expf(z[j] * sa + rt + ct + p.bias) : 0.f;
       }
       if (row_ok) {
         if (col + 32 <= s.N && (s.N & 3) == 0) {
@@ -1089,6 +1227,14 @@ struct EpiConfStore {
     epi_bar_sync();
   }
 };
+template <int BLOCK_N>
+struct EpiConfStore : EpiConfStoreImpl<BLOCK_N, false> {
+  using EpiConfStoreImpl<BLOCK_N, false>::EpiConfStoreImpl;
+};
+template <int BLOCK_N>
+struct EpiConfStoreGuided : EpiConfStoreImpl<BLOCK_N, true> {
+  using EpiConfStoreImpl<BLOCK_N, true>::EpiConfStoreImpl;
+};
 
 // ------------------------------------------------------------------------------------------------
 // Pass 2: recompute the tile and take arg-maxima of the confidence along both directions.
@@ -1097,13 +1243,15 @@ struct EpiConfStore {
 // dual-softmax: alpha=2, colterm=-colLSE, rowterm=-rowLSE (log conf = 2z - rowLSE_i - colLSE_j,
 // monotone in the key along each direction); Sinkhorn: alpha=1, terms = potentials v, u.
 // Replaces conf.max(dim=2) / conf.max(dim=1) of the mutual-nearest test (coarse_matching.py:187-189).
+// kGuided: inadmissible entries get the key kNegBig in both directions, below every admissible unmasked key, so a row
+// (column) without an admissible entry keeps the key kNegBig, which match_flag_kernel and ot_dead_kernel reject.
 struct ArgPart {
   float key;
   int idx;
 };
-template <int BLOCK_N>
-struct EpiScoreArgmax {
-  struct Params {
+template <int BLOCK_N, bool kGuided>
+struct EpiScoreArgmaxImpl {
+  struct Args {
     float scale;
     float alpha;
     const float* colterm;  // [batches*N] (kNegBig disables a column)
@@ -1111,19 +1259,23 @@ struct EpiScoreArgmax {
     ArgPart* row_part;     // [n_chunks][batches*M]
     ArgPart* col_part;     // [m_tiles][batches*N]
   };
-  static constexpr int kSmemBytes = BLOCK_N * 4 + 4 * BLOCK_N * 8 + 128 * 8;
+  using Params = std::conditional_t<kGuided, WithGuide<Args>, Args>;
+  static constexpr int kGuideOffset = BLOCK_N * 4 + 4 * BLOCK_N * 8 + 128 * 8;
+  static constexpr int kSmemBytes = kGuideOffset + (kGuided ? BLOCK_N * 8 : 0);
   const Params& p;
   const GemmShape& s;
   float* s_ct;
   unsigned long long* s_cpart;  // [4][BLOCK_N]
   ArgPart* s_rmerge;            // [128]
+  float2* s_p1;                 // [BLOCK_N] guided only
   float best_key;
   int best_j;
 
-  __device__ EpiScoreArgmax(const Params& p_, uint8_t* smem, const GemmShape& s_) : p(p_), s(s_) {
+  __device__ EpiScoreArgmaxImpl(const Params& p_, uint8_t* smem, const GemmShape& s_) : p(p_), s(s_) {
     s_ct = reinterpret_cast<float*>(smem);
     s_cpart = reinterpret_cast<unsigned long long*>(smem + BLOCK_N * 4);
     s_rmerge = reinterpret_cast<ArgPart*>(smem + BLOCK_N * 4 + 4 * BLOCK_N * 8);
+    s_p1 = reinterpret_cast<float2*>(smem + kGuideOffset);
   }
   __device__ void prefetch(int, int, int) {}
   __device__ void item_begin(int, int, int) {
@@ -1158,9 +1310,12 @@ struct EpiScoreArgmax {
     for (int j = t; j < BLOCK_N; j += kEpiThreads) {
       const int col = n0 + j;
       s_ct[j] = (col < s.N) ? p.colterm[static_cast<long>(batch) * s.N + col] : kNegBig;
+      if constexpr (kGuided) s_p1[j] = guide_point(col, p.guide.w1c, p.guide.img_scale, p.guide.scale1, batch);
     }
     const float rt = (r < s.M) ? p.rowterm[static_cast<long>(batch) * s.M + r] : kNegBig;
     const float sa = p.scale * p.alpha;
+    GuideRow gr{};
+    if constexpr (kGuided) gr = guide_row(p.guide, batch, r, r < s.M);
     epi_bar_sync();
 
     const int c_begin = epi_half() * (BLOCK_N / 64);
@@ -1171,10 +1326,12 @@ struct EpiScoreArgmax {
       load_acc32(acc_row, c * 32, z);
 #pragma unroll
       for (int j = 0; j < 32; ++j) z[j] *= sa;
+      uint32_t adm = ~0u;
+      if constexpr (kGuided) adm = guide_mask32(p.guide.kind, gr, s_p1 + c * 32);
       // row direction: thread-local, strict '>' keeps the first (smallest j) maximum
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
-        const float key = z[j] + s_ct[c * 32 + j];
+        const float key = guide_sel<kGuided>(adm, j, z[j] + s_ct[c * 32 + j]);
         if (key > best_key) {
           best_key = key;
           best_j = n0 + c * 32 + j;
@@ -1185,7 +1342,7 @@ struct EpiScoreArgmax {
       const unsigned long long tag = 0xFFFFFFFFull - static_cast<unsigned long long>(static_cast<uint32_t>(r));
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
-        v[j] = (static_cast<unsigned long long>(f32_ordered(z[j] + rt)) << 32) | tag;
+        v[j] = (static_cast<unsigned long long>(f32_ordered(guide_sel<kGuided>(adm, j, z[j] + rt))) << 32) | tag;
       }
       const unsigned long long best = warp_transpose_reduce(v, OpMaxU64());
       s_cpart[q * BLOCK_N + c * 32 + lane] = best;
@@ -1208,6 +1365,14 @@ struct EpiScoreArgmax {
     }
     epi_bar_sync();
   }
+};
+template <int BLOCK_N>
+struct EpiScoreArgmax : EpiScoreArgmaxImpl<BLOCK_N, false> {
+  using EpiScoreArgmaxImpl<BLOCK_N, false>::EpiScoreArgmaxImpl;
+};
+template <int BLOCK_N>
+struct EpiScoreArgmaxGuided : EpiScoreArgmaxImpl<BLOCK_N, true> {
+  using EpiScoreArgmaxImpl<BLOCK_N, true>::EpiScoreArgmaxImpl;
 };
 
 // ------------------------------------------------------------------------------------------------

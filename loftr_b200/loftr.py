@@ -46,6 +46,39 @@ def _check_match_precision(precision, who):
     raise ValueError(f"{who} must be one of {MATCH_PRECISIONS} (got {precision!r})")
 
 
+GUIDE_KINDS = {"homography": _lib.GUIDE_HOMOGRAPHY, "fundamental": _lib.GUIDE_FUNDAMENTAL}
+
+
+def check_guide(guide, n, device, thr, who):
+    """Validates a guided-matching guide (DESIGN.md §18) for `n` pairs whose features live on `device`, with the
+    coarse threshold `thr`, before any launch and without a host sync; `who` names the caller in the messages.
+    guide: {"kind": "fundamental" | "homography", "model": float32 CUDA [n, 3, 3], "radius": finite float > 0}
+    -> (LB_GUIDE_* kind code, model, radius)."""
+    if not isinstance(guide, dict):
+        raise TypeError(f"{who}: guide must be a dict with the keys kind, model and radius (got {type(guide).__name__})")
+    if set(guide) != {"kind", "model", "radius"}:
+        raise ValueError(f"{who}: guide must have exactly the keys kind, model and radius (got {sorted(map(str, guide))})")
+    kind, model, radius = guide["kind"], guide["model"], guide["radius"]
+    if not isinstance(kind, str) or kind not in GUIDE_KINDS:
+        raise ValueError(f"{who}: guide['kind'] must be one of {tuple(GUIDE_KINDS)} (got {kind!r})")
+    if not torch.is_tensor(model) or model.dtype != torch.float32:
+        raise TypeError(f"{who}: guide['model'] must be a float32 tensor (got "
+                        f"{model.dtype if torch.is_tensor(model) else type(model).__name__})")
+    if tuple(model.shape) != (n, 3, 3):
+        raise ValueError(f"{who}: guide['model'] must be [N, 3, 3] with N = {n} pairs (got {tuple(model.shape)})")
+    if model.device != torch.device(device):
+        raise ValueError(f"{who}: guide['model'] is on {model.device}, the features on {device}")
+    if isinstance(radius, bool) or not isinstance(radius, numbers.Real):
+        raise TypeError(f"{who}: guide['radius'] must be a real number (got {type(radius).__name__})")
+    if not (math.isfinite(radius) and radius > 0):
+        raise ValueError(f"{who}: guide['radius'] must be finite and positive (got {radius!r})")
+    if thr < 0:
+        raise ValueError(f"{who}: a guide needs match_coarse.thr >= 0 (got {thr}): with thr < 0 the reference's "
+                         "mconf != 0 filter would bring back the entries the guide sets to 0")
+    _lib.require_entries(_lib.GUIDE_ENTRIES, f"{who}: guided matching")
+    return GUIDE_KINDS[kind], model.contiguous(), float(radius)
+
+
 def _stream(ref=None):
     """cudaStream_t of torch's current stream ON THE DEVICE THAT OWNS `ref` (a tensor or torch.device); the library
     binds itself to the device of the buffers it is given, so the stream handle must belong to that device too."""
@@ -461,6 +494,7 @@ class CoarseMatching(nn.Module):
 
     def run(self, hi, lo, ld, n, L, S, c, data, mask_u8_0=None, mask_u8_1=None, static=False, capacity=None):
         """Planes of feat_c0 (rows [0, n*L)) / feat_c1 (rows [n*L, ...)) -> coarse match keys in `data`.
+        data["guide"] (optional, `check_guide`): guided matching through lb_coarse_match_guided (DESIGN.md §18).
         Eager (static=False): the lists are trimmed to the match count, read with one host sync.
         Static: no host sync; the match keys are buffers of `capacity` entries (default_capacity when None; entries at
         or past min(count, capacity) unspecified) and data["num_matches"] is the int32 device count [1].  Static needs
@@ -480,7 +514,7 @@ class CoarseMatching(nn.Module):
         mk0 = torch.empty(cap, 2, dtype=torch.float32, device=dev)
         mk1 = torch.empty(cap, 2, dtype=torch.float32, device=dev)
         count = torch.zeros(1, dtype=torch.int32, device=dev)
-        a, keep = self._args(hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1)
+        a, keep, guide = self._args(hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1)
         a.capacity = cap
         a.b_ids, a.i_ids, a.j_ids = b_ids.data_ptr(), i_ids.data_ptr(), j_ids.data_ptr()
         a.mconf, a.mkpts0_c, a.mkpts1_c, a.count = mconf.data_ptr(), mk0.data_ptr(), mk1.data_ptr(), count.data_ptr()
@@ -490,7 +524,10 @@ class CoarseMatching(nn.Module):
             a.conf_matrix = conf.data_ptr()
         nbytes = lib.lb_coarse_match_workspace_bytes(n, L, S)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        if self._precision == "fp16":   # 0: no cap
+        if guide is not None:   # 0: no cap
+            _lib.check(lib.lb_coarse_match_guided(C.byref(a), C.byref(guide), 0 if k is None else min(k, L),
+                                                  int(self._precision == "fp16"), ws.data_ptr(), nbytes, _stream(hi)))
+        elif self._precision == "fp16":   # 0: no cap
             _lib.check(lib.lb_coarse_match_fp16(C.byref(a), 0 if k is None else min(k, L), ws.data_ptr(), nbytes,
                                                 _stream(hi)))
         elif k is None:
@@ -519,7 +556,8 @@ class CoarseMatching(nn.Module):
         return None
 
     def _args(self, hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1):
-        """LbCoarseMatchArgs of the coarse stage without its match-list outputs -> (args, tensors it points into)."""
+        """LbCoarseMatchArgs of the coarse stage without its match-list outputs -> (args, tensors it points into,
+        LbCoarseGuide of data["guide"] or None; None as well when there is no pair to match)."""
         dev = hi.device
         a = _lib.LbCoarseMatchArgs()
         esz = hi.element_size()
@@ -542,7 +580,12 @@ class CoarseMatching(nn.Module):
             s1 = data["scale1"].to(dev, torch.float32).contiguous()
             keep += [s0, s1]
             a.scale0, a.scale1 = s0.data_ptr(), s1.data_ptr()
-        return a, keep
+        guide = None
+        if data.get("guide") is not None and n > 0:
+            kind, model, radius = check_guide(data["guide"], n, dev, self.thr, "CoarseMatching")
+            keep.append(model)
+            guide = _lib.LbCoarseGuide(kind, model.data_ptr(), radius)
+        return a, keep, guide
 
     def query(self, hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1, points0, valid0=None):
         """The coarse stage for caller-given image0 points (LoFTR.match_points, DESIGN.md §17): planes as `run`,
@@ -566,7 +609,7 @@ class CoarseMatching(nn.Module):
                "qpts1_c": torch.empty(n, q, 2, dtype=torch.float32, device=dev),
                "centres": torch.empty(2, nq, 2, dtype=torch.int32, device=dev),
                "win_ids": torch.empty(3, nq, dtype=torch.int64, device=dev)}
-        a, keep = self._args(hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1)
+        a, keep, _ = self._args(hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1)
         qa = _lib.LbCoarseQueryArgs()
         points0 = points0.contiguous()
         keep.append(points0)
@@ -786,9 +829,16 @@ class LoFTR(nn.Module):
     def forward(self, data):
         """Updates `data` in place with the reference's keys; returns None.
         Inputs: image0/image1 [N, 1, H, W] float32 (H, W divisible by 8), optional mask0/mask1 [N, H/8, W/8],
-        optional scale0/scale1 [N, 2]."""
+        optional scale0/scale1 [N, 2], optional guide (guided coarse matching, DESIGN.md §18): {"kind":
+        "fundamental" | "homography", "model": float32 [N, 3, 3] on image0's device, one matrix per pair in the
+        coordinates of mkpts0_f / mkpts1_f, "radius": pixels of image1, finite and > 0}.  Only cell pairs whose coarse
+        keypoints agree with the pair's model within the radius can match, and only they enter the softmax (Sinkhorn)
+        normalisers; a pair whose model has a non-finite entry is matched unguided.  Needs match_coarse.thr >= 0."""
         _require_eval(self)
         _require_cuda(data["image0"], "image0")
+        if data.get("guide") is not None:
+            check_guide(data["guide"], data["image0"].shape[0], data["image0"].device, self.coarse_matching.thr,
+                        "forward")
         self._match_pairs(data, *self._backbone_pairs(data))
 
     @torch.no_grad()
@@ -812,7 +862,8 @@ class LoFTR(nn.Module):
         return ImageFeatures(feat_c, feat_f, masks, images.shape[2:], feat_c.shape[2:], feat_f.shape[2:], key)
 
     @torch.no_grad()
-    def match_features(self, feats0, idx0, feats1, idx1, scale0=None, scale1=None, data=None, estimate=None):
+    def match_features(self, feats0, idx0, feats1, idx1, scale0=None, scale1=None, data=None, estimate=None,
+                       guide=None):
         """Matches pair b = (image idx0[b] of feats0, image idx1[b] of feats1) for every b of the pair list, from banks
         made by `extract_features` (feats1 may be feats0).  Writes into `data` (a new dict when None) and returns it:
         the keys, dtypes and values `forward` writes for the batch image0 = images idx0 of feats0, image1 = images
@@ -827,7 +878,11 @@ class LoFTR(nn.Module):
         a dict of `loftr_b200.estimate_geometry` options ("model", "threshold", "iterations", "seed").  The estimator
         then fits that model to each pair's fine matches (mkpts0_f / mkpts1_f) on the GPU and adds
         data["geom_model"] [B, 3, 3], data["geom_inliers"] [M] bool (one flag per match of the list) and
-        data["geom_num_inliers"] [B] int32; pair b's RNG key is b."""
+        data["geom_num_inliers"] [B] int32; pair b's RNG key is b.
+
+        guide: None, or forward's data["guide"] with "model" [B, 3, 3] in pair-list order: guided coarse matching
+        (DESIGN.md §18).  It combines with `estimate`, which then fits the guided matches; a geom_model of an earlier
+        call guides the next one directly (a failed pair's NaN model leaves that pair unguided)."""
         _require_eval(self)
         _lib.require(_lib.FEATURE_BANK_VERSION, "match_features")
         geom = None
@@ -855,7 +910,10 @@ class LoFTR(nn.Module):
         if (scale0 is None) != (scale1 is None):
             raise ValueError("match_features: give scale0 and scale1 together")
         bs = idx0.numel()
-        work = {}   # forward's inputs for this pair list (masks, scales), then every key forward writes
+        work = {}   # forward's inputs for this pair list (masks, scales, guide), then every key forward writes
+        if guide is not None:
+            check_guide(guide, bs, dev, self.coarse_matching.thr, "match_features")
+            work["guide"] = guide
         if feats0.mask is not None:
             work["mask0"], work["mask1"] = feats0.mask[idx0.long()], feats1.mask[idx1.long()]
         if scale0 is not None:
@@ -872,7 +930,7 @@ class LoFTR(nn.Module):
                                                     self.coarse_matching.max_matches_per_pair)
             geometry.estimate_on_matches(work, bs, bound, geom)
         out = {} if data is None else data
-        out.update({k: v for k, v in work.items() if k not in ("mask0", "mask1", "scale0", "scale1")})
+        out.update({k: v for k, v in work.items() if k not in ("mask0", "mask1", "scale0", "scale1", "guide")})
         return out
 
     @staticmethod
@@ -921,7 +979,10 @@ class LoFTR(nn.Module):
         capacity trades that memory for the risk of overflow, which stays visible in num_matches.  A capacity of n*k
         never overflows.
 
-        Configurations whose output list depends on the data (match_coarse.thr < 0) raise ValueError."""
+        Configurations whose output list depends on the data (match_coarse.thr < 0) raise ValueError.
+
+        data["guide"] (as in `forward`): its model must be on the device as well.  A captured graph bakes in the kind
+        and the radius and reads the model from the same tensor at every replay."""
         _require_static(self, capacity, "forward_static")
         dev = None
         for k in ("image0", "image1", "mask0", "mask1", "scale0", "scale1"):
@@ -935,6 +996,9 @@ class LoFTR(nn.Module):
                 dev = t.device
             elif t.device != dev:
                 raise ValueError(f"forward_static: `{k}` is on {t.device}, image0 on {dev}")
+        if data.get("guide") is not None:
+            check_guide(data["guide"], data["image0"].shape[0], data["image0"].device, self.coarse_matching.thr,
+                        "forward_static")
         self._match_pairs(data, *self._backbone_pairs(data), static=True, capacity=capacity)
 
     @torch.no_grad()
@@ -954,8 +1018,12 @@ class LoFTR(nn.Module):
 
         Each query's outputs depend only on its own point, pair and images.  A query at a forward match's mkpts0_c gets
         that match's j_ids, mconf, mkpts1_c, mkpts1_f and expec_f bit for bit.  Shapes are fixed by [N, Q] and there is
-        no host synchronisation, so the call can be captured by `torch.cuda.graph` after one eager call."""
+        no host synchronisation, so the call can be captured by `torch.cuda.graph` after one eager call.
+        A guide (data["guide"]) is not supported here and raises ValueError."""
         _require_eval(self)
+        if data.get("guide") is not None:
+            raise ValueError("match_points: data['guide'] is not supported (guided matching is available in forward, "
+                             "forward_static and match_features)")
         _lib.require_entries(_lib.POINTS_ENTRIES, "match_points")
         _check_points(data, points0, valid0)
         n, q = points0.shape[:2]
@@ -1230,6 +1298,9 @@ class CapturedMatcher:
                                "invalidate_packed() or a parameter update); call recapture()")
 
     def __call__(self, data):
+        if data.get("guide") is not None:
+            raise ValueError("CapturedMatcher: data['guide'] is not supported (capture LoFTR.forward_static with a "
+                             "guide instead)")
         if self.graph is None:
             raise RuntimeError("loftr_b200.CapturedMatcher: no captured graph; call recapture()")
         self._check_weights()
