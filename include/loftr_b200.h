@@ -62,7 +62,8 @@ extern "C" {
  * 110: lb_gemm_fp16 (test hook of the contraction core on single fp16 planes).
  * Entries added without a version step (a caller finds them by name: a build that lacks one does not export it):
  * lb_coarse_query / lb_fine_preprocess_centres (matching caller-given image0 points);
- * lb_coarse_match_guided (coarse matching restricted to a band around a homography or fundamental matrix). */
+ * lb_coarse_match_guided (coarse matching restricted to a band around a homography or fundamental matrix);
+ * lb_rectify_images / lb_rectify_points (image1 warped into image0's frame through a homography, matches mapped back). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -121,6 +122,29 @@ typedef struct LbImageDesc {
  * guarantees the ranges above.  One launch (timing tag "preprocess"), no workspace, no atomics. */
 int lb_preprocess_images(const LbImageDesc* descs, int n_images, float* out, int H, int W, uint8_t* mask,
                          void* stream);
+
+/* ---- rectified matching (found by name, see lb_version; DESIGN.md §19).  models: [n][9] f32, device, row-major
+ * homography per pair, x1 ~ H x0 in source pixels: network pixel (x, y) of image k sits at (x * sx, y * sy) with
+ * (sx, sy) = scale_k[b] ([n, 2] f32, device), or (1, 1) when scale_k is NULL.  Both entries apply H in fp64 as follows:
+ * a model with a non-finite entry is replaced by the identity; otherwise H is multiplied by the sign of its w at the
+ * centre ((W0 - 1) / 2 * sx0, (H0 - 1) / 2 * sy0) of image0's canvas (+1 when that w is 0).
+ *
+ * lb_rectify_images: out [n, 1, H, W] f32 (16-byte aligned; H, W positive multiples of 8 = image0's canvas), pixel
+ * (x, y) of pair b = image1[b] ([n, 1, H1, W1] f32, contiguous) sampled at (H (x sx0, y sy0, 1))_xy / w / (sx1, sy1):
+ * bilinear, pixel centres at integer coordinates, taps outside the image read as 0, i.e. grid_sample(mode="bilinear",
+ * padding_mode="zeros", align_corners=True); 0 where w <= 0.  Coordinates in fp64, interpolation in fp32.  n at most
+ * 65535.  One launch (timing tag "rectify"), no workspace. */
+int lb_rectify_images(const float* image1, int n, int H1, int W1, const float* models, const float* scale0,
+                      const float* scale1, float* out, int H, int W, void* stream);
+/* lb_rectify_points: pts [m, 2] f32 (x, y) in source pixels of the rectified frame (image0's); pair_ids [m] int64.
+ * out [m, 2] = (H p)_xy / w in fp64, rounded once to fp32: source pixels of image1; NaN where w <= 0, p is not finite
+ * or the pair id is outside [0, n_pairs).  inside (NULL, or [m] bytes): 1 when out / (sx1, sy1) lies in
+ * [0, W1 - 1] x [0, H1 - 1] and, with mask1 ([n_pairs, H1/8, w1c] bytes, w1c = W1/8), its cell (floor(v/8), floor(u/8))
+ * is non-zero.  H0 x W0: image0's canvas (the sign rule above).  M_live: NULL, or a device int: only points
+ * i < min(*M_live, m) are written.  One launch, no workspace. */
+int lb_rectify_points(const float* pts, const long long* pair_ids, long m, const int* M_live, const float* models,
+                      int n_pairs, const float* scale0, const float* scale1, int H0, int W0, int H1, int W1,
+                      const uint8_t* mask1, int w1c, float* out, uint8_t* inside, void* stream);
 
 /* ---- two-view geometry.  Robust fit of one model per pair to matches in a padded layout: pts0 / pts1 [B, K, 2] fp32
  * (x, y) pixels, 8-byte aligned; valid [B, K] bytes (non-zero: a match) or NULL (all K are matches).

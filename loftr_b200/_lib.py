@@ -130,6 +130,10 @@ SIGNATURES = {
     "lb_gemm_fp16": (c_int, [c_void_p, c_void_p, c_long, c_long, c_void_p, c_void_p, c_long, c_long, c_void_p,
                              c_long, c_long, c_int, c_int, c_int, c_int, c_void_p]),
     "lb_preprocess_images": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "lb_rectify_images": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                  c_void_p]),
+    "lb_rectify_points": (c_int, [c_void_p, c_void_p, c_long, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int,
+                                  c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "lb_geometry_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "lb_estimate_geometry": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int,
                                      C.c_ulonglong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -199,7 +203,8 @@ GEMM_FP16_VERSION = 110
 # the paths that need one the library lacks
 POINTS_ENTRIES = ("lb_coarse_query", "lb_fine_preprocess_centres")   # LoFTR.match_points
 GUIDE_ENTRIES = ("lb_coarse_match_guided",)   # data["guide"] / match_features(guide=...), DESIGN.md §18
-_OPTIONAL = set(POINTS_ENTRIES) | set(GUIDE_ENTRIES)
+RECTIFY_ENTRIES = ("lb_rectify_images", "lb_rectify_points")   # data["rectify1"] / warp_images, DESIGN.md §19
+_OPTIONAL = set(POINTS_ENTRIES) | set(GUIDE_ENTRIES) | set(RECTIFY_ENTRIES)
 GEOMETRY_HOMOGRAPHY = 0
 GEOMETRY_FUNDAMENTAL = 1
 GUIDE_HOMOGRAPHY = 0
@@ -279,7 +284,7 @@ def timing_enable(on: bool):
 
 def timing_collect() -> dict:
     """-> {tag: (total_ms, launches)} for every kernel tag (tensor-core kernels, match cap, point queries, image front
-    end, geometry) recorded since timing_enable(True)."""
+    end, rectifying warp, geometry) recorded since timing_enable(True)."""
     lib = load()
     n = lib.lb_timing_num_tags()
     ms = (C.c_double * n)()

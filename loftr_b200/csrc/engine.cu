@@ -57,16 +57,16 @@ static inline int cdiv(long a, long b) { return static_cast<int>((a + b - 1) / b
 
 // ------------------------------------------------------------------------------------------------ timing hook
 // Optional per-launch CUDA-event timing of the tensor-core kernels (bench.py's roofline leg), of the per-pair match
-// cap, of the point queries, of the image front end and of the geometry estimator (its three launches as one record):
-// events are recorded on the launching stream right around the kernels, and only while timing is enabled.  TAG_NONE:
-// not timed.
+// cap, of the point queries, of the image front end, of the rectifying warp and of the geometry estimator (its three
+// launches as one record): events are recorded on the launching stream right around the kernels, and only while
+// timing is enabled.  TAG_NONE: not timed.
 enum Tag { TAG_NONE = -1, TAG_GEMM_TEST = 0, TAG_PROJ, TAG_MERGE_LN, TAG_MLP1, TAG_MLP2_LN, TAG_SCORE_LSE,
            TAG_SCORE_ARGMAX, TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_FULL_ATTN, TAG_MATCH_CAP, TAG_PREPROCESS,
-           TAG_GEOMETRY, TAG_MATCH_QUERY, TAG_COUNT };
+           TAG_GEOMETRY, TAG_MATCH_QUERY, TAG_RECTIFY, TAG_COUNT };
 static const char* kTagNames[TAG_COUNT] = {"gemm_test", "proj_act", "merge_ln", "mlp1_relu", "mlp2_ln_res",
                                            "score_lse", "score_argmax", "fine_merge", "backbone_conv",
                                            "tf_kv_proj_fused", "tf_q_attn_fused", "tf_full_attn", "match_cap",
-                                           "preprocess", "geometry", "match_query"};
+                                           "preprocess", "geometry", "match_query", "rectify"};
 struct TimingRec {
   cudaEvent_t e0, e1;
   int tag;
@@ -1045,6 +1045,40 @@ int lb_preprocess_images(const LbImageDesc* descs, int n_images, float* out, int
   dim3 grid(cdiv(W, kPreprocessBlockX * 4), cdiv(H, kPreprocessBlockY), n_images);
   return launch(TAG_PREPROCESS, preprocess_images_kernel, grid, dim3(kPreprocessBlockX, kPreprocessBlockY), 0,
                 static_cast<cudaStream_t>(stream), descs, out, H, W, mask);
+}
+
+int lb_rectify_images(const float* image1, int n, int H1, int W1, const float* models, const float* scale0,
+                      const float* scale1, float* out, int H, int W, void* stream) {
+  if (H <= 0 || W <= 0 || H % 8 != 0 || W % 8 != 0)
+    return fail("lb_rectify_images: canvas %dx%d must be positive and divisible by 8", H, W);
+  if (n < 0 || n > 65535) return fail("lb_rectify_images: n=%d must be in [0, 65535]", n);
+  if (H1 <= 0 || W1 <= 0) return fail("lb_rectify_images: image1 size %dx%d must be positive", H1, W1);
+  if (!image1 || !models || !out) return fail("lb_rectify_images: image1, models and out are required");
+  if ((reinterpret_cast<uintptr_t>(out) & 15) != 0) return fail("lb_rectify_images: out is not 16-byte aligned");
+  if (n == 0) return 0;
+  DeviceScope dev;
+  LB_TRY(dev.bind(out));
+  dim3 grid(cdiv(W, kRectifyBlockX * 4), cdiv(H, kRectifyBlockY), n);
+  return launch(TAG_RECTIFY, rectify_images_kernel, grid, dim3(kRectifyBlockX, kRectifyBlockY), 0,
+                static_cast<cudaStream_t>(stream), image1, H1, W1, models, scale0, scale1, out, H, W);
+}
+
+int lb_rectify_points(const float* pts, const long long* pair_ids, long m, const int* M_live, const float* models,
+                      int n_pairs, const float* scale0, const float* scale1, int H0, int W0, int H1, int W1,
+                      const uint8_t* mask1, int w1c, float* out, uint8_t* inside, void* stream) {
+  if (m < 0 || n_pairs < 0) return fail("lb_rectify_points: m=%ld and n_pairs=%d must not be negative", m, n_pairs);
+  if (H0 <= 0 || W0 <= 0 || H1 <= 0 || W1 <= 0)
+    return fail("lb_rectify_points: image sizes %dx%d and %dx%d must be positive", H0, W0, H1, W1);
+  if (mask1 && (H1 % 8 != 0 || W1 % 8 != 0 || w1c != W1 / 8))
+    return fail("lb_rectify_points: mask1 needs image1 sides divisible by 8 and w1c = W1 / 8 (got %dx%d, w1c=%d)", H1,
+                W1, w1c);
+  if (m == 0) return 0;
+  if (!pts || !pair_ids || !models || !out) return fail("lb_rectify_points: pts, pair_ids, models and out are required");
+  DeviceScope dev;
+  LB_TRY(dev.bind(out));
+  const RectifyPointsParams p{pts, pair_ids, m, M_live, models, n_pairs, scale0, scale1, H0, W0, H1, W1, mask1, w1c,
+                              out, inside};
+  return launch(TAG_NONE, rectify_points_kernel, cdiv(m, 256), 256, 0, static_cast<cudaStream_t>(stream), p);
 }
 
 // n_out output images; with img_idx, output image b reads image img_idx[b] of feat

@@ -136,6 +136,151 @@ preprocess_images_kernel(const LbImageDesc* __restrict__ descs, float* __restric
 }
 
 // ------------------------------------------------------------------------------------------------
+// Rectified matching (DESIGN.md §19): image1 resampled onto image0's canvas through a per-pair homography x1 ~ H x0,
+// and points of that canvas mapped back into image1.  H acts on source pixels: network pixel (x, y) of image k sits at
+// (x * sx_k, y * sy_k), with (sx_k, sy_k) = scale_k[b], or (1, 1) without scales.
+//
+// Pair b's model as both kernels apply it, in fp64: the identity when an entry is not finite (a failed estimate), and
+// otherwise H times the sign of w at the centre ((W0 - 1) / 2, (H0 - 1) / 2) of image0's canvas (+1 when that w is 0),
+// so that H and -H act alike and w <= 0 marks points beyond the horizon.
+__device__ __forceinline__ void rectify_model(const float* __restrict__ models, long b, double cx, double cy,
+                                              double* h) {
+  bool finite = true;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) {
+    h[k] = static_cast<double>(models[b * 9 + k]);
+    finite = finite && isfinite(h[k]);
+  }
+  if (!finite) {
+#pragma unroll
+    for (int k = 0; k < 9; ++k) h[k] = (k % 4 == 0) ? 1.0 : 0.0;
+    return;
+  }
+  if (h[6] * cx + h[7] * cy + h[8] < 0.0) {
+#pragma unroll
+    for (int k = 0; k < 9; ++k) h[k] = -h[k];
+  }
+}
+
+// (qx, qy, qw) = H (px, py, 1); the one expression both kernels evaluate, so a point and its pixel agree
+__device__ __forceinline__ void rectify_apply(const double* h, double px, double py, double& qx, double& qy,
+                                              double& qw) {
+  qx = h[0] * px + h[1] * py + h[2];
+  qy = h[3] * px + h[4] * py + h[5];
+  qw = h[6] * px + h[7] * py + h[8];
+}
+
+constexpr int kRectifyBlockX = 32;   // threads along x, four output pixels each: a 128-pixel tile row
+constexpr int kRectifyBlockY = 8;
+// grid (cdiv(W, 128), cdiv(H, 8), n): output pixel (x, y) of pair blockIdx.z takes image1 at
+//   (u, v) = (H (x sx0, y sy0, 1))_xy / w / (sx1, sy1)      (image1's network pixels)
+// bilinearly, pixel centres at integer coordinates, taps outside [0, W1 - 1] x [0, H1 - 1] read as 0 (grid_sample with
+// align_corners=True and zero padding); 0 where w <= 0.  The coordinates are fp64 (as in preprocess_images_kernel: in
+// fp32 their rounding would move the weights by ~1e-4 at x ~ 1000) and the interpolation is fp32 with exact weights of
+// 0 at integer coordinates, so an identity model with equal sizes and scales copies image1 bit for bit.  No texture
+// filtering: its weights have 8 fractional bits.  W is a multiple of 8, so a thread's four pixels lie in one row and
+// its float4 store is aligned.
+__global__ void __launch_bounds__(kRectifyBlockX * kRectifyBlockY)
+rectify_images_kernel(const float* __restrict__ image1, int H1, int W1, const float* __restrict__ models,
+                      const float* __restrict__ scale0, const float* __restrict__ scale1, float* __restrict__ out,
+                      int H, int W) {
+  __shared__ double s_h[9];
+  __shared__ double s_scale[4];   // sx0, sy0, sx1, sy1
+  const int b = blockIdx.z;
+  if (threadIdx.x == 0 && threadIdx.y == 0) {
+    const double sx0 = scale0 ? scale0[2 * b] : 1.0, sy0 = scale0 ? scale0[2 * b + 1] : 1.0;
+    double h[9];
+    rectify_model(models, b, 0.5 * (W - 1) * sx0, 0.5 * (H - 1) * sy0, h);
+#pragma unroll
+    for (int k = 0; k < 9; ++k) s_h[k] = h[k];
+    s_scale[0] = sx0;
+    s_scale[1] = sy0;
+    s_scale[2] = scale1 ? scale1[2 * b] : 1.0;
+    s_scale[3] = scale1 ? scale1[2 * b + 1] : 1.0;
+  }
+  __syncthreads();
+  const int x4 = (blockIdx.x * kRectifyBlockX + threadIdx.x) * 4;
+  const int y = blockIdx.y * kRectifyBlockY + threadIdx.y;
+  if (x4 >= W || y >= H) return;
+  double h[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) h[k] = s_h[k];
+  const double sx0 = s_scale[0], py = y * s_scale[1], sx1 = s_scale[2], sy1 = s_scale[3];
+  const float* src = image1 + static_cast<long>(b) * H1 * W1;
+  auto tap = [&](int ix, int iy) {
+    return (ix >= 0 && ix < W1 && iy >= 0 && iy < H1) ? __ldg(src + static_cast<long>(iy) * W1 + ix) : 0.f;
+  };
+  float v[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    double qx, qy, qw;
+    rectify_apply(h, (x4 + i) * sx0, py, qx, qy, qw);
+    v[i] = 0.f;
+    if (!(qw > 0.0)) continue;
+    const double u = qx / qw / sx1, w = qy / qw / sy1;
+    if (!(u > -1.0 && u < W1 && w > -1.0 && w < H1)) continue;   // no tap inside (and no int overflow below)
+    const double u0 = floor(u), w0 = floor(w);
+    const float fx = static_cast<float>(u - u0), fy = static_cast<float>(w - w0);
+    const int ix = static_cast<int>(u0), iy = static_cast<int>(w0);
+    const float a = tap(ix, iy), c = tap(ix + 1, iy);
+    const float d = tap(ix, iy + 1), e = tap(ix + 1, iy + 1);
+    const float top = a + fx * (c - a);
+    const float bot = d + fx * (e - d);
+    v[i] = top + fy * (bot - top);
+  }
+  *reinterpret_cast<float4*>(out + (static_cast<long>(b) * H + y) * W + x4) = make_float4(v[0], v[1], v[2], v[3]);
+}
+
+// Points of the rectified canvas back into image1: point i of pair ids[i] (source pixels of image0's frame) ->
+// H p in fp64, rounded once to fp32 (source pixels of image1); NaN with inside 0 where w <= 0, the point is not
+// finite or the pair id is out of range.  inside[i]: the mapped point divided by scale1 lies in [0, W1 - 1] x
+// [0, H1 - 1] and, with mask1, in a true cell of mask1[b] (cell (floor(v / 8), floor(u / 8)), w1c cells per row).
+// Only i < min(*live, m) when live is given.
+struct RectifyPointsParams {
+  const float* pts;
+  const long long* ids;
+  long m;
+  const int* live;
+  const float* models;
+  int n_pairs;
+  const float* scale0;
+  const float* scale1;
+  int H0, W0, H1, W1;
+  const uint8_t* mask1;
+  int w1c;
+  float* out;
+  uint8_t* inside;
+};
+
+__global__ void rectify_points_kernel(const RectifyPointsParams p) {
+  const long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x;
+  const long m = p.live ? min(p.m, static_cast<long>(max(*p.live, 0))) : p.m;
+  if (i >= m) return;
+  const long long b = p.ids[i];
+  float ox = __int_as_float(0x7fc00000), oy = ox;   // NaN
+  bool in = false;
+  if (b >= 0 && b < p.n_pairs) {
+    const double sx0 = p.scale0 ? p.scale0[2 * b] : 1.0, sy0 = p.scale0 ? p.scale0[2 * b + 1] : 1.0;
+    double h[9];
+    rectify_model(p.models, b, 0.5 * (p.W0 - 1) * sx0, 0.5 * (p.H0 - 1) * sy0, h);
+    double qx, qy, qw;
+    rectify_apply(h, p.pts[2 * i], p.pts[2 * i + 1], qx, qy, qw);
+    if (qw > 0.0) {
+      const double x = qx / qw, y = qy / qw;
+      ox = static_cast<float>(x);
+      oy = static_cast<float>(y);
+      const double u = x / (p.scale1 ? p.scale1[2 * b] : 1.0), v = y / (p.scale1 ? p.scale1[2 * b + 1] : 1.0);
+      in = u >= 0.0 && u <= p.W1 - 1 && v >= 0.0 && v <= p.H1 - 1;
+      if (in && p.mask1)
+        in = p.mask1[(b * (p.H1 >> 3) + static_cast<long>(floor(v / 8))) * p.w1c + static_cast<long>(floor(u / 8))] != 0;
+    }
+  }
+  p.out[2 * i] = ox;
+  p.out[2 * i + 1] = oy;
+  if (p.inside) p.inside[i] = in ? 1 : 0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Linear attention, source side (reference linear_attention.py:43-44):
 //   KV[g,h,d,v] = sum_s K[s,h,d] * V[s,h,v],   Ksum[g,h,d] = sum_s K[s,h,d]
 // over the rows s of group g.  K = elu+1 and the padding mask were already applied by the projection epilogue.  The

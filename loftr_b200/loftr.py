@@ -79,6 +79,44 @@ def check_guide(guide, n, device, thr, who):
     return GUIDE_KINDS[kind], model.contiguous(), float(radius)
 
 
+def check_rectify(model, n, device, who):
+    """Validates a rectifying model (data["rectify1"], DESIGN.md §19) for `n` pairs whose image0 lives on `device`,
+    before any launch and without a host sync; `who` names the caller in the messages.
+    model: float32 CUDA [n, 3, 3], one homography x1 ~ H x0 per pair -> the model as the kernels read it."""
+    if not torch.is_tensor(model) or model.dtype != torch.float32:
+        raise TypeError(f"{who}: rectify1 must be a float32 tensor (got "
+                        f"{model.dtype if torch.is_tensor(model) else type(model).__name__})")
+    if tuple(model.shape) != (n, 3, 3):
+        raise ValueError(f"{who}: rectify1 must be [N, 3, 3] with N = {n} pairs (got {tuple(model.shape)})")
+    if model.device != torch.device(device):
+        raise ValueError(f"{who}: rectify1 is on {model.device}, the images on {device}")
+    _lib.require_entries(_lib.RECTIFY_ENTRIES, f"{who}: rectified matching")
+    if not model.is_cuda:
+        raise ValueError(f"{who}: rectify1 must be a CUDA tensor (the warp and the back-mapping run on the GPU)")
+    return model.contiguous()
+
+
+def _map_back(data, model, pts, ids, live=None, inside=True):
+    """Points of the rectified frame back into image1 through each pair's model (lb_rectify_points, DESIGN.md §19),
+    with the image sizes, scales and mask1 of the caller's `data`.  pts [m, 2] f32 (source pixels of image0's frame),
+    ids int64 [m] (the pair of each point), model [n, 3, 3] (`check_rectify`), live: None or the int32 device count
+    that bounds the points written.  No host sync.
+    -> (mapped [m, 2] f32 in source pixels of image1, inside [m] bool or None when not `inside`)."""
+    dev = pts.device
+    m = pts.shape[0]
+    out = torch.empty(m, 2, dtype=torch.float32, device=dev)
+    flag = torch.empty(m, dtype=torch.bool, device=dev) if inside else None
+    s0, s1, m1 = (None if data.get(k) is None else data[k].to(dev, t).contiguous()
+                  for k, t in (("scale0", torch.float32), ("scale1", torch.float32), ("mask1", torch.uint8)))
+    pts, ids = pts.contiguous(), ids.contiguous()
+    (h0, w0), (h1, w1) = data["image0"].shape[2:], data["image1"].shape[2:]
+    _lib.check(_lib.load().lb_rectify_points(
+        pts.data_ptr(), ids.data_ptr(), m, _lib.ptr(live), model.data_ptr(), model.shape[0], _lib.ptr(s0),
+        _lib.ptr(s1), h0, w0, h1, w1, _lib.ptr(m1), w1 // 8, out.data_ptr(),
+        None if flag is None else flag.view(torch.uint8).data_ptr(), _stream(dev)))
+    return out, flag
+
+
 def _stream(ref=None):
     """cudaStream_t of torch's current stream ON THE DEVICE THAT OWNS `ref` (a tensor or torch.device); the library
     binds itself to the device of the buffers it is given, so the stream handle must belong to that device too."""
@@ -833,9 +871,19 @@ class LoFTR(nn.Module):
         "fundamental" | "homography", "model": float32 [N, 3, 3] on image0's device, one matrix per pair in the
         coordinates of mkpts0_f / mkpts1_f, "radius": pixels of image1, finite and > 0}.  Only cell pairs whose coarse
         keypoints agree with the pair's model within the radius can match, and only they enter the softmax (Sinkhorn)
-        normalisers; a pair whose model has a non-finite entry is matched unguided.  Needs match_coarse.thr >= 0."""
+        normalisers; a pair whose model has a non-finite entry is matched unguided.  Needs match_coarse.thr >= 0.
+
+        Optional rectify1 (rectified matching, DESIGN.md §19): float32 [N, 3, 3] on image0's device, one homography
+        x1 ~ H x0 per pair in the coordinates of mkpts0_f / mkpts1_f.  The call then matches image0 against image1
+        warped onto image0's canvas through H (`warp_images`; scale1 := scale0, mask1 := mask0) and maps mkpts1_c /
+        mkpts1_f back through H into image1; the new key minside1 [M] bool says whether mkpts1_f lies in image1's valid
+        area.  expec_f, j_ids and hw1_* describe the rectified frame (image0's grid).  The caller's image1, scale1 and
+        mask1 are not replaced.  Not combinable with a guide."""
         _require_eval(self)
         _require_cuda(data["image0"], "image0")
+        if data.get("rectify1") is not None:
+            self._match_rectified(data, "forward")
+            return
         if data.get("guide") is not None:
             check_guide(data["guide"], data["image0"].shape[0], data["image0"].device, self.coarse_matching.thr,
                         "forward")
@@ -982,7 +1030,8 @@ class LoFTR(nn.Module):
         Configurations whose output list depends on the data (match_coarse.thr < 0) raise ValueError.
 
         data["guide"] (as in `forward`): its model must be on the device as well.  A captured graph bakes in the kind
-        and the radius and reads the model from the same tensor at every replay."""
+        and the radius and reads the model from the same tensor at every replay.  data["rectify1"] (as in `forward`):
+        a captured graph reads it from the same tensor at every replay as well; minside1 is a capacity buffer too."""
         _require_static(self, capacity, "forward_static")
         dev = None
         for k in ("image0", "image1", "mask0", "mask1", "scale0", "scale1"):
@@ -996,10 +1045,47 @@ class LoFTR(nn.Module):
                 dev = t.device
             elif t.device != dev:
                 raise ValueError(f"forward_static: `{k}` is on {t.device}, image0 on {dev}")
+        if data.get("rectify1") is not None:
+            self._match_rectified(data, "forward_static", static=True, capacity=capacity)
+            return
         if data.get("guide") is not None:
             check_guide(data["guide"], data["image0"].shape[0], data["image0"].device, self.coarse_matching.thr,
                         "forward_static")
         self._match_pairs(data, *self._backbone_pairs(data), static=True, capacity=capacity)
+
+    def _rectified(self, data, who):
+        """The substituted input of a call with data["rectify1"] (DESIGN.md §19), validated before any launch and
+        without a host sync -> (work dict: image0, image1 warped onto image0's canvas, scale1 := scale0 and mask1 :=
+        mask0 when given; the model as `check_rectify` returns it)."""
+        from .preprocess import warp_images   # preprocess imports this module
+        if data.get("guide") is not None:
+            raise ValueError(f"{who}: data['rectify1'] cannot be combined with data['guide']")
+        img0, img1 = data["image0"], data["image1"]
+        model = check_rectify(data["rectify1"], img0.shape[0], img0.device, who)
+        if ("scale0" in data) != ("scale1" in data):
+            raise ValueError(f"{who}: give scale0 and scale1 together")
+        if ("mask0" in data) != ("mask1" in data):
+            raise ValueError(f"{who}: give mask0 and mask1 together")
+        want = (img1.shape[0], img1.shape[2] // 8, img1.shape[3] // 8)
+        if "mask1" in data and tuple(data["mask1"].shape) != want:
+            raise ValueError(f"{who}: mask1 must be [N, H1/8, W1/8] = {want} (got {tuple(data['mask1'].shape)})")
+        work = {"image0": img0,
+                "image1": warp_images(img1, model, img0.shape[2:], data.get("scale0"), data.get("scale1"))}
+        if "scale0" in data:
+            work["scale0"] = work["scale1"] = data["scale0"]
+        if "mask0" in data:
+            work["mask0"] = work["mask1"] = data["mask0"]
+        return work, model
+
+    def _match_rectified(self, data, who, static=False, capacity=None):
+        """forward / forward_static with data["rectify1"]: the call on the substituted input, then mkpts1_c / mkpts1_f
+        mapped back and minside1; every key the call writes goes into `data`, the caller's inputs stay."""
+        work, model = self._rectified(data, who)
+        self._match_pairs(work, *self._backbone_pairs(work), static=static, capacity=capacity)
+        live, ids = work.get("num_matches"), work["m_bids"]
+        work["mkpts1_c"], _ = _map_back(data, model, work["mkpts1_c"], ids, live, inside=False)
+        work["mkpts1_f"], work["minside1"] = _map_back(data, model, work["mkpts1_f"], ids, live)
+        data.update({k: v for k, v in work.items() if k not in _INPUT_KEYS})
 
     @torch.no_grad()
     def match_points(self, data, points0, valid0=None):
@@ -1019,13 +1105,31 @@ class LoFTR(nn.Module):
         Each query's outputs depend only on its own point, pair and images.  A query at a forward match's mkpts0_c gets
         that match's j_ids, mconf, mkpts1_c, mkpts1_f and expec_f bit for bit.  Shapes are fixed by [N, Q] and there is
         no host synchronisation, so the call can be captured by `torch.cuda.graph` after one eager call.
-        A guide (data["guide"]) is not supported here and raises ValueError."""
+        A guide (data["guide"]) is not supported here and raises ValueError.
+
+        data["rectify1"] (as in `forward`): the queries are answered on the substituted input; qpts1_c / qpts1_f are
+        mapped back into image1 and qinside1 [N, Q] bool says whether qpts1_f lies in image1's valid area; qexpec_f
+        and q_j_ids stay in the rectified frame."""
         _require_eval(self)
         if data.get("guide") is not None:
             raise ValueError("match_points: data['guide'] is not supported (guided matching is available in forward, "
                              "forward_static and match_features)")
         _lib.require_entries(_lib.POINTS_ENTRIES, "match_points")
         _check_points(data, points0, valid0)
+        if data.get("rectify1") is None:
+            self._match_points(data, points0, valid0)
+            return
+        work, model = self._rectified(data, "match_points")
+        self._match_points(work, points0, valid0)
+        n, q = points0.shape[:2]
+        ids = torch.arange(n, device=points0.device)[:, None].expand(n, q).reshape(-1)   # query b*Q + k is of pair b
+        work["qpts1_c"] = _map_back(data, model, work["qpts1_c"].view(-1, 2), ids, inside=False)[0].view(n, q, 2)
+        pts, inside = _map_back(data, model, work["qpts1_f"].view(-1, 2), ids)
+        work["qpts1_f"], work["qinside1"] = pts.view(n, q, 2), inside.view(n, q)
+        data.update({k: v for k, v in work.items() if k not in _INPUT_KEYS})
+
+    def _match_points(self, data, points0, valid0):
+        """match_points on validated arguments."""
         n, q = points0.shape[:2]
         dev = points0.device
         if q == 0:
@@ -1151,6 +1255,10 @@ class LoFTR(nn.Module):
                 state_dict[k.replace("matcher.", "", 1)] = state_dict.pop(k)
         self.invalidate_packed()
         return super().load_state_dict(state_dict, *args, **kwargs)
+
+
+# forward's inputs: a rectified call copies every other key of its work dict back to the caller's
+_INPUT_KEYS = ("image0", "image1", "mask0", "mask1", "scale0", "scale1")
 
 
 def _require_static(model, capacity, what):
@@ -1298,9 +1406,10 @@ class CapturedMatcher:
                                "invalidate_packed() or a parameter update); call recapture()")
 
     def __call__(self, data):
-        if data.get("guide") is not None:
-            raise ValueError("CapturedMatcher: data['guide'] is not supported (capture LoFTR.forward_static with a "
-                             "guide instead)")
+        for k, what in (("guide", "a guide"), ("rectify1", "rectify1")):
+            if data.get(k) is not None:
+                raise ValueError(f"CapturedMatcher: data['{k}'] is not supported (capture LoFTR.forward_static with "
+                                 f"{what} instead)")
         if self.graph is None:
             raise RuntimeError("loftr_b200.CapturedMatcher: no captured graph; call recapture()")
         self._check_weights()

@@ -20,7 +20,7 @@ from typing import NamedTuple, Optional
 import torch
 
 from . import _lib
-from .loftr import _stream
+from .loftr import _stream, check_rectify
 
 class PreparedImages(NamedTuple):
     image: torch.Tensor            # [K, 1, H, W] float32 in [0, 1], zero outside each image's valid region
@@ -256,3 +256,40 @@ def prepare_pairs(images0, images1, resize=None, df=8, pad_to=None, channel_orde
     if plan0.resized or plan1.resized:
         data["scale0"], data["scale1"] = p0.scale, p1.scale
     return data
+
+
+def warp_images(images1, model, hw, scale0=None, scale1=None):
+    """image1 of every pair resampled onto image0's canvas through the pair's homography (DESIGN.md §19): the input
+    that `matcher(data)` substitutes for image1 when data["rectify1"] is given, in one kernel launch and without a host
+    sync.
+
+    images1: float32 [N, 1, H1, W1] CUDA.  model: float32 [N, 3, 3] on the same device, x1 ~ H x0 in the coordinates
+    of mkpts0_f / mkpts1_f (source pixels when scales are given; a model with a non-finite entry stands for the
+    identity).  hw: image0's canvas (H, W), both positive multiples of 8.  scale0 / scale1: optional [N, 2] scales of
+    image0 / image1 (both or neither).
+    -> float32 [N, 1, H, W]: output pixel (x, y) is image1 sampled bilinearly at H (x sx0, y sy0) / (sx1, sy1), taps
+    outside image1 read as 0 (grid_sample with align_corners=True and zero padding), and 0 beyond the horizon."""
+    if not torch.is_tensor(images1) or images1.dtype != torch.float32 or images1.dim() != 4 or images1.shape[1] != 1:
+        got = (images1.dtype, tuple(images1.shape)) if torch.is_tensor(images1) else type(images1).__name__
+        raise ValueError(f"warp_images: images1 must be a float32 tensor [N, 1, H1, W1] (got {got})")
+    n = images1.shape[0]
+    if not (isinstance(hw, (tuple, list, torch.Size)) and len(hw) == 2 and all(_is_int(v) and v > 0 and v % 8 == 0
+                                                                                for v in hw)):
+        raise ValueError(f"warp_images: hw must be (H, W), positive multiples of 8 (got {hw!r})")
+    if (scale0 is None) != (scale1 is None):
+        raise ValueError("warp_images: give scale0 and scale1 together")
+    scales = []
+    for name, s in (("scale0", scale0), ("scale1", scale1)):
+        if s is not None:
+            if not torch.is_tensor(s) or tuple(s.shape) != (n, 2):
+                raise ValueError(f"warp_images: {name} must be a tensor [N, 2] with N = {n}")
+            s = s.to(images1.device, torch.float32).contiguous()
+        scales.append(s)
+    model = check_rectify(model, n, images1.device, "warp_images")   # on images1's device, which is then a CUDA one
+    H, W = int(hw[0]), int(hw[1])
+    images1 = images1.contiguous()
+    out = torch.empty(n, 1, H, W, dtype=torch.float32, device=images1.device)
+    _lib.check(_lib.load().lb_rectify_images(images1.data_ptr(), n, images1.shape[2], images1.shape[3],
+                                             model.data_ptr(), _lib.ptr(scales[0]), _lib.ptr(scales[1]),
+                                             out.data_ptr(), H, W, _stream(images1)))
+    return out
