@@ -63,7 +63,8 @@ extern "C" {
  * Entries added without a version step (a caller finds them by name: a build that lacks one does not export it):
  * lb_coarse_query / lb_fine_preprocess_centres (matching caller-given image0 points);
  * lb_coarse_match_guided (coarse matching restricted to a band around a homography or fundamental matrix);
- * lb_rectify_images / lb_rectify_points (image1 warped into image0's frame through a homography, matches mapped back). */
+ * lb_rectify_images / lb_rectify_points (image1 warped into image0's frame through a homography, matches mapped back);
+ * lb_coarse_match_search (coarse matching of K candidate warps per pair, keeping the best candidate's matches). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -344,6 +345,24 @@ typedef struct LbCoarseGuide {
  * max_per_pair: 0 = no cap, >= 1 as lb_coarse_match_capped.  Errors: a NULL guide or model, an unknown kind, a radius
  * that is not finite and positive.  Same workspace as lb_coarse_match. */
 int lb_coarse_match_guided(const LbCoarseMatchArgs* args /*host*/, const LbCoarseGuide* guide /*host*/,
+                           int max_per_pair, int fp16, void* ws, size_t ws_bytes, void* stream);
+
+/* Rectification search (found by name, see lb_version; DESIGN.md §20).  A separate structure, not new fields of
+ * LbCoarseMatchArgs: DESIGN.md §12.  args->n_pairs = N * K candidates, candidate c = b * K + k of pair b. */
+typedef struct LbCoarseSearch {
+  int K;               /* >= 1 candidates per pair; args->n_pairs must be a multiple of K */
+  int* counts;         /* [N, K] int32, device: the candidate's flagged rows (mutual, masks, border, > thr, Sinkhorn
+                        * prefilter), before any per-pair cap */
+  long long* choice;   /* [N] int64, device: the smallest k with the largest count (0 when every count is 0) */
+} LbCoarseSearch;
+/* lb_coarse_match / lb_coarse_match_capped (fp16 = 0) or lb_coarse_match_fp16 (fp16 = 1) over the N * K candidates,
+ * with one more launch between the flag pass and the cap (timing tag "match_search", one CTA per pair): it writes
+ * counts and choice and clears the flags of every candidate but (b, choice[b]).  The cap (max_per_pair: 0 = no cap,
+ * >= 1 as lb_coarse_match_capped) and the compaction then see the winners' rows only: b_ids hold candidate ids c, and
+ * a capacity of the N-pair bound (N * min(L, S), N * L with masks, N * min(max_per_pair, that) with a cap) always
+ * suffices.  Errors: a NULL search, NULL counts or choice with n_pairs > 0, K < 1, n_pairs not a multiple of K.  Same
+ * workspace as lb_coarse_match. */
+int lb_coarse_match_search(const LbCoarseMatchArgs* args /*host*/, const LbCoarseSearch* search /*host*/,
                            int max_per_pair, int fp16, void* ws, size_t ws_bytes, void* stream);
 
 /* Caller-given image0 points of every pair (found by name, see lb_version; LoFTR.match_points, DESIGN.md §17).  A separate structure, not

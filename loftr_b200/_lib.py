@@ -88,6 +88,10 @@ class LbCoarseGuide(C.Structure):
     _fields_ = [("kind", c_int), ("model", c_void_p), ("radius", c_float)]
 
 
+class LbCoarseSearch(C.Structure):
+    _fields_ = [("K", c_int), ("counts", c_void_p), ("choice", c_void_p)]
+
+
 class LbFinePreprocessArgs(C.Structure):
     _fields_ = [
         ("feat_f0", c_void_p), ("feat_f1", c_void_p),
@@ -159,6 +163,8 @@ SIGNATURES = {
     "lb_coarse_match_fp16": (c_int, [C.POINTER(LbCoarseMatchArgs), c_int, c_void_p, c_size_t, c_void_p]),
     "lb_coarse_match_guided": (c_int, [C.POINTER(LbCoarseMatchArgs), C.POINTER(LbCoarseGuide), c_int, c_int, c_void_p,
                                        c_size_t, c_void_p]),
+    "lb_coarse_match_search": (c_int, [C.POINTER(LbCoarseMatchArgs), C.POINTER(LbCoarseSearch), c_int, c_int,
+                                       c_void_p, c_size_t, c_void_p]),
     "lb_coarse_query": (c_int, [C.POINTER(LbCoarseMatchArgs), C.POINTER(LbCoarseQueryArgs), c_int, c_void_p, c_size_t,
                                 c_void_p]),
     "lb_fine_preprocess_workspace_bytes": (c_size_t, [c_long, c_int, c_int]),
@@ -204,7 +210,8 @@ GEMM_FP16_VERSION = 110
 POINTS_ENTRIES = ("lb_coarse_query", "lb_fine_preprocess_centres")   # LoFTR.match_points
 GUIDE_ENTRIES = ("lb_coarse_match_guided",)   # data["guide"] / match_features(guide=...), DESIGN.md §18
 RECTIFY_ENTRIES = ("lb_rectify_images", "lb_rectify_points")   # data["rectify1"] / warp_images, DESIGN.md §19
-_OPTIONAL = set(POINTS_ENTRIES) | set(GUIDE_ENTRIES) | set(RECTIFY_ENTRIES)
+SEARCH_ENTRIES = ("lb_coarse_match_search",)   # data["rectify1_candidates"], DESIGN.md §20
+_OPTIONAL = set(POINTS_ENTRIES) | set(GUIDE_ENTRIES) | set(RECTIFY_ENTRIES) | set(SEARCH_ENTRIES)
 GEOMETRY_HOMOGRAPHY = 0
 GEOMETRY_FUNDAMENTAL = 1
 GUIDE_HOMOGRAPHY = 0
@@ -283,8 +290,8 @@ def timing_enable(on: bool):
 
 
 def timing_collect() -> dict:
-    """-> {tag: (total_ms, launches)} for every kernel tag (tensor-core kernels, match cap, point queries, image front
-    end, rectifying warp, geometry) recorded since timing_enable(True)."""
+    """-> {tag: (total_ms, launches)} for every kernel tag (tensor-core kernels, match cap, rectification search, point
+    queries, image front end, rectifying warp, geometry) recorded since timing_enable(True)."""
     lib = load()
     n = lib.lb_timing_num_tags()
     ms = (C.c_double * n)()

@@ -57,16 +57,16 @@ static inline int cdiv(long a, long b) { return static_cast<int>((a + b - 1) / b
 
 // ------------------------------------------------------------------------------------------------ timing hook
 // Optional per-launch CUDA-event timing of the tensor-core kernels (bench.py's roofline leg), of the per-pair match
-// cap, of the point queries, of the image front end, of the rectifying warp and of the geometry estimator (its three
-// launches as one record): events are recorded on the launching stream right around the kernels, and only while
-// timing is enabled.  TAG_NONE: not timed.
+// cap and the rectification search, of the point queries, of the image front end, of the rectifying warp and of the
+// geometry estimator (its three launches as one record): events are recorded on the launching stream right around the
+// kernels, and only while timing is enabled.  TAG_NONE: not timed.
 enum Tag { TAG_NONE = -1, TAG_GEMM_TEST = 0, TAG_PROJ, TAG_MERGE_LN, TAG_MLP1, TAG_MLP2_LN, TAG_SCORE_LSE,
            TAG_SCORE_ARGMAX, TAG_FINE_MERGE, TAG_CONV, TAG_KV, TAG_QATTN, TAG_FULL_ATTN, TAG_MATCH_CAP, TAG_PREPROCESS,
-           TAG_GEOMETRY, TAG_MATCH_QUERY, TAG_RECTIFY, TAG_COUNT };
+           TAG_GEOMETRY, TAG_MATCH_QUERY, TAG_RECTIFY, TAG_MATCH_SEARCH, TAG_COUNT };
 static const char* kTagNames[TAG_COUNT] = {"gemm_test", "proj_act", "merge_ln", "mlp1_relu", "mlp2_ln_res",
                                            "score_lse", "score_argmax", "fine_merge", "backbone_conv",
                                            "tf_kv_proj_fused", "tf_q_attn_fused", "tf_full_attn", "match_cap",
-                                           "preprocess", "geometry", "match_query", "rectify"};
+                                           "preprocess", "geometry", "match_query", "rectify", "match_search"};
 struct TimingRec {
   cudaEvent_t e0, e1;
   int tag;
@@ -1492,10 +1492,12 @@ static int coarse_rows(const LbCoarseMatchArgs* a, const GuideParams* guide, con
 }
 
 // max_per_pair: 0 = every match; otherwise each pair keeps its max_per_pair most confident matches (match_cap_kernel).
-// guide: NULL, or the guide of lb_coarse_match_guided.
+// guide: NULL, or the guide of lb_coarse_match_guided.  search: NULL, or the search of lb_coarse_match_search
+// (a->n_pairs a multiple of search->K): rectify_search_kernel keeps only the flags of each pair's winning candidate,
+// before the cap.
 template <int kP>
 static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, const GuideParams* guide, void* ws,
-                        size_t ws_bytes, void* stream) {
+                        size_t ws_bytes, void* stream, const LbCoarseSearch* search = nullptr) {
   DeviceScope dev;
   LB_TRY(dev.bind(a->count));
   const int n = a->n_pairs, L = a->L, S = a->S;
@@ -1509,6 +1511,10 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, const Guid
   LB_TRY((guide ? coarse_rows<kP, true>(a, guide, dev, ws, ws_bytes, st, w, sp)
                 : coarse_rows<kP, false>(a, nullptr, dev, ws, ws_bytes, st, w, sp)));
   const long nl = static_cast<long>(n) * L;
+  if (search) {
+    LB_TRY(launch(TAG_MATCH_SEARCH, rectify_search_kernel, n / search->K, kSearchBlock, 0, st, w.flag, L, search->K,
+                  search->counts, search->choice));
+  }
   if (max_per_pair > 0) {
     LB_TRY(launch(TAG_MATCH_CAP, match_cap_kernel, n, kCapBlock, 0, st, w.flag, w.conf, L, max_per_pair));
   }
@@ -1555,6 +1561,20 @@ int lb_coarse_match_guided(const LbCoarseMatchArgs* a, const LbCoarseGuide* g, i
   const GuideParams gp{g->kind, g->model, g->radius, a->img_scale, a->scale0, a->scale1, a->w0c, a->w1c};
   return fp16 ? coarse_match<1>(a, max_per_pair, &gp, ws, ws_bytes, stream)
               : coarse_match<2>(a, max_per_pair, &gp, ws, ws_bytes, stream);
+}
+
+int lb_coarse_match_search(const LbCoarseMatchArgs* a, const LbCoarseSearch* s, int max_per_pair, int fp16, void* ws,
+                           size_t ws_bytes, void* stream) {
+  if (!s || (a->n_pairs > 0 && (!s->counts || !s->choice)))
+    return fail("lb_coarse_match_search: the search and its counts and choice outputs are required");
+  if (s->K < 1) return fail("lb_coarse_match_search: K=%d must be at least 1", s->K);
+  if (a->n_pairs % s->K != 0)
+    return fail("lb_coarse_match_search: n_pairs=%d is not a multiple of K=%d", a->n_pairs, s->K);
+  if (max_per_pair < 0)
+    return fail("lb_coarse_match_search: max_per_pair must be 0 (no cap) or at least 1 (got %d)", max_per_pair);
+  if (fp16 != 0 && fp16 != 1) return fail("lb_coarse_match_search: fp16 must be 0 (split) or 1 (got %d)", fp16);
+  return fp16 ? coarse_match<1>(a, max_per_pair, nullptr, ws, ws_bytes, stream, s)
+              : coarse_match<2>(a, max_per_pair, nullptr, ws, ws_bytes, stream, s);
 }
 
 int lb_coarse_query(const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, int operand_planes, void* ws,

@@ -940,6 +940,50 @@ __global__ void __launch_bounds__(kCapBlock) match_cap_kernel(uint8_t* __restric
   }
 }
 
+// Rectification search (DESIGN.md §20), between the flag pass and the per-pair cap: the n_pairs "pairs" of the coarse
+// stage are N * K candidates, candidate c = b * K + k.  One CTA per pair b counts the flagged rows of each of its K
+// candidates (counts[b * K + k]), picks the smallest k with the largest count (choice[b]; 0 when every count is 0) and
+// clears the flags of the other K - 1 candidates, so that the cap and the compaction see the winner's rows only.
+constexpr int kSearchBlock = 256;
+__global__ void __launch_bounds__(kSearchBlock) rectify_search_kernel(uint8_t* __restrict__ flag, int L, int K,
+                                                                      int* __restrict__ counts,
+                                                                      long long* __restrict__ choice) {
+  __shared__ int s_warp[kSearchBlock / 32];
+  __shared__ int s_best;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long c0 = static_cast<long>(blockIdx.x) * K;
+  int best = 0, best_cnt = -1;   // thread 0's running choice
+  for (int k = 0; k < K; ++k) {
+    const uint8_t* f = flag + (c0 + k) * L;
+    int cnt = 0;
+    for (int i = threadIdx.x; i < L; i += kSearchBlock) cnt += f[i] ? 1 : 0;
+    for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if (lane == 0) s_warp[warp] = cnt;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int total = 0;
+      for (int w = 0; w < kSearchBlock / 32; ++w) total += s_warp[w];
+      counts[c0 + k] = total;
+      if (total > best_cnt) {   // strictly larger: a tie keeps the smaller k
+        best_cnt = total;
+        best = k;
+      }
+    }
+    __syncthreads();   // s_warp is rewritten for the next candidate
+  }
+  if (threadIdx.x == 0) {
+    choice[blockIdx.x] = best;
+    s_best = best;
+  }
+  __syncthreads();
+  const int win = s_best;
+  for (int k = 0; k < K; ++k) {
+    if (k == win) continue;
+    uint8_t* f = flag + (c0 + k) * L;
+    for (int i = threadIdx.x; i < L; i += kSearchBlock) f[i] = 0;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Sinkhorn helpers (log_optimal_transport, third_party/SuperGluePretrainedNetwork/models/superglue.py:
 // 141-170; called from coarse_matching.py:130-131).  The (L+1)x(S+1) couplings matrix is never

@@ -96,6 +96,58 @@ def check_rectify(model, n, device, who):
     return model.contiguous()
 
 
+def check_rectify_candidates(cands, n, device, who):
+    """Validates the candidates of a rectification search (data["rectify1_candidates"], DESIGN.md §20) for `n` pairs
+    whose image0 lives on `device`, before any launch and without a host sync; `who` names the caller in the messages.
+    cands: float32 CUDA [n, K, 3, 3], K >= 1 homographies x1 ~ H x0 per pair (each as data["rectify1"]), n * K at most
+    65535 -> the candidates as the kernels read them."""
+    if not torch.is_tensor(cands) or cands.dtype != torch.float32:
+        raise TypeError(f"{who}: rectify1_candidates must be a float32 tensor (got "
+                        f"{cands.dtype if torch.is_tensor(cands) else type(cands).__name__})")
+    if cands.dim() != 4 or cands.shape[0] != n or tuple(cands.shape[2:]) != (3, 3):
+        raise ValueError(f"{who}: rectify1_candidates must be [N, K, 3, 3] with N = {n} pairs (got "
+                         f"{tuple(cands.shape)})")
+    k = cands.shape[1]
+    if k < 1:
+        raise ValueError(f"{who}: rectify1_candidates needs at least one candidate per pair (got K = 0)")
+    if n * k > 65535:
+        raise ValueError(f"{who}: rectify1_candidates holds N * K = {n * k} candidate pairs, more than the warp's "
+                         "65535")
+    if cands.device != torch.device(device):
+        raise ValueError(f"{who}: rectify1_candidates is on {cands.device}, the images on {device}")
+    _lib.require_entries(_lib.SEARCH_ENTRIES + _lib.RECTIFY_ENTRIES, f"{who}: the rectification search")
+    if not cands.is_cuda:
+        raise ValueError(f"{who}: rectify1_candidates must be a CUDA tensor (the warp and the search run on the GPU)")
+    return cands.contiguous()
+
+
+def _warped_input(data, models, k, who):
+    """The substituted input of a rectified call (DESIGN.md §19), or of a rectification search with k candidates per
+    pair (§20), without a host sync: image0, and image1 of pair b warped onto image0's canvas through models[b * k + j]
+    for j < k ([n * k, 3, 3], `check_rectify`), with pair b's scale1 := scale0 and mask1 := mask0 for each of its k
+    candidates.  The scales and masks are checked first."""
+    from .preprocess import warp_images   # preprocess imports this module
+    if ("scale0" in data) != ("scale1" in data):
+        raise ValueError(f"{who}: give scale0 and scale1 together")
+    if ("mask0" in data) != ("mask1" in data):
+        raise ValueError(f"{who}: give mask0 and mask1 together")
+    img0, img1 = data["image0"], data["image1"]
+    want = (img1.shape[0], img1.shape[2] // 8, img1.shape[3] // 8)
+    if "mask1" in data and tuple(data["mask1"].shape) != want:
+        raise ValueError(f"{who}: mask1 must be [N, H1/8, W1/8] = {want} (got {tuple(data['mask1'].shape)})")
+
+    def rep(t):   # t[b] for each of pair b's k candidates (expand + copy: no host sync)
+        return t if k == 1 or t is None else t.unsqueeze(1).expand(t.shape[0], k, *t.shape[1:]).flatten(0, 1)
+
+    work = {"image0": img0, "image1": warp_images(rep(img1), models, img0.shape[2:], rep(data.get("scale0")),
+                                                  rep(data.get("scale1")))}
+    if "scale0" in data:
+        work["scale0"] = work["scale1"] = rep(data["scale0"])
+    if "mask0" in data:
+        work["mask0"] = work["mask1"] = rep(data["mask0"])
+    return work
+
+
 def _map_back(data, model, pts, ids, live=None, inside=True):
     """Points of the rectified frame back into image1 through each pair's model (lb_rectify_points, DESIGN.md §19),
     with the image sizes, scales and mask1 of the caller's `data`.  pts [m, 2] f32 (source pixels of image0's frame),
@@ -530,9 +582,14 @@ class CoarseMatching(nn.Module):
             per_pair = min(per_pair, max_per_pair)
         return max(n * per_pair, 1)
 
-    def run(self, hi, lo, ld, n, L, S, c, data, mask_u8_0=None, mask_u8_1=None, static=False, capacity=None):
+    def run(self, hi, lo, ld, n, L, S, c, data, mask_u8_0=None, mask_u8_1=None, static=False, capacity=None,
+            search=None):
         """Planes of feat_c0 (rows [0, n*L)) / feat_c1 (rows [n*L, ...)) -> coarse match keys in `data`.
         data["guide"] (optional, `check_guide`): guided matching through lb_coarse_match_guided (DESIGN.md §18).
+        search: None, or K (the rectification search, DESIGN.md §20): the n "pairs" are n / K pairs of K candidates
+        each, and lb_coarse_match_search keeps only each pair's winning candidate's matches.  It writes
+        data["rectify1_counts"] [n / K, K] int32 and data["rectify1_choice"] [n / K] int64; b_ids hold candidate ids and
+        the default capacity is the bound of n / K pairs.
         Eager (static=False): the lists are trimmed to the match count, read with one host sync.
         Static: no host sync; the match keys are buffers of `capacity` entries (default_capacity when None; entries at
         or past min(count, capacity) unspecified) and data["num_matches"] is the int32 device count [1].  Static needs
@@ -543,7 +600,8 @@ class CoarseMatching(nn.Module):
         if k is not None:
             _lib.require(_lib.MATCH_CAP_VERSION, "match_coarse.max_matches_per_pair")
         lib = _lib.load()
-        cap = int(capacity) if capacity is not None else self.default_capacity(n, L, S, mask_u8_0 is not None, k)
+        n_out = n if search is None else n // search   # pairs whose matches the list can hold
+        cap = int(capacity) if capacity is not None else self.default_capacity(n_out, L, S, mask_u8_0 is not None, k)
         dev = hi.device
         b_ids = torch.empty(cap, dtype=torch.int64, device=dev)
         i_ids = torch.empty(cap, dtype=torch.int64, device=dev)
@@ -562,7 +620,15 @@ class CoarseMatching(nn.Module):
             a.conf_matrix = conf.data_ptr()
         nbytes = lib.lb_coarse_match_workspace_bytes(n, L, S)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        if guide is not None:   # 0: no cap
+        if search is not None:   # 0: no cap
+            _lib.require_entries(_lib.SEARCH_ENTRIES, "the rectification search")
+            counts = torch.empty(n_out, search, dtype=torch.int32, device=dev)
+            choice = torch.empty(n_out, dtype=torch.int64, device=dev)
+            srch = _lib.LbCoarseSearch(search, counts.data_ptr(), choice.data_ptr())
+            _lib.check(lib.lb_coarse_match_search(C.byref(a), C.byref(srch), 0 if k is None else min(k, L),
+                                                  int(self._precision == "fp16"), ws.data_ptr(), nbytes, _stream(hi)))
+            data.update({"rectify1_counts": counts, "rectify1_choice": choice})
+        elif guide is not None:   # 0: no cap
             _lib.check(lib.lb_coarse_match_guided(C.byref(a), C.byref(guide), 0 if k is None else min(k, L),
                                                   int(self._precision == "fp16"), ws.data_ptr(), nbytes, _stream(hi)))
         elif self._precision == "fp16":   # 0: no cap
@@ -878,9 +944,22 @@ class LoFTR(nn.Module):
         warped onto image0's canvas through H (`warp_images`; scale1 := scale0, mask1 := mask0) and maps mkpts1_c /
         mkpts1_f back through H into image1; the new key minside1 [M] bool says whether mkpts1_f lies in image1's valid
         area.  expec_f, j_ids and hw1_* describe the rectified frame (image0's grid).  The caller's image1, scale1 and
-        mask1 are not replaced.  Not combinable with a guide."""
+        mask1 are not replaced.  Not combinable with a guide.
+
+        Optional rectify1_candidates (rectification search, DESIGN.md §20): float32 [N, K, 3, 3] on image0's device,
+        K >= 1 homographies per pair as rectify1, N * K <= 65535; `rotation_candidates` gives the four quarter turns.
+        Each pair is matched under every candidate (image0's backbone runs once), and only the candidate with the most
+        coarse matches (before max_matches_per_pair; ties to the smaller k) is kept, capped and refined.  New keys:
+        rectify1_choice [N] int64 (that k), rectify1_counts [N, K] int32 (the coarse match count of every candidate)
+        and minside1; every other key is that of a rectify1 call with the chosen candidate, b_ids / m_bids holding pair
+        ids (bs is N).  The outputs equal those of the rectified call on the N * K candidate pairs restricted to the
+        chosen ones, bit for bit with the tensor-core backbones; with K = 1 they are the rectify1 call's.  Not
+        combinable with rectify1 or a guide."""
         _require_eval(self)
         _require_cuda(data["image0"], "image0")
+        if data.get("rectify1_candidates") is not None:
+            self._match_searched(data, "forward")
+            return
         if data.get("rectify1") is not None:
             self._match_rectified(data, "forward")
             return
@@ -1031,7 +1110,9 @@ class LoFTR(nn.Module):
 
         data["guide"] (as in `forward`): its model must be on the device as well.  A captured graph bakes in the kind
         and the radius and reads the model from the same tensor at every replay.  data["rectify1"] (as in `forward`):
-        a captured graph reads it from the same tensor at every replay as well; minside1 is a capacity buffer too."""
+        a captured graph reads it from the same tensor at every replay as well; minside1 is a capacity buffer too.
+        data["rectify1_candidates"] (as in `forward`): read from the same tensor at every replay too; the default
+        capacity is the bound of the N pairs, since only the winning candidates' matches are listed."""
         _require_static(self, capacity, "forward_static")
         dev = None
         for k in ("image0", "image1", "mask0", "mask1", "scale0", "scale1"):
@@ -1045,6 +1126,9 @@ class LoFTR(nn.Module):
                 dev = t.device
             elif t.device != dev:
                 raise ValueError(f"forward_static: `{k}` is on {t.device}, image0 on {dev}")
+        if data.get("rectify1_candidates") is not None:
+            self._match_searched(data, "forward_static", static=True, capacity=capacity)
+            return
         if data.get("rectify1") is not None:
             self._match_rectified(data, "forward_static", static=True, capacity=capacity)
             return
@@ -1057,25 +1141,11 @@ class LoFTR(nn.Module):
         """The substituted input of a call with data["rectify1"] (DESIGN.md §19), validated before any launch and
         without a host sync -> (work dict: image0, image1 warped onto image0's canvas, scale1 := scale0 and mask1 :=
         mask0 when given; the model as `check_rectify` returns it)."""
-        from .preprocess import warp_images   # preprocess imports this module
         if data.get("guide") is not None:
             raise ValueError(f"{who}: data['rectify1'] cannot be combined with data['guide']")
-        img0, img1 = data["image0"], data["image1"]
+        img0 = data["image0"]
         model = check_rectify(data["rectify1"], img0.shape[0], img0.device, who)
-        if ("scale0" in data) != ("scale1" in data):
-            raise ValueError(f"{who}: give scale0 and scale1 together")
-        if ("mask0" in data) != ("mask1" in data):
-            raise ValueError(f"{who}: give mask0 and mask1 together")
-        want = (img1.shape[0], img1.shape[2] // 8, img1.shape[3] // 8)
-        if "mask1" in data and tuple(data["mask1"].shape) != want:
-            raise ValueError(f"{who}: mask1 must be [N, H1/8, W1/8] = {want} (got {tuple(data['mask1'].shape)})")
-        work = {"image0": img0,
-                "image1": warp_images(img1, model, img0.shape[2:], data.get("scale0"), data.get("scale1"))}
-        if "scale0" in data:
-            work["scale0"] = work["scale1"] = data["scale0"]
-        if "mask0" in data:
-            work["mask0"] = work["mask1"] = data["mask0"]
-        return work, model
+        return _warped_input(data, model, 1, who), model
 
     def _match_rectified(self, data, who, static=False, capacity=None):
         """forward / forward_static with data["rectify1"]: the call on the substituted input, then mkpts1_c / mkpts1_f
@@ -1086,6 +1156,38 @@ class LoFTR(nn.Module):
         work["mkpts1_c"], _ = _map_back(data, model, work["mkpts1_c"], ids, live, inside=False)
         work["mkpts1_f"], work["minside1"] = _map_back(data, model, work["mkpts1_f"], ids, live)
         data.update({k: v for k, v in work.items() if k not in _INPUT_KEYS})
+
+    def _match_searched(self, data, who, static=False, capacity=None):
+        """forward / forward_static with data["rectify1_candidates"] (DESIGN.md §20), without a host sync beyond the
+        eager call's one: image0's backbone once, the warped image1 of all N * K candidates, the coarse stage with the
+        search (CoarseMatching.run), the fine stage over the winners' matches in candidate space; then pair ids and
+        mkpts1_c / mkpts1_f mapped back through the chosen candidates.  The caller's inputs stay."""
+        for key in ("rectify1", "guide"):
+            if data.get(key) is not None:
+                raise ValueError(f"{who}: data['rectify1_candidates'] cannot be combined with data['{key}']")
+        img0 = data["image0"]
+        cands = check_rectify_candidates(data["rectify1_candidates"], img0.shape[0], img0.device, who)
+        n, k = cands.shape[:2]
+        work = _warped_input(data, cands.view(n * k, 3, 3), k, who)
+        (feat_c0, feat_f0), (feat_c1, feat_f1) = self._backbone(img0), self._backbone(work["image1"])
+        work.update({"bs": n * k, "hw0_i": img0.shape[2:], "hw1_i": img0.shape[2:], "hw0_c": feat_c0.shape[2:],
+                     "hw1_c": feat_c1.shape[2:], "hw0_f": feat_f0.shape[2:], "hw1_f": feat_f1.shape[2:]})
+        cand = torch.arange(n * k, dtype=torch.int32, device=img0.device)   # candidate c = b * K + k reads image0[b]
+        self._match_pairs(work, feat_c0, feat_c1, feat_f0, feat_f1, img_idx=(cand // k, cand), static=static,
+                          capacity=capacity, search=k)
+        pair = torch.arange(n, device=img0.device)
+        chosen = cands[pair, work["rectify1_choice"]]
+        work["b_ids"].div_(k, rounding_mode="floor")   # candidate ids -> pair ids
+        if work["m_bids"] is not work["b_ids"]:   # a list of its own only when thr < 0
+            work["m_bids"].div_(k, rounding_mode="floor")
+        live, ids = work.get("num_matches"), work["m_bids"]
+        work["mkpts1_c"], _ = _map_back(data, chosen, work["mkpts1_c"], ids, live, inside=False)
+        work["mkpts1_f"], work["minside1"] = _map_back(data, chosen, work["mkpts1_f"], ids, live)
+        if "conf_matrix" in work:
+            work["conf_matrix"] = work["conf_matrix"].view(n, k, *work["conf_matrix"].shape[1:])[
+                pair, work["rectify1_choice"]]
+        work["bs"] = n
+        data.update({key: v for key, v in work.items() if key not in _INPUT_KEYS})
 
     @torch.no_grad()
     def match_points(self, data, points0, valid0=None):
@@ -1114,6 +1216,9 @@ class LoFTR(nn.Module):
         if data.get("guide") is not None:
             raise ValueError("match_points: data['guide'] is not supported (guided matching is available in forward, "
                              "forward_static and match_features)")
+        if data.get("rectify1_candidates") is not None:
+            raise ValueError("match_points: data['rectify1_candidates'] is not supported (the rectification search is "
+                             "available in forward and forward_static; pass the chosen model as data['rectify1'])")
         _lib.require_entries(_lib.POINTS_ENTRIES, "match_points")
         _check_points(data, points0, valid0)
         if data.get("rectify1") is None:
@@ -1174,19 +1279,22 @@ class LoFTR(nn.Module):
                      "hw0_f": feat_f0.shape[2:], "hw1_f": feat_f1.shape[2:]})
         return feat_c0, feat_c1, feat_f0, feat_f1
 
-    def _match_pairs(self, data, feat_c0, feat_c1, feat_f0, feat_f1, img_idx=None, static=False, capacity=None):
+    def _match_pairs(self, data, feat_c0, feat_c1, feat_f0, feat_f1, img_idx=None, static=False, capacity=None,
+                     search=None):
         """Steps 2-5 of the forward for the data["bs"] pairs whose sizes `data` holds: position encoding and token
         layout, coarse transformer, coarse matching, fine preprocess and transformer, fine matching.
         img_idx: optional (idx0, idx1) int32 [bs]: the maps are then feature banks, read at image idx0[b] / idx1[b] for
         pair b.  static: the match keys are buffers of `capacity` entries (None: the default capacity) and the fine
-        stage is bounded on the device by their count (CoarseMatching.run), so that nothing synchronises with the host."""
+        stage is bounded on the device by their count (CoarseMatching.run), so that nothing synchronises with the host.
+        search: None, or K: the bs pairs are candidates of a rectification search (CoarseMatching.run)."""
         bs, c = data["bs"], feat_c0.shape[1]
         (h0, w0), (h1, w1) = data["hw0_c"], data["hw1_c"]
         L, S = h0 * w0, h1 * w1
         state, m0, m1 = self._coarse_tokens(data, feat_c0, feat_c1, img_idx)
 
         # 3. coarse matching                                                           [loftr.py:67]
-        live = self.coarse_matching.run(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1, static, capacity)
+        live = self.coarse_matching.run(state.cat_hi, state.cat_lo, 2 * c, bs, L, S, c, data, m0, m1, static, capacity,
+                                        search)
 
         # 4. fine-level refinement over M windows: the match count, or the capacity    [loftr.py:70-72]
         fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, bs, L, S, data, live, img_idx)
@@ -1406,7 +1514,7 @@ class CapturedMatcher:
                                "invalidate_packed() or a parameter update); call recapture()")
 
     def __call__(self, data):
-        for k, what in (("guide", "a guide"), ("rectify1", "rectify1")):
+        for k, what in (("guide", "a guide"), ("rectify1", "rectify1"), ("rectify1_candidates", "rectify1_candidates")):
             if data.get(k) is not None:
                 raise ValueError(f"CapturedMatcher: data['{k}'] is not supported (capture LoFTR.forward_static with "
                                  f"{what} instead)")

@@ -293,3 +293,49 @@ def warp_images(images1, model, hw, scale0=None, scale1=None):
                                              model.data_ptr(), _lib.ptr(scales[0]), _lib.ptr(scales[1]),
                                              out.data_ptr(), H, W, _stream(images1)))
     return out
+
+
+def rotation_candidates(size0, size1, scale0=None, scale1=None):
+    """The four quarter turns of image1 relative to image0, as data["rectify1_candidates"] of a rectification search
+    (DESIGN.md §20): for a camera rolled by an unknown multiple of 90 degrees.  Torch operations on size0's device, no
+    host sync.
+
+    size0 / size1: [N, 2] valid (w, h) of image0 / image1 in network pixels (`PreparedImages.size`, or the canvas).
+    scale0 / scale1: optional [N, 2] scales of image0 / image1 (both or neither), as forward's.
+    -> float32 [N, 4, 3, 3]: candidate q is H_q = S1 T(c1) R^q T(-c0) S0^-1, formed in float64, with c = ((w - 1) / 2,
+    (h - 1) / 2) of each image, R = [[0, 1], [-1, 0]] and S = diag(sx, sy, 1) (the identity without scales).  Without
+    scales, image1 = torch.rot90(image0, q, dims=(-2, -1)) warped through candidate q (`warp_images`) is image0 bit
+    for bit, for square and non-square images alike."""
+    sizes = []
+    for name, s in (("size0", size0), ("size1", size1)):
+        if not torch.is_tensor(s) or s.dim() != 2 or s.shape[1] != 2 or s.dtype == torch.bool or s.is_complex():
+            raise ValueError(f"rotation_candidates: {name} must be a real tensor [N, 2] of (w, h) (got "
+                             f"{tuple(s.shape) if torch.is_tensor(s) else type(s).__name__})")
+        sizes.append(s)
+    n, dev = size0.shape[0], size0.device
+    if size1.shape[0] != n:
+        raise ValueError(f"rotation_candidates: size0 and size1 must have the same N (got {n} and {size1.shape[0]})")
+    if (scale0 is None) != (scale1 is None):
+        raise ValueError("rotation_candidates: give scale0 and scale1 together")
+    f64 = torch.float64
+    if scale0 is None:
+        scale0 = scale1 = torch.ones(n, 2, dtype=f64, device=dev)
+    for name, s in (("scale0", scale0), ("scale1", scale1)):
+        if not torch.is_tensor(s) or tuple(s.shape) != (n, 2):
+            raise ValueError(f"rotation_candidates: {name} must be a tensor [N, 2] with N = {n}")
+    one = torch.ones(n, 1, dtype=f64, device=dev)
+
+    def shift(c):   # T(c) [N, 3, 3]
+        t = torch.eye(3, dtype=f64, device=dev).repeat(n, 1, 1)
+        t[:, :2, 2] = c
+        return t
+
+    c0, c1 = ((s.to(dev, f64) - 1) / 2 for s in sizes)
+    s0_inv = torch.diag_embed(torch.cat([1 / scale0.to(dev, f64), one], 1))
+    s1 = torch.diag_embed(torch.cat([scale1.to(dev, f64), one], 1))
+    q = torch.arange(4, dtype=f64, device=dev)
+    cos, sin = (1 - q % 2) * (1 - q), (q % 2) * (2 - q)   # (1, 0, -1, 0), (0, 1, 0, -1): R^q, exactly
+    r = torch.zeros(4, 3, 3, dtype=f64, device=dev)
+    r[:, 0, 0], r[:, 0, 1], r[:, 1, 0], r[:, 1, 1], r[:, 2, 2] = cos, sin, -sin, cos, 1
+    h = (s1 @ shift(c1))[:, None] @ r[None] @ (shift(-c0) @ s0_inv)[:, None]
+    return (h + 0.0).float().contiguous()   # + 0.0: no negative zeros
