@@ -64,7 +64,8 @@ extern "C" {
  * lb_coarse_query / lb_fine_preprocess_centres (matching caller-given image0 points);
  * lb_coarse_match_guided (coarse matching restricted to a band around a homography or fundamental matrix);
  * lb_rectify_images / lb_rectify_points (image1 warped into image0's frame through a homography, matches mapped back);
- * lb_coarse_match_search (coarse matching of K candidate warps per pair, keeping the best candidate's matches). */
+ * lb_coarse_match_search (coarse matching of K candidate warps per pair, keeping the best candidate's matches);
+ * lb_coarse_query_guided / lb_fine_preprocess_centres_indexed (caller-given points on bank pairs, with a guide). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -397,6 +398,14 @@ typedef struct LbCoarseQueryArgs {
  * flag pass (timing tag "match_query"), no per-pair cap and no compaction. */
 int lb_coarse_query(const LbCoarseMatchArgs* args /*host*/, const LbCoarseQueryArgs* query /*host*/,
                     int operand_planes, void* ws, size_t ws_bytes, void* stream);
+/* lb_coarse_query on the guided coarse quantities of lb_coarse_match_guided (found by name; DESIGN.md §21): every
+ * score pass takes the guide's predicate, so j is the row arg-max over the admissible cells of the query's row, valid
+ * is lb_coarse_match_guided's flag test and a row without an admissible, unmasked column has no answer (not inside).
+ * Errors: those of lb_coarse_query, and a NULL guide or model, an unknown kind or a radius that is not finite and
+ * positive, as lb_coarse_match_guided.  Same workspace as lb_coarse_match. */
+int lb_coarse_query_guided(const LbCoarseMatchArgs* args /*host*/, const LbCoarseQueryArgs* query /*host*/,
+                           const LbCoarseGuide* guide /*host*/, int operand_planes, void* ws, size_t ws_bytes,
+                           void* stream);
 
 typedef struct LbFinePreprocessArgs {
   const float* feat_f0;   /* fine maps, any strides (elements): index = n*sn + c*sc + y*sh + x*sw */
@@ -443,6 +452,13 @@ int lb_fine_preprocess_indexed(const LbFinePreprocessArgs* args /*host*/, const 
  * must be in range for every m.  M_live must be NULL.  Same workspace as lb_fine_preprocess. */
 int lb_fine_preprocess_centres(const LbFinePreprocessArgs* args /*host*/, const int* centres, const uint8_t* inside,
                                void* ws, size_t ws_bytes, void* stream);
+/* lb_fine_preprocess_centres with feat_f0 / feat_f1 holding feature banks, read as lb_fine_preprocess_indexed reads
+ * them: pair b's windows come from image img_idx0[b] of feat_f0 and img_idx1[b] of feat_f1, centred on the table's
+ * fine pixels (found by name; DESIGN.md §21).  Errors: NULL centres, inside, img_idx0 or img_idx1 with M > 0, and a
+ * non-NULL M_live.  Same workspace as lb_fine_preprocess. */
+int lb_fine_preprocess_centres_indexed(const LbFinePreprocessArgs* args /*host*/, const int* centres,
+                                       const uint8_t* inside, const int* img_idx0, const int* img_idx1, void* ws,
+                                       size_t ws_bytes, void* stream);
 
 typedef struct LbFineMatchArgs {
   const float* f0;        /* [M*W*W, C] fine transformer output, window side 0 */

@@ -1532,6 +1532,55 @@ static int coarse_match(const LbCoarseMatchArgs* a, int max_per_pair, const Guid
   return 0;
 }
 
+// The guide of a guided entry (`who`), checked -> gp with the coarse keypoints' scales of `a`.
+static int guide_params(const char* who, const LbCoarseMatchArgs* a, const LbCoarseGuide* g, GuideParams& gp) {
+  if (!g || !g->model) return fail("%s: the guide model is null", who);
+  if (g->kind != LB_GUIDE_HOMOGRAPHY && g->kind != LB_GUIDE_FUNDAMENTAL)
+    return fail("%s: unknown guide kind %d", who, g->kind);
+  if (!std::isfinite(g->radius) || !(g->radius > 0.f))
+    return fail("%s: the radius must be finite and positive (got %g)", who, g->radius);
+  gp = GuideParams{g->kind, g->model, g->radius, a->img_scale, a->scale0, a->scale1, a->w0c, a->w1c};
+  return 0;
+}
+
+// lb_coarse_query (guide NULL) and lb_coarse_query_guided: the coarse rows, unguided or under `guide`, then
+// coarse_query_kernel on them.  `who` names the entry in the messages.
+static int coarse_query(const char* who, const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q,
+                        const GuideParams* guide, int operand_planes, void* ws, size_t ws_bytes, void* stream) {
+  if (q->Q <= 0 || a->n_pairs <= 0) return 0;
+  DeviceScope dev;
+  LB_TRY(dev.bind(q->i_ids));
+  if (!q->points0) return fail("%s: points0 is null", who);
+  if (q->stride <= 0 || q->fine_scale <= 0.f || q->Hf0 <= 0 || q->Wf0 <= 0)
+    return fail("%s: bad fine grid (stride %d, fine_scale %g, %d x %d)", who, q->stride, q->fine_scale, q->Hf0,
+                q->Wf0);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CmWs w;
+  SelectParams sp;
+  if (guide) {
+    LB_TRY((operand_planes == 2 ? coarse_rows<2, true>(a, guide, dev, ws, ws_bytes, st, w, sp)
+                                : coarse_rows<1, true>(a, guide, dev, ws, ws_bytes, st, w, sp)));
+  } else {
+    LB_TRY((operand_planes == 2 ? coarse_rows<2, false>(a, nullptr, dev, ws, ws_bytes, st, w, sp)
+                                : coarse_rows<1, false>(a, nullptr, dev, ws, ws_bytes, st, w, sp)));
+  }
+  QueryParams qp;
+  qp.n_pairs = a->n_pairs; qp.Q = q->Q; qp.L = a->L; qp.S = a->S;
+  qp.h0c = a->h0c; qp.w0c = a->w0c; qp.w1c = a->w1c;
+  qp.H0 = q->H0; qp.W0 = q->W0; qp.Hf0 = q->Hf0; qp.Wf0 = q->Wf0;
+  qp.stride = q->stride; qp.s_c = a->img_scale; qp.s_f = q->fine_scale;
+  qp.conf_bias = sp.conf_bias;
+  qp.points0 = q->points0; qp.valid0 = q->valid0;
+  qp.scale0 = a->scale0; qp.scale1 = a->scale1; qp.mask0 = a->mask0;
+  qp.row_key = sp.row_key; qp.row_arg = sp.row_arg; qp.col_arg = sp.col_arg; qp.rowterm = sp.rowterm;
+  qp.flag = sp.flag;
+  qp.i_ids = q->i_ids; qp.j_ids = q->j_ids; qp.conf = q->conf;
+  qp.mutual = q->mutual; qp.valid = q->valid; qp.inside = q->inside;
+  qp.centres = q->centres; qp.win = q->win_ids; qp.pts0_f = q->pts0_f; qp.pts1_c = q->pts1_c;
+  const long nq = static_cast<long>(a->n_pairs) * q->Q;
+  return launch(TAG_MATCH_QUERY, coarse_query_kernel, cdiv(nq, 256), 256, 0, st, qp);
+}
+
 extern "C" {
 
 int lb_coarse_match(const LbCoarseMatchArgs* a, void* ws, size_t ws_bytes, void* stream) {
@@ -1550,15 +1599,11 @@ int lb_coarse_match_fp16(const LbCoarseMatchArgs* a, int max_per_pair, void* ws,
 
 int lb_coarse_match_guided(const LbCoarseMatchArgs* a, const LbCoarseGuide* g, int max_per_pair, int fp16, void* ws,
                            size_t ws_bytes, void* stream) {
-  if (!g || !g->model) return fail("lb_coarse_match_guided: the guide model is null");
-  if (g->kind != LB_GUIDE_HOMOGRAPHY && g->kind != LB_GUIDE_FUNDAMENTAL)
-    return fail("lb_coarse_match_guided: unknown guide kind %d", g->kind);
-  if (!std::isfinite(g->radius) || !(g->radius > 0.f))
-    return fail("lb_coarse_match_guided: the radius must be finite and positive (got %g)", g->radius);
+  GuideParams gp;
+  LB_TRY(guide_params("lb_coarse_match_guided", a, g, gp));
   if (max_per_pair < 0)
     return fail("lb_coarse_match_guided: max_per_pair must be 0 (no cap) or at least 1 (got %d)", max_per_pair);
   if (fp16 != 0 && fp16 != 1) return fail("lb_coarse_match_guided: fp16 must be 0 (split) or 1 (got %d)", fp16);
-  const GuideParams gp{g->kind, g->model, g->radius, a->img_scale, a->scale0, a->scale1, a->w0c, a->w1c};
   return fp16 ? coarse_match<1>(a, max_per_pair, &gp, ws, ws_bytes, stream)
               : coarse_match<2>(a, max_per_pair, &gp, ws, ws_bytes, stream);
 }
@@ -1581,33 +1626,16 @@ int lb_coarse_query(const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, int 
                     size_t ws_bytes, void* stream) {
   if (operand_planes != 1 && operand_planes != 2)
     return fail("lb_coarse_query: operand_planes must be 1 (fp16) or 2 (split) (got %d)", operand_planes);
-  if (q->Q <= 0 || a->n_pairs <= 0) return 0;
-  DeviceScope dev;
-  LB_TRY(dev.bind(q->i_ids));
-  if (!q->points0) return fail("lb_coarse_query: points0 is null");
-  if (q->stride <= 0 || q->fine_scale <= 0.f || q->Hf0 <= 0 || q->Wf0 <= 0)
-    return fail("lb_coarse_query: bad fine grid (stride %d, fine_scale %g, %d x %d)", q->stride, q->fine_scale, q->Hf0,
-                q->Wf0);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CmWs w;
-  SelectParams sp;
-  LB_TRY((operand_planes == 2 ? coarse_rows<2, false>(a, nullptr, dev, ws, ws_bytes, st, w, sp)
-                              : coarse_rows<1, false>(a, nullptr, dev, ws, ws_bytes, st, w, sp)));
-  QueryParams qp;
-  qp.n_pairs = a->n_pairs; qp.Q = q->Q; qp.L = a->L; qp.S = a->S;
-  qp.h0c = a->h0c; qp.w0c = a->w0c; qp.w1c = a->w1c;
-  qp.H0 = q->H0; qp.W0 = q->W0; qp.Hf0 = q->Hf0; qp.Wf0 = q->Wf0;
-  qp.stride = q->stride; qp.s_c = a->img_scale; qp.s_f = q->fine_scale;
-  qp.conf_bias = sp.conf_bias;
-  qp.points0 = q->points0; qp.valid0 = q->valid0;
-  qp.scale0 = a->scale0; qp.scale1 = a->scale1; qp.mask0 = a->mask0;
-  qp.row_key = sp.row_key; qp.row_arg = sp.row_arg; qp.col_arg = sp.col_arg; qp.rowterm = sp.rowterm;
-  qp.flag = sp.flag;
-  qp.i_ids = q->i_ids; qp.j_ids = q->j_ids; qp.conf = q->conf;
-  qp.mutual = q->mutual; qp.valid = q->valid; qp.inside = q->inside;
-  qp.centres = q->centres; qp.win = q->win_ids; qp.pts0_f = q->pts0_f; qp.pts1_c = q->pts1_c;
-  const long nq = static_cast<long>(a->n_pairs) * q->Q;
-  return launch(TAG_MATCH_QUERY, coarse_query_kernel, cdiv(nq, 256), 256, 0, st, qp);
+  return coarse_query("lb_coarse_query", a, q, nullptr, operand_planes, ws, ws_bytes, stream);
+}
+
+int lb_coarse_query_guided(const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, const LbCoarseGuide* g,
+                           int operand_planes, void* ws, size_t ws_bytes, void* stream) {
+  if (operand_planes != 1 && operand_planes != 2)
+    return fail("lb_coarse_query_guided: operand_planes must be 1 (fp16) or 2 (split) (got %d)", operand_planes);
+  GuideParams gp;
+  LB_TRY(guide_params("lb_coarse_query_guided", a, g, gp));
+  return coarse_query("lb_coarse_query_guided", a, q, &gp, operand_planes, ws, ws_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ fine level
@@ -1631,7 +1659,8 @@ size_t lb_fine_preprocess_workspace_bytes(long M, int W, int Cf) {
 }
 
 // img_idx0 / img_idx1: NULL, or pair b's windows are read from image img_idx0[b] of feat_f0 / img_idx1[b] of feat_f1.
-// centres / inside: NULL, or the window centres come from the centre table (lb_fine_preprocess_centres).
+// centres / inside: NULL, or the window centres come from the centre table (lb_fine_preprocess_centres); with img_idx0
+// as well, from the table on bank images (lb_fine_preprocess_centres_indexed).
 static int fine_preprocess(const LbFinePreprocessArgs* a, const int* img_idx0, const int* img_idx1, const int* centres,
                            const uint8_t* inside, void* ws, size_t ws_bytes, void* stream) {
   if (a->M <= 0) return 0;
@@ -1662,9 +1691,10 @@ static int fine_preprocess(const LbFinePreprocessArgs* a, const int* img_idx0, c
                     a->sh0 % 4 == 0 && a->sh1 % 4 == 0 && a->sn0 % 4 == 0 && a->sn1 % 4 == 0 &&
                     (reinterpret_cast<uintptr_t>(a->feat_f0) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->feat_f1) & 15) == 0;
   const unsigned wins = static_cast<unsigned>(2 * a->M);
-  const auto gather = centres    ? (vec8 ? fine_gather_vec8_kernel<false, true> : fine_gather_kernel<false, true>)
-                      : img_idx0 ? (vec8 ? fine_gather_vec8_kernel<true> : fine_gather_kernel<true>)
-                                 : (vec8 ? fine_gather_vec8_kernel<false> : fine_gather_kernel<false>);
+  const auto gather = centres && img_idx0 ? (vec8 ? fine_gather_vec8_kernel<true, true> : fine_gather_kernel<true, true>)
+                      : centres          ? (vec8 ? fine_gather_vec8_kernel<false, true> : fine_gather_kernel<false, true>)
+                      : img_idx0         ? (vec8 ? fine_gather_vec8_kernel<true> : fine_gather_kernel<true>)
+                                         : (vec8 ? fine_gather_vec8_kernel<false> : fine_gather_kernel<false>);
   LB_TRY(launch(TAG_NONE, gather, wins, 256, 0, st, g));
 
   FineBiasParams fb;
@@ -1706,6 +1736,15 @@ int lb_fine_preprocess_centres(const LbFinePreprocessArgs* a, const int* centres
   if (a->M > 0 && (!centres || !inside)) return fail("lb_fine_preprocess_centres: centres and inside are required");
   if (a->M_live) return fail("lb_fine_preprocess_centres: M_live is not supported (every query has a window)");
   return fine_preprocess(a, nullptr, nullptr, centres, inside, ws, ws_bytes, stream);
+}
+
+int lb_fine_preprocess_centres_indexed(const LbFinePreprocessArgs* a, const int* centres, const uint8_t* inside,
+                                       const int* img_idx0, const int* img_idx1, void* ws, size_t ws_bytes,
+                                       void* stream) {
+  if (a->M > 0 && (!centres || !inside || !img_idx0 || !img_idx1))
+    return fail("lb_fine_preprocess_centres_indexed: centres, inside, img_idx0 and img_idx1 are required");
+  if (a->M_live) return fail("lb_fine_preprocess_centres_indexed: M_live is not supported (every query has a window)");
+  return fine_preprocess(a, img_idx0, img_idx1, centres, inside, ws, ws_bytes, stream);
 }
 
 int lb_fine_match(const LbFineMatchArgs* a, void* stream) {

@@ -694,6 +694,8 @@ class CoarseMatching(nn.Module):
     def query(self, hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1, points0, valid0=None):
         """The coarse stage for caller-given image0 points (LoFTR.match_points, DESIGN.md §17): planes as `run`,
         points0 [n, Q, 2] f32 and valid0 (None or bool [n, Q]) on the device, validated by the caller.  No host sync.
+        data["guide"] (optional, `check_guide`): the queries are answered on the guided coarse quantities through
+        lb_coarse_query_guided (DESIGN.md §21).
         -> dict of the per-query outputs (q_i_ids, q_j_ids, qconf, qmutual, qvalid, qinside [n, Q]; qpts0_f, qpts1_c
         [n, Q, 2]) and of what the fine stage reads: "centres" int32 [2, n*Q, 2] and "win_ids" int64 [3, n*Q].
         The per-pair cap (max_matches_per_pair) is not applied."""
@@ -713,7 +715,7 @@ class CoarseMatching(nn.Module):
                "qpts1_c": torch.empty(n, q, 2, dtype=torch.float32, device=dev),
                "centres": torch.empty(2, nq, 2, dtype=torch.int32, device=dev),
                "win_ids": torch.empty(3, nq, dtype=torch.int64, device=dev)}
-        a, keep, _ = self._args(hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1)
+        a, keep, guide = self._args(hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1)
         qa = _lib.LbCoarseQueryArgs()
         points0 = points0.contiguous()
         keep.append(points0)
@@ -731,8 +733,13 @@ class CoarseMatching(nn.Module):
         qa.pts0_f, qa.pts1_c = out["qpts0_f"].data_ptr(), out["qpts1_c"].data_ptr()
         nbytes = lib.lb_coarse_match_workspace_bytes(n, L, S)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        _lib.check(lib.lb_coarse_query(C.byref(a), C.byref(qa), 1 if self._precision == "fp16" else 2, ws.data_ptr(),
-                                       nbytes, _stream(hi)))
+        planes = 1 if self._precision == "fp16" else 2
+        if guide is not None:
+            _lib.require_entries(_lib.BANK_POINTS_ENTRIES, "guided point queries")
+            _lib.check(lib.lb_coarse_query_guided(C.byref(a), C.byref(qa), C.byref(guide), planes, ws.data_ptr(),
+                                                  nbytes, _stream(hi)))
+        else:
+            _lib.check(lib.lb_coarse_query(C.byref(a), C.byref(qa), planes, ws.data_ptr(), nbytes, _stream(hi)))
         return out
 
     @torch.no_grad()
@@ -784,7 +791,8 @@ class FinePreprocess(_PackedCache, nn.Module):
         `img_idx`: (idx0, idx1) int32 device tensors [n]: feat_f0 / feat_f1 are then feature banks and pair b's
         windows are read from their images idx0[b] / idx1[b].
         `centres`: (centres, inside) of CoarseMatching.query: the windows are centred on the fine pixels of the int32
-        table [2, M, 2] rather than on the cells of i_ids / j_ids, and windows m with inside[m] false are zeros."""
+        table [2, M, 2] rather than on the cells of i_ids / j_ids, and windows m with inside[m] false are zeros.  With
+        `img_idx` as well, they are read from the banks' images (lb_fine_preprocess_centres_indexed)."""
         lib = _lib.load()
         W = self.W
         stride = data["hw0_f"][0] // data["hw0_c"][0]
@@ -813,7 +821,11 @@ class FinePreprocess(_PackedCache, nn.Module):
         a.M_live = _lib.ptr(live)
         nbytes = lib.lb_fine_preprocess_workspace_bytes(m, W, cf)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        if centres is not None:
+        if centres is not None and img_idx is not None:
+            _lib.check(lib.lb_fine_preprocess_centres_indexed(
+                C.byref(a), centres[0].data_ptr(), centres[1].data_ptr(), img_idx[0].data_ptr(), img_idx[1].data_ptr(),
+                ws.data_ptr(), nbytes, _stream(feat_f0)))
+        elif centres is not None:
             _lib.check(lib.lb_fine_preprocess_centres(C.byref(a), centres[0].data_ptr(), centres[1].data_ptr(),
                                                       ws.data_ptr(), nbytes, _stream(feat_f0)))
         elif img_idx is None:
@@ -1020,36 +1032,14 @@ class LoFTR(nn.Module):
                                  "estimate_geometry options (model, threshold, iterations, seed)")
             geom = dict(zip(("model", "threshold", "iterations", "seed"), geometry.check_options(**opts)))
             _lib.require(_lib.GEOMETRY_VERSION, "match_features(estimate=...)")
-        key = self._bank_key()
-        dev = next(self.parameters()).device
-        for name, f in (("feats0", feats0), ("feats1", feats1)):
-            if not isinstance(f, ImageFeatures):
-                raise TypeError(f"match_features: `{name}` must be the ImageFeatures of extract_features")
-            if f.weights_key != key:
-                raise RuntimeError(f"match_features: `{name}` was extracted with other backbone weights (load_state_dict, "
-                                   ".to() or a parameter update since); extract the features again")
-        idx0 = self._pair_index(idx0, "idx0", len(feats0), dev)
-        idx1 = self._pair_index(idx1, "idx1", len(feats1), dev)
-        if idx0.shape != idx1.shape:
-            raise ValueError(f"match_features: idx0 and idx1 must have the same length ({idx0.numel()} vs {idx1.numel()})")
-        if (feats0.mask is None) != (feats1.mask is None):
-            raise ValueError("match_features: either both banks carry masks or neither (as mask0 / mask1 of forward)")
-        if (scale0 is None) != (scale1 is None):
-            raise ValueError("match_features: give scale0 and scale1 together")
+        idx0, idx1, dev = self._check_banks(feats0, idx0, feats1, idx1, scale0, scale1, "match_features")
         bs = idx0.numel()
         work = {}   # forward's inputs for this pair list (masks, scales, guide), then every key forward writes
         if guide is not None:
             check_guide(guide, bs, dev, self.coarse_matching.thr, "match_features")
             work["guide"] = guide
-        if feats0.mask is not None:
-            work["mask0"], work["mask1"] = feats0.mask[idx0.long()], feats1.mask[idx1.long()]
-        if scale0 is not None:
-            for name, s, f, idx in (("scale0", scale0, feats0, idx0), ("scale1", scale1, feats1, idx1)):
-                if tuple(s.shape) != (len(f), 2):
-                    raise ValueError(f"match_features: {name} must be [{len(f)}, 2] (got {tuple(s.shape)})")
-                work[name] = s.to(dev)[idx.long()]
-        work.update({"bs": bs, "hw0_i": feats0.hw_i, "hw1_i": feats1.hw_i, "hw0_c": feats0.hw_c, "hw1_c": feats1.hw_c,
-                     "hw0_f": feats0.hw_f, "hw1_f": feats1.hw_f})
+        work.update(_bank_inputs(feats0, idx0, feats1, idx1, scale0, scale1, dev, "match_features"))
+        work.update(_bank_sizes(bs, feats0, feats1))
         self._match_pairs(work, feats0.feat_c, feats1.feat_c, feats0.feat_f, feats1.feat_f, img_idx=(idx0, idx1))
         if geom is not None:
             (h0, w0), (h1, w1) = feats0.hw_c, feats1.hw_c
@@ -1060,20 +1050,86 @@ class LoFTR(nn.Module):
         out.update({k: v for k, v in work.items() if k not in ("mask0", "mask1", "scale0", "scale1", "guide")})
         return out
 
+    @torch.no_grad()
+    def match_points_features(self, feats0, idx0, feats1, idx1, points0, valid0=None, scale0=None, scale1=None,
+                              data=None, guide=None):
+        """`match_points` on pairs drawn from feature banks (DESIGN.md §21): pair b is image idx0[b] of feats0 against
+        image idx1[b] of feats1, as in `match_features` (feats1 may be feats0; the banks' masks and the per-image
+        scales scale0 [K0, 2] / scale1 [K1, 2] are gathered through the indices).  The backbone does not run again, so
+        a sequence of frames, or one reference image tracked into many, pays for each image once.
+
+        points0: float32 [B, Q, 2] and valid0: optional bool [B, Q], one row per entry of the pair list, as in
+        `match_points` (source pixels when scales are given).  Writes into `data` (a new dict when None) and returns it:
+        the keys, dtypes and values `match_points` writes for the stacked batch image0 = images idx0 of feats0, image1 =
+        images idx1 of feats1, bit for bit with the tensor-core backbones.
+
+        guide: None, or `match_features`' guide ("model" [B, 3, 3] in pair-list order; a NaN model leaves its pair
+        unguided).  The queries are then answered on the guided coarse quantities of DESIGN.md §18: j is the row
+        arg-max over the admissible cells, qvalid is the guided flag test, and a row without an admissible, unmasked
+        column is not inside.  A query at a guided `match_features` match's mkpts0_c returns that match bit for bit.
+
+        An empty pair list or Q = 0 gives empty outputs and launches nothing.  The one host sync is the index range
+        check of `match_features`."""
+        who = "match_points_features"
+        _require_eval(self)
+        _lib.require(_lib.FEATURE_BANK_VERSION, who)
+        _lib.require_entries(_lib.POINTS_ENTRIES + _lib.BANK_POINTS_ENTRIES, who)
+        idx0, idx1, dev = self._check_banks(feats0, idx0, feats1, idx1, scale0, scale1, who)
+        bs = idx0.numel()
+        _check_query_args(points0, valid0, bs, who)
+        _check_devices([("points0", points0)] + ([("valid0", valid0)] if valid0 is not None else []), dev, "the model",
+                       who)
+        work = {}   # match_points' inputs for this pair list (masks, scales, guide), then every key it writes
+        if guide is not None:
+            check_guide(guide, bs, dev, self.coarse_matching.thr, who)
+            work["guide"] = guide
+        q = points0.shape[1]
+        work.update(_bank_inputs(feats0, idx0, feats1, idx1, scale0, scale1, dev, who, gather=bool(bs and q)))
+        work.update(_bank_sizes(bs, feats0, feats1))
+        if bs and q:
+            self._match_points(work, points0, valid0, (feats0.feat_c, feats1.feat_c, feats0.feat_f, feats1.feat_f),
+                               (idx0, idx1))
+        else:
+            work.update(_query_outputs(bs, q, dev))
+        out = {} if data is None else data
+        out.update({k: v for k, v in work.items() if k not in ("mask0", "mask1", "scale0", "scale1", "guide")})
+        return out
+
+    def _check_banks(self, feats0, idx0, feats1, idx1, scale0, scale1, who):
+        """The bank arguments of match_features / match_points_features (`who`), checked before any launch ->
+        (idx0, idx1 as contiguous int32 tensors on the model's device, that device)."""
+        key = self._bank_key()
+        dev = next(self.parameters()).device
+        for name, f in (("feats0", feats0), ("feats1", feats1)):
+            if not isinstance(f, ImageFeatures):
+                raise TypeError(f"{who}: `{name}` must be the ImageFeatures of extract_features")
+            if f.weights_key != key:
+                raise RuntimeError(f"{who}: `{name}` was extracted with other backbone weights (load_state_dict, "
+                                   ".to() or a parameter update since); extract the features again")
+        idx0 = self._pair_index(idx0, "idx0", len(feats0), dev, who)
+        idx1 = self._pair_index(idx1, "idx1", len(feats1), dev, who)
+        if idx0.shape != idx1.shape:
+            raise ValueError(f"{who}: idx0 and idx1 must have the same length ({idx0.numel()} vs {idx1.numel()})")
+        if (feats0.mask is None) != (feats1.mask is None):
+            raise ValueError(f"{who}: either both banks carry masks or neither (as mask0 / mask1 of forward)")
+        if (scale0 is None) != (scale1 is None):
+            raise ValueError(f"{who}: give scale0 and scale1 together")
+        return idx0, idx1, dev
+
     @staticmethod
-    def _pair_index(idx, name, n_images, dev):
+    def _pair_index(idx, name, n_images, dev, who="match_features"):
         """Validated pair -> bank image index as a contiguous int32 tensor on `dev` (one host sync for the range)."""
         if not torch.is_tensor(idx) or idx.dtype not in (torch.int32, torch.int64):
-            raise TypeError(f"match_features: `{name}` must be an int32 or int64 tensor (got "
+            raise TypeError(f"{who}: `{name}` must be an int32 or int64 tensor (got "
                             f"{idx.dtype if torch.is_tensor(idx) else type(idx).__name__})")
         if idx.device != dev:
-            raise ValueError(f"match_features: `{name}` is on {idx.device}, the model on {dev}")
+            raise ValueError(f"{who}: `{name}` is on {idx.device}, the model on {dev}")
         if idx.dim() != 1:
-            raise ValueError(f"match_features: `{name}` must be one-dimensional (got shape {tuple(idx.shape)})")
+            raise ValueError(f"{who}: `{name}` must be one-dimensional (got shape {tuple(idx.shape)})")
         if idx.numel():
             lo, hi = torch.stack([idx.min(), idx.max()]).tolist()
             if lo < 0 or hi >= n_images:
-                raise IndexError(f"match_features: `{name}` holds indices in [{lo}, {hi}], outside the bank's "
+                raise IndexError(f"{who}: `{name}` holds indices in [{lo}, {hi}], outside the bank's "
                                  f"[0, {n_images})")
         return idx.to(torch.int32).contiguous()
 
@@ -1233,18 +1289,20 @@ class LoFTR(nn.Module):
         work["qpts1_f"], work["qinside1"] = pts.view(n, q, 2), inside.view(n, q)
         data.update({k: v for k, v in work.items() if k not in _INPUT_KEYS})
 
-    def _match_points(self, data, points0, valid0):
-        """match_points on validated arguments."""
+    def _match_points(self, data, points0, valid0, feats=None, img_idx=None):
+        """match_points / match_points_features on validated arguments.  feats: None (the backbone runs on data's
+        image0 / image1), or the (feat_c0, feat_c1, feat_f0, feat_f1) banks of a pair list, read at img_idx = (idx0,
+        idx1) as in `_match_pairs`; `data` then already holds bs and the sizes."""
         n, q = points0.shape[:2]
         dev = points0.device
         if q == 0:
             data.update(_query_outputs(n, 0, dev))
             return
-        feat_c0, feat_c1, feat_f0, feat_f1 = self._backbone_pairs(data)
+        feat_c0, feat_c1, feat_f0, feat_f1 = self._backbone_pairs(data) if feats is None else feats
         c = feat_c0.shape[1]
         (h0, w0), (h1, w1) = data["hw0_c"], data["hw1_c"]
         L, S = h0 * w0, h1 * w1
-        state, m0, m1 = self._coarse_tokens(data, feat_c0, feat_c1)
+        state, m0, m1 = self._coarse_tokens(data, feat_c0, feat_c1, img_idx)
         out = self.coarse_matching.query(state.cat_hi, state.cat_lo, 2 * c, n, L, S, c, data, m0, m1, points0, valid0)
         centres, win = out.pop("centres"), out.pop("win_ids")
         inside = out["qinside"].reshape(-1)
@@ -1253,7 +1311,7 @@ class LoFTR(nn.Module):
                 if k in data}
         work.update({"b_ids": win[0], "i_ids": win[1], "j_ids": win[2], "mkpts0_c": out["qpts0_f"].view(-1, 2),
                      "mkpts1_c": out["qpts1_c"].view(-1, 2)})
-        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, n, L, S, work,
+        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, n, L, S, work, img_idx=img_idx,
                                           centres=(centres, inside))
         ww = self.fine_preprocess.W ** 2
         self.loftr_fine.run(fstate, n * q, ww, ww)
@@ -1400,25 +1458,57 @@ def _check_points(data, points0, valid0):
         raise ValueError("match_points: give scale0 and scale1 together")
     if ("mask0" in data) != ("mask1" in data):
         raise ValueError("match_points: give mask0 and mask1 together")
-    n = data["image0"].shape[0]
+    _check_query_args(points0, valid0, data["image0"].shape[0], "match_points")
+    named = [(k, data[k]) for k in ("image0", "image1", "mask0", "mask1", "scale0", "scale1") if k in data]
+    _check_devices(named + [("points0", points0)] + ([("valid0", valid0)] if valid0 is not None else []),
+                   data["image0"].device, "image0", "match_points")
+
+
+def _check_query_args(points0, valid0, n, who):
+    """Dtypes and shapes of the queries of `n` pairs (match_points / match_points_features, `who`)."""
     if not torch.is_tensor(points0) or points0.dtype != torch.float32:
-        raise TypeError("match_points: points0 must be a float32 tensor (got "
+        raise TypeError(f"{who}: points0 must be a float32 tensor (got "
                         f"{points0.dtype if torch.is_tensor(points0) else type(points0).__name__})")
     if points0.dim() != 3 or points0.shape[0] != n or points0.shape[2] != 2:
-        raise ValueError(f"match_points: points0 must be [N, Q, 2] with N = {n} pairs (got {tuple(points0.shape)})")
+        raise ValueError(f"{who}: points0 must be [N, Q, 2] with N = {n} pairs (got {tuple(points0.shape)})")
     if valid0 is not None:
         if not torch.is_tensor(valid0) or valid0.dtype != torch.bool:
-            raise TypeError("match_points: valid0 must be a bool tensor")
+            raise TypeError(f"{who}: valid0 must be a bool tensor")
         if tuple(valid0.shape) != tuple(points0.shape[:2]):
-            raise ValueError(f"match_points: valid0 must be [N, Q] = {tuple(points0.shape[:2])} (got "
-                             f"{tuple(valid0.shape)})")
-    dev = data["image0"].device
-    named = [(k, data[k]) for k in ("image0", "image1", "mask0", "mask1", "scale0", "scale1") if k in data]
-    for k, t in named + [("points0", points0)] + ([("valid0", valid0)] if valid0 is not None else []):
+            raise ValueError(f"{who}: valid0 must be [N, Q] = {tuple(points0.shape[:2])} (got {tuple(valid0.shape)})")
+
+
+def _check_devices(named, dev, what, who):
+    """Every (name, tensor) of `named` is a CUDA tensor on `dev`, the device of `what`."""
+    for k, t in named:
         if not torch.is_tensor(t) or not t.is_cuda:
-            raise ValueError(f"match_points: `{k}` must be a CUDA tensor")
+            raise ValueError(f"{who}: `{k}` must be a CUDA tensor")
         if t.device != dev:
-            raise ValueError(f"match_points: `{k}` is on {t.device}, image0 on {dev}")
+            raise ValueError(f"{who}: `{k}` is on {t.device}, {what} on {dev}")
+
+
+def _bank_sizes(bs, feats0, feats1):
+    """The bookkeeping keys forward writes (bs and the image, coarse and fine sizes) for `bs` pairs of two banks."""
+    return {"bs": bs, "hw0_i": feats0.hw_i, "hw1_i": feats1.hw_i, "hw0_c": feats0.hw_c, "hw1_c": feats1.hw_c,
+            "hw0_f": feats0.hw_f, "hw1_f": feats1.hw_f}
+
+
+def _bank_inputs(feats0, idx0, feats1, idx1, scale0, scale1, dev, who, gather=True):
+    """forward's per-pair masks and scales of a checked pair list (LoFTR._check_banks), gathered through the indices
+    -> dict with mask0 / mask1 and scale0 / scale1 where given.  The scale shapes are checked before the gathers;
+    gather=False checks them only (an empty dict, nothing launched)."""
+    if scale0 is not None:
+        for name, s, f in (("scale0", scale0, feats0), ("scale1", scale1, feats1)):
+            if tuple(s.shape) != (len(f), 2):
+                raise ValueError(f"{who}: {name} must be [{len(f)}, 2] (got {tuple(s.shape)})")
+    work = {}
+    if not gather:
+        return work
+    if feats0.mask is not None:
+        work["mask0"], work["mask1"] = feats0.mask[idx0.long()], feats1.mask[idx1.long()]
+    if scale0 is not None:
+        work["scale0"], work["scale1"] = scale0.to(dev)[idx0.long()], scale1.to(dev)[idx1.long()]
+    return work
 
 
 def _weight_refs(model):
