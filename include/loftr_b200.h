@@ -65,7 +65,8 @@ extern "C" {
  * lb_coarse_match_guided (coarse matching restricted to a band around a homography or fundamental matrix);
  * lb_rectify_images / lb_rectify_points (image1 warped into image0's frame through a homography, matches mapped back);
  * lb_coarse_match_search (coarse matching of K candidate warps per pair, keeping the best candidate's matches);
- * lb_coarse_query_guided / lb_fine_preprocess_centres_indexed (caller-given points on bank pairs, with a guide). */
+ * lb_coarse_query_guided / lb_fine_preprocess_centres_indexed (caller-given points on bank pairs, with a guide);
+ * lb_coarse_query_side / lb_coarse_query_reuse (caller-given image1 points, and round trips on one coarse pass). */
 int lb_version(void);
 /* k-block (in elements) the library was built with: convolution weight planes pad Cin per tap to a multiple of it */
 int lb_block_k(void);
@@ -406,6 +407,27 @@ int lb_coarse_query(const LbCoarseMatchArgs* args /*host*/, const LbCoarseQueryA
 int lb_coarse_query_guided(const LbCoarseMatchArgs* args /*host*/, const LbCoarseQueryArgs* query /*host*/,
                            const LbCoarseGuide* guide /*host*/, int operand_planes, void* ws, size_t ws_bytes,
                            void* stream);
+
+/* Point queries from either image (found by name; DESIGN.md §22).  side 0: lb_coarse_query, or with a non-NULL guide
+ * lb_coarse_query_guided.  side 1: the queries are image1 points, and `query` is read with the roles swapped: points0 /
+ * valid0 hold the image1 points (source pixels when args->scale1 is given), H0 / W0 image1's size, Hf0 / Wf0 its fine
+ * map; pts0_f receives the query snapped to image1's fine grid and pts1_c the image0 window centre.  A query is inside
+ * when valid0 allows it, its point (divided by scale1) is finite and in [0, W0 - 1] x [0, H0 - 1], its cell j is
+ * unmasked and the column of j has a valid row; i is that column's arg-max.  i_ids / j_ids, centres and win_ids keep
+ * the (image0, image1) order.  f1 = clamp(floor(p / fine_scale + 0.5)), f0 = stride * (ix, iy) + f1 - stride * (jx, jy).
+ * mutual: row_arg[i] == j and row i has a valid column; valid: mutual and the forward's flag of (b, i); conf: mconf's
+ * expression when mutual, else exp((col_key[j] + colterm[j]) + bias).  Errors: those of lb_coarse_query_guided when a
+ * guide is given, a side that is not 0 or 1, operand_planes not 1 or 2.  Same workspace as lb_coarse_match. */
+int lb_coarse_query_side(const LbCoarseMatchArgs* args /*host*/, const LbCoarseQueryArgs* query /*host*/,
+                         const LbCoarseGuide* guide /*host, NULL: unguided*/, int side, int operand_planes, void* ws,
+                         size_t ws_bytes, void* stream);
+/* The query launch of lb_coarse_query_side alone (one launch, timing tag "match_query"; no score pass): `ws` must hold
+ * what a preceding query entry computed for the same args (guide and operand planes included) on the same stream.
+ * Errors: a side that is not 0 or 1, the query checks of lb_coarse_query, L / S that do not match the coarse grids, an
+ * unknown match_type, a NULL workspace or one smaller than lb_coarse_match_workspace_bytes.  Q <= 0 or n_pairs <= 0
+ * launch nothing. */
+int lb_coarse_query_reuse(const LbCoarseMatchArgs* args /*host*/, const LbCoarseQueryArgs* query /*host*/, int side,
+                          void* ws, size_t ws_bytes, void* stream);
 
 typedef struct LbFinePreprocessArgs {
   const float* feat_f0;   /* fine maps, any strides (elements): index = n*sn + c*sc + y*sh + x*sw */

@@ -169,6 +169,10 @@ SIGNATURES = {
                                 c_void_p]),
     "lb_coarse_query_guided": (c_int, [C.POINTER(LbCoarseMatchArgs), C.POINTER(LbCoarseQueryArgs),
                                        C.POINTER(LbCoarseGuide), c_int, c_void_p, c_size_t, c_void_p]),
+    "lb_coarse_query_side": (c_int, [C.POINTER(LbCoarseMatchArgs), C.POINTER(LbCoarseQueryArgs),
+                                     C.POINTER(LbCoarseGuide), c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "lb_coarse_query_reuse": (c_int, [C.POINTER(LbCoarseMatchArgs), C.POINTER(LbCoarseQueryArgs), c_int, c_void_p,
+                                      c_size_t, c_void_p]),
     "lb_fine_preprocess_workspace_bytes": (c_size_t, [c_long, c_int, c_int]),
     "lb_fine_preprocess": (c_int, [C.POINTER(LbFinePreprocessArgs), c_void_p, c_size_t, c_void_p]),
     "lb_fine_preprocess_indexed": (c_int, [C.POINTER(LbFinePreprocessArgs), c_void_p, c_void_p, c_void_p, c_size_t,
@@ -217,8 +221,10 @@ RECTIFY_ENTRIES = ("lb_rectify_images", "lb_rectify_points")   # data["rectify1"
 SEARCH_ENTRIES = ("lb_coarse_match_search",)   # data["rectify1_candidates"], DESIGN.md §20
 # LoFTR.match_points_features: points on bank pairs (DESIGN.md §21), with and without a guide
 BANK_POINTS_ENTRIES = ("lb_coarse_query_guided", "lb_fine_preprocess_centres_indexed")
+# image1-side point queries and round trips (DESIGN.md §22)
+SIDE_POINTS_ENTRIES = ("lb_coarse_query_side", "lb_coarse_query_reuse")
 _OPTIONAL = set(POINTS_ENTRIES) | set(GUIDE_ENTRIES) | set(RECTIFY_ENTRIES) | set(SEARCH_ENTRIES) | \
-    set(BANK_POINTS_ENTRIES)
+    set(BANK_POINTS_ENTRIES) | set(SIDE_POINTS_ENTRIES)
 GEOMETRY_HOMOGRAPHY = 0
 GEOMETRY_FUNDAMENTAL = 1
 GUIDE_HOMOGRAPHY = 0

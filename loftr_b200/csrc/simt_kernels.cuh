@@ -762,6 +762,102 @@ __global__ void coarse_query_kernel(const QueryParams p) {
   p.pts1_c[2 * q + 1] = static_cast<float>(fy1) * p.s_f * sy1;
 }
 
+// Caller-given image1 points -> the coarse answer of each (DESIGN.md §22), the mirror of coarse_query_kernel: the
+// cell j nearest to the point, its column arg-max i, and the window centres of both images.  A mutual answer gets
+// match_flag_kernel's row-side conf, so it equals mconf bit for bit; any other gets the column-side expression
+// exp((col_key[j] + colterm[j]) + conf_bias).  valid = flag[i] && row_arg[i] == j: the forward keeps (b, i, j).
+// Outputs that are not inside are as in coarse_query_kernel.
+struct QueryColParams {
+  int n_pairs, Q, L, S;
+  int h1c, w1c, w0c;
+  int H1, W1;               // image1 (network pixels)
+  int Hf1, Wf1;             // fine map of image1
+  int stride;               // fine pixels per coarse cell
+  float s_c, s_f;           // image pixels per coarse / fine pixel
+  float conf_bias;
+  const float* points1;     // [n*Q, 2] (x, y), source pixels when scale1 is given
+  const uint8_t* valid1;    // optional [n*Q]
+  const float* scale0;      // optional [n, 2]
+  const float* scale1;
+  const uint8_t* mask1;     // optional [n*S]
+  const float* col_key;     // [n*S]
+  const int* col_arg;
+  const float* colterm;
+  const float* row_key;     // [n*L]
+  const int* row_arg;
+  const float* rowterm;
+  const uint8_t* flag;      // [n*L] match_flag_kernel's test
+  long long* i_ids;         // [n*Q]
+  long long* j_ids;
+  float* conf;
+  uint8_t* mutual;
+  uint8_t* valid;
+  uint8_t* inside;
+  int* centres;             // [2, n*Q, 2] fine-map (x, y) of the image0 / image1 window centres
+  long long* win;           // [3, n*Q] (b, i, j) read by the fine stage
+  float* pts1_f;            // [n*Q, 2] the query snapped to image1's fine grid
+  float* pts0_c;            // [n*Q, 2] the image0 window centre
+};
+__global__ void coarse_query_col_kernel(const QueryColParams p) {
+  const long q = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x;
+  const long nq = static_cast<long>(p.n_pairs) * p.Q;
+  if (q >= nq) return;
+  const int b = static_cast<int>(q / p.Q);
+  float sx0 = 1.f, sy0 = 1.f, sx1 = 1.f, sy1 = 1.f;
+  if (p.scale1) { sx0 = p.scale0[2 * b]; sy0 = p.scale0[2 * b + 1]; sx1 = p.scale1[2 * b]; sy1 = p.scale1[2 * b + 1]; }
+  float px = p.points1[2 * q], py = p.points1[2 * q + 1];
+  if (p.scale1) { px = px / sx1; py = py / sy1; }
+  // the comparisons are false for NaN, so a NaN coordinate fails here
+  bool in = (!p.valid1 || p.valid1[q]) && px >= 0.f && px <= static_cast<float>(p.W1 - 1) && py >= 0.f &&
+            py <= static_cast<float>(p.H1 - 1);
+  int i = 0, j = 0, cx = 0, cy = 0;
+  long gj = 0;
+  if (in) {
+    cx = min(max(static_cast<int>(floorf(px / p.s_c + 0.5f)), 0), p.w1c - 1);
+    cy = min(max(static_cast<int>(floorf(py / p.s_c + 0.5f)), 0), p.h1c - 1);
+    j = cy * p.w1c + cx;
+    gj = static_cast<long>(b) * p.S + j;
+    if (p.mask1 && !p.mask1[gj]) in = false;
+  }
+  if (in) {
+    i = p.col_arg[gj];
+    in = i >= 0 && i < p.L && p.col_key[gj] > -1.0e29f;   // a column without any valid row has no answer
+  }
+  const long nq2 = 2 * nq;
+  if (!in) {
+    const float nan = __int_as_float(0x7fffffff);
+    p.i_ids[q] = -1; p.j_ids[q] = -1;
+    p.conf[q] = 0.f;
+    p.mutual[q] = 0; p.valid[q] = 0; p.inside[q] = 0;
+    p.centres[2 * q] = 0; p.centres[2 * q + 1] = 0; p.centres[2 * (nq + q)] = 0; p.centres[2 * (nq + q) + 1] = 0;
+    p.win[q] = b; p.win[nq + q] = 0; p.win[nq2 + q] = 0;
+    p.pts1_f[2 * q] = nan; p.pts1_f[2 * q + 1] = nan;
+    p.pts0_c[2 * q] = nan; p.pts0_c[2 * q + 1] = nan;
+    return;
+  }
+  const int fx1 = min(max(static_cast<int>(floorf(px / p.s_f + 0.5f)), 0), p.Wf1 - 1);
+  const int fy1 = min(max(static_cast<int>(floorf(py / p.s_f + 0.5f)), 0), p.Hf1 - 1);
+  const int iy = i / p.w0c, ix = i - iy * p.w0c;
+  const int fx0 = p.stride * ix + (fx1 - p.stride * cx);
+  const int fy0 = p.stride * iy + (fy1 - p.stride * cy);
+  const long gi = static_cast<long>(b) * p.L + i;
+  // a row without any valid column (key kNegBig) has no arg-max, as in coarse_query_kernel and match_flag_kernel
+  const bool mutual = p.row_arg[gi] == j && p.row_key[gi] > -1.0e29f;
+  p.i_ids[q] = i; p.j_ids[q] = j;
+  p.conf[q] = mutual ? expf(p.row_key[gi] + p.rowterm[gi] + p.conf_bias)     // match_flag_kernel's conf
+                     : expf(p.col_key[gj] + p.colterm[gj] + p.conf_bias);
+  p.mutual[q] = mutual ? 1 : 0;
+  p.valid[q] = mutual && p.flag[gi] ? 1 : 0;
+  p.inside[q] = 1;
+  p.centres[2 * q] = fx0; p.centres[2 * q + 1] = fy0;
+  p.centres[2 * (nq + q)] = fx1; p.centres[2 * (nq + q) + 1] = fy1;
+  p.win[q] = b; p.win[nq + q] = i; p.win[nq2 + q] = j;
+  p.pts1_f[2 * q] = static_cast<float>(fx1) * p.s_f * sx1;
+  p.pts1_f[2 * q + 1] = static_cast<float>(fy1) * p.s_f * sy1;
+  p.pts0_c[2 * q] = static_cast<float>(fx0) * p.s_f * sx0;
+  p.pts0_c[2 * q + 1] = static_cast<float>(fy0) * p.s_f * sy0;
+}
+
 // Ordered stream compaction (ascending (b, i) like torch.where, coarse_matching.py:194) + coarse
 // keypoints (coarse_matching.py:241-250).
 struct CompactParams {

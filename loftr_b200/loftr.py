@@ -691,28 +691,35 @@ class CoarseMatching(nn.Module):
             guide = _lib.LbCoarseGuide(kind, model.data_ptr(), radius)
         return a, keep, guide
 
-    def query(self, hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1, points0, valid0=None):
+    def query(self, hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1, points0, valid0=None, side=0, ws=None,
+              reuse=False):
         """The coarse stage for caller-given image0 points (LoFTR.match_points, DESIGN.md §17): planes as `run`,
         points0 [n, Q, 2] f32 and valid0 (None or bool [n, Q]) on the device, validated by the caller.  No host sync.
         data["guide"] (optional, `check_guide`): the queries are answered on the guided coarse quantities through
         lb_coarse_query_guided (DESIGN.md §21).
         -> dict of the per-query outputs (q_i_ids, q_j_ids, qconf, qmutual, qvalid, qinside [n, Q]; qpts0_f, qpts1_c
         [n, Q, 2]) and of what the fine stage reads: "centres" int32 [2, n*Q, 2] and "win_ids" int64 [3, n*Q].
-        The per-pair cap (max_matches_per_pair) is not applied."""
+        The per-pair cap (max_matches_per_pair) is not applied.
+        side: 0, or 1 when points0 / valid0 are image1 points (DESIGN.md §22, lb_coarse_query_side): the outputs are
+        then qpts1_f (the snapped query) and qpts0_c (the image0 window centre) in place of qpts0_f / qpts1_c.
+        ws: None, or a uint8 device tensor of lb_coarse_match_workspace_bytes(n, L, S) bytes to use as the workspace.
+        reuse: ws holds what a preceding query on the same planes and `data` computed, and only the query kernel runs
+        (lb_coarse_query_reuse): no score pass."""
         _require_eval(self)
         _lib.require_entries(_lib.POINTS_ENTRIES, "match_points")
         lib = _lib.load()
         dev = hi.device
         q = points0.shape[1]
         nq = n * q
+        snap, centre = ("qpts0_f", "qpts1_c") if side == 0 else ("qpts1_f", "qpts0_c")
         out = {"q_i_ids": torch.empty(n, q, dtype=torch.int64, device=dev),
                "q_j_ids": torch.empty(n, q, dtype=torch.int64, device=dev),
                "qconf": torch.empty(n, q, dtype=torch.float32, device=dev),
                "qmutual": torch.empty(n, q, dtype=torch.bool, device=dev),
                "qvalid": torch.empty(n, q, dtype=torch.bool, device=dev),
                "qinside": torch.empty(n, q, dtype=torch.bool, device=dev),
-               "qpts0_f": torch.empty(n, q, 2, dtype=torch.float32, device=dev),
-               "qpts1_c": torch.empty(n, q, 2, dtype=torch.float32, device=dev),
+               snap: torch.empty(n, q, 2, dtype=torch.float32, device=dev),
+               centre: torch.empty(n, q, 2, dtype=torch.float32, device=dev),
                "centres": torch.empty(2, nq, 2, dtype=torch.int32, device=dev),
                "win_ids": torch.empty(3, nq, dtype=torch.int64, device=dev)}
         a, keep, guide = self._args(hi, lo, ld, n, L, S, c, data, mask_u8_0, mask_u8_1)
@@ -724,17 +731,24 @@ class CoarseMatching(nn.Module):
             valid0 = valid0.contiguous().view(torch.uint8)
             keep.append(valid0)
             qa.valid0 = valid0.data_ptr()
-        (qa.H0, qa.W0), (qa.Hf0, qa.Wf0) = data["hw0_i"], data["hw0_f"]
-        qa.stride = data["hw0_f"][0] // data["hw0_c"][0]
-        qa.fine_scale = data["hw0_i"][0] / data["hw0_f"][0]
+        s = "01"[side]   # the queried image's sizes
+        (qa.H0, qa.W0), (qa.Hf0, qa.Wf0) = data[f"hw{s}_i"], data[f"hw{s}_f"]
+        qa.stride = data[f"hw{s}_f"][0] // data[f"hw{s}_c"][0]
+        qa.fine_scale = data[f"hw{s}_i"][0] / data[f"hw{s}_f"][0]
         qa.i_ids, qa.j_ids, qa.conf = out["q_i_ids"].data_ptr(), out["q_j_ids"].data_ptr(), out["qconf"].data_ptr()
         qa.mutual, qa.valid, qa.inside = (out[k].data_ptr() for k in ("qmutual", "qvalid", "qinside"))
         qa.centres, qa.win_ids = out["centres"].data_ptr(), out["win_ids"].data_ptr()
-        qa.pts0_f, qa.pts1_c = out["qpts0_f"].data_ptr(), out["qpts1_c"].data_ptr()
+        qa.pts0_f, qa.pts1_c = out[snap].data_ptr(), out[centre].data_ptr()
         nbytes = lib.lb_coarse_match_workspace_bytes(n, L, S)
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        if ws is None:
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         planes = 1 if self._precision == "fp16" else 2
-        if guide is not None:
+        if reuse:
+            _lib.check(lib.lb_coarse_query_reuse(C.byref(a), C.byref(qa), side, ws.data_ptr(), ws.numel(), _stream(hi)))
+        elif side:
+            _lib.check(lib.lb_coarse_query_side(C.byref(a), C.byref(qa), None if guide is None else C.byref(guide),
+                                                side, planes, ws.data_ptr(), ws.numel(), _stream(hi)))
+        elif guide is not None:
             _lib.require_entries(_lib.BANK_POINTS_ENTRIES, "guided point queries")
             _lib.check(lib.lb_coarse_query_guided(C.byref(a), C.byref(qa), C.byref(guide), planes, ws.data_ptr(),
                                                   nbytes, _stream(hi)))
@@ -1051,8 +1065,8 @@ class LoFTR(nn.Module):
         return out
 
     @torch.no_grad()
-    def match_points_features(self, feats0, idx0, feats1, idx1, points0, valid0=None, scale0=None, scale1=None,
-                              data=None, guide=None):
+    def match_points_features(self, feats0, idx0, feats1, idx1, points0=None, valid0=None, scale0=None, scale1=None,
+                              data=None, guide=None, *, points1=None, valid1=None, round_trip=False):
         """`match_points` on pairs drawn from feature banks (DESIGN.md §21): pair b is image idx0[b] of feats0 against
         image idx1[b] of feats1, as in `match_features` (feats1 may be feats0; the banks' masks and the per-image
         scales scale0 [K0, 2] / scale1 [K1, 2] are gathered through the indices).  The backbone does not run again, so
@@ -1068,29 +1082,35 @@ class LoFTR(nn.Module):
         arg-max over the admissible cells, qvalid is the guided flag test, and a row without an admissible, unmasked
         column is not inside.  A query at a guided `match_features` match's mkpts0_c returns that match bit for bit.
 
+        points1 / valid1 (keyword-only, instead of points0 / valid0) and round_trip: as in `match_points` (DESIGN.md
+        §22), with the scales of the pair list and under the guide when one is given.
+
         An empty pair list or Q = 0 gives empty outputs and launches nothing.  The one host sync is the index range
         check of `match_features`."""
         who = "match_points_features"
         _require_eval(self)
+        side, points, valid = _query_side(points0, valid0, points1, valid1, round_trip, who)
         _lib.require(_lib.FEATURE_BANK_VERSION, who)
         _lib.require_entries(_lib.POINTS_ENTRIES + _lib.BANK_POINTS_ENTRIES, who)
+        if side or round_trip:
+            _lib.require_entries(_lib.SIDE_POINTS_ENTRIES, who)
         idx0, idx1, dev = self._check_banks(feats0, idx0, feats1, idx1, scale0, scale1, who)
         bs = idx0.numel()
-        _check_query_args(points0, valid0, bs, who)
-        _check_devices([("points0", points0)] + ([("valid0", valid0)] if valid0 is not None else []), dev, "the model",
-                       who)
+        _check_query_args(points, valid, bs, who, side)
+        _check_devices([(f"points{side}", points)] + ([(f"valid{side}", valid)] if valid is not None else []), dev,
+                       "the model", who)
         work = {}   # match_points' inputs for this pair list (masks, scales, guide), then every key it writes
         if guide is not None:
             check_guide(guide, bs, dev, self.coarse_matching.thr, who)
             work["guide"] = guide
-        q = points0.shape[1]
+        q = points.shape[1]
         work.update(_bank_inputs(feats0, idx0, feats1, idx1, scale0, scale1, dev, who, gather=bool(bs and q)))
         work.update(_bank_sizes(bs, feats0, feats1))
         if bs and q:
-            self._match_points(work, points0, valid0, (feats0.feat_c, feats1.feat_c, feats0.feat_f, feats1.feat_f),
-                               (idx0, idx1))
+            self._match_points(work, points, valid, (feats0.feat_c, feats1.feat_c, feats0.feat_f, feats1.feat_f),
+                               (idx0, idx1), side, round_trip)
         else:
-            work.update(_query_outputs(bs, q, dev))
+            work.update(_query_outputs(bs, q, dev, side, round_trip))
         out = {} if data is None else data
         out.update({k: v for k, v in work.items() if k not in ("mask0", "mask1", "scale0", "scale1", "guide")})
         return out
@@ -1246,7 +1266,7 @@ class LoFTR(nn.Module):
         data.update({key: v for key, v in work.items() if key not in _INPUT_KEYS})
 
     @torch.no_grad()
-    def match_points(self, data, points0, valid0=None):
+    def match_points(self, data, points0=None, valid0=None, *, points1=None, valid1=None, round_trip=False):
         """Refines caller-given image0 points to image1 through the coarse and fine stages (DESIGN.md §17).
 
         data: forward's inputs (image0 / image1, optional mask0 / mask1 and scale0 / scale1), all on the device.
@@ -1267,8 +1287,22 @@ class LoFTR(nn.Module):
 
         data["rectify1"] (as in `forward`): the queries are answered on the substituted input; qpts1_c / qpts1_f are
         mapped back into image1 and qinside1 [N, Q] bool says whether qpts1_f lies in image1's valid area; qexpec_f
-        and q_j_ids stay in the rectified frame."""
+        and q_j_ids stay in the rectified frame.
+
+        points1 / valid1 (keyword-only, instead of points0 / valid0): image1 points, answered in image0 on the same
+        coarse and fine evidence (DESIGN.md §22).  The keys follow "qptsX_* is in image X": qpts1_f (the snapped
+        query), qpts0_c (the image0 window centre), qpts0_f (the answer), qexpec_f (in image0's window); q_i_ids /
+        q_j_ids stay the image0 / image1 cells, i being the column arg-max of the query's cell j.  A query at a forward
+        match's mkpts1_c gets that match's ids, mconf and flags bit for bit.
+
+        round_trip: answer the first leg's answers back from the other image, with qinside as their validity, on the
+        same coarse pass (no score pass runs again).  Adds qback_pts [N, Q, 2] (the back answer, in the query's own
+        image), qback_conf, qback_valid, qback_inside [N, Q] (as qconf, qvalid, qinside for the back leg) and qfb_err
+        [N, Q] f32 (|qback_pts - the query| in source pixels, NaN unless both legs are inside).  The back leg equals a
+        call from the other image with points = the first answer and valid = qinside, bit for bit.
+        Neither points1 nor round_trip combines with data["rectify1"]."""
         _require_eval(self)
+        side, points, valid = _query_side(points0, valid0, points1, valid1, round_trip, "match_points")
         if data.get("guide") is not None:
             raise ValueError("match_points: data['guide'] is not supported (guided matching is available in forward, "
                              "forward_static and match_features)")
@@ -1276,10 +1310,14 @@ class LoFTR(nn.Module):
             raise ValueError("match_points: data['rectify1_candidates'] is not supported (the rectification search is "
                              "available in forward and forward_static; pass the chosen model as data['rectify1'])")
         _lib.require_entries(_lib.POINTS_ENTRIES, "match_points")
-        _check_points(data, points0, valid0)
+        if side or round_trip:
+            _lib.require_entries(_lib.SIDE_POINTS_ENTRIES, "match_points")
+        _check_points(data, points, valid, side)
         if data.get("rectify1") is None:
-            self._match_points(data, points0, valid0)
+            self._match_points(data, points, valid, side=side, round_trip=round_trip)
             return
+        if side or round_trip:
+            raise ValueError("match_points: points1 and round_trip cannot be combined with data['rectify1']")
         work, model = self._rectified(data, "match_points")
         self._match_points(work, points0, valid0)
         n, q = points0.shape[:2]
@@ -1289,36 +1327,64 @@ class LoFTR(nn.Module):
         work["qpts1_f"], work["qinside1"] = pts.view(n, q, 2), inside.view(n, q)
         data.update({k: v for k, v in work.items() if k not in _INPUT_KEYS})
 
-    def _match_points(self, data, points0, valid0, feats=None, img_idx=None):
-        """match_points / match_points_features on validated arguments.  feats: None (the backbone runs on data's
-        image0 / image1), or the (feat_c0, feat_c1, feat_f0, feat_f1) banks of a pair list, read at img_idx = (idx0,
-        idx1) as in `_match_pairs`; `data` then already holds bs and the sizes."""
-        n, q = points0.shape[:2]
-        dev = points0.device
+    def _match_points(self, data, points, valid, feats=None, img_idx=None, side=0, round_trip=False):
+        """match_points / match_points_features on validated arguments: `points` / `valid` of image `side`.
+        feats: None (the backbone runs on data's image0 / image1), or the (feat_c0, feat_c1, feat_f0, feat_f1) banks of
+        a pair list, read at img_idx = (idx0, idx1) as in `_match_pairs`; `data` then already holds bs and the sizes.
+        round_trip: the back leg runs on the coarse workspace of the first (DESIGN.md §22)."""
+        n, q = points.shape[:2]
+        dev = points.device
         if q == 0:
-            data.update(_query_outputs(n, 0, dev))
+            data.update(_query_outputs(n, 0, dev, side, round_trip))
             return
         feat_c0, feat_c1, feat_f0, feat_f1 = self._backbone_pairs(data) if feats is None else feats
         c = feat_c0.shape[1]
         (h0, w0), (h1, w1) = data["hw0_c"], data["hw1_c"]
         L, S = h0 * w0, h1 * w1
         state, m0, m1 = self._coarse_tokens(data, feat_c0, feat_c1, img_idx)
-        out = self.coarse_matching.query(state.cat_hi, state.cat_lo, 2 * c, n, L, S, c, data, m0, m1, points0, valid0)
+        coarse = (state.cat_hi, state.cat_lo, 2 * c, n, L, S, c, data, m0, m1)
+        ws = None
+        if round_trip:
+            ws = torch.empty(_lib.load().lb_coarse_match_workspace_bytes(n, L, S), dtype=torch.uint8, device=dev)
+        fine = (feat_f0.float(), feat_f1.float(), state.x, n, L, S, data, img_idx)
+        out = self.coarse_matching.query(*coarse, points, valid, side=side, ws=ws)
+        self._fine_points(out, side, *fine)
+        if round_trip:
+            other = 1 - side
+            back = self.coarse_matching.query(*coarse, out[f"qpts{other}_f"], out["qinside"], side=other, ws=ws,
+                                              reuse=True)
+            self._fine_points(back, other, *fine)
+            pts, inside = back[f"qpts{side}_f"], back["qinside"]
+            err = torch.linalg.vector_norm(pts - points, dim=-1)
+            out.update({"qback_pts": pts, "qback_conf": back["qconf"], "qback_valid": back["qvalid"],
+                        "qback_inside": inside, "qfb_err": err.masked_fill_(~inside, float("nan"))})
+        data.update(out)
+
+    def _fine_points(self, out, side, feat_f0, feat_f1, x, n, L, S, data, img_idx):
+        """The fine stage of the queries of CoarseMatching.query's `out` (image `side`), in place: pops its centres and
+        window ids and adds the answer qpts{1 - side}_f and qexpec_f.  The fine state is freed on return."""
+        q = out["qinside"].shape[1]
         centres, win = out.pop("centres"), out.pop("win_ids")
         inside = out["qinside"].reshape(-1)
-        # the fine stage reads the windows as a match list of N*Q entries: (b, i, j) = win_ids, mkpts1_c = qpts1_c
+        # the fine stage reads the windows as a match list of N*Q entries: (b, i, j) = win_ids
         work = {k: data[k] for k in ("bs", "hw0_i", "hw1_i", "hw0_c", "hw1_c", "hw0_f", "hw1_f", "scale0", "scale1")
                 if k in data}
-        work.update({"b_ids": win[0], "i_ids": win[1], "j_ids": win[2], "mkpts0_c": out["qpts0_f"].view(-1, 2),
-                     "mkpts1_c": out["qpts1_c"].view(-1, 2)})
-        fstate = self.fine_preprocess.run(feat_f0.float(), feat_f1.float(), state.x, n, L, S, work, img_idx=img_idx,
+        work.update({"b_ids": win[0], "i_ids": win[1], "j_ids": win[2]})
+        fstate = self.fine_preprocess.run(feat_f0, feat_f1, x, n, L, S, work, img_idx=img_idx,
                                           centres=(centres, inside))
         ww = self.fine_preprocess.W ** 2
         self.loftr_fine.run(fstate, n * q, ww, ww)
-        self.fine_matching(*fstate.sides(n * q, ww, ww), work)
-        out["qpts1_f"] = work["mkpts1_f"].view(n, q, 2)
+        f0, f1 = fstate.sides(n * q, ww, ww)
+        if side == 0:
+            work.update({"mkpts0_c": out["qpts0_f"].view(-1, 2), "mkpts1_c": out["qpts1_c"].view(-1, 2)})
+            self.fine_matching(f0, f1, work)
+        else:   # the mirror: window1's centre against window0, refined from the image0 centre with scale0
+            if "scale0" in work:
+                work["scale0"], work["scale1"] = work["scale1"], work["scale0"]
+            work.update({"mkpts0_c": out["qpts1_f"].view(-1, 2), "mkpts1_c": out["qpts0_c"].view(-1, 2)})
+            self.fine_matching(f1, f0, work)
+        out[f"qpts{1 - side}_f"] = work["mkpts1_f"].view(n, q, 2)
         out["qexpec_f"] = work["expec_f"].view(n, q, 3).masked_fill_(~out["qinside"][..., None], float("nan"))
-        data.update(out)
 
     def _backbone_pairs(self, data):
         """Step 1 of the forward (no host sync): the backbone on image0 / image1 -> (feat_c0, feat_c1, feat_f0,
@@ -1443,12 +1509,35 @@ _QUERY_KEYS = {"qpts0_f": (torch.float32, 2), "qpts1_c": (torch.float32, 2), "qp
                "qinside": (torch.bool, 0)}
 
 
-def _query_outputs(n, q, dev):
-    """Empty output tensors of LoFTR.match_points for [n, q] queries."""
-    return {k: torch.empty(n, q, *((d,) if d else ()), dtype=t, device=dev) for k, (t, d) in _QUERY_KEYS.items()}
+# the round trip's keys (DESIGN.md §22)
+_BACK_KEYS = {"qback_pts": (torch.float32, 2), "qback_conf": (torch.float32, 0), "qback_valid": (torch.bool, 0),
+              "qback_inside": (torch.bool, 0), "qfb_err": (torch.float32, 0)}
 
 
-def _check_points(data, points0, valid0):
+def _query_outputs(n, q, dev, side=0, round_trip=False):
+    """Empty output tensors of LoFTR.match_points for [n, q] queries of image `side` (qptsX_* keys in image X)."""
+    keys = {k.translate(str.maketrans("01", "10")) if side and k.startswith("qpts") else k: v
+            for k, v in _QUERY_KEYS.items()}
+    if round_trip:
+        keys.update(_BACK_KEYS)
+    return {k: torch.empty(n, q, *((d,) if d else ()), dtype=t, device=dev) for k, (t, d) in keys.items()}
+
+
+def _query_side(points0, valid0, points1, valid1, round_trip, who):
+    """The queried image of a match_points / match_points_features call (`who`) -> (side, points, valid).  Without
+    points1 the points0 checks run as before, so a call that gives neither fails on points0."""
+    if not isinstance(round_trip, bool):
+        raise TypeError(f"{who}: round_trip must be a bool (got {type(round_trip).__name__})")
+    if points1 is None:
+        if valid1 is not None:
+            raise ValueError(f"{who}: valid1 is given without points1")
+        return 0, points0, valid0
+    if points0 is not None or valid0 is not None:
+        raise ValueError(f"{who}: give the queries of one image: points0 (and valid0) or points1 (and valid1)")
+    return 1, points1, valid1
+
+
+def _check_points(data, points0, valid0, side=0):
     """Host-side validation of LoFTR.match_points' arguments, before any launch: shapes and dtypes first, then that
     everything is on image0's CUDA device."""
     for k in ("image0", "image1"):
@@ -1458,24 +1547,26 @@ def _check_points(data, points0, valid0):
         raise ValueError("match_points: give scale0 and scale1 together")
     if ("mask0" in data) != ("mask1" in data):
         raise ValueError("match_points: give mask0 and mask1 together")
-    _check_query_args(points0, valid0, data["image0"].shape[0], "match_points")
+    _check_query_args(points0, valid0, data["image0"].shape[0], "match_points", side)
     named = [(k, data[k]) for k in ("image0", "image1", "mask0", "mask1", "scale0", "scale1") if k in data]
-    _check_devices(named + [("points0", points0)] + ([("valid0", valid0)] if valid0 is not None else []),
+    _check_devices(named + [(f"points{side}", points0)] + ([(f"valid{side}", valid0)] if valid0 is not None else []),
                    data["image0"].device, "image0", "match_points")
 
 
-def _check_query_args(points0, valid0, n, who):
-    """Dtypes and shapes of the queries of `n` pairs (match_points / match_points_features, `who`)."""
+def _check_query_args(points0, valid0, n, who, side=0):
+    """Dtypes and shapes of the queries of `n` pairs (match_points / match_points_features, `who`); the messages name
+    points{side} / valid{side}."""
+    p, v = f"points{side}", f"valid{side}"
     if not torch.is_tensor(points0) or points0.dtype != torch.float32:
-        raise TypeError(f"{who}: points0 must be a float32 tensor (got "
+        raise TypeError(f"{who}: {p} must be a float32 tensor (got "
                         f"{points0.dtype if torch.is_tensor(points0) else type(points0).__name__})")
     if points0.dim() != 3 or points0.shape[0] != n or points0.shape[2] != 2:
-        raise ValueError(f"{who}: points0 must be [N, Q, 2] with N = {n} pairs (got {tuple(points0.shape)})")
+        raise ValueError(f"{who}: {p} must be [N, Q, 2] with N = {n} pairs (got {tuple(points0.shape)})")
     if valid0 is not None:
         if not torch.is_tensor(valid0) or valid0.dtype != torch.bool:
-            raise TypeError(f"{who}: valid0 must be a bool tensor")
+            raise TypeError(f"{who}: {v} must be a bool tensor")
         if tuple(valid0.shape) != tuple(points0.shape[:2]):
-            raise ValueError(f"{who}: valid0 must be [N, Q] = {tuple(points0.shape[:2])} (got {tuple(valid0.shape)})")
+            raise ValueError(f"{who}: {v} must be [N, Q] = {tuple(points0.shape[:2])} (got {tuple(valid0.shape)})")
 
 
 def _check_devices(named, dev, what, who):
