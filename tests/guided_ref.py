@@ -1,20 +1,16 @@
 """Float64 reference of guided coarse matching (DESIGN.md §18) -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
-Built on tests/ref64.py: the similarity, dual-softmax or Sinkhorn and the selection are ref64's; this module adds
+The guided confidence matrix is tests/ref64.py's, given `admissible` as its `adm`: inadmissible similarity entries are
+filled with -INF (the reference's padding fill, coarse_matching.py:111-123) and their conf is set to 0 before the
+selection, which is ref64.coarse_match unchanged.  This module adds what the guide itself needs:
 - `coarse_points`: the coarse keypoints mkpts0_c / mkpts1_c of every cell, in float32 as the kernels compute them;
 - `admissible`: the guide's predicate, evaluated in float32 with the operation order the kernels use (numpy rounds
   every float32 operation separately, as the kernels' explicitly rounded intrinsics do), so it is bit for bit the
   kernels' predicate; and its float64 distance from the band's edge, to leave near-boundary cell pairs out of a
-  comparison;
-- `conf_matrix`: ref64.conf_matrix with the guide's two rules: inadmissible similarity entries are filled with -INF
-  (the reference's padding fill, coarse_matching.py:111-123) and their conf is set to 0 before the selection.
-ref64.coarse_match then selects from that conf_matrix unchanged."""
+  comparison."""
 from __future__ import annotations
 
 import numpy as np
-import torch
-
-import ref64 as R
 
 F32 = np.float32
 
@@ -61,29 +57,3 @@ def admissible(kind, model, radius, p0, p1):
     margin = np.where(finite[:, None, None], margin, np.inf)
     return adm, margin
 
-
-def conf_matrix(feat_c0, feat_c1, mc, adm, mask_c0=None, mask_c1=None, bin_score=None, fp16=False):
-    """ref64.conf_matrix under a guide: `adm` bool [n, L, S] (a tensor on the features' device)."""
-    feat_c0, feat_c1 = R.r16(feat_c0, fp16), R.r16(feat_c1, fp16)
-    c = feat_c0.shape[-1]
-    f0, f1 = feat_c0 / c ** 0.5, feat_c1 / c ** 0.5
-    fill = ~adm
-    if mask_c0 is not None:
-        fill = fill | ~(mask_c0[..., None] & mask_c1[:, None])
-    if mc["match_type"] == "dual_softmax":
-        sim = torch.einsum("nlc,nsc->nls", f0, f1) / mc["dsmax_temperature"]
-        sim = sim.masked_fill(fill, -R.INF)
-        conf = torch.softmax(sim, 1) * torch.softmax(sim, 2)
-    elif mc["match_type"] == "sinkhorn":
-        sim = torch.einsum("nlc,nsc->nls", f0, f1).masked_fill(fill, -R.INF)
-        assign = R.log_optimal_transport(sim, bin_score, mc["skh_iters"]).exp()
-        L, S = sim.shape[1:]
-        conf = assign[:, :-1, :-1].clone()
-        if mc.get("skh_prefilter", False):
-            filter0 = (assign.argmax(dim=2) == S)[:, :-1]
-            filter1 = (assign.argmax(dim=1) == L)[:, :-1]
-            conf[filter0[..., None].expand_as(conf)] = 0
-            conf[filter1[:, None].expand_as(conf)] = 0
-    else:
-        raise NotImplementedError(mc["match_type"])
-    return conf.masked_fill(~adm, 0.0)

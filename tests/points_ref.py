@@ -1,8 +1,8 @@
 """Reference statement of `LoFTR.match_points` (DESIGN.md §17): rules 1, 2 and 4 in numpy, and the fine stage of one
 set of queries in float64 (or float32, the emulation the project rule compares against) from centre-based windows,
-otherwise through tests/ref64.py."""
-import math
-
+otherwise through tests/ref64.py.  Image1 queries (DESIGN.md §22) use the same rules with the images' roles swapped:
+rules 1, 2 and 4 are `query_cells` and `image1_centres` given image1's sizes, scale and mask, rule 3 is
+`column_answer`, and the fine stage is `fine_stage(..., side=1)`."""
 import numpy as np
 import torch
 
@@ -57,11 +57,24 @@ def centred_windows(feat_f, b_ids, centres, W):
     return torch.stack(out) if out else feat_f.new_zeros(0, W * W, c)
 
 
-def fine_stage(model, feat_f0, feat_f1, x0, x1, b_ids, i_ids, j_ids, f0, f1, pts1_c, hw0_i, scale1=None,
-               dtype=torch.float64):
+def column_answer(conf, b, j):
+    """Rule 3 of image1 queries on a float64 confidence matrix conf [N, L, S]: i = the column arg-max of (b, j) (the
+    smallest i of a tie), its conf, and whether (i, j) is mutual (j is the row arg-max of i) -> (i, conf, mutual)."""
+    col = conf[b, :, j]   # [M, L]
+    i = col.argmax(1)
+    c = col.gather(1, i[:, None])[:, 0]
+    mutual = conf[b, i].argmax(1) == torch.as_tensor(j, device=conf.device)
+    return i, c, mutual
+
+
+def fine_stage(model, feat_f0, feat_f1, x0, x1, b_ids, i_ids, j_ids, f0, f1, pts_c, hw0_i, scale=None,
+               dtype=torch.float64, side=0):
     """FinePreprocess + fine transformer + FineMatching (ref64) of the query windows centred on f0 / f1 [M, 2]:
-    feat_f [N, C, h, w], x0 / x1 the coarse transformer outputs [N, L / S, C] (dtype), pts1_c [M, 2] the image1
-    window centres in source pixels -> (expec_f [M, 3], pts1_f [M, 2])."""
+    feat_f [N, C, h, w], x0 / x1 the coarse transformer outputs [N, L / S, C] (dtype).  The windows pass the merge and
+    the fine transformer in (window0, window1) order on either side.  side 0: window0's centre correlated against
+    window1, refined from pts_c [M, 2], the image1 window centres in source pixels, with `scale` = scale1.  side 1 (the
+    mirrored fine match of image1 queries): window1's centre against window0, refined from the image0 window centres
+    with `scale` = scale0 -> (expec_f [M, 3], refined points [M, 2])."""
     dev = feat_f0.device
     cfg = model.config
     W = cfg["fine_window_size"]
@@ -70,29 +83,11 @@ def fine_stage(model, feat_f0, feat_f1, x0, x1, b_ids, i_ids, j_ids, f0, f1, pts
     fw = {k: v.detach().to(dev, dtype) for k, v in model.fine_preprocess.state_dict().items()}
     win0 = centred_windows(feat_f0, b, torch.as_tensor(f0), W)
     win1 = centred_windows(feat_f1, b, torch.as_tensor(f1), W)
-    c_win = torch.cat([x0[b, i], x1[b, j]], 0) @ fw["down_proj.weight"].T + fw["down_proj.bias"]
-    cat = torch.cat([torch.cat([win0, win1], 0), c_win[:, None].expand(-1, W * W, -1)], -1)
-    merged = cat @ fw["merge_feat.weight"].T + fw["merge_feat.bias"]
-    m = len(b)
+    m0, m1 = R.fine_merge(win0, win1, x0[b, i], x1[b, j], W, fw)
     fc = cfg["fine"]
-    g0, g1 = R.transformer(merged[:m], merged[m:], R.layer_weights(model.loftr_fine, dev, dtype=dtype),
+    g0, g1 = R.transformer(m0, m1, R.layer_weights(model.loftr_fine, dev, dtype=dtype),
                            fc["layer_names"], fc["nhead"], attention=fc.get("attention", "linear"))
-    return _fine_matching(g0, g1, torch.as_tensor(pts1_c, device=dev, dtype=dtype), b, hw0_i, feat_f0.shape[2:],
-                          scale1, dtype)
-
-
-def _fine_matching(f0, f1, mkpts1_c, b_ids, hw0_i, hw0_f, scale1, dtype):
-    """ref64.fine_matching in `dtype` (ref64's version is float64 only)."""
-    if dtype == torch.float64:
-        return R.fine_matching(f0, f1, mkpts1_c, b_ids, hw0_i, hw0_f, scale1)
-    m, ww, c = f0.shape
-    W = int(math.isqrt(ww))
-    sim = torch.einsum("mc,mrc->mr", f0[:, ww // 2], f1)
-    heat = torch.softmax(sim / c ** 0.5, dim=1)
-    lin = torch.linspace(-1, 1, W, dtype=dtype, device=f0.device)
-    grid = torch.stack([lin[None, :].expand(W, W), lin[:, None].expand(W, W)], -1).reshape(ww, 2)
-    coords = heat @ grid
-    std = torch.sqrt(torch.clamp(heat @ grid ** 2 - coords ** 2, min=1e-10)).sum(-1)
-    scale = hw0_i[0] / hw0_f[0]
-    s1 = scale * torch.as_tensor(scale1, device=f0.device, dtype=dtype)[b_ids] if scale1 is not None else scale
-    return torch.cat([coords, std[:, None]], -1), mkpts1_c + coords * (W // 2) * s1
+    if side == 1:
+        g0, g1 = g1, g0
+    return R.fine_matching(g0, g1, torch.as_tensor(pts_c, device=dev, dtype=dtype), b, hw0_i, feat_f0.shape[2:],
+                           scale, dtype)

@@ -176,22 +176,26 @@ def log_optimal_transport(scores, alpha, iters):
     return couplings + u[:, :, None] + v[:, None, :] - norm                                    # :148,169
 
 
-def conf_matrix(feat_c0, feat_c1, mc, mask_c0=None, mask_c1=None, bin_score=None, fp16=False):
+def conf_matrix(feat_c0, feat_c1, mc, mask_c0=None, mask_c1=None, bin_score=None, fp16=False, adm=None):
     """CoarseMatching.forward up to conf_matrix (coarse_matching.py:103-143).  feat [N, L|S, C]; masks bool [N, L|S].
-    fp16: the product of the rounded features; the scale 1/sqrt(C) (and 1/T) applies to the exact product."""
+    fp16: the product of the rounded features; the scale 1/sqrt(C) (and 1/T) applies to the exact product.
+    adm: a guide's admissibility, bool [N, L, S] (DESIGN.md §18): inadmissible entries join the padding fill and get
+    conf 0."""
     feat_c0, feat_c1 = r16(feat_c0, fp16), r16(feat_c1, fp16)
     c = feat_c0.shape[-1]
     f0, f1 = feat_c0 / c ** 0.5, feat_c1 / c ** 0.5                                         # :106-107
-    pad = None if mask_c0 is None else ~(mask_c0[..., None] & mask_c1[:, None])
+    fill = None if mask_c0 is None else ~(mask_c0[..., None] & mask_c1[:, None])
+    if adm is not None:
+        fill = ~adm if fill is None else ~adm | fill
     if mc["match_type"] == "dual_softmax":
         sim = torch.einsum("nlc,nsc->nls", f0, f1) / mc["dsmax_temperature"]                 # :110
-        if pad is not None:
-            sim = sim.masked_fill(pad, -INF)                                                  # :111-114
-        return torch.softmax(sim, 1) * torch.softmax(sim, 2)                                  # :115
-    if mc["match_type"] == "sinkhorn":
+        if fill is not None:
+            sim = sim.masked_fill(fill, -INF)                                                 # :111-114
+        conf = torch.softmax(sim, 1) * torch.softmax(sim, 2)                                  # :115
+    elif mc["match_type"] == "sinkhorn":
         sim = torch.einsum("nlc,nsc->nls", f0, f1)                                            # :119
-        if pad is not None:
-            sim = sim.masked_fill(pad, -INF)                                                  # :120-123
+        if fill is not None:
+            sim = sim.masked_fill(fill, -INF)                                                 # :120-123
         assign = log_optimal_transport(sim, bin_score, mc["skh_iters"]).exp()                # :126-128
         L, S = sim.shape[1:]
         conf = assign[:, :-1, :-1].clone()                                                    # :129
@@ -200,8 +204,9 @@ def conf_matrix(feat_c0, feat_c1, mc, mask_c0=None, mask_c1=None, bin_score=None
             filter1 = (assign.argmax(dim=1) == L)[:, :-1]
             conf[filter0[..., None].expand_as(conf)] = 0
             conf[filter1[:, None].expand_as(conf)] = 0
-        return conf
-    raise NotImplementedError(mc["match_type"])
+    else:
+        raise NotImplementedError(mc["match_type"])
+    return conf if adm is None else conf.masked_fill(~adm, 0.0)
 
 
 def coarse_match(conf, mc, hw0_i, hw0_c, hw1_c, mask0=None, mask1=None, scale0=None, scale1=None):
@@ -267,28 +272,35 @@ def fine_preprocess(feat_f0, feat_f1, feat_c0, feat_c1, b_ids, i_ids, j_ids, W, 
     w: 'down_proj.weight/bias', 'merge_feat.weight/bias' float64."""
     win0 = fine_windows(feat_f0, b_ids, i_ids, W, stride)
     win1 = fine_windows(feat_f1, b_ids, j_ids, W, stride)
-    c_win = torch.cat([feat_c0[b_ids, i_ids], feat_c1[b_ids, j_ids]], 0) @ w["down_proj.weight"].T + w["down_proj.bias"]
+    return fine_merge(win0, win1, feat_c0[b_ids, i_ids], feat_c1[b_ids, j_ids], W, w)
+
+
+def fine_merge(win0, win1, xc0, xc1, W, w):
+    """The merge half of FinePreprocess (fine_preprocess.py:49-57): windows win0 / win1 [M, WW, Cf] and the coarse
+    features xc0 / xc1 [M, C] of their cells -> (merged window0, merged window1) [M, WW, Cf]."""
+    c_win = torch.cat([xc0, xc1], 0) @ w["down_proj.weight"].T + w["down_proj.bias"]
     cat = torch.cat([torch.cat([win0, win1], 0), c_win[:, None].expand(-1, W * W, -1)], -1)  # :52-55
     merged = cat @ w["merge_feat.weight"].T + w["merge_feat.bias"]
-    m = len(b_ids)
+    m = len(win0)
     return merged[:m], merged[m:]                                                             # :57
 
 
-def fine_matching(f0, f1, mkpts1_c, b_ids, hw0_i, hw0_f, scale1=None):
-    """FineMatching.forward + get_fine_match (fine_matching.py:27-74) -> (expec_f [M, 3], mkpts1_f [M, 2]).
+def fine_matching(f0, f1, mkpts1_c, b_ids, hw0_i, hw0_f, scale1=None, dtype=F64):
+    """FineMatching.forward + get_fine_match (fine_matching.py:27-74) -> (expec_f [M, 3], mkpts1_f [M, 2]), in `dtype`
+    (float32: the emulation the point queries' kernel error is compared against).
     kornia's spatial_expectation2d / create_meshgrid(normalized): x along the window's second axis, linspace(-1, 1, W)."""
     m, ww, c = f0.shape
     W = int(math.isqrt(ww))
     sim = torch.einsum("mc,mrc->mr", f0[:, ww // 2], f1)                                      # :43-44
     heat = torch.softmax(sim / c ** 0.5, dim=1)                                               # :45-46
-    lin = torch.linspace(-1, 1, W, dtype=F64, device=f0.device)
+    lin = torch.linspace(-1, 1, W, dtype=dtype, device=f0.device)
     grid = torch.stack([lin[None, :].expand(W, W), lin[:, None].expand(W, W)], -1).reshape(ww, 2)   # :50
     coords = heat @ grid                                                                      # :49
     var = heat @ grid ** 2 - coords ** 2                                                      # :53
     std = torch.sqrt(torch.clamp(var, min=1e-10)).sum(-1)                                     # :54
     scale = hw0_i[0] / hw0_f[0]
-    s1 = scale * f64(scale1, f0.device)[b_ids] if scale1 is not None else scale              # :68
-    mk1 = f64(mkpts1_c, f0.device) + coords * (W // 2) * s1                                   # :69
+    s1 = scale * f64(scale1, f0.device).to(dtype)[b_ids] if scale1 is not None else scale    # :68
+    mk1 = f64(mkpts1_c, f0.device).to(dtype) + coords * (W // 2) * s1                         # :69
     return torch.cat([coords, std[:, None]], -1), mk1
 
 

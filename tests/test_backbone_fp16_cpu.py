@@ -128,11 +128,7 @@ def test_constructor_modes_and_refusals():
 
 
 def test_fp16_backbone_refuses_an_older_library(monkeypatch):
-    class OldLib:
-        def lb_version(self):
-            return 107
-
-    monkeypatch.setattr(_lib, "load", lambda: OldLib())
+    util.old_library(monkeypatch, 107)
     assert _lib.BACKBONE_FP16_VERSION == 108
     with pytest.raises(RuntimeError, match=r"version 108 or newer.*is version 107"):
         loftr_b200.LoFTR(loftr_b200.get_cfg("indoor_ds"), backbone_impl="b200_fp16")

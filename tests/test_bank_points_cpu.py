@@ -7,8 +7,8 @@ import pytest
 import torch
 
 import loftr_b200
+import util
 from loftr_b200 import _lib
-from loftr_b200.loftr import ImageFeatures
 
 WHO = "match_points_features"
 
@@ -17,30 +17,17 @@ def _model():
     return loftr_b200.LoFTR(loftr_b200.get_cfg("indoor_ds")).eval()
 
 
-def _bank(model, k=3, masks=False):
-    """A host bank of k 96x128 images tied to the model's current weights (never matched: nothing here launches)."""
-    mask = torch.ones(k, 12, 16, dtype=torch.bool) if masks else None
-    return ImageFeatures(torch.zeros(k, 256, 12, 16), torch.zeros(k, 128, 48, 64), mask, torch.Size((96, 128)),
-                         torch.Size((12, 16)), torch.Size((48, 64)), model._bank_key())
-
-
 def _idx(*v):
     return torch.tensor(v, dtype=torch.int64)
 
 
 @pytest.fixture
 def no_stages(monkeypatch):
-    """The matching stages of the model raise if reached: validation must stop a call before them."""
-    def reached(*a, **k):
-        raise AssertionError("a matching stage was reached")
-    model = _model()
-    for name in ("_match_points", "_coarse_tokens", "_backbone", "_backbone_pairs"):
-        monkeypatch.setattr(model, name, reached)
-    return model
+    return util.stages_unreachable(monkeypatch, _model())
 
 
 def _call(model, bank0=None, idx0=None, bank1=None, idx1=None, pts=None, **kw):
-    bank0 = _bank(model) if bank0 is None else bank0
+    bank0 = util.host_bank(model) if bank0 is None else bank0
     bank1 = bank0 if bank1 is None else bank1
     idx0 = _idx(0, 1) if idx0 is None else idx0
     idx1 = _idx(1, 2) if idx1 is None else idx1
@@ -51,7 +38,7 @@ def _call(model, bank0=None, idx0=None, bank1=None, idx1=None, pts=None, **kw):
 # ------------------------------------------------------------------------------------------------ bank arguments
 def test_bank_checks_name_the_call(no_stages):
     m = no_stages
-    bank = _bank(m)
+    bank = util.host_bank(m)
     with pytest.raises(TypeError, match=rf"{WHO}: `feats0` must be the ImageFeatures of extract_features"):
         _call(m, bank0=object(), bank1=bank)
     with pytest.raises(TypeError, match=rf"{WHO}: `idx1` must be an int32 or int64 tensor \(got torch.float32\)"):
@@ -69,14 +56,14 @@ def test_bank_checks_name_the_call(no_stages):
     with pytest.raises(ValueError, match=rf"{WHO}: idx0 and idx1 must have the same length \(2 vs 1\)"):
         _call(m, idx1=_idx(1))
     with pytest.raises(ValueError, match=rf"{WHO}: either both banks carry masks or neither"):
-        _call(m, bank0=_bank(m, masks=True), bank1=bank)
+        _call(m, bank0=util.host_bank(m, masks=True), bank1=bank)
     with pytest.raises(ValueError, match=rf"{WHO}: give scale0 and scale1 together"):
         _call(m, scale0=torch.ones(3, 2))
 
 
 def test_a_bank_tied_to_other_weights_raises(no_stages):
     m = no_stages
-    bank = _bank(m)
+    bank = util.host_bank(m)
     with torch.no_grad():
         m.backbone.conv1.weight.add_(0.0)   # an in-place update: a new _version
     with pytest.raises(RuntimeError, match=rf"{WHO}: `feats0` was extracted with other backbone weights"):
@@ -136,7 +123,7 @@ def test_empty_pair_list_and_q0_give_empty_outputs(monkeypatch):
     monkeypatch.setattr(LM, "_check_devices", lambda *a, **k: None)
     for name in ("_match_points", "_coarse_tokens", "_backbone"):
         monkeypatch.setattr(m, name, lambda *a, **k: (_ for _ in ()).throw(AssertionError("reached")))
-    bank = _bank(m, masks=True)
+    bank = util.host_bank(m, masks=True)
     for idx, q in ((_idx(0, 2), 0), (_idx(), 5)):
         mine = {"kept": 1}
         out = m.match_points_features(bank, idx, bank, idx, torch.zeros(idx.numel(), q, 2), data=mine,
@@ -165,23 +152,12 @@ def test_entries_are_bound_only_where_exported(monkeypatch):
         assert getattr(lib, name).argtypes == _lib.SIGNATURES[name][1]
     assert lib.lb_version() == 110
     _lib.require_entries(_lib.BANK_POINTS_ENTRIES, WHO)
-
-    class Exports:   # what ctypes.CDLL gives for a build without the two entries: every other declared symbol
-        def __init__(self):
-            for n in _lib.SIGNATURES:
-                if n not in _lib.BANK_POINTS_ENTRIES:
-                    setattr(self, n, type("Fn", (), {})())
-            self.lb_version = lambda: 110
-
-    monkeypatch.setattr(_lib, "_lib", None)
-    monkeypatch.setattr(_lib.C, "CDLL", lambda path: Exports())
-    monkeypatch.setattr(_lib.os.path, "exists", lambda path: True)
-    old = _lib.load()
+    old = util.load_without(monkeypatch, _lib.BANK_POINTS_ENTRIES)
     assert not any(hasattr(old, n) for n in _lib.BANK_POINTS_ENTRIES)
     assert old.lb_coarse_query.argtypes == _lib.SIGNATURES["lb_coarse_query"][1]   # the rest still binds
     _lib.require_entries(_lib.POINTS_ENTRIES + _lib.GUIDE_ENTRIES + _lib.SEARCH_ENTRIES, "other paths")
     m = _model()
-    bank = _bank(m)
+    bank = util.host_bank(m)
     with pytest.raises(RuntimeError, match=rf"{WHO} needs lb_coarse_query_guided, which .* \(version 110\) does not "
                                            "export"):
         _call(m, bank0=bank)

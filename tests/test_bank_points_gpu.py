@@ -7,7 +7,8 @@
 3. guided grid queries return guided `match_features` matches bit for bit, and qvalid is exactly its match set;
 4. every answered guided query's cell pair is admissible (tests/guided_ref.py's bitwise predicate), and a row without
    an admissible column is not answered;
-5. guided off-grid queries against float64 (tests/points_ref.py + tests/guided_ref.py) at the tolerances of §17;
+5. guided off-grid queries against float64 (tests/points_ref.py, tests/guided_ref.py and ref64.conf_matrix under the
+   guide's admissibility) at the tolerances of §17;
 6. a bank tied to stale weights raises."""
 import numpy as np
 import pytest
@@ -23,23 +24,6 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 CASE = {c["name"]: c for c in CASES}
 Q_KEYS = ("qpts0_f", "qpts1_c", "qpts1_f", "qexpec_f", "qconf", "q_i_ids", "q_j_ids", "qmutual", "qvalid", "qinside")
-H_MODEL = np.array([[1.03, 0.04, 6.0], [-0.03, 0.97, -5.0], [2e-5, -1e-5, 1.0]], np.float32)
-
-
-def _model(case, backbone_impl="auto", precision="split"):
-    model, cfg, _ = util.build_model(case, DEV, backbone_impl=backbone_impl, match_precision=precision)
-    return model, cfg
-
-
-def _idx(v):
-    return torch.tensor(v, dtype=torch.int64, device=DEV)
-
-
-def _frames(case):
-    """The case's images, masks and scales as one set of 2n frames (image0 of every pair, then image1)."""
-    d = util.device_inputs(case)
-    cat = lambda k: torch.cat([d[k + "0"], d[k + "1"]]) if k + "0" in d else None
-    return cat("image"), cat("mask"), cat("scale")
 
 
 def _points(idx0, hw, scales, seed, q=160):
@@ -58,15 +42,6 @@ def _points(idx0, hw, scales, seed, q=160):
     return pts.contiguous()
 
 
-def _grid_points(idx0, hw_c, scales):
-    """Every cell keypoint of image0 as the forward computes mkpts0_c -> [B, L, 2]."""
-    hc, wc = hw_c
-    i = torch.arange(hc * wc, device=DEV)
-    cell = torch.stack([i % wc, i // wc], 1).float()[None].expand(len(idx0), -1, -1)
-    s = torch.full((len(idx0), 1, 2), 8.0, device=DEV) if scales is None else 8.0 * scales[idx0][:, None, :]
-    return (cell * s).contiguous()
-
-
 def _stacked(model, imgs0, idx0, imgs1, idx1, pts, masks=None, scales=None, valid0=None):
     """match_points on the explicitly stacked pairs -> the keys it wrote."""
     data = {"image0": imgs0[idx0], "image1": imgs1[idx1]}
@@ -75,29 +50,17 @@ def _stacked(model, imgs0, idx0, imgs1, idx1, pts, masks=None, scales=None, vali
     if scales is not None:
         data["scale0"], data["scale1"] = scales[0][idx0], scales[1][idx1]
     model.match_points(data, pts, valid0)
-    return {k: v for k, v in data.items() if k not in ("image0", "image1", "mask0", "mask1", "scale0", "scale1")}
-
-
-def _assert_bitwise(got, ref, label):
-    assert list(got) == list(ref), f"{label}: keys {list(got)} vs {list(ref)}"
-    for k, v in ref.items():
-        if torch.is_tensor(v):
-            assert got[k].dtype == v.dtype and got[k].shape == v.shape, (label, k)
-            same = torch.equal(torch.nan_to_num(got[k].float()), torch.nan_to_num(v.float())) and \
-                torch.equal(torch.isnan(got[k].float()), torch.isnan(v.float()))
-            assert same, f"{label}: {k} differs from match_points on the stacked pairs"
-        else:
-            assert got[k] == v, (label, k, got[k], v)
+    return util.outputs(data)
 
 
 # ------------------------------------------------------------------------------------------------ 1. = stacked
 MODES = [
     ("ds_b200_split", "ds_thr0", {}),
-    ("ds_b200_fp16match", "ds_thr0", {"precision": "fp16"}),
-    ("ds_fp16backbone_fp16match", "ds_thr0", {"backbone_impl": "b200_fp16", "precision": "fp16"}),
+    ("ds_b200_fp16match", "ds_thr0", {"match_precision": "fp16"}),
+    ("ds_fp16backbone_fp16match", "ds_thr0", {"backbone_impl": "b200_fp16", "match_precision": "fp16"}),
     ("ds_fp16backbone_split", "ds_thr0", {"backbone_impl": "b200_fp16"}),
     ("sinkhorn", "ot_thr0", {}),
-    ("sinkhorn_fp16", "ot_thr0", {"precision": "fp16"}),
+    ("sinkhorn_fp16", "ot_thr0", {"match_precision": "fp16"}),
     ("full_attention", "full", {}),
     ("masked_scaled", "ds_masked_scaled", {}),
 ]
@@ -106,58 +69,64 @@ MODES = [
 @pytest.mark.parametrize("name, case, opts", MODES, ids=[m[0] for m in MODES])
 def test_bank_queries_equal_stacked_match_points_bitwise(name, case, opts):
     case = dict(CASE["ds_thr0"], coarse_attention="full", fine_attention="full") if case == "full" else CASE[case]
-    model, _ = _model(case, **opts)
-    imgs, masks, scales = _frames(case)
+    model, _, _ = util.build_model(case, DEV, **opts)
+    imgs, masks, scales = util.frames(case)
     bank = model.extract_features(imgs, masks)
     n = case["n"]
     assert n == 2
     # a chain 0 -> 1 -> 2 -> 3 over the bank, a repeated pair and a self pair, in one list; feats1 is feats0
-    idx0, idx1 = _idx([0, 1, 2, 2, 3]), _idx([1, 2, 3, 3, 3])
+    idx0, idx1 = util.idx([0, 1, 2, 2, 3]), util.idx([1, 2, 3, 3, 3])
     pts = _points(idx0, imgs.shape[2:], scales, 3)
     valid0 = torch.rand(pts.shape[:2], generator=torch.Generator().manual_seed(1)).to(DEV) > 0.1
     for v in (None, valid0):
         got = model.match_points_features(bank, idx0, bank, idx1, pts, v, scales, scales)
         ref = _stacked(model, imgs, idx0, imgs, idx1, pts, None if masks is None else (masks, masks),
                        None if scales is None else (scales, scales), v)
-        _assert_bitwise(got, ref, name)
+        assert list(got) == list(ref), f"{name}: keys {list(got)} vs {list(ref)}"
+        util.assert_same(got, ref, label=name)
         assert got["qinside"].any(), name
 
 
 def test_outdoor_832_masks_and_scales_bitwise():
     case = BASELINE_CASES["out4"]
-    model, _ = _model(case)
-    imgs, masks, scales = _frames(case)
+    model, _, _ = util.build_model(case, DEV)
+    imgs, masks, scales = util.frames(case)
     bank = model.extract_features(imgs, masks)
-    idx0, idx1 = _idx([0, 1, 2, 7, 3, 3]), _idx([4, 5, 6, 0, 3, 7])
+    idx0, idx1 = util.idx([0, 1, 2, 7, 3, 3]), util.idx([4, 5, 6, 0, 3, 7])
     pts = _points(idx0, imgs.shape[2:], scales, 4, q=400)
     got = model.match_points_features(bank, idx0, bank, idx1, pts, scale0=scales, scale1=scales)
     ref = _stacked(model, imgs, idx0, imgs, idx1, pts, (masks, masks), (scales, scales))
-    _assert_bitwise(got, ref, "outdoor 832")
+    assert list(got) == list(ref)
+    util.assert_same(got, ref, label="outdoor 832")
     assert got["qvalid"].any()
 
 
 def test_chain_with_repeated_indices_and_two_banks():
     """A 5-frame chain t -> t+1 plus repeats, in int32 and int64; and pairs across two banks of different sizes."""
     case = CASE["ds_unequal"]
-    model, _ = _model(case)
+    model, _, _ = util.build_model(case, DEV)
     d = util.device_inputs(case)
     frames = torch.cat([d["image0"], util.device_inputs(case, seed=7)["image0"], util.device_inputs(case, seed=8)[
         "image0"], util.device_inputs(case, seed=9)["image0"], d["image0"].flip(-1)])
     bank = model.extract_features(frames)
     for dt in (torch.int32, torch.int64):
-        idx0, idx1 = _idx([0, 1, 2, 3, 3, 0]).to(dt), _idx([1, 2, 3, 4, 4, 1]).to(dt)
+        idx0, idx1 = util.idx([0, 1, 2, 3, 3, 0]).to(dt), util.idx([1, 2, 3, 4, 4, 1]).to(dt)
         pts = _points(idx0.long(), frames.shape[2:], None, 5)
         pts[4] = pts[3]
         got = model.match_points_features(bank, idx0, bank, idx1, pts)
-        _assert_bitwise(got, _stacked(model, frames, idx0.long(), frames, idx1.long(), pts), f"chain {dt}")
+        ref = _stacked(model, frames, idx0.long(), frames, idx1.long(), pts)
+        assert list(got) == list(ref)
+        util.assert_same(got, ref, label=f"chain {dt}")
         for k in Q_KEYS:   # the repeated pair answers the same queries the same way
-            assert torch.equal(torch.nan_to_num(got[k][3].float()), torch.nan_to_num(got[k][4].float())), k
+            util.assert_same(got[k][4], got[k][3], label=f"chain {dt}: {k} of the repeated pair")
     other = torch.cat([d["image1"], util.device_inputs(case, seed=7)["image1"]])   # 128 x 104
     bank1 = model.extract_features(other)
-    idx0, idx1 = _idx([0, 4, 2]), _idx([1, 0, 1])
+    idx0, idx1 = util.idx([0, 4, 2]), util.idx([1, 0, 1])
     pts = _points(idx0, frames.shape[2:], None, 6)
     got = model.match_points_features(bank, idx0, bank1, idx1, pts)
-    _assert_bitwise(got, _stacked(model, frames, idx0, other, idx1, pts), "two banks")
+    ref = _stacked(model, frames, idx0, other, idx1, pts)
+    assert list(got) == list(ref)
+    util.assert_same(got, ref, label="two banks")
 
 
 def test_torch_backbone_follows_the_match_list_rule():
@@ -165,10 +134,10 @@ def test_torch_backbone_follows_the_match_list_rule():
     match-list rule of DESIGN.md §5 (the same j for at least 99.5% of the answered queries; where j agrees, qconf within
     rtol 1e-3 and qpts1_f within 0.5 px)."""
     case = CASE["ds_thr0"]
-    model, _ = _model(case, backbone_impl="torch")
-    imgs, _, _ = _frames(case)
+    model, _, _ = util.build_model(case, DEV, backbone_impl="torch")
+    imgs, _, _ = util.frames(case)
     bank = model.extract_features(imgs)
-    idx0, idx1 = _idx([0, 1, 2, 0]), _idx([2, 3, 1, 3])
+    idx0, idx1 = util.idx([0, 1, 2, 0]), util.idx([2, 3, 1, 3])
     pts = _points(idx0, imgs.shape[2:], None, 7)
     got = model.match_points_features(bank, idx0, bank, idx1, pts)
     ref = _stacked(model, imgs, idx0, imgs, idx1, pts)
@@ -185,23 +154,19 @@ def test_torch_backbone_follows_the_match_list_rule():
 
 
 # ------------------------------------------------------------------------------------------------ 2-4. guided
-def _guide(model_np, radius, kind="homography"):
-    return {"kind": kind, "model": torch.as_tensor(np.ascontiguousarray(model_np, np.float32)).to(DEV),
-            "radius": radius}
-
-
 def test_all_nan_guide_is_the_unguided_call():
     case = CASE["ds_masked_scaled"]
-    model, _ = _model(case)
-    imgs, masks, scales = _frames(case)
+    model, _, _ = util.build_model(case, DEV)
+    imgs, masks, scales = util.frames(case)
     bank = model.extract_features(imgs, masks)
-    idx0, idx1 = _idx([0, 1, 2]), _idx([2, 3, 0])
+    idx0, idx1 = util.idx([0, 1, 2]), util.idx([2, 3, 0])
     pts = _points(idx0, imgs.shape[2:], scales, 8)
     ref = model.match_points_features(bank, idx0, bank, idx1, pts, scale0=scales, scale1=scales)
     for kind in ("homography", "fundamental"):
         got = model.match_points_features(bank, idx0, bank, idx1, pts, scale0=scales, scale1=scales,
-                                          guide=_guide(np.full((3, 3, 3), np.nan), 4.0, kind))
-        _assert_bitwise(got, ref, f"NaN {kind} guide")
+                                          guide=util.guide(kind, np.full((3, 3, 3), np.nan), 4.0))
+        assert list(got) == list(ref)
+        util.assert_same(got, ref, label=f"NaN {kind} guide")
 
 
 GUIDED = [("ds_thr0", "homography", 20.0), ("ds_thr0", "fundamental", 10.0), ("ot_thr0", "homography", 20.0),
@@ -210,28 +175,22 @@ GUIDED = [("ds_thr0", "homography", 20.0), ("ds_thr0", "fundamental", 10.0), ("o
 
 def _guided_setup(name, kind, radius, precision="split"):
     case = CASE[name]
-    model, cfg = _model(case, precision=precision)
-    imgs, masks, scales = _frames(case)
+    model, cfg, _ = util.build_model(case, DEV, match_precision=precision)
+    imgs, masks, scales = util.frames(case)
     bank = model.extract_features(imgs, masks)
     n = case["n"]
-    idx0, idx1 = _idx(list(range(n)) + [0]), _idx(list(range(n, 2 * n)) + [n])
-    b = len(idx0)
-    models = np.repeat(H_MODEL[None], b, 0)
-    if kind == "fundamental":
-        e1 = np.array([140.0, 60.0, 1.0])
-        ex = np.array([[0, -e1[2], e1[1]], [e1[2], 0, -e1[0]], [-e1[1], e1[0], 0]])
-        f = (ex @ H_MODEL).astype(np.float32)
-        models = np.repeat((f / np.abs(f).max())[None], b, 0)
+    idx0, idx1 = util.idx(list(range(n)) + [0]), util.idx(list(range(n, 2 * n)) + [n])
+    models = np.repeat((util.F_MODEL if kind == "fundamental" else util.H_MODEL)[None], len(idx0), 0)
     models[-1] = np.nan   # the last pair repeats the first, unguided
-    return model, cfg, bank, imgs, masks, scales, idx0, idx1, _guide(models, radius, kind), models
+    return model, cfg, bank, imgs, masks, scales, idx0, idx1, util.guide(kind, models, radius), models
 
 
 @pytest.mark.parametrize("name, kind, radius", GUIDED, ids=[f"{g[0]}_{g[1]}" for g in GUIDED])
 def test_guided_grid_queries_equal_guided_match_features(name, kind, radius):
     model, _, bank, imgs, masks, scales, idx0, idx1, guide, models = _guided_setup(name, kind, radius)
     mf = model.match_features(bank, idx0, bank, idx1, scales, scales, guide=guide)
-    q = model.match_points_features(bank, idx0, bank, idx1, _grid_points(idx0, bank.hw_c, scales), scale0=scales,
-                                    scale1=scales, guide=guide)
+    q = model.match_points_features(bank, idx0, bank, idx1, util.bank_grid_points(idx0, bank.hw_c, scales),
+                                    scale0=scales, scale1=scales, guide=guide)
     b, i = mf["b_ids"], mf["i_ids"]
     assert len(b) > 0 and (b == len(idx0) - 1).any()
     assert q["qinside"][b, i].all() and q["qvalid"][b, i].all()
@@ -261,7 +220,7 @@ def test_row_without_an_admissible_column_is_not_answered():
     models = models.copy()
     models[1] = [[1, 0, 1e5], [0, 1, 1e5], [0, 0, 1]]   # pair 1: every cell maps far outside image1
     pts = _points(idx0, imgs.shape[2:], None, 10)
-    q = model.match_points_features(bank, idx0, bank, idx1, pts, guide=_guide(models, 20.0))
+    q = model.match_points_features(bank, idx0, bank, idx1, pts, guide=util.guide("homography", models, 20.0))
     assert q["qinside"][0].any() and q["qinside"][2].all()
     assert not q["qinside"][1].any()
     for k in ("qpts0_f", "qpts1_c", "qpts1_f", "qexpec_f"):
@@ -287,7 +246,7 @@ def test_guided_offgrid_queries_vs_f64(kind, radius):
     stride = hw_f[0] // hw_c[0]
     p0, p1 = G.coarse_points(nb, hw_c, 8.0), G.coarse_points(nb, hw_c, 8.0)
     adm, _ = G.admissible(kind, models, radius, p0, p1)
-    conf64 = G.conf_matrix(R.f64(x0, DEV), R.f64(x1, DEV), cfg["match_coarse"], torch.as_tensor(adm, device=DEV))
+    conf64 = R.conf_matrix(R.f64(x0, DEV), R.f64(x1, DEV), cfg["match_coarse"], adm=util.to_dev(adm))
     b_ids = torch.arange(nb, device=DEV)[:, None].expand(-1, nq).reshape(-1)[sel]
     i_ids, j_ids = q["q_i_ids"].reshape(-1)[sel], q["q_j_ids"].reshape(-1)[sel]
     rows = conf64[b_ids, i_ids]
@@ -333,10 +292,10 @@ def test_guided_offgrid_queries_vs_f64(kind, radius):
 # ------------------------------------------------------------------------------------------------ 6. stale bank
 def test_a_bank_of_stale_weights_raises():
     case = CASE["ds_thr0"]
-    model, _ = _model(case)
-    imgs, _, _ = _frames(case)
+    model, _, _ = util.build_model(case, DEV)
+    imgs, _, _ = util.frames(case)
     bank = model.extract_features(imgs)
-    idx = _idx([0, 1])
+    idx = util.idx([0, 1])
     pts = _points(idx, imgs.shape[2:], None, 12, q=8)
     model.match_points_features(bank, idx, bank, idx, pts)
     model.load_state_dict(model.state_dict())

@@ -4,6 +4,7 @@ import pytest
 import torch
 
 import loftr_b200
+import util
 from loftr_b200 import _lib
 
 
@@ -12,11 +13,7 @@ def _model():
 
 
 def test_match_features_refuses_an_older_library(monkeypatch):
-    class OldLib:
-        def lb_version(self):
-            return 103
-
-    monkeypatch.setattr(_lib, "load", lambda: OldLib())
+    util.old_library(monkeypatch, 103)
     assert _lib.FEATURE_BANK_VERSION == 104
     with pytest.raises(RuntimeError, match=r"version 104 or newer.*is version 103"):
         _model().match_features(None, None, None, None)

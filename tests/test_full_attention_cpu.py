@@ -73,11 +73,7 @@ def test_unknown_attention_is_rejected(bad):
 
 
 def test_binding_refuses_full_attention_on_an_old_library(monkeypatch):
-    class OldLib:
-        def lb_version(self):
-            return 101
-
-    monkeypatch.setattr(_lib, "load", lambda: OldLib())
+    util.old_library(monkeypatch, 101)
     assert _lib.MIN_VERSION == 101 and _lib.FULL_ATTENTION_VERSION == 102
     cfg = dict(loftr_b200.get_cfg("indoor_ds")["coarse"], attention="full")
     tf = LocalFeatureTransformer(cfg)

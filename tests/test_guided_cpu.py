@@ -1,6 +1,6 @@
 """CPU-side checks of guided coarse matching (DESIGN.md §18): the shared guide validator and the callers that refuse a
 guide, the binding of lb_coarse_match_guided by name and its argument errors, and self-checks of the
-float64 guided reference (tests/guided_ref.py) against ref64."""
+float64 guided reference (tests/guided_ref.py's admissibility under ref64.conf_matrix) against unguided ref64."""
 import ctypes as C
 import math
 
@@ -11,6 +11,7 @@ import torch
 import guided_ref as G
 import loftr_b200
 import ref64 as R
+import util
 from loftr_b200 import _lib
 from loftr_b200.loftr import CapturedMatcher, CoarseMatching, check_guide
 from cases import build_cfg, build_cm_inputs
@@ -85,18 +86,7 @@ def test_guided_entry_is_bound_only_where_exported(monkeypatch):
     assert _lib.GUIDE_ENTRIES == ("lb_coarse_match_guided",) and "lb_coarse_match_guided" not in _lib._SINCE
     assert lib.lb_coarse_match_guided.argtypes == _lib.SIGNATURES["lb_coarse_match_guided"][1]
     _lib.require_entries(_lib.GUIDE_ENTRIES, "guided matching")
-
-    class Exports:   # every other declared symbol, as a build without the guided entry is loaded
-        def __init__(self):
-            for name in _lib.SIGNATURES:
-                if name not in _lib.GUIDE_ENTRIES:
-                    setattr(self, name, type("Fn", (), {})())
-            self.lb_version = lambda: 110
-
-    monkeypatch.setattr(_lib, "_lib", None)
-    monkeypatch.setattr(_lib.C, "CDLL", lambda path: Exports())
-    monkeypatch.setattr(_lib.os.path, "exists", lambda path: True)
-    old = _lib.load()
+    old = util.load_without(monkeypatch, _lib.GUIDE_ENTRIES)
     assert not hasattr(old, "lb_coarse_match_guided")
     assert old.lb_coarse_match_fp16.argtypes == _lib.SIGNATURES["lb_coarse_match_fp16"][1]   # the rest still binds
     with pytest.raises(RuntimeError, match=r"forward: guided matching needs lb_coarse_match_guided.*\(version 110\)"):
@@ -141,8 +131,7 @@ def _guided(inp, case, mc, adm, masked):
         mk0, mk1 = torch.as_tensor(inp["mask0"]), torch.as_tensor(inp["mask1"])
         m0, m1 = mk0.flatten(-2), mk1.flatten(-2)
     f0, f1 = R.f64(inp["feat_c0"]), R.f64(inp["feat_c1"])
-    conf = R.conf_matrix(f0, f1, mc, m0, m1, 1.0) if adm is None else \
-        G.conf_matrix(f0, f1, mc, torch.as_tensor(adm), m0, m1, 1.0)
+    conf = R.conf_matrix(f0, f1, mc, m0, m1, 1.0, adm=None if adm is None else torch.as_tensor(adm))
     return conf, R.coarse_match(conf, mc, (h0 * 8, w0 * 8), (h0, w0), (h1, w1), mk0, mk1)
 
 

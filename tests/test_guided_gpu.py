@@ -1,8 +1,9 @@
 """Guided coarse matching (data["guide"], lb_coarse_match_guided; DESIGN.md §18) on the GPU:
 1. a guide that admits every entry gives the unguided outputs bit for bit, on every path and option;
-2. the guided match lists against the float64 guided reference (tests/guided_ref.py) at the tile, chunk and mask
-   boundaries of tests/test_kernel_edges_gpu.py, with F and H guides whose bands cut through the tiles (the near-tie
-   rule of DESIGN.md §5, mconf at rtol 1e-3); cell pairs within 1e-3 r of the band's edge are left out;
+2. the guided match lists against the float64 guided reference (ref64.conf_matrix under tests/guided_ref.py's
+   admissibility) at the tile, chunk and mask boundaries of tests/test_kernel_edges_gpu.py, with F and H guides whose
+   bands cut through the tiles (the near-tie rule of DESIGN.md §5, mconf at rtol 1e-3); cell pairs within 1e-3 r of the
+   band's edge are left out;
 3. every coarse match lies in the band (recomputed in float64), and conf_matrix is 0 outside it;
 4. per-pair behaviour: a NaN model leaves its pair unguided, a pair does not see the other pairs' models, a model that
    maps every cell outside image1 leaves its pair without matches;
@@ -23,27 +24,9 @@ DEV = "cuda:0"
 _CASE = {c["name"]: c for c in CASES}
 CM_KEYS = ("b_ids", "i_ids", "j_ids", "mconf", "mkpts0_c", "mkpts1_c")
 
-# models in output coordinates (image pixels; source pixels with scales): x1 ~ H x0, and F = [e']_x H
-H_MODEL = np.array([[1.03, 0.04, 6.0], [-0.03, 0.97, -5.0], [2e-5, -1e-5, 1.0]], np.float32)
-_E1 = np.array([140.0, 60.0, 1.0])
-F_MODEL = (np.array([[0, -_E1[2], _E1[1]], [_E1[2], 0, -_E1[0]], [-_E1[1], _E1[0], 0]]) @ H_MODEL).astype(np.float32)
-F_MODEL /= np.abs(F_MODEL).max()
-
-
-def _t(x):
-    return torch.as_tensor(np.ascontiguousarray(x)).to(DEV)
-
-
-def _np(t):
-    return t.detach().cpu().numpy()
-
-
-def _guide(kind, model, radius):
-    return {"kind": kind, "model": _t(np.asarray(model, np.float32)), "radius": radius}
-
 
 def _models(kind, n):
-    return np.repeat((F_MODEL if kind == "fundamental" else H_MODEL)[None], n, 0)
+    return np.repeat((util.F_MODEL if kind == "fundamental" else util.H_MODEL)[None], n, 0)
 
 
 def _cm_setup(case, match_type, precision="split", prefilter=False, cap=None, conf=False, scales=False):
@@ -65,31 +48,27 @@ def _cm_setup(case, match_type, precision="split", prefilter=False, cap=None, co
     base = {"hw0_i": (h0 * 8, w0 * 8), "hw1_i": (h1 * 8, w1 * 8), "hw0_c": (h0, w0), "hw1_c": (h1, w1)}
     if scales:
         rs = np.random.RandomState(7)
-        base["scale0"], base["scale1"] = (_t(rs.uniform(0.7, 1.6, (n, 2)).astype(np.float32)) for _ in range(2))
+        base["scale0"], base["scale1"] = (util.to_dev(rs.uniform(0.7, 1.6, (n, 2)).astype(np.float32))
+                                          for _ in range(2))
     m0 = m1 = None
     if "mask0" in inp:
-        base["mask0"], base["mask1"] = _t(inp["mask0"]), _t(inp["mask1"])
+        base["mask0"], base["mask1"] = util.to_dev(inp["mask0"]), util.to_dev(inp["mask1"])
         m0, m1 = base["mask0"].flatten(-2), base["mask1"].flatten(-2)
 
     def run(guide=None):
         data = dict(base)
         if guide is not None:
             data["guide"] = guide
-        mod(_t(inp["feat_c0"]), _t(inp["feat_c1"]), data, m0, m1)
+        mod(util.to_dev(inp["feat_c0"]), util.to_dev(inp["feat_c1"]), data, m0, m1)
         return data
     return run, inp, mc, base
 
 
 def _points(case, base):
     n = case["n"]
-    s0 = _np(base["scale0"]) if "scale0" in base else None
-    s1 = _np(base["scale1"]) if "scale1" in base else None
+    s0 = util.to_np(base["scale0"]) if "scale0" in base else None
+    s1 = util.to_np(base["scale1"]) if "scale1" in base else None
     return G.coarse_points(n, case["hw0c"], 8.0, s0), G.coarse_points(n, case["hw1c"], 8.0, s1)
-
-
-def _assert_equal(a, b, keys, label):
-    for k in keys:
-        assert torch.equal(a[k], b[k]), f"{label}: {k} differs"
 
 
 # ------------------------------------------------------------------------------------------------ 1. identity
@@ -108,16 +87,16 @@ def test_all_admissible_guide_is_bitwise_unguided(match_type, precision, prefilt
     ref = run()
     assert ref["b_ids"].numel() > 0
     rs = np.random.RandomState(1)
-    for label, guide in (("radius_1e9_F", _guide("fundamental", rs.standard_normal((3, 3, 3)), 1e9)),
-                         ("radius_1e9_H", _guide("homography", _models("homography", 3), 1e9)),
-                         ("nan_model", _guide("homography", np.full((3, 3, 3), np.nan), 2.0))):
+    for label, guide in (("radius_1e9_F", util.guide("fundamental", rs.standard_normal((3, 3, 3)), 1e9)),
+                         ("radius_1e9_H", util.guide("homography", _models("homography", 3), 1e9)),
+                         ("nan_model", util.guide("homography", np.full((3, 3, 3), np.nan), 2.0))):
         got = run(guide)
-        _assert_equal(got, ref, CM_KEYS + ("conf_matrix",), label)
+        util.assert_same(got, ref, CM_KEYS + ("conf_matrix",), label, nan_equal=False)
 
 
 def _e2e_identity_guides(n):
-    return [_guide("homography", np.repeat(H_MODEL[None], n, 0), 1e9),
-            _guide("fundamental", np.full((n, 3, 3), np.nan), 4.0)]
+    return [util.guide("homography", np.repeat(util.H_MODEL[None], n, 0), 1e9),
+            util.guide("fundamental", np.full((n, 3, 3), np.nan), 4.0)]
 
 
 @pytest.mark.parametrize("name", ["ds_thr0", "ds_masked_scaled", "ot_thr0"])
@@ -130,7 +109,7 @@ def test_all_admissible_guide_end_to_end_is_bitwise_unguided(name):
     n = case["n"]
     for guide in _e2e_identity_guides(n):
         got = util.eager(model, dict(inp, guide=guide))
-        _assert_equal(got, ref, LIST_KEYS, "forward")
+        util.assert_same(got, ref, LIST_KEYS, "forward", nan_equal=False)
         st = dict(inp, guide=guide)
         model.forward_static(st)
         util.assert_static_equals_eager(st, ref, "forward_static")   # the live prefix of its capacity buffers
@@ -143,7 +122,8 @@ def test_all_admissible_guide_end_to_end_is_bitwise_unguided(name):
     ref_mf = model.match_features(bank, i0, bank, i1, estimate="fundamental")
     for guide in _e2e_identity_guides(n):
         got = model.match_features(bank, i0, bank, i1, estimate="fundamental", guide=guide)
-        _assert_equal(got, ref_mf, (*LIST_KEYS, "geom_model", "geom_inliers", "geom_num_inliers"), "match_features")
+        util.assert_same(got, ref_mf, (*LIST_KEYS, "geom_model", "geom_inliers", "geom_num_inliers"), "match_features",
+                         nan_equal=False)
         assert "guide" not in got
 
 
@@ -171,25 +151,26 @@ def _vs_f64(case, match_type, kind, radius, precision="split", prefilter=False):
         models = np.repeat(np.array([[1, 0, 40.0], [0, 1, 0], [0, 0, 1]], np.float32)[None], n, 0)
         if kind == "fundamental":
             models = np.repeat(np.array([[0, 0, 0.01], [0, 0, -1], [-0.01, 1, 0]], np.float32)[None], n, 0)
-    got = run(_guide(kind, models, radius))
+    got = run(util.guide(kind, models, radius))
     p0, p1 = _points(case, base)
     adm, margin = G.admissible(kind, models, radius, p0, p1)
     assert 0.005 < adm.mean() < 0.9, adm.mean()
     m0 = m1 = None
     if "mask0" in base:
         m0, m1 = base["mask0"].flatten(-2), base["mask1"].flatten(-2)
-    conf = G.conf_matrix(R.f64(inp["feat_c0"], DEV), R.f64(inp["feat_c1"], DEV), mc, _t(adm), m0, m1, 1.0,
-                         fp16=precision == "fp16")
+    conf = R.conf_matrix(R.f64(inp["feat_c0"], DEV), R.f64(inp["feat_c1"], DEV), mc, m0, m1, 1.0,
+                         fp16=precision == "fp16", adm=util.to_dev(adm))
     ref = R.coarse_match(conf, mc, base["hw0_i"], case["hw0c"], case["hw1c"], base.get("mask0"), base.get("mask1"))
-    ref = {k: _np(v) for k, v in ref.items()}
-    g = {k: _np(got[k]) for k in CM_KEYS}
+    ref = {k: util.to_np(v) for k, v in ref.items()}
+    g = {k: util.to_np(got[k]) for k in CM_KEYS}
     near = margin < 1e-3 * radius
 
     def drop(d):
         keep = ~near[d["b_ids"], d["i_ids"], d["j_ids"]]
         return {k: v[keep] for k, v in d.items()}
     rows, cols = R.top2(conf)
-    stats = util.compare_matches(drop(g), drop(ref), {"row_top2_f64": _np(rows), "col_top2_f64": _np(cols)},
+    gold = {"row_top2_f64": util.to_np(rows), "col_top2_f64": util.to_np(cols)}
+    stats = util.compare_matches(drop(g), drop(ref), gold,
                                  conf_rtol=1e-3, px_tol=0.5, min_overlap=0.995, label=f"guided_{match_type}_{kind}")
     assert stats["n"] > 0
     util.record(f"guided_vs_f64_{match_type}_{precision}_{kind}", {**stats, "admissible": float(adm.mean()),
@@ -218,10 +199,10 @@ def test_matches_lie_in_the_band_and_conf_matrix_is_zero_outside(match_type, kin
     case = {"n": 2, "hw0c": (12, 20), "hw1c": (14, 18), "border_rm": 1}
     run, _, _, base = _cm_setup(case, match_type, scales=True, conf=True)
     models = _models(kind, 2).astype(np.float64)
-    got = run(_guide(kind, models, radius))
-    b = _np(got["b_ids"])
+    got = run(util.guide(kind, models, radius))
+    b = util.to_np(got["b_ids"])
     assert len(b) > 0
-    p0, p1 = _np(got["mkpts0_c"]).astype(np.float64), _np(got["mkpts1_c"]).astype(np.float64)
+    p0, p1 = util.to_np(got["mkpts0_c"]).astype(np.float64), util.to_np(got["mkpts1_c"]).astype(np.float64)
     T = models[b]
     v = np.einsum("mij,mj->mi", T, np.concatenate([p0, np.ones((len(b), 1))], 1))
     if kind == "fundamental":
@@ -231,7 +212,7 @@ def test_matches_lie_in_the_band_and_conf_matrix_is_zero_outside(match_type, kin
     assert dist.max() <= radius * (1 + 1e-5) + 1e-3, dist.max()
     q0, q1 = _points(case, base)
     adm, _ = G.admissible(kind, models, radius, q0, q1)
-    cm = _np(got["conf_matrix"])
+    cm = util.to_np(got["conf_matrix"])
     assert (cm[~adm] == 0).all() and (cm[adm] > 0).any()
 
 
@@ -248,17 +229,17 @@ def test_per_pair_models(match_type):
     models = _models("homography", 3).copy()
     models[1] = np.nan
     models[2] = [[1, 0, 1e5], [0, 1, 1e5], [0, 0, 1]]     # every cell maps far outside image1
-    got = run(_guide("homography", models, 20.0))
-    _assert_equal(pair(got, 1), pair(unguided, 1), CM_KEYS + ("conf_matrix",), "NaN model")
+    got = run(util.guide("homography", models, 20.0))
+    util.assert_same(pair(got, 1), pair(unguided, 1), CM_KEYS + ("conf_matrix",), "NaN model", nan_equal=False)
     assert not (got["b_ids"] == 2).any() and (got["conf_matrix"][2] == 0).all()
     assert (got["b_ids"] == 0).any()
     for k in ("mconf", "mkpts0_c", "mkpts1_c", "conf_matrix"):
         assert torch.isfinite(got[k]).all(), k
     other = models.copy()
-    other[1] = H_MODEL                                     # change the other pairs' models only
+    other[1] = util.H_MODEL                                # change the other pairs' models only
     other[2] = [[0.9, 0.1, -8.0], [0.0, 1.1, 3.0], [0, 0, 1]]
-    got2 = run(_guide("homography", other, 20.0))
-    _assert_equal(pair(got2, 0), pair(got, 0), CM_KEYS + ("conf_matrix",), "independent pairs")
+    got2 = run(util.guide("homography", other, 20.0))
+    util.assert_same(pair(got2, 0), pair(got, 0), CM_KEYS + ("conf_matrix",), "independent pairs", nan_equal=False)
 
 
 # ------------------------------------------------------------------------------------------------ 5. monotone mconf
@@ -266,12 +247,12 @@ def test_per_pair_models(match_type):
 def test_dual_softmax_confidence_grows_under_a_guide(kind, radius):
     case = {"n": 3, "hw0c": (16, 20), "hw1c": (15, 21), "border_rm": 0}
     run, _, _, _ = _cm_setup(case, "dual_softmax")
-    a, g = run(), run(_guide(kind, _models(kind, 3), radius))
-    ka = {k: n for n, k in enumerate(zip(*(_np(a[x]).tolist() for x in ("b_ids", "i_ids", "j_ids"))))}
-    kg = {k: n for n, k in enumerate(zip(*(_np(g[x]).tolist() for x in ("b_ids", "i_ids", "j_ids"))))}
+    a, g = run(), run(util.guide(kind, _models(kind, 3), radius))
+    ka = {k: n for n, k in enumerate(zip(*(util.to_np(a[x]).tolist() for x in ("b_ids", "i_ids", "j_ids"))))}
+    kg = {k: n for n, k in enumerate(zip(*(util.to_np(g[x]).tolist() for x in ("b_ids", "i_ids", "j_ids"))))}
     common = sorted(set(ka) & set(kg))
     assert len(common) > 0
-    ca, cg = _np(a["mconf"])[[ka[k] for k in common]], _np(g["mconf"])[[kg[k] for k in common]]
+    ca, cg = util.to_np(a["mconf"])[[ka[k] for k in common]], util.to_np(g["mconf"])[[kg[k] for k in common]]
     assert (cg >= ca * (1 - 1e-5)).all(), float((cg / ca).min())
     util.record(f"guided_mconf_monotone_{kind}", {"common": len(common), "min_ratio": float((cg / ca).min())})
 
@@ -281,7 +262,7 @@ def test_forward_static_with_guide_replays_from_a_graph():
     case = _CASE["ds_thr0"]
     model, _, _ = util.build_model(case, DEV)
     inp = util.device_inputs(case)
-    guide = _guide("homography", np.repeat(np.eye(3, dtype=np.float32)[None], case["n"], 0), 40.0)
+    guide = util.guide("homography", np.repeat(np.eye(3, dtype=np.float32)[None], case["n"], 0), 40.0)
     eager = util.eager(model, dict(inp, guide=guide))
     unguided = util.eager(model, inp)
     assert eager["b_ids"].numel() > 0

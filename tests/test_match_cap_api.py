@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import loftr_b200
+import util
 from loftr_b200 import _lib
 from loftr_b200.loftr import CoarseMatching
 from match_cap_ref import apply_cap, capped_rows
@@ -49,11 +50,7 @@ def test_default_capacity_with_a_cap():
 
 
 def test_capped_matching_refuses_an_older_library(monkeypatch):
-    class OldLib:
-        def lb_version(self):
-            return 104
-
-    monkeypatch.setattr(_lib, "load", lambda: OldLib())
+    util.old_library(monkeypatch, 104)
     assert _lib.MATCH_CAP_VERSION == 105
     cm = CoarseMatching(_mc_cfg(max_matches_per_pair=16)).eval()
     with pytest.raises(RuntimeError, match=r"version 105 or newer.*is version 104"):

@@ -9,6 +9,7 @@ import torch
 
 import loftr_b200
 import ref64 as R
+import util
 from loftr_b200 import _lib
 from loftr_b200.loftr import CoarseMatching, LocalFeatureTransformer
 
@@ -124,11 +125,7 @@ def test_bad_precisions_are_rejected(bad):
 
 
 def test_fp16_matching_refuses_an_older_library(monkeypatch):
-    class OldLib:
-        def lb_version(self):
-            return 108
-
-    monkeypatch.setattr(_lib, "load", lambda: OldLib())
+    util.old_library(monkeypatch, 108)
     assert _lib.MATCH_FP16_VERSION == 109
     cfg = loftr_b200.get_cfg("indoor_ds")
     with pytest.raises(RuntimeError, match=r"match_precision.*version 109 or newer.*is version 108"):

@@ -10,6 +10,7 @@ import pytest
 import torch
 
 import loftr_b200
+import util
 from loftr_b200 import _lib
 from points_ref import image1_centres, query_cells
 
@@ -109,11 +110,7 @@ def test_valid0_scales_masks_and_devices_are_validated():
 
 @pytest.mark.parametrize("version", [110, 109])
 def test_match_points_refuses_a_library_without_its_entries(monkeypatch, version):
-    class OldLib:   # a build from before the point entries: same versions, no lb_coarse_query / centre gather
-        def lb_version(self):
-            return version
-
-    monkeypatch.setattr(_lib, "load", lambda: OldLib())
+    util.old_library(monkeypatch, version)   # a build from before the point entries: no lb_coarse_query / centre gather
     assert _lib.POINTS_ENTRIES == ("lb_coarse_query", "lb_fine_preprocess_centres")
     model = _model()
     with pytest.raises(RuntimeError, match=rf"match_points needs lb_coarse_query, which .* \(version {version}\) does "
@@ -135,18 +132,7 @@ def test_load_binds_the_point_entries_only_where_exported(monkeypatch, tmp_path)
         assert name not in _lib._SINCE
         assert _lib.SIGNATURES[name][1] == getattr(lib, name).argtypes
     _lib.require_entries(_lib.POINTS_ENTRIES, "match_points")
-
-    class Exports:   # what ctypes.CDLL gives for a build without them: every other declared symbol, no point entries
-        def __init__(self):
-            for name in _lib.SIGNATURES:
-                if name not in _lib.POINTS_ENTRIES:
-                    setattr(self, name, type("Fn", (), {})())
-            self.lb_version = lambda: 110
-
-    monkeypatch.setattr(_lib, "_lib", None)
-    monkeypatch.setattr(_lib.C, "CDLL", lambda path: Exports())
-    monkeypatch.setattr(_lib.os.path, "exists", lambda path: True)
-    old = _lib.load()
+    old = util.load_without(monkeypatch, _lib.POINTS_ENTRIES)
     assert not any(hasattr(old, n) for n in _lib.POINTS_ENTRIES)
     assert old.lb_coarse_match.argtypes == _lib.SIGNATURES["lb_coarse_match"][1]
     with pytest.raises(RuntimeError, match=r"needs lb_coarse_query.*\(version 110\)"):

@@ -16,29 +16,8 @@ CASE = {c["name"]: c for c in CASES}
 Q_KEYS = ("qpts0_f", "qpts1_c", "qpts1_f", "qexpec_f", "qconf", "q_i_ids", "q_j_ids", "qmutual", "qvalid", "qinside")
 
 
-def _model(case, backbone_impl="auto", precision="split"):
-    model, cfg, _ = util.build_model(case, DEV, backbone_impl=backbone_impl, match_precision=precision)
-    return model, cfg
-
-
-def _inputs(data):
-    return {k: v for k, v in data.items() if k in ("image0", "image1", "mask0", "mask1", "scale0", "scale1")}
-
-
-def _grid_points(data):
-    """Every cell keypoint of image0 in source pixels, computed as the forward computes mkpts0_c -> [N, L, 2]."""
-    n, _, h, w = data["image0"].shape
-    hc, wc = h // 8, w // 8
-    i = torch.arange(hc * wc, device=DEV)
-    cell = torch.stack([i % wc, i // wc], 1).float()[None].expand(n, -1, -1)
-    s = torch.full((n, 1, 2), 8.0, device=DEV)
-    if "scale0" in data:
-        s = 8.0 * data["scale0"][:, None, :]
-    return (cell * s).contiguous()
-
-
 def _match(model, data, pts, valid0=None):
-    out = _inputs(data)
+    out = util.inputs(data)
     model.match_points(out, pts, valid0)
     return out
 
@@ -51,16 +30,16 @@ GRID = [
     ("ot_thr0", CASE["ot_thr0"], {}),
     ("ot_prefilter", CASE["ot_prefilter"], {}),
     ("full_attention", dict(CASE["ds_thr0"], coarse_attention="full", fine_attention="full"), {}),
-    ("fp16", CASE["ds_thr0"], {"backbone_impl": "b200_fp16", "precision": "fp16"}),
+    ("fp16", CASE["ds_thr0"], {"backbone_impl": "b200_fp16", "match_precision": "fp16"}),
 ]
 
 
 @pytest.mark.parametrize("name, case, opts", GRID, ids=[g[0] for g in GRID])
 def test_grid_queries_equal_the_forward_bit_for_bit(name, case, opts):
-    model, _ = _model(case, **opts)
+    model, _, _ = util.build_model(case, DEV, **opts)
     data = util.device_inputs(case)
     fwd = util.eager(model, data)
-    q = _match(model, data, _grid_points(data))
+    q = _match(model, data, util.grid_points(data))
     n, L = q["qvalid"].shape
     b, i = fwd["b_ids"], fwd["i_ids"]
     if name == "ot_prefilter":   # the prefilter removes every row and column of this pair: nothing is kept or valid
@@ -97,7 +76,7 @@ def _offgrid_points(n, h, w, seed):
 
 @pytest.mark.parametrize("case", [CASE["ds_thr0"], CASE["ds_unequal"]], ids=["ds_thr0", "ds_unequal"])
 def test_offgrid_queries_vs_f64(case):
-    model, cfg = _model(case)
+    model, cfg, _ = util.build_model(case, DEV)
     data = util.device_inputs(case)
     n, _, h, w = data["image0"].shape
     pts = _offgrid_points(n, h, w, 5)
@@ -164,7 +143,7 @@ def _assert_unanswered(q, sel, label):
 
 def test_edges_valid0_nan_outside_masked_and_duplicates():
     case = CASE["ot_masked"]   # n = 1, 128 x 128, image0 valid in 128 x 96: cells with x >= 12 are masked
-    model, _ = _model(case)
+    model, _, _ = util.build_model(case, DEV)
     data = util.device_inputs(case)
     s = data["scale0"][0]
     img = lambda x, y: [x * float(s[0]), y * float(s[1])]   # network pixels -> source pixels
@@ -189,7 +168,7 @@ def test_edges_valid0_nan_outside_masked_and_duplicates():
 
 def test_row_without_a_valid_column_has_no_answer():
     case = CASE["ds_masked_scaled"]
-    model, _ = _model(case)
+    model, _, _ = util.build_model(case, DEV)
     data = util.device_inputs(case)
     data["mask1"][1] = False   # pair 1: every column masked
     pts = torch.tensor([[[40.0, 40.0], [64.0, 32.0]]] * 2, dtype=torch.float32, device=DEV) * data["scale0"][:, None]
@@ -200,7 +179,7 @@ def test_row_without_a_valid_column_has_no_answer():
 
 def test_q1_n1_and_q0():
     case = CASE["ds_unequal"]
-    model, _ = _model(case)
+    model, _, _ = util.build_model(case, DEV)
     data = util.device_inputs(case)
     q = _match(model, data, torch.tensor([[[17.25, 33.5]]], device=DEV))
     assert q["qinside"].shape == (1, 1) and q["qinside"].item()
@@ -216,14 +195,13 @@ def test_q1_n1_and_q0():
 # ------------------------------------------------------------------------------------------------ independence
 def test_queries_are_independent():
     case = CASE["ds_thr0"]
-    model, _ = _model(case)
+    model, _, _ = util.build_model(case, DEV)
     data = util.device_inputs(case)
     n, _, h, w = data["image0"].shape
     pts = _offgrid_points(n, h, w, 9)
     full = _match(model, data, pts)
     again = _match(model, data, pts)
-    for k in Q_KEYS:   # two eager calls are identical
-        assert torch.equal(torch.nan_to_num(full[k].float()), torch.nan_to_num(again[k].float())), k
+    util.assert_same(again, full, Q_KEYS, "two eager calls")
     for sub in (torch.arange(0, pts.shape[1], 7), torch.tensor([5]), torch.arange(pts.shape[1] - 3, pts.shape[1])):
         part = _match(model, data, pts[:, sub.to(DEV)].contiguous())
         for k in Q_KEYS:
@@ -233,13 +211,13 @@ def test_queries_are_independent():
 # ------------------------------------------------------------------------------------------------ graph capture
 def test_graph_capture_replays_new_points():
     case = CASE["ds_masked_scaled"]
-    model, _ = _model(case)
+    model, _, _ = util.build_model(case, DEV)
     data = util.device_inputs(case)
     n, _, h, w = data["image0"].shape
     s = data["scale0"][:, None]
     pts_a = (_offgrid_points(n, h, w, 1) * s).contiguous()
     pts_b = (_offgrid_points(n, h, w, 2) * s).contiguous()
-    static_in, static_pts = _inputs(data), pts_a.clone()
+    static_in, static_pts = util.inputs(data), pts_a.clone()
     model.match_points(dict(static_in), static_pts)   # eager warm-up (weight packing)
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())
@@ -253,7 +231,4 @@ def test_graph_capture_replays_new_points():
         static_pts.copy_(pts)
         graph.replay()
         torch.cuda.synchronize()
-        ref = _match(model, data, pts)
-        for k in Q_KEYS:
-            assert torch.equal(torch.nan_to_num(out[k].float()), torch.nan_to_num(ref[k].float())), k
-            assert torch.equal(torch.isnan(out[k].float()), torch.isnan(ref[k].float())), k
+        util.assert_same(out, _match(model, data, pts), Q_KEYS, "graph replay")

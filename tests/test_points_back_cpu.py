@@ -8,19 +8,13 @@ import pytest
 import torch
 
 import loftr_b200
+import util
 from loftr_b200 import _lib
 from loftr_b200 import loftr as LM
-from loftr_b200.loftr import ImageFeatures
 
 
 def _model():
     return loftr_b200.LoFTR(loftr_b200.get_cfg("indoor_ds")).eval()
-
-
-def _bank(model, k=3):
-    """A host bank of k 96x128 images tied to the model's current weights (never matched: nothing here launches)."""
-    return ImageFeatures(torch.zeros(k, 256, 12, 16), torch.zeros(k, 128, 48, 64), None, torch.Size((96, 128)),
-                         torch.Size((12, 16)), torch.Size((48, 64)), model._bank_key())
 
 
 def _idx(*v):
@@ -33,18 +27,12 @@ def _data():
 
 @pytest.fixture
 def no_stages(monkeypatch):
-    """The matching stages of the model raise if reached: validation must stop a call before them."""
-    def reached(*a, **k):
-        raise AssertionError("a matching stage was reached")
-    model = _model()
-    for name in ("_match_points", "_coarse_tokens", "_backbone", "_backbone_pairs"):
-        monkeypatch.setattr(model, name, reached)
-    return model
+    return util.stages_unreachable(monkeypatch, _model())
 
 
 def _calls(m):
     """(who, call(**query kwargs)) for both query methods on two pairs."""
-    bank = _bank(m)
+    bank = util.host_bank(m)
     return [("match_points", lambda **kw: m.match_points(_data(), **kw)),
             ("match_points_features", lambda **kw: m.match_points_features(bank, _idx(0, 1), bank, _idx(1, 2), **kw))]
 
@@ -115,7 +103,7 @@ def test_q0_and_an_empty_pair_list_give_empty_outputs(monkeypatch):
         monkeypatch.setattr(m, name, lambda *a, **k: (_ for _ in ()).throw(AssertionError("reached")))
     launches = _lib.load().lb_launch_count
     n_launch = launches()
-    bank = _bank(m)
+    bank = util.host_bank(m)
     side1 = {"qpts1_f", "qpts0_c", "qpts0_f", "qexpec_f", "qconf", "q_i_ids", "q_j_ids", "qmutual", "qvalid",
              "qinside"}
     back = {"qback_pts", "qback_conf", "qback_valid", "qback_inside", "qfb_err"}
@@ -143,18 +131,7 @@ def test_entries_are_bound_only_where_exported(monkeypatch):
         assert name not in _lib._SINCE and name in _lib._OPTIONAL
         assert getattr(lib, name).argtypes == _lib.SIGNATURES[name][1]
     assert lib.lb_version() == 110
-
-    class Exports:   # what ctypes.CDLL gives for a build without the two entries: every other declared symbol
-        def __init__(self):
-            for n in _lib.SIGNATURES:
-                if n not in _lib.SIDE_POINTS_ENTRIES:
-                    setattr(self, n, type("Fn", (), {})())
-            self.lb_version = lambda: 110
-
-    monkeypatch.setattr(_lib, "_lib", None)
-    monkeypatch.setattr(_lib.C, "CDLL", lambda path: Exports())
-    monkeypatch.setattr(_lib.os.path, "exists", lambda path: True)
-    old = _lib.load()
+    old = util.load_without(monkeypatch, _lib.SIDE_POINTS_ENTRIES)
     assert not any(hasattr(old, n) for n in _lib.SIDE_POINTS_ENTRIES)
     _lib.require_entries(_lib.POINTS_ENTRIES + _lib.BANK_POINTS_ENTRIES, "the image0 queries")
     m = _model()

@@ -3,7 +3,7 @@
    mconf and flags bit for bit, with the forward's windows; qmutual / qvalid / the mutual qconf are the image0-side
    answers of the same cell pair (split and fp16, dual-softmax and Sinkhorn with and without the prefilter, linear and
    full attention, 832 x 832 masks and scales);
-2. off-grid image1 queries against float64 (tests/points_back_ref.py): the column arg-max, both qconf expressions, the
+2. off-grid image1 queries against float64 (tests/points_ref.py): the column arg-max, both qconf expressions, the
    centres and the mirrored fine match on the stored stage inputs, at the image edges and window borders; masked cells
    and columns without a valid row are not answered;
 3. the back leg of a round trip equals a separate call from the other image at the first answer, from both sides,
@@ -16,7 +16,7 @@ import pytest
 import torch
 
 from loftr_b200 import _lib
-import points_back_ref as PB
+import points_ref as P
 import ref64 as R
 import util
 from cases import BASELINE_CASES, CASES
@@ -24,36 +24,13 @@ from cases import BASELINE_CASES, CASES
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 CASE = {c["name"]: c for c in CASES}
-INPUTS = ("image0", "image1", "mask0", "mask1", "scale0", "scale1")
 BACK = ("qback_pts", "qback_conf", "qback_valid", "qback_inside", "qfb_err")
-H_MODEL = np.array([[1.03, 0.04, 6.0], [-0.03, 0.97, -5.0], [2e-5, -1e-5, 1.0]], np.float32)
-
-
-def _model(case, backbone_impl="auto", precision="split"):
-    model, cfg, _ = util.build_model(case, DEV, backbone_impl=backbone_impl, match_precision=precision)
-    return model, cfg
-
-
-def _inputs(data):
-    return {k: v for k, v in data.items() if k in INPUTS}
 
 
 def _query(model, data, side, pts, valid=None, **kw):
-    out = _inputs(data)
+    out = util.inputs(data)
     model.match_points(out, **{f"points{side}": pts, f"valid{side}": valid}, **kw)
-    return {k: v for k, v in out.items() if k not in INPUTS}
-
-
-def _grid_points(data, side):
-    """Every cell keypoint of image `side` in source pixels, as the forward computes mkpts{side}_c -> [N, cells, 2]."""
-    n, _, h, w = data[f"image{side}"].shape
-    hc, wc = h // 8, w // 8
-    i = torch.arange(hc * wc, device=DEV)
-    cell = torch.stack([i % wc, i // wc], 1).float()[None].expand(n, -1, -1)
-    s = torch.full((n, 1, 2), 8.0, device=DEV)
-    if f"scale{side}" in data:
-        s = 8.0 * data[f"scale{side}"][:, None, :]
-    return (cell * s).contiguous()
+    return util.outputs(out)
 
 
 def _offgrid_points(n, h, w, seed, q=150):
@@ -67,21 +44,6 @@ def _offgrid_points(n, h, w, seed, q=150):
     return torch.tensor(np.stack(pts), dtype=torch.float32, device=DEV)
 
 
-def _same(a, b):
-    a, b = a.float(), b.float()
-    return a.shape == b.shape and torch.equal(torch.nan_to_num(a), torch.nan_to_num(b)) and \
-        torch.equal(torch.isnan(a), torch.isnan(b))
-
-
-def _assert_bitwise(got, ref, label, keys=None):
-    keys = list(ref) if keys is None else keys
-    for k in keys:
-        if not torch.is_tensor(ref[k]):   # bs and the sizes
-            assert got[k] == ref[k], (label, k)
-            continue
-        assert got[k].dtype == ref[k].dtype and _same(got[k], ref[k]), f"{label}: {k} differs"
-
-
 # ------------------------------------------------------------------------------------------------ 1. mirror
 GRID = [
     ("ds_thr0_border2", CASE["ds_thr0"], {}),
@@ -90,18 +52,18 @@ GRID = [
     ("ot_thr0", CASE["ot_thr0"], {}),
     ("ot_prefilter", CASE["ot_prefilter"], {}),
     ("full_attention", dict(CASE["ds_thr0"], coarse_attention="full", fine_attention="full"), {}),
-    ("fp16", CASE["ds_thr0"], {"backbone_impl": "b200_fp16", "precision": "fp16"}),
-    ("ot_fp16", CASE["ot_thr0"], {"precision": "fp16"}),
+    ("fp16", CASE["ds_thr0"], {"backbone_impl": "b200_fp16", "match_precision": "fp16"}),
+    ("ot_fp16", CASE["ot_thr0"], {"match_precision": "fp16"}),
 ]
 
 
 @pytest.mark.parametrize("name, case, opts", GRID, ids=[g[0] for g in GRID])
 def test_image1_grid_queries_mirror_the_forward(name, case, opts):
-    model, _ = _model(case, **opts)
+    model, _, _ = util.build_model(case, DEV, **opts)
     data = util.device_inputs(case)
     fwd = util.eager(model, data)
-    q = _query(model, data, 1, _grid_points(data, 1))
-    q0 = _query(model, data, 0, _grid_points(data, 0))   # the image0 side of every cell pair
+    q = _query(model, data, 1, util.grid_points(data, 1))
+    q0 = _query(model, data, 0, util.grid_points(data, 0))   # the image0 side of every cell pair
     n, S = q["qvalid"].shape
     b, i, j = fwd["b_ids"], fwd["i_ids"], fwd["j_ids"]
     if name == "ot_prefilter":   # the prefilter removes every row and column of this pair: nothing is kept or valid
@@ -150,7 +112,7 @@ QCONF_RTOL = 1e-3   # |qconf - conf64| / conf64, both expressions (DESIGN.md §2
 @pytest.mark.parametrize("name", ["ds_thr0", "ds_unequal", "ot_thr0"])
 def test_image1_offgrid_queries_vs_f64(name):
     case = CASE[name]
-    model, cfg = _model(case)
+    model, cfg, _ = util.build_model(case, DEV)
     data = util.device_inputs(case)
     n, _, h1, w1 = data["image1"].shape
     pts = _offgrid_points(n, h1, w1, 5)
@@ -165,17 +127,17 @@ def test_image1_offgrid_queries_vs_f64(name):
     nq = pts.shape[1]
     b_ids = torch.arange(n, device=DEV)[:, None].expand(-1, nq).reshape(-1)
     i_ids, j_ids = q["q_i_ids"].reshape(-1), q["q_j_ids"].reshape(-1)
-    # rules 1 and 2 on image1
+    # rules 1 and 2 on image1: image0's with image1's sizes
     cells, f1s = [], []
     for b in range(n):
-        inside, cell, f1 = PB.query_cells(pts[b].cpu().numpy(), None, hw1_i, hw1_c, hw1_f)
+        inside, cell, f1 = P.query_cells(pts[b].cpu().numpy(), None, hw1_i, hw1_c, hw1_f)
         assert inside.all()
         cells.append(cell)
         f1s.append(f1)
     cell, f1 = np.concatenate(cells), np.concatenate(f1s)
     assert (cell[:, 1] * hw1_c[1] + cell[:, 0] == j_ids.cpu().numpy()).all()
     # rule 3: i against the float64 column arg-max, near-ties excepted; qconf within QCONF_RTOL of conf64[b, i, j]
-    i64, _, _ = PB.column_answer(conf64, b_ids, j_ids)
+    i64, _, _ = P.column_answer(conf64, b_ids, j_ids)
     cols = conf64[b_ids, :, j_ids]
     top = cols.topk(2, dim=1).values
     for k in torch.nonzero(i64 != i_ids).flatten().tolist():
@@ -189,14 +151,14 @@ def test_image1_offgrid_queries_vs_f64(name):
         err = rel[sel].max().item()
         util.record(f"points_back_qconf_{name}_{label}", {"max_rel_err": err, "queries": int(sel.sum())})
         assert err <= QCONF_RTOL, f"{label} qconf: relative error {err:.3e}"
-    # rule 4: the centres
-    f0 = PB.image0_centres(cell, f1, i_ids.cpu().numpy(), w0c, stride)
+    # rule 4: the centres, image0's rule with the images swapped
+    f0 = P.image1_centres(cell, f1, i_ids.cpu().numpy(), w0c, stride)
     assert torch.equal(q["qpts1_f"].reshape(-1, 2).cpu(), torch.tensor(2.0 * f1, dtype=torch.float32))
     assert torch.equal(q["qpts0_c"].reshape(-1, 2).cpu(), torch.tensor(2.0 * f0, dtype=torch.float32))
     # rule 5: the mirrored fine match from the kernel's own cell pairs, against float64 and its float32 emulation
     pts0_c = q["qpts0_c"].reshape(-1, 2)
-    refs = {dt: PB.fine_stage_back(model, ff0.to(dt), ff1.to(dt), x0.to(dt), x1.to(dt), b_ids, i_ids, j_ids, f0, f1,
-                                   pts0_c, hw0_i, dtype=dt) for dt in (torch.float64, torch.float32)}
+    refs = {dt: P.fine_stage(model, ff0.to(dt), ff1.to(dt), x0.to(dt), x1.to(dt), b_ids, i_ids, j_ids, f0, f1,
+                             pts0_c, hw0_i, dtype=dt, side=1) for dt in (torch.float64, torch.float32)}
     for k, got in (("qexpec_f", q["qexpec_f"].reshape(-1, 3)), ("qpts0_f", q["qpts0_f"].reshape(-1, 2))):
         idx = 0 if k == "qexpec_f" else 1
         ref, emu = refs[torch.float64][idx], refs[torch.float32][idx].double()
@@ -217,7 +179,7 @@ def _assert_unanswered(q, sel, label):
 
 def test_masked_cells_and_columns_without_a_valid_row():
     case = CASE["ds_masked_scaled"]
-    model, _ = _model(case)
+    model, _, _ = util.build_model(case, DEV)
     data = util.device_inputs(case)
     n, _, h, w = data["image1"].shape
     pts = (_offgrid_points(n, h, w, 6, q=60) * data["scale1"][:, None]).contiguous()
@@ -245,26 +207,26 @@ def _check_round_trip(call, side, pts, label):
     rt = call(side, pts, None, True)
     plain = call(side, pts, None, False)
     assert set(rt) == set(plain) | set(BACK), label
-    _assert_bitwise(rt, plain, f"{label}: first leg", keys=list(plain))
+    util.assert_same(rt, plain, label=f"{label}: first leg")
     other = 1 - side
     back = call(other, rt[f"qpts{other}_f"], rt["qinside"], False)
     for k, ref in (("qback_pts", f"qpts{side}_f"), ("qback_conf", "qconf"), ("qback_valid", "qvalid"),
                    ("qback_inside", "qinside")):
-        assert rt[k].dtype == back[ref].dtype and _same(rt[k], back[ref]), f"{label}: {k} differs from {ref}"
+        util.assert_same(rt[k], back[ref], label=f"{label}: {k} against {ref}")
     err = torch.linalg.vector_norm(rt["qback_pts"] - pts, dim=-1).masked_fill_(~rt["qback_inside"], float("nan"))
-    assert _same(rt["qfb_err"], err), label
+    util.assert_same(rt["qfb_err"], err, label=f"{label}: qfb_err")
     assert rt["qback_inside"].any() and not (rt["qback_inside"] & ~rt["qinside"]).any(), label
     assert torch.isfinite(rt["qfb_err"][rt["qback_inside"]]).all(), label
     return rt
 
 
-RT = [("ds_masked_scaled", {}), ("ds_unequal", {}), ("ot_thr0", {"precision": "fp16"})]
+RT = [("ds_masked_scaled", {}), ("ds_unequal", {}), ("ot_thr0", {"match_precision": "fp16"})]
 
 
 @pytest.mark.parametrize("name, opts", RT, ids=[r[0] for r in RT])
 def test_round_trip_back_leg_equals_a_call_from_the_other_image(name, opts):
     case = CASE[name]
-    model, _ = _model(case, **opts)
+    model, _, _ = util.build_model(case, DEV, **opts)
     data = util.device_inputs(case)
     call = lambda side, pts, valid, rt: _query(model, data, side, pts, valid, round_trip=rt)
     for side in (0, 1):
@@ -279,7 +241,7 @@ def test_round_trip_back_leg_equals_a_call_from_the_other_image(name, opts):
 
 def test_the_back_leg_runs_no_score_pass():
     case = CASE["ds_thr0"]
-    model, _ = _model(case)
+    model, _, _ = util.build_model(case, DEV)
     data = util.device_inputs(case)
     n, _, h, w = data["image0"].shape
     pts = _offgrid_points(n, h, w, 9, q=40)
@@ -298,19 +260,9 @@ def test_the_back_leg_runs_no_score_pass():
 
 
 # ------------------------------------------------------------------------------------------------ 3, 4. banks
-def _idx(v):
-    return torch.tensor(v, dtype=torch.int64, device=DEV)
-
-
-def _frames(case):
-    d = util.device_inputs(case)
-    cat = lambda k: torch.cat([d[k + "0"], d[k + "1"]]) if k + "0" in d else None
-    return cat("image"), cat("mask"), cat("scale")
-
-
 BANK_MODES = [
     ("ds_b200_split", "ds_thr0", {}),
-    ("ds_fp16backbone_fp16match", "ds_thr0", {"backbone_impl": "b200_fp16", "precision": "fp16"}),
+    ("ds_fp16backbone_fp16match", "ds_thr0", {"backbone_impl": "b200_fp16", "match_precision": "fp16"}),
     ("sinkhorn", "ot_thr0", {}),
     ("masked_scaled", "ds_masked_scaled", {}),
 ]
@@ -319,10 +271,10 @@ BANK_MODES = [
 @pytest.mark.parametrize("name, case, opts", BANK_MODES, ids=[m[0] for m in BANK_MODES])
 def test_bank_image1_queries_and_round_trips_equal_stacked(name, case, opts):
     case = CASE[case]
-    model, _ = _model(case, **opts)
-    imgs, masks, scales = _frames(case)
+    model, _, _ = util.build_model(case, DEV, **opts)
+    imgs, masks, scales = util.frames(case)
     bank = model.extract_features(imgs, masks)
-    idx0, idx1 = _idx([0, 1, 2, 2]), _idx([1, 2, 3, 3])
+    idx0, idx1 = util.idx([0, 1, 2, 2]), util.idx([1, 2, 3, 3])
     data = {"image0": imgs[idx0], "image1": imgs[idx1]}
     if masks is not None:
         data["mask0"], data["mask1"] = masks[idx0], masks[idx1]
@@ -337,49 +289,44 @@ def test_bank_image1_queries_and_round_trips_equal_stacked(name, case, opts):
                                               **{f"points{side}": p}, round_trip=rt)
             ref = _query(model, data, side, p, round_trip=rt)
             assert set(got) == set(ref), name
-            _assert_bitwise(got, ref, f"{name} side {side} round_trip {rt}")
+            util.assert_same(got, ref, label=f"{name} side {side} round_trip {rt}")
             assert got["qinside"].any()
-
-
-def _guide(models, radius=20.0, kind="homography"):
-    return {"kind": kind, "model": torch.as_tensor(np.ascontiguousarray(models, np.float32)).to(DEV),
-            "radius": radius}
 
 
 def test_bank_round_trips_with_a_guide_and_an_all_nan_guide():
     case = CASE["ds_thr0"]
-    model, _ = _model(case)
-    imgs, _, _ = _frames(case)
+    model, _, _ = util.build_model(case, DEV)
+    imgs, _, _ = util.frames(case)
     bank = model.extract_features(imgs)
-    idx0, idx1 = _idx([0, 1, 2, 0]), _idx([1, 2, 3, 1])
-    models = np.repeat(H_MODEL[None], 4, 0)
+    idx0, idx1 = util.idx([0, 1, 2, 0]), util.idx([1, 2, 3, 1])
+    models = np.repeat(util.H_MODEL[None], 4, 0)
     models[-1] = np.nan   # the last pair repeats the first, unguided
     h, w = imgs.shape[2:]
     pts = _offgrid_points(4, h, w, 11, q=120)
-    for guide in (_guide(models), None):
+    for guide in (util.guide("homography", models, 20.0), None):
         def call(side, p, valid, rt):
             return model.match_points_features(bank, idx0, bank, idx1, guide=guide, round_trip=rt,
                                                **{f"points{side}": p, f"valid{side}": valid})
         for side in (0, 1):
             _check_round_trip(call, side, pts, f"guide {guide is not None} side {side}")
-    nan_guide = _guide(np.full((4, 3, 3), np.nan))
+    nan_guide = util.guide("homography", np.full((4, 3, 3), np.nan), 20.0)
     for side in (0, 1):
         got = model.match_points_features(bank, idx0, bank, idx1, guide=nan_guide, round_trip=True,
                                           **{f"points{side}": pts})
         ref = model.match_points_features(bank, idx0, bank, idx1, round_trip=True, **{f"points{side}": pts})
-        _assert_bitwise(got, ref, f"NaN guide side {side}")
+        util.assert_same(got, ref, label=f"NaN guide side {side}")
 
 
 # ------------------------------------------------------------------------------------------------ 6. graph capture
 def test_graph_capture_of_a_round_trip_replays_the_eager_call():
     case = CASE["ds_masked_scaled"]
-    model, _ = _model(case)
+    model, _, _ = util.build_model(case, DEV)
     data = util.device_inputs(case)
     n, _, h, w = data["image1"].shape
     s = data["scale1"][:, None]
     pts_a = (_offgrid_points(n, h, w, 12) * s).contiguous()
     pts_b = (_offgrid_points(n, h, w, 13) * s).contiguous()
-    static_in, static_pts = _inputs(data), pts_a.clone()
+    static_in, static_pts = util.inputs(data), pts_a.clone()
     model.match_points(dict(static_in), points1=static_pts, round_trip=True)   # eager warm-up (weight packing)
     stream = torch.cuda.Stream()
     stream.wait_stream(torch.cuda.current_stream())
@@ -394,4 +341,4 @@ def test_graph_capture_of_a_round_trip_replays_the_eager_call():
         graph.replay()
         torch.cuda.synchronize()
         ref = _query(model, data, 1, pts, round_trip=True)
-        _assert_bitwise({k: out[k] for k in ref}, ref, "graph replay")
+        util.assert_same(out, ref, label="graph replay")

@@ -11,6 +11,7 @@ import torch
 
 import loftr_b200
 import preprocess_ref as ref
+import util
 from loftr_b200 import _lib, preprocess
 from preprocess_cases import GREY_HW, GREY_SEED, IMAGE_CASES, SIZE_CASES, image
 
@@ -147,11 +148,7 @@ def test_descs_cache_is_for_device_images():
 
 
 def test_front_end_refuses_an_older_library(monkeypatch):
-    class OldLib:
-        def lb_version(self):
-            return 105
-
-    monkeypatch.setattr(_lib, "load", lambda: OldLib())
+    util.old_library(monkeypatch, 105)
     assert _lib.PREPROCESS_VERSION == 106
     for call in (lambda: loftr_b200.prepare_images([_u8(16, 16)]),
                  lambda: loftr_b200.prepare_pairs([_u8(16, 16)], [_u8(16, 16)])):

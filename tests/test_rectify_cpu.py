@@ -7,6 +7,7 @@ import torch
 
 import loftr_b200
 import rectify_ref as RR
+import util
 from loftr_b200 import _lib
 from loftr_b200.loftr import CapturedMatcher, check_rectify
 
@@ -83,18 +84,7 @@ def test_rectify_entries_are_bound_only_where_exported(monkeypatch):
     _lib.require_entries(_lib.RECTIFY_ENTRIES, "rectified matching")
     names = {lib.lb_timing_tag_name(i).decode() for i in range(lib.lb_timing_num_tags())}
     assert "rectify" in names
-
-    class Exports:   # every other declared symbol, as a build without the rectify entries is loaded
-        def __init__(self):
-            for name in _lib.SIGNATURES:
-                if name not in _lib.RECTIFY_ENTRIES:
-                    setattr(self, name, type("Fn", (), {})())
-            self.lb_version = lambda: 110
-
-    monkeypatch.setattr(_lib, "_lib", None)
-    monkeypatch.setattr(_lib.C, "CDLL", lambda path: Exports())
-    monkeypatch.setattr(_lib.os.path, "exists", lambda path: True)
-    old = _lib.load()
+    old = util.load_without(monkeypatch, _lib.RECTIFY_ENTRIES)
     assert not hasattr(old, "lb_rectify_images") and not hasattr(old, "lb_rectify_points")
     assert old.lb_coarse_match_guided.argtypes == _lib.SIGNATURES["lb_coarse_match_guided"][1]   # the rest still binds
     _lib.require_entries(_lib.GUIDE_ENTRIES + _lib.POINTS_ENTRIES, "other paths")

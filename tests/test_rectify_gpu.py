@@ -10,8 +10,6 @@ GPU:
 4. a pair's outputs do not depend on the other pairs' models;
 5. a match_points query at a rectified match's mkpts0_c returns that match's mapped points;
 6. forward_static with rectify1 captured into a CUDA graph follows the model tensor from replay to replay."""
-import math
-
 import numpy as np
 import pytest
 import torch
@@ -25,47 +23,12 @@ from match_cap_ref import LIST_KEYS
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 _CASE = {c["name"]: c for c in CASES}
-INPUTS = ("image0", "image1", "mask0", "mask1", "scale0", "scale1", "rectify1")
+INPUTS = util.INPUT_KEYS + ("rectify1",)
 ULP1 = 4 * float(np.finfo(np.float32).eps)   # 4 fp32 ulps of 1.0
-
-
-def _t(x, dtype=torch.float32):
-    return torch.as_tensor(np.ascontiguousarray(x)).to(DEV, dtype)
-
-
-def _similarity(c0, c1, deg, zoom, persp=(0.0, 0.0)):
-    """x1 = c1 + zoom R(deg) (x0 - c0), with a perspective row (persp, 1) in the centred frame."""
-    a = math.radians(deg)
-    t0 = np.array([[1, 0, -c0[0]], [0, 1, -c0[1]], [0, 0, 1]])
-    t1 = np.array([[1, 0, c1[0]], [0, 1, c1[1]], [0, 0, 1]])
-    r = np.array([[zoom * math.cos(a), -zoom * math.sin(a), 0], [zoom * math.sin(a), zoom * math.cos(a), 0],
-                  [persp[0], persp[1], 1]])
-    return t1 @ r @ t0
 
 
 def _centre(hw, s=(1.0, 1.0)):
     return (0.5 * (hw[1] - 1) * s[0], 0.5 * (hw[0] - 1) * s[1])
-
-
-def _same(a, b):
-    """Bitwise equality of two outputs, NaN at the same places counting as equal."""
-    if not torch.is_tensor(a):
-        return a == b
-    if a.dtype != b.dtype or a.shape != b.shape:
-        return False
-    if a.is_floating_point():
-        na, nb = torch.isnan(a), torch.isnan(b)
-        return torch.equal(na, nb) and torch.equal(a[~na], b[~nb])
-    return torch.equal(a, b)
-
-
-def _assert_same(got, ref, keys, label):
-    for k in keys:
-        assert _same(got[k], ref[k]), f"{label}: {k} differs"
-
-
-def _outputs(d):
-    return [k for k in d if k not in INPUTS]
 
 
 # ------------------------------------------------------------------------------------------------ 1. the warp
@@ -74,15 +37,17 @@ def _warp_case(name):
     if name == "canvas200_scaled":
         n, hw1, hw = 3, (40, 56), (48, 200)
         s0, s1 = rs.uniform(0.6, 1.4, (n, 2)), rs.uniform(0.6, 1.4, (n, 2))
-        models = [_similarity(_centre(hw, s0[b]), _centre(hw1, s1[b]), deg, zoom, persp)
+        models = [util.similarity(_centre(hw, s0[b]), _centre(hw1, s1[b]), deg, zoom, persp)
                   for b, (deg, zoom, persp) in enumerate(((7, 0.3, (1e-4, -2e-4)), (-20, 0.25, (0, 0)),
                                                            (90, 0.35, (-3e-4, 1e-4))))]
     elif name == "image1_smaller":
         n, hw1, hw, s0, s1 = 2, (24, 32), (64, 96), None, None
-        models = [_similarity(_centre(hw), _centre(hw1), 3, 0.45), _similarity(_centre(hw), (30.0, 20.0), -12, 0.5)]
+        models = [util.similarity(_centre(hw), _centre(hw1), 3, 0.45),
+                  util.similarity(_centre(hw), (30.0, 20.0), -12, 0.5)]
     elif name == "image1_larger":
         n, hw1, hw, s0, s1 = 2, (96, 136), (40, 48), None, None
-        models = [_similarity(_centre(hw), _centre(hw1), 30, 2.5), _similarity(_centre(hw), _centre(hw1), 180, 2.9)]
+        models = [util.similarity(_centre(hw), _centre(hw1), 30, 2.5),
+                  util.similarity(_centre(hw), _centre(hw1), 180, 2.9)]
     elif name == "edges":   # samples on the last row / column, a quarter pixel beyond it, and before the first
         n, hw1, hw, s0, s1 = 4, (32, 40), (32, 40), None, None
         models = [np.array([[1, 0, tx], [0, 1, ty], [0, 0, 1]], np.float64)
@@ -91,7 +56,7 @@ def _warp_case(name):
         n, hw1, hw, s0, s1 = 3, (48, 64), (48, 128), None, None
         models = [np.array([[1, 0, 0], [0, 1, 0], [-0.012, 0, 1.0]]),   # w = 0 at x = 83: the horizon crosses
                   np.full((3, 3), np.nan),
-                  -_similarity(_centre(hw), _centre(hw1), 15, 0.6, (2e-3, 0))]
+                  -util.similarity(_centre(hw), _centre(hw1), 15, 0.6, (2e-3, 0))]
     else:
         raise KeyError(name)
     img = rs.rand(n, 1, *hw1).astype(np.float32)
@@ -106,8 +71,8 @@ WARP_CASES = ["canvas200_scaled", "image1_smaller", "image1_larger", "edges", "h
 @pytest.mark.parametrize("name", WARP_CASES)
 def test_warp_images_vs_float64(name):
     img, models, hw, s0, s1 = _warp_case(name)
-    got = loftr_b200.warp_images(_t(img), _t(models), hw, None if s0 is None else _t(s0),
-                                 None if s1 is None else _t(s1))
+    got = loftr_b200.warp_images(util.to_dev(img), util.to_dev(models), hw, None if s0 is None else util.to_dev(s0),
+                                 None if s1 is None else util.to_dev(s1))
     torch.cuda.synchronize()
     assert got.shape == (img.shape[0], 1, *hw) and got.dtype == torch.float32
     ref, u, v = RR.warp(img, models, hw, s0, s1)
@@ -133,9 +98,9 @@ def test_warp_images_vs_float64(name):
 def test_warp_images_is_bitwise_image1_for_the_identity_with_scales():
     rs = np.random.RandomState(2)
     img = rs.rand(3, 1, 48, 72).astype(np.float32)
-    s = _t(rs.uniform(0.5, 2.5, (3, 2)))
-    models = _t(np.stack([np.eye(3), np.full((3, 3), np.inf), -np.eye(3)]))
-    got = loftr_b200.warp_images(_t(img), models, (48, 72), s, s.clone())
+    s = util.to_dev(rs.uniform(0.5, 2.5, (3, 2)), torch.float32)
+    models = util.to_dev(np.stack([np.eye(3), np.full((3, 3), np.inf), -np.eye(3)]), torch.float32)
+    got = loftr_b200.warp_images(util.to_dev(img), models, (48, 72), s, s.clone())
     assert torch.equal(got.cpu(), torch.from_numpy(img))
 
 
@@ -157,13 +122,10 @@ def _equalised(case):
 def _query_points(data, extra=64, seed=0):
     """Every cell keypoint of image0 (as the forward computes mkpts0_c) and `extra` random points, some outside."""
     n, _, h, w = data["image0"].shape
-    hc, wc = h // 8, w // 8
-    i = torch.arange(hc * wc, device=DEV)
     s = 8.0 * data["scale0"][:, None, :] if "scale0" in data else torch.full((n, 1, 2), 8.0, device=DEV)
-    grid = torch.stack([i % wc, i // wc], 1).float()[None] * s
     g = torch.Generator().manual_seed(seed)
     rnd = (torch.rand(n, extra, 2, generator=g) * 1.2 - 0.1).to(DEV) * torch.tensor([w, h], device=DEV) * s / 8.0
-    return torch.cat([grid, rnd], 1).contiguous()
+    return torch.cat([util.grid_points(data), rnd], 1).contiguous()
 
 
 @pytest.mark.parametrize("name, precision, cap", IDENTITY, ids=[f"{a}_{b}_cap{c}" for a, b, c in IDENTITY])
@@ -178,7 +140,7 @@ def test_identity_model_is_bitwise_the_plain_call(name, precision, cap):
     assert ref["b_ids"].numel() > 0
     for label, rect in (("identity", eye), ("nan", torch.full_like(eye, float("nan"))), ("negated", -eye)):
         got = util.eager(model, dict(inp, rectify1=rect))
-        _assert_same(got, ref, _outputs(ref), f"forward {label}")
+        util.assert_same(got, util.outputs(ref, INPUTS), label=f"forward {label}")
         assert got["minside1"].dtype == torch.bool and got["minside1"].shape == ref["b_ids"].shape
         want = RR.map_back(ref["mkpts1_f"], ref["m_bids"], eye, inp["image0"].shape[2:], inp["image1"].shape[2:],
                            inp.get("scale0"), inp.get("scale1"), inp.get("mask1"))[1]
@@ -192,7 +154,7 @@ def test_identity_model_is_bitwise_the_plain_call(name, precision, cap):
     qref, qgot = dict(inp), dict(inp, rectify1=eye)
     model.match_points(qref, pts)
     model.match_points(qgot, pts)
-    _assert_same(qgot, qref, _outputs(qref), "match_points identity")
+    util.assert_same(qgot, util.outputs(qref, INPUTS), label="match_points identity")
     assert qgot["qinside1"].shape == qref["qinside"].shape
 
 
@@ -203,9 +165,9 @@ def _models_for(inp, seed):
     n, hw0, hw1 = inp["image0"].shape[0], inp["image0"].shape[2:], inp["image1"].shape[2:]
     s0 = inp["scale0"].cpu().numpy() if "scale0" in inp else np.ones((n, 2))
     s1 = inp["scale1"].cpu().numpy() if "scale1" in inp else np.ones((n, 2))
-    m = [_similarity(_centre(hw0, s0[b]), _centre(hw1, s1[b]), rs.uniform(-25, 25), rs.uniform(0.8, 1.25),
+    m = [util.similarity(_centre(hw0, s0[b]), _centre(hw1, s1[b]), rs.uniform(-25, 25), rs.uniform(0.8, 1.25),
                      rs.uniform(-4e-4, 4e-4, 2) / max(s0[b])) for b in range(n)]
-    return _t(np.stack(m))
+    return util.to_dev(np.stack(m), torch.float32)
 
 
 def _substituted(inp, rect):
@@ -241,7 +203,7 @@ def test_rectified_call_is_the_plain_call_on_the_substituted_input(name):
     got = util.eager(model, dict(inp, rectify1=rect))
     plain = util.eager(model, _substituted(inp, rect))
     assert plain["b_ids"].numel() > 0
-    _assert_same(got, plain, [k for k in _outputs(plain) if k not in ("mkpts1_c", "mkpts1_f")], name)
+    util.assert_same(got, plain, [k for k in util.outputs(plain, INPUTS) if k not in ("mkpts1_c", "mkpts1_f")], name)
     _assert_mapped(got, plain["mkpts1_c"], plain["m_bids"], rect, inp, name, "mkpts1_c", None)
     flags = _assert_mapped(got, plain["mkpts1_f"], plain["m_bids"], rect, inp, name, "mkpts1_f", "minside1")
     util.record(f"rectify_composition_{name}", {"matches": int(plain["b_ids"].numel()), "inside": int(flags.sum())})
@@ -250,7 +212,8 @@ def test_rectified_call_is_the_plain_call_on_the_substituted_input(name):
     model.match_points(qgot, pts)
     model.match_points(qplain, pts)
     n, q = pts.shape[:2]
-    _assert_same(qgot, qplain, [k for k in _outputs(qplain) if k not in ("qpts1_c", "qpts1_f")], f"{name} points")
+    util.assert_same(qgot, qplain, [k for k in util.outputs(qplain, INPUTS) if k not in ("qpts1_c", "qpts1_f")],
+                     f"{name} points")
     ids = torch.arange(n).repeat_interleave(q)
     _assert_mapped(qgot, qplain["qpts1_c"].reshape(-1, 2), ids, rect, inp, f"{name} points", "qpts1_c", None)
     _assert_mapped(qgot, qplain["qpts1_f"].reshape(-1, 2), ids, rect, inp, f"{name} points", "qpts1_f", "qinside1")
@@ -267,9 +230,9 @@ def test_pairs_do_not_see_the_other_pairs_models():
     ra, rb = util.eager(model, dict(inp, rectify1=a)), util.eager(model, dict(inp, rectify1=b))
     sa, sb = ra["b_ids"] == 0, rb["b_ids"] == 0
     assert sa.any()
-    _assert_same({k: ra[k][sa] for k in LIST_KEYS + ["minside1"]}, {k: rb[k][sb] for k in LIST_KEYS + ["minside1"]},
-                 LIST_KEYS + ["minside1"], "pair 0")
-    assert not _same(ra["mkpts1_f"][~sa], rb["mkpts1_f"][~sb])
+    keys = LIST_KEYS + ["minside1"]
+    util.assert_same({k: ra[k][sa] for k in keys}, {k: rb[k][sb] for k in keys}, label="pair 0")
+    assert not util.same(ra["mkpts1_f"][~sa], rb["mkpts1_f"][~sb])
 
 
 # ------------------------------------------------------------------------------------------------ 5. point queries
@@ -293,7 +256,7 @@ def test_query_at_a_rectified_match_returns_its_mapped_points(name):
     model.match_points(out, pts, valid)
     for qk, fk in (("qpts1_c", "mkpts1_c"), ("qpts1_f", "mkpts1_f"), ("qinside1", "minside1"), ("q_j_ids", "j_ids"),
                    ("qconf", "mconf"), ("qexpec_f", "expec_f")):
-        assert _same(out[qk][b, slot], fwd[fk]), qk
+        util.assert_same(out[qk][b, slot], fwd[fk], label=qk)
 
 
 # ------------------------------------------------------------------------------------------------ 6. graph replay
@@ -303,7 +266,7 @@ def test_forward_static_with_rectify1_replays_from_a_graph():
     inp = util.device_inputs(case)
     m1, m2 = _models_for(inp, 1), _models_for(inp, 2)
     e1, e2 = util.eager(model, dict(inp, rectify1=m1)), util.eager(model, dict(inp, rectify1=m2))
-    assert e1["b_ids"].numel() > 0 and not _same(e1["mkpts1_f"], e2["mkpts1_f"])
+    assert e1["b_ids"].numel() > 0 and not util.same(e1["mkpts1_f"], e2["mkpts1_f"])
     rect = m1.clone()
     model.forward_static(dict(inp, rectify1=rect))   # eager warm-up
     torch.cuda.synchronize()

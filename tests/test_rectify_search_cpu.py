@@ -10,6 +10,7 @@ import torch
 
 import loftr_b200
 import rectify_search_ref as SR
+import util
 from loftr_b200 import _lib
 from loftr_b200.loftr import CapturedMatcher, check_rectify_candidates
 
@@ -82,18 +83,7 @@ def test_search_entry_is_bound_only_where_exported(monkeypatch):
     _lib.require_entries(_lib.SEARCH_ENTRIES, "the rectification search")
     names = {lib.lb_timing_tag_name(i).decode() for i in range(lib.lb_timing_num_tags())}
     assert {"match_search", "match_cap", "rectify"} <= names
-
-    class Exports:   # every other declared symbol, as a build without the search entry is loaded
-        def __init__(self):
-            for n in _lib.SIGNATURES:
-                if n not in _lib.SEARCH_ENTRIES:
-                    setattr(self, n, type("Fn", (), {})())
-            self.lb_version = lambda: 110
-
-    monkeypatch.setattr(_lib, "_lib", None)
-    monkeypatch.setattr(_lib.C, "CDLL", lambda path: Exports())
-    monkeypatch.setattr(_lib.os.path, "exists", lambda path: True)
-    old = _lib.load()
+    old = util.load_without(monkeypatch, _lib.SEARCH_ENTRIES)
     assert not hasattr(old, name)
     assert old.lb_rectify_images.argtypes == _lib.SIGNATURES["lb_rectify_images"][1]   # the rest still binds
     _lib.require_entries(_lib.RECTIFY_ENTRIES + _lib.GUIDE_ENTRIES, "other paths")

@@ -11,8 +11,6 @@ on the GPU:
    with no match under any candidate gets choice 0 and no matches;
 6. forward_static matches the eager call within the N-pair default capacity, and a CUDA graph follows the candidate
    tensor from replay to replay."""
-import math
-
 import numpy as np
 import pytest
 import torch
@@ -27,36 +25,9 @@ from match_cap_ref import LIST_KEYS
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 _CASE = {c["name"]: c for c in CASES}
-INPUTS = ("image0", "image1", "mask0", "mask1", "scale0", "scale1", "rectify1", "rectify1_candidates")
+INPUTS = util.INPUT_KEYS + ("rectify1", "rectify1_candidates")
 SEARCH_KEYS = ("rectify1_choice", "rectify1_counts")
 KEYS = LIST_KEYS + ["minside1"]
-
-
-def _same(a, b):
-    """Bitwise equality of two outputs, NaN at the same places counting as equal."""
-    if not torch.is_tensor(a):
-        return a == b
-    if a.dtype != b.dtype or a.shape != b.shape:
-        return False
-    if a.is_floating_point():
-        na, nb = torch.isnan(a), torch.isnan(b)
-        return torch.equal(na, nb) and torch.equal(a[~na], b[~nb])
-    return torch.equal(a, b)
-
-
-def _assert_same(got, ref, keys, label):
-    for k in keys:
-        assert _same(got[k], ref[k]), f"{label}: {k} differs"
-
-
-def _similarity(c0, c1, deg, zoom):
-    """x1 = c1 + zoom R(deg) (x0 - c0) as a float64 [3, 3]."""
-    a = math.radians(deg)
-    t0 = np.array([[1, 0, -c0[0]], [0, 1, -c0[1]], [0, 0, 1]])
-    t1 = np.array([[1, 0, c1[0]], [0, 1, c1[1]], [0, 0, 1]])
-    r = np.array([[zoom * math.cos(a), -zoom * math.sin(a), 0], [zoom * math.sin(a), zoom * math.cos(a), 0],
-                  [0, 0, 1]])
-    return t1 @ r @ t0
 
 
 def _candidates(inp, params):
@@ -65,8 +36,8 @@ def _candidates(inp, params):
     n, hw0, hw1 = inp["image0"].shape[0], inp["image0"].shape[2:], inp["image1"].shape[2:]
     s0 = inp["scale0"].cpu().numpy() if "scale0" in inp else np.ones((n, 2))
     s1 = inp["scale1"].cpu().numpy() if "scale1" in inp else np.ones((n, 2))
-    c = [[_similarity((0.5 * (hw0[1] - 1) * s0[b, 0], 0.5 * (hw0[0] - 1) * s0[b, 1]),
-                      (0.5 * (hw1[1] - 1) * s1[b, 0], 0.5 * (hw1[0] - 1) * s1[b, 1]), deg + 3 * b, zoom)
+    c = [[util.similarity((0.5 * (hw0[1] - 1) * s0[b, 0], 0.5 * (hw0[0] - 1) * s0[b, 1]),
+                          (0.5 * (hw1[1] - 1) * s1[b, 0], 0.5 * (hw1[0] - 1) * s1[b, 1]), deg + 3 * b, zoom)
           for deg, zoom in params] for b in range(n)]
     return torch.from_numpy(np.array(c)).float().to(DEV)
 
@@ -94,7 +65,7 @@ def _check_search(model, inp, cands, label):
     assert got["rectify1_counts"].dtype == torch.int32 and got["rectify1_choice"].dtype == torch.int64
     assert np.array_equal(got["rectify1_counts"].cpu().numpy(), counts), label
     assert np.array_equal(got["rectify1_choice"].cpu().numpy(), choice), label
-    _assert_same(got, SR.winners(flat, choice, k, KEYS), KEYS, label)
+    util.assert_same(got, SR.winners(flat, choice, k, KEYS), KEYS, label)
     assert got["bs"] == n and got["m_bids"] is got["b_ids"]
     for key in INPUTS:   # the caller's inputs are not replaced
         if key in inp:
@@ -145,8 +116,7 @@ def test_one_candidate_is_the_rectified_call(name, precision, cap):
     got = util.eager(model, dict(inp, rectify1_candidates=cands))
     ref = util.eager(model, dict(inp, rectify1=cands[:, 0].contiguous()))
     assert ref["b_ids"].numel() > 0
-    outs = [k for k in ref if k not in INPUTS]
-    _assert_same(got, ref, outs, f"{name} K=1")
+    util.assert_same(got, util.outputs(ref, INPUTS), label=f"{name} K=1")
     assert (got["rectify1_choice"] == 0).all()
     assert got["rectify1_counts"].shape == (inp["image0"].shape[0], 1)
     # identity candidates with equal sizes, scales and masks: the plain call
@@ -157,7 +127,7 @@ def test_one_candidate_is_the_rectified_call(name, precision, cap):
     plain = util.eager(model, inp)
     eye = torch.eye(3, device=DEV).repeat(inp["image0"].shape[0], 1, 1, 1)
     got = util.eager(model, dict(inp, rectify1_candidates=eye))
-    _assert_same(got, plain, [k for k in plain if k not in INPUTS], f"{name} identity")
+    util.assert_same(got, util.outputs(plain, INPUTS), label=f"{name} identity")
 
 
 # ------------------------------------------------------------------------------------------------ 4. quarter turns
@@ -187,9 +157,9 @@ def test_pairs_are_independent_nan_is_the_identity_and_empty_pairs_choose_0():
     rb = util.eager(model, dict(inp, rectify1_candidates=b))
     sa, sb = ra["b_ids"] == 0, rb["b_ids"] == 0
     assert sa.any()
-    _assert_same({k: ra[k][sa] for k in KEYS}, {k: rb[k][sb] for k in KEYS}, KEYS, "pair 0")
-    _assert_same({k: ra[k][0] for k in SEARCH_KEYS}, {k: rb[k][0] for k in SEARCH_KEYS}, SEARCH_KEYS, "pair 0")
-    assert not _same(ra["rectify1_counts"][1], rb["rectify1_counts"][1])
+    util.assert_same({k: ra[k][sa] for k in KEYS}, {k: rb[k][sb] for k in KEYS}, label="pair 0")
+    util.assert_same({k: ra[k][0] for k in SEARCH_KEYS}, {k: rb[k][0] for k in SEARCH_KEYS}, label="pair 0")
+    assert not util.same(ra["rectify1_counts"][1], rb["rectify1_counts"][1])
     # a candidate with a non-finite entry is the identity
     eye = a.clone()
     eye[:, 1] = torch.eye(3, device=DEV)
@@ -197,7 +167,7 @@ def test_pairs_are_independent_nan_is_the_identity_and_empty_pairs_choose_0():
     nan[:, 1] = float("nan")
     ri = util.eager(model, dict(inp, rectify1_candidates=eye))
     rn = util.eager(model, dict(inp, rectify1_candidates=nan))
-    _assert_same(rn, ri, KEYS + list(SEARCH_KEYS), "nan candidate")
+    util.assert_same(rn, ri, KEYS + list(SEARCH_KEYS), "nan candidate")
     # no match under any candidate: choice 0, zero counts, an empty list
     empty = _CASE["ds_empty"]
     model, _, _ = util.build_model(empty, DEV)
@@ -219,7 +189,7 @@ def test_forward_static_and_graph_replay_follow_the_candidates():
     c2 = _candidates(inp, [(-6, 1.1), (45, 1.0), (5, 0.95)])[:, :2].contiguous()
     e1 = util.eager(model, dict(inp, rectify1_candidates=c1))
     e2 = util.eager(model, dict(inp, rectify1_candidates=c2))
-    assert e1["b_ids"].numel() > 0 and not _same(e1["rectify1_counts"], e2["rectify1_counts"])
+    assert e1["b_ids"].numel() > 0 and not util.same(e1["rectify1_counts"], e2["rectify1_counts"])
     n, _, h, w = inp["image0"].shape
     L = (h // 8) * (w // 8)
 
@@ -227,7 +197,7 @@ def test_forward_static_and_graph_replay_follow_the_candidates():
         util.assert_static_equals_eager(st, eager, label)
         m = int(st["num_matches"].item())
         assert torch.equal(st["minside1"][:m], eager["minside1"]), label
-        _assert_same(st, eager, SEARCH_KEYS, label)
+        util.assert_same(st, eager, SEARCH_KEYS, label)
 
     st = dict(inp, rectify1_candidates=c1)
     model.forward_static(st)

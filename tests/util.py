@@ -1,7 +1,9 @@
 """Shared helpers of the parity tests: the model with the test weights, the numpy oracle's forward (whole batch and per
-pair, cached), the match-list rule, and the GPU matcher harness (device inputs, eager forward, static = eager)."""
+pair, cached), the match-list rule, the GPU matcher harness (device inputs, eager forward, static = eager, bitwise
+comparison, query points, guides and homographies) and the fake libraries of the binding tests."""
 from __future__ import annotations
 
+import math
 import os
 
 import numpy as np
@@ -61,6 +63,146 @@ def assert_static_equals_eager(st, eager, label):
     assert st["mkpts0_f"] is st["mkpts0_c"]
     for k in ("bs", "hw0_i", "hw1_i", "hw0_c", "hw1_c", "hw0_f", "hw1_f", "W"):
         assert st[k] == eager[k], (label, k)
+
+
+INPUT_KEYS = ("image0", "image1", "mask0", "mask1", "scale0", "scale1")
+# models in output coordinates (image pixels; source pixels with scales): x1 ~ H x0, and F = [e']_x H
+H_MODEL = np.array([[1.03, 0.04, 6.0], [-0.03, 0.97, -5.0], [2e-5, -1e-5, 1.0]], np.float32)
+_E1 = np.array([140.0, 60.0, 1.0])
+F_MODEL = (np.array([[0, -_E1[2], _E1[1]], [_E1[2], 0, -_E1[0]], [-_E1[1], _E1[0], 0]]) @ H_MODEL).astype(np.float32)
+F_MODEL /= np.abs(F_MODEL).max()
+
+
+def inputs(data):
+    """The forward inputs of a batch dict."""
+    return {k: v for k, v in data.items() if k in INPUT_KEYS}
+
+
+def outputs(data, keys=INPUT_KEYS):
+    """The entries of a batch dict that are not inputs (`keys`): what a call wrote."""
+    return {k: v for k, v in data.items() if k not in keys}
+
+
+def same(got, ref, nan_equal=True):
+    """Bitwise equality of two outputs: the same dtype and shape, NaN at the same places (with `nan_equal`; without it
+    a NaN is unequal to everything, as in torch.equal) and every other value equal, compared without any cast.
+    Non-tensors compare with ==."""
+    if not torch.is_tensor(ref):
+        return got == ref
+    if not torch.is_tensor(got) or got.dtype != ref.dtype or got.shape != ref.shape:
+        return False
+    if nan_equal and ref.is_floating_point():
+        ng, nr = torch.isnan(got), torch.isnan(ref)
+        return torch.equal(ng, nr) and torch.equal(got[~ng], ref[~nr])
+    return torch.equal(got, ref)
+
+
+def assert_same(got, ref, keys=None, label="", nan_equal=True):
+    """`same` for two outputs, or for the entries `keys` (default: every key of `ref`) of two output dicts."""
+    if not isinstance(ref, dict):
+        assert same(got, ref, nan_equal), f"{label} differs"
+        return
+    for k in ref if keys is None else keys:
+        assert same(got[k], ref[k], nan_equal), f"{label}: {k} differs"
+
+
+def to_dev(x, dtype=None):
+    """array -> tensor on the GPU (in `dtype`, or the array's own)"""
+    t = torch.as_tensor(np.ascontiguousarray(x))
+    return t.to(DEV) if dtype is None else t.to(DEV, dtype)
+
+
+def to_np(t):
+    return t.detach().cpu().numpy()
+
+
+def idx(v):
+    """int64 image indices on the GPU"""
+    return torch.tensor(v, dtype=torch.int64, device=DEV)
+
+
+def frames(case):
+    """The case's images, masks and scales as one set of 2n frames (image0 of every pair, then image1)."""
+    d = device_inputs(case)
+    cat = lambda k: torch.cat([d[k + "0"], d[k + "1"]]) if k + "0" in d else None
+    return cat("image"), cat("mask"), cat("scale")
+
+
+def grid_points(data, side=0):
+    """Every cell keypoint of image `side` in source pixels, as the forward computes mkpts{side}_c -> [N, cells, 2]."""
+    n, _, h, w = data[f"image{side}"].shape
+    return bank_grid_points(torch.arange(n, device=DEV), (h // 8, w // 8), data.get(f"scale{side}"))
+
+
+def bank_grid_points(ids, hw_c, scales=None):
+    """`grid_points` of the bank images `ids`, whose scales are scales[ids] -> [len(ids), cells, 2]."""
+    hc, wc = hw_c
+    i = torch.arange(hc * wc, device=DEV)
+    cell = torch.stack([i % wc, i // wc], 1).float()[None].expand(len(ids), -1, -1)
+    s = torch.full((len(ids), 1, 2), 8.0, device=DEV) if scales is None else 8.0 * scales[ids][:, None, :]
+    return (cell * s).contiguous()
+
+
+def guide(kind, model, radius):
+    """A guide dict: kind "homography" | "fundamental", model [N, 3, 3] (cast to float32), radius in pixels."""
+    return {"kind": kind, "model": to_dev(np.asarray(model, np.float32)), "radius": radius}
+
+
+def similarity(c0, c1, deg, zoom, persp=(0.0, 0.0)):
+    """x1 = c1 + zoom R(deg) (x0 - c0), with a perspective row (persp, 1) in the centred frame, as a float64 [3, 3]."""
+    a = math.radians(deg)
+    t0 = np.array([[1, 0, -c0[0]], [0, 1, -c0[1]], [0, 0, 1]])
+    t1 = np.array([[1, 0, c1[0]], [0, 1, c1[1]], [0, 0, 1]])
+    r = np.array([[zoom * math.cos(a), -zoom * math.sin(a), 0], [zoom * math.sin(a), zoom * math.cos(a), 0],
+                  [persp[0], persp[1], 1]])
+    return t1 @ r @ t0
+
+
+# ------------------------------------------------------------------------------------------------ fake libraries
+def old_library(monkeypatch, version):
+    """`_lib.load()` returns a library that reports `version` and exports nothing else."""
+    from loftr_b200 import _lib
+
+    class OldLib:
+        def lb_version(self):
+            return version
+
+    monkeypatch.setattr(_lib, "load", lambda: OldLib())
+
+
+def load_without(monkeypatch, names, version=110):
+    """`_lib.load()` on what ctypes.CDLL gives for a build of `version` that exports every declared symbol but `names`
+    -> the loaded library."""
+    from loftr_b200 import _lib
+
+    class Exports:
+        def __init__(self):
+            for n in _lib.SIGNATURES:
+                if n not in names:
+                    setattr(self, n, type("Fn", (), {})())
+            self.lb_version = lambda: version
+
+    monkeypatch.setattr(_lib, "_lib", None)
+    monkeypatch.setattr(_lib.C, "CDLL", lambda path: Exports())
+    monkeypatch.setattr(_lib.os.path, "exists", lambda path: True)
+    return _lib.load()
+
+
+def host_bank(model, k=3, masks=False):
+    """A host bank of k 96x128 images tied to the model's current weights (never matched: nothing here launches)."""
+    from loftr_b200.loftr import ImageFeatures
+    mask = torch.ones(k, 12, 16, dtype=torch.bool) if masks else None
+    return ImageFeatures(torch.zeros(k, 256, 12, 16), torch.zeros(k, 128, 48, 64), mask, torch.Size((96, 128)),
+                         torch.Size((12, 16)), torch.Size((48, 64)), model._bank_key())
+
+
+def stages_unreachable(monkeypatch, model):
+    """The model's matching stages raise if reached, so that a test sees validation stop a call before them -> model"""
+    def reached(*a, **k):
+        raise AssertionError("a matching stage was reached")
+    for name in ("_match_points", "_coarse_tokens", "_backbone", "_backbone_pairs"):
+        monkeypatch.setattr(model, name, reached)
+    return model
 
 
 def _backbone(model, i0, i1):
