@@ -1552,70 +1552,78 @@ static int check_query(const char* who, const LbCoarseQueryArgs* q) {
   return 0;
 }
 
-// The query kernel of `side` on the coarse quantities coarse_rows left in `w`: coarse_query_kernel for image0 points
-// (side 0), coarse_query_col_kernel for image1 points (side 1).  conf = exp(key + term + bias) with the terms and the
-// bias coarse_rows gives match_flag_kernel (DESIGN.md §22): -LSE and 0 for dual-softmax, the Sinkhorn potentials and
+// The query kernel of `side` on the coarse quantities coarse_rows left in `w`: coarse_query_kernel<0> for image0
+// points, coarse_query_kernel<1> for image1 points.  conf = exp(key + term + bias) with the terms and the bias
+// coarse_rows gives match_flag_kernel (DESIGN.md §22): -LSE and 0 for dual-softmax, the Sinkhorn potentials and
 // log(L + S) for Sinkhorn.
 static int query_launch(int side, const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, const CmWs& w,
                         cudaStream_t st) {
   const bool ot = a->match_type == LB_MATCH_SINKHORN;
-  const float norm = -logf(static_cast<float>(a->L + a->S));
-  const float conf_bias = ot ? -norm : 0.f;
   const float* rowterm = ot ? w.row_u : w.row_t;
-  const long nq = static_cast<long>(a->n_pairs) * q->Q;
-  if (side == 0) {
-    QueryParams qp;
-    qp.n_pairs = a->n_pairs; qp.Q = q->Q; qp.L = a->L; qp.S = a->S;
-    qp.h0c = a->h0c; qp.w0c = a->w0c; qp.w1c = a->w1c;
-    qp.H0 = q->H0; qp.W0 = q->W0; qp.Hf0 = q->Hf0; qp.Wf0 = q->Wf0;
-    qp.stride = q->stride; qp.s_c = a->img_scale; qp.s_f = q->fine_scale;
-    qp.conf_bias = conf_bias;
-    qp.points0 = q->points0; qp.valid0 = q->valid0;
-    qp.scale0 = a->scale0; qp.scale1 = a->scale1; qp.mask0 = a->mask0;
-    qp.row_key = w.row_key; qp.row_arg = w.row_arg; qp.col_arg = w.col_arg; qp.rowterm = rowterm;
-    qp.flag = w.flag;
-    qp.i_ids = q->i_ids; qp.j_ids = q->j_ids; qp.conf = q->conf;
-    qp.mutual = q->mutual; qp.valid = q->valid; qp.inside = q->inside;
-    qp.centres = q->centres; qp.win = q->win_ids; qp.pts0_f = q->pts0_f; qp.pts1_c = q->pts1_c;
-    return launch(TAG_MATCH_QUERY, coarse_query_kernel, cdiv(nq, 256), 256, 0, st, qp);
-  }
-  // side 1: the *0 fields of `q` hold image1's points, sizes and fine map, pts0_f the snapped image1 point and
-  // pts1_c the image0 window centre; centres and win_ids keep the (image0, image1) order
-  QueryColParams qp;
+  const float* colterm = ot ? w.col_v : w.col_t;
+  const bool s1 = side == 1;
+  QueryParams qp;
   qp.n_pairs = a->n_pairs; qp.Q = q->Q; qp.L = a->L; qp.S = a->S;
-  qp.h1c = a->h1c; qp.w1c = a->w1c; qp.w0c = a->w0c;
-  qp.H1 = q->H0; qp.W1 = q->W0; qp.Hf1 = q->Hf0; qp.Wf1 = q->Wf0;
+  qp.h0c = a->h0c; qp.w0c = a->w0c; qp.h1c = a->h1c; qp.w1c = a->w1c;
+  // the *0 fields of `q` describe the queried image on either side, pts0_f receives the snapped query and pts1_c the
+  // other image's window centre; centres and win_ids keep the (image0, image1) order
+  qp.Hq = q->H0; qp.Wq = q->W0; qp.Hfq = q->Hf0; qp.Wfq = q->Wf0;
   qp.stride = q->stride; qp.s_c = a->img_scale; qp.s_f = q->fine_scale;
-  qp.conf_bias = conf_bias;
-  qp.points1 = q->points0; qp.valid1 = q->valid0;
-  qp.scale0 = a->scale0; qp.scale1 = a->scale1; qp.mask1 = a->mask1;
-  qp.col_key = w.col_key; qp.col_arg = w.col_arg; qp.colterm = ot ? w.col_v : w.col_t;
-  qp.row_key = w.row_key; qp.row_arg = w.row_arg; qp.rowterm = rowterm;
+  qp.conf_bias = ot ? logf(static_cast<float>(a->L + a->S)) : 0.f;   // coarse_rows' -norm
+  qp.points_q = q->points0; qp.valid_q = q->valid0;
+  qp.scale0 = a->scale0; qp.scale1 = a->scale1; qp.mask_q = s1 ? a->mask1 : a->mask0;
+  qp.key_q = s1 ? w.col_key : w.row_key; qp.arg_q = s1 ? w.col_arg : w.row_arg; qp.term_q = s1 ? colterm : rowterm;
+  qp.key_o = s1 ? w.row_key : w.col_key; qp.arg_o = s1 ? w.row_arg : w.col_arg; qp.term_o = s1 ? rowterm : colterm;
   qp.flag = w.flag;
   qp.i_ids = q->i_ids; qp.j_ids = q->j_ids; qp.conf = q->conf;
   qp.mutual = q->mutual; qp.valid = q->valid; qp.inside = q->inside;
-  qp.centres = q->centres; qp.win = q->win_ids; qp.pts1_f = q->pts0_f; qp.pts0_c = q->pts1_c;
-  return launch(TAG_MATCH_QUERY, coarse_query_col_kernel, cdiv(nq, 256), 256, 0, st, qp);
+  qp.centres = q->centres; qp.win = q->win_ids; qp.pts_qf = q->pts0_f; qp.pts_oc = q->pts1_c;
+  const long nq = static_cast<long>(a->n_pairs) * q->Q;
+  return s1 ? launch(TAG_MATCH_QUERY, coarse_query_kernel<1>, cdiv(nq, 256), 256, 0, st, qp)
+            : launch(TAG_MATCH_QUERY, coarse_query_kernel<0>, cdiv(nq, 256), 256, 0, st, qp);
 }
 
-// lb_coarse_query (guide NULL), lb_coarse_query_guided and lb_coarse_query_side: the coarse rows, unguided or under
-// `guide`, then the query kernel of `side` on them.  `who` names the entry in the messages.
-static int coarse_query(const char* who, const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q,
-                        const GuideParams* guide, int operand_planes, void* ws, size_t ws_bytes, void* stream,
-                        int side = 0) {
+// What a query entry does before the query kernel: the coarse rows, unguided or under a guide, or none (reuse).
+enum QueryRows { kRowsPlain, kRowsGuided, kRowsReuse };
+
+// The body of the query entries; `who` names the entry in the messages.  `g` is checked when `rows` is kRowsGuided,
+// and `operand_planes` unless it is kRowsReuse.  The argument checks come before the return for Q = 0 or no pairs, so
+// they hold on machines without a device; reuse checks everything before it binds one.
+static int coarse_query(const char* who, const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, QueryRows rows,
+                        const LbCoarseGuide* g, int side, int operand_planes, void* ws, size_t ws_bytes,
+                        void* stream) {
+  if (side != 0 && side != 1) return fail("%s: side must be 0 (image0) or 1 (image1) (got %d)", who, side);
+  if (rows != kRowsReuse && operand_planes != 1 && operand_planes != 2)
+    return fail("%s: operand_planes must be 1 (fp16) or 2 (split) (got %d)", who, operand_planes);
+  GuideParams gp;
+  if (rows == kRowsGuided) LB_TRY(guide_params(who, a, g, gp));
   if (q->Q <= 0 || a->n_pairs <= 0) return 0;
-  DeviceScope dev;
-  LB_TRY(dev.bind(q->i_ids));
-  LB_TRY(check_query(who, q));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  DeviceScope dev;
   CmWs w;
-  SelectParams sp;
-  if (guide) {
-    LB_TRY((operand_planes == 2 ? coarse_rows<2, true>(a, guide, dev, ws, ws_bytes, st, w, sp)
-                                : coarse_rows<1, true>(a, guide, dev, ws, ws_bytes, st, w, sp)));
+  if (rows == kRowsReuse) {   // the workspace a preceding query entry filled for the same args on the same stream
+    LB_TRY(check_query(who, q));
+    if (a->L != a->h0c * a->w0c || a->S != a->h1c * a->w1c)
+      return fail("%s: L/S do not match the coarse grid sizes", who);
+    if (a->match_type != LB_MATCH_DUAL_SOFTMAX && a->match_type != LB_MATCH_SINKHORN)
+      return fail("%s: unknown match_type %d", who, a->match_type);
+    if (!ws) return fail("%s: workspace pointer is null", who);
+    Bump b{static_cast<uint8_t*>(ws), ws_bytes};
+    carve_cm(b, w, a->n_pairs, a->L, a->S);
+    if (!b.ok)
+      return fail("%s: workspace of %zu bytes is too small for %d pairs of %d x %d cells (need %zu)", who, ws_bytes,
+                  a->n_pairs, a->L, a->S, lb_coarse_match_workspace_bytes(a->n_pairs, a->L, a->S));
+    LB_TRY(dev.bind(q->i_ids));
   } else {
-    LB_TRY((operand_planes == 2 ? coarse_rows<2, false>(a, nullptr, dev, ws, ws_bytes, st, w, sp)
-                                : coarse_rows<1, false>(a, nullptr, dev, ws, ws_bytes, st, w, sp)));
+    LB_TRY(dev.bind(q->i_ids));
+    LB_TRY(check_query(who, q));
+    using Rows = int (*)(const LbCoarseMatchArgs*, const GuideParams*, const DeviceScope&, void*, size_t,
+                         cudaStream_t, CmWs&, SelectParams&);
+    static constexpr Rows kRows[2][2] = {{coarse_rows<1, false>, coarse_rows<1, true>},
+                                         {coarse_rows<2, false>, coarse_rows<2, true>}};
+    const bool guided = rows == kRowsGuided;
+    SelectParams sp;
+    LB_TRY(kRows[operand_planes - 1][guided](a, guided ? &gp : nullptr, dev, ws, ws_bytes, st, w, sp));
   }
   return query_launch(side, a, q, w, st);
 }
@@ -1663,50 +1671,23 @@ int lb_coarse_match_search(const LbCoarseMatchArgs* a, const LbCoarseSearch* s, 
 
 int lb_coarse_query(const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, int operand_planes, void* ws,
                     size_t ws_bytes, void* stream) {
-  if (operand_planes != 1 && operand_planes != 2)
-    return fail("lb_coarse_query: operand_planes must be 1 (fp16) or 2 (split) (got %d)", operand_planes);
-  return coarse_query("lb_coarse_query", a, q, nullptr, operand_planes, ws, ws_bytes, stream);
+  return coarse_query("lb_coarse_query", a, q, kRowsPlain, nullptr, 0, operand_planes, ws, ws_bytes, stream);
 }
 
 int lb_coarse_query_guided(const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, const LbCoarseGuide* g,
                            int operand_planes, void* ws, size_t ws_bytes, void* stream) {
-  if (operand_planes != 1 && operand_planes != 2)
-    return fail("lb_coarse_query_guided: operand_planes must be 1 (fp16) or 2 (split) (got %d)", operand_planes);
-  GuideParams gp;
-  LB_TRY(guide_params("lb_coarse_query_guided", a, g, gp));
-  return coarse_query("lb_coarse_query_guided", a, q, &gp, operand_planes, ws, ws_bytes, stream);
+  return coarse_query("lb_coarse_query_guided", a, q, kRowsGuided, g, 0, operand_planes, ws, ws_bytes, stream);
 }
 
 int lb_coarse_query_side(const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, const LbCoarseGuide* g, int side,
                          int operand_planes, void* ws, size_t ws_bytes, void* stream) {
-  if (side != 0 && side != 1) return fail("lb_coarse_query_side: side must be 0 (image0) or 1 (image1) (got %d)", side);
-  if (operand_planes != 1 && operand_planes != 2)
-    return fail("lb_coarse_query_side: operand_planes must be 1 (fp16) or 2 (split) (got %d)", operand_planes);
-  if (!g) return coarse_query("lb_coarse_query_side", a, q, nullptr, operand_planes, ws, ws_bytes, stream, side);
-  GuideParams gp;
-  LB_TRY(guide_params("lb_coarse_query_side", a, g, gp));
-  return coarse_query("lb_coarse_query_side", a, q, &gp, operand_planes, ws, ws_bytes, stream, side);
+  return coarse_query("lb_coarse_query_side", a, q, g ? kRowsGuided : kRowsPlain, g, side, operand_planes, ws,
+                      ws_bytes, stream);
 }
 
 int lb_coarse_query_reuse(const LbCoarseMatchArgs* a, const LbCoarseQueryArgs* q, int side, void* ws,
                           size_t ws_bytes, void* stream) {
-  if (side != 0 && side != 1) return fail("lb_coarse_query_reuse: side must be 0 (image0) or 1 (image1) (got %d)", side);
-  if (q->Q <= 0 || a->n_pairs <= 0) return 0;
-  LB_TRY(check_query("lb_coarse_query_reuse", q));
-  if (a->L != a->h0c * a->w0c || a->S != a->h1c * a->w1c)
-    return fail("lb_coarse_query_reuse: L/S do not match the coarse grid sizes");
-  if (a->match_type != LB_MATCH_DUAL_SOFTMAX && a->match_type != LB_MATCH_SINKHORN)
-    return fail("lb_coarse_query_reuse: unknown match_type %d", a->match_type);
-  if (!ws) return fail("lb_coarse_query_reuse: workspace pointer is null");
-  Bump b{static_cast<uint8_t*>(ws), ws_bytes};
-  CmWs w;
-  carve_cm(b, w, a->n_pairs, a->L, a->S);
-  if (!b.ok)
-    return fail("lb_coarse_query_reuse: workspace of %zu bytes is too small for %d pairs of %d x %d cells (need %zu)",
-                ws_bytes, a->n_pairs, a->L, a->S, lb_coarse_match_workspace_bytes(a->n_pairs, a->L, a->S));
-  DeviceScope dev;
-  LB_TRY(dev.bind(q->i_ids));
-  return query_launch(side, a, q, w, static_cast<cudaStream_t>(stream));
+  return coarse_query("lb_coarse_query_reuse", a, q, kRowsReuse, nullptr, side, 0, ws, ws_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ fine level

@@ -673,27 +673,35 @@ __global__ void match_flag_kernel(const SelectParams p) {
   p.conf[gi] = conf;
 }
 
-// Caller-given image0 points -> the coarse answer of each (LoFTR.match_points, DESIGN.md §17): the cell i nearest to
-// the point, its row arg-max j, conf and flags as match_flag_kernel computes them for row i, and the fine window
-// centres of both images.  One thread per query; queries that are not inside get NaN points, conf 0, no flags,
-// ids -1 and fine-stage ids (win) 0, so no later kernel reads through an invalid index.
+// Caller-given points -> the coarse answer of each: image0 points (kSide 0, LoFTR.match_points, DESIGN.md §17) or
+// image1 points (kSide 1, §22).  Fields are named by role: "q" is the queried image, "o" the other; the host maps
+// rows and columns onto them.  Each query takes the q cell nearest to the point, its arg-max in o, conf and flags as
+// match_flag_kernel computes them, and the fine window centres of both images.  One thread per query; queries that are
+// not inside get NaN points, conf 0, no flags, ids -1 and fine-stage ids (win) 0, so no later kernel reads through an
+// invalid index.  ids, centres and win are written in (image0, image1) order.  Where the sides differ:
+//   mutual  side 0: arg_o[answer] == cell; side 1 also needs the answer row to have a valid column.
+//   conf    exp((key + term) + conf_bias) of the queried cell, except a mutual answer on side 1, which takes its row's
+//           (o) expression, so it equals mconf bit for bit.
+//   valid   side 0: flag[i]; side 1: mutual && flag[i], i.e. the forward keeps (b, i, j).
 struct QueryParams {
   int n_pairs, Q, L, S;
-  int h0c, w0c, w1c;
-  int H0, W0;               // image0 (network pixels)
-  int Hf0, Wf0;             // fine map of image0
+  int h0c, w0c, h1c, w1c;
+  int Hq, Wq;               // queried image (network pixels)
+  int Hfq, Wfq;             // fine map of the queried image
   int stride;               // fine pixels per coarse cell
   float s_c, s_f;           // image pixels per coarse / fine pixel
   float conf_bias;
-  const float* points0;     // [n*Q, 2] (x, y), source pixels when scale0 is given
-  const uint8_t* valid0;    // optional [n*Q]
+  const float* points_q;    // [n*Q, 2] (x, y), source pixels when the queried image's scale is given
+  const uint8_t* valid_q;   // optional [n*Q]
   const float* scale0;      // optional [n, 2]
   const float* scale1;
-  const uint8_t* mask0;     // optional [n*L]
-  const float* row_key;     // [n*L]
-  const int* row_arg;
-  const int* col_arg;       // [n*S]
-  const float* rowterm;
+  const uint8_t* mask_q;    // optional, per queried cell
+  const float* key_q;       // per queried cell: best key, arg-max in o, conf term (row_* on side 0, col_* on side 1)
+  const int* arg_q;
+  const float* term_q;
+  const float* key_o;       // per cell of o: the same
+  const int* arg_o;
+  const float* term_o;
   const uint8_t* flag;      // [n*L] match_flag_kernel's test
   long long* i_ids;         // [n*Q]
   long long* j_ids;
@@ -703,33 +711,39 @@ struct QueryParams {
   uint8_t* inside;
   int* centres;             // [2, n*Q, 2] fine-map (x, y) of the image0 / image1 window centres
   long long* win;           // [3, n*Q] (b, i, j) read by the fine stage
-  float* pts0_f;            // [n*Q, 2]
-  float* pts1_c;
+  float* pts_qf;            // [n*Q, 2] the query snapped to the queried image's fine grid
+  float* pts_oc;            // [n*Q, 2] the window centre in o
 };
+template <int kSide>
 __global__ void coarse_query_kernel(const QueryParams p) {
+  constexpr bool k1 = kSide == 1;
   const long q = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x;
   const long nq = static_cast<long>(p.n_pairs) * p.Q;
   if (q >= nq) return;
   const int b = static_cast<int>(q / p.Q);
-  float sx0 = 1.f, sy0 = 1.f, sx1 = 1.f, sy1 = 1.f;
-  if (p.scale0) { sx0 = p.scale0[2 * b]; sy0 = p.scale0[2 * b + 1]; sx1 = p.scale1[2 * b]; sy1 = p.scale1[2 * b + 1]; }
-  float px = p.points0[2 * q], py = p.points0[2 * q + 1];
-  if (p.scale0) { px = px / sx0; py = py / sy0; }
+  const int Nq = k1 ? p.S : p.L, No = k1 ? p.L : p.S;   // cells of q / o
+  const int hqc = k1 ? p.h1c : p.h0c, wqc = k1 ? p.w1c : p.w0c, woc = k1 ? p.w0c : p.w1c;
+  const float* scale_q = k1 ? p.scale1 : p.scale0;
+  const float* scale_o = k1 ? p.scale0 : p.scale1;
+  float sxq = 1.f, syq = 1.f, sxo = 1.f, syo = 1.f;
+  if (scale_q) { sxq = scale_q[2 * b]; syq = scale_q[2 * b + 1]; sxo = scale_o[2 * b]; syo = scale_o[2 * b + 1]; }
+  float px = p.points_q[2 * q], py = p.points_q[2 * q + 1];
+  if (scale_q) { px = px / sxq; py = py / syq; }
   // the comparisons are false for NaN, so a NaN coordinate fails here
-  bool in = (!p.valid0 || p.valid0[q]) && px >= 0.f && px <= static_cast<float>(p.W0 - 1) && py >= 0.f &&
-            py <= static_cast<float>(p.H0 - 1);
-  int i = 0, j = 0, cx = 0, cy = 0;
-  long gi = 0;
+  bool in = (!p.valid_q || p.valid_q[q]) && px >= 0.f && px <= static_cast<float>(p.Wq - 1) && py >= 0.f &&
+            py <= static_cast<float>(p.Hq - 1);
+  int cell = 0, ans = 0, cx = 0, cy = 0;
+  long gq = 0;
   if (in) {
-    cx = min(max(static_cast<int>(floorf(px / p.s_c + 0.5f)), 0), p.w0c - 1);
-    cy = min(max(static_cast<int>(floorf(py / p.s_c + 0.5f)), 0), p.h0c - 1);
-    i = cy * p.w0c + cx;
-    gi = static_cast<long>(b) * p.L + i;
-    if (p.mask0 && !p.mask0[gi]) in = false;
+    cx = min(max(static_cast<int>(floorf(px / p.s_c + 0.5f)), 0), wqc - 1);
+    cy = min(max(static_cast<int>(floorf(py / p.s_c + 0.5f)), 0), hqc - 1);
+    cell = cy * wqc + cx;
+    gq = static_cast<long>(b) * Nq + cell;
+    if (p.mask_q && !p.mask_q[gq]) in = false;
   }
   if (in) {
-    j = p.row_arg[gi];
-    in = j >= 0 && j < p.S && p.row_key[gi] > -1.0e29f;   // a row without any valid column has no answer
+    ans = p.arg_q[gq];
+    in = ans >= 0 && ans < No && p.key_q[gq] > -1.0e29f;   // a cell without any valid partner has no answer
   }
   const long nq2 = 2 * nq;
   if (!in) {
@@ -739,123 +753,35 @@ __global__ void coarse_query_kernel(const QueryParams p) {
     p.mutual[q] = 0; p.valid[q] = 0; p.inside[q] = 0;
     p.centres[2 * q] = 0; p.centres[2 * q + 1] = 0; p.centres[2 * (nq + q)] = 0; p.centres[2 * (nq + q) + 1] = 0;
     p.win[q] = b; p.win[nq + q] = 0; p.win[nq2 + q] = 0;
-    p.pts0_f[2 * q] = nan; p.pts0_f[2 * q + 1] = nan;
-    p.pts1_c[2 * q] = nan; p.pts1_c[2 * q + 1] = nan;
+    p.pts_qf[2 * q] = nan; p.pts_qf[2 * q + 1] = nan;
+    p.pts_oc[2 * q] = nan; p.pts_oc[2 * q + 1] = nan;
     return;
   }
-  const int fx0 = min(max(static_cast<int>(floorf(px / p.s_f + 0.5f)), 0), p.Wf0 - 1);
-  const int fy0 = min(max(static_cast<int>(floorf(py / p.s_f + 0.5f)), 0), p.Hf0 - 1);
-  const int jy = j / p.w1c, jx = j - jy * p.w1c;
-  const int fx1 = p.stride * jx + (fx0 - p.stride * cx);
-  const int fy1 = p.stride * jy + (fy0 - p.stride * cy);
-  p.i_ids[q] = i; p.j_ids[q] = j;
-  p.conf[q] = expf(p.row_key[gi] + p.rowterm[gi] + p.conf_bias);   // match_flag_kernel's conf
-  p.mutual[q] = p.col_arg[static_cast<long>(b) * p.S + j] == i ? 1 : 0;
-  p.valid[q] = p.flag[gi];
-  p.inside[q] = 1;
-  p.centres[2 * q] = fx0; p.centres[2 * q + 1] = fy0;
-  p.centres[2 * (nq + q)] = fx1; p.centres[2 * (nq + q) + 1] = fy1;
-  p.win[q] = b; p.win[nq + q] = i; p.win[nq2 + q] = j;
-  p.pts0_f[2 * q] = static_cast<float>(fx0) * p.s_f * sx0;
-  p.pts0_f[2 * q + 1] = static_cast<float>(fy0) * p.s_f * sy0;
-  p.pts1_c[2 * q] = static_cast<float>(fx1) * p.s_f * sx1;
-  p.pts1_c[2 * q + 1] = static_cast<float>(fy1) * p.s_f * sy1;
-}
-
-// Caller-given image1 points -> the coarse answer of each (DESIGN.md §22), the mirror of coarse_query_kernel: the
-// cell j nearest to the point, its column arg-max i, and the window centres of both images.  A mutual answer gets
-// match_flag_kernel's row-side conf, so it equals mconf bit for bit; any other gets the column-side expression
-// exp((col_key[j] + colterm[j]) + conf_bias).  valid = flag[i] && row_arg[i] == j: the forward keeps (b, i, j).
-// Outputs that are not inside are as in coarse_query_kernel.
-struct QueryColParams {
-  int n_pairs, Q, L, S;
-  int h1c, w1c, w0c;
-  int H1, W1;               // image1 (network pixels)
-  int Hf1, Wf1;             // fine map of image1
-  int stride;               // fine pixels per coarse cell
-  float s_c, s_f;           // image pixels per coarse / fine pixel
-  float conf_bias;
-  const float* points1;     // [n*Q, 2] (x, y), source pixels when scale1 is given
-  const uint8_t* valid1;    // optional [n*Q]
-  const float* scale0;      // optional [n, 2]
-  const float* scale1;
-  const uint8_t* mask1;     // optional [n*S]
-  const float* col_key;     // [n*S]
-  const int* col_arg;
-  const float* colterm;
-  const float* row_key;     // [n*L]
-  const int* row_arg;
-  const float* rowterm;
-  const uint8_t* flag;      // [n*L] match_flag_kernel's test
-  long long* i_ids;         // [n*Q]
-  long long* j_ids;
-  float* conf;
-  uint8_t* mutual;
-  uint8_t* valid;
-  uint8_t* inside;
-  int* centres;             // [2, n*Q, 2] fine-map (x, y) of the image0 / image1 window centres
-  long long* win;           // [3, n*Q] (b, i, j) read by the fine stage
-  float* pts1_f;            // [n*Q, 2] the query snapped to image1's fine grid
-  float* pts0_c;            // [n*Q, 2] the image0 window centre
-};
-__global__ void coarse_query_col_kernel(const QueryColParams p) {
-  const long q = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x;
-  const long nq = static_cast<long>(p.n_pairs) * p.Q;
-  if (q >= nq) return;
-  const int b = static_cast<int>(q / p.Q);
-  float sx0 = 1.f, sy0 = 1.f, sx1 = 1.f, sy1 = 1.f;
-  if (p.scale1) { sx0 = p.scale0[2 * b]; sy0 = p.scale0[2 * b + 1]; sx1 = p.scale1[2 * b]; sy1 = p.scale1[2 * b + 1]; }
-  float px = p.points1[2 * q], py = p.points1[2 * q + 1];
-  if (p.scale1) { px = px / sx1; py = py / sy1; }
-  // the comparisons are false for NaN, so a NaN coordinate fails here
-  bool in = (!p.valid1 || p.valid1[q]) && px >= 0.f && px <= static_cast<float>(p.W1 - 1) && py >= 0.f &&
-            py <= static_cast<float>(p.H1 - 1);
-  int i = 0, j = 0, cx = 0, cy = 0;
-  long gj = 0;
-  if (in) {
-    cx = min(max(static_cast<int>(floorf(px / p.s_c + 0.5f)), 0), p.w1c - 1);
-    cy = min(max(static_cast<int>(floorf(py / p.s_c + 0.5f)), 0), p.h1c - 1);
-    j = cy * p.w1c + cx;
-    gj = static_cast<long>(b) * p.S + j;
-    if (p.mask1 && !p.mask1[gj]) in = false;
-  }
-  if (in) {
-    i = p.col_arg[gj];
-    in = i >= 0 && i < p.L && p.col_key[gj] > -1.0e29f;   // a column without any valid row has no answer
-  }
-  const long nq2 = 2 * nq;
-  if (!in) {
-    const float nan = __int_as_float(0x7fffffff);
-    p.i_ids[q] = -1; p.j_ids[q] = -1;
-    p.conf[q] = 0.f;
-    p.mutual[q] = 0; p.valid[q] = 0; p.inside[q] = 0;
-    p.centres[2 * q] = 0; p.centres[2 * q + 1] = 0; p.centres[2 * (nq + q)] = 0; p.centres[2 * (nq + q) + 1] = 0;
-    p.win[q] = b; p.win[nq + q] = 0; p.win[nq2 + q] = 0;
-    p.pts1_f[2 * q] = nan; p.pts1_f[2 * q + 1] = nan;
-    p.pts0_c[2 * q] = nan; p.pts0_c[2 * q + 1] = nan;
-    return;
-  }
-  const int fx1 = min(max(static_cast<int>(floorf(px / p.s_f + 0.5f)), 0), p.Wf1 - 1);
-  const int fy1 = min(max(static_cast<int>(floorf(py / p.s_f + 0.5f)), 0), p.Hf1 - 1);
-  const int iy = i / p.w0c, ix = i - iy * p.w0c;
-  const int fx0 = p.stride * ix + (fx1 - p.stride * cx);
-  const int fy0 = p.stride * iy + (fy1 - p.stride * cy);
-  const long gi = static_cast<long>(b) * p.L + i;
-  // a row without any valid column (key kNegBig) has no arg-max, as in coarse_query_kernel and match_flag_kernel
-  const bool mutual = p.row_arg[gi] == j && p.row_key[gi] > -1.0e29f;
-  p.i_ids[q] = i; p.j_ids[q] = j;
-  p.conf[q] = mutual ? expf(p.row_key[gi] + p.rowterm[gi] + p.conf_bias)     // match_flag_kernel's conf
-                     : expf(p.col_key[gj] + p.colterm[gj] + p.conf_bias);
+  const int fxq = min(max(static_cast<int>(floorf(px / p.s_f + 0.5f)), 0), p.Wfq - 1);
+  const int fyq = min(max(static_cast<int>(floorf(py / p.s_f + 0.5f)), 0), p.Hfq - 1);
+  const int ay = ans / woc, ax = ans - ay * woc;
+  const int fxo = p.stride * ax + (fxq - p.stride * cx);
+  const int fyo = p.stride * ay + (fyq - p.stride * cy);
+  const long go = static_cast<long>(b) * No + ans;
+  bool mutual = p.arg_o[go] == cell;
+  // a row without any valid column (key kNegBig) has no arg-max, as in match_flag_kernel
+  if constexpr (k1) mutual = mutual && p.key_o[go] > -1.0e29f;
+  const bool conf_o = k1 && mutual;
+  p.conf[q] = expf((conf_o ? p.key_o[go] : p.key_q[gq]) + (conf_o ? p.term_o[go] : p.term_q[gq]) + p.conf_bias);
   p.mutual[q] = mutual ? 1 : 0;
-  p.valid[q] = mutual && p.flag[gi] ? 1 : 0;
+  if constexpr (k1) p.valid[q] = mutual && p.flag[go] ? 1 : 0;
+  else p.valid[q] = p.flag[gq];
   p.inside[q] = 1;
-  p.centres[2 * q] = fx0; p.centres[2 * q + 1] = fy0;
-  p.centres[2 * (nq + q)] = fx1; p.centres[2 * (nq + q) + 1] = fy1;
+  const int i = k1 ? ans : cell, j = k1 ? cell : ans;
+  const long cq = 2 * (k1 ? nq + q : q), co = 2 * (k1 ? q : nq + q);   // centres of q / o
+  p.i_ids[q] = i; p.j_ids[q] = j;
+  p.centres[cq] = fxq; p.centres[cq + 1] = fyq;
+  p.centres[co] = fxo; p.centres[co + 1] = fyo;
   p.win[q] = b; p.win[nq + q] = i; p.win[nq2 + q] = j;
-  p.pts1_f[2 * q] = static_cast<float>(fx1) * p.s_f * sx1;
-  p.pts1_f[2 * q + 1] = static_cast<float>(fy1) * p.s_f * sy1;
-  p.pts0_c[2 * q] = static_cast<float>(fx0) * p.s_f * sx0;
-  p.pts0_c[2 * q + 1] = static_cast<float>(fy0) * p.s_f * sy0;
+  p.pts_qf[2 * q] = static_cast<float>(fxq) * p.s_f * sxq;
+  p.pts_qf[2 * q + 1] = static_cast<float>(fyq) * p.s_f * syq;
+  p.pts_oc[2 * q] = static_cast<float>(fxo) * p.s_f * sxo;
+  p.pts_oc[2 * q + 1] = static_cast<float>(fyo) * p.s_f * syo;
 }
 
 // Ordered stream compaction (ascending (b, i) like torch.where, coarse_matching.py:194) + coarse
