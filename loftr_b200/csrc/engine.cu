@@ -55,6 +55,10 @@ static int fail(const char* fmt, ...) {
 
 static inline int cdiv(long a, long b) { return static_cast<int>((a + b - 1) / b); }
 
+// CUDA's limit on gridDim.y and gridDim.z.  Entry points whose launches put a caller's count there refuse larger
+// counts before launching anything (DESIGN.md §4.3).
+constexpr int kMaxGridYZ = 65535;
+
 // ------------------------------------------------------------------------------------------------ timing hook
 // Optional per-launch CUDA-event timing of the tensor-core kernels (bench.py's roofline leg), of the per-pair match
 // cap and the rectification search, of the point queries, of the image front end, of the rectifying warp and of the
@@ -1084,6 +1088,7 @@ int lb_rectify_points(const float* pts, const long long* pair_ids, long m, const
 // n_out output images; with img_idx, output image b reads image img_idx[b] of feat
 static int coarse_prep(const float* feat, int nhwc, const float* pe, const int* img_idx, int n_out, int C, int h,
                        int w, int pe_h, int pe_w, float* x_f32, void* cat_hi, void* cat_lo, void* stream) {
+  if (n_out > kMaxGridYZ) return fail("coarse_prep: n_out=%d images exceed the grid.z limit %d", n_out, kMaxGridYZ);
   if (n_out <= 0) return 0;
   DeviceScope dev;
   LB_TRY(dev.bind(x_f32));
@@ -1120,10 +1125,13 @@ template <int kP>
 static int transformer_forward(const LbEncoderLayerWeights* layers, const int* kinds, int n_layers, int d_model,
                                int nhead, const LbTransformerState* st, void* ws, size_t ws_bytes, void* stream) {
   if (st->n_groups <= 0) return 0;
-  DeviceScope dev;
-  LB_TRY(dev.bind(st->x_f32));
   const int C = d_model, H = nhead;
   const bool coarse = (C == 256 && H == 8);
+  // the coarse attention kernels put the images of a pass in grid.z (kv_gemm_kernel, full_attn_wgmma_kernel)
+  if (coarse && st->n_groups > kMaxGridYZ)
+    return fail("coarse transformer: n_groups=%d pairs exceed the grid.z limit %d", st->n_groups, kMaxGridYZ);
+  DeviceScope dev;
+  LB_TRY(dev.bind(st->x_f32));
   const bool fine = (C == 128 && H == 8);
   if (!coarse && !fine) return fail("unsupported transformer shape d_model=%d nhead=%d (built: 256/8 and 128/8)", C, H);
   const int* live = st->n_groups_live;
@@ -1137,7 +1145,10 @@ static int transformer_forward(const LbEncoderLayerWeights* layers, const int* k
            st->group_rows0 > st->group_rows1 ? st->group_rows0 : st->group_rows1);
   if (!b.ok) return fail("transformer workspace too small: need %zu bytes", lb_transformer_workspace_bytes(C, H, st->n_groups, st->group_rows0, st->group_rows1));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const bool same_groups = st->group_rows0 == st->group_rows1;
+  // One self pass over both sets doubles the images in grid.z: above kMaxGridYZ / 2 coarse pairs the sets get a pass
+  // each.  Groups are independent and the pass's splits (kv_splits) are 1 at these counts, so the bits are the same.
+  const bool same_groups =
+      st->group_rows0 == st->group_rows1 && (!coarse || 2L * st->n_groups <= kMaxGridYZ);
   for (int l = 0; l < n_layers; ++l) {
     const LbEncoderLayerWeights& lw = layers[l];
     const bool last = l == n_layers - 1;   // the fp32 copy of the features is only written after the last layer

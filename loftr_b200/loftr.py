@@ -46,6 +46,16 @@ def _check_match_precision(precision, who):
     raise ValueError(f"{who} must be one of {MATCH_PRECISIONS} (got {precision!r})")
 
 
+MAX_PAIRS = 65535   # pairs per call: the coarse transformer's attention kernels put a pass's images in grid.z
+
+
+def check_pairs(n, who):
+    """Refuses more than MAX_PAIRS pairs in one call (`who` names the caller), before anything is launched."""
+    if n > MAX_PAIRS:
+        raise ValueError(f"{who}: {n} pairs exceed the {MAX_PAIRS} pairs of one call (CUDA's grid.z limit); "
+                         "split the pair list into calls of at most that many")
+
+
 GUIDE_KINDS = {"homography": _lib.GUIDE_HOMOGRAPHY, "fundamental": _lib.GUIDE_FUNDAMENTAL}
 
 
@@ -513,6 +523,8 @@ class LocalFeatureTransformer(_PackedCache, nn.Module):
     def forward(self, feat0, feat1, mask0=None, mask1=None):
         """feat0 [N, L, C], feat1 [N, S, C] (+ optional bool masks [N, L], [N, S]) -> updated features."""
         assert self.d_model == feat0.size(2), "the feature number of src and transformer must be equal"
+        if self.d_model // self.nhead == 32:   # the coarse shape: one group per pair (the fine one has no such limit)
+            check_pairs(feat0.shape[0], "LocalFeatureTransformer")
         _require_cuda(feat0, "feat0")
         n, l, c = feat0.shape
         s = feat1.shape[1]
@@ -980,8 +992,11 @@ class LoFTR(nn.Module):
         and minside1; every other key is that of a rectify1 call with the chosen candidate, b_ids / m_bids holding pair
         ids (bs is N).  The outputs equal those of the rectified call on the N * K candidate pairs restricted to the
         chosen ones, bit for bit with the tensor-core backbones; with K = 1 they are the rectify1 call's.  Not
-        combinable with rectify1 or a guide."""
+        combinable with rectify1 or a guide.
+
+        At most MAX_PAIRS (65535) pairs per call."""
         _require_eval(self)
+        check_pairs(data["image0"].shape[0], "forward")
         _require_cuda(data["image0"], "image0")
         if data.get("rectify1_candidates") is not None:
             self._match_searched(data, "forward")
@@ -1130,6 +1145,7 @@ class LoFTR(nn.Module):
         idx1 = self._pair_index(idx1, "idx1", len(feats1), dev, who)
         if idx0.shape != idx1.shape:
             raise ValueError(f"{who}: idx0 and idx1 must have the same length ({idx0.numel()} vs {idx1.numel()})")
+        check_pairs(idx0.numel(), who)
         if (feats0.mask is None) != (feats1.mask is None):
             raise ValueError(f"{who}: either both banks carry masks or neither (as mask0 / mask1 of forward)")
         if (scale0 is None) != (scale1 is None):
@@ -1190,6 +1206,7 @@ class LoFTR(nn.Module):
         data["rectify1_candidates"] (as in `forward`): read from the same tensor at every replay too; the default
         capacity is the bound of the N pairs, since only the winning candidates' matches are listed."""
         _require_static(self, capacity, "forward_static")
+        check_pairs(data["image0"].shape[0], "forward_static")
         dev = None
         for k in ("image0", "image1", "mask0", "mask1", "scale0", "scale1"):
             if k not in data:
@@ -1543,6 +1560,7 @@ def _check_points(data, points0, valid0, side=0):
     for k in ("image0", "image1"):
         if k not in data:
             raise ValueError(f"match_points: data must hold `{k}`")
+    check_pairs(data["image0"].shape[0], "match_points")
     if ("scale0" in data) != ("scale1" in data):
         raise ValueError("match_points: give scale0 and scale1 together")
     if ("mask0" in data) != ("mask1" in data):
